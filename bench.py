@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- simulation steps/s of the Eulerian fluid step (BASELINE.json metric) on N B200s.
+"""bench.py -- simulation steps/s of the Eulerian fluid step (BASELINE.json metric) on N H100s.
 
 Contract: `python bench.py --gpus N --steps K --warmup W` prints ONE JSON line (rank 0).
 One *step* = one `tfluids.simulate` call (torch/lib/simulate.lua:175-327) on a 128^3 MAC
@@ -12,13 +12,15 @@ vorticity confinement and the CNN pressure projection -- BASELINE.json configs[2
   e2e       the same step through the C-ABI host-buffer call (tfl_host_sim_step): pinned
             host p/U/density copied in, step, copied back, every step
   roofline  the dominant kernel's ALGORITHMIC bytes / its measured mean duration vs the
-            measured HBM copy bandwidth (MEASURED_PEAKS.json)
+            measured HBM copy bandwidth (MEASURED_PEAKS.json), else the H100 SXM data sheet's 3.35 TB/s
   cpu_baseline  the reference's own CPU operators (oracle/_ref, compiled in place) -- or the C
             restatement when that is absent -- timed on this box's host cores on a bounded
             sample (one full 128^3 step without the conv stack is ~1 s on 8 cores; the sample
             used is stated)
 
 `--impl reference` times that CPU path alone and prints the same line shape.
+`--dump-outputs DIR` writes the p, U and density the timed path left after its last step as DIR/<name>.npy
+(float32; a fixed seeded sample when the fields exceed 64 MB), so that two builds can be compared output for output.
 Multi-GPU (N > 1, launched with torchrun): weak scaling -- every rank advances an
 independent 128^3 grid (the batch-of-grids decomposition north_star allows); no data-path
 collective; time = max over ranks.
@@ -59,44 +61,16 @@ def use_all_host_cores():
     return n
 
 
-def ncu_traffic(kernel_regexes, path=None):
-    """dram read + write bytes per launch of the named kernels, summed, from the tracked ncu raw table of the
-    current build (profiles/r02_advect_ncu_raw.csv: `ncu -i ... --page raw --csv`); None when absent."""
-    import csv
-    import re
-    path = path or os.path.join(ROOT, "profiles", "r02_advect_ncu_raw.csv")
-    if not os.path.exists(path):
-        return None, None
-    rows = list(csv.reader(open(path)))
-    hdr = next((r for r in rows if "Kernel Name" in r), None)
-    if hdr is None:
-        return None, None
-    ki = hdr.index("Kernel Name")
-    cols = [i for i, h in enumerate(hdr) if h in ("dram__bytes_read.sum", "dram__bytes_write.sum")]
-    units = rows[rows.index(hdr) + 1]
-    scale = {"byte": 1.0, "Kbyte": 1e3, "Mbyte": 1e6, "Gbyte": 1e9}
-    total = 0.0
-    for rx in kernel_regexes:
-        vals = []
-        for r in rows[rows.index(hdr) + 2:]:
-            if len(r) > ki and re.search(rx, r[ki]):
-                vals.append(sum(float(r[i].replace(",", "")) * scale.get(units[i], 1.0) for i in cols))
-        if not vals:
-            return None, None
-        total += sum(vals) / len(vals)
-    return total, os.path.relpath(path, ROOT)
-
-
 def peaks():
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         d = json.load(open(p))
-        return d.get("hbm_gbs", 6650.0), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+        return d.get("hbm_gbs", 3350.0), "measured (MEASURED_PEAKS.json)"
+    return 3350.0, "H100 SXM data sheet (HBM3), not measured"
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -131,6 +105,26 @@ class ClockSampler(threading.Thread):
             return {"sm_mhz": None, "sm_max_mhz": self.max_mhz, "reasons": ["unsampled"]}
         return {"sm_mhz": float(np.median(self.samples)), "sm_max_mhz": self.max_mhz,
                 "reasons": sorted(self.reasons)}
+
+
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, fields):
+    """fields: name -> tensor.  Written as float32 .npy; when their total exceeds DUMP_LIMIT_BYTES each is cut to
+    the same seeded sample of flat indices (saved beside it as <name>_index.npy, float64)."""
+    os.makedirs(out_dir, exist_ok=True)
+    total = sum(t.numel() * 4 for t in fields.values())
+    for name, t in fields.items():
+        a = t.detach().float().cpu().numpy().ravel()
+        if total > DUMP_LIMIT_BYTES:
+            k = a.size * DUMP_LIMIT_BYTES // (3 * total)          # 4-byte values + 8-byte indices fit the limit
+            idx = np.sort(np.random.default_rng(0).choice(a.size, k, replace=False))
+            np.save(os.path.join(out_dir, name + "_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        else:
+            a = a.reshape(tuple(t.shape))
+        np.save(os.path.join(out_dir, name + ".npy"), a.astype(np.float32))
 
 
 def make_problem(n=N_GRID, velocity="smooth"):
@@ -293,6 +287,8 @@ def main():
     ap.add_argument("--steps", type=int, default=50)
     ap.add_argument("--warmup", type=int, default=5)
     ap.add_argument("--impl", default="b200")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="after the timed steps, write the p / U / density of the last timed step to DIR/<name>.npy")
     ap.add_argument("--grid", type=int, default=N_GRID)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-slab", action="store_true", help="skip the 256^3 z-slab (BASELINE config 5) sub-record")
@@ -325,7 +321,7 @@ def main():
         gb = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch_np.items()}
         gm = fmodel.ProjectionModel(mnp["layers"], True)
         ctx = tfluids.context()
-        # L2 flush buffer (> 126 MB) written between timed iterations.
+        # L2 flush buffer (5x the H100's 50 MB L2) written between timed iterations.
         flush = torch.empty(256 * 1024 * 1024 // 4, dtype=torch.float32, device="cuda")
 
         def timed_steps(state, steps, warmup):
@@ -381,6 +377,9 @@ def main():
         except Exception as e:                      # a box that cannot capture: the kernel-by-kernel number is the headline
             graph_error = "%s: %s" % (type(e).__name__, e)
             graph_ms, graph_launches = total_ms, launches
+        if args.dump_outputs and rank == 0:
+            stream.synchronize()
+            dump_outputs(args.dump_outputs, {"p": gb["pDiv"], "U": gb["UDiv"], "density": gb["density"]})
         # trace-length regime of the timed steps (the advection cost is data dependent)
         max_u_dt = float(gb["UDiv"].abs().max().item()) * mconf["dt"]
         if world > 1:
@@ -471,7 +470,6 @@ def main():
         k_ms = float(np.mean(ks)) if min(ks) > 0 else op_ms
         algo_bytes = ALGO_BYTES["advect_vel"] * n ** 3
         achieved = algo_bytes / (k_ms * 1e-3) / 1e9
-        traffic, traffic_src = ncu_traffic([r"k_advect_vel_tile"]) if n == 128 else (None, None)
 
         # ---- BASELINE config 4: 100-iteration Jacobi sweep (stencil HBM roofline) ----------
         extra = []
@@ -584,10 +582,7 @@ def main():
                                                   "alone with CUDA events around its launch",
                      "operator_ms": op_ms,
                      "achieved": achieved, "peak": peak, "unit": "GB/s", "frac": achieved / peak,
-                     "traffic": traffic, "traffic_source": traffic_src,
-                     "algorithmic_bytes": algo_bytes, "peak_source": peak_src, "kernel_ms": k_ms,
-                     "limiter": "instruction issue, not HBM: 1567 warp-instructions per 32 voxels at 72 % issue-active "
-                                "(profiles/r02_advect_tile_*)"},
+                     "algorithmic_bytes": algo_bytes, "peak_source": peak_src, "kernel_ms": k_ms},
         "roofline_extra": extra,
         "slab": slab,
         "cpu_baseline": cpu,

@@ -1,6 +1,6 @@
-"""fluidnet_b200 -- B200-native Eulerian fluid step behind the tfluids operator surface.
+"""fluidnet_b200 -- H100-native Eulerian fluid step behind the tfluids operator surface.
 
-The product is `libtfl.so` (hand-written sm_100a CUDA behind the C ABI in include/tfl.h).
+The product is `libtfl.so` (hand-written sm_90a CUDA behind the C ABI in include/tfl.h).
 This package is the thin host-side mirror of the reference's Lua interface
 (torch/tfluids/init.lua, torch/lib/simulate.lua, torch/lib/model.lua) so that host code
 written against `tfluids.*` keeps its call sites:

@@ -94,8 +94,6 @@ struct tfl_cnn {
   int mode = 0;              // 0 fp32 FMA, 1 TF32 tensor cores, 2 3xTF32 tensor cores
   bool tc_ok = false;
   float* wB[2][3] = {{nullptr, nullptr, nullptr}, {nullptr, nullptr, nullptr}};   // [split][layer]
-  float* wTS[3] = {nullptr, nullptr, nullptr};   // weight blocks of the TMEM-operand kernel
-  int use_ts = 1;            // mode 2 prefers the TMEM-operand kernel where it applies
   float* tail = nullptr;     // w4[8][8], b4[8], w5[8], b5[1]
   float* act[3] = {nullptr, nullptr, nullptr};   // padded channels-last activation buffers
   ConvTcGeo act_geo = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
@@ -334,7 +332,7 @@ float get_dx(const Geo& g) {     // third_party/grid.cc:37-40 on the GLOBAL grid
 
 extern "C" {
 
-const char* tfl_version(void) { return "libtfl 0.1 (sm_100a)"; }
+const char* tfl_version(void) { return "libtfl 0.1 (sm_90a)"; }
 
 int tfl_advect_method_from_string(const char* s) {
   if (!s) return -1;
@@ -1046,12 +1044,6 @@ int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
         cudaMalloc((void**)&m->wB[split][l], packed.size() * 4);
         cudaMemcpy(m->wB[split][l], packed.data(), packed.size() * 4, cudaMemcpyHostToDevice);
       }
-    for (int l = 0; l < 3; l++) {
-      std::vector<float> packed(conv_ts_b_floats());
-      conv_ts_pack_weights(weights[l], cin[l], packed.data());
-      cudaMalloc((void**)&m->wTS[l], packed.size() * 4);
-      cudaMemcpy(m->wTS[l], packed.data(), packed.size() * 4, cudaMemcpyHostToDevice);
-    }
     std::vector<float> tail(64 + 8 + 8 + 1);
     memcpy(tail.data(), weights[3], 64 * 4);
     memcpy(tail.data() + 64, biases[3], 8 * 4);
@@ -1075,7 +1067,7 @@ int tfl_cnn_set_mode(tfl_ctx* ctx, tfl_cnn* m, int mode) {
   return 0;
 }
 int tfl_cnn_get_mode(const tfl_cnn* m) { return m ? m->mode : -1; }
-// Undocumented debugging hook: 0 forces the shared-memory-operand kernel in 3xTF32 mode.
+// Undocumented debugging hook.
 // mode: -1 automatic, 0 two-kernel advectVel, 1 / 2 tile kernel with that halo; variant: tile shape.
 int tfl_debug_advect_tile(tfl_ctx* ctx, int mode, int variant) {
   if (!ctx) return 1;
@@ -1105,10 +1097,8 @@ float tfl_debug_last_advect_kernel_ms(tfl_ctx* ctx) {
   return ms;
 }
 
-int tfl_debug_cnn_use_ts(tfl_cnn* m, int on) { if (m) m->use_ts = on; return 0; }
 // Undocumented debugging hook (not in tfl.h): per-CTA phase timestamps of the tensor-core conv.
 int tfl_debug_conv_timestamps(void* dev_buf) { conv_tc_set_debug((long long*)dev_buf); return 0; }
-int tfl_debug_conv_ts_counters(void* dev_buf) { conv_ts_set_debug((long long*)dev_buf); return 0; }
 
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
   DeviceGuard guard_(ctx);
@@ -1121,8 +1111,6 @@ void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
     for (int l = 0; l < 3; l++)
       if (m->wB[sp][l]) cudaFree(m->wB[sp][l]);
   if (m->tail) cudaFree(m->tail);
-  for (float* p : m->wTS)
-    if (p) cudaFree(p);
   for (float* p : m->act)
     if (p) cudaFree(p);
   delete m;
@@ -1149,12 +1137,6 @@ static int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
 static void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo = 0, int p_hi = -1) {
   const ConvTcGeo& tg = m->act_geo;
   if (p_hi < 0) p_hi = tg.nz;
-  if (m->mode == 2 && m->use_ts && conv_ts_supported(tg)) {        // (whole slab: this kernel marches over z)
-    launch_conv3_ts(m->act[0], m->act[1], nullptr, m->wTS[0], m->b[0], nullptr, 1, 0, tg, st);
-    launch_conv3_ts(m->act[1], m->act[2], nullptr, m->wTS[1], m->b[1], nullptr, 2, 0, tg, st);
-    launch_conv3_ts(m->act[2], nullptr, p_net, m->wTS[2], m->b[2], m->tail, 2, 1, tg, st);
-    return;
-  }
   const int split = m->mode == 2 ? 1 : 0;
   ConvTcGeo g1 = tg, g2 = tg, g3 = tg;
   g3.z_lo = std::max(0, p_lo);     g3.z_hi = std::min(tg.nz, p_hi);
@@ -2044,7 +2026,7 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
     const size_t side = (size_t)d.cnt * d.nchan;                  // floats per message
     if (side > s->xbuf_side) return fail(ctx, "slab exchange buffer too small");
     const bool lo = s->rank > 0, hi = s->rank < s->world - 1;
-    const int blocks = (int)std::min<size_t>((2 * side + 255) / 256, 148 * 4);
+    const int blocks = (int)std::min<size_t>((2 * side + 255) / 256, 132 * 4);
     if (s->peer_ok) {
       // inbox layout: buffer (phase, from-below = 0 / from-above = 1) at ((phase * 2 + from) * xbuf_side), counters behind
       auto buf = [&](float* base, int from) { return base + ((size_t)phase * 2 + from) * s->xbuf_side; };

@@ -1,31 +1,31 @@
-// Tensor-core (tcgen05 / TMEM) implementation of the 3x3x3 convolution layers of the 3-D
+// Tensor-core (Hopper wgmma) implementation of the 3x3x3 convolution layers of the 3-D
 // pressure-projection network (torch/lib/model.lua:219-226: 3->8, 8->8, 8->8 with k=3, then
-// 8->8 and 8->1 with k=1, ReLU between layers).  sm_100a only.
+// 8->8 and 8->1 with k=1, ReLU between layers).  sm_90a only.
 //
 // Formulation (implicit GEMM, no im2col buffer):
 //   * activations live in global memory channels-last in two float4 planes (channels 0-3 and
 //     4-7) over a grid padded by one zero voxel on every side, so halo loads need no bounds
 //     tests and the zero padding of the convolution is simply "there";
-//   * a CTA stages a (32 x 10 x 10)-position box of both planes into shared memory
+//   * a CTA stages a (32 x PY x PZ)-position box of both planes into shared memory
 //     (cp.async, 16 B per position and plane).  In that box the positions are LINEAR
-//     (x fastest, pitch 32), so ANY 128 consecutive positions form a valid K-major,
-//     no-swizzle UMMA A operand: 8-row core matrices are 128 B apart (SBO), the two
+//     (x fastest, pitch 32), so ANY 64 consecutive positions form a valid K-major,
+//     no-swizzle wgmma A operand: 8-row core matrices are 128 B apart (SBO), the two
 //     4-channel K chunks are one plane apart (LBO), and shifting the operand by a filter
 //     tap (dy, dz) is a pure start-address offset;
 //   * the three x-taps of a (dy, dz) pair share ONE A operand: B holds their weights side by
-//     side (N = 3 taps x 8 output channels, padded to 32), so 9 MMAs (M=128, N=32, K=8,
-//     kind::tf32, fp32 accumulate in TMEM) cover the 27 taps, and the x shift is applied in
-//     the epilogue: out[x] = D_{-1}[x-1] + D_0[x] + D_{+1}[x+1].  An M tile is 4 rows of 32
-//     x-positions, a TMEM lane quarter is exactly one row, so that shift is two warp
-//     shuffles per output channel;
+//     side (N = 3 taps x 8 output channels = 24), so 9 wgmma (M=64, N=24, K=8, tf32 inputs,
+//     fp32 accumulate in registers) cover the 27 taps, and the x shift is applied in the
+//     epilogue: out[x] = D_{-1}[x-1] + D_0[x] + D_{+1}[x+1].  An M tile is 2 rows of 32
+//     x-positions; the accumulators go through a small shared-memory buffer per warpgroup
+//     so that every thread can read its x-1 / x+1 neighbours;
 //   * 3xTF32 mode (SPLIT): A and B are split into tf32 "hi" and fp32-residual "lo" parts;
-//     hi*hi, hi*lo (same MMA, N = 48) and lo*hi (second MMA) are accumulated, which restores
-//     ~fp32 accuracy at 2x the MMA count;
-//   * the epilogue (tcgen05.ld -> registers) adds bias, applies ReLU and either writes the
-//     next layer's padded channels-last planes or, for the last 3x3x3 layer, also runs the
-//     two 1x1x1 layers and writes the pressure.
-// Accumulators are double buffered in TMEM so the epilogue of M tile t overlaps the MMAs
-// of tile t+1; two CTAs per SM overlap one CTA's loads with the other's math.
+//     hi*hi, hi*lo (same wgmma, N = 48) and lo*hi (second wgmma, N = 24) are accumulated,
+//     which restores ~fp32 accuracy at 2x the MMA count;
+//   * the epilogue adds bias, applies ReLU and either writes the next layer's padded
+//     channels-last planes or, for the last 3x3x3 layer, also runs the two 1x1x1 layers and
+//     writes the pressure.
+// Two warpgroups per CTA take alternate M tiles; two CTAs per SM overlap one CTA's loads with
+// the other's math (the boxes are sized so that two fit the SM's 228 KB of shared memory).
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -37,15 +37,16 @@ namespace {
 
 constexpr int kTX = 32;                 // positions per row in the staged box (30 outputs + 2 halo)
 constexpr int kGroups = 9;              // (dz, dy) pairs
-constexpr int kThreads = 288;           // 8 epilogue warps (2 warpgroups) + 1 MMA-issuer warp
+constexpr int kThreads = 256;           // 2 warpgroups
+constexpr int kDPitch = 24;             // floats per position in the accumulator staging buffer
 
 // CTA box: 3xTF32 keeps 4 planes (hi/lo x 2 channel groups) in shared memory, so its box is
-// smaller to still fit two CTAs per SM (2 x ~112 KB).
+// smaller to still fit two CTAs per SM.
 template <bool SPLIT> struct Tile {
-  static constexpr int TY = SPLIT ? 4 : 8;      // output rows per CTA (multiple of 4)
-  static constexpr int TZ = SPLIT ? 6 : 8;      // output planes per CTA
+  static constexpr int TY = SPLIT ? 4 : 8;      // output rows per CTA (multiple of 2)
+  static constexpr int TZ = SPLIT ? 5 : 6;      // output planes per CTA
   static constexpr int PY = TY + 2, PZ = TZ + 2;
-  static constexpr int RB = TY / 4;             // 4-row blocks (= M tiles) per plane
+  static constexpr int RB = TY / 2;             // 2-row blocks (= M tiles) per plane
   static constexpr int POS = kTX * PY * PZ;
   static constexpr int PLANE_BYTES = POS * 16;
   static constexpr int MTILES = TZ * RB;
@@ -54,60 +55,45 @@ template <bool SPLIT> struct Tile {
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
 }
-__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
-  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count));
-}
-__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
-  uint32_t done;
-  do {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-        "selp.u32 %0, 1, 0, p;\n\t}"
-        : "=r"(done)
-        : "r"(bar), "r"(parity)
-        : "memory");
-  } while (!done);
-}
 __device__ __forceinline__ void cp_async16(uint32_t dst, const void* src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(dst), "l"(src) : "memory");
 }
-// K-major, no-swizzle shared-memory matrix descriptor (sm_100 "version 1"):
-// start address, leading byte offset (between the two 16-byte K chunks) and stride byte
-// offset (between 8-row core matrices), all in 16-byte units.
+// K-major, no-swizzle wgmma shared-memory matrix descriptor: start address, leading byte offset
+// (between the two 16-byte K chunks) and stride byte offset (between 8-row core matrices), all
+// in 16-byte units.
 __device__ __forceinline__ uint64_t make_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes) {
   uint64_t d = 0;
   d |= (uint64_t)((saddr >> 4) & 0x3FFF);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
   return d;
 }
-// kind::tf32 instruction descriptor: fp32 accumulate, A and B tf32, both K-major.
-__host__ __device__ constexpr uint32_t make_idesc(int M, int N) {
-  return (1u << 4) | (2u << 7) | (2u << 10) | ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
-__device__ __forceinline__ void umma_tf32(uint32_t tmem_d, uint64_t da, uint64_t db, uint32_t idesc,
-                                          uint32_t accumulate) {
+// D[64 x 24] (+)= A[64 x 8] * B[8 x 24], tf32 inputs, fp32 accumulators in registers.
+__device__ __forceinline__ void wgmma_n24(float (&d)[12], uint64_t da, uint64_t db, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::tf32 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(da), "l"(db), "r"(idesc), "r"(accumulate)
-      : "memory");
+      "setp.ne.b32 p, %14, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n24k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11}, %12, %13, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar)
-               : "memory");
+// D[64 x 48] (+)= A[64 x 8] * B[8 x 48].
+__device__ __forceinline__ void wgmma_n48(float (&d)[24], uint64_t da, uint64_t db, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %26, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n48k8.f32.tf32.tf32 "
+      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23}, "
+      "%24, %25, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+        "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+        "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23])
+      : "l"(da), "l"(db), "r"(accumulate));
 }
-// 32 lanes x 8 consecutive 32-bit columns -> 8 registers per thread (no wait).
-__device__ __forceinline__ void tmem_ld8(uint32_t taddr, uint32_t* r) {
-  asm volatile("tcgen05.ld.sync.aligned.32x32b.x8.b32 {%0,%1,%2,%3,%4,%5,%6,%7}, [%8];"
-               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7])
-               : "r"(taddr));
+__device__ __forceinline__ void wg_barrier(int id) {
+  asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
 }
 __device__ __forceinline__ float4 tf32_hi(float4 v) {
   float4 h;
@@ -131,13 +117,10 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   constexpr int A_BYTES = (SPLIT ? 4 : 2) * T::PLANE_BYTES;
   constexpr int B_GROUP_BYTES = 2 * NB * 16;
   constexpr int B_BYTES = kGroups * B_GROUP_BYTES;
-  constexpr int COLS_PER_BUF = SPLIT ? 128 : 32;     // TMEM columns per accumulator buffer
-  constexpr int TMEM_COLS = 2 * COLS_PER_BUF;
   uint8_t* sA = smem;
   uint8_t* sB = smem + A_BYTES;
-  uint64_t* bars = (uint64_t*)(smem + A_BYTES + B_BYTES);   // full[2], empty[2]
-  uint32_t* tmem_slot = (uint32_t*)(bars + 4);
-  float* sTail = (float*)(tmem_slot + 4);           // bias[8] (+ w4[64] b4[8] w5[8] b5[1] when FINAL)
+  float* sD = (float*)(smem + A_BYTES + B_BYTES);            // [2 warpgroups][64][kDPitch]
+  float* sTail = sD + 2 * 64 * kDPitch;                      // bias[8] (+ w4[64] b4[8] w5[8] b5[1] when FINAL)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
   const int tx = blockIdx.x, ty = blockIdx.y;
@@ -145,20 +128,6 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   const int cta_lin = (blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x;
   if (dbg && tid == 0) dbg[cta_lin * 8 + 0] = clock64();
   const int tzb = blockIdx.z % g.ntz, b = blockIdx.z / g.ntz;
-
-  if (tid == 0) {
-    mbar_init(smem_u32(&bars[0]), 1);       // full[0], full[1]: one tcgen05.commit per batch
-    mbar_init(smem_u32(&bars[1]), 1);
-    mbar_init(smem_u32(&bars[2]), 128);     // empty[0], empty[1]: the owning epilogue warpgroup arrives
-    mbar_init(smem_u32(&bars[3]), 128);
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-  }
-  if (warp == 8) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(tmem_slot)),
-                 "r"(TMEM_COLS));
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::);
-  }
 
   // ---- stage the input box ------------------------------------------------------------
   const long long plane_g = (long long)(g.nz + 2) * g.py * g.px;            // float4 per global plane
@@ -218,133 +187,108 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   for (int i = tid; i < n_tail; i += kThreads) sTail[i] = (i < 8) ? bias[i] : tail[i - 8];
   asm volatile("cp.async.commit_group;" ::: "memory");
   asm volatile("cp.async.wait_group 0;" ::: "memory");
+  // generic-proxy writes (st.shared, cp.async) -> visible to the wgmma (async proxy) reads
   asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = *tmem_slot;
   if (dbg && tid == 0) { dbg[cta_lin * 8 + 1] = clock64(); unsigned smid; asm("mov.u32 %0, %%smid;" : "=r"(smid)); dbg[cta_lin * 8 + 7] = smid; }
 
-  if (warp == 8) {
-    // ===== MMA issuer: one elected thread =====
-    if (lane == 0) {
-      const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-      constexpr uint32_t IDESC_MAIN = make_idesc(128, NB);
-      constexpr uint32_t IDESC_LO = make_idesc(128, 32);
-      // Descriptors are loop invariant up to a start-address offset per M tile: build them once
-      // so that the issue loop is one 32-bit add + one tcgen05.mma per instruction.
-      uint64_t db[kGroups], da0[kGroups];
+  // ---- warpgroup wg takes M tiles t = wg, wg + 2, ... ------------------------------------
+  const int wg = warp >> 2, wq = warp & 3;
+  const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
+  constexpr uint32_t LO_PLANES_16 = (uint32_t)(2 * T::PLANE_BYTES) >> 4;
+  float* myD = sD + wg * 64 * kDPitch;
+  const float* sBias = sTail;
+  const int tw = tid & 127, p = tw >> 1, half = tw & 1;     // epilogue: position p, channels 4*half..+3
+  const int xl = p & 31, ry = p >> 5;
+  const int pm = xl > 0 ? p - 1 : p, pp = xl < 31 ? p + 1 : p;
+  for (int t = wg; t < T::MTILES; t += 2) {
+    // M tile t: padded plane 1 + t / RB, rows 1 + 2 * (t % RB) .. +1, positions 0..31.
+    const uint32_t toff = (uint32_t)((((t / T::RB) * T::PY + 2 * (t % T::RB)) * kTX) * 16);
+    float acc[SPLIT ? 24 : 12] = {}, acl[12] = {};
+    asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-      for (int gi = 0; gi < kGroups; gi++) {
-        const int dz = gi / 3 - 1, dy = gi % 3 - 1;
-        db[gi] = make_desc(sB_u + gi * B_GROUP_BYTES, NB * 16, 128);
-        da0[gi] = make_desc(sA_u + (uint32_t)((((1 + dz) * T::PY + (1 + dy)) * kTX) * 16), T::PLANE_BYTES, 128);
-      }
-      constexpr uint32_t LO_PLANES_16 = (uint32_t)(2 * T::PLANE_BYTES) >> 4;
-      for (int t = 0; t < T::MTILES; t++) {
-        const int buf = t & 1;
-        if (t >= 2) {
-          mbar_wait(smem_u32(&bars[2 + buf]), (uint32_t)(((t >> 1) - 1) & 1));
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
-        // M tile t: padded plane 1 + t / RB, rows 1 + 4 * (t % RB) .. +3, positions 0..31.
-        const uint32_t toff16 = (uint32_t)((((t / T::RB) * T::PY + 4 * (t % T::RB)) * kTX));   // 16-byte units
-        const uint32_t d_addr = tmem_base + (uint32_t)(buf * COLS_PER_BUF);
-#pragma unroll
-        for (int gi = 0; gi < kGroups; gi++) {
-          const uint64_t da = da0[gi] + toff16;
-          umma_tf32(d_addr, da, db[gi], IDESC_MAIN, gi > 0 ? 1u : 0u);
-          if (SPLIT) umma_tf32(d_addr + 64, da + LO_PLANES_16, db[gi], IDESC_LO, gi > 0 ? 1u : 0u);
-        }
-        umma_commit(smem_u32(&bars[buf]));
-        if (dbg && t == 0) dbg[cta_lin * 8 + 2] = clock64();
-      }
-      if (dbg) dbg[cta_lin * 8 + 3] = clock64();
-    }
-  } else {
-    // ===== epilogue warpgroups: warpgroup wg owns accumulator buffer wg (tiles t = wg, wg+2, ...) =====
-    const int wg = warp >> 2, q = warp & 3;
-    const float* sBias = sTail;
-    for (int t = wg; t < T::MTILES; t += 2) {
-      mbar_wait(smem_u32(&bars[wg]), (uint32_t)((t >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      if (dbg && tid == 0 && t == 0) dbg[cta_lin * 8 + 4] = clock64();
-      const uint32_t taddr = tmem_base + (uint32_t)(wg * COLS_PER_BUF) + ((uint32_t)(q * 32) << 16);
-      uint32_t r0[24];
-      tmem_ld8(taddr + 0, r0);
-      tmem_ld8(taddr + 8, r0 + 8);
-      tmem_ld8(taddr + 16, r0 + 16);
-      float dm[8], d0[8], dp[8];
-      if (SPLIT) {
-        uint32_t r1[24], r2[24];
-        tmem_ld8(taddr + 24, r1);
-        tmem_ld8(taddr + 32, r1 + 8);
-        tmem_ld8(taddr + 40, r1 + 16);
-        tmem_ld8(taddr + 64, r2);
-        tmem_ld8(taddr + 72, r2 + 8);
-        tmem_ld8(taddr + 80, r2 + 16);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-          dm[i] = __uint_as_float(r0[i]) + (__uint_as_float(r1[i]) + __uint_as_float(r2[i]));
-          d0[i] = __uint_as_float(r0[8 + i]) + (__uint_as_float(r1[8 + i]) + __uint_as_float(r2[8 + i]));
-          dp[i] = __uint_as_float(r0[16 + i]) + (__uint_as_float(r1[16 + i]) + __uint_as_float(r2[16 + i]));
-        }
+    for (int gi = 0; gi < kGroups; gi++) {
+      const int dz = gi / 3 - 1, dy = gi % 3 - 1;
+      const uint32_t a_addr = sA_u + toff + (uint32_t)((((1 + dz) * T::PY + (1 + dy)) * kTX) * 16);
+      const uint64_t da = make_desc(a_addr, T::PLANE_BYTES, 128);
+      const uint64_t db = make_desc(sB_u + gi * B_GROUP_BYTES, NB * 16, 128);
+      if constexpr (SPLIT) {
+        wgmma_n48(acc, da, db, gi > 0 ? 1u : 0u);
+        wgmma_n24(acl, da + LO_PLANES_16, db, gi > 0 ? 1u : 0u);
       } else {
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-        for (int i = 0; i < 8; i++) {
-          dm[i] = __uint_as_float(r0[i]);
-          d0[i] = __uint_as_float(r0[8 + i]);
-          dp[i] = __uint_as_float(r0[16 + i]);
-        }
+        wgmma_n24(acc, da, db, gi > 0 ? 1u : 0u);
       }
-      // TMEM reads of this buffer are done -> hand it back to the MMA issuer.
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      mbar_arrive(smem_u32(&bars[2 + wg]));
+    }
+    asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+    asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+    if (dbg && tid == 0 && t == 0) dbg[cta_lin * 8 + 2] = clock64();
 
-      float h[8];
+    // accumulator fragment: element (row 16 wq + lane / 4 + 8 i, column 8 k + 2 (lane % 4) + j) is acc[4 k + 2 i + j]
+#pragma unroll
+    for (int k = 0; k < 3; k++)
+#pragma unroll
+      for (int i = 0; i < 2; i++) {
+        const int row = 16 * wq + (lane >> 2) + 8 * i, col = 8 * k + 2 * (lane & 3);
+        float2 v;
+        if constexpr (SPLIT) {
+          v.x = acc[4 * k + 2 * i] + (acc[12 + 4 * k + 2 * i] + acl[4 * k + 2 * i]);
+          v.y = acc[4 * k + 2 * i + 1] + (acc[12 + 4 * k + 2 * i + 1] + acl[4 * k + 2 * i + 1]);
+        } else {
+          v.x = acc[4 * k + 2 * i];
+          v.y = acc[4 * k + 2 * i + 1];
+        }
+        *(float2*)(myD + row * kDPitch + col) = v;
+      }
+    wg_barrier(1 + wg);
+
+    const float4 dm = *(const float4*)(myD + pm * kDPitch + 4 * half);
+    const float4 d0 = *(const float4*)(myD + p * kDPitch + 8 + 4 * half);
+    const float4 dp = *(const float4*)(myD + pp * kDPitch + 16 + 4 * half);
+    const float* bs = sBias + 4 * half;
+    float h[4];
+    h[0] = (dm.x + d0.x) + dp.x + bs[0];
+    h[1] = (dm.y + d0.y) + dp.y + bs[1];
+    h[2] = (dm.z + d0.z) + dp.z + bs[2];
+    h[3] = (dm.w + d0.w) + dp.w + bs[3];
+#pragma unroll
+    for (int o = 0; o < 4; o++) h[o] = h[o] > 0.0f ? h[o] : 0.0f;
+    const int xg = x0 + xl - 1;                         // unpadded coordinates of this position's voxel
+    const int yg = y0 + 2 * (t % T::RB) + ry;
+    const int zg = z0 + t / T::RB;
+    const bool valid = xl >= 1 && xl <= 30 && xg < g.nx && yg < g.ny && zg < g.z_hi;
+    if (!FINAL) {
+      if (valid) {
+        const long long o = b * batch_g + ((long long)(zg + 1) * g.py + (yg + 1)) * g.px + (xg + 1);
+        out[o + half * plane_g] = make_float4(h[0], h[1], h[2], h[3]);
+      }
+    } else {
+      float hh[8];
+#pragma unroll
+      for (int o = 0; o < 4; o++) {
+        const float other = __shfl_xor_sync(0xffffffffu, h[o], 1);
+        hh[o] = half ? other : h[o];
+        hh[4 + o] = half ? h[o] : other;
+      }
+      const float* w4 = sTail + 8;      // [o][c]
+      const float* b4 = w4 + 64;
+      const float* w5 = b4 + 8;
+      const float b5 = w5[8];
+      float pacc = b5;
 #pragma unroll
       for (int o = 0; o < 8; o++) {
-        const float a = __shfl_up_sync(0xffffffffu, dm[o], 1);
-        const float c = __shfl_down_sync(0xffffffffu, dp[o], 1);
-        const float v = (a + d0[o]) + c + sBias[o];
-        h[o] = v > 0.0f ? v : 0.0f;
-      }
-      const int xg = x0 + lane - 1;                         // unpadded coordinates of this lane's voxel
-      const int yg = y0 + 4 * (t % T::RB) + q;
-      const int zg = z0 + t / T::RB;
-      const bool valid = lane >= 1 && lane <= 30 && xg < g.nx && yg < g.ny && zg < g.z_hi;
-      if (!FINAL) {
-        if (valid) {
-          const long long o = b * batch_g + ((long long)(zg + 1) * g.py + (yg + 1)) * g.px + (xg + 1);
-          out[o] = make_float4(h[0], h[1], h[2], h[3]);
-          out[o + plane_g] = make_float4(h[4], h[5], h[6], h[7]);
-        }
-      } else {
-        const float* w4 = sTail + 8;      // [o][c]
-        const float* b4 = w4 + 64;
-        const float* w5 = b4 + 8;
-        const float b5 = w5[8];
-        float pacc = b5;
+        float a = b4[o];
 #pragma unroll
-        for (int o = 0; o < 8; o++) {
-          float a = b4[o];
-#pragma unroll
-          for (int c = 0; c < 8; c++) a = fmaf(h[c], w4[o * 8 + c], a);
-          a = a > 0.0f ? a : 0.0f;
-          pacc = fmaf(a, w5[o], pacc);
-        }
-        if (valid) p_net[(long long)b * g.nz * g.ny * g.nx + ((long long)zg * g.ny + yg) * g.nx + xg] = pacc;
+        for (int c = 0; c < 8; c++) a = fmaf(hh[c], w4[o * 8 + c], a);
+        a = a > 0.0f ? a : 0.0f;
+        pacc = fmaf(a, w5[o], pacc);
       }
+      if (valid && half == 0) p_net[(long long)b * g.nz * g.ny * g.nx + ((long long)zg * g.ny + yg) * g.nx + xg] = pacc;
     }
+    wg_barrier(1 + wg);                                 // myD is rewritten by the next tile
   }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (dbg && tid == 0) dbg[cta_lin * 8 + 5] = clock64();
-  if (warp == 8) {
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "r"(TMEM_COLS));
+  if (dbg) {
+    __syncthreads();
+    if (tid == 0) dbg[cta_lin * 8 + 5] = clock64();
   }
 }
 
@@ -353,7 +297,7 @@ void launch_one(const float4* in, float4* out, float* p_net, const float* wB, co
                 const float* tail, const ConvTcGeo& g, cudaStream_t st) {
   using T = Tile<SPLIT>;
   constexpr int NB = SPLIT ? 48 : 32;
-  const size_t smem = (size_t)(SPLIT ? 4 : 2) * T::PLANE_BYTES + kGroups * 2 * NB * 16 + 64 + 4 * 96;
+  const size_t smem = (size_t)(SPLIT ? 4 : 2) * T::PLANE_BYTES + kGroups * 2 * NB * 16 + 2 * 64 * kDPitch * 4 + 4 * 96;
   auto kern = k_conv3_tc<IN_PLANES, FINAL, SPLIT>;
   static unsigned long long configured = 0;       // per device (function attributes are)
   int dev = 0;

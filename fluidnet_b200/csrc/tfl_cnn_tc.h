@@ -24,12 +24,4 @@ int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, 
                     const float* tail, int in_planes, int final_layer, int split, const ConvTcGeo& g,
                     cudaStream_t st);
 
-// ---- tfl_cnn_ts.cu: A operand in tensor memory (3xTF32 only, nx <= 128) ----
-int conv_ts_b_floats();
-void conv_ts_set_debug(long long* dev_buf);
-void conv_ts_pack_weights(const float* w /*[8][cin][3][3][3]*/, int cin, float* out);
-bool conv_ts_supported(const ConvTcGeo& g);
-int launch_conv3_ts(const float* in, float* out, float* p_net, const float* wB, const float* bias,
-                    const float* tail, int in_planes, int final_layer, const ConvTcGeo& g, cudaStream_t st);
-
 }  // namespace tfl

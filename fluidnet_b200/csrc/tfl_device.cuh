@@ -1,6 +1,6 @@
 // Device-side building blocks shared by the stencil kernels: grid geometry, flag tests,
 // MAC-grid sampling, Manta-style trilinear interpolation and the obstacle-aware line
-// trace.  Written for sm_100a; every translation unit that includes this header for a
+// trace.  Written for sm_90a; every translation unit that includes this header for a
 // parity-critical kernel is compiled with -fmad=false (the CPU reference has no FMA
 // contraction), IEEE division / sqrt (nvcc defaults, no --use_fast_math).
 //

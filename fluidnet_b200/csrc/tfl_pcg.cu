@@ -815,7 +815,7 @@ int normalize_pressure_mean(void* workspace, float* p, const float* flags, int n
   k_label_init<<<blocks_for(cells), 256, 0, st>>>(flags, parent, g, status);
   k_label_union<true><<<blocks_for(cells), 256, 0, st>>>(parent, g, status);
   k_label_flatten<<<blocks_for(cells), 256, 0, st>>>(parent, csize, g);
-  int dev = 0, sms = 148;
+  int dev = 0, sms = 132;
   cudaGetDevice(&dev);
   cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
   const unsigned blocks = (unsigned)std::min<long long>((cells + 255) / 256, (long long)sms * 8);

@@ -1295,7 +1295,7 @@ int launch_clearance(const FT* flags, unsigned char* clear, unsigned char* tmp, 
                      cudaStream_t st) {
   const long long total = g.n * g.nb;
   const int block = 256;
-  const int grid = (int)std::min<long long>((total + block - 1) / block, 148 * 8);
+  const int grid = (int)std::min<long long>((total + block - 1) / block, 132 * 8);
   if (g.is3d) {                            // (a 3-D grid with fewer than 3 planes gets clearance 0)
     k_clear_x<FT><<<grid, block, 0, st>>>(flags, clear, g, gate);
     k_clear_axis<1, false><<<grid, block, 0, st>>>(clear, tmp, g, gate);

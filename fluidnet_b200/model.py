@@ -73,7 +73,7 @@ class ProjectionModel:
     MODES = {"fp32": 0, "tf32": 1, "tf32x3": 2}
 
     def set_mode(self, mode):
-        """'fp32' (CUDA-core FMA), 'tf32' or 'tf32x3' (tcgen05 tensor cores)."""
+        """'fp32' (CUDA-core FMA), 'tf32' or 'tf32x3' (wgmma tensor cores)."""
         self.ctx.check(self.ctx.lib.tfl_cnn_set_mode(self.ctx.h, self.h, self.MODES[mode]))
 
     def get_mode(self):

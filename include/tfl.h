@@ -1,5 +1,5 @@
 /*
- * libtfl -- C ABI of the B200-native Eulerian fluid step (drop-in for the tfluids
+ * libtfl -- C ABI of the H100-native Eulerian fluid step (drop-in for the tfluids
  * operators that FluidNet's `tfluids.simulate` calls).
  *
  * Every entry point replaces one reference `lua_CFunction` (registered in
@@ -207,7 +207,7 @@ int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
                          tfl_cnn** out);
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* cnn);
 /* Arithmetic of the convolution stack: 0 = fp32 FMA on the CUDA cores; 1 = TF32 tensor cores
- * (tcgen05, fp32 accumulate); 2 = 3xTF32 tensor cores (error-compensated split, fp32-class
+ * (wgmma, fp32 accumulate); 2 = 3xTF32 tensor cores (error-compensated split, fp32-class
  * accuracy; the default where available).  Modes 1 and 2 cover the 3-D 'default' architecture. */
 int tfl_cnn_set_mode(tfl_ctx* ctx, tfl_cnn* cnn, int mode);
 int tfl_cnn_get_mode(const tfl_cnn* cnn);

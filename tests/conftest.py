@@ -9,7 +9,7 @@ if ROOT not in sys.path:
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def pytest_collection_modifyitems(config, items):
@@ -34,7 +34,5 @@ def orc():
 
 @pytest.fixture(scope="session")
 def ref():
-    import oracle
-    if not oracle.have_reference():
-        pytest.skip("oracle/_ref not built (no /root/reference here)")
-    return oracle.Reference()
+    import ref_record
+    return ref_record.reference()

@@ -29,7 +29,7 @@ def test_library_exports_every_symbol():
     for s in header_symbols():
         assert hasattr(lib, s), "libtfl.so does not export " + s
     lib.tfl_version.restype = ctypes.c_char_p
-    assert b"sm_100a" in lib.tfl_version()
+    assert b"sm_90a" in lib.tfl_version()
     assert lib.tfl_advect_method_from_string(b"maccormackOurs") == 5
     assert lib.tfl_advect_method_from_string(b"bogus") == -1
 

@@ -1,6 +1,6 @@
 """bench.py pieces that can be checked without a GPU: the synthetic problem of the measured arm is built
 by the product's own host code (no oracle on that path) and equals what the oracle's builder gives, and
-the reference arm prints the contract's JSON line."""
+the reference arm prints the contract's JSON line, and --dump-outputs writes what it promises."""
 import json
 import os
 import subprocess
@@ -36,12 +36,21 @@ def test_reference_arm_json_line():
     assert d["cpu_baseline"]["kind"] in ("reference", "port")
 
 
-def test_roofline_traffic_is_read_from_the_tracked_ncu_table():
-    """bench.py's roofline.traffic comes from profiles/r02_advect_ncu_raw.csv (the ncu --set full capture of the
-    current advection kernels), never from a literal: the parser finds the kernel and gives DRAM bytes per launch."""
+def test_dump_outputs_writes_float32_within_the_limit(tmp_path, monkeypatch):
+    """--dump-outputs: whole fields under the limit; above it, the same seeded sample of each field every run."""
+    import torch
     sys.path.insert(0, ROOT)
     import bench
-    traffic, src = bench.ncu_traffic([r"k_advect_vel_tile"])
-    assert src == os.path.join("profiles", "r02_advect_ncu_raw.csv")
-    assert 5e6 < traffic < 2e8, traffic           # bytes per launch at 128^3 (algorithmic: 58.7 MB)
-    assert bench.ncu_traffic([r"no_such_kernel"]) == (None, None)
+    f = {"p": torch.arange(1000, dtype=torch.float32).reshape(1, 1, 10, 10, 10), "U": torch.ones(1, 3, 10, 10, 10)}
+    bench.dump_outputs(str(tmp_path / "whole"), f)
+    p = np.load(tmp_path / "whole" / "p.npy")
+    assert p.dtype == np.float32 and p.shape == (1, 1, 10, 10, 10) and np.array_equal(p.ravel(), np.arange(1000))
+    monkeypatch.setattr(bench, "DUMP_LIMIT_BYTES", 4000)
+    for d in ("a", "b"):
+        bench.dump_outputs(str(tmp_path / d), f)
+    total = sum(os.path.getsize(os.path.join(tmp_path, "a", n)) - 128 for n in os.listdir(tmp_path / "a"))
+    assert total <= 4000
+    for n in ("p", "p_index", "U", "U_index"):
+        assert np.array_equal(np.load(tmp_path / "a" / (n + ".npy")), np.load(tmp_path / "b" / (n + ".npy")))
+    idx = np.load(tmp_path / "a" / "p_index.npy")
+    assert idx.dtype == np.float64 and np.array_equal(np.load(tmp_path / "a" / "p.npy"), idx.astype(np.float32))

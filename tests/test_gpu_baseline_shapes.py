@@ -1,7 +1,7 @@
 """Parity at the shapes BASELINE.json names, on the kernels bench.py times.
 
 The per-operator tests use edges of 14-40 cells; the bench runs 64^3 / 128^3 grids, where other kernel
-variants are selected by shape (4-voxels-per-thread point-wise stages, full 128-lane tcgen05 conv rows,
+variants are selected by shape (4-voxels-per-thread point-wise stages, tensor-core conv rows,
 64-wide advection blocks, the clear-space advection path over a large obstacle-free interior).  These
 tests put exactly those launches against the CPU oracle (which finishes a 128^3 operator in < 2 s):
 

@@ -5,15 +5,14 @@ import numpy as np
 import pytest
 
 from oracle import api
+import ref_record
 from cases import bits_equal, describe_diff
 import pcg_cases
 
 
 @pytest.fixture(scope="module")
 def ref():
-    if not api.have_reference():
-        pytest.skip("oracle/_ref not built")
-    return api.Reference()
+    return ref_record.reference()
 
 
 @pytest.fixture(scope="module")

@@ -7,6 +7,7 @@ import pytest
 
 import oracle
 from oracle import api
+import ref_record
 from cases import bits_equal, describe_diff
 from fluidnet_b200 import synth
 
@@ -18,9 +19,7 @@ METHODS = list(oracle.ADVECT_METHODS)
 
 @pytest.fixture(scope="module")
 def ref():
-    if not api.have_reference():
-        pytest.skip("oracle/_ref not built")
-    return api.Reference()
+    return ref_record.reference()
 
 
 def fields(shape, is3d, seed):

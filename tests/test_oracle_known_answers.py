@@ -10,16 +10,14 @@ import numpy as np
 import pytest
 
 import oracle
+import ref_record
 from cases import bits_equal, describe_diff
 
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden")
 
 
 def backends():
-    out = [oracle.Oracle()]
-    if oracle.have_reference():
-        out.append(oracle.Reference())
-    return out
+    return [oracle.Oracle(), ref_record.reference()]
 
 
 @pytest.mark.parametrize("be", backends(), ids=lambda b: b.name)

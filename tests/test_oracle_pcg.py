@@ -10,6 +10,7 @@ import pytest
 import oracle
 from oracle import api
 import pcg_cases
+import ref_record
 
 
 @pytest.fixture(scope="module")
@@ -19,9 +20,7 @@ def orc():
 
 @pytest.mark.parametrize("is3d", [True, False])
 def test_components_match_reference(orc, is3d):
-    if not api.have_reference():
-        pytest.skip("oracle/_ref not built")
-    ref = api.Reference()
+    ref = ref_record.reference()
     for seed in range(3):
         flags, _, _ = pcg_cases.make(orc, is3d, nb=2, seed=seed)
         rng = np.random.default_rng(seed)

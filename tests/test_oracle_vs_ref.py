@@ -1,6 +1,6 @@
 """Pins the C restatement (oracle/tfluids_oracle.c) against the reference's own CPU code
 compiled in place (oracle/_ref): bit-exact on seeded inputs for every operator and
-advection method.  Skipped where /root/reference (hence oracle/_ref) is unavailable."""
+advection method.  Where oracle/_ref is not built, against its recorded answers (tests/ref_record.py)."""
 import numpy as np
 import pytest
 
