@@ -15,7 +15,8 @@
 //   * the three x-taps of a (dy, dz) pair share ONE A operand: B holds their weights side by
 //     side (N = 3 taps x 8 output channels = 24), so 9 wgmma (M=64, N=24, K=8, tf32 inputs,
 //     fp32 accumulate in registers) cover the 27 taps, and the x shift is applied in the
-//     epilogue: out[x] = D_{-1}[x-1] + D_0[x] + D_{+1}[x+1].  An M tile is 2 rows of 32
+//     epilogue: out[x] = D_{-1}[x-1] + D_0[x] + D_{+1}[x+1].  Layer 1 (3 channels, one plane)
+//     puts two (dy, dz) taps into the two K chunks instead, 5 wgmma (see Layout).  An M tile is 2 rows of 32
 //     x-positions; the accumulators go through a small shared-memory buffer per warpgroup
 //     so that every thread can read its x-1 / x+1 neighbours;
 //   * 3xTF32 mode (SPLIT): A and B are split into tf32 "hi" and fp32-residual "lo" parts;
@@ -51,6 +52,32 @@ template <bool SPLIT> struct Tile {
   static constexpr int PLANE_BYTES = POS * 16;
   static constexpr int MTILES = TZ * RB;
 };
+
+// Shared-memory layout of one layer: the staged planes (hi, then lo when SPLIT), the B groups, the
+// accumulator staging buffer and the bias / tail constants.
+//   IN_PLANES == 2: planes [c0-3 | c4-7] (x hi/lo), 9 B groups, one (dz, dy) tap per group; K chunk 1
+//                   is the second channel group, one plane further (LBO = PLANE_BYTES).
+//   IN_PLANES == 1: (layer 1, 3 channels) every plane is followed by 64 zero positions and the two K
+//                   chunks of a group are two taps of the same 4 channels (layer1_dz / _dy), so 5 B groups
+//                   cover the 9 (dz, dy) taps.
+template <int IN_PLANES, bool SPLIT> struct Layout {
+  using T = Tile<SPLIT>;
+  static constexpr int NB = SPLIT ? 48 : 32;
+  static constexpr int GROUPS = IN_PLANES == 1 ? 5 : kGroups;
+  static constexpr int ZERO_BYTES = IN_PLANES == 1 ? 64 * 16 : 0;
+  static constexpr int PSTRIDE = T::PLANE_BYTES + ZERO_BYTES;     // bytes between staged planes
+  static constexpr int LO_OFF = IN_PLANES * PSTRIDE;               // hi -> lo operand (SPLIT)
+  static constexpr int A_BYTES = (SPLIT ? 2 : 1) * LO_OFF;
+  static constexpr int B_GROUP_BYTES = 2 * NB * 16;
+  static constexpr int B_BYTES = GROUPS * B_GROUP_BYTES;
+  static constexpr int BYTES = A_BYTES + B_BYTES + 2 * 64 * kDPitch * 4 + 4 * 96;
+};
+
+// Layer 1 (one 4-channel plane): group gi's K chunk 0 is tap (layer1_dz(gi), layer1_dy(gi)); K chunk 1
+// is the tap one z-plane further for gi < 3 (dz = -1 / 0 pairs), one row further for gi == 3
+// ((dz, dy) = (1, -1) / (1, 0)), and zeros for gi == 4 (the single tap (1, 1)).
+__host__ __device__ constexpr int layer1_dz(int gi) { return gi < 3 ? -1 : 1; }
+__host__ __device__ constexpr int layer1_dy(int gi) { return gi < 3 ? gi - 1 : (gi == 3 ? -1 : 1); }
 
 __device__ __forceinline__ uint32_t smem_u32(const void* p) {
   return (uint32_t)__cvta_generic_to_shared(p);
@@ -113,13 +140,10 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
            ConvTcGeo g) {
   extern __shared__ __align__(1024) uint8_t smem[];
   using T = Tile<SPLIT>;
-  constexpr int NB = SPLIT ? 48 : 32;
-  constexpr int A_BYTES = (SPLIT ? 4 : 2) * T::PLANE_BYTES;
-  constexpr int B_GROUP_BYTES = 2 * NB * 16;
-  constexpr int B_BYTES = kGroups * B_GROUP_BYTES;
+  using L = Layout<IN_PLANES, SPLIT>;
   uint8_t* sA = smem;
-  uint8_t* sB = smem + A_BYTES;
-  float* sD = (float*)(smem + A_BYTES + B_BYTES);            // [2 warpgroups][64][kDPitch]
+  uint8_t* sB = smem + L::A_BYTES;
+  float* sD = (float*)(smem + L::A_BYTES + L::B_BYTES);      // [2 warpgroups][64][kDPitch]
   float* sTail = sD + 2 * 64 * kDPitch;                      // bias[8] (+ w4[64] b4[8] w5[8] b5[1] when FINAL)
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
@@ -144,8 +168,7 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
       const long long go = ((long long)gz * g.py + gy) * g.px + gx;
 #pragma unroll
       for (int h = 0; h < IN_PLANES; h++)
-        cp_async16(smem_u32(sA + h * T::PLANE_BYTES + idx * 16), inb + h * plane_g + go);
-      if (IN_PLANES == 1) *(float4*)(sA + T::PLANE_BYTES + idx * 16) = make_float4(0.f, 0.f, 0.f, 0.f);
+        cp_async16(smem_u32(sA + h * L::PSTRIDE + idx * 16), inb + h * plane_g + go);
     }
   } else {
     // 3xTF32: the hi/lo split happens in registers on the way in.  All loads are issued
@@ -169,20 +192,21 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
       const int idx = tid + it * kThreads;
       if (idx < T::POS) {
 #pragma unroll
-        for (int h = 0; h < 2; h++) {
-          float4 hi = make_float4(0.f, 0.f, 0.f, 0.f), lo = hi;
-          if (h < IN_PLANES) {
-            const float4 w = v[it][h < IN_PLANES ? h : 0];
-            hi = tf32_hi(w);
-            lo = make_float4(w.x - hi.x, w.y - hi.y, w.z - hi.z, w.w - hi.w);
-          }
-          *(float4*)(sA + h * T::PLANE_BYTES + idx * 16) = hi;
-          *(float4*)(sA + (2 + h) * T::PLANE_BYTES + idx * 16) = lo;
+        for (int h = 0; h < IN_PLANES; h++) {
+          const float4 w = v[it][h];
+          const float4 hi = tf32_hi(w);
+          const float4 lo = make_float4(w.x - hi.x, w.y - hi.y, w.z - hi.z, w.w - hi.w);
+          *(float4*)(sA + h * L::PSTRIDE + idx * 16) = hi;
+          *(float4*)(sA + L::LO_OFF + h * L::PSTRIDE + idx * 16) = lo;
         }
       }
     }
   }
-  for (int i = tid; i < B_BYTES / 16; i += kThreads) cp_async16(smem_u32(sB + i * 16), (const float4*)wB + i);
+  // Layer 1's single-tap group reads its K chunk 1 from these zeros (its B rows are zero too, but
+  // 0 * NaN would not be).
+  for (int i = tid; i < L::ZERO_BYTES / 16 * (SPLIT ? 2 : 1); i += kThreads)
+    *(float4*)(sA + (i >> 6) * L::PSTRIDE + T::PLANE_BYTES + (i & 63) * 16) = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = tid; i < L::B_BYTES / 16; i += kThreads) cp_async16(smem_u32(sB + i * 16), (const float4*)wB + i);
   const int n_tail = FINAL ? (8 + 64 + 8 + 8 + 1) : 8;
   for (int i = tid; i < n_tail; i += kThreads) sTail[i] = (i < 8) ? bias[i] : tail[i - 8];
   asm volatile("cp.async.commit_group;" ::: "memory");
@@ -195,7 +219,7 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   // ---- warpgroup wg takes M tiles t = wg, wg + 2, ... ------------------------------------
   const int wg = warp >> 2, wq = warp & 3;
   const uint32_t sA_u = smem_u32(sA), sB_u = smem_u32(sB);
-  constexpr uint32_t LO_PLANES_16 = (uint32_t)(2 * T::PLANE_BYTES) >> 4;
+  constexpr uint32_t LO_16 = (uint32_t)L::LO_OFF >> 4;
   float* myD = sD + wg * 64 * kDPitch;
   const float* sBias = sTail;
   const int tw = tid & 127, p = tw >> 1, half = tw & 1;     // epilogue: position p, channels 4*half..+3
@@ -207,14 +231,20 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
     float acc[SPLIT ? 24 : 12] = {}, acl[12] = {};
     asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-    for (int gi = 0; gi < kGroups; gi++) {
-      const int dz = gi / 3 - 1, dy = gi % 3 - 1;
-      const uint32_t a_addr = sA_u + toff + (uint32_t)((((1 + dz) * T::PY + (1 + dy)) * kTX) * 16);
-      const uint64_t da = make_desc(a_addr, T::PLANE_BYTES, 128);
-      const uint64_t db = make_desc(sB_u + gi * B_GROUP_BYTES, NB * 16, 128);
+    for (int gi = 0; gi < L::GROUPS; gi++) {
+      const int dz = IN_PLANES == 1 ? layer1_dz(gi) : gi / 3 - 1;
+      const int dy = IN_PLANES == 1 ? layer1_dy(gi) : gi % 3 - 1;
+      const uint32_t a_off = toff + (uint32_t)((((1 + dz) * T::PY + (1 + dy)) * kTX) * 16);
+      // offset of K chunk 1 from chunk 0 (see Layout)
+      const uint32_t lbo = IN_PLANES == 2 ? (uint32_t)T::PLANE_BYTES
+                         : gi < 3         ? (uint32_t)(T::PY * kTX * 16)
+                         : gi == 3        ? (uint32_t)(kTX * 16)
+                                          : (uint32_t)T::PLANE_BYTES - a_off;
+      const uint64_t da = make_desc(sA_u + a_off, lbo, 128);
+      const uint64_t db = make_desc(sB_u + gi * L::B_GROUP_BYTES, L::NB * 16, 128);
       if constexpr (SPLIT) {
         wgmma_n48(acc, da, db, gi > 0 ? 1u : 0u);
-        wgmma_n24(acl, da + LO_PLANES_16, db, gi > 0 ? 1u : 0u);
+        wgmma_n24(acl, da + LO_16, db, gi > 0 ? 1u : 0u);
       } else {
         wgmma_n24(acc, da, db, gi > 0 ? 1u : 0u);
       }
@@ -269,19 +299,21 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
         hh[o] = half ? other : h[o];
         hh[4 + o] = half ? h[o] : other;
       }
-      const float* w4 = sTail + 8;      // [o][c]
-      const float* b4 = w4 + 64;
-      const float* w5 = b4 + 8;
-      const float b5 = w5[8];
-      float pacc = b5;
+      // The two threads of a position each take 4 of the 8 hidden channels of the 1x1x1 layers.
+      const float* w4 = sTail + 8 + 32 * half;        // rows 4 half .. 4 half + 3 of w4[o][c]
+      const float* b4 = sTail + 8 + 64 + 4 * half;
+      const float* w5 = sTail + 8 + 64 + 8 + 4 * half;
+      const float b5 = sTail[8 + 64 + 8 + 8];
+      float part = 0.0f;
 #pragma unroll
-      for (int o = 0; o < 8; o++) {
+      for (int o = 0; o < 4; o++) {
         float a = b4[o];
 #pragma unroll
         for (int c = 0; c < 8; c++) a = fmaf(hh[c], w4[o * 8 + c], a);
         a = a > 0.0f ? a : 0.0f;
-        pacc = fmaf(a, w5[o], pacc);
+        part = fmaf(a, w5[o], part);
       }
+      const float pacc = b5 + (part + __shfl_xor_sync(0xffffffffu, part, 1));
       if (valid && half == 0) p_net[(long long)b * g.nz * g.ny * g.nx + ((long long)zg * g.ny + yg) * g.nx + xg] = pacc;
     }
     wg_barrier(1 + wg);                                 // myD is rewritten by the next tile
@@ -296,8 +328,7 @@ template <int IN_PLANES, bool FINAL, bool SPLIT>
 void launch_one(const float4* in, float4* out, float* p_net, const float* wB, const float* bias,
                 const float* tail, const ConvTcGeo& g, cudaStream_t st) {
   using T = Tile<SPLIT>;
-  constexpr int NB = SPLIT ? 48 : 32;
-  const size_t smem = (size_t)(SPLIT ? 4 : 2) * T::PLANE_BYTES + kGroups * 2 * NB * 16 + 2 * 64 * kDPitch * 4 + 4 * 96;
+  const size_t smem = Layout<IN_PLANES, SPLIT>::BYTES;
   auto kern = k_conv3_tc<IN_PLANES, FINAL, SPLIT>;
   static unsigned long long configured = 0;       // per device (function attributes are)
   int dev = 0;
@@ -336,13 +367,24 @@ void conv_tc_set_debug(long long* dev_buf) { cudaMemcpyToSymbol(g_tc_dbg, &dev_b
 int conv_tc_b_floats(int split) { return kGroups * 2 * (split ? 48 : 32) * 4; }
 
 // Host-side packing of one layer's weights [cout=8][cin][3][3][3] into the B operand blocks
-// (tf32 "hi" truncation and fp32 residual "lo" when split).
+// (tf32 "hi" truncation and fp32 residual "lo" when split).  A block is [K chunk][NB][4 channels].
+// cin > 4: block dz * 3 + dy holds tap (dz, dy), channels 4 kc .. 4 kc + 3 in K chunk kc.
+// cin <= 4 (layer 1): blocks 0-4 hold the tap pairs of layer1_dz / layer1_dy, channels 0-3 in both
+// K chunks; block 4's K chunk 1 stays zero.
 void conv_tc_pack_weights(const float* w, int cin, int split, float* out) {
   const int NB = split ? 48 : 32;
   for (int i = 0; i < kGroups * 2 * NB * 4; i++) out[i] = 0.0f;
   for (int dz = 0; dz < 3; dz++)
     for (int dy = 0; dy < 3; dy++) {
-      float* blk = out + (size_t)(dz * 3 + dy) * 2 * NB * 4;
+      int blk_i = dz * 3 + dy, kc0 = 0;
+      if (cin <= 4) {
+        if (dz < 2) {
+          blk_i = dy; kc0 = dz;                 // (dz, dy) = (-1, dy) / (0, dy)
+        } else {
+          blk_i = dy < 2 ? 3 : 4; kc0 = dy < 2 ? dy : 0;   // (1, -1) / (1, 0), then (1, 1) alone
+        }
+      }
+      float* blk = out + (size_t)blk_i * 2 * NB * 4;
       for (int kx = 0; kx < 3; kx++)
         for (int o = 0; o < 8; o++)
           for (int c = 0; c < cin; c++) {
@@ -350,9 +392,9 @@ void conv_tc_pack_weights(const float* w, int cin, int split, float* out) {
             union { float f; uint32_t u; } hi;
             hi.f = v;
             if (split) hi.u &= 0xFFFFE000u;
-            const int n = kx * 8 + o;
-            blk[((c >> 2) * NB + n) * 4 + (c & 3)] = hi.f;
-            if (split) blk[((c >> 2) * NB + 24 + n) * 4 + (c & 3)] = v - hi.f;
+            const int n = kx * 8 + o, kc = kc0 + (c >> 2);
+            blk[(kc * NB + n) * 4 + (c & 3)] = hi.f;
+            if (split) blk[(kc * NB + 24 + n) * 4 + (c & 3)] = v - hi.f;
           }
     }
 }
