@@ -1100,6 +1100,60 @@ float tfl_debug_last_advect_kernel_ms(tfl_ctx* ctx) {
 // Undocumented debugging hook (not in tfl.h): per-CTA phase timestamps of the tensor-core conv.
 int tfl_debug_conv_timestamps(void* dev_buf) { conv_tc_set_debug((long long*)dev_buf); return 0; }
 
+// Undocumented test hooks (not in tfl.h): one tensor-core 3x3x3 layer on caller-owned buffers.
+// tfl_debug_conv_tc_layout: the padded pitches (px, py) of make_conv_tc_geo, so callers can lay out
+// in / out ([nb][2 planes][nz+2][py][px] float4); p_net is plain [nb][nz][ny][nx].
+int tfl_debug_conv_tc_layout(int nb, int nz, int ny, int nx, int32_t out[2]) {
+  const ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  out[0] = g.px;
+  out[1] = g.py;
+  return 0;
+}
+
+// tfl_debug_conv3_tc: weights [8][cin][3][3][3] and bias [8] on the host, packed with conv_tc_pack_weights;
+// tail (final layer only): w4[8][8], b4[8], w5[8], b5[1] as in tfl_cnn_create_graph.  Output planes
+// [z_lo, z_hi) only.  Synchronises before returning.
+int tfl_debug_conv3_tc(tfl_ctx* ctx, const float* in, float* out, float* p_net, const float* w_host,
+                       const float* bias_host, const float* tail_host, int cin, int final_layer, int split,
+                       int nb, int nz, int ny, int nx, int z_lo, int z_hi) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (cin != 3 && cin != 8) return fail(ctx, "debug_conv3_tc: cin must be 3 or 8 (got %d)", cin);
+  if (final_layer && cin != 8) return fail(ctx, "debug_conv3_tc: the final layer takes 8 channels");
+  if (final_layer && (!tail_host || !p_net)) return fail(ctx, "debug_conv3_tc: the final layer needs tail and p_net");
+  if (!final_layer && !out) return fail(ctx, "debug_conv3_tc: nil out");
+  if (!in || !w_host || !bias_host) return fail(ctx, "debug_conv3_tc: nil argument");
+  if (nb < 1 || nz < 1 || ny < 1 || nx < 1) return fail(ctx, "debug_conv3_tc: bad grid %dx%dx%dx%d", nb, nz, ny, nx);
+  if (z_lo < 0 || z_hi > nz || z_lo >= z_hi) return fail(ctx, "debug_conv3_tc: z range [%d, %d) not in [0, %d]", z_lo, z_hi, nz);
+  ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  g.z_lo = z_lo;
+  g.z_hi = z_hi;
+  std::vector<float> packed(conv_tc_b_floats(split));
+  conv_tc_pack_weights(w_host, cin, split, packed.data());
+  float *wB = nullptr, *bias = nullptr, *tail = nullptr;
+  auto release = [&]() {
+    if (wB) cudaFree(wB);
+    if (bias) cudaFree(bias);
+    if (tail) cudaFree(tail);
+  };
+  const int n_tail = 64 + 8 + 8 + 1;
+  if (cudaMalloc((void**)&wB, packed.size() * 4) != cudaSuccess || cudaMalloc((void**)&bias, 8 * 4) != cudaSuccess ||
+      (final_layer && cudaMalloc((void**)&tail, n_tail * 4) != cudaSuccess)) {
+    release();
+    return fail(ctx, "debug_conv3_tc: cudaMalloc failed");
+  }
+  cudaMemcpy(wB, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice);
+  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
+  if (final_layer) cudaMemcpy(tail, tail_host, n_tail * 4, cudaMemcpyHostToDevice);
+  launch_conv3_tc(in, out, p_net, wB, bias, tail, cin == 3 ? 1 : 2, final_layer, split, g, ctx->stream);
+  const int rc = check_launch(ctx, "debug_conv3_tc");
+  const cudaError_t se = cudaStreamSynchronize(ctx->stream);
+  release();
+  if (rc) return rc;
+  if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc: %s", cudaGetErrorString(se));
+  return 0;
+}
+
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);

@@ -20,14 +20,15 @@ from fluidnet_b200 import synth
 pytestmark = pytest.mark.gpu
 
 
-def make_batch(n, is3d, plume=True, geometry=True, amp=3.0):
-    nz = n if is3d else 1
-    flags = synth.make_flags(n, n, nz, is3d, nb=1, geometry=geometry)
-    U = synth.make_smooth_velocity(flags, is3d, amp=amp)
+def make_batch(n, is3d, plume=True, geometry=True, amp=3.0, shape=None, nb=1, seed=1234):
+    """An n^2 / n^3 grid, or shape = (nz, ny, nx); with nb > 1 every entry has its own velocity field."""
+    nz, ny, nx = shape if shape is not None else ((n if is3d else 1), n, n)
+    flags = synth.make_flags(nx, ny, nz, is3d, nb=nb, geometry=geometry)
+    U = synth.make_smooth_velocity(flags, is3d, amp=amp, seed=seed)
     oracle.Oracle().setWallBcsForward(U, flags)
     batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
     if plume:
-        oracle.create_plume_bcs(batch, [1.0], n / 128.0 * 4, 0.15)
+        oracle.create_plume_bcs(batch, [1.0], nx / 128.0 * 4, 0.15)
     return batch
 
 
@@ -64,14 +65,36 @@ def test_step_jacobi_bit_exact(orc, is3d, n, fused):
 MODE_TOL = {"fp32": 2e-5, "tf32x3": 2e-5, "tf32": 3e-3}
 
 
-@pytest.mark.parametrize("is3d,n,mode", [(True, 24, "fp32"), (True, 24, "tf32x3"), (True, 24, "tf32"),
-                                         (True, 37, "tf32x3"), (True, 37, "tf32"), (False, 48, "fp32")],
-                         ids=["3d24-fp32", "3d24-tf32x3", "3d24-tf32", "3d37-tf32x3", "3d37-tf32", "2d48-fp32"])
-def test_cnn_projection_forward(orc, is3d, n, mode):
+FORWARD_CASES = {          # id: (is3d, (nz, ny, nx), nb, mode, zero_u_entry)
+    "3d24-fp32": (True, (24, 24, 24), 1, "fp32", None),
+    "3d24-tf32x3": (True, (24, 24, 24), 1, "tf32x3", None),
+    "3d24-tf32": (True, (24, 24, 24), 1, "tf32", None),
+    "3d37-tf32x3": (True, (37, 37, 37), 1, "tf32x3", None),
+    "3d37-tf32": (True, (37, 37, 37), 1, "tf32", None),
+    "2d48-fp32": (False, (1, 48, 48), 1, "fp32", None),
+    # non-cubic, nb = 2: odd nz (per-thread atomics in k_cnn_mask_stats) and even nz (block sums)
+    "3d13x18x23-nb2-fp32": (True, (13, 18, 23), 2, "fp32", None),
+    "3d13x18x23-nb2-tf32x3": (True, (13, 18, 23), 2, "tf32x3", None),
+    "3d13x18x23-nb2-tf32": (True, (13, 18, 23), 2, "tf32", None),
+    "3d10x21x34-nb2-fp32": (True, (10, 21, 34), 2, "fp32", None),
+    "3d10x21x34-nb2-tf32x3": (True, (10, 21, 34), 2, "tf32x3", None),
+    "3d10x21x34-nb2-tf32": (True, (10, 21, 34), 2, "tf32", None),
+    # entry 0 has UDiv = 0, so its input scale clamps to the threshold; entry 1 does not
+    "3d12x16x20-nb2-zeroU-tf32x3": (True, (12, 16, 20), 2, "tf32x3", 0),
+    "2d40x56-nb2-fp32": (False, (1, 40, 56), 2, "fp32", None),
+}
+
+
+@pytest.mark.parametrize("case", list(FORWARD_CASES))
+def test_cnn_projection_forward(orc, case):
     """BASELINE config 2 (shape-reduced for the CPU oracle): model:forward only, for every
-    arithmetic mode of the conv stack (37^3 exercises partial tensor-core tiles)."""
+    arithmetic mode of the conv stack (37^3 exercises partial tensor-core tiles), on non-cubic grids and
+    batches of two.  Each batch entry is checked on its own: its scale, and p / U relative to its own max."""
     from gpu_backend import make_gpu_model
-    batch = make_batch(n, is3d, plume=False)
+    is3d, shape, nb, mode, zero_u = FORWARD_CASES[case]
+    batch = make_batch(0, is3d, plume=False, shape=shape, nb=nb)
+    if zero_u is not None:
+        batch["UDiv"][zero_u] = 0.0
     mnp = synth.make_model(is3d)
     p0 = (synth.make_density(batch["flags"], seed=77) - np.float32(0.5)) * np.float32(0.1)
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
@@ -80,11 +103,37 @@ def test_cnn_projection_forward(orc, is3d, n, mode):
     gm.set_mode(mode)
     gp, gU = gm.forward((torch.from_numpy(p0).cuda(), torch.from_numpy(batch["UDiv"]).cuda(),
                          torch.from_numpy(batch["flags"]).cuda()), return_scale=True)
-    assert abs(gm.last_scale[0] - wscale[0]) <= 1e-5 * wscale[0]
-    close(gp.cpu().numpy(), wp, MODE_TOL[mode], "p")
-    close(gU.cpu().numpy(), wU, MODE_TOL[mode], "U")
+    gp, gU = gp.cpu().numpy(), gU.cpu().numpy()
+    if zero_u is not None:
+        assert wscale[zero_u] == np.float32(1e-5) and wscale[1 - zero_u] > np.float32(1e-5)
+    for b in range(nb):
+        assert abs(gm.last_scale[b] - wscale[b]) <= 1e-5 * wscale[b], (b, gm.last_scale, wscale)
+        close(gp[b], wp[b], MODE_TOL[mode], "p[%d]" % b)
+        close(gU[b], wU[b], MODE_TOL[mode], "U[%d]" % b)
     # occupancy / wall logic is exact: every face the oracle zeroes is exactly zero here.
-    assert np.array_equal(gU.cpu().numpy() == 0, wU == 0)
+    assert np.array_equal(gU == 0, wU == 0)
+
+
+def test_cnn_model_state_across_shapes_and_modes():
+    """One model through grid changes (each reallocates its padded activation buffers), mode changes and new
+    inputs on the same grid: every result equals that of a fresh model for the same shape and mode, so the zero
+    borders of the activation buffers survive between calls."""
+    from gpu_backend import make_gpu_model
+    mnp = synth.make_model(True)
+    A, B = ((12, 16, 20), 1), ((9, 13, 31), 2)
+    gm = make_gpu_model(mnp)
+    for (shape, nb), mode, seed in ((A, "tf32x3", 0), (B, "tf32", 0), (A, "fp32", 0), (A, "tf32x3", 1),
+                                    (A, "tf32x3", 2), (B, "tf32x3", 1)):
+        batch = make_batch(0, True, plume=False, shape=shape, nb=nb, seed=1234 + seed)
+        p0 = (synth.make_density(batch["flags"], seed=77 + seed) - np.float32(0.5)) * np.float32(0.1)
+        inputs = (torch.from_numpy(p0).cuda(), torch.from_numpy(batch["UDiv"]).cuda(),
+                  torch.from_numpy(batch["flags"]).cuda())
+        gm.set_mode(mode)
+        fresh = make_gpu_model(mnp)
+        fresh.set_mode(mode)
+        what = "%s nb%d %s seed %d" % (shape, nb, mode, seed)
+        for got, want, k in zip(gm.forward(inputs), fresh.forward(inputs), ("p", "U")):
+            close(got.cpu().numpy(), want.cpu().numpy(), 1e-6, "%s %s" % (what, k))
 
 
 @pytest.mark.parametrize("fused", [False, True], ids=["ops", "fused"])
