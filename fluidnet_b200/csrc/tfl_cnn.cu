@@ -152,6 +152,40 @@ __global__ void k_pixel_shuffle(const float* __restrict__ in, float* __restrict_
   out[t] = __ldg(in + ((b * cin_total + ch) * nz + z) * (long long)ny * nx + (long long)y * nx + x);
 }
 
+// Join of the multi-resolution banks (lib/model.lua:297-318).  Bank i (1-based, i >= 2) is
+// [nb][c][nz / rz][ny / r][nx / r] with r = 2^(i-1) (rz = r in 3-D, 1 in 2-D), upsampled nearest to the
+// full grid on the fly.  concat: out is [nb][nbanks * c][nz][ny][nx] and bank i lands at channel offset
+// (i-1) c (bank 1 is already in place); add: out is [nb][c][nz][ny][nx], holds bank 1 and gets banks 2..N
+// added in bank order, as CAddTable does.
+struct BankPtrs {
+  const float* p[kMaxBankPtrs];
+};
+__global__ void k_bank_join(BankPtrs banks, int nbanks, float* __restrict__ out, int c, int nz, int ny, int nx,
+                            int is3d, int add, long long total) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const long long n = (long long)nz * ny * nx;
+  const int x = (int)(t % nx), y = (int)((t / nx) % ny), z = (int)((t / ((long long)nx * ny)) % nz);
+  const long long bc = t / n;                      // b * c + ch
+  const long long b = bc / c, ch = bc % c;
+  if (add) {
+    float v = out[t];
+    for (int i = 1; i < nbanks; i++) {
+      const int bx = nx >> i, by = ny >> i, bz = is3d ? nz >> i : nz;
+      const int zi = is3d ? z >> i : z;
+      v = v + __ldg(banks.p[i] + ((bc * bz + zi) * by + (y >> i)) * bx + (x >> i));
+    }
+    out[t] = v;
+  } else {
+    const long long cell = t % n;
+    for (int i = 1; i < nbanks; i++) {
+      const int bx = nx >> i, by = ny >> i, bz = is3d ? nz >> i : nz;
+      const int zi = is3d ? z >> i : z;
+      out[((b * nbanks + i) * c + ch) * n + cell] = __ldg(banks.p[i] + ((bc * bz + zi) * by + (y >> i)) * bx + (x >> i));
+    }
+  }
+}
+
 template <int COUT, int KS, bool IS3D>
 static bool conv_launch(const float* in, float* out, const float* w, const float* b, int cin, int act,
                         const Geo& g, cudaStream_t st) {
@@ -207,6 +241,15 @@ void launch_pixel_shuffle(const float* in, float* out, int nb, int n_out, int nz
                           cudaStream_t st) {
   const long long total = (long long)nb * n_out * nz * (is3d ? s : 1) * ny * s * nx * s;
   k_pixel_shuffle<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, out, n_out, nz, ny, nx, s, is3d, total);
+}
+int launch_bank_join(const float* const* banks, int nbanks, float* out, int nb, int c, int nz, int ny, int nx,
+                     int is3d, int add, cudaStream_t st) {
+  if (nbanks < 2 || nbanks > kMaxBankPtrs) return -1;
+  BankPtrs bp = {};
+  for (int i = 1; i < nbanks; i++) bp.p[i] = banks[i];
+  const long long total = (long long)nb * c * nz * ny * nx;
+  k_bank_join<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(bp, nbanks, out, c, nz, ny, nx, is3d, add, total);
+  return 1;
 }
 
 }  // namespace tfl

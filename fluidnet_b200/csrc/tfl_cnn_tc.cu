@@ -133,11 +133,14 @@ __device__ __forceinline__ float4 tf32_hi(float4 v) {
 
 __device__ long long* g_tc_dbg = nullptr;   // optional phase timestamps (tests/dbg only)
 
-template <int IN_PLANES, bool FINAL, bool SPLIT>
+// JOIN (final layer only): the input box is the sum of the banks of `js`, each staged from its own resolution
+// with nearest indexing (see TcJoinSrc), and the epilogue may write / add / read a partial sum (part_mode).
+template <int IN_PLANES, bool FINAL, bool SPLIT, bool JOIN = false>
 __global__ void __launch_bounds__(kThreads, 2)
 k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __restrict__ p_net,
            const float* __restrict__ wB, const float* __restrict__ bias, const float* __restrict__ tail,
-           ConvTcGeo g) {
+           ConvTcGeo g, TcJoinSrc js) {
+  static_assert(!JOIN || (FINAL && IN_PLANES == 2), "the join is the last 3x3x3 layer");
   extern __shared__ __align__(1024) uint8_t smem[];
   using T = Tile<SPLIT>;
   using L = Layout<IN_PLANES, SPLIT>;
@@ -158,7 +161,51 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   const long long batch_g = plane_g * 2;
   const int x0 = tx * 30, y0 = ty * T::TY, z0 = g.z_lo + tzb * T::TZ;         // padded coords of box origin
   const float4* inb = in + b * batch_g;
-  if (!SPLIT) {
+  if constexpr (JOIN) {
+    // Padded full-resolution coordinate g inside the grid -> bank coordinate ((g - 1) >> shift) + 1; outside,
+    // the bank's (0, 0, 0) border voxel, which is zero.  Banks are summed in order (CAddTable).
+    constexpr int PER = (T::POS + kThreads - 1) / kThreads;
+    float4 v[PER][2];
+#pragma unroll
+    for (int it = 0; it < PER; it++) {
+      const int idx = tid + it * kThreads;
+      const int l = idx & 31, r = idx >> 5;
+      const int yy = r % T::PY, zz = r / T::PY;
+      const int gx = x0 + l, gy = y0 + yy, gz = z0 + zz;
+      const bool interior = idx < T::POS && gx >= 1 && gx <= g.nx && gy >= 1 && gy <= g.ny && gz >= 1 && gz <= g.nz;
+      v[it][0] = make_float4(0.f, 0.f, 0.f, 0.f);
+      v[it][1] = v[it][0];
+      for (int k = 0; k < js.n; k++) {
+        const int sh = js.shift[k];
+        const int bx = interior ? ((gx - 1) >> sh) + 1 : 0;
+        const int by = interior ? ((gy - 1) >> sh) + 1 : 0;
+        const int bz = interior ? ((gz - 1) >> sh) + 1 : 0;
+        const long long plane_k = (long long)(js.nz[k] + 2) * js.py[k] * js.px[k];
+        const float4* src = (const float4*)js.p[k] + b * 2 * plane_k + ((long long)bz * js.py[k] + by) * js.px[k] + bx;
+        const float4 a0 = __ldg(src), a1 = __ldg(src + plane_k);
+        v[it][0] = make_float4(v[it][0].x + a0.x, v[it][0].y + a0.y, v[it][0].z + a0.z, v[it][0].w + a0.w);
+        v[it][1] = make_float4(v[it][1].x + a1.x, v[it][1].y + a1.y, v[it][1].z + a1.z, v[it][1].w + a1.w);
+      }
+    }
+#pragma unroll
+    for (int it = 0; it < PER; it++) {
+      const int idx = tid + it * kThreads;
+      if (idx < T::POS) {
+#pragma unroll
+        for (int h = 0; h < 2; h++) {
+          const float4 w = v[it][h];
+          if constexpr (SPLIT) {
+            const float4 hi = tf32_hi(w);
+            const float4 lo = make_float4(w.x - hi.x, w.y - hi.y, w.z - hi.z, w.w - hi.w);
+            *(float4*)(sA + h * L::PSTRIDE + idx * 16) = hi;
+            *(float4*)(sA + L::LO_OFF + h * L::PSTRIDE + idx * 16) = lo;
+          } else {
+            *(float4*)(sA + h * L::PSTRIDE + idx * 16) = w;
+          }
+        }
+      }
+    }
+  } else if (!SPLIT) {
     for (int idx = tid; idx < T::POS; idx += kThreads) {
       const int l = idx & 31, r = idx >> 5;
       const int yy = r % T::PY, zz = r / T::PY;
@@ -275,23 +322,48 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
     const float4 d0 = *(const float4*)(myD + p * kDPitch + 8 + 4 * half);
     const float4 dp = *(const float4*)(myD + pp * kDPitch + 16 + 4 * half);
     const float* bs = sBias + 4 * half;
-    float h[4];
-    h[0] = (dm.x + d0.x) + dp.x + bs[0];
-    h[1] = (dm.y + d0.y) + dp.y + bs[1];
-    h[2] = (dm.z + d0.z) + dp.z + bs[2];
-    h[3] = (dm.w + d0.w) + dp.w + bs[3];
-#pragma unroll
-    for (int o = 0; o < 4; o++) h[o] = h[o] > 0.0f ? h[o] : 0.0f;
     const int xg = x0 + xl - 1;                         // unpadded coordinates of this position's voxel
     const int yg = y0 + 2 * (t % T::RB) + ry;
     const int zg = z0 + t / T::RB;
     const bool valid = xl >= 1 && xl <= 30 && xg < g.nx && yg < g.ny && zg < g.z_hi;
+    float h[4];
+    bool tail_wanted = true;
+    if constexpr (JOIN) {
+      h[0] = (dm.x + d0.x) + dp.x;
+      h[1] = (dm.y + d0.y) + dp.y;
+      h[2] = (dm.z + d0.z) + dp.z;
+      h[3] = (dm.w + d0.w) + dp.w;
+      float4* part = (float4*)(js.partial + ((((long long)b * g.nz + zg) * g.ny + yg) * g.nx + xg) * 8 + 4 * half);
+      if (js.part_mode == 1 || js.part_mode == 2) {
+        tail_wanted = false;
+        if (valid) {
+          float4 o4 = make_float4(h[0], h[1], h[2], h[3]);
+          if (js.part_mode == 2) {
+            const float4 q = *part;
+            o4 = make_float4(o4.x + q.x, o4.y + q.y, o4.z + q.z, o4.w + q.w);
+          }
+          *part = o4;
+        }
+      } else if (js.part_mode == 3 && valid) {
+        const float4 q = *part;
+        h[0] += q.x; h[1] += q.y; h[2] += q.z; h[3] += q.w;
+      }
+#pragma unroll
+      for (int o = 0; o < 4; o++) h[o] += bs[o];
+    } else {
+      h[0] = (dm.x + d0.x) + dp.x + bs[0];
+      h[1] = (dm.y + d0.y) + dp.y + bs[1];
+      h[2] = (dm.z + d0.z) + dp.z + bs[2];
+      h[3] = (dm.w + d0.w) + dp.w + bs[3];
+    }
+#pragma unroll
+    for (int o = 0; o < 4; o++) h[o] = h[o] > 0.0f ? h[o] : 0.0f;
     if (!FINAL) {
       if (valid) {
         const long long o = b * batch_g + ((long long)(zg + 1) * g.py + (yg + 1)) * g.px + (xg + 1);
         out[o + half * plane_g] = make_float4(h[0], h[1], h[2], h[3]);
       }
-    } else {
+    } else if (tail_wanted) {          // uniform over the launch (part_mode)
       float hh[8];
 #pragma unroll
       for (int o = 0; o < 4; o++) {
@@ -324,12 +396,12 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   }
 }
 
-template <int IN_PLANES, bool FINAL, bool SPLIT>
+template <int IN_PLANES, bool FINAL, bool SPLIT, bool JOIN = false>
 void launch_one(const float4* in, float4* out, float* p_net, const float* wB, const float* bias,
-                const float* tail, const ConvTcGeo& g, cudaStream_t st) {
+                const float* tail, const ConvTcGeo& g, cudaStream_t st, const TcJoinSrc& js = TcJoinSrc{}) {
   using T = Tile<SPLIT>;
   const size_t smem = Layout<IN_PLANES, SPLIT>::BYTES;
-  auto kern = k_conv3_tc<IN_PLANES, FINAL, SPLIT>;
+  auto kern = k_conv3_tc<IN_PLANES, FINAL, SPLIT, JOIN>;
   static unsigned long long configured = 0;       // per device (function attributes are)
   int dev = 0;
   cudaGetDevice(&dev);
@@ -342,7 +414,26 @@ void launch_one(const float4* in, float4* out, float* p_net, const float* wB, co
   gg.ntz = ntz;
   gg.nty = (g.ny + T::TY - 1) / T::TY;
   dim3 grid(g.ntx, gg.nty, ntz * g.nb);
-  kern<<<grid, kThreads, smem, st>>>(in, out, p_net, wB, bias, tail, gg);
+  kern<<<grid, kThreads, smem, st>>>(in, out, p_net, wB, bias, tail, gg, js);
+}
+
+// 2x2x2 average of the first float4 plane (k_pool's summation order), zero fourth channel.
+__global__ void k_tc_pyramid(const float4* __restrict__ in, ConvTcGeo gi, float4* __restrict__ out, ConvTcGeo go,
+                             long long total) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const int x = (int)(t % go.nx), y = (int)((t / go.nx) % go.ny), z = (int)((t / ((long long)go.nx * go.ny)) % go.nz);
+  const long long b = t / ((long long)go.nx * go.ny * go.nz);
+  const float4* ib = in + b * 2 * (long long)(gi.nz + 2) * gi.py * gi.px;
+  float sx = 0.0f, sy = 0.0f, sz = 0.0f;
+  for (int dz = 0; dz < 2; dz++)
+    for (int dy = 0; dy < 2; dy++)
+      for (int dx = 0; dx < 2; dx++) {
+        const float4 v = __ldg(ib + ((long long)(2 * z + dz + 1) * gi.py + (2 * y + dy + 1)) * gi.px + (2 * x + dx + 1));
+        sx += v.x; sy += v.y; sz += v.z;
+      }
+  out[b * 2 * (long long)(go.nz + 2) * go.py * go.px + ((long long)(z + 1) * go.py + (y + 1)) * go.px + (x + 1)] =
+      make_float4(sx / 8.0f, sy / 8.0f, sz / 8.0f, 0.0f);
 }
 
 }  // namespace
@@ -397,6 +488,19 @@ void conv_tc_pack_weights(const float* w, int cin, int split, float* out) {
             if (split) blk[(kc * NB + 24 + n) * 4 + (c & 3)] = v - hi.f;
           }
     }
+}
+
+int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, const float* bias, const float* tail,
+                         int split, const ConvTcGeo& g, cudaStream_t st) {
+  if (src.n < 1 || src.n > kTcMaxBanks) return -1;
+  if (split) launch_one<2, true, true, true>(nullptr, nullptr, p_net, wB, bias, tail, g, st, src);
+  else launch_one<2, true, false, true>(nullptr, nullptr, p_net, wB, bias, tail, g, st, src);
+  return 1;
+}
+
+void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, cudaStream_t st) {
+  const long long total = (long long)gout.nb * gout.nz * gout.ny * gout.nx;
+  k_tc_pyramid<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float4*)in, gin, (float4*)out, gout, total);
 }
 
 int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, const float* bias,

@@ -24,4 +24,25 @@ int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, 
                     const float* tail, int in_planes, int final_layer, int split, const ConvTcGeo& g,
                     cudaStream_t st);
 
+// Join layer of the multi-resolution banks (lib/model.lua:292-318) on the tensor cores: the last 3x3x3 layer
+// reads its 8 input channels as the sum over src[0..n) of bank src[k] upsampled nearest by 2^shift[k], staged
+// straight from the bank's own padded buffer (geometry px / py / nz), so no full-resolution copy exists.
+//   part_mode 0: bias, ReLU and the 1x1x1 tail -> p_net (as launch_conv3_tc with final_layer);
+//   part_mode 1 / 2: write / add the x-tap-summed pre-activations to `partial` ([nb][nz][ny][nx][8] fp32), no
+//                    bias, no tail (the other banks of a 'concat' join);
+//   part_mode 3: add `partial` before the bias, then as part_mode 0.
+constexpr int kTcMaxBanks = 8;
+struct TcJoinSrc {
+  const float* p[kTcMaxBanks];
+  int px[kTcMaxBanks], py[kTcMaxBanks], nz[kTcMaxBanks], shift[kTcMaxBanks];
+  int n;
+  int part_mode;
+  float* partial;
+};
+int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, const float* bias, const float* tail,
+                         int split, const ConvTcGeo& g, cudaStream_t st);
+// Bank pyramid on the padded channels-last layout: out's interior = 2x2x2 average of in's interior, first
+// float4 plane only (the 3 input channels and a zero fourth).  Borders of out are left as they are (zero).
+void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, cudaStream_t st);
+
 }  // namespace tfl

@@ -104,6 +104,12 @@ void launch_pool(const float* in, float* out, int nbc, int nz, int ny, int nx, i
                  cudaStream_t st);
 void launch_pixel_shuffle(const float* in, float* out, int nb, int n_out, int nz, int ny, int nx, int s, int is3d,
                           cudaStream_t st);
+// Join of multi-resolution banks: banks[i] (i = 1 .. nbanks-1; banks[0] unused) is bank i+1 at 2^-i the
+// resolution of the full [nz][ny][nx] grid (z kept in 2-D), c channels; upsampled nearest and written at
+// channel offset i c of out [nb][nbanks c][n] (add == 0) or added in bank order to out [nb][c][n] (add == 1).
+constexpr int kMaxBankPtrs = 8;
+int launch_bank_join(const float* const* banks, int nbanks, float* out, int nb, int c, int nz, int ny, int nx,
+                     int is3d, int add, cudaStream_t st);
 
 // ---- tfl_pcg.cu: matrix-free PCG pressure solve ----
 struct PcgScratch {            // owned by the context, grow-only

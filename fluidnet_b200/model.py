@@ -10,7 +10,7 @@ import ctypes as C
 import numpy as np
 import torch
 
-from . import tfluids
+from . import _lib, tfluids
 from ._lib import TflError
 
 
@@ -23,10 +23,14 @@ def default_layers(is3D):
 
 class ProjectionModel:
     def __init__(self, layers, is3D, device=None, normalizeInputThreshold=1e-5, pool=None, up=None,
-                 poolType="avg", nonlinType="relu"):
+                 poolType="avg", nonlinType="relu", banks=None):
         """layers: [(weight ndarray [cout * up^d][cin][kz][ky][kx], bias ndarray [cout * up^d]), ...]
         pool / up: per-layer pooling and ConvolutionUpsample sizes of the 'tog' graph (lib/model.lua:164-226),
-        None = all 1 ('default', 'yang'); poolType 'avg' | 'max'; nonlinType 'relu' | 'sigmoid'."""
+        None = all 1 ('default', 'yang'); poolType 'avg' | 'max'; nonlinType 'relu' | 'sigmoid'.
+        banks: multi-resolution banks (lib/model.lua:252-361), {"num": banksNum, "split_stage": banksSplitStage,
+        "join_stage": banksJoinStage, "aggregate": 'concat' | 'add'} (stages numbered from 1); layers[l] of a
+        banked stage (split_stage <= l + 1 < join_stage) is then a list of num (weight, bias) pairs, bank 1 first.
+        None: a single bank."""
         self.is3D = bool(is3D)
         self.threshold = float(normalizeInputThreshold)
         self.ctx = tfluids.context(device)
@@ -35,40 +39,69 @@ class ProjectionModel:
         up = [1] * n if up is None else [int(v) for v in up]
         assert len(pool) == n and len(up) == n
         assert poolType in ("avg", "max") and nonlinType in ("relu", "sigmoid")
+        self.banks = dict(banks) if banks is not None else None
+        if banks is not None:
+            assert banks["aggregate"] in ("concat", "add"), "banksAggregateMethod must be 'concat' or 'add'"
         self._keep = []
         cin = (C.c_int32 * n)()
         cout = (C.c_int32 * n)()
         ks = (C.c_int32 * n)()
         cpool = (C.c_int32 * n)(*pool)
         cup = (C.c_int32 * n)(*up)
-        wp = (C.POINTER(C.c_float) * n)()
-        bp = (C.POINTER(C.c_float) * n)()
-        for l, (w, b) in enumerate(layers):
-            w = np.ascontiguousarray(w, dtype=np.float32)
-            b = np.ascontiguousarray(b, dtype=np.float32)
-            assert w.ndim == 5 and b.ndim == 1 and b.shape[0] == w.shape[0]
-            assert w.shape[3] == w.shape[4] and w.shape[2] == (w.shape[4] if is3D else 1)
-            fan = up[l] ** (3 if is3D else 2)
-            assert w.shape[0] % fan == 0, "ConvolutionUpsample layer: cout must be a multiple of up^d"
+        # An invalid banks table is left to the library, which refuses it before it reads any weight.
+        banks_ok = banks is not None and banks["num"] >= 1 and 1 <= banks["split_stage"] < banks["join_stage"] < n
+        convs = []          # (w, b) stage by stage, bank 1 .. num for a banked stage
+        for l, layer in enumerate(layers):
+            per_bank = list(layer) if isinstance(layer[0], (tuple, list)) else [layer]
+            if banks_ok and banks["num"] > 1 and banks["split_stage"] <= l + 1 < banks["join_stage"]:
+                assert len(per_bank) == banks["num"], "stage %d needs one (weight, bias) per bank" % (l + 1)
+            elif banks is None or banks_ok:
+                assert len(per_bank) == 1, "stage %d is not banked" % (l + 1)
+            for bk, (w, b) in enumerate(per_bank):
+                w = np.ascontiguousarray(w, dtype=np.float32)
+                b = np.ascontiguousarray(b, dtype=np.float32)
+                assert w.ndim == 5 and b.ndim == 1 and b.shape[0] == w.shape[0]
+                assert w.shape[3] == w.shape[4] and w.shape[2] == (w.shape[4] if is3D else 1)
+                fan = up[l] ** (3 if is3D else 2)
+                assert w.shape[0] % fan == 0, "ConvolutionUpsample layer: cout must be a multiple of up^d"
+                shape = (w.shape[0] // fan, w.shape[1], w.shape[4])
+                if bk == 0:
+                    cout[l], cin[l], ks[l] = shape
+                else:
+                    assert shape == (cout[l], cin[l], ks[l]), "the banks of stage %d differ in shape" % (l + 1)
+                convs.append((w, b))
+        nc = len(convs)
+        wp = (C.POINTER(C.c_float) * nc)()
+        bp = (C.POINTER(C.c_float) * nc)()
+        for i, (w, b) in enumerate(convs):
             self._keep += [w, b]
-            cout[l], cin[l], ks[l] = w.shape[0] // fan, w.shape[1], w.shape[4]
-            wp[l] = w.ctypes.data_as(C.POINTER(C.c_float))
-            bp[l] = b.ctypes.data_as(C.POINTER(C.c_float))
+            wp[i] = w.ctypes.data_as(C.POINTER(C.c_float))
+            bp[i] = b.ctypes.data_as(C.POINTER(C.c_float))
         h = C.c_void_p()
-        self.ctx.check(self.ctx.lib.tfl_cnn_create_graph(self.ctx.h, 1 if is3D else 0, n, cin, cout, ks, cpool, cup,
-                                                         1 if poolType == "max" else 0,
-                                                         1 if nonlinType == "sigmoid" else 0, wp, bp, C.byref(h)))
+        args = (self.ctx.h, 1 if is3D else 0, n, cin, cout, ks, cpool, cup, 1 if poolType == "max" else 0,
+                1 if nonlinType == "sigmoid" else 0)
+        if banks is None:
+            self.ctx.check(self.ctx.lib.tfl_cnn_create_graph(*args, wp, bp, C.byref(h)))
+        else:
+            cb = _lib.CnnBanks(int(banks["num"]), int(banks["split_stage"]), int(banks["join_stage"]),
+                               1 if banks["aggregate"] == "add" else 0)
+            self.ctx.check(self.ctx.lib.tfl_cnn_create_banked(*args, C.byref(cb), wp, bp, C.byref(h)))
         self.h = h
         self.last_scale = None
 
     @classmethod
     def from_reference_file(cls, model_path, mconf_path=None, device=None):
         """A model saved by the reference (torch/lib/save_model.lua: Torch7 binary network + `_mconf.bin`),
-        read without Torch7 (fluidnet_b200/torch7.py).  Returns (model, mconf)."""
+        read without Torch7 (fluidnet_b200/torch7.py).  Returns (model, mconf).
+        The graph follows the mconf (modelType, nonlinType, poolType, the bank keys, normalizeInputThreshold), each
+        convolution goes to the (bank, stage) of its nngraph annotation, and the shapes are checked against the
+        architecture.  Options and modules the library does not compute raise ValueError naming them."""
         from . import torch7
         ref = torch7.load_reference_model(model_path, mconf_path)
-        thr = ref["mconf"].get("normalizeInputThreshold", 1e-5)
-        return cls(ref["layers"], ref["is3D"], device=device, normalizeInputThreshold=thr), ref["mconf"]
+        opts = torch7.model_options(ref["mconf"])
+        stages = torch7.graph_stages(ref["model"])
+        torch7.check_stages(stages, ref["mconf"], opts)
+        return cls(stages, ref["is3D"], device=device, **opts), ref["mconf"]
 
     MODES = {"fp32": 0, "tf32": 1, "tf32x3": 2}
 

@@ -81,11 +81,13 @@ def make_density(flags, seed=1235):
     return np.ascontiguousarray(d)
 
 
-def make_model(is3d=True, seed=4321, model_type="default"):
+def make_model(is3d=True, seed=4321, model_type="default", banks=None):
     """Random-init weights of a reference architecture (torch/lib/model.lua:164-226: 'default', 'tog',
     'yang'), Torch `reset` convention uniform +-1/sqrt(fan_in).  Inputs: pDiv, div, occupancy
     (lib/default_conf.lua:76-81).  'tog' layers carry pooling / ConvolutionUpsample sizes: the weights of
-    an upsampling layer have cout * up^d output channels."""
+    an upsampling layer have cout * up^d output channels.
+    banks: {"num", "split_stage", "join_stage", "aggregate"} (lib/model.lua:252-361); a banked stage's entry
+    in "layers" is then a list of num (weight, bias) pairs, and a 'concat' join stage takes num x the channels."""
     rs = np.random.RandomState(seed)
     extra = {}
     if model_type == "default":
@@ -105,17 +107,26 @@ def make_model(is3d=True, seed=4321, model_type="default"):
         extra = {"nonlinType": "sigmoid"}
     else:
         raise ValueError(model_type)
+    nbanks = banks["num"] if banks is not None else 1
     layers = []
     cin = 3
-    for cout, k, u in zip(osize, ksize, usize):
+    for stage, (cout, k, u) in enumerate(zip(osize, ksize, usize), start=1):
+        if nbanks > 1 and stage == banks["join_stage"] and banks["aggregate"] == "concat":
+            cin *= nbanks
+        banked = nbanks > 1 and banks["split_stage"] <= stage < banks["join_stage"]
         kz = k if is3d else 1
         fan_in = cin * kz * k * k
         bound = 1.0 / np.sqrt(fan_in)
         ct = cout * u ** (3 if is3d else 2)
-        w = ((rs.rand(ct, cin, kz, k, k) * 2 - 1) * bound).astype(np.float32)
-        b = ((rs.rand(ct) * 2 - 1) * bound).astype(np.float32)
-        layers.append((np.ascontiguousarray(w), np.ascontiguousarray(b)))
+        convs = []
+        for _ in range(nbanks if banked else 1):
+            w = ((rs.rand(ct, cin, kz, k, k) * 2 - 1) * bound).astype(np.float32)
+            b = ((rs.rand(ct) * 2 - 1) * bound).astype(np.float32)
+            convs.append((np.ascontiguousarray(w), np.ascontiguousarray(b)))
+        layers.append(convs if banked else convs[0])
         cin = cout
     out = {"is3D": is3d, "layers": layers}
     out.update(extra)
+    if banks is not None:
+        out["banks"] = dict(banks)
     return out

@@ -11,6 +11,7 @@ object; storages write their length and the raw elements; every other class (nn 
 writes one table with its fields.  torch.Cuda* tensors / storages are written like their Float versions.
 Host-side only, no GPU involved.
 """
+import re
 import struct
 
 import numpy as np
@@ -198,6 +199,10 @@ def conv_layers(model):
                 _walk(mod, set(), convs)
     else:
         _walk(model, set(), convs)
+    return _conv_layers_of(convs)
+
+
+def _conv_layers_of(convs):
     layers = []
     for c in convs:
         w = np.asarray(c["weight"], np.float32)
@@ -211,6 +216,170 @@ def conv_layers(model):
     return layers
 
 
+_CONV_STAGE = re.compile(r"^Bank (\d+): conv stage (\d+)$")
+
+# Node modules of the graphs this library computes (lib/model.lua:27-401 with the options model_options accepts).
+_ALLOWED = {
+    "nn.Identity", "nn.SelectTable", "nn.Select", "nn.Unsqueeze", "nn.JoinTable", "nn.CAddTable", "nn.ApplyScale",
+    "nn.Sequential", "tfluids.SetWallBcs", "tfluids.VelocityDivergence", "tfluids.FlagsToOccupancy",
+    "tfluids.VelocityUpdate", "tfluids.VolumetricUpSamplingNearest", "nn.SpatialUpSamplingNearest",
+    "nn.ReLU", "cudnn.ReLU", "nn.Sigmoid", "cudnn.Sigmoid",
+    "nn.SpatialConvolution", "nn.VolumetricConvolution", "cudnn.SpatialConvolution", "cudnn.VolumetricConvolution",
+    "nn.SpatialConvolutionUpsample", "nn.VolumetricConvolutionUpsample",
+    "nn.SpatialAveragePooling", "nn.VolumetricAveragePooling", "cudnn.SpatialAveragePooling",
+    "cudnn.VolumetricAveragePooling", "nn.SpatialMaxPooling", "nn.VolumetricMaxPooling", "cudnn.SpatialMaxPooling",
+    "cudnn.VolumetricMaxPooling",
+}
+
+# (osize, ksize, psize, usize) per modelType, lib/model.lua:163-239.
+_ARCH = {
+    (False, "default"): ([16, 16, 16, 16, 1], [3, 3, 3, 3, 1], [1] * 5, [1] * 5),
+    (False, "tog"): ([16, 32, 32, 64, 64, 32, 1], [5, 5, 5, 5, 1, 1, 3], [2, 1, 1, 1, 1, 1, 1], [1, 1, 1, 1, 1, 1, 2]),
+    (False, "yang"): ([6, 6, 6, 1], [3, 1, 1, 1], [1] * 4, [1] * 4),
+    (True, "default"): ([8, 8, 8, 8, 1], [3, 3, 3, 1, 1], [1] * 5, [1] * 5),
+    (True, "tog"): ([16, 16, 16, 16, 32, 32, 1], [3, 3, 3, 3, 1, 1, 3], [2, 2, 1, 1, 1, 1, 1], [1, 1, 1, 1, 1, 2, 2]),
+    (True, "yang"): ([6, 6, 6, 1], [3, 1, 1, 1], [1] * 4, [1] * 4),
+}
+
+
+def _node_modules(model):
+    """(module, annotation name or None) of every node of an nngraph gModule, in forward order."""
+    nodes = model.get("forwardnodes") if isinstance(model, T7Object) else None
+    out = []
+    for i in sorted(nodes or {}):
+        data = nodes[i].get("data") if isinstance(nodes[i], T7Object) else None
+        mod = data.get("module") if isinstance(data, dict) else None
+        if mod is None:
+            continue
+        ann = data.get("annotations")
+        out.append((mod, ann.get("name") if isinstance(ann, dict) else None))
+    return out
+
+
+def graph_stages(model):
+    """The convolutions of a reference gModule grouped by stage: [[(weight, bias) of bank 1, bank 2, ...], ...].
+    Each convolution is assigned from its node's annotation "Bank i: conv stage l" (lib/model.lua:337); the final
+    convolution has none.  Raises ValueError, naming it, for a module outside the graphs the library computes
+    (batch normalisation, gated or dilated convolutions, low-rank convolution Sequentials, ...)."""
+    mods = _node_modules(model)
+    if not mods:
+        raise ValueError("torch7 model: not an nngraph gModule (no forwardnodes)")
+    found = {}
+    final = []
+    for mod, name in mods:
+        cls = mod.cls if isinstance(mod, T7Object) else type(mod).__name__
+        if cls not in _ALLOWED:
+            raise ValueError("torch7 model: module %s is not supported by this library" % cls)
+        convs = []
+        _walk(mod, set(), convs)
+        if cls == "nn.Sequential":
+            if convs:
+                raise ValueError("torch7 model: a convolution inside nn.Sequential (low-rank convolution) is not "
+                                 "supported by this library")
+            continue
+        if not convs:
+            continue
+        layer = _conv_layers_of(convs)
+        if len(layer) != 1:
+            raise ValueError("torch7 model: module %s holds %d convolutions" % (cls, len(layer)))
+        m = _CONV_STAGE.match(name or "")
+        if m:
+            key = (int(m.group(2)), int(m.group(1)))
+            if key in found:
+                raise ValueError("torch7 model: two convolutions annotated %r" % name)
+            found[key] = layer[0]
+        else:
+            final.append(layer[0])
+    if len(final) != 1:
+        raise ValueError("torch7 model: expected one final (unannotated) convolution, found %d" % len(final))
+    n_stages = max([s for s, _ in found] + [0]) + 1
+    stages = []
+    for s in range(1, n_stages):
+        banks = sorted(b for st, b in found if st == s)
+        if not banks:
+            raise ValueError("torch7 model: no convolution is annotated with stage %d" % s)
+        if banks != list(range(1, len(banks) + 1)):
+            raise ValueError("torch7 model: stage %d has convolutions of banks %s" % (s, banks))
+        convs = [found[(s, b)] for b in banks]
+        stages.append(convs if len(convs) > 1 else convs[0])
+    stages.append(final[0])
+    return stages
+
+
+def model_options(mconf, n_stages=None):
+    """ProjectionModel keyword arguments for a reference mconf (lib/default_conf.lua, lib/model.lua:27-401):
+    pool / up from modelType, poolType, nonlinType, banks, normalizeInputThreshold.  Raises ValueError, naming
+    the option, for anything the library does not compute."""
+    def opt(key, default=None):
+        return mconf.get(key, default)
+
+    def refuse(what):
+        raise ValueError("mconf: %s is not supported by this library" % what)
+
+    if opt("addBatchNorm"):
+        refuse("addBatchNorm = true")
+    if opt("addPressureSkip"):
+        refuse("addPressureSkip = true")
+    chans = opt("inputChannels") or {"pDiv": True, "div": True, "flags": True}
+    on = sorted(k for k, v in chans.items() if v)
+    if on != ["div", "flags", "pDiv"]:
+        refuse("inputChannels = {%s} (only pDiv, div, flags)" % ", ".join(on))
+    if opt("normalizeInput", True) is not True:
+        refuse("normalizeInput = false")
+    if opt("normalizeInputFunc", "std") != "std":
+        refuse("normalizeInputFunc = %r" % opt("normalizeInputFunc"))
+    if opt("normalizeInputChan", "UDiv") != "UDiv":
+        refuse("normalizeInputChan = %r" % opt("normalizeInputChan"))
+    nonlin = opt("nonlinType", "relu")
+    if nonlin not in ("relu", "sigmoid"):
+        refuse("nonlinType = %r" % nonlin)
+    pool_type = opt("poolType", "avg")
+    if pool_type not in ("avg", "max"):
+        refuse("poolType = %r" % pool_type)
+    key = (bool(opt("is3D")), opt("modelType", "default"))
+    if key not in _ARCH:
+        refuse("modelType = %r" % key[1])
+    _, _, psize, usize = _ARCH[key]
+    out = {"pool": list(psize), "up": list(usize), "poolType": pool_type, "nonlinType": nonlin,
+           "normalizeInputThreshold": float(opt("normalizeInputThreshold", 1e-5))}
+    num = int(opt("banksNum", 1))
+    if num > 1:
+        if opt("banksType", "mres") != "mres":
+            refuse("banksType = %r" % opt("banksType"))
+        if opt("banksWeightShare"):
+            refuse("banksWeightShare = true")
+        agg = opt("banksAggregateMethod", "concat")
+        if agg not in ("concat", "add"):
+            refuse("banksAggregateMethod = %r" % agg)
+        out["banks"] = {"num": num, "split_stage": int(opt("banksSplitStage", 1)),
+                        "join_stage": int(opt("banksJoinStage", 3)), "aggregate": agg}
+    return out
+
+
+def check_stages(stages, mconf, options):
+    """The file's convolutions against the architecture the mconf describes (lib/model.lua:163-361)."""
+    is3d = bool(mconf.get("is3D"))
+    osize, ksize, _, usize = _ARCH[(is3d, mconf.get("modelType", "default"))]
+    if len(stages) != len(osize):
+        raise ValueError("torch7 model: %d stages, modelType %r has %d" % (len(stages), mconf.get("modelType"), len(osize)))
+    bk = options.get("banks")
+    cin = 3
+    for s, layer in enumerate(stages, start=1):
+        convs = layer if isinstance(layer, list) else [layer]
+        banked = bk is not None and bk["split_stage"] <= s < bk["join_stage"]
+        if len(convs) != (bk["num"] if banked else 1):
+            raise ValueError("torch7 model: stage %d has %d banks, the mconf gives %d" %
+                             (s, len(convs), bk["num"] if banked else 1))
+        if bk is not None and s == bk["join_stage"] and bk["aggregate"] == "concat":
+            cin *= bk["num"]
+        want = (osize[s - 1] * usize[s - 1] ** (3 if is3d else 2), cin, ksize[s - 1])
+        for w, _ in convs:
+            if (w.shape[0], w.shape[1], w.shape[4]) != want:
+                raise ValueError("torch7 model: stage %d convolution is (cout, cin, k) = %s, the mconf gives %s" %
+                                 (s, (w.shape[0], w.shape[1], w.shape[4]), want))
+        cin = osize[s - 1]
+
+
 def load_reference_model(model_path, mconf_path=None):
     """The pieces fluidnet_b200.model.ProjectionModel needs from a model saved by the reference
     (torch/lib/save_model.lua): {'is3D', 'layers', 'mconf'}.  `mconf_path` defaults to
@@ -219,4 +388,4 @@ def load_reference_model(model_path, mconf_path=None):
     model = load(model_path)
     if isinstance(model, dict) and "model" in model:
         model = model["model"]
-    return {"is3D": bool(mconf.get("is3D")), "layers": conv_layers(model), "mconf": mconf}
+    return {"is3D": bool(mconf.get("is3D")), "layers": conv_layers(model), "mconf": mconf, "model": model}

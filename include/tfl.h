@@ -205,10 +205,30 @@ int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
                          const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                          int nonlin_sigmoid, const float* const* weights, const float* const* biases,
                          tfl_cnn** out);
+/* Multi-resolution banks (lib/model.lua:252-361, banksType 'mres'): num = banksNum, split_stage =
+ * banksSplitStage, join_stage = banksJoinStage (stages numbered 1..n_layers, 1 <= split < join < n_layers),
+ * aggregate_add = 0 for banksAggregateMethod 'concat', 1 for 'add'. */
+typedef struct tfl_cnn_banks {
+  int32_t num, split_stage, join_stage, aggregate_add;
+} tfl_cnn_banks;
+/* tfl_cnn_create_graph with banks.  Before stage split, bank 1 is the hidden layer and bank i a 2x average
+ * pool of bank i-1; stages split .. join-1 run one convolution (+ shuffle, non-linearity, pooling) per bank;
+ * before stage join, bank i is upsampled (nearest) by 2^(i-1) and the banks are concatenated along the
+ * channels in bank order (cin[join-1] = num * cout[join-2]) or summed left to right.  cin, cout, ksize, pool
+ * and up are per stage; weights / biases list the convolutions stage by stage, bank 1 .. num for a banked
+ * stage.  banks == NULL or num == 1: exactly tfl_cnn_create_graph.  The grid at the split resolution must be
+ * divisible by 2^(num-1).  Banked models run on whole grids (not on z-slabs); the 3-D 'default' graph with
+ * split_stage 1 and join_stage 3 (num <= 8) runs on the tensor cores (3xTF32 by default), every other one on the
+ * fp32 path. */
+int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                          const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                          int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
+                          const float* const* biases, tfl_cnn** out);
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* cnn);
 /* Arithmetic of the convolution stack: 0 = fp32 FMA on the CUDA cores; 1 = TF32 tensor cores
  * (wgmma, fp32 accumulate); 2 = 3xTF32 tensor cores (error-compensated split, fp32-class
- * accuracy; the default where available).  Modes 1 and 2 cover the 3-D 'default' architecture. */
+ * accuracy; the default where available).  Modes 1 and 2 cover the 3-D 'default' architecture, single-bank
+ * or with banks split at stage 1 and joined at stage 3. */
 int tfl_cnn_set_mode(tfl_ctx* ctx, tfl_cnn* cnn, int mode);
 int tfl_cnn_get_mode(const tfl_cnn* cnn);
 /* model:forward({pDiv, UDiv, flags}) -> {p, U} (lib/model.lua:421-450).  threshold is
