@@ -27,6 +27,9 @@ struct tfl_ctx {
   char* arena = nullptr;
   size_t arena_bytes = 0;
   size_t arena_used = 0;
+  // Generation counters of the buffers a step graph captures: bumped whenever the buffer is freed and allocated
+  // again, so that tfl_step_graph_launch can refuse a graph that would replay freed memory.
+  unsigned long long arena_gen = 0;
   unsigned long long* counters = nullptr;   // [0] trace faults, [1] bad occupancy cells
   double* dscratch = nullptr;               // small double scratch (reductions), 256 entries
   long long launches = 0;
@@ -55,6 +58,7 @@ struct tfl_ctx {
     int nb = 0, nz = 0, ny = 0, nx = 0;
     int* changed = nullptr;                 // device word
     const float* fresh_for = nullptr;       // set inside a slab step: the cache already mirrors these flags
+    unsigned long long gen = 0;             // bumped on every reallocation of `bytes` (see arena_gen)
   } fcache;
   // advectVel over shared-memory tiles (tfl_advect_tile.cu): the kernel reports the longest trace of a call
   // into a device word that is copied, asynchronously, into a pinned host word; the NEXT calls pick the tile
@@ -103,6 +107,7 @@ struct tfl_cnn {
   float* tail = nullptr;     // w4[8][8], b4[8], w5[8], b5[1]
   float* act[3] = {nullptr, nullptr, nullptr};   // padded channels-last activation buffers
   ConvTcGeo act_geo = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  unsigned long long act_gen = 0;   // bumped whenever act / bact / part are reallocated (see tfl_ctx::arena_gen)
   // banked tensor-core path (split 1, join 3): per split, layers 1 / 2 of bank i at wBk[2 i] / wBk[2 i + 1]; the
   // join layer's weights (one for 'add', bank i's 8-channel slice at wBj[i] for 'concat'); banks 2..N own three
   // padded buffers each (pyramid input, layer 1, layer 2) at their resolution; 'concat' adds an fp32 partial sum.
@@ -164,6 +169,7 @@ int arena_reserve(tfl_ctx* ctx, size_t bytes) {
   if (ctx->arena) cudaFree(ctx->arena);
   ctx->arena = nullptr;
   ctx->arena_bytes = 0;
+  ctx->arena_gen++;
   void* p = nullptr;
   TFL_CUDA(ctx, cudaMalloc(&p, bytes));
   ctx->arena = (char*)p;
@@ -253,6 +259,7 @@ int flag_cache_ensure(tfl_ctx* ctx, const Geo& g) {
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (fc.bytes) cudaFree(fc.bytes);
   fc.bytes = nullptr;
+  fc.gen++;
   void* p = nullptr;
   TFL_CUDA(ctx, cudaMalloc(&p, 3 * cells + 64));
   fc.bytes = (unsigned char*)p;
@@ -1370,6 +1377,7 @@ static int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
                   g.nz, r);
   }
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  m->act_gen++;
   m->act_geo = make_conv_tc_geo(g.nb, g.nz, g.ny, g.nx);
   for (int i = 0; i < 3; i++) {
     if (m->act[i]) cudaFree(m->act[i]);
@@ -2646,11 +2654,16 @@ int tfl_slab_sim_exchange_stats(tfl_ctx* ctx, tfl_slab_sim* s, float ms[4], int6
 // fused step, their fork / join events, the memsets and the telemetry copy become graph nodes) and replayed
 // with one launch.  Pointers and every host-side choice of the captured call (fused or per-operator path,
 // advection tile halo) are frozen into the graph; results equal tfl_simulate_step's.
+// The graph also holds pointers into buffers the library owns: the context's scratch arena and flag cache, and
+// the model's activation buffers.  Each carries a generation counter; a launch after any of them was reallocated
+// is refused (the replay would read and write freed memory).
 // ---------------------------------------------------------------------------------------
 struct tfl_step_graph {
   cudaGraph_t graph = nullptr;
   cudaGraphExec_t exec = nullptr;
   long long launches = 0;       // kernels in one replay
+  unsigned long long arena_gen = 0, fcache_gen = 0, act_gen = 0;   // generations of the captured buffers
+  tfl_cnn* cnn = nullptr;       // the captured model (its act_gen is checked), or null
 };
 
 extern "C" {
@@ -2696,6 +2709,10 @@ int tfl_step_graph_create(tfl_ctx* ctx, const tfl_state* state, const tfl_mconf*
     tfl_step_graph_destroy(ctx, g);
     return fail(ctx, "step_graph: cudaGraphInstantiate failed");
   }
+  g->arena_gen = ctx->arena_gen;
+  g->fcache_gen = ctx->fcache.gen;
+  g->cnn = cnn;
+  g->act_gen = cnn ? cnn->act_gen : 0;
   *out = g;
   return 0;
 }
@@ -2704,6 +2721,13 @@ int tfl_step_graph_launch(tfl_ctx* ctx, tfl_step_graph* g) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!g || !g->exec) return fail(ctx, "step_graph is nil");
+  const char* stale = g->arena_gen != ctx->arena_gen      ? "the context's scratch arena"
+                      : g->fcache_gen != ctx->fcache.gen  ? "the context's flag cache"
+                      : g->cnn && g->act_gen != g->cnn->act_gen ? "the model's activation buffers"
+                                                                : nullptr;
+  if (stale)
+    return fail(ctx, "step_graph: stale graph: %s reallocated since the capture (a call on another grid shape or a "
+                     "larger grid); replaying would touch freed memory: capture the step again", stale);
   TFL_CUDA(ctx, cudaGraphLaunch(g->exec, ctx->stream));
   ctx->launches += g->launches;
   return 0;

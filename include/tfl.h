@@ -291,7 +291,14 @@ int tfl_host_sim_step(tfl_ctx* ctx, tfl_host_sim* hs, float* p, float* U, float*
 /* The step as a CUDA graph: tfl_simulate_step captured once (kernels of both internal streams, memsets, the
  * telemetry copy) and replayed with one launch per step.  The context must run on a non-default stream and one
  * tfl_simulate_step with the same state must have run before (capturing cannot allocate).  State pointers,
- * mconf and every host-side choice of the captured call are frozen into the graph. */
+ * mconf and every host-side choice of the captured call are frozen into the graph.
+ * The graph also holds pointers into buffers the library owns, and these calls free and reallocate them:
+ *   - any call on the context that needs more scratch than it has (an operator or step on a larger grid);
+ *   - tfl_advect_scalar / tfl_advect_vel with a traced method, tfl_simulate_step or another step on a grid of
+ *     another shape, smaller ones included (the context's flag cache);
+ *   - tfl_cnn_project or a step with the captured model on another grid (the model's activation buffers).
+ * After any of them tfl_step_graph_launch fails, naming the buffer, and replays nothing: capture again (after one
+ * tfl_simulate_step).  Destroying the model or the context while a graph that uses them exists is a caller error. */
 typedef struct tfl_step_graph tfl_step_graph;
 int tfl_step_graph_create(tfl_ctx* ctx, const tfl_state* state, const tfl_mconf* mconf, tfl_cnn* cnn,
                           tfl_step_graph** out);
