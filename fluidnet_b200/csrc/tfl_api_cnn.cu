@@ -1,0 +1,719 @@
+// C ABI of the projection network (include/tfl.h): model creation, modes, the fp32 graph executor and the
+// tensor-core stacks (tfl_cnn*.cu), and the test hooks of the tensor-core layers.
+#include <string.h>
+#include <algorithm>
+#include <cmath>
+#include <vector>
+
+#include "tfl_api_internal.h"
+
+constexpr int kMaxBanks = kMaxBankPtrs;     // banks a join kernel takes
+
+namespace {
+
+// Packs a [8][cin][3][3][3] weight for launch_conv3_tc / launch_conv3_tc_join and uploads it; nullptr if the
+// allocation fails.
+float* upload_tc_weights(const float* w, int cin, int split) {
+  std::vector<float> packed(conv_tc_b_floats(split));
+  conv_tc_pack_weights(w, cin, split, packed.data());
+  float* d = nullptr;
+  if (cudaMalloc((void**)&d, packed.size() * 4) != cudaSuccess) return nullptr;
+  cudaMemcpy(d, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice);
+  return d;
+}
+
+// Bank i's 8-channel slice of a 'concat' join weight [8][8 nbanks][3][3][3] (one bank: the whole weight).
+std::vector<float> concat_slice(const float* w, int nbanks, int i) {
+  std::vector<float> slice(8 * 8 * 27);
+  for (int o = 0; o < 8; o++)
+    memcpy(slice.data() + (size_t)o * 8 * 27, w + ((size_t)o * 8 * nbanks + 8 * i) * 27, 8 * 27 * 4);
+  return slice;
+}
+
+// The join layer of a banked stack (split 1, join 3) -> p_net, reading bank i's layer-2 output l2[i] (geometry
+// geo[i], 2^-i of bank 1's resolution) with nearest indexing.  'add': one launch summing the banks, weights wj[0];
+// 'concat': one launch per bank with its slice wj[i], banks N..2 writing / adding the fp32 partial sum `part`,
+// bank 1 last adding it before the bias, ReLU and tail (one bank: no partial sum).
+void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, int nbanks, bool add, float* part, float* p_net,
+                    float* const* wj, const float* bias, const float* tail, int split, const ConvTcGeo& g,
+                    cudaStream_t st) {
+  auto src_of = [&](int first, int n, int mode) {
+    TcJoinSrc js = {};
+    for (int k = 0; k < n; k++) {
+      const int i = first + k;
+      js.p[k] = l2[i];
+      js.px[k] = geo[i].px; js.py[k] = geo[i].py; js.nz[k] = geo[i].nz; js.shift[k] = i;
+    }
+    js.n = n;
+    js.part_mode = mode;
+    js.partial = part;
+    return js;
+  };
+  if (add) {
+    launch_conv3_tc_join(src_of(0, nbanks, 0), p_net, wj[0], bias, tail, split, g, st);
+  } else {
+    for (int i = nbanks - 1; i >= 0; i--)
+      launch_conv3_tc_join(src_of(i, 1, nbanks == 1 ? 0 : (i == nbanks - 1 ? 1 : (i > 0 ? 2 : 3))), p_net, wj[i], bias,
+                           tail, split, g, st);
+  }
+}
+
+}  // namespace
+
+// Tensor-core path: padded channels-last activations owned by the model (their zero borders
+// must survive between calls, so they do not live in the shared arena).
+int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
+  if (m->act_geo.nb == g.nb && m->act_geo.nz == g.nz && m->act_geo.ny == g.ny && m->act_geo.nx == g.nx) return 0;
+  if (m->nbanks > 1) {
+    const int r = 1 << (m->nbanks - 1);
+    if (g.nx % r || g.ny % r || g.nz % r)
+      return fail(ctx, "cnn: grid %dx%dx%d at bank split stage 1 is not divisible by 2^(banksNum-1) = %d", g.nx, g.ny,
+                  g.nz, r);
+  }
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  m->act_gen++;
+  m->act_geo = make_conv_tc_geo(g.nb, g.nz, g.ny, g.nx);
+  for (int i = 0; i < 3; i++) {
+    if (m->act[i]) cudaFree(m->act[i]);
+    m->act[i] = nullptr;
+    TFL_CUDA(ctx, cudaMalloc((void**)&m->act[i], conv_tc_act_bytes(m->act_geo)));
+    TFL_CUDA(ctx, cudaMemset(m->act[i], 0, conv_tc_act_bytes(m->act_geo)));
+  }
+  for (float* p : m->bact) cudaFree(p);
+  m->bact.clear();
+  m->bgeo.clear();
+  if (m->part) cudaFree(m->part);
+  m->part = nullptr;
+  for (int i = 1; i < m->nbanks; i++) {
+    const ConvTcGeo bg = make_conv_tc_geo(g.nb, g.nz >> i, g.ny >> i, g.nx >> i);
+    m->bgeo.push_back(bg);
+    for (int q = 0; q < 3; q++) {
+      float* p = nullptr;
+      TFL_CUDA(ctx, cudaMalloc((void**)&p, conv_tc_act_bytes(bg)));
+      m->bact.push_back(p);
+      TFL_CUDA(ctx, cudaMemset(p, 0, conv_tc_act_bytes(bg)));
+    }
+  }
+  if (m->nbanks > 1 && !m->bank_add)
+    TFL_CUDA(ctx, cudaMalloc((void**)&m->part, (size_t)g.nb * g.nz * g.ny * g.nx * 8 * 4));
+  return 0;
+}
+
+// Banked stack (split 1, join 3) on tensor cores: pyramid of the padded input, layers 1 and 2 of every bank at its
+// own resolution, then the join layer reading the banks' layer-2 outputs with nearest indexing.  'add': one launch
+// summing the banks; 'concat': one launch per bank (N..2 into the fp32 partial sum, bank 1 last with the tail).
+static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st) {
+  const ConvTcGeo& tg = m->act_geo;
+  const int split = m->mode == 2 ? 1 : 0, nbk = m->nbanks;
+  const float* in[kTcMaxBanks];
+  const float* l2[kTcMaxBanks];
+  ConvTcGeo geo[kTcMaxBanks];
+  in[0] = m->act[0];
+  geo[0] = tg;
+  for (int i = 1; i < nbk; i++) {
+    geo[i] = m->bgeo[i - 1];
+    float* dst = m->bact[3 * (i - 1)];
+    launch_tc_pyramid(in[i - 1], geo[i - 1], dst, geo[i], st);
+    in[i] = dst;
+  }
+  for (int i = 0; i < nbk; i++) {
+    float* o1 = i == 0 ? m->act[1] : m->bact[3 * (i - 1) + 1];
+    float* o2 = i == 0 ? m->act[2] : m->bact[3 * (i - 1) + 2];
+    launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, 1, 0, split, geo[i], st);
+    launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, geo[i], st);
+    l2[i] = o2;
+  }
+  launch_tc_join(l2, geo, nbk, m->bank_add, m->part, p_net, m->wBj[split].data(), m->b[m->conv0[2]], m->tail, split, tg,
+                 st);
+}
+
+// The three 3x3x3 layers (+ fused 1x1x1 tail) on tensor cores: act[0] -> act[1] -> act[2] -> p_net.
+// p_lo / p_hi: planes on which p_net is wanted (default all).  Layer l then only has to produce the planes the
+// later layers' 3x3x3 stencils reach from there; on a z-slab that spares most of the ghost planes.
+void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo, int p_hi) {
+  if (m->nbanks > 1) {       // whole grids only (the z-slab entry points refuse banked models)
+    run_conv_stack_banked(m, p_net, st);
+    return;
+  }
+  const ConvTcGeo& tg = m->act_geo;
+  if (p_hi < 0) p_hi = tg.nz;
+  const int split = m->mode == 2 ? 1 : 0;
+  ConvTcGeo g1 = tg, g2 = tg, g3 = tg;
+  g3.z_lo = std::max(0, p_lo);     g3.z_hi = std::min(tg.nz, p_hi);
+  g2.z_lo = std::max(0, p_lo - 1); g2.z_hi = std::min(tg.nz, p_hi + 1);
+  g1.z_lo = std::max(0, p_lo - 2); g1.z_hi = std::min(tg.nz, p_hi + 2);
+  launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, 1, 0, split, g1, st);
+  launch_conv3_tc(m->act[1], m->act[2], nullptr, m->wBk[split][1], m->b[1], nullptr, 2, 0, split, g2, st);
+  launch_conv3_tc(m->act[2], nullptr, p_net, m->wBj[split][0], m->b[2], m->tail, 2, 1, split, g3, st);
+}
+
+extern "C" {
+
+// ---------------------------------------------------------------------------------------
+// CNN projection
+// ---------------------------------------------------------------------------------------
+int tfl_cnn_create(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                   const int32_t* ksize, const float* const* weights, const float* const* biases,
+                   tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  return tfl_cnn_create_graph(ctx, is_3d, n_layers, cin, cout, ksize, nullptr, nullptr, 0, 0, weights, biases, out);
+}
+
+static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
+                           const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
+                           const float* const* biases, tfl_cnn** out);
+
+int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
+                         const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                         int nonlin_sigmoid, const float* const* weights, const float* const* biases,
+                         tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  return cnn_create_impl(ctx, is_3d, n_layers, cin, cout_logical, ksize, pool, up, pool_is_max, nonlin_sigmoid,
+                         nullptr, weights, biases, out);
+}
+
+int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                          const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                          int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
+                          const float* const* biases, tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (banks) {     // the assertions of lib/model.lua:246-252 (checked whatever banksNum is)
+    if (banks->num < 1) return fail(ctx, "cnn: banksNum >= 1 failed (got %d)", banks->num);
+    if (!(banks->split_stage < banks->join_stage))
+      return fail(ctx, "cnn: banksSplitStage < banksJoinStage failed (%d, %d)", banks->split_stage, banks->join_stage);
+    if (banks->split_stage < 1 || banks->split_stage >= n_layers)
+      return fail(ctx, "cnn: banksSplitStage >= 1 and banksSplitStage < #osize failed (%d, %d stages)",
+                  banks->split_stage, n_layers);
+    if (banks->join_stage < 1 || banks->join_stage >= n_layers)
+      return fail(ctx, "cnn: banksJoinStage >= 1 and banksJoinStage < #osize failed (%d, %d stages)",
+                  banks->join_stage, n_layers);
+    if (banks->num > kMaxBanks) return fail(ctx, "cnn: at most %d banks are supported (got %d)", kMaxBanks, banks->num);
+    if (banks->num == 1) banks = nullptr;
+  }
+  return cnn_create_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
+                         weights, biases, out);
+}
+
+static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
+                           const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
+                           const float* const* biases, tfl_cnn** out) {
+  if (!out || n_layers < 1) return fail(ctx, "cnn: bad arguments");
+  const int nbanks = banks ? banks->num : 1;
+  const int bsplit = banks ? banks->split_stage - 1 : 0, bjoin = banks ? banks->join_stage - 1 : 0;
+  auto convs_of = [&](int l) { return (nbanks > 1 && l >= bsplit && l < bjoin) ? nbanks : 1; };
+  // Channels the convolution of layer l really emits: cout * up^d (ConvolutionUpsample, model_utils.lua:74-76).
+  std::vector<int32_t> cout_conv(n_layers);
+  bool plain = !nonlin_sigmoid;
+  for (int l = 0; l < n_layers; l++) {
+    const int u = up ? up[l] : 1, pl = pool ? pool[l] : 1;
+    if (u < 1 || pl < 1) return fail(ctx, "cnn: pooling / upsampling sizes must be >= 1");
+    if (u > 1 && pl > 1) return fail(ctx, "Pooling and upsampling in the same layer!");          // model.lua:326
+    if (l == n_layers - 1 && pl != 1) return fail(ctx, "Pooling is not allowed in the last layer");  // model.lua:245
+    cout_conv[l] = cout_logical[l] * u * u * (is_3d ? u : 1);
+    if (u != 1 || pl != 1) plain = false;
+  }
+  const int32_t* cout = cout_conv.data();
+  if (cout_logical[n_layers - 1] != 1) return fail(ctx, "Last layer osize must be 1 (pressure)");   // model.lua:244
+  if (cin[0] != 3) return fail(ctx, "cnn: the first layer must take 3 channels (pDiv, div, occupancy)");
+  if (nbanks > 1) plain = false;
+  tfl_cnn* m = new tfl_cnn();
+  m->plain = plain;
+  m->pool_is_max = pool_is_max ? 1 : 0;
+  m->nonlin = nonlin_sigmoid ? 2 : 1;
+  m->is3d = is_3d ? 1 : 0;
+  m->n_layers = n_layers;
+  m->nbanks = nbanks;
+  m->split = bsplit;
+  m->join = bjoin;
+  m->bank_add = banks && banks->aggregate_add ? 1 : 0;
+  int wi = 0;     // index into weights / biases
+  for (int l = 0; l < n_layers; l++) {
+    if (l > 0 && nbanks > 1 && l == bjoin && !m->bank_add && cin[l] != nbanks * cout_logical[l - 1]) {
+      delete m;
+      return fail(ctx, "cnn: stage %d concatenates %d banks of %d channels, so it needs cin = %d (got %d)", l + 1,
+                  nbanks, cout_logical[l - 1], nbanks * cout_logical[l - 1], cin[l]);
+    }
+    if (l > 0 && !(nbanks > 1 && l == bjoin && !m->bank_add) && cin[l] != cout_logical[l - 1]) {
+      delete m;
+      return fail(ctx, "cnn: channel mismatch at layer %d", l);
+    }
+    m->pool.push_back(pool ? pool[l] : 1);
+    m->up.push_back(up ? up[l] : 1);
+    m->conv0.push_back(wi);
+    if (ksize[l] % 2 != 1) { delete m; return fail(ctx, "convolution size must be odd"); }   // model_utils.lua:70
+    const int kz = is_3d ? ksize[l] : 1;
+    const int taps = kz * ksize[l] * ksize[l];
+    for (int bk = 0; bk < convs_of(l); bk++, wi++) {
+      std::vector<float> relaid((size_t)cin[l] * taps * cout[l]);
+      for (int o = 0; o < cout[l]; o++)
+        for (int c = 0; c < cin[l]; c++)
+          for (int t = 0; t < taps; t++)
+            relaid[((size_t)c * taps + t) * cout[l] + o] = weights[wi][((size_t)o * cin[l] + c) * taps + t];
+      float *dw = nullptr, *db = nullptr;
+      if (cudaMalloc((void**)&dw, relaid.size() * 4) != cudaSuccess ||
+          cudaMalloc((void**)&db, cout[l] * 4) != cudaSuccess) { tfl_cnn_destroy(ctx, m); return fail(ctx, "cnn: cudaMalloc failed"); }
+      cudaMemcpy(dw, relaid.data(), relaid.size() * 4, cudaMemcpyHostToDevice);
+      cudaMemcpy(db, biases[wi], cout[l] * 4, cudaMemcpyHostToDevice);
+      m->cin.push_back(cin[l]); m->cout.push_back(cout[l]); m->ks.push_back(ksize[l]);
+      m->w.push_back(dw); m->b.push_back(db);
+    }
+    if (cout[l] > m->max_c) m->max_c = cout[l];
+  }
+  {   // largest activation of the graph, in channels x cells-of-the-input-grid
+    double rel = 1.0;
+    m->max_rel = 3.0;
+    for (int l = 0; l < n_layers; l++) {
+      if (nbanks > 1 && l == bjoin) m->max_rel = std::max(m->max_rel, rel * cin[l]);   // the joined banks
+      m->max_rel = std::max(m->max_rel, rel * cout[l]);                          // convolution output
+      const int u = m->up[l], pl = m->pool[l];
+      rel *= (double)u * u * (is_3d ? u : 1);
+      m->max_rel = std::max(m->max_rel, rel * cout_logical[l]);                  // after the pixel shuffle
+      rel /= (double)pl * pl * (is_3d ? pl : 1);
+    }
+    if (rel != 1.0) { tfl_cnn_destroy(ctx, m); return fail(ctx, "cnn: pooling and upsampling do not return to the input resolution"); }
+    if ((double)m->max_c < m->max_rel) m->max_c = (int)std::ceil(m->max_rel);
+  }
+  // Tensor-core eligibility: the 3-D 'default' graph (lib/model.lua:219-226), single-bank or with banks split
+  // before stage 1 and joined before stage 3.
+  static const int want[5][3] = {{3, 8, 3}, {8, 8, 3}, {8, 8, 3}, {8, 8, 1}, {8, 1, 1}};
+  m->tc_ok = is_3d && n_layers == 5 && !nonlin_sigmoid &&
+             (nbanks == 1 || (bsplit == 0 && bjoin == 2 && nbanks <= kTcMaxBanks));
+  for (int l = 0; m->tc_ok && l < 5; l++) {
+    const int want_cin = (l == 2 && !m->bank_add) ? 8 * nbanks : want[l][0];
+    m->tc_ok = m->pool[l] == 1 && m->up[l] == 1 && cin[l] == want_cin && cout[l] == want[l][1] && ksize[l] == want[l][2];
+  }
+  if (m->tc_ok) {
+    const int j0 = m->conv0[2], nj = m->bank_add ? 1 : nbanks;
+    for (int split = 0; split < 2; split++) {
+      for (int i = 0; i < nbanks; i++) {                 // layers 1 and 2 of bank i
+        m->wBk[split].push_back(upload_tc_weights(weights[m->conv0[0] + i], 3, split));
+        m->wBk[split].push_back(upload_tc_weights(weights[m->conv0[1] + i], 8, split));
+      }
+      for (int i = 0; i < nj; i++)
+        m->wBj[split].push_back(upload_tc_weights(concat_slice(weights[j0], nj, i).data(), 8, split));
+    }
+    std::vector<float> tail(64 + 8 + 8 + 1);
+    memcpy(tail.data(), weights[m->conv0[3]], 64 * 4);
+    memcpy(tail.data() + 64, biases[m->conv0[3]], 8 * 4);
+    memcpy(tail.data() + 72, weights[m->conv0[4]], 8 * 4);
+    tail[80] = biases[m->conv0[4]][0];
+    cudaMalloc((void**)&m->tail, tail.size() * 4);
+    cudaMemcpy(m->tail, tail.data(), tail.size() * 4, cudaMemcpyHostToDevice);
+    m->mode = 2;
+  }
+  *out = m;
+  return 0;
+}
+
+int tfl_cnn_set_mode(tfl_ctx* ctx, tfl_cnn* m, int mode) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!m || mode < 0 || mode > 2) return fail(ctx, "cnn_set_mode: bad arguments");
+  if (mode > 0 && m->nbanks > 1 && !m->tc_ok)
+    return fail(ctx, "cnn_set_mode: the tensor-core path covers the 3-D 'default' architecture, single-bank or with "
+                     "banks split at stage 1 and joined at stage 3; this banked model runs on the fp32 path");
+  if (mode > 0 && !m->tc_ok)
+    return fail(ctx, "cnn_set_mode: the tensor-core path covers the 3-D 'default' architecture only");
+  m->mode = mode;
+  return 0;
+}
+int tfl_cnn_get_mode(const tfl_cnn* m) { return m ? m->mode : -1; }
+
+// Undocumented debugging hook (not in tfl.h): per-CTA phase timestamps of the tensor-core conv.
+int tfl_debug_conv_timestamps(void* dev_buf) { conv_tc_set_debug((long long*)dev_buf); return 0; }
+
+// Undocumented test hooks (not in tfl.h): one tensor-core 3x3x3 layer on caller-owned buffers.
+// tfl_debug_conv_tc_layout: the padded pitches (px, py) of make_conv_tc_geo, so callers can lay out
+// in / out ([nb][2 planes][nz+2][py][px] float4); p_net is plain [nb][nz][ny][nx].
+int tfl_debug_conv_tc_layout(int nb, int nz, int ny, int nx, int32_t out[2]) {
+  const ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  out[0] = g.px;
+  out[1] = g.py;
+  return 0;
+}
+
+// tfl_debug_conv3_tc: weights [8][cin][3][3][3] and bias [8] on the host, packed with conv_tc_pack_weights;
+// tail (final layer only): w4[8][8], b4[8], w5[8], b5[1] as in tfl_cnn_create_graph.  Output planes
+// [z_lo, z_hi) only.  Synchronises before returning.
+int tfl_debug_conv3_tc(tfl_ctx* ctx, const float* in, float* out, float* p_net, const float* w_host,
+                       const float* bias_host, const float* tail_host, int cin, int final_layer, int split,
+                       int nb, int nz, int ny, int nx, int z_lo, int z_hi) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (cin != 3 && cin != 8) return fail(ctx, "debug_conv3_tc: cin must be 3 or 8 (got %d)", cin);
+  if (final_layer && cin != 8) return fail(ctx, "debug_conv3_tc: the final layer takes 8 channels");
+  if (final_layer && (!tail_host || !p_net)) return fail(ctx, "debug_conv3_tc: the final layer needs tail and p_net");
+  if (!final_layer && !out) return fail(ctx, "debug_conv3_tc: nil out");
+  if (!in || !w_host || !bias_host) return fail(ctx, "debug_conv3_tc: nil argument");
+  if (nb < 1 || nz < 1 || ny < 1 || nx < 1) return fail(ctx, "debug_conv3_tc: bad grid %dx%dx%dx%d", nb, nz, ny, nx);
+  if (z_lo < 0 || z_hi > nz || z_lo >= z_hi) return fail(ctx, "debug_conv3_tc: z range [%d, %d) not in [0, %d]", z_lo, z_hi, nz);
+  ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  g.z_lo = z_lo;
+  g.z_hi = z_hi;
+  float *wB = upload_tc_weights(w_host, cin, split), *bias = nullptr, *tail = nullptr;
+  auto release = [&]() {
+    if (wB) cudaFree(wB);
+    if (bias) cudaFree(bias);
+    if (tail) cudaFree(tail);
+  };
+  const int n_tail = 64 + 8 + 8 + 1;
+  if (!wB || cudaMalloc((void**)&bias, 8 * 4) != cudaSuccess ||
+      (final_layer && cudaMalloc((void**)&tail, n_tail * 4) != cudaSuccess)) {
+    release();
+    return fail(ctx, "debug_conv3_tc: cudaMalloc failed");
+  }
+  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
+  if (final_layer) cudaMemcpy(tail, tail_host, n_tail * 4, cudaMemcpyHostToDevice);
+  launch_conv3_tc(in, out, p_net, wB, bias, tail, cin == 3 ? 1 : 2, final_layer, split, g, ctx->stream);
+  const int rc = check_launch(ctx, "debug_conv3_tc");
+  const cudaError_t se = cudaStreamSynchronize(ctx->stream);
+  release();
+  if (rc) return rc;
+  if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc: %s", cudaGetErrorString(se));
+  return 0;
+}
+
+// tfl_debug_conv3_tc_join: the join layer of a banked model (split 1, join 3) on caller-owned bank buffers.
+// banks[i] (device) is bank i+1's layer-2 output in the padded layout of make_conv_tc_geo(nb, nz >> i, ny >> i,
+// nx >> i); w_host [8][cin][3][3][3] with cin = 8 (add) or 8 nbanks (concat), bias [8], tail as in
+// tfl_debug_conv3_tc.  Writes p_net [nb][nz][ny][nx].  Synchronises before returning.
+int tfl_debug_conv3_tc_join(tfl_ctx* ctx, const float* const* banks, int nbanks, int add, float* p_net,
+                            const float* w_host, const float* bias_host, const float* tail_host, int split, int nb,
+                            int nz, int ny, int nx) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (nbanks < 1 || nbanks > kTcMaxBanks) return fail(ctx, "debug_conv3_tc_join: bad bank count %d", nbanks);
+  if (!banks || !p_net || !w_host || !bias_host || !tail_host) return fail(ctx, "debug_conv3_tc_join: nil argument");
+  const int r = 1 << (nbanks - 1);
+  if (nb < 1 || nz < 1 || ny < 1 || nx < 1 || nz % r || ny % r || nx % r)
+    return fail(ctx, "debug_conv3_tc_join: grid %dx%dx%dx%d is not divisible by %d", nb, nz, ny, nx, r);
+  const ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  const int cin = add ? 8 : 8 * nbanks, nw = add ? 1 : nbanks;
+  std::vector<float*> wj(nw, nullptr);
+  float *bias = nullptr, *tail = nullptr, *part = nullptr;
+  auto release = [&]() {
+    for (float* p : wj) if (p) cudaFree(p);
+    if (bias) cudaFree(bias);
+    if (tail) cudaFree(tail);
+    if (part) cudaFree(part);
+  };
+  bool ok = cudaMalloc((void**)&bias, 8 * 4) == cudaSuccess && cudaMalloc((void**)&tail, 81 * 4) == cudaSuccess &&
+            (add || cudaMalloc((void**)&part, (size_t)nb * nz * ny * nx * 8 * 4) == cudaSuccess);
+  for (int i = 0; ok && i < nw; i++)
+    ok = (wj[i] = upload_tc_weights(concat_slice(w_host, cin / 8, i).data(), 8, split)) != nullptr;
+  if (!ok) {
+    release();
+    return fail(ctx, "debug_conv3_tc_join: cudaMalloc failed");
+  }
+  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
+  cudaMemcpy(tail, tail_host, 81 * 4, cudaMemcpyHostToDevice);
+  ConvTcGeo geo[kTcMaxBanks];
+  for (int i = 0; i < nbanks; i++) geo[i] = make_conv_tc_geo(nb, nz >> i, ny >> i, nx >> i);
+  launch_tc_join(banks, geo, nbanks, add, part, p_net, wj.data(), bias, tail, split, g, ctx->stream);
+  const int rc = check_launch(ctx, "debug_conv3_tc_join");
+  const cudaError_t se = cudaStreamSynchronize(ctx->stream);
+  release();
+  if (rc) return rc;
+  if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc_join: %s", cudaGetErrorString(se));
+  return 0;
+}
+
+void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!m) return;
+  if (ctx) cudaStreamSynchronize(ctx->stream);
+  for (float* p : m->w) cudaFree(p);
+  for (float* p : m->b) cudaFree(p);
+  if (m->tail) cudaFree(m->tail);
+  for (float* p : m->act)
+    if (p) cudaFree(p);
+  for (int sp = 0; sp < 2; sp++) {
+    for (float* p : m->wBk[sp]) cudaFree(p);
+    for (float* p : m->wBj[sp]) cudaFree(p);
+  }
+  for (float* p : m->bact) cudaFree(p);
+  if (m->part) cudaFree(m->part);
+  delete m;
+}
+
+// One rotating buffer of bank i (0-based, i >= 1): bank i holds 2^-d i of bank 1's cells, and every
+// activation of bank 1 fits max_rel.
+static size_t cnn_bank_buf_bytes(const tfl_cnn* m, const Geo& g, int i) {
+  const double cells = (double)g.n * g.nb;
+  return (size_t)(cells * m->max_rel / (double)(1LL << ((m->is3d ? 3 : 2) * i)) + 64) * 4;
+}
+
+static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const float* U_div,
+                            const float* flags, float* p_out, float* U_out, float threshold, const Geo& g,
+                            char* scratch, float** scale_dev_out) {
+  // scratch layout (caller reserved): U1 [nc], x0 [3], actA [max_c], actB [max_c], scale [nb]
+  const size_t cells = (size_t)g.n * g.nb;
+  size_t off = 0;
+  auto take = [&](size_t bytes) { char* p = scratch + off; off = (off + bytes + 255) & ~(size_t)255; return p; };
+  float* U1 = (float*)take(cells * 4 * g.nc);
+  float* x0 = (float*)take(cells * 4 * 3);
+  float* actA = (float*)take(cells * 4 * m->max_c);      // max_c covers max_rel (set at creation)
+  float* actB = (float*)take(cells * 4 * m->max_c);
+  float* scale = (float*)take(sizeof(float) * g.nb);
+  double* sums = ctx->dscratch + 64;
+  cudaStream_t st = ctx->stream;
+  TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
+  launch_cnn_mask_stats(U_div, flags, U1, sums, g.zlo, g.zhi, g, st);
+  launch_cnn_scale(sums, scale, g.nb, (long long)g.nc * g.n, threshold, st);
+  if (m->mode > 0 && m->tc_ok && !ctx->slab) {
+    if (cnn_ensure_act(ctx, m, g)) return 1;
+    const ConvTcGeo& tg = m->act_geo;
+    launch_cnn_inputs_padded(p_div, U1, flags, scale, m->act[0], tg.px, tg.py, g, st);
+    float* p_net = actA;      // plain [b][z][y][x]
+    run_conv_stack(m, p_net, st);
+    launch_cnn_finish(p_net, U1, flags, scale, p_out, U_out, g, st);
+    ctx->launches += 7;
+    if (scale_dev_out) *scale_dev_out = scale;
+    return check_launch(ctx, "cnn_project (tensor cores)");
+  }
+  launch_cnn_inputs(p_div, U1, flags, scale, x0, g, st);
+  ctx->launches += 3;
+  const float* in = x0;
+  if (m->plain) {
+    float* bufs[2] = {actA, actB};
+    for (int l = 0; l < m->n_layers; l++) {
+      float* o = bufs[l & 1];
+      const int act = (l < m->n_layers - 1) ? 1 : 0;
+      if (launch_conv_direct(in, o, m->w[l], m->b[l], m->cin[l], m->cout[l], m->ks[l], act, g, st) < 0)
+        return fail(ctx, "cnn: unsupported layer shape cout=%d k=%d", m->cout[l], m->ks[l]);
+      ctx->launches += 1;
+      in = o;
+    }
+  } else {
+    // 'tog' / 'yang' graphs: conv (+ pixel shuffle) -> non-linearity -> pooling, layer by layer, on grids
+    // whose resolution follows the pooling / upsampling sizes (lib/model.lua:262-340, single bank).
+    if (ctx->slab) return fail(ctx, "cnn: pooled / upsampled graphs run on whole grids only");
+    float* bufs[3] = {actA, actB, (float*)take((size_t)((double)cells * m->max_rel + 64) * 4)};
+    // Banks 2..N rotate through three buffers of their own (bank i is 2^-d(i-1) the size of bank 1).
+    float* bank_bufs[kMaxBanks][3] = {};
+    for (int i = 1; i < m->nbanks; i++)
+      for (int q = 0; q < 3; q++) bank_bufs[i][q] = (float*)take(cnn_bank_buf_bytes(m, g, i));
+    // One stage of one bank: convolution ci (+ pixel shuffle) -> non-linearity -> pooling, on grid gl, through
+    // the rotating buffers bb.  out_bstride > 0: the stage's result is written with that batch stride (floats),
+    // so that it lands in place in a concatenation of banks.
+    auto run_stage = [&](int ci, int l, const float* src, float* const* bb, Geo& gl, long long out_bstride,
+                         const float** result) -> int {
+      auto other = [&](const float* a) {
+        for (int q = 0; q < 3; q++) if (bb[q] != a) return bb[q];
+        return bb[0];
+      };
+      const int u = m->up[l], pl = m->pool[l];
+      const int act = (l < m->n_layers - 1) ? m->nonlin : 0;     // element-wise: commutes with the shuffle
+      const int shuffled = m->cout[ci] / (u * u * (gl.is3d ? u : 1));
+      // per batch entry when the last operation of the stage writes with a batch stride
+      const int nloop_conv = (out_bstride > 0 && u == 1 && pl == 1) ? gl.nb : 1;
+      float* o = other(src);
+      for (int b = 0; b < nloop_conv; b++) {
+        Geo gb = gl;
+        if (nloop_conv > 1) gb.nb = 1;
+        const long long ioff = nloop_conv > 1 ? (long long)b * m->cin[ci] * gl.n : 0;
+        const long long ooff = nloop_conv > 1 ? (long long)b * out_bstride : 0;
+        if (launch_conv_direct(src + ioff, o + ooff, m->w[ci], m->b[ci], m->cin[ci], m->cout[ci], m->ks[ci], act, gb, st) < 0)
+          return fail(ctx, "cnn: unsupported layer shape cout=%d k=%d", m->cout[ci], m->ks[ci]);
+        ctx->launches += 1;
+      }
+      const float* cur = o;
+      int chans = m->cout[ci];
+      if (u > 1) {
+        chans = shuffled;
+        float* sh = other(cur);
+        const int nloop = (out_bstride > 0 && pl == 1) ? gl.nb : 1;
+        const long long nin = (long long)m->cout[ci] * gl.n;
+        for (int b = 0; b < nloop; b++) {
+          launch_pixel_shuffle(cur + (nloop > 1 ? b * nin : 0), sh + (nloop > 1 ? b * out_bstride : 0),
+                               nloop > 1 ? 1 : gl.nb, chans, gl.nz, gl.ny, gl.nx, u, gl.is3d, st);
+          ctx->launches += 1;
+        }
+        gl.nx *= u; gl.ny *= u; if (gl.is3d) gl.nz *= u;
+        cur = sh;
+      }
+      if (pl > 1) {
+        if (gl.nx % pl || gl.ny % pl || (gl.is3d && gl.nz % pl))
+          return fail(ctx, "cnn: grid %dx%dx%d is not divisible by the pooling size %d", gl.nx, gl.ny, gl.nz, pl);
+        float* po = other(cur);
+        const int nloop = out_bstride > 0 ? gl.nb : 1;
+        const long long nin = (long long)chans * gl.nx * gl.ny * gl.nz;
+        for (int b = 0; b < nloop; b++) {
+          launch_pool(cur + (nloop > 1 ? b * nin : 0), po + (nloop > 1 ? b * out_bstride : 0),
+                      (nloop > 1 ? 1 : gl.nb) * chans, gl.nz, gl.ny, gl.nx, pl, gl.is3d, m->pool_is_max, st);
+          ctx->launches += 1;
+        }
+        gl.nx /= pl; gl.ny /= pl; if (gl.is3d) gl.nz /= pl;
+        cur = po;
+      }
+      gl.n = (long long)gl.nx * gl.ny * gl.nz;
+      gl.gnz = gl.nz; gl.zlo = 0; gl.zhi = gl.nz;
+      *result = cur;
+      return 0;
+    };
+    const int nbk = m->nbanks;
+    const float* bank_in[kMaxBanks] = {};
+    Geo bank_g[kMaxBanks];
+    Geo gl = g;
+    for (int l = 0; l < m->n_layers; l++) {
+      if (nbk > 1 && l == m->split) {
+        // Gaussian pyramid (lib/model.lua:276-289): bank i = 2x average pool of bank i-1.
+        const int r = 1 << (nbk - 1);
+        if (gl.nx % r || gl.ny % r || (gl.is3d && gl.nz % r))
+          return fail(ctx, "cnn: grid %dx%dx%d at bank split stage %d is not divisible by 2^(banksNum-1) = %d",
+                      gl.nx, gl.ny, gl.nz, l + 1, r);
+        bank_in[0] = in;
+        bank_g[0] = gl;
+        for (int i = 1; i < nbk; i++) {
+          Geo gi = bank_g[i - 1];
+          launch_pool(bank_in[i - 1], bank_bufs[i][0], gi.nb * m->cin[m->conv0[l]], gi.nz, gi.ny, gi.nx, 2, gi.is3d, 0, st);
+          ctx->launches += 1;
+          gi.nx /= 2; gi.ny /= 2; if (gi.is3d) gi.nz /= 2;
+          gi.n = (long long)gi.nx * gi.ny * gi.nz;
+          gi.gnz = gi.nz; gi.zlo = 0; gi.zhi = gi.nz;
+          bank_g[i] = gi;
+          bank_in[i] = bank_bufs[i][0];
+        }
+      }
+      if (nbk > 1 && l >= m->split && l < m->join) {
+        const bool last = l == m->join - 1;
+        for (int i = 0; i < nbk; i++) {
+          const Geo& g1 = bank_g[0];
+          const int c_out = m->cout[m->conv0[l]] / (m->up[l] * m->up[l] * (g.is3d ? m->up[l] : 1));
+          // concat: bank 1's result is the first c_out channels of [nb][nbk c_out][n] at the join resolution
+          const long long n_join = (long long)(g1.nx * m->up[l] / m->pool[l]) * (g1.ny * m->up[l] / m->pool[l]) *
+                                   (g.is3d ? g1.nz * m->up[l] / m->pool[l] : g1.nz);
+          const long long bstride = (last && i == 0 && !m->bank_add && g.nb > 1) ? (long long)nbk * c_out * n_join : 0;
+          if (run_stage(m->conv0[l] + i, l, bank_in[i], i == 0 ? bufs : bank_bufs[i], bank_g[i], bstride, &bank_in[i]))
+            return 1;
+        }
+        if (last) {   // lib/model.lua:292-318: upsample banks 2..N, then JoinTable or CAddTable
+          const Geo& g1 = bank_g[0];
+          for (int i = 1; i < nbk; i++)
+            if (bank_g[i].nx << i != g1.nx || bank_g[i].ny << i != g1.ny || (g.is3d && bank_g[i].nz << i != g1.nz))
+              return fail(ctx, "cnn: bank %d does not upsample to the resolution of bank 1 (grid not divisible)", i + 1);
+          const int c_out = m->cout[m->conv0[l]] / (m->up[l] * m->up[l] * (g.is3d ? m->up[l] : 1));
+          if (launch_bank_join(bank_in, nbk, (float*)bank_in[0], g1.nb, c_out, g1.nz, g1.ny, g1.nx, g.is3d,
+                               m->bank_add, st) < 0)
+            return fail(ctx, "cnn: bad bank count %d", nbk);
+          ctx->launches += 1;
+          in = bank_in[0];
+          gl = g1;
+        }
+        continue;
+      }
+      if (run_stage(m->conv0[l], l, in, bufs, gl, 0, &in)) return 1;
+    }
+    if (gl.nx != g.nx || gl.ny != g.ny || gl.nz != g.nz) return fail(ctx, "cnn: graph does not return to the input resolution");
+  }
+  launch_cnn_finish(in, U1, flags, scale, p_out, U_out, g, st);
+  ctx->launches += 1;
+  if (scale_dev_out) *scale_dev_out = scale;
+  return check_launch(ctx, "cnn_project");
+}
+
+static size_t cnn_scratch_bytes(const tfl_cnn* m, const Geo& g) {
+  const size_t cells = (size_t)g.n * g.nb;
+  size_t bytes = cells * 4 * (g.nc + 3 + 2 * (size_t)m->max_c) + 4 * g.nb + 8 * 256;
+  if (!m->plain) bytes += (size_t)((double)cells * m->max_rel + 64) * 4 + 256;     // third rotating buffer
+  for (int i = 1; i < m->nbanks; i++) bytes += 3 * (cnn_bank_buf_bytes(m, g, i) + 256);
+  return bytes;
+}
+
+int tfl_cnn_project(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, const tfl_grid* U_div,
+                    const tfl_grid* flags, const tfl_grid* p_out, const tfl_grid* U_out, float threshold,
+                    float* scale_out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!m) return fail(ctx, "cnn is nil");
+  if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, p_div, "pDiv") || check_vel(ctx, U_div, flags) ||
+      check_scalar(ctx, p_out, "p") || check_vel(ctx, U_out, flags))
+    return 1;
+  if (!same_spatial(flags, p_div) || !same_spatial(flags, p_out) || U_out->nc != U_div->nc)
+    return fail(ctx, "Size mismatch");
+  if ((U_div->nc == 3) != (m->is3d != 0)) return fail(ctx, "model / data dimensionality mismatch");
+  if (ctx->slab) return fail(ctx, "cnn_project on a z-slab goes through the multi-GPU driver");
+  Geo g;
+  if (make_geo(ctx, flags, m->is3d, &g)) return 1;
+  if (arena_reserve(ctx, cnn_scratch_bytes(m, g))) return 1;
+  float* scale_dev = nullptr;
+  if (cnn_project_impl(ctx, m, p_div->data, U_div->data, flags->data, p_out->data, U_out->data, threshold, g,
+                       ctx->arena, &scale_dev))
+    return 1;
+  if (scale_out) {
+    TFL_CUDA(ctx, cudaMemcpyAsync(scale_out, scale_dev, sizeof(float) * g.nb, cudaMemcpyDeviceToHost, ctx->stream));
+    TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  }
+  return 0;
+}
+
+// z-slab variant of model:forward, split around the one global reduction (the input scale):
+//   tfl_cnn_stats              U1 = SetWallBcs mask * U on every local plane where the mask is
+//                              computable, and (sum, sum of squares) over the OWNED planes into
+//                              dev_sums[2 * nb] (device doubles the caller all-reduces, e.g. with NCCL);
+//   tfl_cnn_project_from_sums  everything after the reduction.  The conv stack runs on the whole
+//                              local slab (halo planes included), so results are valid on planes at
+//                              least 4 planes away from a local end that is not a global end.
+int tfl_cnn_stats(tfl_ctx* ctx, const tfl_grid* U_div, const tfl_grid* flags, const tfl_grid* U1,
+                  double* dev_sums) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (check_scalar(ctx, flags, "flags") || check_vel(ctx, U_div, flags) || check_vel(ctx, U1, flags)) return 1;
+  if (!dev_sums) return fail(ctx, "cnn_stats: nil sums");
+  Geo g;
+  if (make_geo(ctx, flags, U_div->nc == 3, &g)) return 1;
+  Geo gw = g;
+  if (ctx->slab) {
+    gw.zlo = (g.zoff == 0) ? 0 : 1;
+    gw.zhi = (g.zoff + g.nz == g.gnz) ? g.nz : g.nz - 1;
+  }
+  TFL_CUDA(ctx, cudaMemsetAsync(dev_sums, 0, sizeof(double) * 2 * g.nb, ctx->stream));
+  launch_cnn_mask_stats(U_div->data, flags->data, U1->data, dev_sums, g.zlo, g.zhi, gw, ctx->stream);
+  ctx->launches += 1;
+  return check_launch(ctx, "cnn_stats");
+}
+
+int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, const tfl_grid* U1,
+                              const tfl_grid* flags, const double* dev_sums, const tfl_grid* p_out,
+                              const tfl_grid* U_out, float threshold) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!m) return fail(ctx, "cnn is nil");
+  if (m->nbanks > 1) return fail(ctx, "cnn_project_from_sums: banked models run on whole grids only, not on z-slabs");
+  if (!m->tc_ok || m->mode == 0) return fail(ctx, "cnn_project_from_sums needs the tensor-core path (3-D default net)");
+  if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, p_div, "pDiv") || check_vel(ctx, U1, flags) ||
+      check_scalar(ctx, p_out, "p") || check_vel(ctx, U_out, flags))
+    return 1;
+  Geo g;
+  if (make_geo(ctx, flags, 1, &g)) return 1;
+  if (cnn_ensure_act(ctx, m, g)) return 1;
+  const size_t cells = (size_t)g.n * g.nb;
+  if (arena_reserve(ctx, carve_bytes({cells * 4, 4 * (size_t)g.nb}))) return 1;
+  Carver cv(ctx);
+  float* p_net = cv.take<float>(cells);
+  float* scale = cv.take<float>(g.nb);
+  cudaStream_t st = ctx->stream;
+  // scale from the (already reduced) sums; the sample count is that of the GLOBAL grid.
+  launch_cnn_scale(dev_sums, scale, g.nb, (long long)g.nc * g.nx * g.ny * g.gnz, threshold, st);
+  Geo gi = g;            // the divergence reads U1 one plane up
+  if (ctx->slab) {
+    gi.zlo = (g.zoff == 0) ? 0 : 1;
+    gi.zhi = (g.zoff + g.nz == g.gnz) ? g.nz : g.nz - 2;
+  }
+  const ConvTcGeo& tg = m->act_geo;
+  launch_cnn_inputs_padded(p_div->data, U1->data, flags->data, scale, m->act[0], tg.px, tg.py, gi, st);
+  // the velocity update of the computed planes [zlo, zhi) reads p on [zlo - 1, zhi)
+  if (ctx->slab) run_conv_stack(m, p_net, st, g.zlo - 1, g.zhi);
+  else run_conv_stack(m, p_net, st);
+  launch_cnn_finish(p_net, U1->data, flags->data, scale, p_out->data, U_out->data, g, st);
+  ctx->launches += 6;
+  return check_launch(ctx, "cnn_project_from_sums");
+}
+
+}  // extern "C"

@@ -1,0 +1,237 @@
+// Internal interface of the C ABI units: tfl_api.cu (context, memory, operators, step drivers),
+// tfl_api_cnn.cu (projection network) and tfl_api_slab.cu (z-slab driver).
+#pragma once
+#include <cuda_runtime.h>
+#include <stdarg.h>
+#include <stdio.h>
+#include <nvtx3/nvToolsExt.h>
+#include <nccl.h>      // types and prototypes only: libnccl is loaded on demand (dlopen), see tfl_api_slab.cu
+#include <initializer_list>
+#include <string>
+#include <vector>
+
+#include "tfl_kernels.h"
+#include "tfl_cnn_tc.h"
+
+using namespace tfl;
+
+struct tfl_ctx {
+  int device = 0;
+  cudaStream_t stream = nullptr;
+  bool own_stream = true;
+  std::string err;
+  char* arena = nullptr;
+  size_t arena_bytes = 0;
+  size_t arena_used = 0;
+  // Generation counters of the buffers a step graph captures: bumped whenever the buffer is freed and allocated
+  // again, so that tfl_step_graph_launch can refuse a graph that would replay freed memory.
+  unsigned long long arena_gen = 0;
+  unsigned long long* counters = nullptr;   // [0] trace faults, [1] bad occupancy cells
+  double* dscratch = nullptr;               // small double scratch (reductions), 256 entries
+  long long launches = 0;
+  bool slab = false;
+  int zoff = 0, gnz = 0, zlo = 0, zhi = 0;
+  int slab_margin = 2;                      // extra planes on which forward passes are evaluated
+  cudaStream_t side_stream = nullptr;       // density advection runs beside velocity advection
+  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  // Host-buffer step (tfl_host_sim_step): copies run on their own streams and the step waits for each
+  // input only where it is first read / hands each output over as soon as it is final.
+  cudaStream_t copy_in = nullptr, copy_out = nullptr;
+  cudaEvent_t ev_u_in = nullptr, ev_d_in = nullptr, ev_p_in = nullptr, ev_d_ready = nullptr, ev_d_out = nullptr;
+  struct {
+    bool active = false;
+    float* density_host = nullptr;          // where the advected density goes once it is final
+    size_t density_bytes = 0;
+    bool density_sent = false;
+  } ov;
+  PcgScratch pcg;                           // grow-only buffers of the PCG solve
+  // Byte copy of the step's flags and their clearance field (advection fast path), kept between steps:
+  // each step re-derives the bytes, compares them with the copy on the device and rebuilds the
+  // clearance only if something changed (no host round trip).
+  struct {
+    unsigned char* bytes = nullptr;         // [3][cells]: flags, clearance, scratch
+    size_t cells = 0;
+    int nb = 0, nz = 0, ny = 0, nx = 0;
+    int* changed = nullptr;                 // device word
+    const float* fresh_for = nullptr;       // set inside a slab step: the cache already mirrors these flags
+    unsigned long long gen = 0;             // bumped on every reallocation of `bytes` (see arena_gen)
+  } fcache;
+  // advectVel over shared-memory tiles (tfl_advect_tile.cu): the kernel reports the longest trace of a call
+  // into a device word that is copied, asynchronously, into a pinned host word; the NEXT calls pick the tile
+  // halo from it (stale by a step or two -- it only selects a code path, never a result).
+  struct {
+    unsigned int* dev = nullptr;
+    unsigned int* host = nullptr;           // pinned
+    int mode = -1;                          // -1 automatic, 0 two-kernel version, 1 / 2 forced halo
+    int variant = 0;                        // tile shape (tuning)
+    int calls_since_probe = 0;
+    // bench.py's roofline: CUDA events right around the tile kernel's launch (off unless asked for)
+    bool timed = false;
+    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+  } tile;
+  // z-slab decomposition over several GPUs (tfl_comm_init / tfl_slab_sim_*): the communicator lives here
+  ncclComm_t comm = nullptr;
+  int comm_rank = 0, comm_world = 1;
+  bool in_slab_step = false;
+};
+
+struct tfl_cnn {
+  int is3d = 1;
+  int n_layers = 0;
+  std::vector<int> cin, cout, ks;   // per convolution (= per stage unless banked)
+  std::vector<float*> w;     // device, [cin][tap][cout]
+  std::vector<float*> b;     // device, [cout]
+  // multi-resolution banks (lib/model.lua:252-361): stages [split, join) (0-based here) hold one convolution
+  // per bank; conv0[l] is the index of stage l's first convolution.  nbanks == 1: single bank.
+  int nbanks = 1, split = 0, join = 0, bank_add = 0;
+  std::vector<int> conv0;
+  int max_c = 0;
+  // per-layer extras of the 'tog' / 'yang' graphs (lib/model.lua:164-239): the convolution emits
+  // cout * up^d channels that a pixel shuffle turns into cout channels at `up` times the resolution, a
+  // pooling of size `pool` follows the non-linearity.  plain = every pool / up is 1 and the non-linearity is ReLU.
+  std::vector<int> pool, up;
+  int pool_is_max = 0;
+  int nonlin = 1;            // 1 ReLU, 2 sigmoid (activation codes of tfl_cnn.cu)
+  bool plain = true;
+  double max_rel = 0.0;      // largest channels x (cells relative to the input grid) of any stage
+  // tensor-core path (3-D 'default' architecture, single-bank or with banks split at stage 1 and joined at stage 3)
+  int mode = 0;              // 0 fp32 FMA, 1 TF32 tensor cores, 2 3xTF32 tensor cores
+  bool tc_ok = false;
+  float* tail = nullptr;     // w4[8][8], b4[8], w5[8], b5[1]
+  float* act[3] = {nullptr, nullptr, nullptr};   // padded channels-last activation buffers
+  ConvTcGeo act_geo = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  unsigned long long act_gen = 0;   // bumped whenever act / bact / part are reallocated (see tfl_ctx::arena_gen)
+  // Packed weights per split: layers 1 / 2 of bank i at wBk[2 i] / wBk[2 i + 1]; the join layer's weights (one for
+  // 'add', bank i's 8-channel slice at wBj[i] for 'concat', which for one bank is the whole layer 3).  Banks 2..N
+  // own three padded buffers each (pyramid input, layer 1, layer 2) at their resolution; 'concat' with N > 1 adds
+  // an fp32 partial sum.
+  std::vector<float*> wBk[2], wBj[2];
+  std::vector<float*> bact;
+  std::vector<ConvTcGeo> bgeo;
+  float* part = nullptr;
+};
+
+// Every entry point runs on the context's device whatever the caller's current device is, and leaves the
+// caller's current device as it found it (a host with several contexts / GPUs in one thread).
+// One NVTX range per entry point (named after the function): nsys / ncu --nvtx timelines show the operators.
+// nvtx3 is header-only and costs a null-pointer test when no tool is attached.
+struct NvtxRange {
+  explicit NvtxRange(const char* name) { nvtxRangePushA(name); }
+  ~NvtxRange() { nvtxRangePop(); }
+};
+
+struct DeviceGuard {
+  int prev = -1;
+  bool switched = false;
+  explicit DeviceGuard(const tfl_ctx* ctx) {
+    if (!ctx) return;
+    if (cudaGetDevice(&prev) == cudaSuccess && prev != ctx->device) switched = cudaSetDevice(ctx->device) == cudaSuccess;
+  }
+  ~DeviceGuard() { if (switched) cudaSetDevice(prev); }
+};
+
+inline int fail(tfl_ctx* ctx, const char* fmt, ...) {
+  char buf[512];
+  va_list ap;
+  va_start(ap, fmt);
+  vsnprintf(buf, sizeof(buf), fmt, ap);
+  va_end(ap);
+  if (ctx) ctx->err = buf;
+  return 1;
+}
+
+#define TFL_CUDA(ctx, call)                                                            \
+  do {                                                                                 \
+    cudaError_t e_ = (call);                                                           \
+    if (e_ != cudaSuccess) return fail(ctx, "%s: %s", #call, cudaGetErrorString(e_));  \
+  } while (0)
+
+inline int check_launch(tfl_ctx* ctx, const char* what) {
+  cudaError_t e = cudaGetLastError();
+  if (e != cudaSuccess) return fail(ctx, "%s: launch failed: %s", what, cudaGetErrorString(e));
+  return 0;
+}
+
+// Bump allocator over one growing device buffer (the reference's getTempStorage,
+// tfluids/init.lua:35-64).  Growing synchronises; steady state does not allocate.
+inline int arena_reserve(tfl_ctx* ctx, size_t bytes) {
+  if (bytes <= ctx->arena_bytes) return 0;
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (ctx->arena) cudaFree(ctx->arena);
+  ctx->arena = nullptr;
+  ctx->arena_bytes = 0;
+  ctx->arena_gen++;
+  void* p = nullptr;
+  TFL_CUDA(ctx, cudaMalloc(&p, bytes));
+  ctx->arena = (char*)p;
+  ctx->arena_bytes = bytes;
+  return 0;
+}
+struct Carver {
+  tfl_ctx* ctx;
+  size_t off = 0;
+  explicit Carver(tfl_ctx* c) : ctx(c) {}
+  template <typename T>
+  T* take(size_t count) {
+    const size_t a = (off + 255) & ~(size_t)255;
+    off = a + count * sizeof(T);
+    return (T*)(ctx->arena + a);
+  }
+};
+inline size_t carve_bytes(std::initializer_list<size_t> sizes) {
+  size_t off = 0;
+  for (size_t s : sizes) off = ((off + 255) & ~(size_t)255) + s;
+  return off + 256;
+}
+
+inline bool same_spatial(const tfl_grid* a, const tfl_grid* b) {
+  return a->nb == b->nb && a->nz == b->nz && a->ny == b->ny && a->nx == b->nx;
+}
+
+// Mirrors the shape asserts of init.lua (e.g. :100-120, :177-191).
+inline int check_scalar(tfl_ctx* ctx, const tfl_grid* g, const char* name) {
+  if (!g || !g->data) return fail(ctx, "%s is nil", name);
+  if (g->nc != 1) return fail(ctx, "%s is not scalar", name);
+  if (g->nb < 1 || g->nz < 1 || g->ny < 1 || g->nx < 1) return fail(ctx, "%s: Dimension mismatch", name);
+  return 0;
+}
+inline int check_vel(tfl_ctx* ctx, const tfl_grid* U, const tfl_grid* flags) {
+  if (!U || !U->data) return fail(ctx, "U is nil");
+  if (U->nc != 2 && U->nc != 3) return fail(ctx, "2D velocity field must have only 2 channels");
+  if (U->nc == 2 && flags->nz != 1) return fail(ctx, "2D velocity field but zdepth > 1");
+  if (!same_spatial(U, flags)) return fail(ctx, "Size mismatch");
+  return 0;
+}
+
+inline int make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is3d, Geo* g) {
+  g->nx = flags->nx; g->ny = flags->ny; g->nz = flags->nz; g->nb = flags->nb;
+  g->is3d = is3d ? 1 : 0;
+  g->nc = is3d ? 3 : 2;
+  g->n = (long long)flags->nx * flags->ny * flags->nz;
+  g->faults = ctx->counters;
+  if (ctx->slab) {
+    if (!is3d) return fail(ctx, "slab decomposition needs a 3D grid");
+    g->zoff = ctx->zoff; g->gnz = ctx->gnz; g->zlo = ctx->zlo; g->zhi = ctx->zhi;
+    if (g->zlo < 0 || g->zhi > g->nz || g->zlo >= g->zhi || g->zoff < 0 || g->zoff + g->nz > g->gnz)
+      return fail(ctx, "slab range does not fit the local grid");
+  } else {
+    g->zoff = 0; g->gnz = flags->nz; g->zlo = 0; g->zhi = flags->nz;
+  }
+  if (!is3d && flags->nz != 1) return fail(ctx, "2D grid must have zsize == 1");
+  if (g->n * (long long)g->nb * 3 >= (1LL << 31) * 4) return fail(ctx, "grid too large");
+  return 0;
+}
+
+// The step's body forces (lib/simulate.lua:216-239) for a grid of global extent nx x ny x gnz: the vectors that
+// tfl_add_buoyancy / tfl_add_gravity take, the vorticity confinement amplitude, and whether each one runs
+// (buoyancy also needs a density).
+struct StepForces {
+  bool buoyancy, gravity, vorticity;
+  float buoy[3], grav[3];
+  float vort_amp;
+};
+StepForces step_forces(const tfl_mconf* mc, int nx, int ny, int gnz);
+
+// Tensor-core path of the projection network (tfl_api_cnn.cu).
+int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g);
+void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo = 0, int p_hi = -1);

@@ -1,0 +1,607 @@
+// C ABI of the z-slab driver (include/tfl.h): the NCCL loader, the halo exchange and all-reduce kernels, and
+// tfl_comm_* / tfl_slab_sim_*.
+#include <dlfcn.h>
+#include <string.h>
+#include <algorithm>
+#include <vector>
+
+#include "tfl_api_internal.h"
+
+// ---------------------------------------------------------------------------------------
+// One domain split into z-slabs over the GPUs of a node (SURVEY.md 8e).  The reference is
+// single-GPU; this is the multi-GPU form of the same step: rank r owns the planes [z0, z1) of every
+// field plus `halo` ghost planes per interior side, every kernel works in GLOBAL coordinates
+// (tfl_set_slab), and ghost planes are refreshed by neighbour ncclSend / ncclRecv pairs one
+// message per neighbour and direction (a gather kernel packs the planes of every channel, a scatter kernel
+// unpacks them), grouped into one NCCL operation per phase:
+//     exchange U, density (halo = 2 * margin + 2)  -> advectScalar, advectVel
+//     exchange U, density (4)                      -> buoyancy / gravity on owned +- 3, vorticity confinement
+//     exchange U, p (5)                            -> wall mask + (sum, sum^2) on owned planes
+//     all-reduce of the two doubles                -> conv stack on the local slab, velocity update
+// ---------------------------------------------------------------------------------------
+namespace {
+
+struct NcclApi {
+  void* lib = nullptr;
+  decltype(&ncclGetUniqueId) GetUniqueId = nullptr;
+  decltype(&ncclCommInitRank) CommInitRank = nullptr;
+  decltype(&ncclCommDestroy) CommDestroy = nullptr;
+  decltype(&ncclGroupStart) GroupStart = nullptr;
+  decltype(&ncclGroupEnd) GroupEnd = nullptr;
+  decltype(&ncclSend) Send = nullptr;
+  decltype(&ncclRecv) Recv = nullptr;
+  decltype(&ncclAllReduce) AllReduce = nullptr;
+  decltype(&ncclGetErrorString) GetErrorString = nullptr;
+};
+NcclApi* nccl_api() {
+  static NcclApi api;
+  static bool tried = false;
+  if (!tried) {
+    tried = true;
+    // a host that already carries an NCCL (e.g. the one bundled with PyTorch) gets that copy back
+    void* h = dlopen("libnccl.so.2", RTLD_NOW | RTLD_GLOBAL);
+    if (!h) h = dlopen("libnccl.so", RTLD_NOW | RTLD_GLOBAL);
+    if (h) {
+      api.lib = h;
+#define TFL_NCCL_SYM(name) api.name = (decltype(api.name))dlsym(h, "nccl" #name)
+      TFL_NCCL_SYM(GetUniqueId); TFL_NCCL_SYM(CommInitRank); TFL_NCCL_SYM(CommDestroy); TFL_NCCL_SYM(GroupStart);
+      TFL_NCCL_SYM(GroupEnd); TFL_NCCL_SYM(Send); TFL_NCCL_SYM(Recv); TFL_NCCL_SYM(AllReduce); TFL_NCCL_SYM(GetErrorString);
+#undef TFL_NCCL_SYM
+      if (!api.GetUniqueId || !api.CommInitRank || !api.CommDestroy || !api.GroupStart || !api.GroupEnd || !api.Send ||
+          !api.Recv || !api.AllReduce || !api.GetErrorString)
+        api.lib = nullptr;
+    }
+  }
+  return api.lib ? &api : nullptr;
+}
+#define TFL_NCCL(ctx, call)                                                                       \
+  do {                                                                                            \
+    ncclResult_t r_ = (call);                                                                     \
+    if (r_ != ncclSuccess) return fail(ctx, "%s: %s", #call, nccl_api()->GetErrorString(r_));     \
+  } while (0)
+
+}  // namespace
+
+// floats reserved behind the halo counters of an inbox for the all-reduce: [2 parities][world <= 64][2] doubles, then
+// [2][64] step counters
+constexpr int kSumAreaFloats = 2 * 64 * 2 * 2 + 2 * 64;
+
+struct tfl_slab_sim {
+  int gnz = 0, ny = 0, nx = 0, margin = 2, halo = 6;
+  int rank = 0, world = 1;
+  int z0 = 0, z1 = 0, lo_halo = 0, hi_halo = 0, zoff = 0, nz = 0, own_lo = 0, own_hi = 0;
+  size_t cells = 0, plane = 0;      // local cells / cells per plane
+  tfl_state st;
+  float* U1 = nullptr;
+  double* sums = nullptr;
+  float* xbuf = nullptr;            // [send down | send up | recv from below | recv from above], xbuf_side floats each
+  size_t xbuf_side = 0;
+  // Peer-memory halo exchange (CUDA IPC over NVLink, tfl_slab_sim_ipc_*): this rank's inbox -- per phase and side a
+  // receive buffer of xbuf_side floats that the neighbour's push kernel fills with remote stores, and a step counter
+  // it raises afterwards -- and the neighbours' inboxes mapped into this process.
+  float* inbox = nullptr;           // cudaMalloc'ed, exported: [3 phases][2 sides][xbuf_side] floats, then 64 counters
+  float* peer_inbox[2] = {nullptr, nullptr};   // lower / upper neighbour's inbox (cudaIpcOpenMemHandle)
+  std::vector<float*> all_inbox;               // every rank's inbox (own pointer at [rank]): the all-reduce's targets
+  float** all_inbox_dev = nullptr;             // the same table on the device
+  unsigned int* push_done = nullptr;           // CTAs of the running push kernel that finished their stores
+  bool peer_ok = false;
+  unsigned int step_no = 0;
+  std::vector<void*> owned;
+  cudaEvent_t ev[4][2] = {{nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}};
+  size_t bytes_sent[3] = {0, 0, 0};
+};
+
+extern "C" {
+
+int tfl_comm_unique_id(tfl_ctx* ctx, char* id_out) {
+  NcclApi* nc = nccl_api();
+  if (!nc) return fail(ctx, "comm: libnccl.so.2 not found");
+  static_assert(sizeof(ncclUniqueId) <= TFL_COMM_ID_BYTES, "unique id fits the ABI buffer");
+  ncclUniqueId id;
+  TFL_NCCL(ctx, nc->GetUniqueId(&id));
+  memset(id_out, 0, TFL_COMM_ID_BYTES);
+  memcpy(id_out, &id, sizeof(id));
+  return 0;
+}
+
+int tfl_comm_init(tfl_ctx* ctx, const char* id_bytes, int32_t rank, int32_t world) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!ctx || world < 1 || rank < 0 || rank >= world) return fail(ctx, "comm_init: bad rank / world");
+  tfl_comm_destroy(ctx);
+  ctx->comm_rank = rank;
+  ctx->comm_world = world;
+  if (world == 1 || !id_bytes) return 0;       // nil id: a rank's workload without its neighbours (profiling)
+  NcclApi* nc = nccl_api();
+  if (!nc) return fail(ctx, "comm_init: libnccl.so.2 not found");
+  ncclUniqueId id;
+  memcpy(&id, id_bytes, sizeof(id));
+  TFL_NCCL(ctx, nc->CommInitRank(&ctx->comm, world, id, rank));
+  return 0;
+}
+
+int tfl_comm_destroy(tfl_ctx* ctx) {
+  if (ctx && ctx->comm) {
+    DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+    cudaStreamSynchronize(ctx->stream);
+    nccl_api()->CommDestroy(ctx->comm);
+    ctx->comm = nullptr;
+  }
+  if (ctx) { ctx->comm_rank = 0; ctx->comm_world = 1; }
+  return 0;
+}
+
+void tfl_slab_sim_destroy(tfl_ctx* ctx, tfl_slab_sim* s) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!s) return;
+  if (ctx) cudaStreamSynchronize(ctx->stream);
+  for (int r = 0; r < (int)s->all_inbox.size(); r++) if (r != s->rank && s->all_inbox[r]) cudaIpcCloseMemHandle(s->all_inbox[r]);
+  for (void* p : s->owned) cudaFree(p);
+  for (auto& pr : s->ev) for (cudaEvent_t e : pr) if (e) cudaEventDestroy(e);
+  delete s;
+}
+
+// All host arrays are GLOBAL [c][gnz][ny][nx] fields, identical on every rank; each rank keeps its slab.
+int tfl_slab_sim_create(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32_t margin, const float* flags,
+                        const float* U_bc, const float* U_bc_inv, const float* d_bc, const float* d_bc_inv,
+                        tfl_slab_sim** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!out || !flags || gnz < 3 || ny < 3 || nx < 3 || margin < 2) return fail(ctx, "slab_sim: bad arguments (margin >= 2)");
+  tfl_slab_sim* s = new tfl_slab_sim();
+  memset(&s->st, 0, sizeof(s->st));
+  s->gnz = gnz; s->ny = ny; s->nx = nx; s->margin = margin; s->halo = 2 * margin + 2;
+  s->rank = ctx->comm_rank; s->world = ctx->comm_world;
+  const int base = gnz / s->world, rem = gnz % s->world;
+  if (s->world > 1 && base < s->halo) { delete s; return fail(ctx, "slab_sim: slabs of %d planes are thinner than the halo (%d)", base, s->halo); }
+  s->z0 = s->rank * base + std::min(s->rank, rem);
+  s->z1 = s->z0 + base + (s->rank < rem ? 1 : 0);
+  s->lo_halo = std::min(s->halo, s->z0);
+  s->hi_halo = std::min(s->halo, gnz - s->z1);
+  s->zoff = s->z0 - s->lo_halo;
+  s->nz = (s->z1 - s->z0) + s->lo_halo + s->hi_halo;
+  s->own_lo = s->lo_halo;
+  s->own_hi = s->lo_halo + (s->z1 - s->z0);
+  s->plane = (size_t)ny * nx;
+  s->cells = s->plane * s->nz;
+  const size_t gcells = s->plane * gnz;
+  auto mk = [&](tfl_grid* g, int nc, const float* host) -> int {
+    g->nb = 1; g->nc = nc; g->nz = s->nz; g->ny = ny; g->nx = nx;
+    void* p = nullptr;
+    if (cudaMalloc(&p, s->cells * nc * 4) != cudaSuccess) return 1;
+    s->owned.push_back(p);
+    g->data = (float*)p;
+    if (!host) return cudaMemset(p, 0, s->cells * nc * 4) != cudaSuccess;
+    for (int c = 0; c < nc; c++)
+      if (cudaMemcpy((float*)p + c * s->cells, host + c * gcells + (size_t)s->zoff * s->plane, s->cells * 4,
+                     cudaMemcpyHostToDevice) != cudaSuccess)
+        return 1;
+    return 0;
+  };
+  int bad = 0;
+  bad |= mk(&s->st.flags, 1, flags);
+  bad |= mk(&s->st.p, 1, nullptr);
+  bad |= mk(&s->st.U, 3, nullptr);
+  bad |= mk(&s->st.density, 1, nullptr);
+  if (U_bc && U_bc_inv) { bad |= mk(&s->st.U_bc, 3, U_bc); bad |= mk(&s->st.U_bc_inv_mask, 3, U_bc_inv); }
+  if (d_bc && d_bc_inv) { bad |= mk(&s->st.density_bc, 1, d_bc); bad |= mk(&s->st.density_bc_inv_mask, 1, d_bc_inv); }
+  void* p = nullptr;
+  bad |= cudaMalloc(&p, s->cells * 3 * 4) != cudaSuccess;
+  if (!bad) { s->owned.push_back(p); s->U1 = (float*)p; }
+  bad |= cudaMalloc(&p, 2 * sizeof(double)) != cudaSuccess;
+  if (!bad) { s->owned.push_back(p); s->sums = (double*)p; }
+  s->xbuf_side = (size_t)s->halo * s->plane * 4;          // the widest exchange: halo planes of 4 channels
+  bad |= cudaMalloc(&p, 4 * s->xbuf_side * sizeof(float)) != cudaSuccess;
+  if (!bad) { s->owned.push_back(p); s->xbuf = (float*)p; }
+  if (s->world > 1) {
+    const size_t inbox_bytes = (6 * s->xbuf_side + 64 + kSumAreaFloats) * sizeof(float);
+    bad |= cudaMalloc(&p, inbox_bytes) != cudaSuccess;
+    if (!bad) { s->owned.push_back(p); s->inbox = (float*)p; bad |= cudaMemset(p, 0, inbox_bytes) != cudaSuccess; }
+    bad |= cudaMalloc(&p, sizeof(unsigned int)) != cudaSuccess;
+    if (!bad) { s->owned.push_back(p); s->push_done = (unsigned int*)p; bad |= cudaMemset(p, 0, sizeof(unsigned int)) != cudaSuccess; }
+  }
+  for (auto& pr : s->ev) for (cudaEvent_t& e : pr) bad |= cudaEventCreate(&e) != cudaSuccess;
+  if (bad) { tfl_slab_sim_destroy(ctx, s); return fail(ctx, "slab_sim: allocation failed"); }
+  *out = s;
+  return 0;
+}
+
+// info: zoff, nz, own_lo, own_hi, z0, z1 (local storage and owned planes of this rank)
+int tfl_slab_sim_layout(const tfl_slab_sim* s, tfl_state* state_out, int32_t info[6]) {
+  if (!s) return 1;
+  if (state_out) *state_out = s->st;
+  if (info) { info[0] = s->zoff; info[1] = s->nz; info[2] = s->own_lo; info[3] = s->own_hi; info[4] = s->z0; info[5] = s->z1; }
+  return 0;
+}
+
+// GLOBAL host arrays -> this rank's slab (ghost planes included); any pointer may be NULL.
+int tfl_slab_sim_upload(tfl_ctx* ctx, tfl_slab_sim* s, const float* p, const float* U, const float* density) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!s) return fail(ctx, "slab_sim is nil");
+  const size_t gcells = s->plane * s->gnz, off = (size_t)s->zoff * s->plane;
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (p) TFL_CUDA(ctx, cudaMemcpy(s->st.p.data, p + off, s->cells * 4, cudaMemcpyHostToDevice));
+  if (density) TFL_CUDA(ctx, cudaMemcpy(s->st.density.data, density + off, s->cells * 4, cudaMemcpyHostToDevice));
+  if (U) for (int c = 0; c < 3; c++)
+    TFL_CUDA(ctx, cudaMemcpy(s->st.U.data + c * s->cells, U + c * gcells + off, s->cells * 4, cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// This rank's OWNED planes -> the same planes of GLOBAL host arrays (the rest is left alone).
+int tfl_slab_sim_download(tfl_ctx* ctx, tfl_slab_sim* s, float* p, float* U, float* density) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!s) return fail(ctx, "slab_sim is nil");
+  const size_t gcells = s->plane * s->gnz, goff = (size_t)s->z0 * s->plane, loff = (size_t)s->own_lo * s->plane;
+  const size_t cnt = (size_t)(s->z1 - s->z0) * s->plane * 4;
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (p) TFL_CUDA(ctx, cudaMemcpy(p + goff, s->st.p.data + loff, cnt, cudaMemcpyDeviceToHost));
+  if (density) TFL_CUDA(ctx, cudaMemcpy(density + goff, s->st.density.data + loff, cnt, cudaMemcpyDeviceToHost));
+  if (U) for (int c = 0; c < 3; c++)
+    TFL_CUDA(ctx, cudaMemcpy(U + c * gcells + goff, s->st.U.data + c * s->cells + loff, cnt, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+}  // extern "C"
+
+namespace {
+
+// Gather / scatter of the planes one halo exchange moves: every channel of the listed fields, `cnt` floats per
+// channel and side, to / from one contiguous buffer per neighbour (one NCCL message per neighbour and direction
+// instead of one per channel: 4 p2p operations in the group instead of 16).
+struct SlabPack {
+  float* chan[8];
+  int nchan;
+  long long cnt;                    // floats per channel and side = width * ny * nx
+  long long src_lo, src_hi;         // float offset (within a channel) of the planes sent down / up
+  long long dst_lo, dst_hi;         // ... of the ghost planes filled from below / above
+  float* send_lo; float* send_hi; float* recv_lo; float* recv_hi;     // null: no neighbour on that side
+};
+template <bool UNPACK>
+__global__ void k_slab_pack(SlabPack d) {
+  const long long per_side = d.cnt * d.nchan;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < 2 * per_side; t += (long long)gridDim.x * blockDim.x) {
+    const int side = t >= per_side;
+    const long long r = t - side * per_side;
+    const int c = (int)(r / d.cnt);
+    const long long e = r - c * d.cnt;
+    if (!UNPACK) {
+      float* buf = side ? d.send_hi : d.send_lo;
+      if (buf) buf[r] = d.chan[c][(side ? d.src_hi : d.src_lo) + e];
+    } else {
+      const float* buf = side ? d.recv_hi : d.recv_lo;
+      if (buf) d.chan[c][(side ? d.dst_hi : d.dst_lo) + e] = buf[r];
+    }
+  }
+}
+
+// Peer-memory exchange, sending half: every channel's boundary planes are written straight into the neighbours'
+// inboxes (remote stores over NVLink), and when the last CTA has finished, the step number is stored (system
+// scope, after a system-wide fence) into the neighbours' counters.
+__global__ void k_slab_push(SlabPack d, float* peer_lo_buf, float* peer_hi_buf, unsigned int* peer_lo_flag,
+                            unsigned int* peer_hi_flag, unsigned int step, unsigned int* done) {
+  const long long per_side = d.cnt * d.nchan;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < 2 * per_side; t += (long long)gridDim.x * blockDim.x) {
+    const int side = t >= per_side;
+    const long long r = t - side * per_side;
+    const int c = (int)(r / d.cnt);
+    const long long e = r - c * d.cnt;
+    float* buf = side ? peer_hi_buf : peer_lo_buf;
+    if (buf) buf[r] = d.chan[c][(side ? d.src_hi : d.src_lo) + e];
+  }
+  __threadfence_system();
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned int prev = atomicAdd(done, 1u);
+    if (prev == gridDim.x - 1) {               // every CTA's stores are fenced: publish
+      *done = 0u;
+      __threadfence_system();
+      if (peer_lo_flag) asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(peer_lo_flag), "r"(step) : "memory");
+      if (peer_hi_flag) asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(peer_hi_flag), "r"(step) : "memory");
+    }
+  }
+}
+// ... receiving half: wait until the neighbours' counters have reached this step, then scatter the inbox into the
+// ghost planes.  The wait is bounded (a neighbour that never arrives raises the fault counter instead of hanging
+// the GPU).
+__global__ void k_slab_pull(SlabPack d, const float* buf_lo, const float* buf_hi, const unsigned int* flag_lo,
+                            const unsigned int* flag_hi, unsigned int step, unsigned long long* faults) {
+  __shared__ int ok;
+  if (threadIdx.x == 0) {
+    ok = 1;
+    const long long t0 = clock64();
+    for (int sde = 0; sde < 2; sde++) {
+      const unsigned int* f = sde ? flag_hi : flag_lo;
+      if (!f) continue;
+      for (;;) {
+        unsigned int v;
+        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
+        if ((int)(v - step) >= 0) break;
+        if (clock64() - t0 > 4000000000LL) { ok = 0; break; }       // ~2 s
+        __nanosleep(200);
+      }
+    }
+    if (!ok && blockIdx.x == 0 && faults) atomicAdd(faults, 1ULL);
+  }
+  __syncthreads();
+  if (!ok) return;
+  const long long per_side = d.cnt * d.nchan;
+  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < 2 * per_side; t += (long long)gridDim.x * blockDim.x) {
+    const int side = t >= per_side;
+    const long long r = t - side * per_side;
+    const int c = (int)(r / d.cnt);
+    const long long e = r - c * d.cnt;
+    const float* buf = side ? buf_hi : buf_lo;
+    if (buf) d.chan[c][(side ? d.dst_hi : d.dst_lo) + e] = __ldcg(buf + r);
+  }
+}
+
+// All-reduce of the two partial sums over peer memory: every rank stores its pair into slot [parity][rank] of every
+// rank's inbox and raises that rank's counter [parity][rank]; then waits for all counters of its own inbox and adds
+// the pairs in rank order (the same order on every rank: identical results everywhere, independent of timing).
+// Slots alternate with the step's parity: a rank that is still reading step s cannot be overwritten by step s + 1.
+__device__ __forceinline__ double* sum_slot(float* inbox, size_t xbuf_side, int parity, int r) {
+  return reinterpret_cast<double*>(inbox + 6 * xbuf_side + 64) + ((size_t)parity * 64 + r) * 2;
+}
+__device__ __forceinline__ unsigned int* sum_flag(float* inbox, size_t xbuf_side, int parity, int r) {
+  return reinterpret_cast<unsigned int*>(inbox + 6 * xbuf_side + 64 + 2 * 64 * 2 * 2) + parity * 64 + r;
+}
+__global__ void k_sum_push(const double* __restrict__ mine, float* const* __restrict__ inboxes, size_t xbuf_side, int rank,
+                           int world, unsigned int step) {
+  const int t = threadIdx.x;
+  if (t >= world) return;
+  const int parity = step & 1;
+  double* slot = sum_slot(inboxes[t], xbuf_side, parity, rank);
+  slot[0] = mine[0];
+  slot[1] = mine[1];
+  __threadfence_system();
+  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(sum_flag(inboxes[t], xbuf_side, parity, rank)), "r"(step) : "memory");
+}
+__global__ void k_sum_pull(double* __restrict__ out, float* inbox, size_t xbuf_side, int world, unsigned int step,
+                           unsigned long long* faults) {
+  __shared__ int ok;
+  const int t = threadIdx.x, parity = step & 1;
+  if (t == 0) ok = 1;
+  __syncthreads();
+  if (t < world) {
+    const long long t0 = clock64();
+    for (;;) {
+      unsigned int v;
+      asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(sum_flag(inbox, xbuf_side, parity, t)) : "memory");
+      if ((int)(v - step) >= 0) break;
+      if (clock64() - t0 > 4000000000LL) { ok = 0; break; }
+      __nanosleep(100);
+    }
+  }
+  __syncthreads();
+  if (t == 0) {
+    if (!ok) { if (faults) atomicAdd(faults, 1ULL); return; }
+    double s0 = 0.0, s1 = 0.0;
+    for (int r = 0; r < world; r++) {
+      const volatile double* slot = sum_slot(inbox, xbuf_side, parity, r);
+      s0 += slot[0];
+      s1 += slot[1];
+    }
+    out[0] = s0;
+    out[1] = s1;
+  }
+}
+
+// Refresh `width` ghost planes on both sides of the listed fields from the neighbours' owned planes.
+int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl_grid*> fields, int width, int phase) {
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][0], ctx->stream));
+  s->bytes_sent[phase] = 0;
+  if (s->world > 1 && width > 0 && (ctx->comm || s->peer_ok)) {
+    if (width > s->halo) return fail(ctx, "slab exchange of %d planes exceeds the halo (%d)", width, s->halo);
+    SlabPack d;
+    d.nchan = 0;
+    for (const tfl_grid* f : fields)
+      for (int c = 0; c < f->nc && d.nchan < 8; c++) d.chan[d.nchan++] = f->data + (size_t)c * s->cells;
+    d.cnt = (long long)width * s->plane;
+    d.src_lo = (long long)s->own_lo * s->plane;
+    d.src_hi = (long long)(s->own_hi - width) * s->plane;
+    d.dst_lo = (long long)(s->own_lo - width) * s->plane;
+    d.dst_hi = (long long)s->own_hi * s->plane;
+    const size_t side = (size_t)d.cnt * d.nchan;                  // floats per message
+    if (side > s->xbuf_side) return fail(ctx, "slab exchange buffer too small");
+    const bool lo = s->rank > 0, hi = s->rank < s->world - 1;
+    const int blocks = (int)std::min<size_t>((2 * side + 255) / 256, 132 * 4);
+    if (s->peer_ok) {
+      // inbox layout: buffer (phase, from-below = 0 / from-above = 1) at ((phase * 2 + from) * xbuf_side), counters behind
+      auto buf = [&](float* base, int from) { return base + ((size_t)phase * 2 + from) * s->xbuf_side; };
+      auto flag = [&](float* base, int from) { return (unsigned int*)(base + 6 * s->xbuf_side) + phase * 2 + from; };
+      d.send_lo = d.send_hi = d.recv_lo = d.recv_hi = nullptr;
+      // my first owned planes land in the lower neighbour's "from above" slot, my last ones in the upper neighbour's "from below"
+      k_slab_push<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(s->peer_inbox[0], 1) : nullptr, hi ? buf(s->peer_inbox[1], 0) : nullptr,
+                                                   lo ? flag(s->peer_inbox[0], 1) : nullptr, hi ? flag(s->peer_inbox[1], 0) : nullptr,
+                                                   s->step_no, s->push_done);
+      k_slab_pull<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(s->inbox, 0) : nullptr, hi ? buf(s->inbox, 1) : nullptr,
+                                                   lo ? flag(s->inbox, 0) : nullptr, hi ? flag(s->inbox, 1) : nullptr,
+                                                   s->step_no, ctx->counters);
+      s->bytes_sent[phase] = (size_t)(lo + hi) * side * 4;
+      ctx->launches += 2;
+    } else {
+      NcclApi* nc = nccl_api();
+      d.send_lo = lo ? s->xbuf : nullptr;
+      d.send_hi = hi ? s->xbuf + s->xbuf_side : nullptr;
+      d.recv_lo = lo ? s->xbuf + 2 * s->xbuf_side : nullptr;
+      d.recv_hi = hi ? s->xbuf + 3 * s->xbuf_side : nullptr;
+      k_slab_pack<false><<<blocks, 256, 0, ctx->stream>>>(d);
+      TFL_NCCL(ctx, nc->GroupStart());
+      if (lo) {                                       // lower neighbour: my first owned planes go down
+        TFL_NCCL(ctx, nc->Send(d.send_lo, side, ncclFloat, s->rank - 1, ctx->comm, ctx->stream));
+        TFL_NCCL(ctx, nc->Recv(d.recv_lo, side, ncclFloat, s->rank - 1, ctx->comm, ctx->stream));
+        s->bytes_sent[phase] += side * 4;
+      }
+      if (hi) {                                       // upper neighbour
+        TFL_NCCL(ctx, nc->Send(d.send_hi, side, ncclFloat, s->rank + 1, ctx->comm, ctx->stream));
+        TFL_NCCL(ctx, nc->Recv(d.recv_hi, side, ncclFloat, s->rank + 1, ctx->comm, ctx->stream));
+        s->bytes_sent[phase] += side * 4;
+      }
+      TFL_NCCL(ctx, nc->GroupEnd());
+      k_slab_pack<true><<<blocks, 256, 0, ctx->stream>>>(d);
+      ctx->launches += 2;
+    }
+  }
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][1], ctx->stream));
+  return 0;
+}
+
+struct SlabScope {       // slab placement of the context for the enclosed calls
+  tfl_ctx* ctx;
+  SlabScope(tfl_ctx* c, const tfl_slab_sim* s, int zlo, int zhi) : ctx(c) {
+    c->slab = true; c->zoff = s->zoff; c->gnz = s->gnz; c->zlo = zlo; c->zhi = zhi; c->slab_margin = s->margin;
+  }
+  ~SlabScope() { ctx->slab = false; ctx->slab_margin = 2; }
+};
+
+}  // namespace
+
+extern "C" {
+
+// One tfluids.simulate (convnet path, lib/simulate.lua:175-327) on this rank's slab.  Asynchronous.
+int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cnn* cnn) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!s || !mc || !cnn) return fail(ctx, "slab_sim_step: nil argument");
+  if (mc->sim_method != TFL_SIM_CONVNET) return fail(ctx, "slab_sim_step: only simMethod 'convnet' is decomposed");
+  if (cnn->nbanks > 1) return fail(ctx, "slab_sim_step: banked models run on whole grids only, not on z-slabs");
+  if (s->world != ctx->comm_world || s->rank != ctx->comm_rank) return fail(ctx, "slab_sim_step: communicator changed");
+  const tfl_state& st = s->st;
+  s->step_no += 1;                      // what the peers' counters must reach in this step's exchanges
+  struct StepMark {                     // the flags are refreshed once per step (the two advections share them)
+    tfl_ctx* c;
+    explicit StepMark(tfl_ctx* cc) : c(cc) { c->in_slab_step = true; c->fcache.fresh_for = nullptr; }
+    ~StepMark() { c->in_slab_step = false; c->fcache.fresh_for = nullptr; }
+  } mark_(ctx);
+  auto bcs = [&]() -> int {           // on the owned planes: ghost planes are always refreshed from their owners
+    SlabScope scope(ctx, s, s->own_lo, s->own_hi);
+    if (st.U_bc.data && tfl_apply_bc(ctx, &st.U, &st.U_bc_inv_mask, &st.U_bc)) return 1;
+    if (st.density_bc.data && tfl_apply_bc(ctx, &st.density, &st.density_bc_inv_mask, &st.density_bc)) return 1;
+    return 0;
+  };
+  if (slab_exchange(ctx, s, {&st.U, &st.density}, s->halo, 0)) return 1;
+  {
+    SlabScope scope(ctx, s, s->own_lo, s->own_hi);
+    if (tfl_advect_scalar(ctx, mc->dt, &st.density, &st.U, &st.flags, mc->advection_method, 0, mc->maccormack_strength, nullptr)) return 1;
+    if (tfl_advect_vel(ctx, mc->dt, &st.U, &st.flags, mc->advection_method, mc->maccormack_strength, nullptr)) return 1;
+  }
+  if (bcs()) return 1;
+  if (slab_exchange(ctx, s, {&st.U, &st.density}, 4, 1)) return 1;
+  const StepForces fo = step_forces(mc, s->nx, s->ny, s->gnz);
+  {
+    // point-wise forces also on the three ghost planes the confinement stencil reads across the cut
+    SlabScope scope(ctx, s, s->own_lo - std::min(3, s->lo_halo), s->own_hi + std::min(3, s->hi_halo));
+    if (fo.buoyancy && tfl_add_buoyancy(ctx, &st.U, &st.flags, &st.density, fo.buoy, mc->dt)) return 1;
+    if (fo.gravity && tfl_add_gravity(ctx, &st.U, &st.flags, fo.grav, mc->dt)) return 1;
+  }
+  if (fo.vorticity) {
+    SlabScope scope(ctx, s, s->own_lo, s->own_hi);
+    if (tfl_vorticity_confinement(ctx, &st.U, &st.flags, fo.vort_amp)) return 1;
+  }
+  if (bcs()) return 1;
+  if (slab_exchange(ctx, s, {&st.U, &st.p}, 5, 2)) return 1;
+  tfl_grid u1 = st.U;
+  u1.data = s->U1;
+  {
+    SlabScope scope(ctx, s, s->own_lo, s->own_hi);
+    if (tfl_cnn_stats(ctx, &st.U, &st.flags, &u1, s->sums)) return 1;
+  }
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0], ctx->stream));
+  if (s->world > 1 && s->peer_ok && s->all_inbox_dev) {
+    k_sum_push<<<1, 64, 0, ctx->stream>>>(s->sums, s->all_inbox_dev, s->xbuf_side, s->rank, s->world, s->step_no);
+    k_sum_pull<<<1, 64, 0, ctx->stream>>>(s->sums, s->inbox, s->xbuf_side, s->world, s->step_no, ctx->counters);
+    ctx->launches += 2;
+  } else if (s->world > 1 && ctx->comm) {
+    TFL_NCCL(ctx, nccl_api()->AllReduce(s->sums, s->sums, 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
+  }
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][1], ctx->stream));
+  {
+    SlabScope scope(ctx, s, s->own_lo, s->own_hi);
+    if (tfl_cnn_project_from_sums(ctx, cnn, &st.p, &u1, &st.flags, s->sums, &st.p, &st.U, mc->normalize_input_threshold)) return 1;
+  }
+  if (bcs()) return 1;
+  SlabScope scope(ctx, s, s->own_lo, s->own_hi);
+  return tfl_clamp(ctx, &st.U, -1e6f, 1e6f);
+}
+
+// Peer-memory halos: export this rank's inbox (64-byte CUDA IPC handle) ...
+int tfl_slab_sim_ipc_export(tfl_ctx* ctx, tfl_slab_sim* s, char* handle_out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!s || !handle_out) return fail(ctx, "slab_sim_ipc_export: nil argument");
+  if (!s->inbox) return fail(ctx, "slab_sim_ipc_export: a single rank has no neighbours");
+  static_assert(sizeof(cudaIpcMemHandle_t) <= TFL_IPC_HANDLE_BYTES, "IPC handle fits the ABI buffer");
+  cudaIpcMemHandle_t h;
+  TFL_CUDA(ctx, cudaIpcGetMemHandle(&h, s->inbox));
+  memset(handle_out, 0, TFL_IPC_HANDLE_BYTES);
+  memcpy(handle_out, &h, sizeof(h));
+  return 0;
+}
+
+// ... and map every rank's (handles: world x TFL_IPC_HANDLE_BYTES in rank order; NULL switches back to NCCL).
+// From then on tfl_slab_sim_step exchanges halos with push / pull kernels over NVLink instead of NCCL send / recv
+// and reduces the two sums through the same inboxes.  Every rank must connect before any rank steps (the host
+// application's barrier).
+int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* s, const char* handles) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!s || !s->inbox) return fail(ctx, "slab_sim_ipc_connect: nil argument");
+  auto drop = [&]() {
+    for (int r = 0; r < (int)s->all_inbox.size(); r++)
+      if (r != s->rank && s->all_inbox[r]) cudaIpcCloseMemHandle(s->all_inbox[r]);
+    s->all_inbox.clear();
+    s->peer_inbox[0] = s->peer_inbox[1] = nullptr;
+    s->peer_ok = false;
+  };
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  drop();
+  if (!handles) return 0;                          // back to NCCL (e.g. another rank could not map its peers)
+  if (s->world > 64) return fail(ctx, "slab_sim_ipc_connect: more than 64 ranks");
+  s->all_inbox.assign(s->world, nullptr);
+  s->all_inbox[s->rank] = s->inbox;
+  for (int r = 0; r < s->world; r++) {
+    if (r == s->rank) continue;
+    cudaIpcMemHandle_t h;
+    memcpy(&h, handles + (size_t)r * TFL_IPC_HANDLE_BYTES, sizeof(h));
+    void* q = nullptr;
+    const cudaError_t e = cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess);
+    if (e != cudaSuccess) {
+      cudaGetLastError();
+      drop();
+      return fail(ctx, "slab_sim_ipc_connect: cudaIpcOpenMemHandle(rank %d): %s (the exchanges stay on NCCL)", r, cudaGetErrorString(e));
+    }
+    s->all_inbox[r] = (float*)q;
+  }
+  if (!s->all_inbox_dev) {
+    void* p = nullptr;
+    TFL_CUDA(ctx, cudaMalloc(&p, 64 * sizeof(float*)));
+    s->owned.push_back(p);
+    s->all_inbox_dev = (float**)p;
+  }
+  TFL_CUDA(ctx, cudaMemcpy(s->all_inbox_dev, s->all_inbox.data(), s->world * sizeof(float*), cudaMemcpyHostToDevice));
+  if (s->rank > 0) s->peer_inbox[0] = s->all_inbox[s->rank - 1];
+  if (s->rank < s->world - 1) s->peer_inbox[1] = s->all_inbox[s->rank + 1];
+  s->peer_ok = true;
+  return 0;
+}
+
+// Device time of the last step's three halo exchanges and of its all-reduce (ms) and the bytes this rank sent in
+// each exchange.  Synchronises.
+int tfl_slab_sim_exchange_stats(tfl_ctx* ctx, tfl_slab_sim* s, float ms[4], int64_t bytes[3]) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!s) return fail(ctx, "slab_sim is nil");
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  for (int i = 0; i < 4; i++) {
+    ms[i] = 0.0f;
+    if (cudaEventElapsedTime(&ms[i], s->ev[i][0], s->ev[i][1]) != cudaSuccess) { cudaGetLastError(); ms[i] = -1.0f; }
+  }
+  for (int i = 0; i < 3; i++) bytes[i] = (int64_t)s->bytes_sent[i];
+  return 0;
+}
+
+}  // extern "C"

@@ -1,7 +1,7 @@
 // MAC-grid stencil kernels of the Eulerian step (everything except the conv stack).
 // Compiled with -fmad=false: results are bit-identical to the reference CPU operators
 // (see oracle/ and tests/).  One thread per cell, x fastest (coalesced rows); neighbour
-// reuse comes from L1/L2.  Launchers at the bottom are called by tfl_api.cu.
+// reuse comes from L1/L2.  Launchers at the bottom are called by the operators of tfl_api.cu.
 //
 // Reference operators restated here (paths relative to /root/reference/torch/tfluids):
 //   advectScalar   third_party/tfluids.cc:23-588     advectVel   third_party/tfluids.cc:594-920
