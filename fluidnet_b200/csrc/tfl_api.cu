@@ -600,25 +600,36 @@ int tfl_precond_from_string(const char* name) {
   return -1;
 }
 
-int tfl_solve_linear_system_pcg(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
-                                int is_3d, int precond, float tol, int max_iter, float* residual,
-                                int* iterations) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, p, "p") || check_scalar(ctx, div, "div")) return 1;
-  if (!same_spatial(flags, p) || !same_spatial(flags, div)) return fail(ctx, "size mismatch");
+// Arguments and workspace of the PCG entry points (the solve and the preconditioner hook): out and rhs are the
+// scalar grids written and read beside flags.
+static int pcg_check_args(tfl_ctx* ctx, const tfl_grid* out, const char* out_name, const tfl_grid* flags,
+                          const tfl_grid* rhs, const char* rhs_name, int is_3d, int precond) {
+  if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, out, out_name) || check_scalar(ctx, rhs, rhs_name)) return 1;
+  if (!same_spatial(flags, out) || !same_spatial(flags, rhs)) return fail(ctx, "size mismatch");
   if (!is_3d && flags->nz != 1) return fail(ctx, "d > 1 for a 2D domain");
   if (precond < TFL_PRECOND_NONE || precond > TFL_PRECOND_IC0)
     return fail(ctx, "Incorrect preconType ('none', 'ic0', 'ilu0')");      // generic/tfluids.cu:1551
   if (ctx->slab) return fail(ctx, "PCG does not shard (triangular solves): single GPU only");
   if ((long long)flags->nb * flags->nz * flags->ny * flags->nx >= (1ll << 31)) return fail(ctx, "PCG: grid too large");
-  if (arena_reserve(ctx, pcg_workspace_bytes(flags->nb, flags->nz, flags->ny, flags->nx))) return 1;
+  return arena_reserve(ctx, pcg_workspace_bytes(flags->nb, flags->nz, flags->ny, flags->nx)) ? 1 : 0;
+}
+
+static int pcg_report(tfl_ctx* ctx, int rc, const char* what) {
+  if (rc == 3) return fail(ctx, "%s: %s", what, cudaGetErrorString(cudaGetLastError()));
+  if (rc) return fail(ctx, "%s", pcg_status_string(rc));
+  return check_launch(ctx, what);
+}
+
+int tfl_solve_linear_system_pcg(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
+                                int is_3d, int precond, float tol, int max_iter, float* residual,
+                                int* iterations) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (pcg_check_args(ctx, p, "p", flags, div, "div", is_3d, precond)) return 1;
   const int rc = pcg_solve(ctx->pcg, ctx->arena, p->data, flags->data, div->data, flags->nb, flags->nz, flags->ny,
                            flags->nx, is_3d, precond, tol, max_iter, residual, iterations, &ctx->launches,
                            ctx->stream);
-  if (rc == 3) { cudaError_t e = cudaGetLastError(); return fail(ctx, "solveLinearSystemPCG: %s", cudaGetErrorString(e)); }
-  if (rc) return fail(ctx, "%s", pcg_status_string(rc));
-  return check_launch(ctx, "solveLinearSystemPCG");
+  return pcg_report(ctx, rc, "solveLinearSystemPCG");
 }
 
 int tfl_normalize_pressure_mean(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags, int is_3d) {
@@ -740,6 +751,19 @@ extern "C" int tfl_debug_pcg_groups(tfl_ctx* ctx, int groups) {
   if (!ctx) return 1;
   ctx->pcg.groups_override = groups;
   return 0;
+}
+
+// Debug hook: the PCG preconditioner alone, z = M^-1 r (0 outside every system of two or more cells),
+// through the labelling, system build and sweeps of tfl_solve_linear_system_pcg.  geometry (4 ints, may be
+// null): NYP, planes per CTA, plane chunks, cooperative grid of the sweeps.
+extern "C" int tfl_debug_pcg_precond(tfl_ctx* ctx, const tfl_grid* z, const tfl_grid* flags, const tfl_grid* r,
+                                     int is_3d, int precond, int* geometry) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (pcg_check_args(ctx, z, "z", flags, r, "r", is_3d, precond)) return 1;
+  const int rc = pcg_precond(ctx->pcg, ctx->arena, z->data, flags->data, r->data, flags->nb, flags->nz, flags->ny,
+                             flags->nx, is_3d, precond, geometry, &ctx->launches, ctx->stream);
+  return pcg_report(ctx, rc, "pcg precond");
 }
 
 extern "C" int tfl_debug_pcg_timing(tfl_ctx* ctx, void* dev_buf) {

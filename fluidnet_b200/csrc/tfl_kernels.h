@@ -129,6 +129,11 @@ const char* pcg_status_string(int rc);
 int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, const float* div, int nb, int nz, int ny,
               int nx, int is3d, int precond, float tol, int max_iter, float* residual, int* iterations,
               long long* launches, cudaStream_t st);
+// Debug: the preconditioner alone.  Same labelling, system and sweeps as pcg_solve; z = M^-1 r in the
+// natural layout (0 outside every system of two or more cells); geometry = NYP, planes per CTA,
+// chunks, cooperative grid of the sweeps.  Synchronises `st`.
+int pcg_precond(PcgScratch& sc, void* workspace, float* z, const float* flags, const float* r, int nb, int nz, int ny,
+                int nx, int is3d, int precond, int* geometry, long long* launches, cudaStream_t st);
 void pcg_release(PcgScratch& sc);
 int normalize_pressure_mean(void* workspace, float* p, const float* flags, int nb, int nz, int ny, int nx, int is3d,
                             long long* launches, cudaStream_t st);

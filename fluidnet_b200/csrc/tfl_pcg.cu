@@ -295,9 +295,10 @@ __global__ void k_xsum(const unsigned short* __restrict__ cf, const int* __restr
 }
 
 // copyPressureFromSystem (:1165-1188): p = x - mean(x of the component); cells outside any solved
-// system keep the 0 of THCudaTensor_zero (:1337).
+// system keep the 0 of THCudaTensor_zero (:1337).  remove_mean = 0: x as it is (the preconditioner hook).
 __global__ void k_writeback(float* __restrict__ p, const int* __restrict__ parent, const int* __restrict__ csize,
-                            const int* __restrict__ cid, const float* __restrict__ x, CompScalars sc, PcgGeo g) {
+                            const int* __restrict__ cid, const float* __restrict__ x, CompScalars sc, PcgGeo g,
+                            int remove_mean) {
   const long long c = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (c >= g.n * g.nb) return;
   float out = 0.0f;
@@ -307,7 +308,7 @@ __global__ void k_writeback(float* __restrict__ p, const int* __restrict__ paren
     const int b = (int)(c / g.n);
     const long long cc = c % g.n;
     const int i = (int)(cc % g.nx), j = (int)((cc / g.nx) % g.ny), k = (int)(cc / ((long long)g.nx * g.ny));
-    const float mean = (float)(sc.xsum[id] / (double)sc.cnt[id]);
+    const float mean = remove_mean ? (float)(sc.xsum[id] / (double)sc.cnt[id]) : 0.0f;
     out = x[skew_index(g, b * g.nz + k, j, i)] - mean;
   }
   p[c] = out;
@@ -479,7 +480,10 @@ __global__ void __launch_bounds__(1024, 1) k_sweep(SweepArgs a, PcgGeo g) {
           const Slot f = ring[u];
           const int prv = (u & 1) ^ 1;            // tick0 is a multiple of 4: parities are compile-time
           const float ym = sm[prv * W];
-          const float zm = (gq > 0 ? sm[prv * W + below_off] : f.nb * f.nb2) * use_z;
+          // The plane below passes on * pre * y of its cell through shared memory; global memory holds
+          // only pre and y, so that term is masked with THIS cell's bit (a fluid z-neighbour belongs to
+          // the same component, and an un-preconditioned cell must reduce to z = r).
+          const float zm = (gq > 0 ? sm[prv * W + below_off] : ((f.c & kPreOn) ? f.nb * f.nb2 : 0.0f)) * use_z;
           const float on = (f.c & kPreOn) ? 1.0f : 0.0f;
           float out;
           if (FACTOR) {
@@ -628,11 +632,33 @@ const char* pcg_status_string(int rc) {
   }
 }
 
-int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, const float* div, int nb, int nz, int ny,
-              int nx, int is3d, int precond, float tol, int max_iter, float* residual, int* iterations,
-              long long* launches, cudaStream_t st) {
-#define PCG_CUDA(call) do { if ((call) != cudaSuccess) return 3; } while (0)
+namespace {
+
+// What the solve and the preconditioner hook share: geometry, components, the system arrays in the
+// skewed layout, the per-component scalars and the launch shape of the sweeps.
+struct PcgSystem {
   PcgGeo g;
+  int *parent, *csize, *cid;
+  unsigned short* cf;
+  int* comp;
+  float *r, *z, *pre, *p0, *p1, *w, *x;
+  int* header;                 // [0] active, [1] nan, [2] faults, [3] ncomp, [4] border status
+  int ncomp;
+  CompScalars cs;
+  SweepArgs sa;
+  int sweep_threads, sweep_grid;
+  size_t sweep_smem;
+  unsigned ew_blocks;
+};
+
+#define PCG_CUDA(call) do { if ((call) != cudaSuccess) return 3; } while (0)
+
+// Geometry and launch shape of the sweeps, labelling, and (when there is a system of two or more
+// cells, s.ncomp > 0) the per-component scalars, the progress words and the system arrays.  `out`
+// is zeroed: cells outside every system keep that 0.  Returns 0 or a status for pcg_status_string.
+int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, const float* div, int nb, int nz,
+              int ny, int nx, int is3d, int precond, long long* launches, cudaStream_t st, PcgSystem& s) {
+  PcgGeo& g = s.g;
   g.nx = nx; g.ny = ny; g.nz = nz; g.nb = nb; g.is3d = is3d ? 1 : 0;
   g.S = nx + ny - 1;
   g.NYP = (ny + 31) / 32 * 32;
@@ -656,41 +682,44 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
     PCG_CUDA(cudaFuncSetAttribute(k_sweep<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     PCG_CUDA(cudaFuncSetAttribute(k_sweep<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
   }
+  s.sweep_threads = g.GP * g.NYP + 64;
+  s.sweep_smem = (size_t)g.GP * 2 * (g.NYP + 2) * sizeof(float);
+  int occ = 0;
+  PCG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_sweep<false>, s.sweep_threads, s.sweep_smem));
+  if (occ < 1) return 3;
+  s.sweep_grid = std::min(g.chunks, occ * sc.sm_count);
+  s.ew_blocks = (unsigned)std::min<long long>((g.slots + 255) / 256, (long long)sc.sm_count * 8);
   // carve the workspace
   char* base = (char*)workspace;
   size_t off = 0;
   auto take = [&](size_t bytes) { off = (off + 255) & ~(size_t)255; char* r_ = base + off; off += bytes; return r_; };
-  int* parent = (int*)take(cells * 4);
-  int* csize = (int*)take(cells * 4);
-  int* cid = (int*)take(cells * 4);
-  unsigned short* cf = (unsigned short*)take(g.slots * 2);
-  int* comp = (int*)take(g.slots * 4);
-  float* r = (float*)take(g.slots * 4);
-  float* z = (float*)take(g.slots * 4);
-  float* pre = (float*)take(g.slots * 4);
-  float* p0 = (float*)take(g.slots * 4);
-  float* p1 = (float*)take(g.slots * 4);
-  float* w = (float*)take(g.slots * 4);
-  float* x = (float*)take(g.slots * 4);
-  int* header = (int*)take(64);               // [0] active, [1] nan, [2] faults, [3] ncomp, [4] border status
+  s.parent = (int*)take(cells * 4);
+  s.csize = (int*)take(cells * 4);
+  s.cid = (int*)take(cells * 4);
+  s.cf = (unsigned short*)take(g.slots * 2);
+  s.comp = (int*)take(g.slots * 4);
+  s.r = (float*)take(g.slots * 4);
+  s.z = (float*)take(g.slots * 4);
+  s.pre = (float*)take(g.slots * 4);
+  s.p0 = (float*)take(g.slots * 4);
+  s.p1 = (float*)take(g.slots * 4);
+  s.w = (float*)take(g.slots * 4);
+  s.x = (float*)take(g.slots * 4);
+  s.header = (int*)take(64);
 
-  PCG_CUDA(cudaMemsetAsync(header, 0, 64, st));
-  PCG_CUDA(cudaMemsetAsync(csize, 0, cells * 4, st));
-  k_label_init<<<blocks_for(cells), 256, 0, st>>>(flags, parent, g, header + 4);
-  k_label_union<false><<<blocks_for(cells), 256, 0, st>>>(parent, g, header + 4);
-  k_label_flatten<<<blocks_for(cells), 256, 0, st>>>(parent, csize, g);
-  k_label_assign<<<blocks_for(cells), 256, 0, st>>>(parent, csize, cid, g, header + 3);
+  PCG_CUDA(cudaMemsetAsync(s.header, 0, 64, st));
+  PCG_CUDA(cudaMemsetAsync(s.csize, 0, cells * 4, st));
+  k_label_init<<<blocks_for(cells), 256, 0, st>>>(flags, s.parent, g, s.header + 4);
+  k_label_union<false><<<blocks_for(cells), 256, 0, st>>>(s.parent, g, s.header + 4);
+  k_label_flatten<<<blocks_for(cells), 256, 0, st>>>(s.parent, s.csize, g);
+  k_label_assign<<<blocks_for(cells), 256, 0, st>>>(s.parent, s.csize, s.cid, g, s.header + 3);
   *launches += 4;
-  PCG_CUDA(cudaMemcpyAsync(sc.host, header, 32, cudaMemcpyDeviceToHost, st));
+  PCG_CUDA(cudaMemcpyAsync(sc.host, s.header, 32, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
   if (sc.host[4]) return 1;
-  const int ncomp = sc.host[3];
-  PCG_CUDA(cudaMemsetAsync(p, 0, cells * 4, st));                       // :1337
-  if (ncomp == 0) {
-    if (residual) *residual = -INFINITY;                               // :1343
-    if (iterations) *iterations = 0;
-    return 0;
-  }
+  const int ncomp = s.ncomp = sc.host[3];
+  PCG_CUDA(cudaMemsetAsync(out, 0, cells * 4, st));                     // :1337
+  if (ncomp == 0) return 0;
   // per-component scalars
   const size_t per = 6 * 8 + 3 * 4;
   if ((size_t)ncomp * per + 256 > sc.comp_cap) {
@@ -699,14 +728,14 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
     PCG_CUDA(cudaMalloc(&sc.comp_buf, sc.comp_cap));
   }
   PCG_CUDA(cudaMemsetAsync(sc.comp_buf, 0, (size_t)ncomp * per + 256, st));
-  CompScalars cs;
+  CompScalars& cs = s.cs;
   {
     double* d = (double*)sc.comp_buf;
     cs.rz_new = d; cs.rz_old = d + ncomp; cs.pw = d + 2 * (size_t)ncomp; cs.rr_new = d + 3 * (size_t)ncomp;
     cs.rr_cur = d + 4 * (size_t)ncomp; cs.xsum = d + 5 * (size_t)ncomp;
     int* q = (int*)(d + 6 * (size_t)ncomp);
     cs.cnt = q; cs.done = q + ncomp; cs.iters = q + 2 * (size_t)ncomp;
-    cs.header = header;
+    cs.header = s.header;
   }
   if ((size_t)g.chunks * 2 > sc.prog_cap) {
     if (sc.prog) cudaFree(sc.prog);
@@ -716,51 +745,70 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
     sc.epoch = 0;
   }
   // system arrays
-  PCG_CUDA(cudaMemsetAsync(cf, 0, g.slots * 2, st));
-  PCG_CUDA(cudaMemsetAsync(comp, 0xff, g.slots * 4, st));
-  for (float* v : {r, z, pre, p0, p1, w, x}) PCG_CUDA(cudaMemsetAsync(v, 0, g.slots * 4, st));
-  k_build<<<blocks_for(cells), 256, 0, st>>>(flags, div, parent, csize, cid, cf, comp, r, cs.cnt, g, precond);
+  PCG_CUDA(cudaMemsetAsync(s.cf, 0, g.slots * 2, st));
+  PCG_CUDA(cudaMemsetAsync(s.comp, 0xff, g.slots * 4, st));
+  for (float* v : {s.r, s.z, s.pre, s.p0, s.p1, s.w, s.x}) PCG_CUDA(cudaMemsetAsync(v, 0, g.slots * 4, st));
+  k_build<<<blocks_for(cells), 256, 0, st>>>(flags, div, s.parent, s.csize, s.cid, s.cf, s.comp, s.r, cs.cnt, g,
+                                             precond);
   *launches += 1;
 
-  const unsigned ew_blocks = (unsigned)std::min<long long>((g.slots + 255) / 256, (long long)sc.sm_count * 8);
-  const int no_precond = precond == 0;
-  SweepArgs sa;
-  sa.cf = cf; sa.comp = comp; sa.r = r; sa.z = z; sa.pre = pre;
+  SweepArgs& sa = s.sa;
+  sa.cf = s.cf; sa.comp = s.comp; sa.r = s.r; sa.z = s.z; sa.pre = s.pre;
   sa.prog_f = sc.prog; sa.prog_b = sc.prog + g.chunks;
-  sa.rz = cs.rz_new; sa.faults = header + 2;
+  sa.rz = cs.rz_new; sa.faults = s.header + 2;
   sa.timing = (unsigned long long*)sc.debug_timing;
-  const int sweep_threads = g.GP * g.NYP + 64;
-  const size_t sweep_smem = (size_t)g.GP * 2 * (g.NYP + 2) * sizeof(float);
-  int occ = 0;
-  PCG_CUDA(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&occ, k_sweep<false>, sweep_threads, sweep_smem));
-  if (occ < 1) return 3;
-  const int sweep_grid = std::min(g.chunks, occ * sc.sm_count);
-  auto launch_sweep = [&](bool factor) -> cudaError_t {
-    sa.base = sc.epoch;
-    sc.epoch += (unsigned long long)g.S + 1;
-    void* args[] = {(void*)&sa, (void*)&g};
-    *launches += 1;
-    return cudaLaunchCooperativeKernel(factor ? (void*)k_sweep<true> : (void*)k_sweep<false>, dim3(sweep_grid),
-                                       dim3(sweep_threads), args, sweep_smem, st);
-  };
-  if (!no_precond) PCG_CUDA(launch_sweep(true));
-  k_rr_init<<<ew_blocks, 256, 0, st>>>(cf, comp, r, cs, g.slots);
+  return 0;
+}
+
+// One cooperative launch of the sweep pipeline: the IC(0) factor (pre) or one solve z = M^-1 r.
+cudaError_t launch_sweep(PcgScratch& sc, PcgSystem& s, bool factor, long long* launches, cudaStream_t st) {
+  s.sa.base = sc.epoch;
+  sc.epoch += (unsigned long long)s.g.S + 1;
+  void* args[] = {(void*)&s.sa, (void*)&s.g};
+  *launches += 1;
+  return cudaLaunchCooperativeKernel(factor ? (void*)k_sweep<true> : (void*)k_sweep<false>, dim3(s.sweep_grid),
+                                     dim3(s.sweep_threads), args, s.sweep_smem, st);
+}
+
+}  // namespace
+
+int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, const float* div, int nb, int nz, int ny,
+              int nx, int is3d, int precond, float tol, int max_iter, float* residual, int* iterations,
+              long long* launches, cudaStream_t st) {
+  PcgSystem s;
+  const int rc = pcg_setup(sc, workspace, p, flags, div, nb, nz, ny, nx, is3d, precond, launches, st, s);
+  if (rc) return rc;
+  if (s.ncomp == 0) {
+    if (residual) *residual = -INFINITY;                               // :1343
+    if (iterations) *iterations = 0;
+    return 0;
+  }
+  const PcgGeo& g = s.g;
+  const long long cells = g.n * nb;
+  const int ncomp = s.ncomp;
+  const CompScalars& cs = s.cs;
+  int* header = s.header;
+  const unsigned ew_blocks = s.ew_blocks;
+  const int no_precond = precond == 0;
+  if (!no_precond) PCG_CUDA(launch_sweep(sc, s, true, launches, st));
+  k_rr_init<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, s.r, cs, g.slots);
   const double tol2 = (double)tol * (double)tol;
   k_scalars<<<(ncomp + 255) / 256, 256, 0, st>>>(cs, ncomp, tol2, max_iter, 1, no_precond);
   *launches += 2;
   PCG_CUDA(cudaMemcpyAsync(sc.host, header, 16, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
-  float* p_old = p0;
-  float* p_new = p1;
+  float* p_old = s.p0;
+  float* p_new = s.p1;
   // The host only needs to learn when every component has terminated; termination itself (tolerance or
   // iteration cap) is decided per component on the device, so reading back every 4th iteration changes
   // nothing in the result -- iterations past a component's end are no-ops for it.
   while (sc.host[0] > 0 && !sc.host[1] && !sc.host[2]) {
     for (int rep = 0; rep < 4; rep++) {
       PCG_CUDA(cudaMemsetAsync(header, 0, 4, st));
-      if (!no_precond) PCG_CUDA(launch_sweep(false));
-      k_direction_spmv<<<ew_blocks, g.NYP, 0, st>>>(cf, comp, no_precond ? r : z, p_old, p_new, w, cs, g, no_precond);
-      k_update<<<ew_blocks, 256, 0, st>>>(cf, comp, p_new, w, x, r, cs, g.slots, no_precond);
+      if (!no_precond) PCG_CUDA(launch_sweep(sc, s, false, launches, st));
+      k_direction_spmv<<<ew_blocks, g.NYP, 0, st>>>(s.cf, s.comp, no_precond ? s.r : s.z, p_old, p_new, s.w, cs, g,
+                                                    no_precond);
+      k_update<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, p_new, s.w, s.x, s.r, cs, g.slots, no_precond);
       k_scalars<<<(ncomp + 255) / 256, 256, 0, st>>>(cs, ncomp, tol2, max_iter, 0, no_precond);
       *launches += 3;
       float* tswap = p_old; p_old = p_new; p_new = tswap;
@@ -770,8 +818,8 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   }
   if (sc.host[2]) return 5;
   if (sc.host[1]) return 2;
-  k_xsum<<<ew_blocks, 256, 0, st>>>(cf, comp, x, cs, g.slots);
-  k_writeback<<<blocks_for(cells), 256, 0, st>>>(p, parent, csize, cid, x, cs, g);
+  k_xsum<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, s.x, cs, g.slots);
+  k_writeback<<<blocks_for(cells), 256, 0, st>>>(p, s.parent, s.csize, s.cid, s.x, cs, g, 1);
   *launches += 2;
   // residual = max over components of sqrt(r.r) (:1728), iterations = the longest component
   std::vector<double> rr(ncomp);
@@ -779,7 +827,7 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   PCG_CUDA(cudaMemcpyAsync(rr.data(), cs.rr_cur, sizeof(double) * ncomp, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaMemcpyAsync(it.data(), cs.iters, sizeof(int) * ncomp, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
-  if (cudaGetLastError() != cudaSuccess) return 3;
+  if (cudaPeekAtLastError() != cudaSuccess) return 3;         // the caller reads (and clears) the error
   float worst = -INFINITY;
   int worst_it = 0;
   for (int c = 0; c < ncomp; c++) {
@@ -790,6 +838,25 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   if (residual) *residual = worst;
   if (iterations) *iterations = worst_it;
   return 0;
+}
+
+int pcg_precond(PcgScratch& sc, void* workspace, float* z, const float* flags, const float* r, int nb, int nz, int ny,
+                int nx, int is3d, int precond, int* geometry, long long* launches, cudaStream_t st) {
+  PcgSystem s;
+  const int rc = pcg_setup(sc, workspace, z, flags, r, nb, nz, ny, nx, is3d, precond, launches, st, s);
+  if (rc) return rc;
+  if (geometry) {
+    geometry[0] = s.g.NYP; geometry[1] = s.g.GP; geometry[2] = s.g.chunks; geometry[3] = s.sweep_grid;
+  }
+  if (s.ncomp == 0) return 0;
+  PCG_CUDA(launch_sweep(sc, s, true, launches, st));
+  PCG_CUDA(launch_sweep(sc, s, false, launches, st));
+  PCG_CUDA(cudaMemcpyAsync(sc.host, s.header, 16, cudaMemcpyDeviceToHost, st));
+  PCG_CUDA(cudaStreamSynchronize(st));
+  if (sc.host[2]) return 5;
+  k_writeback<<<blocks_for(s.g.n * nb), 256, 0, st>>>(z, s.parent, s.csize, s.cid, s.z, s.cs, s.g, 0);
+  *launches += 1;
+  return cudaPeekAtLastError() == cudaSuccess ? 0 : 3;
 #undef PCG_CUDA
 }
 
