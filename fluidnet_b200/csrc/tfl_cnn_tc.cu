@@ -26,7 +26,16 @@
 //     channels-last planes or, for the last 3x3x3 layer, also runs the two 1x1x1 layers and
 //     writes the pressure.
 // Two warpgroups per CTA take alternate M tiles; two CTAs per SM overlap one CTA's loads with
-// the other's math (the boxes are sized so that two fit the SM's 228 KB of shared memory).
+// the other's math (the boxes are sized so that two fit the SM's 228 KB of shared memory).  The
+// box kernel k_conv3_tc runs the join layer of banked models and layers 1-3 at nx > kWWMax.
+//
+// Layers 1-3 at nx <= kWWMax (k_conv3_tc_z): a persistent CTA (one per SM, four warpgroups) takes
+// work items of TY output rows x the whole row x ZC output planes x one batch entry and streams
+// along z through a ring of three staged planes.  A staged row is padded x = 1 .. ww (ww = 64 or
+// kWWMax), so no x halo is staged or computed: D of the zero border voxels x = 0 and x = nx + 1 is
+// zero and the epilogue uses 0 for it, and at nx = 128 a row is exactly two M tiles of 64.  The
+// next plane is loaded into registers while the current plane's MMAs run and is split and stored
+// after them, between two __syncthreads per plane.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -71,6 +80,45 @@ template <int IN_PLANES, bool SPLIT> struct Layout {
   static constexpr int B_GROUP_BYTES = 2 * NB * 16;
   static constexpr int B_BYTES = GROUPS * B_GROUP_BYTES;
   static constexpr int BYTES = A_BYTES + B_BYTES + 2 * 64 * kDPitch * 4 + 4 * 96;
+};
+
+// Layers 1-3 at nx <= kWWMax: four warpgroups; a staged row holds ww = 64 or kWWMax positions.
+constexpr int kZWarpGroups = 4;
+constexpr int kZThreads = 128 * kZWarpGroups;
+constexpr int kWWMax = 128;
+
+// Shared memory of k_conv3_tc_z for staged rows of ww positions:
+//   ring   3 slots; a slot is one staged padded plane, PY rows x ww positions, as two 16-byte K chunks
+//          [chunk 0 | chunk 1] of GB = PY * ww * 16 bytes each (hi, then lo when SPLIT, LO = 2 GB further);
+//          IN_PLANES == 2: chunk c is channel group c of the plane (LBO = GB);
+//          IN_PLANES == 1: (layer 1, 3 channels) chunk 0 is the plane and chunk 1 the NEXT plane, so the two
+//          K chunks of a group are the taps (dz, dy) and (dz + 1, dy) (LBO = GB); every staged plane is
+//          written twice, into its own slot's chunk 0 and the previous plane's chunk 1.  Group 3 pairs the
+//          rows (dz, dy) = (1, -1) / (1, 0) of chunk 0 (LBO = one row), group 4 is the single tap (1, 1)
+//          whose chunk 1 reads 64 zero positions (its B rows are zero too, but 0 * NaN would not be);
+//   zeros  (layer 1) 64 positions;
+//   B      the weight groups; D: one row buffer of ww x kDPitch floats per warpgroup; then bias / tail.
+template <int IN_PLANES, bool SPLIT> struct ZLayout {
+  static constexpr int TY = SPLIT ? 4 : 8;      // output rows of a work item
+  static constexpr int PY = TY + 2;
+  static constexpr int NB = SPLIT ? 48 : 32;
+  static constexpr int GROUPS = IN_PLANES == 1 ? 5 : kGroups;
+  static constexpr int ZERO_BYTES = IN_PLANES == 1 ? 64 * 16 : 0;
+  static constexpr int B_GROUP_BYTES = 2 * NB * 16;
+  static constexpr int B_BYTES = GROUPS * B_GROUP_BYTES;
+  static constexpr int SLOT_CHUNKS = SPLIT ? 4 : 2;
+  static constexpr size_t bytes(int ww) {
+    return (size_t)3 * SLOT_CHUNKS * PY * ww * 16 + ZERO_BYTES + B_BYTES + (size_t)kZWarpGroups * ww * kDPitch * 4 +
+           4 * 96;
+  }
+};
+
+// Work decomposition of one k_conv3_tc_z launch: item = (b * nzc + zc) * nty + ty.
+struct ZSched {
+  int ww;        // staged positions per row: padded x = 1 .. ww (64 or kWWMax, >= nx)
+  int nty;       // TY-row blocks
+  int zc, nzc;   // output planes per item, z chunks
+  int items;
 };
 
 // Layer 1 (one 4-channel plane): group gi's K chunk 0 is tap (layer1_dz(gi), layer1_dy(gi)); K chunk 1
@@ -132,6 +180,224 @@ __device__ __forceinline__ float4 tf32_hi(float4 v) {
 }
 
 __device__ long long* g_tc_dbg = nullptr;   // optional phase timestamps (tests/dbg only)
+
+// Bias, ReLU and (FINAL) the two 1x1x1 layers of one position's 4 channels (4 * half ..), as the two threads of a
+// position share them; writes the next layer's padded plane or the pressure when `valid`.
+template <bool FINAL>
+__device__ __forceinline__ void conv_epilogue(float (&h)[4], bool valid, int half, const float* sTail, float4* out,
+                                              float* p_net, long long out_idx, long long plane_g, long long p_idx) {
+#pragma unroll
+  for (int o = 0; o < 4; o++) h[o] = h[o] > 0.0f ? h[o] : 0.0f;
+  if constexpr (!FINAL) {
+    if (valid) out[out_idx + half * plane_g] = make_float4(h[0], h[1], h[2], h[3]);
+  } else {
+    float hh[8];
+#pragma unroll
+    for (int o = 0; o < 4; o++) {
+      const float other = __shfl_xor_sync(0xffffffffu, h[o], 1);
+      hh[o] = half ? other : h[o];
+      hh[4 + o] = half ? h[o] : other;
+    }
+    // The two threads of a position each take 4 of the 8 hidden channels of the 1x1x1 layers.
+    const float* w4 = sTail + 8 + 32 * half;        // rows 4 half .. 4 half + 3 of w4[o][c]
+    const float* b4 = sTail + 8 + 64 + 4 * half;
+    const float* w5 = sTail + 8 + 64 + 8 + 4 * half;
+    const float b5 = sTail[8 + 64 + 8 + 8];
+    float part = 0.0f;
+#pragma unroll
+    for (int o = 0; o < 4; o++) {
+      float a = b4[o];
+#pragma unroll
+      for (int c = 0; c < 8; c++) a = fmaf(hh[c], w4[o * 8 + c], a);
+      a = a > 0.0f ? a : 0.0f;
+      part = fmaf(a, w5[o], part);
+    }
+    const float pacc = b5 + (part + __shfl_xor_sync(0xffffffffu, part, 1));
+    if (valid && half == 0) p_net[p_idx] = pacc;
+  }
+}
+
+// Layers 1-3 (see the file comment and ZLayout).
+template <int IN_PLANES, bool FINAL, bool SPLIT>
+__global__ void __launch_bounds__(kZThreads, 1)
+k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __restrict__ p_net,
+             const float* __restrict__ wB, const float* __restrict__ bias, const float* __restrict__ tail,
+             ConvTcGeo g, ZSched s) {
+  extern __shared__ __align__(1024) uint8_t smem[];
+  using L = ZLayout<IN_PLANES, SPLIT>;
+  constexpr int TY = L::TY, PY = L::PY;
+  const int ww = s.ww, ntile = ww >> 6;
+  const int gbytes = PY * ww * 16;                    // one K chunk of a slot
+  const int lo_off = 2 * gbytes;                      // hi -> lo (SPLIT)
+  const int slot_bytes = L::SLOT_CHUNKS * gbytes;
+  uint8_t* sRing = smem;
+  uint8_t* sZero = smem + 3 * slot_bytes;
+  uint8_t* sB = sZero + L::ZERO_BYTES;
+  float* sD = (float*)(sB + L::B_BYTES);              // [kZWarpGroups][ww][kDPitch]
+  float* sTail = sD + kZWarpGroups * ww * kDPitch;    // bias[8] (+ w4[64] b4[8] w5[8] b5[1] when FINAL)
+
+  const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
+  long long* dbg = g_tc_dbg;
+  if (dbg && tid == 0) dbg[blockIdx.x * 8 + 0] = clock64();
+
+  for (int i = tid; i < L::ZERO_BYTES / 16; i += kZThreads) ((float4*)sZero)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int i = tid; i < L::B_BYTES / 16; i += kZThreads) ((float4*)sB)[i] = __ldg((const float4*)wB + i);
+  const int n_tail = FINAL ? (8 + 64 + 8 + 8 + 1) : 8;
+  for (int i = tid; i < n_tail; i += kZThreads) sTail[i] = (i < 8) ? bias[i] : tail[i - 8];
+
+  const long long plane_g = (long long)(g.nz + 2) * g.py * g.px;            // float4 per global plane
+  const long long batch_g = plane_g * 2;
+  const int npos = PY * ww;                                                 // staged positions of a plane
+  constexpr int PER = (PY * kWWMax + kZThreads - 1) / kZThreads;
+  float4 v[PER][IN_PLANES];
+
+  const int wg = warp >> 2, wq = warp & 3;
+  const uint32_t sRing_u = smem_u32(sRing), sB_u = smem_u32(sB), sZero_u = smem_u32(sZero);
+  float* myD = sD + wg * ww * kDPitch;
+  const int tw = tid & 127, half = tw & 1;
+  const float* bs = sTail + 4 * half;
+
+  for (int item = blockIdx.x; item < s.items; item += gridDim.x) {
+    const int ty = item % s.nty, zc = (item / s.nty) % s.nzc, b = item / s.nty / s.nzc;
+    const int y0 = ty * TY;                                             // padded row of staged row 0
+    const int za = g.z_lo + zc * s.zc, zb = min(za + s.zc, g.z_hi);     // output planes [za, zb)
+    const float4* inb = in + b * batch_g;
+
+    // padded plane pz -> registers (positions outside the buffer read the zero border voxel (0, 0, 0))
+    auto load = [&](int pz) {
+#pragma unroll
+      for (int it = 0; it < PER; it++) {
+        const int idx = tid + it * kZThreads;
+        const int row = idx / ww, gx = 1 + idx - row * ww, gy = y0 + row;
+        const bool inside = idx < npos && gx < g.px && gy < g.py;
+        const long long go = inside ? ((long long)pz * g.py + gy) * g.px + gx : 0;
+#pragma unroll
+        for (int h = 0; h < IN_PLANES; h++) v[it][h] = __ldg(inb + h * plane_g + go);
+      }
+    };
+    // registers -> slot pz % 3 (layer 1: also chunk 1 of plane pz - 1's slot), split into hi / lo when SPLIT
+    auto store = [&](int pz) {
+      uint8_t* slot = sRing + (pz % 3) * slot_bytes;
+      uint8_t* prev = sRing + ((pz + 2) % 3) * slot_bytes;
+#pragma unroll
+      for (int it = 0; it < PER; it++) {
+        const int idx = tid + it * kZThreads;
+        if (idx < npos) {
+#pragma unroll
+          for (int c = 0; c < 2; c++) {
+            const float4 w = v[it][IN_PLANES == 2 ? c : 0];
+            uint8_t* dst = (IN_PLANES == 1 && c == 1 ? prev : slot) + c * gbytes + idx * 16;
+            if constexpr (SPLIT) {
+              const float4 hi = tf32_hi(w);
+              *(float4*)dst = hi;
+              *(float4*)(dst + lo_off) = make_float4(w.x - hi.x, w.y - hi.y, w.z - hi.z, w.w - hi.w);
+            } else {
+              *(float4*)dst = w;
+            }
+          }
+        }
+      }
+    };
+
+    // output plane z reads padded planes z, z + 1, z + 2
+    for (int k = 0; k < 3; k++) {
+      load(za + k);
+      store(za + k);
+    }
+    // generic-proxy writes (st.shared) -> visible to the wgmma (async proxy) reads
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+    if (dbg && tid == 0 && item == blockIdx.x) dbg[blockIdx.x * 8 + 1] = clock64();
+
+    for (int z = za; z < zb; z++) {
+      const bool more = z + 1 < zb;
+      if (more) load(z + 3);                       // in flight during this plane's MMAs
+      uint32_t base[3];                            // slot of padded plane z + 1 + dz
+#pragma unroll
+      for (int d = 0; d < 3; d++) base[d] = sRing_u + (uint32_t)(((z + d) % 3) * slot_bytes);
+
+      // warpgroup wg takes rows wg, wg + 4, ...; a row is ntile M tiles of 64 positions
+      for (int r = wg; r < TY && y0 + r < g.ny; r += kZWarpGroups) {
+        for (int t = 0; t < ntile; t++) {
+          const uint32_t row_off = (uint32_t)(((r + 1) * ww + 64 * t) * 16);
+          float acc[SPLIT ? 24 : 12] = {}, acl[12] = {};
+          asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
+#pragma unroll
+          for (int gi = 0; gi < L::GROUPS; gi++) {
+            const int dz = IN_PLANES == 1 ? layer1_dz(gi) : gi / 3 - 1;
+            const int dy = IN_PLANES == 1 ? layer1_dy(gi) : gi % 3 - 1;
+            const uint32_t a = base[1 + dz] + row_off + (uint32_t)(dy * ww * 16);
+            const bool zero_k1 = IN_PLANES == 1 && gi == 4;
+            const uint32_t lbo = IN_PLANES == 1 && gi == 3 ? (uint32_t)(ww * 16) : zero_k1 ? sZero_u - a : (uint32_t)gbytes;
+            const uint64_t da = make_desc(a, lbo, 128);
+            const uint64_t db = make_desc(sB_u + gi * L::B_GROUP_BYTES, L::NB * 16, 128);
+            if constexpr (SPLIT) {
+              const uint32_t al = a + (uint32_t)lo_off;
+              wgmma_n48(acc, da, db, gi > 0 ? 1u : 0u);
+              wgmma_n24(acl, make_desc(al, zero_k1 ? sZero_u - al : lbo, 128), db, gi > 0 ? 1u : 0u);
+            } else {
+              wgmma_n24(acc, da, db, gi > 0 ? 1u : 0u);
+            }
+          }
+          asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+          asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+          if (dbg && tid == 0 && item == blockIdx.x && z == za && t == 0) dbg[blockIdx.x * 8 + 2] = clock64();
+
+          // accumulator fragment: element (row 16 wq + lane / 4 + 8 i, column 8 k + 2 (lane % 4) + j) is acc[4 k + 2 i + j]
+          float* tD = myD + 64 * t * kDPitch;
+#pragma unroll
+          for (int k = 0; k < 3; k++)
+#pragma unroll
+            for (int i = 0; i < 2; i++) {
+              const int row = 16 * wq + (lane >> 2) + 8 * i, col = 8 * k + 2 * (lane & 3);
+              float2 d2;
+              if constexpr (SPLIT) {
+                d2.x = acc[4 * k + 2 * i] + (acc[12 + 4 * k + 2 * i] + acl[4 * k + 2 * i]);
+                d2.y = acc[4 * k + 2 * i + 1] + (acc[12 + 4 * k + 2 * i + 1] + acl[4 * k + 2 * i + 1]);
+              } else {
+                d2.x = acc[4 * k + 2 * i];
+                d2.y = acc[4 * k + 2 * i + 1];
+              }
+              *(float2*)(tD + row * kDPitch + col) = d2;
+            }
+        }
+        wg_barrier(1 + wg);
+
+        // epilogue: staged position i (padded x = i + 1), channels 4 half .. 4 half + 3; D of the zero border
+        // voxels x = 0 and x = nx + 1 is 0
+        const int yg = y0 + r;
+        for (int j = 0; j < ntile; j++) {
+          const int i = (tw >> 1) + 64 * j, xp = i + 1;
+          const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+          const float4 dm = i >= 1 ? *(const float4*)(myD + (i - 1) * kDPitch + 4 * half) : zero4;
+          const float4 d0 = *(const float4*)(myD + i * kDPitch + 8 + 4 * half);
+          const float4 dp = xp < g.nx ? *(const float4*)(myD + (i + 1) * kDPitch + 16 + 4 * half) : zero4;
+          float h[4];
+          h[0] = (dm.x + d0.x) + dp.x + bs[0];
+          h[1] = (dm.y + d0.y) + dp.y + bs[1];
+          h[2] = (dm.z + d0.z) + dp.z + bs[2];
+          h[3] = (dm.w + d0.w) + dp.w + bs[3];
+          conv_epilogue<FINAL>(h, xp <= g.nx, half, sTail, out, p_net,
+                               b * batch_g + ((long long)(z + 1) * g.py + (yg + 1)) * g.px + xp, plane_g,
+                               (long long)b * g.nz * g.ny * g.nx + ((long long)z * g.ny + yg) * g.nx + (xp - 1));
+        }
+        wg_barrier(1 + wg);                        // myD is rewritten by the next row
+      }
+      __syncthreads();                             // every warpgroup is done with padded plane z's slot
+      if (more) {
+        store(z + 3);
+        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      }
+      __syncthreads();
+    }
+  }
+  if (dbg && tid == 0) {
+    dbg[blockIdx.x * 8 + 5] = clock64();
+    unsigned smid;
+    asm("mov.u32 %0, %%smid;" : "=r"(smid));
+    dbg[blockIdx.x * 8 + 7] = smid;
+  }
+}
 
 // JOIN (final layer only): the input box is the sum of the banks of `js`, each staged from its own resolution
 // with nearest indexing (see TcJoinSrc), and the epilogue may write / add / read a partial sum (part_mode).
@@ -417,6 +683,51 @@ void launch_one(const float4* in, float4* out, float* p_net, const float* wB, co
   kern<<<grid, kThreads, smem, st>>>(in, out, p_net, wB, bias, tail, gg, js);
 }
 
+// Work items of one k_conv3_tc_z launch on `nsm` SMs.  ZC (output planes per item) minimises the rounds of the
+// persistent grid times the planes a round stages (ZC + 2); ties go to the larger ZC (fewer items, fewer halo
+// planes).  128^3, 132 SMs: 3xTF32 32 row blocks x ZC 32 = 128 items, TF32 16 x 16 = 128 items, one round.
+// Needs nx <= kWWMax and z_hi > z_lo.
+ZSched z_schedule(const ConvTcGeo& g, int ty, int nsm) {
+  ZSched s;
+  s.zc = 1;
+  s.ww = g.nx > 64 ? kWWMax : 64;
+  s.nty = (g.ny + ty - 1) / ty;
+  const long long cols = (long long)g.nb * s.nty;
+  const int nzo = g.z_hi - g.z_lo;
+  long long best = -1;
+  for (int zc = 1; zc <= nzo; zc++) {
+    const long long items = cols * ((nzo + zc - 1) / zc);
+    const long long grid = items < nsm ? items : nsm;
+    const long long cost = (items + grid - 1) / grid * (zc + 2);
+    if (best < 0 || cost <= best) {
+      best = cost;
+      s.zc = zc;
+    }
+  }
+  s.nzc = (nzo + s.zc - 1) / s.zc;
+  s.items = (int)(cols * s.nzc);
+  return s;
+}
+
+template <int IN_PLANES, bool FINAL, bool SPLIT>
+void launch_z(const float4* in, float4* out, float* p_net, const float* wB, const float* bias, const float* tail,
+              const ConvTcGeo& g, cudaStream_t st) {
+  using L = ZLayout<IN_PLANES, SPLIT>;
+  if (g.z_hi <= g.z_lo || g.nb < 1 || g.ny < 1 || g.nx < 1) return;     // nothing to compute
+  auto kern = k_conv3_tc_z<IN_PLANES, FINAL, SPLIT>;
+  static unsigned long long configured = 0;       // per device (function attributes are)
+  int dev = 0, nsm = 0;
+  cudaGetDevice(&dev);
+  if (!((configured >> (dev & 63)) & 1ULL)) {
+    cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)L::bytes(kWWMax));
+    configured |= 1ULL << (dev & 63);
+  }
+  cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
+  const ZSched s = z_schedule(g, L::TY, nsm);
+  const int grid = s.items < nsm ? s.items : nsm;
+  kern<<<grid, kZThreads, L::bytes(s.ww), st>>>(in, out, p_net, wB, bias, tail, g, s);
+}
+
 // 2x2x2 average of the first float4 plane (k_pool's summation order), zero fourth channel.
 __global__ void k_tc_pyramid(const float4* __restrict__ in, ConvTcGeo gi, float4* __restrict__ out, ConvTcGeo go,
                              long long total) {
@@ -508,9 +819,13 @@ int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, 
                     cudaStream_t st) {
   const float4* i4 = (const float4*)in;
   float4* o4 = (float4*)out;
+  // Rows up to kWWMax positions stream along z without an x halo; wider rows would need overlapping row windows
+  // whose 64-position M tiles compute more positions per kept voxel than the box's 32-wide rows (256^3: 320 or 384
+  // per row against 288), so they keep the one-shot box.
 #define TFL_TC_CASE(P, F, S)                                                   \
   if (in_planes == P && (final_layer != 0) == F && (split != 0) == S) {        \
-    launch_one<P, F, S>(i4, o4, p_net, wB, bias, tail, g, st);                 \
+    if (g.nx <= kWWMax) launch_z<P, F, S>(i4, o4, p_net, wB, bias, tail, g, st); \
+    else launch_one<P, F, S>(i4, o4, p_net, wB, bias, tail, g, st);            \
     return 1;                                                                  \
   }
   TFL_TC_CASE(1, false, false) TFL_TC_CASE(2, false, false) TFL_TC_CASE(2, true, false)

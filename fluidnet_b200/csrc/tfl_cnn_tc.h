@@ -8,7 +8,7 @@ namespace tfl {
 struct ConvTcGeo {
   int nb, nz, ny, nx;
   int px, py;             // padded pitches of the channels-last activation planes (x, y)
-  int ntx, nty, ntz;      // CTA tiles
+  int ntx, nty, ntz;      // CTA tiles of the one-shot box kernel (k_conv3_tc)
   int z_lo, z_hi;         // output planes of a launch (default: all; a z-slab computes only what its owned planes need)
 };
 
