@@ -52,7 +52,9 @@ SYMBOLS = [
     "tfl_comm_unique_id", "tfl_comm_init", "tfl_comm_destroy", "tfl_slab_sim_create", "tfl_slab_sim_destroy",
     "tfl_slab_sim_layout", "tfl_slab_sim_upload", "tfl_slab_sim_download", "tfl_slab_sim_step",
     "tfl_slab_sim_exchange_stats", "tfl_slab_sim_ipc_export", "tfl_slab_sim_ipc_connect",
+    "tfl_slab_sim_jacobi_stats", "tfl_slab_jacobi_schedule", "tfl_jacobi_slab_block",
 ]
+JACOBI_BLOCK_INTS = 6
 COMM_ID_BYTES = 128
 IPC_HANDLE_BYTES = 64
 
@@ -150,6 +152,12 @@ def load():
     lib.tfl_slab_sim_ipc_export.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p]
     lib.tfl_slab_sim_ipc_connect.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p]
     lib.tfl_slab_sim_exchange_stats.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int64)]
+    lib.tfl_slab_sim_jacobi_stats.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float),
+                                              C.POINTER(C.c_int64)]
+    lib.tfl_slab_jacobi_schedule.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
+    lib.tfl_jacobi_slab_block.argtypes = [C.c_void_p, G, G, G, G, C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                          C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
     lib.tfl_alloc_host.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p)]
     lib.tfl_free_host.argtypes = [C.c_void_p, C.c_void_p]
     _lib = lib

@@ -952,6 +952,116 @@ k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restric
   }
 }
 
+// One block of Jacobi sweeps on a plane range of a z-slab in ONE cooperative launch (the Jacobi path of
+// tfl_slab_sim_step).  Same residency as k_jacobi_resident -- a thread group owns a 128 x 8 x KZ block for the whole
+// launch, p in registers, div and the block's y rows in shared memory, a grid-wide barrier between sweeps -- but the
+// blocks tile the local planes [z_lo, z_hi) only, and sweep s computes [z_lo + s * shr_lo, z_hi - s * shr_hi): the
+// range loses one plane per sweep on each side whose ghost planes came from a neighbour.  Cells outside a sweep's
+// range keep their value and are not stored; no cell of a later, narrower range reads them.  Same per-cell
+// expression (bit-identical to one k_jacobi_iter4 launch per sweep on the same ranges and buffers).
+// Co-residency: one 1024-thread CTA per SM (64 registers per thread), kJG blocks of 128 x 8 x KZ cells per CTA, so
+// at most 132 * 4 * 4096 * KZ / 4 cells on an H100: 2.16M with KZ = 4, 3.24M with KZ = 6 -- the deepest block whose
+// shared memory (kJG x KZ x (18 rows of 32 float4 + the x halo)) fits one SM: 217.5 KiB.  The dispatcher takes the
+// shallowest KZ that fits.  The x halo goes through shared memory to spare registers.
+template <int KZ>
+__global__ void __launch_bounds__(256 * kJG, 1)
+k_jacobi_block(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb, Geo g,
+               int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks) {
+  cooperative_groups::grid_group grid = cooperative_groups::this_grid();
+  extern __shared__ float4 jsm[];
+  constexpr int kGroupF4 = KZ * (kJY + 2) * 32 + KZ * kJY * 32 + KZ * kJY * 2 / 4;
+  float4* gsm = jsm + threadIdx.z * kGroupF4;
+  float4 (*rows)[kJY + 2][32] = reinterpret_cast<float4 (*)[kJY + 2][32]>(gsm);               // [KZ][kJY + 2][32]
+  float4 (*dvs)[kJY][32] = reinterpret_cast<float4 (*)[kJY][32]>(gsm + KZ * (kJY + 2) * 32);   // [KZ][kJY][32]
+  float (*xh)[kJY][2] = reinterpret_cast<float (*)[kJY][2]>(gsm + KZ * (2 * kJY + 2) * 32);     // [KZ][kJY][2]: x halo
+  const int tx = threadIdx.x, ty = threadIdx.y;
+  const int blk = blockIdx.x * kJG + threadIdx.z;
+  const bool live = blk < nblocks;                         // a group without a block only takes part in the barriers
+  const int nxt = g.nx / 128, nyt = g.ny / kJY;
+  const int bx = blk % nxt, by = (blk / nxt) % nyt, bz = blk / (nxt * nyt);
+  const int i0 = (bx * 32 + tx) * 4;
+  const int j = by * kJY + ty;
+  const int nchunks = (z_hi - z_lo + KZ - 1) / KZ;
+  const int b = live ? bz / nchunks : 0;
+  const int k0 = live ? z_lo + (bz % nchunks) * KZ : 0;
+  const int np = live ? min(KZ, z_hi - k0) : 0;            // planes of this block
+  const int sy = g.nx, sz = g.nx * g.ny;
+  const long long base = live ? b * g.n + (long long)k0 * sz + (long long)j * sy + i0 : 0;
+  const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+  const bool has_left = tx == 0 && i0 > 0, has_right = tx == 31 && i0 + 4 < g.nx;
+  unsigned m4[KZ];
+  float4 pc[KZ];
+#pragma unroll
+  for (int k = 0; k < KZ; k++) {
+    const bool in = k < np;
+    m4[k] = in ? __ldg((const unsigned*)(mask + base + (long long)k * sz)) : 0x01010101u;
+    dvs[k][ty][tx] = in ? __ldg((const float4*)(div + base + (long long)k * sz)) : zero4;
+    pc[k] = in ? __ldcg((const float4*)(pa + base + (long long)k * sz)) : zero4;
+  }
+  for (int s = 0; s < sweeps; s++) {
+    const float* prev = (s & 1) ? pb : pa;                 // sweep 0 reads pa and writes pb
+    float* cur = (s & 1) ? pa : pb;
+    const float* pp = prev + base;                         // per-sweep pointers keep the plane offsets 32-bit
+    float* cp = cur + base;
+    // this block's planes of the sweep's range: [klo, khi)
+    const int klo = max(z_lo + s * shr_lo - k0, 0), khi = min(z_hi - s * shr_hi - k0, np);
+    const float4 zlo = (klo == 0 && khi > 0 && k0 > 0) ? __ldcg((const float4*)(pp - sz)) : zero4;
+    const float4 zhi = (khi == np && np > klo && k0 + np < g.nz) ? __ldcg((const float4*)(pp + np * sz)) : zero4;
+#pragma unroll
+    for (int k = 0; k < KZ; k++) {
+      const float* c = pp + k * sz;
+      const bool in = k >= klo && k < khi;
+      if (ty == 0) rows[k][0][tx] = (in && j > 0) ? __ldcg((const float4*)(c - sy)) : zero4;
+      if (ty == kJY - 1) rows[k][kJY + 1][tx] = (in && j + 1 < g.ny) ? __ldcg((const float4*)(c + sy)) : zero4;
+      if (tx == 0) xh[k][ty][0] = (in && has_left) ? __ldcg(c - 1) : 0.0f;
+      if (tx == 31) xh[k][ty][1] = (in && has_right) ? __ldcg(c + 4) : 0.0f;
+      rows[k][ty + 1][tx] = pc[k];
+    }
+    asm volatile("bar.sync %0, 256;" ::"r"(1 + (int)threadIdx.z) : "memory");      // this group's rows are in place
+    float4 below = zlo;
+#pragma unroll
+    for (int k = 0; k < KZ; k++) {
+      const bool in = k >= klo && k < khi;
+      const float4 ctr = pc[k];
+      const float4 above = k + 1 < KZ ? (k + 1 < np ? pc[k + 1] : zhi) : zhi;
+      float out[4] = {0.0f, 0.0f, 0.0f, 0.0f};
+      const unsigned mm = m4[k];
+      float lf = __shfl_up_sync(0xffffffffu, ctr.w, 1);        // every lane takes part, whatever its mask
+      float rt = __shfl_down_sync(0xffffffffu, ctr.x, 1);
+      if (tx == 0) lf = xh[k][ty][0];
+      if (tx == 31) rt = xh[k][ty][1];
+      if (in && (mm & 0x01010101u) != 0x01010101u) {
+        const float4 ym = rows[k][ty][tx], yp = rows[k][ty + 2][tx], dv = dvs[k][ty][tx];
+        const float pcv[4] = {ctr.x, ctr.y, ctr.z, ctr.w};
+        const float xm[4] = {lf, ctr.x, ctr.y, ctr.z};
+        const float xp[4] = {ctr.y, ctr.z, ctr.w, rt};
+        const float ymv[4] = {ym.x, ym.y, ym.z, ym.w}, ypv[4] = {yp.x, yp.y, yp.z, yp.w};
+        const float zmv[4] = {below.x, below.y, below.z, below.w}, zpv[4] = {above.x, above.y, above.z, above.w};
+        const float dvv[4] = {dv.x, dv.y, dv.z, dv.w};
+#pragma unroll
+        for (int q = 0; q < 4; q++) {
+          const unsigned m = (mm >> (8 * q)) & 0xFFu;
+          if (m & 1) continue;
+          const float p1 = (m & 2) ? pcv[q] : xm[q];
+          const float p2 = (m & 4) ? pcv[q] : xp[q];
+          const float p3 = (m & 8) ? pcv[q] : ymv[q];
+          const float p4 = (m & 16) ? pcv[q] : ypv[q];
+          const float p5 = (m & 32) ? pcv[q] : zmv[q];
+          const float p6 = (m & 64) ? pcv[q] : zpv[q];
+          out[q] = (p1 + p2 + p3 + p4 + p5 + p6 + dvv[q]) / 6.0f;
+        }
+      }
+      if (in) {
+        const float4 o4 = make_float4(out[0], out[1], out[2], out[3]);
+        *(float4*)(cp + k * sz) = o4;
+        pc[k] = o4;
+      }
+      below = ctr;
+    }
+    if (s + 1 < sweeps) grid.sync();                       // also orders the shared rows against the next sweep
+  }
+}
+
 // sum over one batch element of (a - b)^2, accumulated in double: out[b] += ...
 __global__ void k_sqdiff(const float* __restrict__ a, const float* __restrict__ bb, long long n,
                          double* __restrict__ out) {
@@ -1190,6 +1300,63 @@ bool launch_jacobi_sweeps(const unsigned char* mask, const float* div, float* pa
     return false;
   }
   return true;
+}
+namespace {
+// Resident CTAs of k_jacobi_block<KZ> on the current device (0 when it cannot be launched cooperatively).
+template <int KZ>
+int jacobi_block_capacity(int smem) {
+  static int capacities[64];         // per device (0: not asked yet, -1: cannot)
+  int dev = 0;
+  cudaGetDevice(&dev);
+  int& capacity = capacities[dev & 63];
+  if (capacity == 0) {
+    int sms = 0, per_sm = 0, coop = 0;
+    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
+    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
+    capacity = -1;
+    if (coop && cudaFuncSetAttribute(k_jacobi_block<KZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_jacobi_block<KZ>, 256 * kJG, smem) == cudaSuccess &&
+        sms * per_sm > 0)
+      capacity = sms * per_sm;
+    cudaGetLastError();
+  }
+  return capacity > 0 ? capacity : 0;
+}
+template <int KZ>
+int try_jacobi_block(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo, int z_hi,
+                     int shr_lo, int shr_hi, int sweeps, cudaStream_t st) {
+  const int smem = kJG * (KZ * (kJY + 2) * 32 + KZ * kJY * 32 + KZ * kJY * 2 / 4) * (int)sizeof(float4);
+  int nblocks = (g.nx / 128) * (g.ny / kJY) * ((z_hi - z_lo + KZ - 1) / KZ) * g.nb;
+  const int ctas = (nblocks + kJG - 1) / kJG;
+  if (ctas > jacobi_block_capacity<KZ>(smem)) return 0;
+  dim3 block(32, kJY, kJG), grid(ctas, 1, 1);
+  Geo gg = g;
+  void* args[] = {(void*)&mask, (void*)&div, (void*)&pa, (void*)&pb, (void*)&gg, (void*)&z_lo, (void*)&z_hi,
+                  (void*)&shr_lo, (void*)&shr_hi, (void*)&sweeps, (void*)&nblocks};
+  if (cudaLaunchCooperativeKernel((const void*)k_jacobi_block<KZ>, grid, block, args, smem, st) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return KZ;
+}
+}  // namespace
+int launch_jacobi_block(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo,
+                        int z_hi, int shr_lo, int shr_hi, int sweeps, bool deep, cudaStream_t st) {
+  const bool aligned = ((uintptr_t)mask % 4 == 0) && ((uintptr_t)div % 16 == 0) && ((uintptr_t)pa % 16 == 0) &&
+                       ((uintptr_t)pb % 16 == 0);
+  if (!g.is3d || !aligned || g.nx % 128 != 0 || g.ny % kJY != 0 || sweeps < 1 || z_lo >= z_hi) return 0;
+  // the shallowest block that fits: more, thinner CTAs spread a small range over more SMs
+  const int kz = try_jacobi_block<4>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);
+  return kz || !deep ? kz : try_jacobi_block<6>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);
+}
+void launch_jacobi_range_sweeps(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,
+                                int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, cudaStream_t st) {
+  for (int s = 0; s < sweeps; s++) {
+    Geo gs = g;
+    gs.zlo = z_lo + s * shr_lo;
+    gs.zhi = z_hi - s * shr_hi;
+    launch_jacobi_iter(mask, div, (s & 1) ? pb : pa, (s & 1) ? pa : pb, gs, st);
+  }
 }
 void launch_sqdiff(const float* a, const float* b, long long n, int nb, double* out, cudaStream_t st) {
   long long blocks = (n + 1023) / 1024;

@@ -97,6 +97,12 @@ int tfl_slab_sim_download(tfl_ctx*, tfl_slab_sim* sim, float* p, float* U, float
 int tfl_slab_sim_step(tfl_ctx*, tfl_slab_sim* sim, const tfl_mconf* mconf, tfl_cnn* cnn);
 int tfl_slab_sim_ipc_export(tfl_ctx*, tfl_slab_sim* sim, char* handle_out);
 int tfl_slab_sim_ipc_connect(tfl_ctx*, tfl_slab_sim* sim, const char* handles);
+int tfl_slab_sim_jacobi_stats(tfl_ctx*, tfl_slab_sim* sim, int32_t* exchanges, float* ms, int64_t* bytes);
+int tfl_slab_jacobi_schedule(int32_t gnz, int32_t world, int32_t rank, int32_t margin, int32_t max_iter,
+                             int32_t planes[3], int32_t* blocks, int32_t cap);
+int tfl_jacobi_slab_block(tfl_ctx*, const tfl_grid* pa, const tfl_grid* pb, const tfl_grid* flags,
+                          const tfl_grid* div, int is_3d, int32_t z_lo, int32_t z_hi, int32_t shrink_lo,
+                          int32_t shrink_hi, int32_t sweeps, int32_t path, int32_t* path_out);
 ]]
 
 local lib = ffi.load('tfl')          -- libtfl.so on the library path
@@ -326,6 +332,25 @@ end
 function tfluids.slabUpload(sim, p, U, density) check(lib.tfl_slab_sim_upload(ctx, sim, p, U, density)) end
 function tfluids.slabStep(sim, cmconf, model) check(lib.tfl_slab_sim_step(ctx, sim, cmconf, model)) end
 function tfluids.slabDownload(sim, p, U, density) check(lib.tfl_slab_sim_download(ctx, sim, p, U, density)) end
+function tfluids.slabJacobiStats(sim)                -- p exchanges of the last 'jacobi' step: count, ms, bytes
+  local n, ms, by = ffi.new('int32_t[1]'), ffi.new('float[1]'), ffi.new('int64_t[1]')
+  check(lib.tfl_slab_sim_jacobi_stats(ctx, sim, n, ms, by))
+  return n[0], ms[0], tonumber(by[0])
+end
+function tfluids.slabJacobiSchedule(gnz, world, rank, margin, maxIter)   -- {planes = {lo, hi, uWidth}, blocks = {...}}
+  local planes = ffi.new('int32_t[3]')
+  local n = lib.tfl_slab_jacobi_schedule(gnz, world, rank, margin, maxIter, planes, nil, 0)
+  assert(n > 0, 'slabJacobiSchedule: bad arguments')
+  local raw = ffi.new('int32_t[?]', 6 * n)
+  lib.tfl_slab_jacobi_schedule(gnz, world, rank, margin, maxIter, planes, raw, n)
+  local blocks = {}
+  for b = 0, n - 1 do
+    local o = 6 * b
+    blocks[b + 1] = {sweeps = raw[o], exchange = raw[o + 1], zLo = raw[o + 2], zHi = raw[o + 3],
+                     shrinkLo = raw[o + 4], shrinkHi = raw[o + 5]}
+  end
+  return {planes = {planes[0], planes[1], planes[2]}, blocks = blocks}
+end
 
 function tfluids.synchronize() check(lib.tfl_sync(ctx)) end
 

@@ -14,6 +14,17 @@ before each phase whose stencil reaches across the cut:
                                      all-reduce of the two sums (the input scale), conv stack on the
                                      whole local slab, velocity update on owned planes
 
+simMethod 'jacobi' (no model) replaces the last phase: setWallBcsForward on the owned planes, then
+
+    exchange U           (w)      -> divergence and Jacobi mask on owned +- (w - 1) planes
+    Jacobi from p = 0 in blocks of up to `halo` sweeps (jacobi_schedule): after an exchange of p of
+    width w a block's sweep s computes owned +- (w - 1 - s) planes, so one exchange serves a block;
+    p starts at zero everywhere (no exchange before the first block), the last block leaves p right
+    one plane below the owned ones for the velocity update on owned planes.
+
+It has no reduction at all, so p, U and density equal the single-GPU step bit for bit.  'pcg' is not
+decomposed (its IC(0) triangular solves sweep the whole domain in order).
+
 There is no data-path collective other than those neighbour exchanges and the 2-double all-reduce.
 A line trace or stencil that leaves the local slab (halo too small for the velocity) increments
 the library's fault counter instead of reading out of bounds; `SlabSimulator.check()` raises.
@@ -23,6 +34,38 @@ import ctypes as C
 
 import torch
 import torch.distributed as dist
+
+from . import _lib
+
+
+def jacobi_schedule(gnz, world, rank, margin, max_iter):
+    """The Jacobi sweep schedule of one rank (tfl_slab_jacobi_schedule): ((first, past-last local plane with valid
+    divergence and mask, width of the U exchange), [(sweeps, p exchange width before the block or 0, first /
+    past-last local plane of the block's sweep 0, shrink at the bottom, shrink at the top), ...])."""
+    lib = _lib.load()
+    planes = (C.c_int32 * 3)()
+    n = lib.tfl_slab_jacobi_schedule(gnz, world, rank, margin, max_iter, planes, None, 0)
+    if n < 1:
+        raise ValueError("no Jacobi schedule for gnz=%d world=%d rank=%d margin=%d maxIter=%d"
+                         % (gnz, world, rank, margin, max_iter))
+    raw = (C.c_int32 * (_lib.JACOBI_BLOCK_INTS * n))()
+    lib.tfl_slab_jacobi_schedule(gnz, world, rank, margin, max_iter, planes, raw, n)
+    k = _lib.JACOBI_BLOCK_INTS
+    return tuple(planes), [tuple(raw[b * k:(b + 1) * k]) for b in range(n)]
+
+
+def _sim_method(mconf):
+    """'convnet' or 'jacobi' and the sweep count (refuses what the slab step does not decompose)."""
+    method = mconf.get("simMethod") or "convnet"
+    if method == "pcg":
+        raise ValueError("simMethod 'pcg' is not decomposed over z-slabs: the IC(0) triangular solves of its "
+                         "preconditioner sweep the whole domain in order")
+    if method not in ("convnet", "jacobi"):
+        raise ValueError("mconf.simMethod (%s) is not a valid option" % method)
+    iters = mconf.get("maxIter")
+    if method == "jacobi" and iters is not None and int(iters) < 1:
+        raise ValueError("At least 1 iteration is needed (maxIter < 1)")
+    return method, int(iters or 100)
 
 
 class SlabDecomposition:
@@ -84,18 +127,21 @@ class SlabDecomposition:
 
 
 class SlabSimulator:
-    """tfluids.simulate (convnet path) for one domain split in z across the ranks of `group`."""
+    """tfluids.simulate (simMethod 'convnet' or 'jacobi') for one domain split in z across the ranks of `group`."""
 
-    def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=2, group=None):
+    def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=2, group=None,
+                 jacobi_path=-1):
         """batch: dict of GLOBAL torch CPU tensors (pDiv, UDiv, flags, density and the BC arrays),
-        identical on every rank.  margin: planes a backward trace may reach (ceil(max|u| dt) + 1)."""
+        identical on every rank.  margin: planes a backward trace may reach (ceil(max|u| dt) + 1).
+        model_layers: None for simMethod 'jacobi'.  jacobi_path: tfl_jacobi_slab_block's path (-1 automatic)."""
         from . import tfluids, model as fmodel
         self.tfluids = tfluids
         self.group = group
         self.rank = dist.get_rank(group) if rank is None else rank
         self.world = dist.get_world_size(group) if world is None else world
         self.mconf = dict(mconf)
-        assert (self.mconf.get("simMethod") or "convnet") == "convnet"
+        method, iters = _sim_method(self.mconf)
+        self.jacobi = method == "jacobi"
         gnz = batch["flags"].shape[2]
         assert margin >= 2, "margin < 2 makes the halo narrower than the widest fixed exchange (5 planes)"
         self.dec = SlabDecomposition(gnz, self.rank, self.world, halo=2 * margin + 2)
@@ -103,8 +149,15 @@ class SlabSimulator:
         self.device = torch.device(device)
         self.s = {k: self.dec.scatter(v).to(self.device) for k, v in batch.items() if v is not None}
         self.ctx = tfluids.context(self.device)
-        self.model = fmodel.ProjectionModel(model_layers, True, device=self.device,
-                                            normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
+        if self.jacobi:
+            self.model = None
+            self.jsched = jacobi_schedule(gnz, self.world, self.rank, margin, iters)
+            self.jacobi_path = jacobi_path
+            self.div = torch.zeros_like(self.s["pDiv"])
+            self.p2 = torch.zeros_like(self.s["pDiv"])
+        else:
+            self.model = fmodel.ProjectionModel(model_layers, True, device=self.device,
+                                                normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
         self.U1 = torch.empty_like(self.s["UDiv"])
         self.sums = torch.zeros(2, dtype=torch.float64, device=self.device)
 
@@ -163,6 +216,14 @@ class SlabSimulator:
         if (m.get("vorticityConfinementAmp") or 0) > 0:
             with self._slab(d.own_lo, d.own_hi):
                 t.vorticityConfinement(U, flags, dx * m["vorticityConfinementAmp"])
+        if self.jacobi:
+            with self._slab(d.own_lo, d.own_hi):
+                t.setWallBcsForward(U, flags)
+            self._bc()
+            yield from self._jacobi(p, U, flags)
+            self._bc()
+            t.clamp(U, -1e6, 1e6)
+            return
         self._bc()
         yield ("halo", [U, p], 5)
         c, lib = self.ctx, self.ctx.lib
@@ -177,6 +238,31 @@ class SlabSimulator:
                                                   float(self.model.threshold)))
         self._bc()
         t.clamp(U, -1e6, 1e6)
+
+    def _jacobi(self, p, U, flags):
+        """lib/simulate.lua:275-303 with pTol = 0 on this slab, in the blocks of jacobi_schedule."""
+        t, d, c = self.tfluids, self.dec, self.ctx
+        (plo, phi, u_width), blocks = self.jsched
+        yield ("halo", [U], u_width)
+        with self._slab(plo, phi):
+            t.velocityDivergenceForward(U, flags, self.div)
+        p.zero_()
+        self.p2.zero_()
+        bufs, done = [p, self.p2], 0
+        for sweeps, width, zlo, zhi, shr_lo, shr_hi in blocks:
+            if width:
+                yield ("halo", [bufs[done & 1]], width)
+            if sweeps:
+                with self._slab(zlo, zhi):
+                    c.use_current_stream()
+                    c.check(c.lib.tfl_jacobi_slab_block(c.h, t._grid(bufs[done & 1]), t._grid(bufs[(done + 1) & 1]),
+                                                        t._grid(flags), t._grid(self.div), 1, zlo, zhi, shr_lo, shr_hi,
+                                                        sweeps, self.jacobi_path, None))
+            done += sweeps
+        if done & 1:
+            p.copy_(self.p2)
+        with self._slab(d.own_lo, d.own_hi):
+            t.velocityUpdateForward(U, flags, p)
 
     def check(self):
         """Raises if any stencil / trace left the local slab since the last check."""
@@ -231,9 +317,10 @@ class NativeSlabSimulator:
             dist.broadcast_object_list(ident, src=0, group=group)
         self.ctx.check(lib.tfl_comm_init(self.ctx.h, ident[0] if ident[0] else b"\0" * _lib.COMM_ID_BYTES, self.rank, self.world))
         self.mconf = dict(mconf)
+        method, _ = _sim_method(self.mconf)
         self.mc = simulate.make_mconf(self.mconf)
-        self.model = fmodel.ProjectionModel(model_layers, True, device=self.device,
-                                            normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
+        self.model = None if method == "jacobi" else fmodel.ProjectionModel(
+            model_layers, True, device=self.device, normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
 
         def host(key):
             t = batch.get(key)
@@ -272,13 +359,20 @@ class NativeSlabSimulator:
 
     def step(self):
         self.ctx.use_current_stream()
-        self.ctx.check(self.ctx.lib.tfl_slab_sim_step(self.ctx.h, self.h, C.byref(self.mc), self.model.h))
+        self.ctx.check(self.ctx.lib.tfl_slab_sim_step(self.ctx.h, self.h, C.byref(self.mc),
+                                                      self.model.h if self.model is not None else None))
 
     def exchange_stats(self):
         """(ms of the three halo exchanges and the all-reduce of the last step, bytes sent per exchange)."""
         ms, by = (C.c_float * 4)(), (C.c_int64 * 3)()
         self.ctx.check(self.ctx.lib.tfl_slab_sim_exchange_stats(self.ctx.h, self.h, ms, by))
         return list(ms), list(by)
+
+    def jacobi_stats(self):
+        """(count, ms, bytes sent) of the last step's p exchanges (simMethod 'jacobi')."""
+        n, ms, by = C.c_int32(), C.c_float(), C.c_int64()
+        self.ctx.check(self.ctx.lib.tfl_slab_sim_jacobi_stats(self.ctx.h, self.h, C.byref(n), C.byref(ms), C.byref(by)))
+        return n.value, ms.value, by.value
 
     def check(self):
         f = torch.tensor([self.ctx.trace_faults()], dtype=torch.float64, device=self.device)

@@ -325,11 +325,45 @@ void tfl_slab_sim_destroy(tfl_ctx* ctx, tfl_slab_sim* sim);
 int tfl_slab_sim_layout(const tfl_slab_sim* sim, tfl_state* state_out, int32_t info[6]);
 int tfl_slab_sim_upload(tfl_ctx* ctx, tfl_slab_sim* sim, const float* p, const float* U, const float* density);
 int tfl_slab_sim_download(tfl_ctx* ctx, tfl_slab_sim* sim, float* p, float* U, float* density);
-/* One tfluids.simulate (convnet path) on this rank's slab: three neighbour halo exchanges (one packed ncclSend /
- * ncclRecv per neighbour and direction, one NCCL group per phase) and one 2-double all-reduce.  Asynchronous.
- * A trace that leaves the local slab (margin too small) raises tfl_trace_faults. */
+/* One tfluids.simulate on this rank's slab.  Asynchronous.  A trace that leaves the local slab (margin too small)
+ * raises tfl_trace_faults.
+ * simMethod 'convnet': three neighbour halo exchanges (one packed ncclSend / ncclRecv per neighbour and direction,
+ * one NCCL group per phase) and one 2-double all-reduce.
+ * simMethod 'jacobi' (cnn may be NULL): the two exchanges before the forces, then setWallBcsForward, one exchange
+ * of U, the divergence, mconf->max_iter sweeps (0: 100) from p = 0 with pTol = 0 in the blocks of
+ * tfl_slab_jacobi_schedule (one p exchange before every block but the first), the velocity update.  No global
+ * reduction: p, U and density are bit-identical to tfl_simulate_step's.
+ * simMethod 'pcg' is refused (its IC(0) triangular solves do not shard over z), and so are banked models. */
 int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* sim, const tfl_mconf* mconf, tfl_cnn* cnn);
+/* Device time (ms) of the last step's three halo exchanges and of its all-reduce (0 on the Jacobi path), and the
+ * bytes this rank sent in each exchange.  Synchronises. */
 int tfl_slab_sim_exchange_stats(tfl_ctx* ctx, tfl_slab_sim* sim, float ms[4], int64_t bytes[3]);
+/* The last step's p exchanges of the Jacobi path: count, summed device time (ms), bytes sent.  Synchronises. */
+int tfl_slab_sim_jacobi_stats(tfl_ctx* ctx, tfl_slab_sim* sim, int32_t* exchanges, float* ms, int64_t* bytes);
+/* The Jacobi sweep schedule of rank `rank` (pure function; the step, and any host that emulates it, use it).  With
+ * halo = 2 * margin + 2, a block of k sweeps after a p exchange of width w computes owned +- (w - 1 - s) planes in its
+ * sweep s (0-based) on each side with a neighbour, and the whole local slab up to the global ends on the others.
+ * Writes min(count, cap) blocks of TFL_JACOBI_BLOCK_INTS int32, in the rank's LOCAL plane indices:
+ *   {sweeps (0 .. halo), width of the p exchange before the block (0: none), first plane, past-last plane of
+ *    sweep 0, 1 if the range loses a plane per sweep at the bottom, ... at the top},
+ * and planes = {first, past-last local plane on which the divergence and the mask must be valid, width of the U
+ * exchange that makes them so}.  Returns the block count: 1 for one rank, ceil((max_iter + 1) / halo) otherwise;
+ * -1 for bad arguments (max_iter < 1, margin < 2, slabs thinner than the halo). */
+#define TFL_JACOBI_BLOCK_INTS 6
+int tfl_slab_jacobi_schedule(int32_t gnz, int32_t world, int32_t rank, int32_t margin, int32_t max_iter,
+                             int32_t planes[3], int32_t* blocks, int32_t cap);
+/* One block of Jacobi sweeps under the context's slab placement (tfl_set_slab: offset and global extent; the
+ * placement's plane range is not used): sweep s = 0 .. sweeps-1 computes local planes
+ * [z_lo + s * shrink_lo, z_hi - s * shrink_hi) of p from the other buffer -- even sweeps read pa and write pb, odd
+ * sweeps the reverse -- with the mask of the solve computed from flags on [z_lo, z_hi).  Planes outside a sweep's
+ * range are not written.  path: 0 one launch per sweep, 1 the whole block in one cooperative launch (3-D,
+ * nx % 128 == 0, ny % 8 == 0 and the range co-resident on the device: 3.24M cells on an H100; refused otherwise),
+ * -1 automatic (the one launch for ranges of up to 2.16M cells, where it measured faster); path_out (may be
+ * NULL) receives the path taken.  The result equals `sweeps` tfl_solve_linear_system_jacobi sweeps bit for bit on
+ * every plane the last sweep computes. */
+int tfl_jacobi_slab_block(tfl_ctx* ctx, const tfl_grid* pa, const tfl_grid* pb, const tfl_grid* flags,
+                          const tfl_grid* div, int is_3d, int32_t z_lo, int32_t z_hi, int32_t shrink_lo,
+                          int32_t shrink_hi, int32_t sweeps, int32_t path, int32_t* path_out);
 /* The exchanges over peer memory instead of NCCL: every rank exports its inbox as a CUDA IPC handle, the host
  * application gives every rank the handles of ALL ranks (world x TFL_IPC_HANDLE_BYTES, rank order), and after
  * tfl_slab_sim_ipc_connect on EVERY rank (host-side barrier before the first step) a halo exchange is one kernel
