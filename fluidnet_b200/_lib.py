@@ -52,7 +52,7 @@ SYMBOLS = [
     "tfl_comm_unique_id", "tfl_comm_init", "tfl_comm_destroy", "tfl_slab_sim_create", "tfl_slab_sim_destroy",
     "tfl_slab_sim_layout", "tfl_slab_sim_upload", "tfl_slab_sim_download", "tfl_slab_sim_step",
     "tfl_slab_sim_exchange_stats", "tfl_slab_sim_ipc_export", "tfl_slab_sim_ipc_connect",
-    "tfl_slab_sim_jacobi_stats", "tfl_slab_jacobi_schedule", "tfl_jacobi_slab_block",
+    "tfl_slab_sim_jacobi_stats", "tfl_slab_jacobi_schedule", "tfl_jacobi_slab_block", "tfl_slab_cnn_margin",
 ]
 JACOBI_BLOCK_INTS = 6
 COMM_ID_BYTES = 128
@@ -156,6 +156,7 @@ def load():
                                               C.POINTER(C.c_int64)]
     lib.tfl_slab_jacobi_schedule.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                              C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
+    lib.tfl_slab_cnn_margin.argtypes = [C.c_int32]
     lib.tfl_jacobi_slab_block.argtypes = [C.c_void_p, G, G, G, G, C.c_int, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                           C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
     lib.tfl_alloc_host.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p)]

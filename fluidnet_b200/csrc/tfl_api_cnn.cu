@@ -8,6 +8,9 @@
 #include "tfl_api_internal.h"
 
 constexpr int kMaxBanks = kMaxBankPtrs;     // banks a join kernel takes
+constexpr char kSlabTcOnly[] =
+    "the z-slab projection runs on the tensor-core path only (the 3-D 'default' graph, single-bank or with banks "
+    "split at stage 1 and joined at stage 3, in mode 1 or 2)";
 
 namespace {
 
@@ -30,20 +33,23 @@ std::vector<float> concat_slice(const float* w, int nbanks, int i) {
   return slice;
 }
 
-// The join layer of a banked stack (split 1, join 3) -> p_net, reading bank i's layer-2 output l2[i] (geometry
-// geo[i], 2^-i of bank 1's resolution) with nearest indexing.  'add': one launch summing the banks, weights wj[0];
-// 'concat': one launch per bank with its slice wj[i], banks N..2 writing / adding the fp32 partial sum `part`,
-// bank 1 last adding it before the bias, ReLU and tail (one bank: no partial sum).
-void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, int nbanks, bool add, float* part, float* p_net,
-                    float* const* wj, const float* bias, const float* tail, int split, const ConvTcGeo& g,
-                    cudaStream_t st) {
+// The join layer of a banked stack (split 1, join 3) -> p_net on the output planes [g.z_lo, g.z_hi), reading bank
+// i's layer-2 output l2[i] (geometry geo[i], 2^-i of bank 1's resolution) with nearest indexing.  z-slab: local
+// full-resolution plane 0 is global plane zoff, bank i's local plane 0 its global coarse plane org[i] (whole grids:
+// all 0).  'add': one launch summing the banks, weights wj[0]; 'concat': one launch per bank with its slice wj[i],
+// banks N..2 writing / adding the fp32 partial sum `part`, bank 1 last adding it before the bias, ReLU and tail (one
+// bank: no partial sum).
+void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org, int zoff, int nbanks, bool add,
+                    float* part, float* p_net, float* const* wj, const float* bias, const float* tail, int split,
+                    const ConvTcGeo& g, cudaStream_t st) {
   auto src_of = [&](int first, int n, int mode) {
     TcJoinSrc js = {};
     for (int k = 0; k < n; k++) {
       const int i = first + k;
       js.p[k] = l2[i];
-      js.px[k] = geo[i].px; js.py[k] = geo[i].py; js.nz[k] = geo[i].nz; js.shift[k] = i;
+      js.px[k] = geo[i].px; js.py[k] = geo[i].py; js.nz[k] = geo[i].nz; js.shift[k] = i; js.org[k] = org[i];
     }
+    js.zoff = zoff;
     js.n = n;
     js.part_mode = mode;
     js.partial = part;
@@ -60,19 +66,53 @@ void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, int nbanks, bo
 
 }  // namespace
 
+// The reach of a banked model, with s = 2^(banksNum-1) the coarsest bank's scale: p on the planes the velocity
+// update reads (owned - 1 .. owned_hi - 1) needs the network input on 3 s + 1 planes below the owned ones and 3 s
+// above (the coarse plane of the join's stencil end, two coarse 3x3x3 layers, the s fine planes a coarse plane
+// pools, each at its worst alignment to the rank's boundary), the input reads U one plane up and the wall mask flags
+// one plane down.  So the slab holds 3 s + 2 ghost planes on each interior side (the input is computed up to two
+// planes short of the local end), which a halo of 2 margin + 2 provides from margin = 3 s / 2 on.
+int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, int nx, int zoff, int nz, int own_lo,
+                   int own_hi) {
+  if (!m->tc_ok || m->mode == 0) return fail(ctx, "slab: %s", kSlabTcOnly);
+  if (m->nbanks == 1) return 0;
+  const int need = tfl_slab_cnn_margin(m->nbanks), s = 1 << (m->nbanks - 1), depth = 3 * s + 2;
+  if (margin < need)
+    return fail(ctx, "slab: a %d-bank model needs a z-slab margin >= %d (tfl_slab_cnn_margin), got %d", m->nbanks,
+                need, margin);
+  if (gnz % s || ny % s || nx % s)
+    return fail(ctx, "slab: the z-slab's global grid %dx%dx%d is not divisible by 2^(banksNum-1) = %d", nx, ny, gnz, s);
+  if ((zoff > 0 && own_lo < depth) || (zoff + nz < gnz && nz - own_hi < depth))
+    return fail(ctx, "slab: a %d-bank model needs %d ghost planes on each interior side of the z-slab (margin >= %d); "
+                     "this one has %d below and %d above", m->nbanks, depth, need, own_lo, nz - own_hi);
+  return 0;
+}
+
 // Tensor-core path: padded channels-last activations owned by the model (their zero borders
 // must survive between calls, so they do not live in the shared arena).
+// z-slab (g.zoff, g.gnz): bank i holds the global coarse planes [ceil(zoff / 2^i), floor((zoff + nz) / 2^i)).
 int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
-  if (m->act_geo.nb == g.nb && m->act_geo.nz == g.nz && m->act_geo.ny == g.ny && m->act_geo.nx == g.nx) return 0;
+  if (m->act_geo.nb == g.nb && m->act_geo.nz == g.nz && m->act_geo.ny == g.ny && m->act_geo.nx == g.nx &&
+      (m->nbanks == 1 || m->act_zoff == g.zoff))
+    return 0;
   if (m->nbanks > 1) {
     const int r = 1 << (m->nbanks - 1);
-    if (g.nx % r || g.ny % r || g.nz % r)
+    if (ctx->slab && (g.nx % r || g.ny % r || g.gnz % r))
+      return fail(ctx, "cnn: the z-slab's global grid %dx%dx%d is not divisible by 2^(banksNum-1) = %d", g.nx, g.ny,
+                  g.gnz, r);
+    if (!ctx->slab && (g.nx % r || g.ny % r || g.nz % r))
       return fail(ctx, "cnn: grid %dx%dx%d at bank split stage 1 is not divisible by 2^(banksNum-1) = %d", g.nx, g.ny,
                   g.nz, r);
+    for (int i = 1, org = g.zoff; i < m->nbanks; i++) {
+      org = (org + 1) >> 1;
+      if (((g.zoff + g.nz) >> i) - org < 1)
+        return fail(ctx, "cnn: the z-slab of %d planes holds no plane of bank %d", g.nz, i + 1);
+    }
   }
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   m->act_gen++;
   m->act_geo = make_conv_tc_geo(g.nb, g.nz, g.ny, g.nx);
+  m->act_zoff = g.zoff;
   for (int i = 0; i < 3; i++) {
     if (m->act[i]) cudaFree(m->act[i]);
     m->act[i] = nullptr;
@@ -82,11 +122,14 @@ int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
   for (float* p : m->bact) cudaFree(p);
   m->bact.clear();
   m->bgeo.clear();
+  m->borg.clear();
   if (m->part) cudaFree(m->part);
   m->part = nullptr;
-  for (int i = 1; i < m->nbanks; i++) {
-    const ConvTcGeo bg = make_conv_tc_geo(g.nb, g.nz >> i, g.ny >> i, g.nx >> i);
+  for (int i = 1, org = g.zoff; i < m->nbanks; i++) {
+    org = (org + 1) >> 1;
+    const ConvTcGeo bg = make_conv_tc_geo(g.nb, ((g.zoff + g.nz) >> i) - org, g.ny >> i, g.nx >> i);
     m->bgeo.push_back(bg);
+    m->borg.push_back(org);
     for (int q = 0; q < 3; q++) {
       float* p = nullptr;
       TFL_CUDA(ctx, cudaMalloc((void**)&p, conv_tc_act_bytes(bg)));
@@ -102,41 +145,55 @@ int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
 // Banked stack (split 1, join 3) on tensor cores: pyramid of the padded input, layers 1 and 2 of every bank at its
 // own resolution, then the join layer reading the banks' layer-2 outputs with nearest indexing.  'add': one launch
 // summing the banks; 'concat': one launch per bank (N..2 into the fp32 partial sum, bank 1 last with the tail).
-static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st) {
+// p_net is wanted on the local planes [p_lo, p_hi): bank i's layers 1 and 2 run on the coarse planes the join reads
+// from there (and the 3x3x3 stencil of layer 2 on those), the pyramid on all of the bank's planes.
+static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo, int p_hi) {
   const ConvTcGeo& tg = m->act_geo;
-  const int split = m->mode == 2 ? 1 : 0, nbk = m->nbanks;
+  const int split = m->mode == 2 ? 1 : 0, nbk = m->nbanks, zoff = m->act_zoff;
   const float* in[kTcMaxBanks];
   const float* l2[kTcMaxBanks];
   ConvTcGeo geo[kTcMaxBanks];
+  int org[kTcMaxBanks];
   in[0] = m->act[0];
   geo[0] = tg;
+  org[0] = zoff;
   for (int i = 1; i < nbk; i++) {
     geo[i] = m->bgeo[i - 1];
+    org[i] = m->borg[i - 1];
     float* dst = m->bact[3 * (i - 1)];
-    launch_tc_pyramid(in[i - 1], geo[i - 1], dst, geo[i], st);
+    // coarse plane c pools the planes 2 c, 2 c + 1 of the level above (global indices): local 2 c + (org[i-1] & 1)
+    launch_tc_pyramid(in[i - 1], geo[i - 1], dst, geo[i], org[i - 1] & 1, st);
     in[i] = dst;
   }
   for (int i = 0; i < nbk; i++) {
     float* o1 = i == 0 ? m->act[1] : m->bact[3 * (i - 1) + 1];
     float* o2 = i == 0 ? m->act[2] : m->bact[3 * (i - 1) + 2];
-    launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, 1, 0, split, geo[i], st);
-    launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, geo[i], st);
+    // the join reads bank i at the coarse planes of the full-resolution planes [p_lo - 1, p_hi]
+    const int c_lo = ((zoff + p_lo - 1) >> i) - org[i], c_hi = ((zoff + p_hi) >> i) - org[i] + 1;
+    ConvTcGeo g1 = geo[i], g2 = geo[i];
+    g2.z_lo = std::max(0, c_lo);     g2.z_hi = std::min(geo[i].nz, c_hi);
+    g1.z_lo = std::max(0, c_lo - 1); g1.z_hi = std::min(geo[i].nz, c_hi + 1);
+    launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, 1, 0, split, g1, st);
+    launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, g2, st);
     l2[i] = o2;
   }
-  launch_tc_join(l2, geo, nbk, m->bank_add, m->part, p_net, m->wBj[split].data(), m->b[m->conv0[2]], m->tail, split, tg,
-                 st);
+  ConvTcGeo g3 = tg;
+  g3.z_lo = std::max(0, p_lo);
+  g3.z_hi = std::min(tg.nz, p_hi);
+  launch_tc_join(l2, geo, org, zoff, nbk, m->bank_add, m->part, p_net, m->wBj[split].data(), m->b[m->conv0[2]],
+                 m->tail, split, g3, st);
 }
 
 // The three 3x3x3 layers (+ fused 1x1x1 tail) on tensor cores: act[0] -> act[1] -> act[2] -> p_net.
 // p_lo / p_hi: planes on which p_net is wanted (default all).  Layer l then only has to produce the planes the
 // later layers' 3x3x3 stencils reach from there; on a z-slab that spares most of the ghost planes.
 void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo, int p_hi) {
-  if (m->nbanks > 1) {       // whole grids only (the z-slab entry points refuse banked models)
-    run_conv_stack_banked(m, p_net, st);
+  if (p_hi < 0) p_hi = m->act_geo.nz;
+  if (m->nbanks > 1) {
+    run_conv_stack_banked(m, p_net, st, p_lo, p_hi);
     return;
   }
   const ConvTcGeo& tg = m->act_geo;
-  if (p_hi < 0) p_hi = tg.nz;
   const int split = m->mode == 2 ? 1 : 0;
   ConvTcGeo g1 = tg, g2 = tg, g3 = tg;
   g3.z_lo = std::max(0, p_lo);     g3.z_hi = std::min(tg.nz, p_hi);
@@ -382,17 +439,65 @@ int tfl_debug_conv3_tc(tfl_ctx* ctx, const float* in, float* out, float* p_net, 
 // banks[i] (device) is bank i+1's layer-2 output in the padded layout of make_conv_tc_geo(nb, nz >> i, ny >> i,
 // nx >> i); w_host [8][cin][3][3][3] with cin = 8 (add) or 8 nbanks (concat), bias [8], tail as in
 // tfl_debug_conv3_tc.  Writes p_net [nb][nz][ny][nx].  Synchronises before returning.
+static int debug_join_impl(tfl_ctx* ctx, const float* const* banks, int nbanks, int add, float* p_net,
+                           const float* w_host, const float* bias_host, const float* tail_host, int split, int nb,
+                           int nz, int ny, int nx, int zoff, const int32_t* bank_nz, const int32_t* bank_org, int z_lo,
+                           int z_hi);
+
 int tfl_debug_conv3_tc_join(tfl_ctx* ctx, const float* const* banks, int nbanks, int add, float* p_net,
                             const float* w_host, const float* bias_host, const float* tail_host, int split, int nb,
                             int nz, int ny, int nx) {
   DeviceGuard guard_(ctx);
   if (!ctx) return 1;
   if (nbanks < 1 || nbanks > kTcMaxBanks) return fail(ctx, "debug_conv3_tc_join: bad bank count %d", nbanks);
-  if (!banks || !p_net || !w_host || !bias_host || !tail_host) return fail(ctx, "debug_conv3_tc_join: nil argument");
   const int r = 1 << (nbanks - 1);
   if (nb < 1 || nz < 1 || ny < 1 || nx < 1 || nz % r || ny % r || nx % r)
     return fail(ctx, "debug_conv3_tc_join: grid %dx%dx%dx%d is not divisible by %d", nb, nz, ny, nx, r);
-  const ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  int32_t bnz[kTcMaxBanks], borg[kTcMaxBanks] = {};
+  for (int i = 0; i < nbanks; i++) bnz[i] = nz >> i;
+  return debug_join_impl(ctx, banks, nbanks, add, p_net, w_host, bias_host, tail_host, split, nb, nz, ny, nx, 0, bnz,
+                         borg, 0, nz);
+}
+
+// tfl_debug_conv3_tc_join_slab: the same join on a z-slab.  p_net's local planes [0, nz) are the global planes
+// zoff + z; bank i (i >= 1) holds bank_nz[i] planes from global coarse plane bank_org[i] on (bank_nz[0] and
+// bank_org[0] are ignored: bank 1 is nz planes from zoff).  Writes the output planes [z_lo, z_hi) of p_net only.
+int tfl_debug_conv3_tc_join_slab(tfl_ctx* ctx, const float* const* banks, int nbanks, int add, float* p_net,
+                                 const float* w_host, const float* bias_host, const float* tail_host, int split,
+                                 int nb, int nz, int ny, int nx, int zoff, const int32_t* bank_nz,
+                                 const int32_t* bank_org, int z_lo, int z_hi) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (nbanks < 1 || nbanks > kTcMaxBanks) return fail(ctx, "debug_conv3_tc_join_slab: bad bank count %d", nbanks);
+  if (!bank_nz || !bank_org) return fail(ctx, "debug_conv3_tc_join_slab: nil argument");
+  const int r = 1 << (nbanks - 1);
+  if (nb < 1 || nz < 1 || ny < 1 || nx < 1 || ny % r || nx % r || zoff < 0)
+    return fail(ctx, "debug_conv3_tc_join_slab: bad grid %dx%dx%dx%d", nb, nz, ny, nx);
+  if (z_lo < 0 || z_hi > nz || z_lo >= z_hi) return fail(ctx, "debug_conv3_tc_join_slab: bad z range [%d, %d)", z_lo, z_hi);
+  int32_t bnz[kTcMaxBanks], borg[kTcMaxBanks];
+  bnz[0] = nz;
+  borg[0] = zoff;
+  for (int i = 1; i < nbanks; i++) {
+    bnz[i] = bank_nz[i];
+    borg[i] = bank_org[i];
+    // the staged boxes may index ((z + zoff) >> i) - org for any z in [0, nz): inside the bank's padded planes
+    const int lo = (zoff >> i) - borg[i], hi = ((zoff + nz - 1) >> i) - borg[i];
+    if (bnz[i] < 1 || lo < -1 || hi > bnz[i])
+      return fail(ctx, "debug_conv3_tc_join_slab: bank %d (%d planes from %d) does not cover the slab", i + 1, bnz[i],
+                  borg[i]);
+  }
+  return debug_join_impl(ctx, banks, nbanks, add, p_net, w_host, bias_host, tail_host, split, nb, nz, ny, nx, zoff,
+                         bnz, borg, z_lo, z_hi);
+}
+
+static int debug_join_impl(tfl_ctx* ctx, const float* const* banks, int nbanks, int add, float* p_net,
+                           const float* w_host, const float* bias_host, const float* tail_host, int split, int nb,
+                           int nz, int ny, int nx, int zoff, const int32_t* bank_nz, const int32_t* bank_org, int z_lo,
+                           int z_hi) {
+  if (!banks || !p_net || !w_host || !bias_host || !tail_host) return fail(ctx, "debug_conv3_tc_join: nil argument");
+  ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  g.z_lo = z_lo;
+  g.z_hi = z_hi;
   const int cin = add ? 8 : 8 * nbanks, nw = add ? 1 : nbanks;
   std::vector<float*> wj(nw, nullptr);
   float *bias = nullptr, *tail = nullptr, *part = nullptr;
@@ -413,13 +518,37 @@ int tfl_debug_conv3_tc_join(tfl_ctx* ctx, const float* const* banks, int nbanks,
   cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
   cudaMemcpy(tail, tail_host, 81 * 4, cudaMemcpyHostToDevice);
   ConvTcGeo geo[kTcMaxBanks];
-  for (int i = 0; i < nbanks; i++) geo[i] = make_conv_tc_geo(nb, nz >> i, ny >> i, nx >> i);
-  launch_tc_join(banks, geo, nbanks, add, part, p_net, wj.data(), bias, tail, split, g, ctx->stream);
+  int org[kTcMaxBanks];
+  for (int i = 0; i < nbanks; i++) {
+    geo[i] = make_conv_tc_geo(nb, bank_nz[i], ny >> i, nx >> i);
+    org[i] = bank_org[i];
+  }
+  launch_tc_join(banks, geo, org, zoff, nbanks, add, part, p_net, wj.data(), bias, tail, split, g, ctx->stream);
   const int rc = check_launch(ctx, "debug_conv3_tc_join");
   const cudaError_t se = cudaStreamSynchronize(ctx->stream);
   release();
   if (rc) return rc;
   if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc_join: %s", cudaGetErrorString(se));
+  return 0;
+}
+
+// tfl_debug_tc_pyramid: one level of the bank pyramid on caller-owned padded buffers: in is
+// make_conv_tc_geo(nb, nz_in, ny, nx), out make_conv_tc_geo(nb, nz_out, ny / 2, nx / 2); out's planes [z_lo, z_hi)
+// pool in's planes 2 z + z_phase, 2 z + z_phase + 1.  Synchronises before returning.
+int tfl_debug_tc_pyramid(tfl_ctx* ctx, const float* in, float* out, int nb, int nz_in, int ny, int nx, int nz_out,
+                         int z_phase, int z_lo, int z_hi) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (!in || !out) return fail(ctx, "debug_tc_pyramid: nil argument");
+  if (nb < 1 || ny < 2 || nx < 2 || ny % 2 || nx % 2 || (z_phase != 0 && z_phase != 1) || z_lo < 0 || z_hi > nz_out ||
+      z_lo >= z_hi || 2 * z_hi + z_phase > nz_in)
+    return fail(ctx, "debug_tc_pyramid: bad arguments");
+  ConvTcGeo go = make_conv_tc_geo(nb, nz_out, ny / 2, nx / 2);
+  go.z_lo = z_lo;
+  go.z_hi = z_hi;
+  launch_tc_pyramid(in, make_conv_tc_geo(nb, nz_in, ny, nx), out, go, z_phase, ctx->stream);
+  if (check_launch(ctx, "debug_tc_pyramid")) return 1;
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return 0;
 }
 
@@ -657,9 +786,10 @@ int tfl_cnn_project(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, const tfl_g
 //   tfl_cnn_stats              U1 = SetWallBcs mask * U on every local plane where the mask is
 //                              computable, and (sum, sum of squares) over the OWNED planes into
 //                              dev_sums[2 * nb] (device doubles the caller all-reduces, e.g. with NCCL);
-//   tfl_cnn_project_from_sums  everything after the reduction.  The conv stack runs on the whole
-//                              local slab (halo planes included), so results are valid on planes at
-//                              least 4 planes away from a local end that is not a global end.
+//   tfl_cnn_project_from_sums  everything after the reduction.  The conv stack runs on the planes the
+//                              owned ones need, which must lie at least 4 planes (a banked model:
+//                              3 * 2^(banksNum-1) + 1, cnn_slab_check) away from a local end that is not
+//                              a global end.
 int tfl_cnn_stats(tfl_ctx* ctx, const tfl_grid* U_div, const tfl_grid* flags, const tfl_grid* U1,
                   double* dev_sums) {
   DeviceGuard guard_(ctx);
@@ -685,13 +815,16 @@ int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!m) return fail(ctx, "cnn is nil");
-  if (m->nbanks > 1) return fail(ctx, "cnn_project_from_sums: banked models run on whole grids only, not on z-slabs");
-  if (!m->tc_ok || m->mode == 0) return fail(ctx, "cnn_project_from_sums needs the tensor-core path (3-D default net)");
+  if (!m->tc_ok || m->mode == 0) return fail(ctx, "cnn_project_from_sums: %s", kSlabTcOnly);
+  if (!dev_sums) return fail(ctx, "cnn_project_from_sums: nil sums");
   if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, p_div, "pDiv") || check_vel(ctx, U1, flags) ||
       check_scalar(ctx, p_out, "p") || check_vel(ctx, U_out, flags))
     return 1;
   Geo g;
   if (make_geo(ctx, flags, 1, &g)) return 1;
+  if (ctx->slab && m->nbanks > 1 &&
+      cnn_slab_check(ctx, m, ctx->slab_margin, g.gnz, g.ny, g.nx, g.zoff, g.nz, g.zlo, g.zhi))
+    return 1;
   if (cnn_ensure_act(ctx, m, g)) return 1;
   const size_t cells = (size_t)g.n * g.nb;
   if (arena_reserve(ctx, carve_bytes({cells * 4, 4 * (size_t)g.nb}))) return 1;

@@ -100,14 +100,17 @@ struct tfl_cnn {
   float* tail = nullptr;     // w4[8][8], b4[8], w5[8], b5[1]
   float* act[3] = {nullptr, nullptr, nullptr};   // padded channels-last activation buffers
   ConvTcGeo act_geo = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
+  int act_zoff = 0;          // global plane of act's local plane 0 (z-slab; 0 on whole grids)
   unsigned long long act_gen = 0;   // bumped whenever act / bact / part are reallocated (see tfl_ctx::arena_gen)
   // Packed weights per split: layers 1 / 2 of bank i at wBk[2 i] / wBk[2 i + 1]; the join layer's weights (one for
   // 'add', bank i's 8-channel slice at wBj[i] for 'concat', which for one bank is the whole layer 3).  Banks 2..N
   // own three padded buffers each (pyramid input, layer 1, layer 2) at their resolution; 'concat' with N > 1 adds
-  // an fp32 partial sum.
+  // an fp32 partial sum.  On a z-slab, bank i's local plane 0 is its global coarse plane borg[i - 1] =
+  // ceil(act_zoff / 2^i), and it holds the coarse planes whose 2^i fine planes all lie in the local slab.
   std::vector<float*> wBk[2], wBj[2];
   std::vector<float*> bact;
   std::vector<ConvTcGeo> bgeo;
+  std::vector<int> borg;
   float* part = nullptr;
 };
 
@@ -235,3 +238,9 @@ StepForces step_forces(const tfl_mconf* mc, int nx, int ny, int gnz);
 // Tensor-core path of the projection network (tfl_api_cnn.cu).
 int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g);
 void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo = 0, int p_hi = -1);
+// Whether the model runs on a z-slab of a [gnz][ny][nx] domain with this margin whose local planes [0, nz) start at
+// global plane zoff and own [own_lo, own_hi): the tensor-core path, and for banked models the margin of
+// tfl_slab_cnn_margin, ghost planes that deep and a global grid divisible by 2^(banksNum-1).  Fails naming the
+// z-slab; launches nothing.
+int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, int nx, int zoff, int nz, int own_lo,
+                   int own_hi);

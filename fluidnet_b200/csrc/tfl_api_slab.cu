@@ -606,6 +606,15 @@ int tfl_slab_jacobi_schedule(int32_t gnz, int32_t world, int32_t rank, int32_t m
   return nblk;
 }
 
+// The projection network's ghost depth (cnn_slab_check): 3 s + 2 planes for the coarsest bank's scale s =
+// 2^(banks_num-1), i.e. a halo 2 margin + 2 from margin = ceil(3 s / 2), and never below the single-bank minimum 2.
+// 2 margin + 1 of it is the U / p exchange before the projection.
+int tfl_slab_cnn_margin(int32_t banks_num) {
+  if (banks_num <= 1) return 2;
+  if (banks_num > kTcMaxBanks) return -1;
+  return std::max(2, (3 * (1 << (banks_num - 1)) + 1) / 2);
+}
+
 }  // extern "C"
 
 namespace {
@@ -678,7 +687,8 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
   if (!jacobi && mc->sim_method != TFL_SIM_CONVNET)
     return fail(ctx, "slab_sim_step: mconf.simMethod (%d) is not a valid option", mc->sim_method);
   if (!jacobi && !cnn) return fail(ctx, "slab_sim_step: simMethod 'convnet' needs a model");
-  if (!jacobi && cnn->nbanks > 1) return fail(ctx, "slab_sim_step: banked models run on whole grids only, not on z-slabs");
+  if (!jacobi && cnn_slab_check(ctx, cnn, s->margin, s->gnz, s->ny, s->nx, s->zoff, s->nz, s->own_lo, s->own_hi))
+    return fail(ctx, "slab_sim_step: %s", ctx->err.c_str());
   if (jacobi && mc->max_iter < 0) return fail(ctx, "slab_sim_step: At least 1 iteration is needed (maxIter < 1)");
   if (s->world != ctx->comm_world || s->rank != ctx->comm_rank) return fail(ctx, "slab_sim_step: communicator changed");
   const tfl_state& st = s->st;
@@ -725,7 +735,8 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
     return tfl_clamp(ctx, &st.U, -1e6f, 1e6f);
   }
   if (bcs()) return 1;
-  if (slab_exchange(ctx, s, {&st.U, &st.p}, 5, 2)) return 1;
+  // the network input's reach across the cut (5 planes for a single bank)
+  if (slab_exchange(ctx, s, {&st.U, &st.p}, 2 * tfl_slab_cnn_margin(cnn->nbanks) + 1, 2)) return 1;
   tfl_grid u1 = st.U;
   u1.data = s->U1;
   {

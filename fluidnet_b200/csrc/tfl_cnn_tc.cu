@@ -428,8 +428,9 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   const int x0 = tx * 30, y0 = ty * T::TY, z0 = g.z_lo + tzb * T::TZ;         // padded coords of box origin
   const float4* inb = in + b * batch_g;
   if constexpr (JOIN) {
-    // Padded full-resolution coordinate g inside the grid -> bank coordinate ((g - 1) >> shift) + 1; outside,
-    // the bank's (0, 0, 0) border voxel, which is zero.  Banks are summed in order (CAddTable).
+    // Padded full-resolution coordinate g inside the grid -> bank coordinate ((g - 1) >> shift) + 1 (z: global
+    // planes, ((g - 1 + zoff) >> shift) - org + 1); outside, the bank's (0, 0, 0) border voxel, which is zero.
+    // Banks are summed in order (CAddTable).
     constexpr int PER = (T::POS + kThreads - 1) / kThreads;
     float4 v[PER][2];
 #pragma unroll
@@ -445,7 +446,7 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
         const int sh = js.shift[k];
         const int bx = interior ? ((gx - 1) >> sh) + 1 : 0;
         const int by = interior ? ((gy - 1) >> sh) + 1 : 0;
-        const int bz = interior ? ((gz - 1) >> sh) + 1 : 0;
+        const int bz = interior ? ((gz - 1 + js.zoff) >> sh) - js.org[k] + 1 : 0;
         const long long plane_k = (long long)(js.nz[k] + 2) * js.py[k] * js.px[k];
         const float4* src = (const float4*)js.p[k] + b * 2 * plane_k + ((long long)bz * js.py[k] + by) * js.px[k] + bx;
         const float4 a0 = __ldg(src), a1 = __ldg(src + plane_k);
@@ -728,19 +729,23 @@ void launch_z(const float4* in, float4* out, float* p_net, const float* wB, cons
   kern<<<grid, kZThreads, L::bytes(s.ww), st>>>(in, out, p_net, wB, bias, tail, g, s);
 }
 
-// 2x2x2 average of the first float4 plane (k_pool's summation order), zero fourth channel.
+// 2x2x2 average of the first float4 plane (k_pool's summation order), zero fourth channel; output planes
+// [go.z_lo, go.z_hi), input planes shifted by z_phase.
 __global__ void k_tc_pyramid(const float4* __restrict__ in, ConvTcGeo gi, float4* __restrict__ out, ConvTcGeo go,
-                             long long total) {
+                             int z_phase, long long total) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= total) return;
-  const int x = (int)(t % go.nx), y = (int)((t / go.nx) % go.ny), z = (int)((t / ((long long)go.nx * go.ny)) % go.nz);
-  const long long b = t / ((long long)go.nx * go.ny * go.nz);
+  const int nzr = go.z_hi - go.z_lo;
+  const int x = (int)(t % go.nx), y = (int)((t / go.nx) % go.ny);
+  const int z = go.z_lo + (int)((t / ((long long)go.nx * go.ny)) % nzr);
+  const long long b = t / ((long long)go.nx * go.ny * nzr);
   const float4* ib = in + b * 2 * (long long)(gi.nz + 2) * gi.py * gi.px;
   float sx = 0.0f, sy = 0.0f, sz = 0.0f;
   for (int dz = 0; dz < 2; dz++)
     for (int dy = 0; dy < 2; dy++)
       for (int dx = 0; dx < 2; dx++) {
-        const float4 v = __ldg(ib + ((long long)(2 * z + dz + 1) * gi.py + (2 * y + dy + 1)) * gi.px + (2 * x + dx + 1));
+        const float4 v =
+            __ldg(ib + ((long long)(2 * z + z_phase + dz + 1) * gi.py + (2 * y + dy + 1)) * gi.px + (2 * x + dx + 1));
         sx += v.x; sy += v.y; sz += v.z;
       }
   out[b * 2 * (long long)(go.nz + 2) * go.py * go.px + ((long long)(z + 1) * go.py + (y + 1)) * go.px + (x + 1)] =
@@ -809,9 +814,12 @@ int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, co
   return 1;
 }
 
-void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, cudaStream_t st) {
-  const long long total = (long long)gout.nb * gout.nz * gout.ny * gout.nx;
-  k_tc_pyramid<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float4*)in, gin, (float4*)out, gout, total);
+void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, int z_phase,
+                       cudaStream_t st) {
+  const long long total = (long long)gout.nb * (gout.z_hi - gout.z_lo) * gout.ny * gout.nx;
+  if (total <= 0) return;
+  k_tc_pyramid<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float4*)in, gin, (float4*)out, gout, z_phase,
+                                                                 total);
 }
 
 int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, const float* bias,

@@ -31,18 +31,24 @@ int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, 
 //   part_mode 1 / 2: write / add the x-tap-summed pre-activations to `partial` ([nb][nz][ny][nx][8] fp32), no
 //                    bias, no tail (the other banks of a 'concat' join);
 //   part_mode 3: add `partial` before the bias, then as part_mode 0.
+// On a z-slab the full-resolution plane z (local) is global plane z + zoff, and local plane 0 of bank k is its
+// global coarse plane org[k]: bank k is read at plane ((z + zoff) >> shift[k]) - org[k].  Whole grids: all zero.
 constexpr int kTcMaxBanks = 8;
 struct TcJoinSrc {
   const float* p[kTcMaxBanks];
-  int px[kTcMaxBanks], py[kTcMaxBanks], nz[kTcMaxBanks], shift[kTcMaxBanks];
+  int px[kTcMaxBanks], py[kTcMaxBanks], nz[kTcMaxBanks], shift[kTcMaxBanks], org[kTcMaxBanks];
+  int zoff;
   int n;
   int part_mode;
   float* partial;
 };
 int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, const float* bias, const float* tail,
                          int split, const ConvTcGeo& g, cudaStream_t st);
-// Bank pyramid on the padded channels-last layout: out's interior = 2x2x2 average of in's interior, first
-// float4 plane only (the 3 input channels and a zero fourth).  Borders of out are left as they are (zero).
-void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, cudaStream_t st);
+// Bank pyramid on the padded channels-last layout: out's plane z = 2x2x2 average of in's planes 2 z + z_phase and
+// 2 z + z_phase + 1 (interior, first float4 plane only: the 3 input channels and a zero fourth), for the output
+// planes [gout.z_lo, gout.z_hi).  z_phase (0 or 1) aligns the pooling to the global grid on a z-slab whose
+// fine level starts at an odd global plane.  Other planes and the borders of out are left as they are.
+void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, int z_phase,
+                       cudaStream_t st);
 
 }  // namespace tfl

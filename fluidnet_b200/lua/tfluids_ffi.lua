@@ -100,6 +100,7 @@ int tfl_slab_sim_ipc_connect(tfl_ctx*, tfl_slab_sim* sim, const char* handles);
 int tfl_slab_sim_jacobi_stats(tfl_ctx*, tfl_slab_sim* sim, int32_t* exchanges, float* ms, int64_t* bytes);
 int tfl_slab_jacobi_schedule(int32_t gnz, int32_t world, int32_t rank, int32_t margin, int32_t max_iter,
                              int32_t planes[3], int32_t* blocks, int32_t cap);
+int tfl_slab_cnn_margin(int32_t banks_num);
 int tfl_jacobi_slab_block(tfl_ctx*, const tfl_grid* pa, const tfl_grid* pb, const tfl_grid* flags,
                           const tfl_grid* div, int is_3d, int32_t z_lo, int32_t z_hi, int32_t shrink_lo,
                           int32_t shrink_hi, int32_t sweeps, int32_t path, int32_t* path_out);
@@ -350,6 +351,11 @@ function tfluids.slabJacobiSchedule(gnz, world, rank, margin, maxIter)   -- {pla
                      shrinkLo = raw[o + 4], shrinkHi = raw[o + 5]}
   end
   return {planes = {planes[0], planes[1], planes[2]}, blocks = blocks}
+end
+function tfluids.slabCnnMargin(banksNum)             -- smallest slab margin of a model with banksNum banks
+  local m = lib.tfl_slab_cnn_margin(banksNum)
+  assert(m > 0, 'slabCnnMargin: banksNum above 8')
+  return m
 end
 
 function tfluids.synchronize() check(lib.tfl_sync(ctx)) end

@@ -13,6 +13,8 @@ before each phase whose stencil reaches across the cut:
     exchange U, p        (5)      -> CNN projection: wall mask + sum/sumsq on owned planes,
                                      all-reduce of the two sums (the input scale), conv stack on the
                                      whole local slab, velocity update on owned planes
+                                     (banked models: 2 * cnn_margin(banksNum) + 1 planes; the halo
+                                     then needs margin >= cnn_margin(banksNum))
 
 simMethod 'jacobi' (no model) replaces the last phase: setWallBcsForward on the owned planes, then
 
@@ -52,6 +54,27 @@ def jacobi_schedule(gnz, world, rank, margin, max_iter):
     lib.tfl_slab_jacobi_schedule(gnz, world, rank, margin, max_iter, planes, raw, n)
     k = _lib.JACOBI_BLOCK_INTS
     return tuple(planes), [tuple(raw[b * k:(b + 1) * k]) for b in range(n)]
+
+
+def cnn_margin(banks_num):
+    """The smallest slab margin a projection network with `banks_num` banks runs with (tfl_slab_cnn_margin): 2 for
+    one bank, ceil(3 * 2^(banks_num-1) / 2) for more -- the coarsest bank's stencil reaches 3 * 2^(banks_num-1) + 2
+    planes across a rank boundary, and the halo holds 2 * margin + 2."""
+    m = _lib.load().tfl_slab_cnn_margin(int(banks_num))
+    if m < 1:
+        raise ValueError("no z-slab margin for %d banks (at most 8)" % banks_num)
+    return m
+
+
+def _resolve_margin(margin, banks):
+    """margin=None -> the model's minimum (2 for a single bank); an explicit margin below it raises ValueError."""
+    n = banks["num"] if banks else 1
+    need = cnn_margin(n)
+    if margin is None:
+        return max(2, need)
+    if n > 1 and margin < need:
+        raise ValueError("a %d-bank model needs a z-slab margin >= %d (got %d)" % (n, need, margin))
+    return margin
 
 
 def _sim_method(mconf):
@@ -129,11 +152,14 @@ class SlabDecomposition:
 class SlabSimulator:
     """tfluids.simulate (simMethod 'convnet' or 'jacobi') for one domain split in z across the ranks of `group`."""
 
-    def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=2, group=None,
-                 jacobi_path=-1):
+    def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=None, group=None,
+                 jacobi_path=-1, banks=None, conv_mode=None):
         """batch: dict of GLOBAL torch CPU tensors (pDiv, UDiv, flags, density and the BC arrays),
-        identical on every rank.  margin: planes a backward trace may reach (ceil(max|u| dt) + 1).
-        model_layers: None for simMethod 'jacobi'.  jacobi_path: tfl_jacobi_slab_block's path (-1 automatic)."""
+        identical on every rank.  margin: planes a backward trace may reach (ceil(max|u| dt) + 1); None: the
+        smallest the model runs with (cnn_margin), 2 for a single bank.
+        model_layers: None for simMethod 'jacobi'.  jacobi_path: tfl_jacobi_slab_block's path (-1 automatic).
+        banks / conv_mode: ProjectionModel's banks and, if given, its mode ('tf32' or 'tf32x3'; slabs run on the
+        tensor cores only)."""
         from . import tfluids, model as fmodel
         self.tfluids = tfluids
         self.group = group
@@ -142,6 +168,7 @@ class SlabSimulator:
         self.mconf = dict(mconf)
         method, iters = _sim_method(self.mconf)
         self.jacobi = method == "jacobi"
+        margin = _resolve_margin(margin, None if self.jacobi else banks)
         gnz = batch["flags"].shape[2]
         assert margin >= 2, "margin < 2 makes the halo narrower than the widest fixed exchange (5 planes)"
         self.dec = SlabDecomposition(gnz, self.rank, self.world, halo=2 * margin + 2)
@@ -156,8 +183,10 @@ class SlabSimulator:
             self.div = torch.zeros_like(self.s["pDiv"])
             self.p2 = torch.zeros_like(self.s["pDiv"])
         else:
-            self.model = fmodel.ProjectionModel(model_layers, True, device=self.device,
+            self.model = fmodel.ProjectionModel(model_layers, True, device=self.device, banks=banks,
                                                 normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
+            if conv_mode is not None:
+                self.model.set_mode(conv_mode)
         self.U1 = torch.empty_like(self.s["UDiv"])
         self.sums = torch.zeros(2, dtype=torch.float64, device=self.device)
 
@@ -225,7 +254,7 @@ class SlabSimulator:
             t.clamp(U, -1e6, 1e6)
             return
         self._bc()
-        yield ("halo", [U, p], 5)
+        yield ("halo", [U, p], 2 * cnn_margin(self.model.banks["num"] if self.model.banks else 1) + 1)
         c, lib = self.ctx, self.ctx.lib
         with self._slab(d.own_lo, d.own_hi):
             c.use_current_stream()
@@ -298,13 +327,17 @@ class NativeSlabSimulator:
     This is what a LuaJIT host would drive; torch.distributed is used here only to hand rank 0's NCCL id to the
     other ranks (any transport would do) and, in `gather`, by the tests."""
 
-    def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=2, group=None,
-                 peer_halos=True):
+    def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=None, group=None,
+                 peer_halos=True, banks=None, conv_mode=None):
+        """Arguments as SlabSimulator's (margin=None: the model's smallest, cnn_margin)."""
         import numpy as np
         from . import tfluids, model as fmodel, simulate, _lib
         self.group = group
         self.rank = dist.get_rank(group) if rank is None else rank
         self.world = dist.get_world_size(group) if world is None else world
+        self.mconf = dict(mconf)
+        method, _ = _sim_method(self.mconf)
+        margin = _resolve_margin(margin, None if method == "jacobi" else banks)
         self.device = torch.device(device)
         self.ctx = tfluids.context(self.device)
         lib = self.ctx.lib
@@ -316,11 +349,12 @@ class NativeSlabSimulator:
                 ident = [buf.raw]
             dist.broadcast_object_list(ident, src=0, group=group)
         self.ctx.check(lib.tfl_comm_init(self.ctx.h, ident[0] if ident[0] else b"\0" * _lib.COMM_ID_BYTES, self.rank, self.world))
-        self.mconf = dict(mconf)
-        method, _ = _sim_method(self.mconf)
         self.mc = simulate.make_mconf(self.mconf)
         self.model = None if method == "jacobi" else fmodel.ProjectionModel(
-            model_layers, True, device=self.device, normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
+            model_layers, True, device=self.device, banks=banks,
+            normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
+        if self.model is not None and conv_mode is not None:
+            self.model.set_mode(conv_mode)
 
         def host(key):
             t = batch.get(key)

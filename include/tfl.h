@@ -217,9 +217,9 @@ typedef struct tfl_cnn_banks {
  * channels in bank order (cin[join-1] = num * cout[join-2]) or summed left to right.  cin, cout, ksize, pool
  * and up are per stage; weights / biases list the convolutions stage by stage, bank 1 .. num for a banked
  * stage.  banks == NULL or num == 1: exactly tfl_cnn_create_graph.  The grid at the split resolution must be
- * divisible by 2^(num-1).  Banked models run on whole grids (not on z-slabs); the 3-D 'default' graph with
- * split_stage 1 and join_stage 3 (num <= 8) runs on the tensor cores (3xTF32 by default), every other one on the
- * fp32 path. */
+ * divisible by 2^(num-1).  The 3-D 'default' graph with split_stage 1 and join_stage 3 (num <= 8) runs on the
+ * tensor cores (3xTF32 by default), also on z-slabs (tfl_slab_sim_step with margin >= tfl_slab_cnn_margin(num));
+ * every other banked graph runs on the fp32 path, on whole grids only. */
 int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                           const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
@@ -241,8 +241,10 @@ int tfl_cnn_project(tfl_ctx* ctx, tfl_cnn* cnn, const tfl_grid* p_div, const tfl
 /* z-slab variant of model:forward, split around its one global reduction (the input scale):
  * tfl_cnn_stats writes U1 = wall-mask * U and the (sum, sum of squares) of U1 over the OWNED planes
  * into dev_sums[2 * nb] (device doubles, to be all-reduced by the caller, e.g. NCCL);
- * tfl_cnn_project_from_sums does the rest.  The conv stack runs on the whole local slab, so results
- * are exact on planes >= 4 planes away from a local end that is not a global end. */
+ * tfl_cnn_project_from_sums does the rest, on the tensor-core path only: it computes p on the owned planes and the
+ * one below them and U on the owned planes, which needs the inputs on 4 planes beyond each owned end that is not a
+ * global end (3 * 2^(banksNum-1) + 1 for a banked model, whose margin set by tfl_set_slab_margin must then be at
+ * least tfl_slab_cnn_margin(banksNum) and whose global grid must be divisible by 2^(banksNum-1)). */
 int tfl_cnn_stats(tfl_ctx* ctx, const tfl_grid* U_div, const tfl_grid* flags, const tfl_grid* U1,
                   double* dev_sums);
 int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* cnn, const tfl_grid* p_div, const tfl_grid* U1,
@@ -333,7 +335,11 @@ int tfl_slab_sim_download(tfl_ctx* ctx, tfl_slab_sim* sim, float* p, float* U, f
  * of U, the divergence, mconf->max_iter sweeps (0: 100) from p = 0 with pTol = 0 in the blocks of
  * tfl_slab_jacobi_schedule (one p exchange before every block but the first), the velocity update.  No global
  * reduction: p, U and density are bit-identical to tfl_simulate_step's.
- * simMethod 'pcg' is refused (its IC(0) triangular solves do not shard over z), and so are banked models. */
+ * simMethod 'pcg' is refused (its IC(0) triangular solves do not shard over z).  The model runs on the tensor cores
+ * (mode 1 or 2): the 3-D 'default' graph, single-bank or with banks split at stage 1 and joined at stage 3, for which
+ * the slab's margin must be at least tfl_slab_cnn_margin(banksNum) and the global grid divisible by
+ * 2^(banksNum-1); the U / p exchange before the projection is then 2 * tfl_slab_cnn_margin(banksNum) + 1 planes wide
+ * (5 for a single bank).  Other models are refused before anything is launched. */
 int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* sim, const tfl_mconf* mconf, tfl_cnn* cnn);
 /* Device time (ms) of the last step's three halo exchanges and of its all-reduce (0 on the Jacobi path), and the
  * bytes this rank sent in each exchange.  Synchronises. */
@@ -352,6 +358,11 @@ int tfl_slab_sim_jacobi_stats(tfl_ctx* ctx, tfl_slab_sim* sim, int32_t* exchange
 #define TFL_JACOBI_BLOCK_INTS 6
 int tfl_slab_jacobi_schedule(int32_t gnz, int32_t world, int32_t rank, int32_t margin, int32_t max_iter,
                              int32_t planes[3], int32_t* blocks, int32_t cap);
+/* The smallest slab margin (tfl_slab_sim_create) a projection network with banks_num banks runs with (pure
+ * function): 2 for banks_num <= 1, ceil(3 * 2^(banks_num-1) / 2) for 2 .. 8 banks (3, 6, 12, ...), -1 above.  The
+ * coarsest bank's stencil reaches 3 * 2^(banks_num-1) + 2 planes across a rank boundary, which the halo of
+ * 2 * margin + 2 planes must hold.  Use max(this, the advection's margin). */
+int tfl_slab_cnn_margin(int32_t banks_num);
 /* One block of Jacobi sweeps under the context's slab placement (tfl_set_slab: offset and global extent; the
  * placement's plane range is not used): sweep s = 0 .. sweeps-1 computes local planes
  * [z_lo + s * shrink_lo, z_hi - s * shrink_hi) of p from the other buffer -- even sweeps read pa and write pb, odd
