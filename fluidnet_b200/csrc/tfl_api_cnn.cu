@@ -1,5 +1,5 @@
 // C ABI of the projection network (include/tfl.h): model creation, modes, the fp32 graph executor and the
-// tensor-core stacks (tfl_cnn*.cu), and the test hooks of the tensor-core layers.
+// tensor-core stacks (tfl_cnn*.cu), and the test hooks of the tensor-core layers and of the fp32 kernels.
 #include <string.h>
 #include <algorithm>
 #include <cmath>
@@ -23,6 +23,17 @@ float* upload_tc_weights(const float* w, int cin, int split) {
   if (cudaMalloc((void**)&d, packed.size() * 4) != cudaSuccess) return nullptr;
   cudaMemcpy(d, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice);
   return d;
+}
+
+// A convolution weight in Torch layout [cout][cin][taps] re-laid out as the [cin][tap][cout] that
+// launch_conv_direct and launch_conv_any read.
+std::vector<float> relayout_conv_weights(const float* w, int cin, int cout, int taps) {
+  std::vector<float> relaid((size_t)cin * taps * cout);
+  for (int o = 0; o < cout; o++)
+    for (int c = 0; c < cin; c++)
+      for (int t = 0; t < taps; t++)
+        relaid[((size_t)c * taps + t) * cout + o] = w[((size_t)o * cin + c) * taps + t];
+  return relaid;
 }
 
 // Bank i's 8-channel slice of a 'concat' join weight [8][8 nbanks][3][3][3] (one bank: the whole weight).
@@ -62,6 +73,27 @@ void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org
       launch_conv3_tc_join(src_of(i, 1, nbanks == 1 ? 0 : (i == nbanks - 1 ? 1 : (i > 0 ? 2 : 3))), p_net, wj[i], bias,
                            tail, split, g, st);
   }
+}
+
+// The whole-grid geometry of the fp32 test hooks, and their grid check and closing synchronisation.
+Geo whole_grid(tfl_ctx* ctx, int nb, int nz, int ny, int nx, int is3d) {
+  Geo g = {};
+  g.nx = nx; g.ny = ny; g.nz = nz; g.gnz = nz; g.zoff = 0; g.zlo = 0; g.zhi = nz; g.nb = nb;
+  g.is3d = is3d ? 1 : 0;
+  g.nc = is3d ? 3 : 2;
+  g.n = (long long)nx * ny * nz;
+  g.faults = ctx->counters;
+  return g;
+}
+bool bad_grid(int nb, int nz, int ny, int nx, int is3d) {
+  return nb < 1 || nz < 1 || ny < 1 || nx < 1 || (!is3d && nz != 1) || (long long)nz * ny * nx >= (1LL << 31);
+}
+int finish_debug(tfl_ctx* ctx, const char* what) {
+  const int rc = check_launch(ctx, what);
+  const cudaError_t se = cudaStreamSynchronize(ctx->stream);
+  if (rc) return rc;
+  if (se != cudaSuccess) return fail(ctx, "%s: %s", what, cudaGetErrorString(se));
+  return 0;
 }
 
 }  // namespace
@@ -306,11 +338,7 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
     const int kz = is_3d ? ksize[l] : 1;
     const int taps = kz * ksize[l] * ksize[l];
     for (int bk = 0; bk < convs_of(l); bk++, wi++) {
-      std::vector<float> relaid((size_t)cin[l] * taps * cout[l]);
-      for (int o = 0; o < cout[l]; o++)
-        for (int c = 0; c < cin[l]; c++)
-          for (int t = 0; t < taps; t++)
-            relaid[((size_t)c * taps + t) * cout[l] + o] = weights[wi][((size_t)o * cin[l] + c) * taps + t];
+      const std::vector<float> relaid = relayout_conv_weights(weights[wi], cin[l], cout[l], taps);
       float *dw = nullptr, *db = nullptr;
       if (cudaMalloc((void**)&dw, relaid.size() * 4) != cudaSuccess ||
           cudaMalloc((void**)&db, cout[l] * 4) != cudaSuccess) { tfl_cnn_destroy(ctx, m); return fail(ctx, "cnn: cudaMalloc failed"); }
@@ -550,6 +578,88 @@ int tfl_debug_tc_pyramid(tfl_ctx* ctx, const float* in, float* out, int nb, int 
   if (check_launch(ctx, "debug_tc_pyramid")) return 1;
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return 0;
+}
+
+// Undocumented test hooks (not in tfl.h): the fp32 path's kernels (tfl_cnn.cu) on caller-owned device buffers, on
+// the context's stream.  Each synchronises before returning.
+// tfl_debug_conv_fp32: one convolution in [nb][cin][nz][ny][nx] -> out [nb][cout][nz][ny][nx] (nz = 1 in 2-D),
+// weights [cout][cin][kz][k][k] (kz = k in 3-D, else 1) and bias [cout] on the host, re-laid out as
+// tfl_cnn_create_graph does.  generic = 0: launch_conv_direct (the specialised kernel where the shape has one and its
+// weights fit shared memory, else the generic one); generic = 1: the generic kernel.  *kernel: the kernel that ran,
+// 1 direct or 2 generic.
+int tfl_debug_conv_fp32(tfl_ctx* ctx, const float* in, float* out, const float* w_host, const float* bias_host,
+                        int cin, int cout, int ks, int act, int is3d, int nb, int nz, int ny, int nx, int generic,
+                        int32_t* kernel) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (!in || !out || !w_host || !bias_host || !kernel) return fail(ctx, "debug_conv_fp32: nil argument");
+  if (cin < 1 || cout < 1 || ks < 1 || ks % 2 != 1 || act < 0 || act > 2 || (generic != 0 && generic != 1))
+    return fail(ctx, "debug_conv_fp32: bad layer cin=%d cout=%d k=%d act=%d generic=%d", cin, cout, ks, act, generic);
+  if (bad_grid(nb, nz, ny, nx, is3d)) return fail(ctx, "debug_conv_fp32: bad grid %dx%dx%dx%d", nb, nz, ny, nx);
+  const int taps = (is3d ? ks : 1) * ks * ks;
+  const std::vector<float> relaid = relayout_conv_weights(w_host, cin, cout, taps);
+  float *dw = nullptr, *db = nullptr;
+  if (cudaMalloc((void**)&dw, relaid.size() * 4) != cudaSuccess || cudaMalloc((void**)&db, cout * 4) != cudaSuccess) {
+    if (dw) cudaFree(dw);
+    return fail(ctx, "debug_conv_fp32: cudaMalloc failed");
+  }
+  cudaMemcpy(dw, relaid.data(), relaid.size() * 4, cudaMemcpyHostToDevice);
+  cudaMemcpy(db, bias_host, cout * 4, cudaMemcpyHostToDevice);
+  const Geo g = whole_grid(ctx, nb, nz, ny, nx, is3d);
+  const int ran = generic ? launch_conv_any(in, out, dw, db, cin, cout, ks, act, g, ctx->stream)
+                          : launch_conv_direct(in, out, dw, db, cin, cout, ks, act, g, ctx->stream);
+  const int rc = finish_debug(ctx, "debug_conv_fp32");
+  cudaFree(dw);
+  cudaFree(db);
+  if (rc) return rc;
+  if (ran < 0) return fail(ctx, "debug_conv_fp32: no kernel for cout=%d k=%d", cout, ks);
+  *kernel = ran;
+  return 0;
+}
+
+// tfl_debug_pool: launch_pool, in [nbc][nz][ny][nx] -> out [nbc][nz / pz][ny / p][nx / p] (pz = p in 3-D, else 1);
+// the grid must be divisible, as the graph executor checks before it pools.
+int tfl_debug_pool(tfl_ctx* ctx, const float* in, float* out, int nbc, int nz, int ny, int nx, int p, int is3d,
+                   int is_max) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (!in || !out) return fail(ctx, "debug_pool: nil argument");
+  if (p < 1 || bad_grid(nbc, nz, ny, nx, is3d) || nx % p || ny % p || (is3d && nz % p))
+    return fail(ctx, "debug_pool: grid %dx%dx%dx%d does not pool by %d", nbc, nz, ny, nx, p);
+  launch_pool(in, out, nbc, nz, ny, nx, p, is3d, is_max ? 1 : 0, ctx->stream);
+  return finish_debug(ctx, "debug_pool");
+}
+
+// tfl_debug_pixel_shuffle: launch_pixel_shuffle, in [nb][n_out s^d][nz][ny][nx] -> out [nb][n_out][nz sz][ny s][nx s]
+// (sz = s in 3-D, else 1).
+int tfl_debug_pixel_shuffle(tfl_ctx* ctx, const float* in, float* out, int nb, int n_out, int nz, int ny, int nx,
+                            int s, int is3d) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (!in || !out) return fail(ctx, "debug_pixel_shuffle: nil argument");
+  if (n_out < 1 || s < 1 || bad_grid(nb, nz, ny, nx, is3d))
+    return fail(ctx, "debug_pixel_shuffle: bad arguments n_out=%d s=%d grid %dx%dx%dx%d", n_out, s, nb, nz, ny, nx);
+  launch_pixel_shuffle(in, out, nb, n_out, nz, ny, nx, s, is3d, ctx->stream);
+  return finish_debug(ctx, "debug_pixel_shuffle");
+}
+
+// tfl_debug_bank_join: launch_bank_join.  banks (host array of device pointers; banks[0] is not read) as in
+// tfl_kernels.h; out [nb][nbanks c][nz][ny][nx] holding bank 1 in its first c channels ('concat', add = 0) or
+// [nb][c][nz][ny][nx] holding bank 1 (add = 1).  The grid must be divisible by 2^(nbanks-1) (z in 3-D only).
+int tfl_debug_bank_join(tfl_ctx* ctx, const float* const* banks, int nbanks, float* out, int nb, int c, int nz,
+                        int ny, int nx, int is3d, int add) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (nbanks < 2 || nbanks > kMaxBankPtrs) return fail(ctx, "debug_bank_join: bad bank count %d", nbanks);
+  if (!banks || !out) return fail(ctx, "debug_bank_join: nil argument");
+  for (int i = 1; i < nbanks; i++)
+    if (!banks[i]) return fail(ctx, "debug_bank_join: nil bank %d", i + 1);
+  const int r = 1 << (nbanks - 1);
+  if (c < 1 || bad_grid(nb, nz, ny, nx, is3d) || nx % r || ny % r || (is3d && nz % r))
+    return fail(ctx, "debug_bank_join: grid %dx%dx%dx%d is not divisible by %d", nb, nz, ny, nx, r);
+  if (launch_bank_join(banks, nbanks, out, nb, c, nz, ny, nx, is3d, add ? 1 : 0, ctx->stream) < 0)
+    return fail(ctx, "debug_bank_join: bad bank count %d", nbanks);
+  return finish_debug(ctx, "debug_bank_join");
 }
 
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {

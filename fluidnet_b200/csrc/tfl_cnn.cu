@@ -219,16 +219,21 @@ int launch_conv_direct(const float* in, float* out, const float* wdev, const flo
   if (cout == CO && ksize == KS_) {                                                   \
     const bool ok_ = g.is3d ? conv_launch<CO, KS_, true>(in, out, wdev, bdev, cin, act, g, st)    \
                             : conv_launch<CO, KS_, false>(in, out, wdev, bdev, cin, act, g, st);  \
-    if (ok_) return 1;                                                                \
+    if (ok_) return kConvDirect;                                                      \
   }
   TFL_CONV_CASE(8, 3) TFL_CONV_CASE(8, 1) TFL_CONV_CASE(1, 1) TFL_CONV_CASE(16, 3) TFL_CONV_CASE(16, 1)
   TFL_CONV_CASE(1, 3) TFL_CONV_CASE(6, 3) TFL_CONV_CASE(6, 1) TFL_CONV_CASE(32, 1) TFL_CONV_CASE(16, 5)
   TFL_CONV_CASE(32, 5) TFL_CONV_CASE(64, 5) TFL_CONV_CASE(64, 1)
 #undef TFL_CONV_CASE
+  return launch_conv_any(in, out, wdev, bdev, cin, cout, ksize, act, g, st);
+}
+
+int launch_conv_any(const float* in, float* out, const float* wdev, const float* bdev, int cin, int cout, int ksize,
+                    int act, const Geo& g, cudaStream_t st) {
   if (g.zlo != 0 || g.zhi != g.nz || g.zoff != 0) return -1;      // the generic kernel works on whole grids only
   const long long total = (long long)g.nb * cout * g.n;
   k_conv_any<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, out, wdev, bdev, cin, cout, ksize, act, g);
-  return 1;
+  return kConvGeneric;
 }
 
 void launch_pool(const float* in, float* out, int nbc, int nz, int ny, int nx, int p, int is3d, int is_max,

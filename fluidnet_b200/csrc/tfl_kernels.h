@@ -106,8 +106,14 @@ void launch_cnn_finish_fused(const float* p_net, float* U, const unsigned char* 
 // Generic direct convolution (fp32 FMA): in [b][cin][z][y][x] -> out [b][cout][z][y][x].
 // wdev: device weights re-laid out as [cin][tap][cout_pad], bias [cout].
 // act: 0 none, 1 ReLU, 2 sigmoid.
+// Returns the kernel that ran: kConvDirect (k_conv_direct, a specialised (cout, k) whose weights fit shared
+// memory) or kConvGeneric (k_conv_any, every other shape, whole grids only); -1 if none can run.
+enum : int { kConvDirect = 1, kConvGeneric = 2 };
 int launch_conv_direct(const float* in, float* out, const float* wdev, const float* bdev, int cin, int cout,
                        int ksize, int act, const Geo& g, cudaStream_t st);
+// The generic kernel alone (launch_conv_direct's fallback): same operands, same accumulation order.
+int launch_conv_any(const float* in, float* out, const float* wdev, const float* bdev, int cin, int cout, int ksize,
+                    int act, const Geo& g, cudaStream_t st);
 void launch_pool(const float* in, float* out, int nbc, int nz, int ny, int nx, int p, int is3d, int is_max,
                  cudaStream_t st);
 void launch_pixel_shuffle(const float* in, float* out, int nb, int n_out, int nz, int ny, int nx, int s, int is3d,
