@@ -948,7 +948,8 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
 
 // Whether tfl_simulate_step takes the fused pipeline for this state, configuration and model.
 static bool fused_step_applies(const tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, const tfl_cnn* cnn) {
-  return mc->sim_method == TFL_SIM_CONVNET && cnn && cnn->tc_ok && cnn->mode > 0 && !ctx->slab && s->flags.nb == 1 &&
+  return mc->sim_method == TFL_SIM_CONVNET && cnn && cnn->tc_ok && cnn->mode > 0 && cnn->default_inputs && !ctx->slab &&
+         s->flags.nb == 1 &&
          !s->p_bc.data && mc->advection_method >= 0 && mc->advection_method <= 5;
 }
 

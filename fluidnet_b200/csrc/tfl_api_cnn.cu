@@ -11,6 +11,9 @@ constexpr int kMaxBanks = kMaxBankPtrs;     // banks a join kernel takes
 constexpr char kSlabTcOnly[] =
     "the z-slab projection runs on the tensor-core path only (the 3-D 'default' graph, single-bank or with banks "
     "split at stage 1 and joined at stage 3, in mode 1 or 2)";
+constexpr char kSlabDefaultInputs[] =
+    "the z-slab projection takes the default input block only (inputChannels pDiv, div, flags; normalizeInput with "
+    "'std' of UDiv; no addPressureSkip)";
 
 namespace {
 
@@ -34,6 +37,14 @@ std::vector<float> relayout_conv_weights(const float* w, int cin, int cout, int 
       for (int t = 0; t < taps; t++)
         relaid[((size_t)c * taps + t) * cout + o] = w[((size_t)o * cin + c) * taps + t];
   return relaid;
+}
+
+// A layer-1 weight [8][cin][3][3][3] zero-padded to [8][8][3][3][3] (the two-plane input of a set with UDiv).
+std::vector<float> pad_cin8(const float* w, int cin) {
+  std::vector<float> padded(8 * 8 * 27, 0.0f);
+  for (int o = 0; o < 8; o++)
+    memcpy(padded.data() + (size_t)o * 8 * 27, w + (size_t)o * cin * 27, (size_t)cin * 27 * 4);
+  return padded;
 }
 
 // Bank i's 8-channel slice of a 'concat' join weight [8][8 nbanks][3][3][3] (one bank: the whole weight).
@@ -106,6 +117,7 @@ int finish_debug(tfl_ctx* ctx, const char* what) {
 // planes short of the local end), which a halo of 2 margin + 2 provides from margin = 3 s / 2 on.
 int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, int nx, int zoff, int nz, int own_lo,
                    int own_hi) {
+  if (!m->default_inputs) return fail(ctx, "slab: %s", kSlabDefaultInputs);
   if (!m->tc_ok || m->mode == 0) return fail(ctx, "slab: %s", kSlabTcOnly);
   if (m->nbanks == 1) return 0;
   const int need = tfl_slab_cnn_margin(m->nbanks), s = 1 << (m->nbanks - 1), depth = 3 * s + 2;
@@ -194,7 +206,7 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
     org[i] = m->borg[i - 1];
     float* dst = m->bact[3 * (i - 1)];
     // coarse plane c pools the planes 2 c, 2 c + 1 of the level above (global indices): local 2 c + (org[i-1] & 1)
-    launch_tc_pyramid(in[i - 1], geo[i - 1], dst, geo[i], org[i - 1] & 1, st);
+    launch_tc_pyramid(in[i - 1], geo[i - 1], dst, geo[i], org[i - 1] & 1, st, m->tc_planes);
     in[i] = dst;
   }
   for (int i = 0; i < nbk; i++) {
@@ -205,7 +217,8 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
     ConvTcGeo g1 = geo[i], g2 = geo[i];
     g2.z_lo = std::max(0, c_lo);     g2.z_hi = std::min(geo[i].nz, c_hi);
     g1.z_lo = std::max(0, c_lo - 1); g1.z_hi = std::min(geo[i].nz, c_hi + 1);
-    launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, 1, 0, split, g1, st);
+    launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, m->tc_planes, 0, split,
+                    g1, st);
     launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, g2, st);
     l2[i] = o2;
   }
@@ -231,7 +244,7 @@ void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo, int p_h
   g3.z_lo = std::max(0, p_lo);     g3.z_hi = std::min(tg.nz, p_hi);
   g2.z_lo = std::max(0, p_lo - 1); g2.z_hi = std::min(tg.nz, p_hi + 1);
   g1.z_lo = std::max(0, p_lo - 2); g1.z_hi = std::min(tg.nz, p_hi + 2);
-  launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, 1, 0, split, g1, st);
+  launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, m->tc_planes, 0, split, g1, st);
   launch_conv3_tc(m->act[1], m->act[2], nullptr, m->wBk[split][1], m->b[1], nullptr, 2, 0, split, g2, st);
   launch_conv3_tc(m->act[2], nullptr, p_net, m->wBj[split][0], m->b[2], m->tail, 2, 1, split, g3, st);
 }
@@ -251,8 +264,13 @@ int tfl_cnn_create(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, co
 
 static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
-                           const float* const* biases, tfl_cnn** out);
+                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                           const float* const* weights, const float* const* biases, tfl_cnn** out);
+static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                              int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                              const float* const* weights, const float* const* biases, tfl_cnn** out);
+static const tfl_cnn_inputs kDefaultInputs = {1, 0, 1, 1, 0, 0, 0};
 
 int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
                          const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
@@ -261,7 +279,7 @@ int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   return cnn_create_impl(ctx, is_3d, n_layers, cin, cout_logical, ksize, pool, up, pool_is_max, nonlin_sigmoid,
-                         nullptr, weights, biases, out);
+                         nullptr, &kDefaultInputs, weights, biases, out);
 }
 
 int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
@@ -270,6 +288,47 @@ int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* 
                           const float* const* biases, tfl_cnn** out) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
+  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
+                            &kDefaultInputs, weights, biases, out);
+}
+
+int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                         const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                         int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                         const float* const* weights, const float* const* biases, tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  const tfl_cnn_inputs in = inputs ? *inputs : kDefaultInputs;
+  // lib/model.lua:27-150 and :357-361; checkYangSettings, lib/model_utils.lua:211-227.
+  if (!in.p_div && !in.u_div && !in.div) return fail(ctx, "Are you sure you dont want any (U, div or p) fields?");
+  if (!in.u_div && !in.div)
+    return fail(ctx, "cnn: inputChannels needs UDiv or div: tfluids.VelocityUpdate takes UDiv, which the graph "
+                     "selects only for them (lib/model.lua:69-72, :380)");
+  if (in.normalize && in.norm_func != 0 && in.norm_func != 1) return fail(ctx, "Incorrect normalize input function");
+  if (in.normalize && (in.norm_chan < 0 || in.norm_chan > 2)) return fail(ctx, "Incorrect normalize input channel.");
+  if (in.normalize && in.norm_chan == 2 && !in.div)
+    return fail(ctx, "cnn: normalizeInputChan 'div' needs inputChannels.div (lib/model.lua:108-116)");
+  if (!out || n_layers < 1 || !cin || !cout || !ksize) return fail(ctx, "cnn: bad arguments");
+  bool unit_sizes = true;     // no pooling, no upsampling
+  for (int l = 0; l < n_layers; l++) unit_sizes = unit_sizes && (!pool || pool[l] == 1) && (!up || up[l] == 1);
+  // 'yang' (lib/model.lua:228-239): osize {6, 6, 6, 1}, ksize {3, 1, 1, 1}
+  const bool yang = n_layers == 4 && unit_sizes && cout[0] == 6 && cout[1] == 6 && cout[2] == 6 && cout[3] == 1 &&
+                    ksize[0] == 3 && ksize[1] == 1 && ksize[2] == 1 && ksize[3] == 1;
+  if (yang && !in.p_div) return fail(ctx, "ERROR: yang model must have pDiv input");
+  if (yang && !in.div) return fail(ctx, "ERROR: yang model must have div input");
+  if (yang && in.u_div) return fail(ctx, "ERROR: yang model must not have UDiv input");
+  if (in.pressure_skip && (n_layers < 2 || ksize[n_layers - 1] != 1 || (up && up[n_layers - 1] != 1)))
+    return fail(ctx, "cnn: addPressureSkip joins pDiv to the hidden layer before the last convolution at full "
+                     "resolution, which needs a 1x1 last convolution without upsampling (lib/model.lua:357-361; "
+                     "not 'tog')");
+  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, &in,
+                            weights, biases, out);
+}
+
+static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                              int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                              const float* const* weights, const float* const* biases, tfl_cnn** out) {
   if (banks) {     // the assertions of lib/model.lua:246-252 (checked whatever banksNum is)
     if (banks->num < 1) return fail(ctx, "cnn: banksNum >= 1 failed (got %d)", banks->num);
     if (!(banks->split_stage < banks->join_stage))
@@ -284,14 +343,18 @@ int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* 
     if (banks->num == 1) banks = nullptr;
   }
   return cnn_create_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                         weights, biases, out);
+                         inputs, weights, biases, out);
 }
 
 static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
-                           const float* const* biases, tfl_cnn** out) {
+                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                           const float* const* weights, const float* const* biases, tfl_cnn** out) {
   if (!out || n_layers < 1) return fail(ctx, "cnn: bad arguments");
+  const tfl_cnn_inputs& in = *inputs;
+  const int in_sel = (in.p_div ? kCnnInPDiv : 0) | (in.u_div ? kCnnInUDiv : 0) | (in.div ? kCnnInDiv : 0);
+  const int in_ch = (in.p_div ? 1 : 0) + (in.u_div ? (is_3d ? 3 : 2) : 0) + (in.div ? 1 : 0) + 1;
+  const bool skip = in.pressure_skip != 0;
   const int nbanks = banks ? banks->num : 1;
   const int bsplit = banks ? banks->split_stage - 1 : 0, bjoin = banks ? banks->join_stage - 1 : 0;
   auto convs_of = [&](int l) { return (nbanks > 1 && l >= bsplit && l < bjoin) ? nbanks : 1; };
@@ -308,9 +371,31 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   }
   const int32_t* cout = cout_conv.data();
   if (cout_logical[n_layers - 1] != 1) return fail(ctx, "Last layer osize must be 1 (pressure)");   // model.lua:244
-  if (cin[0] != 3) return fail(ctx, "cnn: the first layer must take 3 channels (pDiv, div, occupancy)");
+  if (in_sel == (kCnnInPDiv | kCnnInDiv) && cin[0] != 3)
+    return fail(ctx, "cnn: the first layer must take 3 channels (pDiv, div, occupancy)");
+  if (cin[0] != in_ch)
+    return fail(ctx, "cnn: the input block has %d channels (pDiv, UDiv, div, occupancy as selected), the first layer "
+                     "takes %d", in_ch, cin[0]);
+  // The last convolution's channels without the pressure skip's pDiv (its last input channel, lib/model.lua:357-361).
+  std::vector<int32_t> cin_net(cin, cin + n_layers);
+  if (skip) {
+    if (cin[n_layers - 1] != cout_logical[n_layers - 2] + 1)
+      return fail(ctx, "cnn: with addPressureSkip the last convolution takes cout[%d] + 1 = %d channels (got %d)",
+                  n_layers - 2, cout_logical[n_layers - 2] + 1, cin[n_layers - 1]);
+    cin_net[n_layers - 1] -= 1;
+  }
+  cin = cin_net.data();
   if (nbanks > 1) plain = false;
   tfl_cnn* m = new tfl_cnn();
+  m->in_sel = in_sel;
+  m->in_ch = in_ch;
+  m->norm_func = in.normalize ? (in.norm_func == 1 ? kCnnScaleNorm : kCnnScaleStd) : kCnnScaleOne;
+  m->norm_chan = in.norm_chan == 1 ? kCnnStatPDiv : (in.norm_chan == 2 ? kCnnStatDiv : kCnnStatU);
+  if (!in.normalize) m->norm_chan = kCnnStatU;
+  m->skip = skip;
+  m->default_inputs = in_sel == (kCnnInPDiv | kCnnInDiv) && m->norm_func == kCnnScaleStd && m->norm_chan == kCnnStatU &&
+                      !skip;
+  m->tc_planes = (in_sel & kCnnInUDiv) ? 2 : 1;
   m->plain = plain;
   m->pool_is_max = pool_is_max ? 1 : 0;
   m->nonlin = nonlin_sigmoid ? 2 : 1;
@@ -338,6 +423,8 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
     const int kz = is_3d ? ksize[l] : 1;
     const int taps = kz * ksize[l] * ksize[l];
     for (int bk = 0; bk < convs_of(l); bk++, wi++) {
+      // the skip's layer is 1x1 with one output: its hidden channels' weights come first, pDiv's last
+      if (skip && l == n_layers - 1) m->w_skip = weights[wi][cin[l]];
       const std::vector<float> relaid = relayout_conv_weights(weights[wi], cin[l], cout[l], taps);
       float *dw = nullptr, *db = nullptr;
       if (cudaMalloc((void**)&dw, relaid.size() * 4) != cudaSuccess ||
@@ -351,7 +438,7 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   }
   {   // largest activation of the graph, in channels x cells-of-the-input-grid
     double rel = 1.0;
-    m->max_rel = 3.0;
+    m->max_rel = in_ch;      // the network input (pooled into the banks at stage 1)
     for (int l = 0; l < n_layers; l++) {
       if (nbanks > 1 && l == bjoin) m->max_rel = std::max(m->max_rel, rel * cin[l]);   // the joined banks
       m->max_rel = std::max(m->max_rel, rel * cout[l]);                          // convolution output
@@ -365,18 +452,21 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   }
   // Tensor-core eligibility: the 3-D 'default' graph (lib/model.lua:219-226), single-bank or with banks split
   // before stage 1 and joined before stage 3.
-  static const int want[5][3] = {{3, 8, 3}, {8, 8, 3}, {8, 8, 3}, {8, 8, 1}, {8, 1, 1}};
+  static const int want[5][3] = {{0, 8, 3}, {8, 8, 3}, {8, 8, 3}, {8, 8, 1}, {8, 1, 1}};   // cin[0]: any input set
   m->tc_ok = is_3d && n_layers == 5 && !nonlin_sigmoid &&
              (nbanks == 1 || (bsplit == 0 && bjoin == 2 && nbanks <= kTcMaxBanks));
   for (int l = 0; m->tc_ok && l < 5; l++) {
-    const int want_cin = (l == 2 && !m->bank_add) ? 8 * nbanks : want[l][0];
+    const int want_cin = l == 0 ? in_ch : (l == 2 && !m->bank_add) ? 8 * nbanks : want[l][0];
     m->tc_ok = m->pool[l] == 1 && m->up[l] == 1 && cin[l] == want_cin && cout[l] == want[l][1] && ksize[l] == want[l][2];
   }
   if (m->tc_ok) {
     const int j0 = m->conv0[2], nj = m->bank_add ? 1 : nbanks;
     for (int split = 0; split < 2; split++) {
       for (int i = 0; i < nbanks; i++) {                 // layers 1 and 2 of bank i
-        m->wBk[split].push_back(upload_tc_weights(weights[m->conv0[0] + i], 3, split));
+        // layer 1: the input set on one float4 plane, or (with UDiv) on two with zero weights past in_ch
+        m->wBk[split].push_back(m->tc_planes == 1 ? upload_tc_weights(weights[m->conv0[0] + i], in_ch, split)
+                                                  : upload_tc_weights(pad_cin8(weights[m->conv0[0] + i], in_ch).data(),
+                                                                      8, split));
         m->wBk[split].push_back(upload_tc_weights(weights[m->conv0[1] + i], 8, split));
       }
       for (int i = 0; i < nj; i++)
@@ -563,9 +653,8 @@ static int debug_join_impl(tfl_ctx* ctx, const float* const* banks, int nbanks, 
 // tfl_debug_tc_pyramid: one level of the bank pyramid on caller-owned padded buffers: in is
 // make_conv_tc_geo(nb, nz_in, ny, nx), out make_conv_tc_geo(nb, nz_out, ny / 2, nx / 2); out's planes [z_lo, z_hi)
 // pool in's planes 2 z + z_phase, 2 z + z_phase + 1.  Synchronises before returning.
-int tfl_debug_tc_pyramid(tfl_ctx* ctx, const float* in, float* out, int nb, int nz_in, int ny, int nx, int nz_out,
-                         int z_phase, int z_lo, int z_hi) {
-  DeviceGuard guard_(ctx);
+static int debug_tc_pyramid_impl(tfl_ctx* ctx, const float* in, float* out, int nb, int nz_in, int ny, int nx,
+                                 int nz_out, int z_phase, int z_lo, int z_hi, int planes) {
   if (!ctx) return 1;
   if (!in || !out) return fail(ctx, "debug_tc_pyramid: nil argument");
   if (nb < 1 || ny < 2 || nx < 2 || ny % 2 || nx % 2 || (z_phase != 0 && z_phase != 1) || z_lo < 0 || z_hi > nz_out ||
@@ -574,10 +663,43 @@ int tfl_debug_tc_pyramid(tfl_ctx* ctx, const float* in, float* out, int nb, int 
   ConvTcGeo go = make_conv_tc_geo(nb, nz_out, ny / 2, nx / 2);
   go.z_lo = z_lo;
   go.z_hi = z_hi;
-  launch_tc_pyramid(in, make_conv_tc_geo(nb, nz_in, ny, nx), out, go, z_phase, ctx->stream);
+  launch_tc_pyramid(in, make_conv_tc_geo(nb, nz_in, ny, nx), out, go, z_phase, ctx->stream, planes);
   if (check_launch(ctx, "debug_tc_pyramid")) return 1;
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   return 0;
+}
+int tfl_debug_tc_pyramid(tfl_ctx* ctx, const float* in, float* out, int nb, int nz_in, int ny, int nx, int nz_out,
+                         int z_phase, int z_lo, int z_hi) {
+  DeviceGuard guard_(ctx);
+  return debug_tc_pyramid_impl(ctx, in, out, nb, nz_in, ny, nx, nz_out, z_phase, z_lo, z_hi, 1);
+}
+// tfl_debug_tc_pyramid2: the same level on both float4 planes (the input of a set with UDiv), all four channels of
+// each pooled.
+int tfl_debug_tc_pyramid2(tfl_ctx* ctx, const float* in, float* out, int nb, int nz_in, int ny, int nx, int nz_out,
+                          int z_phase, int z_lo, int z_hi) {
+  DeviceGuard guard_(ctx);
+  return debug_tc_pyramid_impl(ctx, in, out, nb, nz_in, ny, nx, nz_out, z_phase, z_lo, z_hi, 2);
+}
+
+// tfl_debug_cnn_inputs_padded: the model's tensor-core input (launch_cnn_inputs_padded with its channel set and
+// planes) from caller-owned device p_div [nb][n], U1 [nb][3][n] (already wall-masked), flags [nb][n] and the host
+// scale [nb], into out (make_conv_tc_geo(nb, nz, ny, nx) layout).  Synchronises before returning.
+int tfl_debug_cnn_inputs_padded(tfl_ctx* ctx, const tfl_cnn* m, const float* p_div, const float* U1,
+                                const float* flags, const float* scale_host, float* out, int nb, int nz, int ny,
+                                int nx) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (!m || !p_div || !U1 || !flags || !scale_host || !out) return fail(ctx, "debug_cnn_inputs_padded: nil argument");
+  if (!m->is3d || bad_grid(nb, nz, ny, nx, 1)) return fail(ctx, "debug_cnn_inputs_padded: bad grid or 2-D model");
+  float* scale = nullptr;
+  TFL_CUDA(ctx, cudaMalloc((void**)&scale, 4 * nb));
+  cudaMemcpy(scale, scale_host, 4 * nb, cudaMemcpyHostToDevice);
+  const ConvTcGeo tg = make_conv_tc_geo(nb, nz, ny, nx);
+  launch_cnn_inputs_padded(p_div, U1, flags, scale, out, tg.px, tg.py, whole_grid(ctx, nb, nz, ny, nx, 1),
+                           ctx->stream, m->in_sel, m->tc_planes);
+  const int rc = finish_debug(ctx, "debug_cnn_inputs_padded");
+  cudaFree(scale);
+  return rc;
 }
 
 // Undocumented test hooks (not in tfl.h): the fp32 path's kernels (tfl_cnn.cu) on caller-owned device buffers, on
@@ -691,32 +813,41 @@ static size_t cnn_bank_buf_bytes(const tfl_cnn* m, const Geo& g, int i) {
 static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const float* U_div,
                             const float* flags, float* p_out, float* U_out, float threshold, const Geo& g,
                             char* scratch, float** scale_dev_out) {
-  // scratch layout (caller reserved): U1 [nc], x0 [3], actA [max_c], actB [max_c], scale [nb]
+  // scratch layout (caller reserved): U1 [nc], x0 [cin[0]], actA [max_c], actB [max_c], scale [nb]
   const size_t cells = (size_t)g.n * g.nb;
   size_t off = 0;
   auto take = [&](size_t bytes) { char* p = scratch + off; off = (off + bytes + 255) & ~(size_t)255; return p; };
   float* U1 = (float*)take(cells * 4 * g.nc);
-  float* x0 = (float*)take(cells * 4 * 3);
+  float* x0 = (float*)take(cells * 4 * m->in_ch);
   float* actA = (float*)take(cells * 4 * m->max_c);      // max_c covers max_rel (set at creation)
   float* actB = (float*)take(cells * 4 * m->max_c);
   float* scale = (float*)take(sizeof(float) * g.nb);
   double* sums = ctx->dscratch + 64;
   cudaStream_t st = ctx->stream;
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
-  launch_cnn_mask_stats(U_div, flags, U1, sums, g.zlo, g.zhi, g, st);
-  launch_cnn_scale(sums, scale, g.nb, (long long)g.nc * g.n, threshold, st);
+  launch_cnn_mask_stats(U_div, flags, U1, sums, g.zlo, g.zhi, g, st, m->norm_chan, p_div);
+  if (m->norm_chan == kCnnStatDiv) {
+    launch_cnn_div_stats(U1, flags, sums, g.zlo, g.zhi, g, st);
+    ctx->launches += 1;
+  }
+  launch_cnn_scale(sums, scale, g.nb, m->norm_chan == kCnnStatU ? (long long)g.nc * g.n : g.n, threshold, st,
+                   m->norm_func);
   if (m->mode > 0 && m->tc_ok && !ctx->slab) {
     if (cnn_ensure_act(ctx, m, g)) return 1;
     const ConvTcGeo& tg = m->act_geo;
-    launch_cnn_inputs_padded(p_div, U1, flags, scale, m->act[0], tg.px, tg.py, g, st);
+    launch_cnn_inputs_padded(p_div, U1, flags, scale, m->act[0], tg.px, tg.py, g, st, m->in_sel, m->tc_planes);
     float* p_net = actA;      // plain [b][z][y][x]
     run_conv_stack(m, p_net, st);
+    if (m->skip) {
+      launch_cnn_skip(p_net, p_div, scale, m->w_skip, g, st);
+      ctx->launches += 1;
+    }
     launch_cnn_finish(p_net, U1, flags, scale, p_out, U_out, g, st);
     ctx->launches += 7;
     if (scale_dev_out) *scale_dev_out = scale;
     return check_launch(ctx, "cnn_project (tensor cores)");
   }
-  launch_cnn_inputs(p_div, U1, flags, scale, x0, g, st);
+  launch_cnn_inputs(p_div, U1, flags, scale, x0, g, st, m->in_sel);
   ctx->launches += 3;
   const float* in = x0;
   if (m->plain) {
@@ -851,6 +982,10 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
     }
     if (gl.nx != g.nx || gl.ny != g.ny || gl.nz != g.nz) return fail(ctx, "cnn: graph does not return to the input resolution");
   }
+  if (m->skip) {
+    launch_cnn_skip((float*)in, p_div, scale, m->w_skip, g, st);     // `in` is one of this call's scratch buffers
+    ctx->launches += 1;
+  }
   launch_cnn_finish(in, U1, flags, scale, p_out, U_out, g, st);
   ctx->launches += 1;
   if (scale_dev_out) *scale_dev_out = scale;
@@ -859,7 +994,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
 
 static size_t cnn_scratch_bytes(const tfl_cnn* m, const Geo& g) {
   const size_t cells = (size_t)g.n * g.nb;
-  size_t bytes = cells * 4 * (g.nc + 3 + 2 * (size_t)m->max_c) + 4 * g.nb + 8 * 256;
+  size_t bytes = cells * 4 * (g.nc + m->in_ch + 2 * (size_t)m->max_c) + 4 * g.nb + 8 * 256;
   if (!m->plain) bytes += (size_t)((double)cells * m->max_rel + 64) * 4 + 256;     // third rotating buffer
   for (int i = 1; i < m->nbanks; i++) bytes += 3 * (cnn_bank_buf_bytes(m, g, i) + 256);
   return bytes;
@@ -925,6 +1060,7 @@ int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!m) return fail(ctx, "cnn is nil");
+  if (!m->default_inputs) return fail(ctx, "cnn_project_from_sums: %s", kSlabDefaultInputs);
   if (!m->tc_ok || m->mode == 0) return fail(ctx, "cnn_project_from_sums: %s", kSlabTcOnly);
   if (!dev_sums) return fail(ctx, "cnn_project_from_sums: nil sums");
   if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, p_div, "pDiv") || check_vel(ctx, U1, flags) ||

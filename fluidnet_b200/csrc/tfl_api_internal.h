@@ -94,6 +94,15 @@ struct tfl_cnn {
   int nonlin = 1;            // 1 ReLU, 2 sigmoid (activation codes of tfl_cnn.cu)
   bool plain = true;
   double max_rel = 0.0;      // largest channels x (cells relative to the input grid) of any stage
+  // input block (tfl_cnn_inputs): in_sel the kCnnIn* channels, in_ch = cin[0]; norm_func a kCnnScale* code (kCnnScaleOne
+  // when normalizeInput is off), norm_chan the kCnnStat* field.  With the pressure skip the last convolution keeps
+  // its hidden channels and w_skip, its pDiv weight, is added by launch_cnn_skip.
+  int in_sel = kCnnInPDiv | kCnnInDiv, in_ch = 3;
+  int norm_func = kCnnScaleStd, norm_chan = kCnnStatU;
+  bool skip = false;
+  float w_skip = 0.0f;
+  bool default_inputs = true;
+  int tc_planes = 1;         // float4 planes of the tensor-core input (2 when UDiv is an input)
   // tensor-core path (3-D 'default' architecture, single-bank or with banks split at stage 1 and joined at stage 3)
   int mode = 0;              // 0 fp32 FMA, 1 TF32 tensor cores, 2 3xTF32 tensor cores
   bool tc_ok = false;

@@ -730,26 +730,29 @@ void launch_z(const float4* in, float4* out, float* p_net, const float* wB, cons
 }
 
 // 2x2x2 average of the first float4 plane (k_pool's summation order), zero fourth channel; output planes
-// [go.z_lo, go.z_hi), input planes shifted by z_phase.
+// [go.z_lo, go.z_hi), input planes shifted by z_phase.  planes = 2: both float4 planes, all four channels each.
 __global__ void k_tc_pyramid(const float4* __restrict__ in, ConvTcGeo gi, float4* __restrict__ out, ConvTcGeo go,
-                             int z_phase, long long total) {
+                             int z_phase, int planes, long long total) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= total) return;
   const int nzr = go.z_hi - go.z_lo;
   const int x = (int)(t % go.nx), y = (int)((t / go.nx) % go.ny);
   const int z = go.z_lo + (int)((t / ((long long)go.nx * go.ny)) % nzr);
   const long long b = t / ((long long)go.nx * go.ny * nzr);
-  const float4* ib = in + b * 2 * (long long)(gi.nz + 2) * gi.py * gi.px;
-  float sx = 0.0f, sy = 0.0f, sz = 0.0f;
-  for (int dz = 0; dz < 2; dz++)
-    for (int dy = 0; dy < 2; dy++)
-      for (int dx = 0; dx < 2; dx++) {
-        const float4 v =
-            __ldg(ib + ((long long)(2 * z + z_phase + dz + 1) * gi.py + (2 * y + dy + 1)) * gi.px + (2 * x + dx + 1));
-        sx += v.x; sy += v.y; sz += v.z;
-      }
-  out[b * 2 * (long long)(go.nz + 2) * go.py * go.px + ((long long)(z + 1) * go.py + (y + 1)) * go.px + (x + 1)] =
-      make_float4(sx / 8.0f, sy / 8.0f, sz / 8.0f, 0.0f);
+  const long long iplane = (long long)(gi.nz + 2) * gi.py * gi.px, oplane = (long long)(go.nz + 2) * go.py * go.px;
+  for (int q = 0; q < planes; q++) {
+    const float4* ib = in + (b * 2 + q) * iplane;
+    float sx = 0.0f, sy = 0.0f, sz = 0.0f, sw = 0.0f;
+    for (int dz = 0; dz < 2; dz++)
+      for (int dy = 0; dy < 2; dy++)
+        for (int dx = 0; dx < 2; dx++) {
+          const float4 v =
+              __ldg(ib + ((long long)(2 * z + z_phase + dz + 1) * gi.py + (2 * y + dy + 1)) * gi.px + (2 * x + dx + 1));
+          sx += v.x; sy += v.y; sz += v.z; sw += v.w;
+        }
+    out[(b * 2 + q) * oplane + ((long long)(z + 1) * go.py + (y + 1)) * go.px + (x + 1)] =
+        make_float4(sx / 8.0f, sy / 8.0f, sz / 8.0f, planes == 2 ? sw / 8.0f : 0.0f);
+  }
 }
 
 }  // namespace
@@ -815,11 +818,11 @@ int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, co
 }
 
 void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, int z_phase,
-                       cudaStream_t st) {
+                       cudaStream_t st, int planes) {
   const long long total = (long long)gout.nb * (gout.z_hi - gout.z_lo) * gout.ny * gout.nx;
   if (total <= 0) return;
   k_tc_pyramid<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float4*)in, gin, (float4*)out, gout, z_phase,
-                                                                 total);
+                                                                 planes, total);
 }
 
 int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, const float* bias,

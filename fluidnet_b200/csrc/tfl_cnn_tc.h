@@ -48,7 +48,8 @@ int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, co
 // 2 z + z_phase + 1 (interior, first float4 plane only: the 3 input channels and a zero fourth), for the output
 // planes [gout.z_lo, gout.z_hi).  z_phase (0 or 1) aligns the pooling to the global grid on a z-slab whose
 // fine level starts at an odd global plane.  Other planes and the borders of out are left as they are.
+// planes = 2 (the input of a set with UDiv): both float4 planes, all four channels of each.
 void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, int z_phase,
-                       cudaStream_t st);
+                       cudaStream_t st, int planes = 1);
 
 }  // namespace tfl

@@ -71,14 +71,29 @@ void launch_apply_bc(float* x, const float* inv, const float* bc, long long n, c
 void launch_clamp(float* x, float lo, float hi, long long n, cudaStream_t st);
 
 // CNN pre/post stages (exact float semantics of lib/model.lua's non-conv nodes).
+// The input block (tfl_cnn_inputs): channel set bits, the field the scale is computed from, the scale function.
+enum : int { kCnnInPDiv = 1, kCnnInUDiv = 2, kCnnInDiv = 4 };
+enum : int { kCnnStatU = 0, kCnnStatPDiv = 1, kCnnStatDiv = 2 };
+enum : int { kCnnScaleStd = 0, kCnnScaleNorm = 1, kCnnScaleOne = 2 };
+// U1 = wall mask * U; sums[b] += (sum f, sum f^2) over the planes [own_lo, own_hi) of f = U1 (stat kCnnStatU) or
+// p_div (kCnnStatPDiv); kCnnStatDiv accumulates nothing here (launch_cnn_div_stats, once U1 is complete).
 void launch_cnn_mask_stats(const float* U, const float* flags, float* U1, double* sums, int own_lo, int own_hi,
-                           const Geo& g, cudaStream_t st);
+                           const Geo& g, cudaStream_t st, int stat = kCnnStatU, const float* p_div = nullptr);
+void launch_cnn_div_stats(const float* U1, const float* flags, double* sums, int own_lo, int own_hi, const Geo& g,
+                          cudaStream_t st);
+// n_per_batch: the sample count of the field (std only).
 void launch_cnn_scale(const double* sums, float* scale, int nb, long long n_per_batch, float threshold,
-                      cudaStream_t st);
+                      cudaStream_t st, int func = kCnnScaleStd);
+// x0 [nb][cin][n]: the channels of `sel` in the order pDiv, UDiv, div, occupancy, scaled.
 void launch_cnn_inputs(const float* p_div, const float* U1, const float* flags, const float* scale,
-                       float* x0, const Geo& g, cudaStream_t st);
+                       float* x0, const Geo& g, cudaStream_t st, int sel = kCnnInPDiv | kCnnInDiv);
+// The same channels in the padded channels-last layout of tfl_cnn_tc.cu, on the first float4 plane (planes = 1,
+// up to 3 channels and a zero fourth) or on both (planes = 2, zero-padded to 8 channels).
 void launch_cnn_inputs_padded(const float* p_div, const float* U1, const float* flags, const float* scale,
-                              float* x0, int px, int py, const Geo& g, cudaStream_t st);
+                              float* x0, int px, int py, const Geo& g, cudaStream_t st,
+                              int sel = kCnnInPDiv | kCnnInDiv, int planes = 1);
+// addPressureSkip with a 1x1 last convolution: p_net += w_skip * (p_div / scale).
+void launch_cnn_skip(float* p_net, const float* p_div, const float* scale, float w_skip, const Geo& g, cudaStream_t st);
 void launch_cnn_finish(const float* p_net, const float* U1, const float* flags, const float* scale,
                        float* p_out, float* U_out, const Geo& g, cudaStream_t st);
 

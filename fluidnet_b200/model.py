@@ -1,8 +1,8 @@
 """Pressure-projection model (forward only) -- mirror of torch/lib/model.lua.
 
 `ProjectionModel` plays the role of the nngraph module built by torch.defineModelGraph
-(lib/model.lua:27-401) for the 'default' input set {pDiv, div, flags}: `forward({pDiv, UDiv,
-flags})` returns `{p, U}` (lib/model.lua:421-450).  The whole graph runs inside libtfl.so
+(lib/model.lua:27-401), input block included (inputChannels, normalizeInput*, addPressureSkip):
+`forward({pDiv, UDiv, flags})` returns `{p, U}` (lib/model.lua:421-450).  The whole graph runs inside libtfl.so
 (tfl_cnn_project); weights are plain float32 arrays in Torch layout [cout][cin][kz][ky][kx].
 """
 import ctypes as C
@@ -14,6 +14,18 @@ from . import _lib, tfluids
 from ._lib import TflError
 
 
+DEFAULT_INPUTS = {"pDiv": True, "UDiv": False, "div": True, "flags": True}
+NORM_FUNCS = {"std": 0, "norm": 1}
+NORM_CHANS = {"UDiv": 0, "pDiv": 1, "div": 2}
+
+
+def input_channel_count(inputChannels, is3D):
+    """cin[0] of the network for an inputChannels table (lib/model.lua:28-46): pDiv, UDiv (2 or 3), div, flags."""
+    ch = dict(DEFAULT_INPUTS, **(inputChannels or {}))
+    return (1 if ch["pDiv"] else 0) + ((3 if is3D else 2) if ch["UDiv"] else 0) + (1 if ch["div"] else 0) + \
+        (1 if ch["flags"] else 0)
+
+
 def default_layers(is3D):
     """(cin, cout, k) of the 'default' modelType (lib/model.lua:179-186 2-D, :219-226 3-D)."""
     if is3D:
@@ -23,14 +35,28 @@ def default_layers(is3D):
 
 class ProjectionModel:
     def __init__(self, layers, is3D, device=None, normalizeInputThreshold=1e-5, pool=None, up=None,
-                 poolType="avg", nonlinType="relu", banks=None):
+                 poolType="avg", nonlinType="relu", banks=None, inputChannels=None, normalizeInput=True,
+                 normalizeInputFunc="std", normalizeInputChan="UDiv", addPressureSkip=False):
         """layers: [(weight ndarray [cout * up^d][cin][kz][ky][kx], bias ndarray [cout * up^d]), ...]
         pool / up: per-layer pooling and ConvolutionUpsample sizes of the 'tog' graph (lib/model.lua:164-226),
         None = all 1 ('default', 'yang'); poolType 'avg' | 'max'; nonlinType 'relu' | 'sigmoid'.
         banks: multi-resolution banks (lib/model.lua:252-361), {"num": banksNum, "split_stage": banksSplitStage,
         "join_stage": banksJoinStage, "aggregate": 'concat' | 'add'} (stages numbered from 1); layers[l] of a
         banked stage (split_stage <= l + 1 < join_stage) is then a list of num (weight, bias) pairs, bank 1 first.
-        None: a single bank."""
+        None: a single bank.
+        inputChannels ({"pDiv", "UDiv", "div", "flags"} -> bool, missing keys at their defaults pDiv, div, flags),
+        normalizeInput, normalizeInputFunc ('std' | 'norm'), normalizeInputChan ('UDiv' | 'pDiv' | 'div') and
+        addPressureSkip are the mconf keys of lib/model.lua:27-150, :357-387; layers[0] takes the selected channels and
+        with the skip the last layer takes one more, pDiv.  The library refuses what the reference cannot build."""
+        ch = dict(DEFAULT_INPUTS, **(inputChannels or {}))
+        if not ch["flags"]:
+            raise TflError("Are you sure you dont want flags on input?")          # lib/model.lua:39-43
+        if normalizeInputFunc not in NORM_FUNCS:
+            raise TflError("Incorrect normalize input function")                  # :103
+        if normalizeInputChan not in NORM_CHANS:
+            raise TflError("Incorrect normalize input channel.")                  # :114
+        cin_ = _lib.CnnInputs(int(bool(ch["pDiv"])), int(bool(ch["UDiv"])), int(bool(ch["div"])), int(bool(normalizeInput)),
+                              NORM_FUNCS[normalizeInputFunc], NORM_CHANS[normalizeInputChan], int(bool(addPressureSkip)))
         self.is3D = bool(is3D)
         self.threshold = float(normalizeInputThreshold)
         self.ctx = tfluids.context(device)
@@ -80,12 +106,12 @@ class ProjectionModel:
         h = C.c_void_p()
         args = (self.ctx.h, 1 if is3D else 0, n, cin, cout, ks, cpool, cup, 1 if poolType == "max" else 0,
                 1 if nonlinType == "sigmoid" else 0)
-        if banks is None:
-            self.ctx.check(self.ctx.lib.tfl_cnn_create_graph(*args, wp, bp, C.byref(h)))
-        else:
+        cb = None
+        if banks is not None:
             cb = _lib.CnnBanks(int(banks["num"]), int(banks["split_stage"]), int(banks["join_stage"]),
                                1 if banks["aggregate"] == "add" else 0)
-            self.ctx.check(self.ctx.lib.tfl_cnn_create_banked(*args, C.byref(cb), wp, bp, C.byref(h)))
+        self.ctx.check(self.ctx.lib.tfl_cnn_create_model(*args, C.byref(cb) if cb is not None else None, C.byref(cin_),
+                                                         wp, bp, C.byref(h)))
         self.h = h
         self.last_scale = None
 
@@ -93,12 +119,12 @@ class ProjectionModel:
     def from_reference_file(cls, model_path, mconf_path=None, device=None):
         """A model saved by the reference (torch/lib/save_model.lua: Torch7 binary network + `_mconf.bin`),
         read without Torch7 (fluidnet_b200/torch7.py).  Returns (model, mconf).
-        The graph follows the mconf (modelType, nonlinType, poolType, the bank keys, normalizeInputThreshold), each
+        The graph follows the mconf (modelType, nonlinType, poolType, the bank keys, the input block), each
         convolution goes to the (bank, stage) of its nngraph annotation, and the shapes are checked against the
         architecture.  Options and modules the library does not compute raise ValueError naming them."""
         from . import torch7
         ref = torch7.load_reference_model(model_path, mconf_path)
-        opts = torch7.model_options(ref["mconf"])
+        opts = torch7.model_options(ref["mconf"], inputs=True)
         stages = torch7.graph_stages(ref["model"])
         torch7.check_stages(stages, ref["mconf"], opts)
         return cls(stages, ref["is3D"], device=device, **opts), ref["mconf"]

@@ -81,13 +81,15 @@ def make_density(flags, seed=1235):
     return np.ascontiguousarray(d)
 
 
-def make_model(is3d=True, seed=4321, model_type="default", banks=None):
+def make_model(is3d=True, seed=4321, model_type="default", banks=None, inputs=None):
     """Random-init weights of a reference architecture (torch/lib/model.lua:164-226: 'default', 'tog',
     'yang'), Torch `reset` convention uniform +-1/sqrt(fan_in).  Inputs: pDiv, div, occupancy
     (lib/default_conf.lua:76-81).  'tog' layers carry pooling / ConvolutionUpsample sizes: the weights of
     an upsampling layer have cout * up^d output channels.
     banks: {"num", "split_stage", "join_stage", "aggregate"} (lib/model.lua:252-361); a banked stage's entry
-    in "layers" is then a list of num (weight, bias) pairs, and a 'concat' join stage takes num x the channels."""
+    in "layers" is then a list of num (weight, bias) pairs, and a 'concat' join stage takes num x the channels.
+    inputs: the input-block keywords of model.ProjectionModel (inputChannels, normalizeInput*, addPressureSkip),
+    kept under "inputs"; the first layer takes the selected channels, the last one more with addPressureSkip."""
     rs = np.random.RandomState(seed)
     extra = {}
     if model_type == "default":
@@ -109,10 +111,14 @@ def make_model(is3d=True, seed=4321, model_type="default", banks=None):
         raise ValueError(model_type)
     nbanks = banks["num"] if banks is not None else 1
     layers = []
-    cin = 3
+    ch = {"pDiv": True, "UDiv": False, "div": True, "flags": True}
+    ch.update((inputs or {}).get("inputChannels") or {})
+    cin = int(ch["pDiv"]) + (3 if is3d else 2) * int(ch["UDiv"]) + int(ch["div"]) + int(ch["flags"])
     for stage, (cout, k, u) in enumerate(zip(osize, ksize, usize), start=1):
         if nbanks > 1 and stage == banks["join_stage"] and banks["aggregate"] == "concat":
             cin *= nbanks
+        if stage == len(osize) and (inputs or {}).get("addPressureSkip"):
+            cin += 1
         banked = nbanks > 1 and banks["split_stage"] <= stage < banks["join_stage"]
         kz = k if is3d else 1
         fan_in = cin * kz * k * k
@@ -129,4 +135,6 @@ def make_model(is3d=True, seed=4321, model_type="default", banks=None):
     out.update(extra)
     if banks is not None:
         out["banks"] = dict(banks)
+    if inputs is not None:
+        out["inputs"] = dict(inputs)
     return out

@@ -306,10 +306,64 @@ def graph_stages(model):
     return stages
 
 
-def model_options(mconf, n_stages=None):
+def input_options(mconf):
+    """The input block of a reference mconf (lib/model.lua:27-150, :357-387; defaults lib/default_conf.lua:45-47,
+    76-81, 103-106) as ProjectionModel keyword arguments.  Raises ValueError naming the key for every combination the
+    reference cannot build, with the reference's own message where it has one."""
+    def opt(key, default=None):
+        return mconf.get(key, default)
+
+    def bad(key, why):
+        raise ValueError("mconf: %s: %s" % (key, why))
+
+    chans = {"pDiv": False, "UDiv": False, "div": False, "flags": False}
+    given = opt("inputChannels") or {"pDiv": True, "div": True, "flags": True}
+    for k, v in given.items():
+        if k not in chans:
+            bad("inputChannels", "unknown channel %r" % k)
+        chans[k] = bool(v)
+    if not chans["flags"]:
+        bad("inputChannels", "Are you sure you dont want flags on input?")                      # model.lua:39-43
+    if not (chans["pDiv"] or chans["UDiv"] or chans["div"]):
+        bad("inputChannels", "Are you sure you dont want any (U, div or p) fields?")            # :50-52
+    if not (chans["UDiv"] or chans["div"]):
+        bad("inputChannels", "tfluids.VelocityUpdate needs UDiv, which is selected only when UDiv or div is an "
+                             "input (lib/model.lua:69-72, :380)")
+    normalize = opt("normalizeInput", True)
+    if normalize not in (True, False):
+        bad("normalizeInput", "%r is not a boolean" % (normalize,))
+    func = opt("normalizeInputFunc", "std")
+    chan = opt("normalizeInputChan", "UDiv")
+    if normalize:
+        if func not in ("std", "norm"):
+            bad("normalizeInputFunc", "Incorrect normalize input function (%r)" % (func,))       # :103
+        if chan not in ("UDiv", "pDiv", "div"):
+            bad("normalizeInputChan", "Incorrect normalize input channel. (%r)" % (chan,))       # :114
+        if chan == "div" and not chans["div"]:
+            bad("normalizeInputChan", "'div' needs inputChannels.div (lib/model.lua:108-116: div is nil)")
+    else:
+        func, chan = "std", "UDiv"      # unused without the scale node
+    model_type = opt("modelType", "default")
+    if model_type == "yang":                                                                     # model_utils.lua:211-227
+        if not chans["pDiv"]:
+            bad("inputChannels", "ERROR: yang model must have pDiv input")
+        if not chans["div"]:
+            bad("inputChannels", "ERROR: yang model must have div input")
+        if chans["UDiv"]:
+            bad("inputChannels", "ERROR: yang model must not have UDiv input")
+    skip = bool(opt("addPressureSkip", False))
+    if skip and model_type == "tog":
+        bad("addPressureSkip", "'tog' joins pDiv to a half-resolution hidden layer before its upsampling last "
+                               "convolution, which lib/model.lua:357-361 cannot build")
+    return {"inputChannels": chans, "normalizeInput": bool(normalize), "normalizeInputFunc": func,
+            "normalizeInputChan": chan, "addPressureSkip": skip}
+
+
+def model_options(mconf, n_stages=None, inputs=False):
     """ProjectionModel keyword arguments for a reference mconf (lib/default_conf.lua, lib/model.lua:27-401):
-    pool / up from modelType, poolType, nonlinType, banks, normalizeInputThreshold.  Raises ValueError, naming
-    the option, for anything the library does not compute."""
+    pool / up from modelType, poolType, nonlinType, banks, normalizeInputThreshold, and with inputs=True the input
+    block (input_options).  Raises ValueError, naming the option, for anything the library does not compute.  Without
+    inputs=True a non-default input block is refused too: a caller that drops those keys would build another model."""
     def opt(key, default=None):
         return mconf.get(key, default)
 
@@ -318,18 +372,21 @@ def model_options(mconf, n_stages=None):
 
     if opt("addBatchNorm"):
         refuse("addBatchNorm = true")
-    if opt("addPressureSkip"):
-        refuse("addPressureSkip = true")
-    chans = opt("inputChannels") or {"pDiv": True, "div": True, "flags": True}
-    on = sorted(k for k, v in chans.items() if v)
-    if on != ["div", "flags", "pDiv"]:
-        refuse("inputChannels = {%s} (only pDiv, div, flags)" % ", ".join(on))
-    if opt("normalizeInput", True) is not True:
-        refuse("normalizeInput = false")
-    if opt("normalizeInputFunc", "std") != "std":
-        refuse("normalizeInputFunc = %r" % opt("normalizeInputFunc"))
-    if opt("normalizeInputChan", "UDiv") != "UDiv":
-        refuse("normalizeInputChan = %r" % opt("normalizeInputChan"))
+    if not inputs:
+        if opt("addPressureSkip"):
+            refuse("addPressureSkip = true (model_options(mconf, inputs=True) builds it)")
+        chans = opt("inputChannels") or {"pDiv": True, "div": True, "flags": True}
+        on = sorted(k for k, v in chans.items() if v)
+        if on != ["div", "flags", "pDiv"]:
+            refuse("inputChannels = {%s} (only pDiv, div, flags; model_options(mconf, inputs=True) builds the others)"
+                   % ", ".join(on))
+        if opt("normalizeInput", True) is not True:
+            refuse("normalizeInput = false (model_options(mconf, inputs=True) builds it)")
+        if opt("normalizeInputFunc", "std") != "std":
+            refuse("normalizeInputFunc = %r (model_options(mconf, inputs=True) builds 'norm')" % opt("normalizeInputFunc"))
+        if opt("normalizeInputChan", "UDiv") != "UDiv":
+            refuse("normalizeInputChan = %r (model_options(mconf, inputs=True) builds 'pDiv', 'div')"
+                   % opt("normalizeInputChan"))
     nonlin = opt("nonlinType", "relu")
     if nonlin not in ("relu", "sigmoid"):
         refuse("nonlinType = %r" % nonlin)
@@ -353,17 +410,22 @@ def model_options(mconf, n_stages=None):
             refuse("banksAggregateMethod = %r" % agg)
         out["banks"] = {"num": num, "split_stage": int(opt("banksSplitStage", 1)),
                         "join_stage": int(opt("banksJoinStage", 3)), "aggregate": agg}
+    if inputs:
+        out.update(input_options(mconf))
     return out
 
 
 def check_stages(stages, mconf, options):
-    """The file's convolutions against the architecture the mconf describes (lib/model.lua:163-361)."""
+    """The file's convolutions against the architecture the mconf describes (lib/model.lua:163-361), the first taking
+    the mconf's input channels and the last one more with addPressureSkip."""
     is3d = bool(mconf.get("is3D"))
     osize, ksize, _, usize = _ARCH[(is3d, mconf.get("modelType", "default"))]
     if len(stages) != len(osize):
         raise ValueError("torch7 model: %d stages, modelType %r has %d" % (len(stages), mconf.get("modelType"), len(osize)))
     bk = options.get("banks")
-    cin = 3
+    ins = input_options(mconf)
+    ch = ins["inputChannels"]
+    cin = int(ch["pDiv"]) + (3 if is3d else 2) * int(ch["UDiv"]) + int(ch["div"]) + int(ch["flags"])
     for s, layer in enumerate(stages, start=1):
         convs = layer if isinstance(layer, list) else [layer]
         banked = bk is not None and bk["split_stage"] <= s < bk["join_stage"]
@@ -372,6 +434,8 @@ def check_stages(stages, mconf, options):
                              (s, len(convs), bk["num"] if banked else 1))
         if bk is not None and s == bk["join_stage"] and bk["aggregate"] == "concat":
             cin *= bk["num"]
+        if s == len(osize) and ins["addPressureSkip"]:
+            cin += 1                    # lib/model.lua:357-361: [hidden, pDiv]
         want = (osize[s - 1] * usize[s - 1] ** (3 if is3d else 2), cin, ksize[s - 1])
         for w, _ in convs:
             if (w.shape[0], w.shape[1], w.shape[4]) != want:

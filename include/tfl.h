@@ -191,7 +191,8 @@ int tfl_clamp(tfl_ctx* ctx, const tfl_grid* x, float lo, float hi);
  * cubic (3-D) or square (2-D) kernel of edge ksize[l], bias, and ReLU after every layer
  * but the last.  weights[l] is a HOST pointer to [cout][cin][kz][ky][kx] floats (Torch
  * layout, kz == 1 in 2-D); biases[l] to [cout].  cin[0] must be 3 (pDiv, div, occupancy:
- * the 'default' input set, lib/default_conf.lua:76-81) and cout[last] must be 1. */
+ * the 'default' input set, lib/default_conf.lua:76-81; other sets: tfl_cnn_create_model) and cout[last]
+ * must be 1. */
 int tfl_cnn_create(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                    const int32_t* ksize, const float* const* weights, const float* const* biases,
                    tfl_cnn** out);
@@ -224,6 +225,31 @@ int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* 
                           const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
                           const float* const* biases, tfl_cnn** out);
+/* The network's input block (lib/model.lua:27-150, :357-387; defaults lib/default_conf.lua:45-47, 76-81, 103-106).
+ * p_div, u_div, div: inputChannels.{pDiv, UDiv, div}; the network input joins, in this order, pDiv, UDiv (2 or 3
+ * channels, after the wall mask), div and the occupancy of the flags, which are always an input.  normalize:
+ * normalizeInput; norm_func: normalizeInputFunc 0 'std' (unbiased) or 1 'norm' (L2); norm_chan: normalizeInputChan
+ * 0 'UDiv', 1 'pDiv' or 2 'div', the field the per-entry scale max(f(field), threshold) is computed from.
+ * pressure_skip: addPressureSkip, the last (1x1) convolution also takes the scaled pDiv (cin[last] = cout[last-1]
+ * + 1, pDiv its last input channel).  Defaults: {1, 0, 1, 1, 0, 0, 0}. */
+typedef struct tfl_cnn_inputs {
+  int32_t p_div, u_div, div;
+  int32_t normalize;
+  int32_t norm_func;              /* 0 std, 1 norm */
+  int32_t norm_chan;              /* 0 UDiv, 1 pDiv, 2 div */
+  int32_t pressure_skip;
+} tfl_cnn_inputs;
+/* tfl_cnn_create_banked with the input block `inputs` (NULL: the defaults, exactly tfl_cnn_create_banked).
+ * cin[0] must be the channel count of the set.  Combinations the reference cannot build are refused: no pDiv,
+ * UDiv or div; neither UDiv nor div (the velocity update needs UDiv); normalizeInputChan 'div' without the div
+ * input; 'yang' with another set than pDiv, div; the skip on a graph whose last convolution is not 1x1 ('tog').
+ * Any set runs on the fp32 path and, for the 3-D 'default' graph (single-bank or banks split 1 / join 3), on the
+ * tensor cores; models with a non-default block run whole grids only (no z-slabs) and step through the
+ * per-operator path of tfl_simulate_step. */
+int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                         const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                         int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                         const float* const* weights, const float* const* biases, tfl_cnn** out);
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* cnn);
 /* Arithmetic of the convolution stack: 0 = fp32 FMA on the CUDA cores; 1 = TF32 tensor cores
  * (wgmma, fp32 accumulate); 2 = 3xTF32 tensor cores (error-compensated split, fp32-class
