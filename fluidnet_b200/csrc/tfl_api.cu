@@ -792,6 +792,14 @@ int tfl_clamp(tfl_ctx* ctx, const tfl_grid* x, float lo, float hi) {
   return for_computed_planes(ctx, x, "clamp",
                              [&](long long off, long long n) { launch_clamp(x->data + off, lo, hi, n, ctx->stream); });
 }
+// Debug hook: the grid checks every operator makes on its flags descriptor (make_geo), alone.  The data pointer
+// is never read and nothing is launched, so any extent can be asked about without allocating it.
+int tfl_debug_make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is_3d) {
+  if (!ctx || !flags) return 1;
+  Geo g;
+  return make_geo(ctx, flags, is_3d, &g);
+}
+
 // Undocumented debugging hook.
 // mode: -1 automatic, 0 two-kernel advectVel, 1 / 2 tile kernel with that halo; variant: tile shape.
 int tfl_debug_advect_tile(tfl_ctx* ctx, int mode, int variant) {

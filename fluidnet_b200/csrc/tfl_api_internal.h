@@ -230,7 +230,9 @@ inline int make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is3d, Geo* g) {
     g->zoff = 0; g->gnz = flags->nz; g->zlo = 0; g->zhi = flags->nz;
   }
   if (!is3d && flags->nz != 1) return fail(ctx, "2D grid must have zsize == 1");
-  if (g->n * (long long)g->nb * 3 >= (1LL << 31) * 4) return fail(ctx, "grid too large");
+  // cell() (tfl_device.cuh) indexes one (batch, channel) block in 32 bits; the second bound keeps the whole
+  // velocity field within 2^33 cells.
+  if (g->n >= (1LL << 31) || g->n * (long long)g->nb * 3 >= (1LL << 31) * 4) return fail(ctx, "grid too large");
   return 0;
 }
 
