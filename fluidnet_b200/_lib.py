@@ -29,6 +29,11 @@ class CnnBanks(C.Structure):
                 ("aggregate_add", C.c_int32)]
 
 
+class CnnBanksEx(C.Structure):
+    _fields_ = [("num", C.c_int32), ("split_stage", C.c_int32), ("join_stage", C.c_int32),
+                ("aggregate_add", C.c_int32), ("dilate", C.c_int32)]
+
+
 class CnnInputs(C.Structure):
     _fields_ = [("p_div", C.c_int32), ("u_div", C.c_int32), ("div", C.c_int32), ("normalize", C.c_int32),
                 ("norm_func", C.c_int32), ("norm_chan", C.c_int32), ("pressure_skip", C.c_int32)]
@@ -51,7 +56,7 @@ SYMBOLS = [
     "tfl_solve_linear_system_jacobi", "tfl_solve_linear_system_pcg", "tfl_precond_from_string", "tfl_normalize_pressure_mean",
     "tfl_volumetric_up_sampling_nearest_forward", "tfl_rectangular_blur", "tfl_signed_distance_field", "tfl_velocity_divergence_backward",
     "tfl_velocity_update_backward", "tfl_volumetric_up_sampling_nearest_backward", "tfl_empty_domain", "tfl_flags_to_occupancy", "tfl_apply_bc",
-    "tfl_clamp", "tfl_cnn_create", "tfl_cnn_create_graph", "tfl_cnn_create_banked", "tfl_cnn_create_model", "tfl_cnn_destroy", "tfl_cnn_set_mode", "tfl_cnn_get_mode", "tfl_cnn_project", "tfl_simulate_step",
+    "tfl_clamp", "tfl_cnn_create", "tfl_cnn_create_graph", "tfl_cnn_create_banked", "tfl_cnn_create_model", "tfl_cnn_create_model_ex", "tfl_cnn_destroy", "tfl_cnn_set_mode", "tfl_cnn_get_mode", "tfl_cnn_project", "tfl_simulate_step",
     "tfl_host_sim_create", "tfl_host_sim_destroy", "tfl_host_sim_step",
     "tfl_step_graph_create", "tfl_step_graph_launch", "tfl_step_graph_destroy",
     "tfl_comm_unique_id", "tfl_comm_init", "tfl_comm_destroy", "tfl_slab_sim_create", "tfl_slab_sim_destroy",
@@ -128,6 +133,11 @@ def load():
                                          C.c_int, C.POINTER(CnnBanks), C.POINTER(CnnInputs),
                                          C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
                                          C.POINTER(C.c_void_p)]
+    lib.tfl_cnn_create_model_ex.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                            C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int,
+                                            C.c_int, C.POINTER(CnnBanksEx), C.POINTER(CnnInputs),
+                                            C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
+                                            C.POINTER(C.c_void_p)]
     lib.tfl_cnn_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int32),
                                    C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                    C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),

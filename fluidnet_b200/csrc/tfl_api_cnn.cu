@@ -11,6 +11,8 @@ constexpr int kMaxBanks = kMaxBankPtrs;     // banks a join kernel takes
 constexpr char kSlabTcOnly[] =
     "the z-slab projection runs on the tensor-core path only (the 3-D 'default' graph, single-bank or with banks "
     "split at stage 1 and joined at stage 3, in mode 1 or 2)";
+constexpr char kSlabDilate[] =
+    "the z-slab projection does not run banksType 'dilate' (dilated banks run on whole grids only)";
 constexpr char kSlabDefaultInputs[] =
     "the z-slab projection takes the default input block only (inputChannels pDiv, div, flags; normalizeInput with "
     "'std' of UDiv; no addPressureSkip)";
@@ -60,16 +62,18 @@ std::vector<float> concat_slice(const float* w, int nbanks, int i) {
 // full-resolution plane 0 is global plane zoff, bank i's local plane 0 its global coarse plane org[i] (whole grids:
 // all 0).  'add': one launch summing the banks, weights wj[0]; 'concat': one launch per bank with its slice wj[i],
 // banks N..2 writing / adding the fp32 partial sum `part`, bank 1 last adding it before the bias, ReLU and tail (one
-// bank: no partial sum).
+// bank: no partial sum).  phases: banks 2..N are dilated banks held as phase sub-grids (geo[i] =
+// make_conv_tc_phase_geo(.., i)) rather than multi-resolution banks.
 void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org, int zoff, int nbanks, bool add,
                     float* part, float* p_net, float* const* wj, const float* bias, const float* tail, int split,
-                    const ConvTcGeo& g, cudaStream_t st) {
+                    const ConvTcGeo& g, cudaStream_t st, bool phases = false) {
   auto src_of = [&](int first, int n, int mode) {
     TcJoinSrc js = {};
     for (int k = 0; k < n; k++) {
       const int i = first + k;
       js.p[k] = l2[i];
       js.px[k] = geo[i].px; js.py[k] = geo[i].py; js.nz[k] = geo[i].nz; js.shift[k] = i; js.org[k] = org[i];
+      js.phase[k] = phases && i > 0 ? 1 : 0;
     }
     js.zoff = zoff;
     js.n = n;
@@ -117,6 +121,7 @@ int finish_debug(tfl_ctx* ctx, const char* what) {
 // planes short of the local end), which a halo of 2 margin + 2 provides from margin = 3 s / 2 on.
 int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, int nx, int zoff, int nz, int own_lo,
                    int own_hi) {
+  if (m->bank_dilate) return fail(ctx, "slab: %s", kSlabDilate);
   if (!m->default_inputs) return fail(ctx, "slab: %s", kSlabDefaultInputs);
   if (!m->tc_ok || m->mode == 0) return fail(ctx, "slab: %s", kSlabTcOnly);
   if (m->nbanks == 1) return 0;
@@ -135,11 +140,12 @@ int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, 
 // Tensor-core path: padded channels-last activations owned by the model (their zero borders
 // must survive between calls, so they do not live in the shared arena).
 // z-slab (g.zoff, g.gnz): bank i holds the global coarse planes [ceil(zoff / 2^i), floor((zoff + nz) / 2^i)).
+// Dilated banks: bank i's buffers hold its 8^i phase sub-grids per batch entry (make_conv_tc_phase_geo).
 int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
   if (m->act_geo.nb == g.nb && m->act_geo.nz == g.nz && m->act_geo.ny == g.ny && m->act_geo.nx == g.nx &&
       (m->nbanks == 1 || m->act_zoff == g.zoff))
     return 0;
-  if (m->nbanks > 1) {
+  if (m->nbanks > 1 && !m->bank_dilate) {
     const int r = 1 << (m->nbanks - 1);
     if (ctx->slab && (g.nx % r || g.ny % r || g.gnz % r))
       return fail(ctx, "cnn: the z-slab's global grid %dx%dx%d is not divisible by 2^(banksNum-1) = %d", g.nx, g.ny,
@@ -170,8 +176,9 @@ int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
   if (m->part) cudaFree(m->part);
   m->part = nullptr;
   for (int i = 1, org = g.zoff; i < m->nbanks; i++) {
-    org = (org + 1) >> 1;
-    const ConvTcGeo bg = make_conv_tc_geo(g.nb, ((g.zoff + g.nz) >> i) - org, g.ny >> i, g.nx >> i);
+    org = m->bank_dilate ? 0 : (org + 1) >> 1;     // dilated banks: whole grids only (cnn_slab_check)
+    const ConvTcGeo bg = m->bank_dilate ? make_conv_tc_phase_geo(g.nb, g.nz, g.ny, g.nx, i)
+                                        : make_conv_tc_geo(g.nb, ((g.zoff + g.nz) >> i) - org, g.ny >> i, g.nx >> i);
     m->bgeo.push_back(bg);
     m->borg.push_back(org);
     for (int q = 0; q < 3; q++) {
@@ -187,7 +194,9 @@ int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
 }
 
 // Banked stack (split 1, join 3) on tensor cores: pyramid of the padded input, layers 1 and 2 of every bank at its
-// own resolution, then the join layer reading the banks' layer-2 outputs with nearest indexing.  'add': one launch
+// own resolution, then the join layer reading the banks' layer-2 outputs with nearest indexing.  Dilated banks:
+// the input copied into each bank's phase sub-grids, layers 1 and 2 as ordinary 3x3x3 layers on those (layer 1's
+// voxels outside a short phase re-zeroed), and the join reading them through its phase index map.  'add': one launch
 // summing the banks; 'concat': one launch per bank (N..2 into the fp32 partial sum, bank 1 last with the tail).
 // p_net is wanted on the local planes [p_lo, p_hi): bank i's layers 1 and 2 run on the coarse planes the join reads
 // from there (and the 3x3x3 stencil of layer 2 on those), the pyramid on all of the bank's planes.
@@ -205,20 +214,30 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
     geo[i] = m->bgeo[i - 1];
     org[i] = m->borg[i - 1];
     float* dst = m->bact[3 * (i - 1)];
-    // coarse plane c pools the planes 2 c, 2 c + 1 of the level above (global indices): local 2 c + (org[i-1] & 1)
-    launch_tc_pyramid(in[i - 1], geo[i - 1], dst, geo[i], org[i - 1] & 1, st, m->tc_planes);
+    if (m->bank_dilate) {
+      // dilated bank i: the network input laid out as its 8^i phase sub-grids
+      launch_tc_phase_copy(in[0], tg, dst, geo[i], i, m->tc_planes, st);
+    } else {
+      // coarse plane c pools the planes 2 c, 2 c + 1 of the level above (global indices): local 2 c + (org[i-1] & 1)
+      launch_tc_pyramid(in[i - 1], geo[i - 1], dst, geo[i], org[i - 1] & 1, st, m->tc_planes);
+    }
     in[i] = dst;
   }
   for (int i = 0; i < nbk; i++) {
     float* o1 = i == 0 ? m->act[1] : m->bact[3 * (i - 1) + 1];
     float* o2 = i == 0 ? m->act[2] : m->bact[3 * (i - 1) + 2];
-    // the join reads bank i at the coarse planes of the full-resolution planes [p_lo - 1, p_hi]
-    const int c_lo = ((zoff + p_lo - 1) >> i) - org[i], c_hi = ((zoff + p_hi) >> i) - org[i] + 1;
     ConvTcGeo g1 = geo[i], g2 = geo[i];
-    g2.z_lo = std::max(0, c_lo);     g2.z_hi = std::min(geo[i].nz, c_hi);
-    g1.z_lo = std::max(0, c_lo - 1); g1.z_hi = std::min(geo[i].nz, c_hi + 1);
+    if (!m->bank_dilate) {
+      // the join reads bank i at the coarse planes of the full-resolution planes [p_lo - 1, p_hi]
+      const int c_lo = ((zoff + p_lo - 1) >> i) - org[i], c_hi = ((zoff + p_hi) >> i) - org[i] + 1;
+      g2.z_lo = std::max(0, c_lo);     g2.z_hi = std::min(geo[i].nz, c_hi);
+      g1.z_lo = std::max(0, c_lo - 1); g1.z_hi = std::min(geo[i].nz, c_hi + 1);
+    }
     launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, m->tc_planes, 0, split,
                     g1, st);
+    // a phase shorter than the sub-grid (d does not divide an axis): its extra voxels are padding for layer 2
+    if (m->bank_dilate && i > 0 && ((tg.nx | tg.ny | tg.nz) & ((1 << i) - 1)))
+      launch_tc_phase_zero(o1, geo[i], i, tg, st);
     launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, g2, st);
     l2[i] = o2;
   }
@@ -226,7 +245,7 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
   g3.z_lo = std::max(0, p_lo);
   g3.z_hi = std::min(tg.nz, p_hi);
   launch_tc_join(l2, geo, org, zoff, nbk, m->bank_add, m->part, p_net, m->wBj[split].data(), m->b[m->conv0[2]],
-                 m->tail, split, g3, st);
+                 m->tail, split, g3, st, m->bank_dilate != 0);
 }
 
 // The three 3x3x3 layers (+ fused 1x1x1 tail) on tensor cores: act[0] -> act[1] -> act[2] -> p_net.
@@ -264,12 +283,18 @@ int tfl_cnn_create(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, co
 
 static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                           int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate, const tfl_cnn_inputs* inputs,
                            const float* const* weights, const float* const* biases, tfl_cnn** out);
 static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                               const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                              int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
-                              const float* const* weights, const float* const* biases, tfl_cnn** out);
+                              int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
+                              const tfl_cnn_inputs* inputs, const float* const* weights, const float* const* biases,
+                              tfl_cnn** out);
+static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                                 const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                                 int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
+                                 const tfl_cnn_inputs* inputs, const float* const* weights,
+                                 const float* const* biases, tfl_cnn** out);
 static const tfl_cnn_inputs kDefaultInputs = {1, 0, 1, 1, 0, 0, 0};
 
 int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
@@ -279,7 +304,7 @@ int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   return cnn_create_impl(ctx, is_3d, n_layers, cin, cout_logical, ksize, pool, up, pool_is_max, nonlin_sigmoid,
-                         nullptr, &kDefaultInputs, weights, biases, out);
+                         nullptr, 0, &kDefaultInputs, weights, biases, out);
 }
 
 int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
@@ -288,7 +313,7 @@ int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* 
                           const float* const* biases, tfl_cnn** out) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
-  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
+  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, 0,
                             &kDefaultInputs, weights, biases, out);
 }
 
@@ -298,6 +323,29 @@ int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
                          const float* const* weights, const float* const* biases, tfl_cnn** out) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
+  return cnn_create_model_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, 0,
+                               inputs, weights, biases, out);
+}
+
+int tfl_cnn_create_model_ex(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                            int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                            const float* const* weights, const float* const* biases, tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (banks && banks->dilate != 0 && banks->dilate != 1)
+    return fail(ctx, "cnn: banks dilate must be 0 ('mres') or 1 ('dilate') (got %d)", banks->dilate);
+  tfl_cnn_banks b = {};
+  if (banks) b = {banks->num, banks->split_stage, banks->join_stage, banks->aggregate_add};
+  return cnn_create_model_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid,
+                               banks ? &b : nullptr, banks ? banks->dilate : 0, inputs, weights, biases, out);
+}
+
+static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                                 const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                                 int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
+                                 const tfl_cnn_inputs* inputs, const float* const* weights,
+                                 const float* const* biases, tfl_cnn** out) {
   const tfl_cnn_inputs in = inputs ? *inputs : kDefaultInputs;
   // lib/model.lua:27-150 and :357-361; checkYangSettings, lib/model_utils.lua:211-227.
   if (!in.p_div && !in.u_div && !in.div) return fail(ctx, "Are you sure you dont want any (U, div or p) fields?");
@@ -321,14 +369,15 @@ int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
     return fail(ctx, "cnn: addPressureSkip joins pDiv to the hidden layer before the last convolution at full "
                      "resolution, which needs a 1x1 last convolution without upsampling (lib/model.lua:357-361; "
                      "not 'tog')");
-  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, &in,
-                            weights, biases, out);
+  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
+                            dilate, &in, weights, biases, out);
 }
 
 static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                               const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                              int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
-                              const float* const* weights, const float* const* biases, tfl_cnn** out) {
+                              int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
+                              const tfl_cnn_inputs* inputs, const float* const* weights, const float* const* biases,
+                              tfl_cnn** out) {
   if (banks) {     // the assertions of lib/model.lua:246-252 (checked whatever banksNum is)
     if (banks->num < 1) return fail(ctx, "cnn: banksNum >= 1 failed (got %d)", banks->num);
     if (!(banks->split_stage < banks->join_stage))
@@ -340,15 +389,18 @@ static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32
       return fail(ctx, "cnn: banksJoinStage >= 1 and banksJoinStage < #osize failed (%d, %d stages)",
                   banks->join_stage, n_layers);
     if (banks->num > kMaxBanks) return fail(ctx, "cnn: at most %d banks are supported (got %d)", kMaxBanks, banks->num);
+    // getConvLayer's assertion for banks 2..N, dilated by 2^(i-1) (lib/model_utils.lua:125)
+    for (int l = banks->split_stage - 1; dilate && banks->num > 1 && up && l < banks->join_stage - 1; l++)
+      if (up[l] > 1) return fail(ctx, "upsampling not supported for dilated convolutions. (stage %d)", l + 1);
     if (banks->num == 1) banks = nullptr;
   }
   return cnn_create_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                         inputs, weights, biases, out);
+                         banks ? dilate : 0, inputs, weights, biases, out);
 }
 
 static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                           int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                           int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate, const tfl_cnn_inputs* inputs,
                            const float* const* weights, const float* const* biases, tfl_cnn** out) {
   if (!out || n_layers < 1) return fail(ctx, "cnn: bad arguments");
   const tfl_cnn_inputs& in = *inputs;
@@ -405,6 +457,7 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   m->split = bsplit;
   m->join = bjoin;
   m->bank_add = banks && banks->aggregate_add ? 1 : 0;
+  m->bank_dilate = nbanks > 1 && dilate ? 1 : 0;
   int wi = 0;     // index into weights / biases
   for (int l = 0; l < n_layers; l++) {
     if (l > 0 && nbanks > 1 && l == bjoin && !m->bank_add && cin[l] != nbanks * cout_logical[l - 1]) {
@@ -436,11 +489,14 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
     }
     if (cout[l] > m->max_c) m->max_c = cout[l];
   }
-  {   // largest activation of the graph, in channels x cells-of-the-input-grid
+  {   // largest activation of the graph, in channels x cells-of-the-input-grid (banks 2..N have buffers of their
+      // own, cnn_bank_buf_bytes; the joined banks are counted here)
     double rel = 1.0;
-    m->max_rel = in_ch;      // the network input (pooled into the banks at stage 1)
+    m->max_rel = in_ch;      // the network input (pooled into, or shared by, the banks at stage 1)
     for (int l = 0; l < n_layers; l++) {
       if (nbanks > 1 && l == bjoin) m->max_rel = std::max(m->max_rel, rel * cin[l]);   // the joined banks
+      if (nbanks > 1 && l >= bsplit && l < bjoin)     // one bank's activations (no upsampling in a dilated stage)
+        m->bank_rel = std::max(m->bank_rel, rel * std::max(cout[l], cout_logical[l]));
       m->max_rel = std::max(m->max_rel, rel * cout[l]);                          // convolution output
       const int u = m->up[l], pl = m->pool[l];
       rel *= (double)u * u * (is_3d ? u : 1);
@@ -450,8 +506,8 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
     if (rel != 1.0) { tfl_cnn_destroy(ctx, m); return fail(ctx, "cnn: pooling and upsampling do not return to the input resolution"); }
     if ((double)m->max_c < m->max_rel) m->max_c = (int)std::ceil(m->max_rel);
   }
-  // Tensor-core eligibility: the 3-D 'default' graph (lib/model.lua:219-226), single-bank or with banks split
-  // before stage 1 and joined before stage 3.
+  // Tensor-core eligibility: the 3-D 'default' graph (lib/model.lua:219-226), single-bank or with banks (either type)
+  // split before stage 1 and joined before stage 3.
   static const int want[5][3] = {{0, 8, 3}, {8, 8, 3}, {8, 8, 3}, {8, 8, 1}, {8, 1, 1}};   // cin[0]: any input set
   m->tc_ok = is_3d && n_layers == 5 && !nonlin_sigmoid &&
              (nbanks == 1 || (bsplit == 0 && bjoin == 2 && nbanks <= kTcMaxBanks));
@@ -551,6 +607,43 @@ int tfl_debug_conv3_tc(tfl_ctx* ctx, const float* in, float* out, float* p_net, 
   if (rc) return rc;
   if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc: %s", cudaGetErrorString(se));
   return 0;
+}
+
+// tfl_debug_conv3_tc_dilated: one tensor-core 3x3x3 layer (not the final one) dilated by 2^sh the way a dilated bank
+// runs it: in (make_conv_tc_geo(nb, nz, ny, nx) layout, cin 3 on one float4 plane or 8 on two) is copied into phase
+// sub-grids, the layer runs on those, layer-1 style re-zeroing of short phases follows, and the sub-grids are gathered
+// back into the interior of out (same layout, 8 channels; nothing else of out is written).  Synchronises.
+int tfl_debug_conv3_tc_dilated(tfl_ctx* ctx, const float* in, float* out, const float* w_host, const float* bias_host,
+                               int cin, int split, int nb, int nz, int ny, int nx, int sh) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (cin != 3 && cin != 8) return fail(ctx, "debug_conv3_tc_dilated: cin must be 3 or 8 (got %d)", cin);
+  if (!in || !out || !w_host || !bias_host) return fail(ctx, "debug_conv3_tc_dilated: nil argument");
+  if (sh < 0 || sh > 7 || bad_grid(nb, nz, ny, nx, 1))
+    return fail(ctx, "debug_conv3_tc_dilated: bad grid %dx%dx%dx%d or dilation 2^%d", nb, nz, ny, nx, sh);
+  const ConvTcGeo gf = make_conv_tc_geo(nb, nz, ny, nx), gs = make_conv_tc_phase_geo(nb, nz, ny, nx, sh);
+  float *wB = upload_tc_weights(w_host, cin, split), *bias = nullptr, *sin = nullptr, *sout = nullptr;
+  auto release = [&]() {
+    for (float* p : {wB, bias, sin, sout})
+      if (p) cudaFree(p);
+  };
+  if (!wB || cudaMalloc((void**)&bias, 8 * 4) != cudaSuccess ||
+      cudaMalloc((void**)&sin, conv_tc_act_bytes(gs)) != cudaSuccess ||
+      cudaMalloc((void**)&sout, conv_tc_act_bytes(gs)) != cudaSuccess) {
+    release();
+    return fail(ctx, "debug_conv3_tc_dilated: cudaMalloc failed");
+  }
+  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
+  cudaMemset(sin, 0, conv_tc_act_bytes(gs));
+  cudaMemset(sout, 0, conv_tc_act_bytes(gs));
+  const int planes = cin == 3 ? 1 : 2;
+  launch_tc_phase_copy(in, gf, sin, gs, sh, planes, ctx->stream);
+  launch_conv3_tc(sin, sout, nullptr, wB, bias, nullptr, planes, 0, split, gs, ctx->stream);
+  launch_tc_phase_zero(sout, gs, sh, gf, ctx->stream);
+  launch_tc_phase_gather(sout, gs, out, gf, sh, ctx->stream);
+  const int rc = finish_debug(ctx, "debug_conv3_tc_dilated");
+  release();
+  return rc;
 }
 
 // tfl_debug_conv3_tc_join: the join layer of a banked model (split 1, join 3) on caller-owned bank buffers.
@@ -709,10 +802,28 @@ int tfl_debug_cnn_inputs_padded(tfl_ctx* ctx, const tfl_cnn* m, const float* p_d
 // tfl_cnn_create_graph does.  generic = 0: launch_conv_direct (the specialised kernel where the shape has one and its
 // weights fit shared memory, else the generic one); generic = 1: the generic kernel.  *kernel: the kernel that ran,
 // 1 direct or 2 generic.
+static int debug_conv_fp32_impl(tfl_ctx* ctx, const float* in, float* out, const float* w_host, const float* bias_host,
+                                int cin, int cout, int ks, int act, int is3d, int nb, int nz, int ny, int nx,
+                                int generic, int dil, int32_t* kernel);
 int tfl_debug_conv_fp32(tfl_ctx* ctx, const float* in, float* out, const float* w_host, const float* bias_host,
                         int cin, int cout, int ks, int act, int is3d, int nb, int nz, int ny, int nx, int generic,
                         int32_t* kernel) {
   DeviceGuard guard_(ctx);
+  return debug_conv_fp32_impl(ctx, in, out, w_host, bias_host, cin, cout, ks, act, is3d, nb, nz, ny, nx, generic, 1,
+                              kernel);
+}
+// tfl_debug_conv_fp32_dilated: the same with dilation dil >= 1 on every axis (padding dil (k-1)/2).
+int tfl_debug_conv_fp32_dilated(tfl_ctx* ctx, const float* in, float* out, const float* w_host, const float* bias_host,
+                                int cin, int cout, int ks, int act, int is3d, int nb, int nz, int ny, int nx,
+                                int generic, int dil, int32_t* kernel) {
+  DeviceGuard guard_(ctx);
+  if (ctx && dil < 1) return fail(ctx, "debug_conv_fp32: bad dilation %d", dil);
+  return debug_conv_fp32_impl(ctx, in, out, w_host, bias_host, cin, cout, ks, act, is3d, nb, nz, ny, nx, generic, dil,
+                              kernel);
+}
+static int debug_conv_fp32_impl(tfl_ctx* ctx, const float* in, float* out, const float* w_host, const float* bias_host,
+                                int cin, int cout, int ks, int act, int is3d, int nb, int nz, int ny, int nx,
+                                int generic, int dil, int32_t* kernel) {
   if (!ctx) return 1;
   if (!in || !out || !w_host || !bias_host || !kernel) return fail(ctx, "debug_conv_fp32: nil argument");
   if (cin < 1 || cout < 1 || ks < 1 || ks % 2 != 1 || act < 0 || act > 2 || (generic != 0 && generic != 1))
@@ -728,8 +839,8 @@ int tfl_debug_conv_fp32(tfl_ctx* ctx, const float* in, float* out, const float* 
   cudaMemcpy(dw, relaid.data(), relaid.size() * 4, cudaMemcpyHostToDevice);
   cudaMemcpy(db, bias_host, cout * 4, cudaMemcpyHostToDevice);
   const Geo g = whole_grid(ctx, nb, nz, ny, nx, is3d);
-  const int ran = generic ? launch_conv_any(in, out, dw, db, cin, cout, ks, act, g, ctx->stream)
-                          : launch_conv_direct(in, out, dw, db, cin, cout, ks, act, g, ctx->stream);
+  const int ran = generic ? launch_conv_any(in, out, dw, db, cin, cout, ks, act, g, ctx->stream, dil)
+                          : launch_conv_direct(in, out, dw, db, cin, cout, ks, act, g, ctx->stream, dil);
   const int rc = finish_debug(ctx, "debug_conv_fp32");
   cudaFree(dw);
   cudaFree(db);
@@ -803,12 +914,17 @@ void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
   delete m;
 }
 
-// One rotating buffer of bank i (0-based, i >= 1): bank i holds 2^-d i of bank 1's cells, and every
-// activation of bank 1 fits max_rel.
+// One rotating buffer of bank i (0-based, i >= 1): a multi-resolution bank holds 2^-d i of bank 1's cells, and every
+// activation of bank 1 fits max_rel; a dilated bank has bank 1's resolution and needs its own largest activation,
+// bank_rel (the joined banks live in bank 1's buffers).
 static size_t cnn_bank_buf_bytes(const tfl_cnn* m, const Geo& g, int i) {
   const double cells = (double)g.n * g.nb;
+  if (m->bank_dilate) return (size_t)(cells * m->bank_rel + 64) * 4;
   return (size_t)(cells * m->max_rel / (double)(1LL << ((m->is3d ? 3 : 2) * i)) + 64) * 4;
 }
+// Rotating buffers of each of banks 2..N: a dilated stage is convolution -> non-linearity -> pooling (no pixel
+// shuffle), so its result can go back to the buffer its input came from, and two suffice.
+static int cnn_bank_nbufs(const tfl_cnn* m) { return m->bank_dilate ? 2 : 3; }
 
 static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const float* U_div,
                             const float* flags, float* p_out, float* U_out, float threshold, const Geo& g,
@@ -865,17 +981,21 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
     // whose resolution follows the pooling / upsampling sizes (lib/model.lua:262-340, single bank).
     if (ctx->slab) return fail(ctx, "cnn: pooled / upsampled graphs run on whole grids only");
     float* bufs[3] = {actA, actB, (float*)take((size_t)((double)cells * m->max_rel + 64) * 4)};
-    // Banks 2..N rotate through three buffers of their own (bank i is 2^-d(i-1) the size of bank 1).
+    // Banks 2..N rotate through three buffers of their own (a multi-resolution bank i is 2^-d(i-1) the size of
+    // bank 1, a dilated one the same size).
     float* bank_bufs[kMaxBanks][3] = {};
-    for (int i = 1; i < m->nbanks; i++)
-      for (int q = 0; q < 3; q++) bank_bufs[i][q] = (float*)take(cnn_bank_buf_bytes(m, g, i));
-    // One stage of one bank: convolution ci (+ pixel shuffle) -> non-linearity -> pooling, on grid gl, through
-    // the rotating buffers bb.  out_bstride > 0: the stage's result is written with that batch stride (floats),
-    // so that it lands in place in a concatenation of banks.
+    for (int i = 1; i < m->nbanks; i++) {
+      for (int q = 0; q < cnn_bank_nbufs(m); q++) bank_bufs[i][q] = (float*)take(cnn_bank_buf_bytes(m, g, i));
+      if (cnn_bank_nbufs(m) == 2) bank_bufs[i][2] = bank_bufs[i][0];     // run_stage alternates the two
+    }
+    // One stage of one bank: convolution ci (dilated by dil) (+ pixel shuffle) -> non-linearity -> pooling, on grid
+    // gl, through the rotating buffers bb, never writing `keep` (an input other banks still read).  out_bstride > 0:
+    // the stage's result is written with that batch stride (floats), so that it lands in place in a concatenation
+    // of banks; dst (may be null): the stage's result goes there rather than to one of bb.
     auto run_stage = [&](int ci, int l, const float* src, float* const* bb, Geo& gl, long long out_bstride,
-                         const float** result) -> int {
+                         const float** result, int dil, const float* keep, float* dst) -> int {
       auto other = [&](const float* a) {
-        for (int q = 0; q < 3; q++) if (bb[q] != a) return bb[q];
+        for (int q = 0; q < 3; q++) if (bb[q] != a && bb[q] != keep) return bb[q];
         return bb[0];
       };
       const int u = m->up[l], pl = m->pool[l];
@@ -883,13 +1003,14 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
       const int shuffled = m->cout[ci] / (u * u * (gl.is3d ? u : 1));
       // per batch entry when the last operation of the stage writes with a batch stride
       const int nloop_conv = (out_bstride > 0 && u == 1 && pl == 1) ? gl.nb : 1;
-      float* o = other(src);
+      float* o = (dst && u == 1 && pl == 1) ? dst : other(src);
       for (int b = 0; b < nloop_conv; b++) {
         Geo gb = gl;
         if (nloop_conv > 1) gb.nb = 1;
         const long long ioff = nloop_conv > 1 ? (long long)b * m->cin[ci] * gl.n : 0;
         const long long ooff = nloop_conv > 1 ? (long long)b * out_bstride : 0;
-        if (launch_conv_direct(src + ioff, o + ooff, m->w[ci], m->b[ci], m->cin[ci], m->cout[ci], m->ks[ci], act, gb, st) < 0)
+        if (launch_conv_direct(src + ioff, o + ooff, m->w[ci], m->b[ci], m->cin[ci], m->cout[ci], m->ks[ci], act, gb, st,
+                               dil) < 0)
           return fail(ctx, "cnn: unsupported layer shape cout=%d k=%d", m->cout[ci], m->ks[ci]);
         ctx->launches += 1;
       }
@@ -897,7 +1018,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
       int chans = m->cout[ci];
       if (u > 1) {
         chans = shuffled;
-        float* sh = other(cur);
+        float* sh = (dst && pl == 1) ? dst : other(cur);
         const int nloop = (out_bstride > 0 && pl == 1) ? gl.nb : 1;
         const long long nin = (long long)m->cout[ci] * gl.n;
         for (int b = 0; b < nloop; b++) {
@@ -911,7 +1032,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
       if (pl > 1) {
         if (gl.nx % pl || gl.ny % pl || (gl.is3d && gl.nz % pl))
           return fail(ctx, "cnn: grid %dx%dx%d is not divisible by the pooling size %d", gl.nx, gl.ny, gl.nz, pl);
-        float* po = other(cur);
+        float* po = dst ? dst : other(cur);
         const int nloop = out_bstride > 0 ? gl.nb : 1;
         const long long nin = (long long)chans * gl.nx * gl.ny * gl.nz;
         for (int b = 0; b < nloop; b++) {
@@ -932,7 +1053,13 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
     Geo bank_g[kMaxBanks];
     Geo gl = g;
     for (int l = 0; l < m->n_layers; l++) {
-      if (nbk > 1 && l == m->split) {
+      if (nbk > 1 && l == m->split && m->bank_dilate) {
+        // Dilated banks (lib/model.lua:279-285): every bank reads the hidden layer as it is.
+        for (int i = 0; i < nbk; i++) {
+          bank_in[i] = in;
+          bank_g[i] = gl;
+        }
+      } else if (nbk > 1 && l == m->split) {
         // Gaussian pyramid (lib/model.lua:276-289): bank i = 2x average pool of bank i-1.
         const int r = 1 << (nbk - 1);
         if (gl.nx % r || gl.ny % r || (gl.is3d && gl.nz % r))
@@ -953,22 +1080,39 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
       }
       if (nbk > 1 && l >= m->split && l < m->join) {
         const bool last = l == m->join - 1;
+        // Dilated banks joined by 'concat' write their last stage straight into their channel slots of bank 1's
+        // result; the shared input of the split stage stays intact until every bank has read it.
+        const bool in_slot = m->bank_dilate && last && !m->bank_add;
+        const float* shared = (m->bank_dilate && l == m->split) ? in : nullptr;
+        // concat: bank 1's result is the first c_out channels of [nb][nbk c_out][n] at the join resolution (taken
+        // before the stage runs: run_stage moves bank_g[0] to the stage's output grid)
+        const Geo gs = bank_g[0];
+        const int c_out = m->cout[m->conv0[l]] / (m->up[l] * m->up[l] * (g.is3d ? m->up[l] : 1));
+        const long long n_join = (long long)(gs.nx * m->up[l] / m->pool[l]) * (gs.ny * m->up[l] / m->pool[l]) *
+                                 (g.is3d ? gs.nz * m->up[l] / m->pool[l] : gs.nz);
         for (int i = 0; i < nbk; i++) {
-          const Geo& g1 = bank_g[0];
-          const int c_out = m->cout[m->conv0[l]] / (m->up[l] * m->up[l] * (g.is3d ? m->up[l] : 1));
-          // concat: bank 1's result is the first c_out channels of [nb][nbk c_out][n] at the join resolution
-          const long long n_join = (long long)(g1.nx * m->up[l] / m->pool[l]) * (g1.ny * m->up[l] / m->pool[l]) *
-                                   (g.is3d ? g1.nz * m->up[l] / m->pool[l] : g1.nz);
-          const long long bstride = (last && i == 0 && !m->bank_add && g.nb > 1) ? (long long)nbk * c_out * n_join : 0;
-          if (run_stage(m->conv0[l] + i, l, bank_in[i], i == 0 ? bufs : bank_bufs[i], bank_g[i], bstride, &bank_in[i]))
+          const long long bstride = (last && (i == 0 || in_slot) && !m->bank_add && g.nb > 1)
+                                        ? (long long)nbk * c_out * n_join : 0;
+          float* dst = (in_slot && i > 0) ? (float*)bank_in[0] + (long long)i * c_out * n_join : nullptr;
+          if (run_stage(m->conv0[l] + i, l, bank_in[i], i == 0 ? bufs : bank_bufs[i], bank_g[i], bstride, &bank_in[i],
+                        m->bank_dilate ? 1 << i : 1, shared, dst))
             return 1;
         }
-        if (last) {   // lib/model.lua:292-318: upsample banks 2..N, then JoinTable or CAddTable
+        if (last && m->bank_dilate) {   // lib/model.lua:300-318: no upsampling; 'concat' is already in place
+          if (m->bank_add) {
+            const Geo& gj = bank_g[0];
+            if (launch_bank_join(bank_in, nbk, (float*)bank_in[0], gj.nb, c_out, gj.nz, gj.ny, gj.nx, g.is3d, 1, st,
+                                 1) < 0)
+              return fail(ctx, "cnn: bad bank count %d", nbk);
+            ctx->launches += 1;
+          }
+          in = bank_in[0];
+          gl = bank_g[0];
+        } else if (last) {   // lib/model.lua:292-318: upsample banks 2..N, then JoinTable or CAddTable
           const Geo& g1 = bank_g[0];
           for (int i = 1; i < nbk; i++)
             if (bank_g[i].nx << i != g1.nx || bank_g[i].ny << i != g1.ny || (g.is3d && bank_g[i].nz << i != g1.nz))
               return fail(ctx, "cnn: bank %d does not upsample to the resolution of bank 1 (grid not divisible)", i + 1);
-          const int c_out = m->cout[m->conv0[l]] / (m->up[l] * m->up[l] * (g.is3d ? m->up[l] : 1));
           if (launch_bank_join(bank_in, nbk, (float*)bank_in[0], g1.nb, c_out, g1.nz, g1.ny, g1.nx, g.is3d,
                                m->bank_add, st) < 0)
             return fail(ctx, "cnn: bad bank count %d", nbk);
@@ -978,7 +1122,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
         }
         continue;
       }
-      if (run_stage(m->conv0[l], l, in, bufs, gl, 0, &in)) return 1;
+      if (run_stage(m->conv0[l], l, in, bufs, gl, 0, &in, 1, nullptr, nullptr)) return 1;
     }
     if (gl.nx != g.nx || gl.ny != g.ny || gl.nz != g.nz) return fail(ctx, "cnn: graph does not return to the input resolution");
   }
@@ -996,7 +1140,7 @@ static size_t cnn_scratch_bytes(const tfl_cnn* m, const Geo& g) {
   const size_t cells = (size_t)g.n * g.nb;
   size_t bytes = cells * 4 * (g.nc + m->in_ch + 2 * (size_t)m->max_c) + 4 * g.nb + 8 * 256;
   if (!m->plain) bytes += (size_t)((double)cells * m->max_rel + 64) * 4 + 256;     // third rotating buffer
-  for (int i = 1; i < m->nbanks; i++) bytes += 3 * (cnn_bank_buf_bytes(m, g, i) + 256);
+  for (int i = 1; i < m->nbanks; i++) bytes += cnn_bank_nbufs(m) * (cnn_bank_buf_bytes(m, g, i) + 256);
   return bytes;
 }
 
@@ -1060,6 +1204,7 @@ int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!m) return fail(ctx, "cnn is nil");
+  if (m->bank_dilate) return fail(ctx, "cnn_project_from_sums: %s", kSlabDilate);
   if (!m->default_inputs) return fail(ctx, "cnn_project_from_sums: %s", kSlabDefaultInputs);
   if (!m->tc_ok || m->mode == 0) return fail(ctx, "cnn_project_from_sums: %s", kSlabTcOnly);
   if (!dev_sums) return fail(ctx, "cnn_project_from_sums: nil sums");

@@ -84,6 +84,10 @@ struct tfl_cnn {
   // multi-resolution banks (lib/model.lua:252-361): stages [split, join) (0-based here) hold one convolution
   // per bank; conv0[l] is the index of stage l's first convolution.  nbanks == 1: single bank.
   int nbanks = 1, split = 0, join = 0, bank_add = 0;
+  // banksType 'dilate' (nbanks > 1 only): no pyramid, bank i's convolutions in [split, join) dilated by 2^i (0-based
+  // i), every bank at bank 1's resolution, no upsampling at the join.  On the tensor cores bank i's buffers hold its
+  // phase sub-grids (make_conv_tc_phase_geo).
+  int bank_dilate = 0;
   std::vector<int> conv0;
   int max_c = 0;
   // per-layer extras of the 'tog' / 'yang' graphs (lib/model.lua:164-239): the convolution emits
@@ -94,6 +98,7 @@ struct tfl_cnn {
   int nonlin = 1;            // 1 ReLU, 2 sigmoid (activation codes of tfl_cnn.cu)
   bool plain = true;
   double max_rel = 0.0;      // largest channels x (cells relative to the input grid) of any stage
+  double bank_rel = 0.0;     // the same over one bank's activations in the banked stages (conv output, pooled)
   // input block (tfl_cnn_inputs): in_sel the kCnnIn* channels, in_ch = cin[0]; norm_func a kCnnScale* code (kCnnScaleOne
   // when normalizeInput is off), norm_chan the kCnnStat* field.  With the pressure skip the last convolution keeps
   // its hidden channels and w_skip, its pDiv weight, is added by launch_cnn_skip.

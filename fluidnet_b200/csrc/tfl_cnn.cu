@@ -17,11 +17,13 @@ __device__ __forceinline__ float activate(float r, int act) {
   return r;
 }
 
-// weights in smem as [cin][tap][COUT]; taps ordered (dz, dy, dx).
-template <int COUT, int KS, bool IS3D>
+// weights in smem as [cin][tap][COUT]; taps ordered (dz, dy, dx).  DIL: tap t reads the input at offset
+// (t - (k-1)/2) dil on every axis (nn.{Spatial,Volumetric}DilatedConvolution, stride 1, padding dil (k-1)/2); without
+// it dil is not read and the kernel is the undilated one.
+template <int COUT, int KS, bool IS3D, bool DIL>
 __global__ void __launch_bounds__(256)
 k_conv_direct(const float* __restrict__ in, float* __restrict__ out, const float* __restrict__ w,
-              const float* __restrict__ bias, int cin, int act, Geo g) {
+              const float* __restrict__ bias, int cin, int act, Geo g, int dil) {
   extern __shared__ float sw[];
   constexpr int KZ = IS3D ? KS : 1;
   constexpr int TAPS = KZ * KS * KS;
@@ -44,22 +46,23 @@ k_conv_direct(const float* __restrict__ in, float* __restrict__ out, const float
 
   constexpr int P = (KS - 1) / 2;
   constexpr int PZ = (KZ - 1) / 2;
+  const int d = DIL ? dil : 1;
   const int kg = k + g.zoff;
   for (int c = 0; c < cin; c++) {
     const float* ib = in + ((long long)b * cin + c) * g.n;
     const float* wc = sw + c * TAPS * COUT;
 #pragma unroll
     for (int dz = 0; dz < KZ; dz++) {
-      const int zg = kg + dz - PZ;
+      const int zg = DIL ? kg + (dz - PZ) * d : kg + dz - PZ;
       if (zg < 0 || zg >= g.gnz) continue;           // zero padding at the GLOBAL boundary
       const int zl = zg - g.zoff;
 #pragma unroll
       for (int dy = 0; dy < KS; dy++) {
-        const int yy = j + dy - P;
+        const int yy = DIL ? j + (dy - P) * d : j + dy - P;
         if (yy < 0 || yy >= g.ny) continue;
 #pragma unroll
         for (int dx = 0; dx < KS; dx++) {
-          const int xx = i + dx - P;
+          const int xx = DIL ? i + (dx - P) * d : i + dx - P;
           if (xx < 0 || xx >= g.nx) continue;
           const float v = __ldg(ib + ((long long)zl * g.ny + yy) * g.nx + xx);
           const float* wt = wc + ((dz * KS + dy) * KS + dx) * COUT;
@@ -79,9 +82,10 @@ k_conv_direct(const float* __restrict__ in, float* __restrict__ out, const float
 
 // Any (cout, k): one thread per output value, weights [cin][tap][cout] read through the cache.  The
 // fallback for layer shapes outside the specialised table (e.g. the 256-channel 1x1x1 convolution
-// inside a VolumetricConvolutionUpsample); same accumulation order as k_conv_direct.
+// inside a VolumetricConvolutionUpsample); same accumulation order as k_conv_direct, and the same DIL switch.
+template <bool DIL>
 __global__ void k_conv_any(const float* __restrict__ in, float* __restrict__ out, const float* __restrict__ w,
-                           const float* __restrict__ bias, int cin, int cout, int ks, int act, Geo g) {
+                           const float* __restrict__ bias, int cin, int cout, int ks, int act, Geo g, int dil) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   const long long total = (long long)g.nb * cout * g.n;
   if (t >= total) return;
@@ -92,18 +96,19 @@ __global__ void k_conv_any(const float* __restrict__ in, float* __restrict__ out
   const int kz = g.is3d ? ks : 1;
   const int P = (ks - 1) / 2, PZ = (kz - 1) / 2;
   const int taps = kz * ks * ks;
+  const int d = DIL ? dil : 1;
   float acc = __ldg(bias + o);
   for (int c = 0; c < cin; c++) {
     const float* ib = in + ((long long)b * cin + c) * g.n;
     const float* wc = w + (long long)c * taps * cout;
     for (int dz = 0; dz < kz; dz++) {
-      const int zz = k + dz - PZ;
+      const int zz = DIL ? k + (dz - PZ) * d : k + dz - PZ;
       if (zz < 0 || zz >= g.nz) continue;
       for (int dy = 0; dy < ks; dy++) {
-        const int yy = j + dy - P;
+        const int yy = DIL ? j + (dy - P) * d : j + dy - P;
         if (yy < 0 || yy >= g.ny) continue;
         for (int dx = 0; dx < ks; dx++) {
-          const int xx = i + dx - P;
+          const int xx = DIL ? i + (dx - P) * d : i + dx - P;
           if (xx < 0 || xx >= g.nx) continue;
           acc = fmaf(__ldg(ib + ((long long)zz * g.ny + yy) * g.nx + xx), __ldg(wc + ((dz * ks + dy) * ks + dx) * cout + o), acc);
         }
@@ -156,10 +161,12 @@ __global__ void k_pixel_shuffle(const float* __restrict__ in, float* __restrict_
 // [nb][c][nz / rz][ny / r][nx / r] with r = 2^(i-1) (rz = r in 3-D, 1 in 2-D), upsampled nearest to the
 // full grid on the fly.  concat: out is [nb][nbanks * c][nz][ny][nx] and bank i lands at channel offset
 // (i-1) c (bank 1 is already in place); add: out is [nb][c][nz][ny][nx], holds bank 1 and gets banks 2..N
-// added in bank order, as CAddTable does.
+// added in bank order, as CAddTable does.  FULL: every bank is at the full resolution (banksType 'dilate', no
+// upsampling, lib/model.lua:300-303); r = 1.
 struct BankPtrs {
   const float* p[kMaxBankPtrs];
 };
+template <bool FULL>
 __global__ void k_bank_join(BankPtrs banks, int nbanks, float* __restrict__ out, int c, int nz, int ny, int nx,
                             int is3d, int add, long long total) {
   const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
@@ -171,24 +178,26 @@ __global__ void k_bank_join(BankPtrs banks, int nbanks, float* __restrict__ out,
   if (add) {
     float v = out[t];
     for (int i = 1; i < nbanks; i++) {
-      const int bx = nx >> i, by = ny >> i, bz = is3d ? nz >> i : nz;
-      const int zi = is3d ? z >> i : z;
-      v = v + __ldg(banks.p[i] + ((bc * bz + zi) * by + (y >> i)) * bx + (x >> i));
+      const int s = FULL ? 0 : i;
+      const int bx = nx >> s, by = ny >> s, bz = is3d ? nz >> s : nz;
+      const int zi = is3d ? z >> s : z;
+      v = v + __ldg(banks.p[i] + ((bc * bz + zi) * by + (y >> s)) * bx + (x >> s));
     }
     out[t] = v;
   } else {
     const long long cell = t % n;
     for (int i = 1; i < nbanks; i++) {
-      const int bx = nx >> i, by = ny >> i, bz = is3d ? nz >> i : nz;
-      const int zi = is3d ? z >> i : z;
-      out[((b * nbanks + i) * c + ch) * n + cell] = __ldg(banks.p[i] + ((bc * bz + zi) * by + (y >> i)) * bx + (x >> i));
+      const int s = FULL ? 0 : i;
+      const int bx = nx >> s, by = ny >> s, bz = is3d ? nz >> s : nz;
+      const int zi = is3d ? z >> s : z;
+      out[((b * nbanks + i) * c + ch) * n + cell] = __ldg(banks.p[i] + ((bc * bz + zi) * by + (y >> s)) * bx + (x >> s));
     }
   }
 }
 
-template <int COUT, int KS, bool IS3D>
+template <int COUT, int KS, bool IS3D, bool DIL>
 static bool conv_launch(const float* in, float* out, const float* w, const float* b, int cin, int act,
-                        const Geo& g, cudaStream_t st) {
+                        const Geo& g, int dil, cudaStream_t st) {
   const int nzr = g.zhi - g.zlo;
   dim3 block = IS3D ? dim3(32, 4, 2) : dim3(32, 8, 1);
   dim3 grid((g.nx + block.x - 1) / block.x, (g.ny + block.y - 1) / block.y,
@@ -201,7 +210,7 @@ static bool conv_launch(const float* in, float* out, const float* w, const float
     int dev = 0;
     cudaGetDevice(&dev);
     if (smem > allowed[dev & 63]) {
-      if (cudaFuncSetAttribute(k_conv_direct<COUT, KS, IS3D>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+      if (cudaFuncSetAttribute(k_conv_direct<COUT, KS, IS3D, DIL>, cudaFuncAttributeMaxDynamicSharedMemorySize,
                                (int)smem) != cudaSuccess) {
         cudaGetLastError();
         return false;
@@ -209,30 +218,35 @@ static bool conv_launch(const float* in, float* out, const float* w, const float
       allowed[dev & 63] = smem;
     }
   }
-  k_conv_direct<COUT, KS, IS3D><<<grid, block, smem, st>>>(in, out, w, b, cin, act, g);
+  k_conv_direct<COUT, KS, IS3D, DIL><<<grid, block, smem, st>>>(in, out, w, b, cin, act, g, dil);
   return true;
 }
 
 int launch_conv_direct(const float* in, float* out, const float* wdev, const float* bdev, int cin, int cout,
-                       int ksize, int act, const Geo& g, cudaStream_t st) {
-#define TFL_CONV_CASE(CO, KS_)                                                        \
-  if (cout == CO && ksize == KS_) {                                                   \
-    const bool ok_ = g.is3d ? conv_launch<CO, KS_, true>(in, out, wdev, bdev, cin, act, g, st)    \
-                            : conv_launch<CO, KS_, false>(in, out, wdev, bdev, cin, act, g, st);  \
-    if (ok_) return kConvDirect;                                                      \
+                       int ksize, int act, const Geo& g, cudaStream_t st, int dil) {
+#define TFL_CONV_CASE(CO, KS_)                                                                          \
+  if (cout == CO && ksize == KS_) {                                                                     \
+    const bool ok_ = dil > 1 ? (g.is3d ? conv_launch<CO, KS_, true, true>(in, out, wdev, bdev, cin, act, g, dil, st)  \
+                                       : conv_launch<CO, KS_, false, true>(in, out, wdev, bdev, cin, act, g, dil, st)) \
+                             : (g.is3d ? conv_launch<CO, KS_, true, false>(in, out, wdev, bdev, cin, act, g, 1, st)    \
+                                       : conv_launch<CO, KS_, false, false>(in, out, wdev, bdev, cin, act, g, 1, st)); \
+    if (ok_) return kConvDirect;                                                                        \
   }
   TFL_CONV_CASE(8, 3) TFL_CONV_CASE(8, 1) TFL_CONV_CASE(1, 1) TFL_CONV_CASE(16, 3) TFL_CONV_CASE(16, 1)
   TFL_CONV_CASE(1, 3) TFL_CONV_CASE(6, 3) TFL_CONV_CASE(6, 1) TFL_CONV_CASE(32, 1) TFL_CONV_CASE(16, 5)
   TFL_CONV_CASE(32, 5) TFL_CONV_CASE(64, 5) TFL_CONV_CASE(64, 1)
 #undef TFL_CONV_CASE
-  return launch_conv_any(in, out, wdev, bdev, cin, cout, ksize, act, g, st);
+  return launch_conv_any(in, out, wdev, bdev, cin, cout, ksize, act, g, st, dil);
 }
 
 int launch_conv_any(const float* in, float* out, const float* wdev, const float* bdev, int cin, int cout, int ksize,
-                    int act, const Geo& g, cudaStream_t st) {
+                    int act, const Geo& g, cudaStream_t st, int dil) {
   if (g.zlo != 0 || g.zhi != g.nz || g.zoff != 0) return -1;      // the generic kernel works on whole grids only
   const long long total = (long long)g.nb * cout * g.n;
-  k_conv_any<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, out, wdev, bdev, cin, cout, ksize, act, g);
+  if (dil > 1)
+    k_conv_any<true><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, out, wdev, bdev, cin, cout, ksize, act, g, dil);
+  else
+    k_conv_any<false><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, out, wdev, bdev, cin, cout, ksize, act, g, 1);
   return kConvGeneric;
 }
 
@@ -248,12 +262,15 @@ void launch_pixel_shuffle(const float* in, float* out, int nb, int n_out, int nz
   k_pixel_shuffle<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(in, out, n_out, nz, ny, nx, s, is3d, total);
 }
 int launch_bank_join(const float* const* banks, int nbanks, float* out, int nb, int c, int nz, int ny, int nx,
-                     int is3d, int add, cudaStream_t st) {
+                     int is3d, int add, cudaStream_t st, int full) {
   if (nbanks < 2 || nbanks > kMaxBankPtrs) return -1;
   BankPtrs bp = {};
   for (int i = 1; i < nbanks; i++) bp.p[i] = banks[i];
   const long long total = (long long)nb * c * nz * ny * nx;
-  k_bank_join<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(bp, nbanks, out, c, nz, ny, nx, is3d, add, total);
+  if (full)
+    k_bank_join<true><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(bp, nbanks, out, c, nz, ny, nx, is3d, add, total);
+  else
+    k_bank_join<false><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(bp, nbanks, out, c, nz, ny, nx, is3d, add, total);
   return 1;
 }
 

@@ -448,7 +448,12 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
         const int by = interior ? ((gy - 1) >> sh) + 1 : 0;
         const int bz = interior ? ((gz - 1 + js.zoff) >> sh) - js.org[k] + 1 : 0;
         const long long plane_k = (long long)(js.nz[k] + 2) * js.py[k] * js.px[k];
-        const float4* src = (const float4*)js.p[k] + b * 2 * plane_k + ((long long)bz * js.py[k] + by) * js.px[k] + bx;
+        // phase sub-grids: batch entry of (b, the voxel's phase); outside the grid any entry's border voxel is zero
+        const int pm = (1 << sh) - 1;
+        const long long bk = js.phase[k] ? (((long long)b << (3 * sh)) | (((gz - 1) & pm) << (2 * sh)) |
+                                            (((gy - 1) & pm) << sh) | ((gx - 1) & pm))
+                                         : b;
+        const float4* src = (const float4*)js.p[k] + bk * 2 * plane_k + ((long long)bz * js.py[k] + by) * js.px[k] + bx;
         const float4 a0 = __ldg(src), a1 = __ldg(src + plane_k);
         v[it][0] = make_float4(v[it][0].x + a0.x, v[it][0].y + a0.y, v[it][0].z + a0.z, v[it][0].w + a0.w);
         v[it][1] = make_float4(v[it][1].x + a1.x, v[it][1].y + a1.y, v[it][1].z + a1.z, v[it][1].w + a1.w);
@@ -755,7 +760,85 @@ __global__ void k_tc_pyramid(const float4* __restrict__ in, ConvTcGeo gi, float4
   }
 }
 
+// Phase sub-grid voxel t (over gs.nb entries x gs.nz x gs.ny x gs.nx) -> its full-resolution voxel; false outside the
+// full grid gf.
+__device__ __forceinline__ bool phase_voxel(long long t, const ConvTcGeo& gs, int sh, const ConvTcGeo& gf, long long* e,
+                                            int* sx, int* sy, int* sz, long long* b, int* x, int* y, int* z) {
+  *sx = (int)(t % gs.nx);
+  *sy = (int)((t / gs.nx) % gs.ny);
+  *sz = (int)((t / ((long long)gs.nx * gs.ny)) % gs.nz);
+  *e = t / ((long long)gs.nx * gs.ny * gs.nz);
+  const int m = (1 << sh) - 1;
+  const int r = (int)(*e & ((1LL << (3 * sh)) - 1));
+  *b = *e >> (3 * sh);
+  *x = (*sx << sh) | (r & m);
+  *y = (*sy << sh) | ((r >> sh) & m);
+  *z = (*sz << sh) | (r >> (2 * sh));
+  return *x < gf.nx && *y < gf.ny && *z < gf.nz;
+}
+
+__global__ void k_tc_phase_copy(const float4* __restrict__ in, ConvTcGeo gf, float4* __restrict__ out, ConvTcGeo gs,
+                                int sh, int planes, long long total) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  long long e, b;
+  int sx, sy, sz, x, y, z;
+  const bool valid = phase_voxel(t, gs, sh, gf, &e, &sx, &sy, &sz, &b, &x, &y, &z);
+  const long long fplane = (long long)(gf.nz + 2) * gf.py * gf.px, splane = (long long)(gs.nz + 2) * gs.py * gs.px;
+  for (int q = 0; q < planes; q++) {
+    const float4 v = valid ? __ldg(in + (b * 2 + q) * fplane + ((long long)(z + 1) * gf.py + (y + 1)) * gf.px + (x + 1))
+                           : make_float4(0.f, 0.f, 0.f, 0.f);
+    out[(e * 2 + q) * splane + ((long long)(sz + 1) * gs.py + (sy + 1)) * gs.px + (sx + 1)] = v;
+  }
+}
+
+__global__ void k_tc_phase_zero(float4* __restrict__ buf, ConvTcGeo gs, int sh, ConvTcGeo gf, long long total) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  long long e, b;
+  int sx, sy, sz, x, y, z;
+  if (phase_voxel(t, gs, sh, gf, &e, &sx, &sy, &sz, &b, &x, &y, &z)) return;
+  const long long splane = (long long)(gs.nz + 2) * gs.py * gs.px;
+  for (int q = 0; q < 2; q++)
+    buf[(e * 2 + q) * splane + ((long long)(sz + 1) * gs.py + (sy + 1)) * gs.px + (sx + 1)] = make_float4(0.f, 0.f, 0.f, 0.f);
+}
+
+__global__ void k_tc_phase_gather(const float4* __restrict__ in, ConvTcGeo gs, float4* __restrict__ out, ConvTcGeo gf,
+                                  int sh, long long total) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  long long e, b;
+  int sx, sy, sz, x, y, z;
+  if (!phase_voxel(t, gs, sh, gf, &e, &sx, &sy, &sz, &b, &x, &y, &z)) return;
+  const long long fplane = (long long)(gf.nz + 2) * gf.py * gf.px, splane = (long long)(gs.nz + 2) * gs.py * gs.px;
+  for (int q = 0; q < 2; q++)
+    out[(b * 2 + q) * fplane + ((long long)(z + 1) * gf.py + (y + 1)) * gf.px + (x + 1)] =
+        __ldg(in + (e * 2 + q) * splane + ((long long)(sz + 1) * gs.py + (sy + 1)) * gs.px + (sx + 1));
+}
+
 }  // namespace
+
+ConvTcGeo make_conv_tc_phase_geo(int nb, int nz, int ny, int nx, int sh) {
+  const int d = 1 << sh;
+  return make_conv_tc_geo(nb << (3 * sh), (nz + d - 1) >> sh, (ny + d - 1) >> sh, (nx + d - 1) >> sh);
+}
+static long long phase_cells(const ConvTcGeo& gs) { return (long long)gs.nb * gs.nz * gs.ny * gs.nx; }
+void launch_tc_phase_copy(const float* in, const ConvTcGeo& gfull, float* out, const ConvTcGeo& gsub, int sh,
+                          int planes, cudaStream_t st) {
+  const long long total = phase_cells(gsub);
+  k_tc_phase_copy<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float4*)in, gfull, (float4*)out, gsub, sh,
+                                                                    planes, total);
+}
+void launch_tc_phase_zero(float* buf, const ConvTcGeo& gsub, int sh, const ConvTcGeo& gfull, cudaStream_t st) {
+  const long long total = phase_cells(gsub);
+  k_tc_phase_zero<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((float4*)buf, gsub, sh, gfull, total);
+}
+void launch_tc_phase_gather(const float* in, const ConvTcGeo& gsub, float* out, const ConvTcGeo& gfull, int sh,
+                            cudaStream_t st) {
+  const long long total = phase_cells(gsub);
+  k_tc_phase_gather<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((const float4*)in, gsub, (float4*)out, gfull, sh,
+                                                                      total);
+}
 
 ConvTcGeo make_conv_tc_geo(int nb, int nz, int ny, int nx) {
   ConvTcGeo g;

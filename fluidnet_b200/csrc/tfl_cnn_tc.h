@@ -33,10 +33,13 @@ int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, 
 //   part_mode 3: add `partial` before the bias, then as part_mode 0.
 // On a z-slab the full-resolution plane z (local) is global plane z + zoff, and local plane 0 of bank k is its
 // global coarse plane org[k]: bank k is read at plane ((z + zoff) >> shift[k]) - org[k].  Whole grids: all zero.
+// phase[k] = 1: bank k is a dilated bank at full resolution held as phase sub-grids (launch_tc_phase_copy, d =
+// 2^shift[k]): the full-resolution voxel v is sub-grid voxel v >> shift[k] of batch entry (b, v & (d-1)).
 constexpr int kTcMaxBanks = 8;
 struct TcJoinSrc {
   const float* p[kTcMaxBanks];
   int px[kTcMaxBanks], py[kTcMaxBanks], nz[kTcMaxBanks], shift[kTcMaxBanks], org[kTcMaxBanks];
+  int phase[kTcMaxBanks];
   int zoff;
   int n;
   int part_mode;
@@ -51,5 +54,20 @@ int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, co
 // planes = 2 (the input of a set with UDiv): both float4 planes, all four channels of each.
 void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const ConvTcGeo& gout, int z_phase,
                        cudaStream_t st, int planes = 1);
+
+// Phase decomposition of a dilated bank (banksType 'dilate', dilation d = 2^sh): a 3x3x3 convolution with dilation d
+// on an nz x ny x nx grid is d^3 ordinary 3x3x3 convolutions, one on each sub-lattice {v = s d + r}, each zero-padded
+// at its own border.  The sub-grids are batch entries e = ((b d + rz) d + ry) d + rx of make_conv_tc_phase_geo, of
+// ceil(n / d) voxels per axis; a sub-grid voxel whose full-resolution voxel lies outside the grid (n % d != 0, or
+// d > n) must read as zero.  launch_tc_phase_copy lays a padded full-resolution buffer (geometry gfull) out that way
+// (zeros there); launch_tc_phase_zero zeroes those voxels of a layer's output (both planes) so that the next layer
+// reads them as padding; launch_tc_phase_gather copies the sub-grids back to the interior of a full-resolution buffer
+// (both planes).
+ConvTcGeo make_conv_tc_phase_geo(int nb, int nz, int ny, int nx, int sh);
+void launch_tc_phase_copy(const float* in, const ConvTcGeo& gfull, float* out, const ConvTcGeo& gsub, int sh,
+                          int planes, cudaStream_t st);
+void launch_tc_phase_zero(float* buf, const ConvTcGeo& gsub, int sh, const ConvTcGeo& gfull, cudaStream_t st);
+void launch_tc_phase_gather(const float* in, const ConvTcGeo& gsub, float* out, const ConvTcGeo& gfull, int sh,
+                            cudaStream_t st);
 
 }  // namespace tfl

@@ -121,14 +121,16 @@ void launch_cnn_finish_fused(const float* p_net, float* U, const unsigned char* 
 // Generic direct convolution (fp32 FMA): in [b][cin][z][y][x] -> out [b][cout][z][y][x].
 // wdev: device weights re-laid out as [cin][tap][cout_pad], bias [cout].
 // act: 0 none, 1 ReLU, 2 sigmoid.
+// dil > 1: dilated convolution (nn.{Spatial,Volumetric}DilatedConvolution with dilation dil on every axis, stride 1,
+// padding dil (k-1)/2: same grid out as in); dil = 1 runs the undilated kernels.
 // Returns the kernel that ran: kConvDirect (k_conv_direct, a specialised (cout, k) whose weights fit shared
 // memory) or kConvGeneric (k_conv_any, every other shape, whole grids only); -1 if none can run.
 enum : int { kConvDirect = 1, kConvGeneric = 2 };
 int launch_conv_direct(const float* in, float* out, const float* wdev, const float* bdev, int cin, int cout,
-                       int ksize, int act, const Geo& g, cudaStream_t st);
+                       int ksize, int act, const Geo& g, cudaStream_t st, int dil = 1);
 // The generic kernel alone (launch_conv_direct's fallback): same operands, same accumulation order.
 int launch_conv_any(const float* in, float* out, const float* wdev, const float* bdev, int cin, int cout, int ksize,
-                    int act, const Geo& g, cudaStream_t st);
+                    int act, const Geo& g, cudaStream_t st, int dil = 1);
 void launch_pool(const float* in, float* out, int nbc, int nz, int ny, int nx, int p, int is3d, int is_max,
                  cudaStream_t st);
 void launch_pixel_shuffle(const float* in, float* out, int nb, int n_out, int nz, int ny, int nx, int s, int is3d,
@@ -136,9 +138,10 @@ void launch_pixel_shuffle(const float* in, float* out, int nb, int n_out, int nz
 // Join of multi-resolution banks: banks[i] (i = 1 .. nbanks-1; banks[0] unused) is bank i+1 at 2^-i the
 // resolution of the full [nz][ny][nx] grid (z kept in 2-D), c channels; upsampled nearest and written at
 // channel offset i c of out [nb][nbanks c][n] (add == 0) or added in bank order to out [nb][c][n] (add == 1).
+// full = 1: every bank is at the full resolution (dilated banks), no upsampling.
 constexpr int kMaxBankPtrs = 8;
 int launch_bank_join(const float* const* banks, int nbanks, float* out, int nb, int c, int nz, int ny, int nx,
-                     int is3d, int add, cudaStream_t st);
+                     int is3d, int add, cudaStream_t st, int full = 0);
 
 // ---- tfl_pcg.cu: matrix-free PCG pressure solve ----
 struct PcgScratch {            // owned by the context, grow-only

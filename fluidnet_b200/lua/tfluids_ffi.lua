@@ -83,6 +83,11 @@ int tfl_cnn_create_model(tfl_ctx*, int is_3d, int n_layers, const int32_t* cin, 
                          const int32_t* pool, const int32_t* up, int pool_is_max, int nonlin_sigmoid,
                          const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs, const float* const* weights,
                          const float* const* biases, tfl_cnn** out);
+typedef struct tfl_cnn_banks_ex { int32_t num, split_stage, join_stage, aggregate_add, dilate; } tfl_cnn_banks_ex;
+int tfl_cnn_create_model_ex(tfl_ctx*, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                            int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                            const float* const* weights, const float* const* biases, tfl_cnn** out);
 int tfl_simulate_step(tfl_ctx*, const tfl_state*, const tfl_mconf*, tfl_cnn*);
 typedef struct tfl_step_graph tfl_step_graph;
 typedef struct tfl_slab_sim tfl_slab_sim;

@@ -40,10 +40,11 @@ class ProjectionModel:
         """layers: [(weight ndarray [cout * up^d][cin][kz][ky][kx], bias ndarray [cout * up^d]), ...]
         pool / up: per-layer pooling and ConvolutionUpsample sizes of the 'tog' graph (lib/model.lua:164-226),
         None = all 1 ('default', 'yang'); poolType 'avg' | 'max'; nonlinType 'relu' | 'sigmoid'.
-        banks: multi-resolution banks (lib/model.lua:252-361), {"num": banksNum, "split_stage": banksSplitStage,
-        "join_stage": banksJoinStage, "aggregate": 'concat' | 'add'} (stages numbered from 1); layers[l] of a
-        banked stage (split_stage <= l + 1 < join_stage) is then a list of num (weight, bias) pairs, bank 1 first.
-        None: a single bank.
+        banks: banks of convolutions (lib/model.lua:252-361), {"num": banksNum, "split_stage": banksSplitStage,
+        "join_stage": banksJoinStage, "aggregate": 'concat' | 'add', "type": 'mres' | 'dilate'} (stages numbered
+        from 1; a missing "type" is banksType 'mres', multi-resolution banks; 'dilate' dilates bank i's convolutions by
+        2^(i-1) at full resolution); layers[l] of a banked stage (split_stage <= l + 1 < join_stage) is then a list of
+        num (weight, bias) pairs, bank 1 first.  None: a single bank.
         inputChannels ({"pDiv", "UDiv", "div", "flags"} -> bool, missing keys at their defaults pDiv, div, flags),
         normalizeInput, normalizeInputFunc ('std' | 'norm'), normalizeInputChan ('UDiv' | 'pDiv' | 'div') and
         addPressureSkip are the mconf keys of lib/model.lua:27-150, :357-387; layers[0] takes the selected channels and
@@ -68,6 +69,7 @@ class ProjectionModel:
         self.banks = dict(banks) if banks is not None else None
         if banks is not None:
             assert banks["aggregate"] in ("concat", "add"), "banksAggregateMethod must be 'concat' or 'add'"
+            assert banks.get("type", "mres") in ("mres", "dilate"), "banksType must be 'mres' or 'dilate'"
         self._keep = []
         cin = (C.c_int32 * n)()
         cout = (C.c_int32 * n)()
@@ -108,10 +110,10 @@ class ProjectionModel:
                 1 if nonlinType == "sigmoid" else 0)
         cb = None
         if banks is not None:
-            cb = _lib.CnnBanks(int(banks["num"]), int(banks["split_stage"]), int(banks["join_stage"]),
-                               1 if banks["aggregate"] == "add" else 0)
-        self.ctx.check(self.ctx.lib.tfl_cnn_create_model(*args, C.byref(cb) if cb is not None else None, C.byref(cin_),
-                                                         wp, bp, C.byref(h)))
+            cb = _lib.CnnBanksEx(int(banks["num"]), int(banks["split_stage"]), int(banks["join_stage"]),
+                                 1 if banks["aggregate"] == "add" else 0, 1 if banks.get("type") == "dilate" else 0)
+        self.ctx.check(self.ctx.lib.tfl_cnn_create_model_ex(*args, C.byref(cb) if cb is not None else None,
+                                                            C.byref(cin_), wp, bp, C.byref(h)))
         self.h = h
         self.last_scale = None
 
@@ -124,8 +126,8 @@ class ProjectionModel:
         architecture.  Options and modules the library does not compute raise ValueError naming them."""
         from . import torch7
         ref = torch7.load_reference_model(model_path, mconf_path)
-        opts = torch7.model_options(ref["mconf"], inputs=True)
-        stages = torch7.graph_stages(ref["model"])
+        opts = torch7.model_options(ref["mconf"], inputs=True, dilate=True)
+        stages = torch7.graph_stages(ref["model"], dilate=opts.get("banks", {}).get("type") == "dilate")
         torch7.check_stages(stages, ref["mconf"], opts)
         return cls(stages, ref["is3D"], device=device, **opts), ref["mconf"]
 

@@ -86,8 +86,9 @@ def make_model(is3d=True, seed=4321, model_type="default", banks=None, inputs=No
     'yang'), Torch `reset` convention uniform +-1/sqrt(fan_in).  Inputs: pDiv, div, occupancy
     (lib/default_conf.lua:76-81).  'tog' layers carry pooling / ConvolutionUpsample sizes: the weights of
     an upsampling layer have cout * up^d output channels.
-    banks: {"num", "split_stage", "join_stage", "aggregate"} (lib/model.lua:252-361); a banked stage's entry
-    in "layers" is then a list of num (weight, bias) pairs, and a 'concat' join stage takes num x the channels.
+    banks: {"num", "split_stage", "join_stage", "aggregate"[, "type"]} (lib/model.lua:252-361); a banked stage's
+    entry in "layers" is then a list of num (weight, bias) pairs, and a 'concat' join stage takes num x the channels.
+    "type" ('mres' or 'dilate') is carried through; both types draw the same weights.
     inputs: the input-block keywords of model.ProjectionModel (inputChannels, normalizeInput*, addPressureSkip),
     kept under "inputs"; the first layer takes the selected channels, the last one more with addPressureSkip."""
     rs = np.random.RandomState(seed)

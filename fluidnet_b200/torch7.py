@@ -231,6 +231,33 @@ _ALLOWED = {
     "cudnn.VolumetricMaxPooling",
 }
 
+# The convolutions of banks 2..N of a banksType 'dilate' model (lib/model_utils.lua:122-146).
+_DILATED = {"nn.SpatialDilatedConvolution", "nn.VolumetricDilatedConvolution"}
+
+
+def _check_dilation(conv, cls, bank):
+    """banksType 'dilate' (lib/model.lua:319-322, lib/model_utils.lua:122-146): the convolution of bank i >= 2 is an
+    nn.{Spatial,Volumetric}DilatedConvolution with dilation 2^(i-1) on every axis, stride 1 and padding
+    2^(i-1) (k-1)/2; bank 1's convolutions and the ones outside the banks are ordinary ones."""
+    where = "bank %d's convolution" % bank if bank else "the final convolution"
+    if cls not in _DILATED:
+        if bank and bank > 1:
+            raise ValueError("torch7 model: %s of a banksType 'dilate' model is %s, not a dilated convolution"
+                             % (where, cls))
+        return
+    if not bank or bank == 1:
+        raise ValueError("torch7 model: %s is %s; only banks 2.. of a banksType 'dilate' model are dilated"
+                         % (where, cls))
+    d = 2 ** (bank - 1)
+    for a in (("T", "W", "H") if cls == "nn.VolumetricDilatedConvolution" else ("W", "H")):
+        k = int(conv["k" + a])
+        got = tuple(None if conv.get(f) is None else int(conv.get(f)) for f in ("dilation" + a, "pad" + a, "d" + a))
+        want = (d, d * (k - 1) // 2, 1)
+        if got != want:
+            raise ValueError("torch7 model: %s (%s) has (dilation, pad, stride) %s = %s on axis %s; banksType "
+                             "'dilate' gives %s" % (where, cls, "dilation%s, pad%s, d%s" % (a, a, a), got, a, want))
+
+
 # (osize, ksize, psize, usize) per modelType, lib/model.lua:163-239.
 _ARCH = {
     (False, "default"): ([16, 16, 16, 16, 1], [3, 3, 3, 3, 1], [1] * 5, [1] * 5),
@@ -256,11 +283,13 @@ def _node_modules(model):
     return out
 
 
-def graph_stages(model):
+def graph_stages(model, dilate=False):
     """The convolutions of a reference gModule grouped by stage: [[(weight, bias) of bank 1, bank 2, ...], ...].
     Each convolution is assigned from its node's annotation "Bank i: conv stage l" (lib/model.lua:337); the final
     convolution has none.  Raises ValueError, naming it, for a module outside the graphs the library computes
-    (batch normalisation, gated or dilated convolutions, low-rank convolution Sequentials, ...)."""
+    (batch normalisation, gated convolutions, low-rank convolution Sequentials, ...).  Dilated convolutions are such a
+    module unless dilate=True, which reads a banksType 'dilate' model: bank i >= 2's convolutions must then be dilated
+    by 2^(i-1) (see _check_dilation) and all others undilated."""
     mods = _node_modules(model)
     if not mods:
         raise ValueError("torch7 model: not an nngraph gModule (no forwardnodes)")
@@ -268,7 +297,7 @@ def graph_stages(model):
     final = []
     for mod, name in mods:
         cls = mod.cls if isinstance(mod, T7Object) else type(mod).__name__
-        if cls not in _ALLOWED:
+        if cls not in _ALLOWED and not (dilate and cls in _DILATED):
             raise ValueError("torch7 model: module %s is not supported by this library" % cls)
         convs = []
         _walk(mod, set(), convs)
@@ -283,6 +312,8 @@ def graph_stages(model):
         if len(layer) != 1:
             raise ValueError("torch7 model: module %s holds %d convolutions" % (cls, len(layer)))
         m = _CONV_STAGE.match(name or "")
+        if dilate:
+            _check_dilation(convs[0], cls, int(m.group(1)) if m else None)
         if m:
             key = (int(m.group(2)), int(m.group(1)))
             if key in found:
@@ -359,11 +390,13 @@ def input_options(mconf):
             "normalizeInputChan": chan, "addPressureSkip": skip}
 
 
-def model_options(mconf, n_stages=None, inputs=False):
+def model_options(mconf, n_stages=None, inputs=False, dilate=False):
     """ProjectionModel keyword arguments for a reference mconf (lib/default_conf.lua, lib/model.lua:27-401):
     pool / up from modelType, poolType, nonlinType, banks, normalizeInputThreshold, and with inputs=True the input
     block (input_options).  Raises ValueError, naming the option, for anything the library does not compute.  Without
-    inputs=True a non-default input block is refused too: a caller that drops those keys would build another model."""
+    inputs=True a non-default input block is refused too: a caller that drops those keys would build another model.
+    Likewise banksType 'dilate' is accepted with dilate=True only (banks["type"] = 'dilate'; the file's convolutions
+    then come from graph_stages(model, dilate=True))."""
     def opt(key, default=None):
         return mconf.get(key, default)
 
@@ -401,8 +434,11 @@ def model_options(mconf, n_stages=None, inputs=False):
            "normalizeInputThreshold": float(opt("normalizeInputThreshold", 1e-5))}
     num = int(opt("banksNum", 1))
     if num > 1:
-        if opt("banksType", "mres") != "mres":
-            refuse("banksType = %r" % opt("banksType"))
+        btype = opt("banksType", "mres")
+        if btype == "dilate" and not dilate:
+            refuse("banksType = 'dilate' (model_options(mconf, dilate=True) builds it)")
+        if btype not in ("mres", "dilate"):
+            refuse("banksType = %r" % btype)
         if opt("banksWeightShare"):
             refuse("banksWeightShare = true")
         agg = opt("banksAggregateMethod", "concat")
@@ -410,6 +446,11 @@ def model_options(mconf, n_stages=None, inputs=False):
             refuse("banksAggregateMethod = %r" % agg)
         out["banks"] = {"num": num, "split_stage": int(opt("banksSplitStage", 1)),
                         "join_stage": int(opt("banksJoinStage", 3)), "aggregate": agg}
+        if btype == "dilate":
+            out["banks"]["type"] = "dilate"
+            s, j = out["banks"]["split_stage"], out["banks"]["join_stage"]
+            if any(u > 1 for u in usize[s - 1:j - 1]):                                  # model_utils.lua:125
+                raise ValueError("mconf: banksType = 'dilate': upsampling not supported for dilated convolutions.")
     if inputs:
         out.update(input_options(mconf))
     return out

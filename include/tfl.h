@@ -250,6 +250,26 @@ int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
                          const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                          int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
                          const float* const* weights, const float* const* biases, tfl_cnn** out);
+/* Banks of either type: tfl_cnn_banks plus dilate = 0 for banksType 'mres', 1 for 'dilate' (lib/model.lua:279-285,
+ * :300-303, :319-322; lib/model_utils.lua:122-146).  Dilated banks build no pyramid: every bank takes the hidden layer
+ * of the split stage as it is, bank i's convolutions in stages split .. join-1 are dilated by 2^(i-1) on every axis
+ * (stride 1, padding 2^(i-1) (k-1)/2, so each bank stays at bank 1's resolution), each followed by its non-linearity
+ * and pooling, and the join concatenates or sums the banks without upsampling.  The weights are laid out as for
+ * 'mres'.  The grid needs no divisibility beyond what pooling asks; up[l] > 1 in a banked stage is refused
+ * ("upsampling not supported for dilated convolutions.").  num == 1 is the single-bank graph. */
+typedef struct tfl_cnn_banks_ex {
+  int32_t num, split_stage, join_stage, aggregate_add;
+  int32_t dilate;
+} tfl_cnn_banks_ex;
+/* tfl_cnn_create_model with tfl_cnn_banks_ex (dilate = 0: exactly tfl_cnn_create_model).  Dilated banks run on whole
+ * grids (tfl_cnn_project, tfl_simulate_step, step graphs, tfl_host_sim_step): on the fp32 path for every graph, and
+ * for the 3-D 'default' graph with split_stage 1 and join_stage 3 (num <= 8) on the tensor cores (3xTF32 by default,
+ * TF32), each dilated bank as 8^(i-1) ordinary convolutions on its phase sub-grids.  The z-slab entry points refuse
+ * them. */
+int tfl_cnn_create_model_ex(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                            int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                            const float* const* weights, const float* const* biases, tfl_cnn** out);
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* cnn);
 /* Arithmetic of the convolution stack: 0 = fp32 FMA on the CUDA cores; 1 = TF32 tensor cores
  * (wgmma, fp32 accumulate); 2 = 3xTF32 tensor cores (error-compensated split, fp32-class
