@@ -39,6 +39,11 @@ class CnnInputs(C.Structure):
                 ("norm_func", C.c_int32), ("norm_chan", C.c_int32), ("pressure_skip", C.c_int32)]
 
 
+class CnnNorm(C.Structure):
+    _fields_ = [("relu6", C.c_int32), ("batch_norm", C.c_int32), ("batch_stats", C.c_int32),
+                ("bn", C.POINTER(C.POINTER(C.c_float))), ("eps", C.POINTER(C.c_float))]
+
+
 class State(C.Structure):
     _fields_ = [(n, Grid) for n in ("p", "U", "flags", "density", "U_bc", "U_bc_inv_mask",
                                     "density_bc", "density_bc_inv_mask", "p_bc", "p_bc_inv_mask",
@@ -56,7 +61,7 @@ SYMBOLS = [
     "tfl_solve_linear_system_jacobi", "tfl_solve_linear_system_pcg", "tfl_precond_from_string", "tfl_normalize_pressure_mean",
     "tfl_volumetric_up_sampling_nearest_forward", "tfl_rectangular_blur", "tfl_signed_distance_field", "tfl_velocity_divergence_backward",
     "tfl_velocity_update_backward", "tfl_volumetric_up_sampling_nearest_backward", "tfl_empty_domain", "tfl_flags_to_occupancy", "tfl_apply_bc",
-    "tfl_clamp", "tfl_cnn_create", "tfl_cnn_create_graph", "tfl_cnn_create_banked", "tfl_cnn_create_model", "tfl_cnn_create_model_ex", "tfl_cnn_destroy", "tfl_cnn_set_mode", "tfl_cnn_get_mode", "tfl_cnn_project", "tfl_simulate_step",
+    "tfl_clamp", "tfl_cnn_create", "tfl_cnn_create_graph", "tfl_cnn_create_banked", "tfl_cnn_create_model", "tfl_cnn_create_model_ex", "tfl_cnn_create_model_norm", "tfl_cnn_destroy", "tfl_cnn_set_mode", "tfl_cnn_get_mode", "tfl_cnn_project", "tfl_simulate_step",
     "tfl_host_sim_create", "tfl_host_sim_destroy", "tfl_host_sim_step",
     "tfl_step_graph_create", "tfl_step_graph_launch", "tfl_step_graph_destroy",
     "tfl_comm_unique_id", "tfl_comm_init", "tfl_comm_destroy", "tfl_slab_sim_create", "tfl_slab_sim_destroy",
@@ -138,6 +143,11 @@ def load():
                                             C.c_int, C.POINTER(CnnBanksEx), C.POINTER(CnnInputs),
                                             C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
                                             C.POINTER(C.c_void_p)]
+    lib.tfl_cnn_create_model_norm.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int32), C.POINTER(C.c_int32),
+                                              C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int,
+                                              C.c_int, C.POINTER(CnnBanksEx), C.POINTER(CnnInputs), C.POINTER(CnnNorm),
+                                              C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),
+                                              C.POINTER(C.c_void_p)]
     lib.tfl_cnn_create.argtypes = [C.c_void_p, C.c_int, C.c_int, C.POINTER(C.c_int32),
                                    C.POINTER(C.c_int32), C.POINTER(C.c_int32),
                                    C.POINTER(C.POINTER(C.c_float)), C.POINTER(C.POINTER(C.c_float)),

@@ -13,6 +13,8 @@ constexpr char kSlabTcOnly[] =
     "split at stage 1 and joined at stage 3, in mode 1 or 2)";
 constexpr char kSlabDilate[] =
     "the z-slab projection does not run banksType 'dilate' (dilated banks run on whole grids only)";
+constexpr char kSlabBatchNorm[] =
+    "the z-slab projection does not run batch normalization (addBatchNorm models run on whole grids only)";
 constexpr char kSlabDefaultInputs[] =
     "the z-slab projection takes the default input block only (inputChannels pDiv, div, flags; normalizeInput with "
     "'std' of UDiv; no addPressureSkip)";
@@ -41,6 +43,37 @@ std::vector<float> relayout_conv_weights(const float* w, int cin, int cout, int 
   return relaid;
 }
 
+// Convolution wi's batch normalization (c channels) from norm->bn[wi] / eps[wi]: for batch statistics its weight and
+// bias on the device, for running statistics y = a x + c with a = w / sqrt(running_var + eps), c = b - running_mean a
+// (in double, rounded once).
+void bn_running_affine(const tfl_cnn_norm* norm, int wi, int c, double* a, double* cc) {
+  const float* p = norm->bn[wi];
+  for (int ch = 0; ch < c; ch++) {
+    a[ch] = (double)p[ch] / std::sqrt((double)p[3 * c + ch] + (double)norm->eps[wi]);
+    cc[ch] = (double)p[c + ch] - (double)p[2 * c + ch] * a[ch];
+  }
+}
+int cnn_upload_bn(tfl_ctx* ctx, tfl_cnn* m, const tfl_cnn_norm* norm, int wi, int c) {
+  const float* p = norm->bn[wi];
+  if (!p) return fail(ctx, "cnn: addBatchNorm: the batch normalization parameters of convolution %d are missing", wi + 1);
+  const float eps = norm->eps[wi];
+  if (!(eps >= 0.0f)) return fail(ctx, "cnn: batch normalization eps of convolution %d must be >= 0 (got %g)", wi + 1, eps);
+  std::vector<float> h(2 * c);
+  std::vector<double> a(c), cc(c);
+  if (!m->bn_batch) bn_running_affine(norm, wi, c, a.data(), cc.data());
+  for (int ch = 0; ch < c; ch++) {
+    h[ch] = m->bn_batch ? p[ch] : (float)a[ch];
+    h[c + ch] = m->bn_batch ? p[c + ch] : (float)cc[ch];
+  }
+  float* d = nullptr;
+  if (cudaMalloc((void**)&d, 2 * c * 4) != cudaSuccess) return fail(ctx, "cnn: cudaMalloc failed");
+  cudaMemcpy(d, h.data(), 2 * c * 4, cudaMemcpyHostToDevice);
+  (m->bn_batch ? m->bn_wb : m->bn_ac).push_back(d);
+  m->bn_eps.push_back(eps);
+  m->bn_max_c = std::max(m->bn_max_c, c);
+  return 0;
+}
+
 // A layer-1 weight [8][cin][3][3][3] zero-padded to [8][8][3][3][3] (the two-plane input of a set with UDiv).
 std::vector<float> pad_cin8(const float* w, int cin) {
   std::vector<float> padded(8 * 8 * 27, 0.0f);
@@ -66,7 +99,7 @@ std::vector<float> concat_slice(const float* w, int nbanks, int i) {
 // make_conv_tc_phase_geo(.., i)) rather than multi-resolution banks.
 void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org, int zoff, int nbanks, bool add,
                     float* part, float* p_net, float* const* wj, const float* bias, const float* tail, int split,
-                    const ConvTcGeo& g, cudaStream_t st, bool phases = false) {
+                    const ConvTcGeo& g, cudaStream_t st, bool phases = false, const TcEpi& ep = TcEpi()) {
   auto src_of = [&](int first, int n, int mode) {
     TcJoinSrc js = {};
     for (int k = 0; k < n; k++) {
@@ -82,11 +115,11 @@ void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org
     return js;
   };
   if (add) {
-    launch_conv3_tc_join(src_of(0, nbanks, 0), p_net, wj[0], bias, tail, split, g, st);
+    launch_conv3_tc_join(src_of(0, nbanks, 0), p_net, wj[0], bias, tail, split, g, st, ep);
   } else {
     for (int i = nbanks - 1; i >= 0; i--)
       launch_conv3_tc_join(src_of(i, 1, nbanks == 1 ? 0 : (i == nbanks - 1 ? 1 : (i > 0 ? 2 : 3))), p_net, wj[i], bias,
-                           tail, split, g, st);
+                           tail, split, g, st, ep);
   }
 }
 
@@ -121,6 +154,7 @@ int finish_debug(tfl_ctx* ctx, const char* what) {
 // planes short of the local end), which a halo of 2 margin + 2 provides from margin = 3 s / 2 on.
 int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, int nx, int zoff, int nz, int own_lo,
                    int own_hi) {
+  if (m->bn) return fail(ctx, "slab: %s", kSlabBatchNorm);
   if (m->bank_dilate) return fail(ctx, "slab: %s", kSlabDilate);
   if (!m->default_inputs) return fail(ctx, "slab: %s", kSlabDefaultInputs);
   if (!m->tc_ok || m->mode == 0) return fail(ctx, "slab: %s", kSlabTcOnly);
@@ -203,6 +237,8 @@ int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
 static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo, int p_hi) {
   const ConvTcGeo& tg = m->act_geo;
   const int split = m->mode == 2 ? 1 : 0, nbk = m->nbanks, zoff = m->act_zoff;
+  TcEpi act;                                  // relu6 (banked models with batch normalization run on the fp32 path)
+  act.relu6 = m->nonlin == 3;
   const float* in[kTcMaxBanks];
   const float* l2[kTcMaxBanks];
   ConvTcGeo geo[kTcMaxBanks];
@@ -234,18 +270,19 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
       g1.z_lo = std::max(0, c_lo - 1); g1.z_hi = std::min(geo[i].nz, c_hi + 1);
     }
     launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, m->tc_planes, 0, split,
-                    g1, st);
+                    g1, st, act);
     // a phase shorter than the sub-grid (d does not divide an axis): its extra voxels are padding for layer 2
     if (m->bank_dilate && i > 0 && ((tg.nx | tg.ny | tg.nz) & ((1 << i) - 1)))
       launch_tc_phase_zero(o1, geo[i], i, tg, st);
-    launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, g2, st);
+    launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, g2, st,
+                    act);
     l2[i] = o2;
   }
   ConvTcGeo g3 = tg;
   g3.z_lo = std::max(0, p_lo);
   g3.z_hi = std::min(tg.nz, p_hi);
   launch_tc_join(l2, geo, org, zoff, nbk, m->bank_add, m->part, p_net, m->wBj[split].data(), m->b[m->conv0[2]],
-                 m->tail, split, g3, st, m->bank_dilate != 0);
+                 m->tail, split, g3, st, m->bank_dilate != 0, act);
 }
 
 // The three 3x3x3 layers (+ fused 1x1x1 tail) on tensor cores: act[0] -> act[1] -> act[2] -> p_net.
@@ -263,9 +300,42 @@ void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo, int p_h
   g3.z_lo = std::max(0, p_lo);     g3.z_hi = std::min(tg.nz, p_hi);
   g2.z_lo = std::max(0, p_lo - 1); g2.z_hi = std::min(tg.nz, p_hi + 1);
   g1.z_lo = std::max(0, p_lo - 2); g1.z_hi = std::min(tg.nz, p_hi + 2);
-  launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, m->tc_planes, 0, split, g1, st);
-  launch_conv3_tc(m->act[1], m->act[2], nullptr, m->wBk[split][1], m->b[1], nullptr, 2, 0, split, g2, st);
-  launch_conv3_tc(m->act[2], nullptr, p_net, m->wBj[split][0], m->b[2], m->tail, 2, 1, split, g3, st);
+  TcEpi e1, e2, e3;
+  e1.relu6 = e2.relu6 = e3.relu6 = m->nonlin == 3;
+  if (m->bn && !m->bn_batch) {
+    // running statistics: BN1 / BN2 in the producing epilogues (after the activation, valid voxels only: the zero
+    // padding of the next layer lies after BN), BN3 / BN4 folded into the tail at creation
+    e1.ac = m->bn_ac[0];
+    e2.ac = m->bn_ac[1];
+  }
+  if (!m->bn_batch) {
+    launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, m->tc_planes, 0, split, g1, st, e1);
+    launch_conv3_tc(m->act[1], m->act[2], nullptr, m->wBk[split][1], m->b[1], nullptr, 2, 0, split, g2, st, e2);
+    launch_conv3_tc(m->act[2], nullptr, p_net, m->wBj[split][0], m->b[2], m->tail, 2, 1, split, g3, st, e3);
+    return;
+  }
+  // Batch statistics (whole grids only): each BN needs its layer's whole output first.  Layers 1 and 2: statistics
+  // of the interior, then y = a x + c in place on it; layer 3 writes its output to act[1] (free again), and the tail
+  // runs as two passes over it -- pass A accumulates BN4's statistics of h4 = act(w4 BN3(h3) + b4), pass B
+  // recomputes h4 and writes p_net = w5 BN4(h4) + b5.
+  double* part = m->bn_part;
+  float* ac = m->bn_tcac;                     // [4][2][8]
+  const long long count = (long long)tg.nb * tg.nz * tg.ny * tg.nx;
+  auto stats = [&](const float* buf, int l) {
+    launch_tc_bn_stats(buf, tg, part, st);
+    launch_bn_finalize(part, 8, count, m->bn_wb[l], m->bn_wb[l] + 8, m->bn_eps[l], ac + 16 * l, nullptr, st);
+  };
+  launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, m->tc_planes, 0, split, tg, st, e1);
+  stats(m->act[1], 0);
+  launch_tc_bn_apply(m->act[1], tg, ac, st);
+  launch_conv3_tc(m->act[1], m->act[2], nullptr, m->wBk[split][1], m->b[1], nullptr, 2, 0, split, tg, st, e2);
+  stats(m->act[2], 1);
+  launch_tc_bn_apply(m->act[2], tg, ac + 16, st);
+  launch_conv3_tc(m->act[2], m->act[1], nullptr, m->wBj[split][0], m->b[2], nullptr, 2, 0, split, tg, st, e3);
+  stats(m->act[1], 2);
+  launch_tc_bn_tail(m->act[1], tg, ac + 32, m->tail, e3.relu6, 0, part, nullptr, nullptr, st);
+  launch_bn_finalize(part, 8, count, m->bn_wb[3], m->bn_wb[3] + 8, m->bn_eps[3], ac + 48, nullptr, st);
+  launch_tc_bn_tail(m->act[1], tg, ac + 32, m->tail, e3.relu6, 1, nullptr, ac + 48, p_net, st);
 }
 
 extern "C" {
@@ -284,17 +354,23 @@ int tfl_cnn_create(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, co
 static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                            int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate, const tfl_cnn_inputs* inputs,
-                           const float* const* weights, const float* const* biases, tfl_cnn** out);
+                           const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
+                           tfl_cnn** out);
 static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                               const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                               int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                              const tfl_cnn_inputs* inputs, const float* const* weights, const float* const* biases,
-                              tfl_cnn** out);
+                              const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
+                              const float* const* biases, tfl_cnn** out);
 static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                                  const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                                  int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                                 const tfl_cnn_inputs* inputs, const float* const* weights,
+                                 const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
                                  const float* const* biases, tfl_cnn** out);
+static int cnn_create_model_ex_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                                    const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                                    int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                                    const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
+                                    tfl_cnn** out);
 static const tfl_cnn_inputs kDefaultInputs = {1, 0, 1, 1, 0, 0, 0};
 
 int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
@@ -304,7 +380,7 @@ int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   return cnn_create_impl(ctx, is_3d, n_layers, cin, cout_logical, ksize, pool, up, pool_is_max, nonlin_sigmoid,
-                         nullptr, 0, &kDefaultInputs, weights, biases, out);
+                         nullptr, 0, &kDefaultInputs, nullptr, weights, biases, out);
 }
 
 int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
@@ -314,7 +390,7 @@ int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* 
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, 0,
-                            &kDefaultInputs, weights, biases, out);
+                            &kDefaultInputs, nullptr, weights, biases, out);
 }
 
 int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
@@ -324,7 +400,7 @@ int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   return cnn_create_model_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, 0,
-                               inputs, weights, biases, out);
+                               inputs, nullptr, weights, biases, out);
 }
 
 int tfl_cnn_create_model_ex(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
@@ -333,18 +409,42 @@ int tfl_cnn_create_model_ex(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t
                             const float* const* weights, const float* const* biases, tfl_cnn** out) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
+  return cnn_create_model_ex_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
+                                  inputs, nullptr, weights, biases, out);
+}
+
+int tfl_cnn_create_model_norm(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                              int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                              const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
+                              tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (norm && norm->relu6 && nonlin_sigmoid)
+    return fail(ctx, "cnn: nonlinType is either 'relu6' or 'sigmoid', not both");
+  if (norm && norm->batch_norm && (!norm->bn || !norm->eps))
+    return fail(ctx, "cnn: addBatchNorm needs the batch normalization parameters (bn) and eps of every module");
+  return cnn_create_model_ex_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
+                                  inputs, norm, weights, biases, out);
+}
+
+static int cnn_create_model_ex_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                                    const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                                    int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                                    const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
+                                    tfl_cnn** out) {
   if (banks && banks->dilate != 0 && banks->dilate != 1)
     return fail(ctx, "cnn: banks dilate must be 0 ('mres') or 1 ('dilate') (got %d)", banks->dilate);
   tfl_cnn_banks b = {};
   if (banks) b = {banks->num, banks->split_stage, banks->join_stage, banks->aggregate_add};
   return cnn_create_model_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid,
-                               banks ? &b : nullptr, banks ? banks->dilate : 0, inputs, weights, biases, out);
+                               banks ? &b : nullptr, banks ? banks->dilate : 0, inputs, norm, weights, biases, out);
 }
 
 static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                                  const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                                  int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                                 const tfl_cnn_inputs* inputs, const float* const* weights,
+                                 const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
                                  const float* const* biases, tfl_cnn** out) {
   const tfl_cnn_inputs in = inputs ? *inputs : kDefaultInputs;
   // lib/model.lua:27-150 and :357-361; checkYangSettings, lib/model_utils.lua:211-227.
@@ -370,14 +470,14 @@ static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const in
                      "resolution, which needs a 1x1 last convolution without upsampling (lib/model.lua:357-361; "
                      "not 'tog')");
   return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                            dilate, &in, weights, biases, out);
+                            dilate, &in, norm, weights, biases, out);
 }
 
 static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
                               const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                               int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                              const tfl_cnn_inputs* inputs, const float* const* weights, const float* const* biases,
-                              tfl_cnn** out) {
+                              const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
+                              const float* const* biases, tfl_cnn** out) {
   if (banks) {     // the assertions of lib/model.lua:246-252 (checked whatever banksNum is)
     if (banks->num < 1) return fail(ctx, "cnn: banksNum >= 1 failed (got %d)", banks->num);
     if (!(banks->split_stage < banks->join_stage))
@@ -395,13 +495,14 @@ static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32
     if (banks->num == 1) banks = nullptr;
   }
   return cnn_create_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                         banks ? dilate : 0, inputs, weights, biases, out);
+                         banks ? dilate : 0, inputs, norm, weights, biases, out);
 }
 
 static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                            int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate, const tfl_cnn_inputs* inputs,
-                           const float* const* weights, const float* const* biases, tfl_cnn** out) {
+                           const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
+                           tfl_cnn** out) {
   if (!out || n_layers < 1) return fail(ctx, "cnn: bad arguments");
   const tfl_cnn_inputs& in = *inputs;
   const int in_sel = (in.p_div ? kCnnInPDiv : 0) | (in.u_div ? kCnnInUDiv : 0) | (in.div ? kCnnInDiv : 0);
@@ -438,7 +539,11 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   }
   cin = cin_net.data();
   if (nbanks > 1) plain = false;
+  const bool relu6 = norm && norm->relu6, bn = norm && norm->batch_norm;
+  if (relu6 || bn) plain = false;     // the stage loop applies BN; relu6 is activation code 3
   tfl_cnn* m = new tfl_cnn();
+  m->bn = bn;
+  m->bn_batch = bn && norm->batch_stats;
   m->in_sel = in_sel;
   m->in_ch = in_ch;
   m->norm_func = in.normalize ? (in.norm_func == 1 ? kCnnScaleNorm : kCnnScaleStd) : kCnnScaleOne;
@@ -450,7 +555,7 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   m->tc_planes = (in_sel & kCnnInUDiv) ? 2 : 1;
   m->plain = plain;
   m->pool_is_max = pool_is_max ? 1 : 0;
-  m->nonlin = nonlin_sigmoid ? 2 : 1;
+  m->nonlin = nonlin_sigmoid ? 2 : (relu6 ? 3 : 1);
   m->is3d = is_3d ? 1 : 0;
   m->n_layers = n_layers;
   m->nbanks = nbanks;
@@ -486,6 +591,10 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
       cudaMemcpy(db, biases[wi], cout[l] * 4, cudaMemcpyHostToDevice);
       m->cin.push_back(cin[l]); m->cout.push_back(cout[l]); m->ks.push_back(ksize[l]);
       m->w.push_back(dw); m->b.push_back(db);
+      if (bn && l < n_layers - 1 && cnn_upload_bn(ctx, m, norm, wi, cout_logical[l])) {
+        tfl_cnn_destroy(ctx, m);
+        return 1;
+      }
     }
     if (cout[l] > m->max_c) m->max_c = cout[l];
   }
@@ -509,7 +618,7 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   // Tensor-core eligibility: the 3-D 'default' graph (lib/model.lua:219-226), single-bank or with banks (either type)
   // split before stage 1 and joined before stage 3.
   static const int want[5][3] = {{0, 8, 3}, {8, 8, 3}, {8, 8, 3}, {8, 8, 1}, {8, 1, 1}};   // cin[0]: any input set
-  m->tc_ok = is_3d && n_layers == 5 && !nonlin_sigmoid &&
+  m->tc_ok = is_3d && n_layers == 5 && !nonlin_sigmoid && !(bn && nbanks > 1) &&
              (nbanks == 1 || (bsplit == 0 && bjoin == 2 && nbanks <= kTcMaxBanks));
   for (int l = 0; m->tc_ok && l < 5; l++) {
     const int want_cin = l == 0 ? in_ch : (l == 2 && !m->bank_add) ? 8 * nbanks : want[l][0];
@@ -533,6 +642,31 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
     memcpy(tail.data() + 64, biases[m->conv0[3]], 8 * 4);
     memcpy(tail.data() + 72, weights[m->conv0[4]], 8 * 4);
     tail[80] = biases[m->conv0[4]][0];
+    if (bn && !m->bn_batch) {
+      // running statistics: BN3 (after layer 3's activation) into w4 / b4, BN4 (after layer 4's) into w5 / b5, exact in
+      // real arithmetic: w4 (a3 h + c3) + b4 = (w4 a3) h + (b4 + w4 c3), w5 (a4 h + c4) + b5 = (w5 a4) h + (b5 + w5 c4)
+      double a3[8], c3[8], a4[8], c4[8];
+      bn_running_affine(norm, 2, 8, a3, c3);
+      bn_running_affine(norm, 3, 8, a4, c4);
+      double b5 = tail[80];
+      for (int o = 0; o < 8; o++) {
+        double b4 = tail[64 + o];
+        for (int c = 0; c < 8; c++) {
+          b4 += (double)tail[o * 8 + c] * c3[c];
+          tail[o * 8 + c] = (float)((double)tail[o * 8 + c] * a3[c]);
+        }
+        tail[64 + o] = (float)b4;
+        b5 += (double)tail[72 + o] * c4[o];
+        tail[72 + o] = (float)((double)tail[72 + o] * a4[o]);
+      }
+      tail[80] = (float)b5;
+    }
+    if (bn && m->bn_batch &&
+        (cudaMalloc((void**)&m->bn_part, sizeof(double) * 2 * (kBnBlocks + 1) * 8) != cudaSuccess ||
+         cudaMalloc((void**)&m->bn_tcac, sizeof(float) * 4 * 16) != cudaSuccess)) {
+      tfl_cnn_destroy(ctx, m);
+      return fail(ctx, "cnn: cudaMalloc failed");
+    }
     cudaMalloc((void**)&m->tail, tail.size() * 4);
     cudaMemcpy(m->tail, tail.data(), tail.size() * 4, cudaMemcpyHostToDevice);
     m->mode = 2;
@@ -545,6 +679,9 @@ int tfl_cnn_set_mode(tfl_ctx* ctx, tfl_cnn* m, int mode) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!m || mode < 0 || mode > 2) return fail(ctx, "cnn_set_mode: bad arguments");
+  if (mode > 0 && m->bn && m->nbanks > 1)
+    return fail(ctx, "cnn_set_mode: banked models with batch normalization (addBatchNorm) run on the fp32 path; the "
+                     "tensor-core path takes batch normalization on the single-bank 3-D 'default' graph");
   if (mode > 0 && m->nbanks > 1 && !m->tc_ok)
     return fail(ctx, "cnn_set_mode: the tensor-core path covers the 3-D 'default' architecture, single-bank or with "
                      "banks split at stage 1 and joined at stage 3; this banked model runs on the fp32 path");
@@ -607,6 +744,59 @@ int tfl_debug_conv3_tc(tfl_ctx* ctx, const float* in, float* out, float* p_net, 
   if (rc) return rc;
   if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc: %s", cudaGetErrorString(se));
   return 0;
+}
+
+// tfl_debug_conv3_tc_bn: one tensor-core 3x3x3 layer (not the final one) with the batch normalization of the
+// projection network on caller-owned padded buffers (layout as tfl_debug_conv3_tc).  relu6: the epilogue clamps at 6;
+// ep_ac_host ([2][8] a, c, may be NULL): running-statistics BN in the epilogue, y = a act(h) + c on the voxels
+// written; batch = 1: then batch statistics over out's interior (launch_tc_bn_stats, launch_bn_finalize with
+// bn_w_host / bn_b_host [8] (may be NULL: 1 / 0) and eps) and y = a x + c in place on the interior; stats_host
+// ([8][2] mean, biased variance) and ac_host ([2][8]) receive what the finalize computed.  Synchronises.
+int tfl_debug_conv3_tc_bn(tfl_ctx* ctx, const float* in, float* out, const float* w_host, const float* bias_host,
+                          int cin, int split, int relu6, const float* ep_ac_host, int batch, const float* bn_w_host,
+                          const float* bn_b_host, float eps, double* stats_host, float* ac_host, int nb, int nz, int ny,
+                          int nx) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (cin != 3 && cin != 8) return fail(ctx, "debug_conv3_tc_bn: cin must be 3 or 8 (got %d)", cin);
+  if (!in || !out || !w_host || !bias_host || (batch && (!stats_host || !ac_host)))
+    return fail(ctx, "debug_conv3_tc_bn: nil argument");
+  if (bad_grid(nb, nz, ny, nx, 1) || !(eps >= 0.0f)) return fail(ctx, "debug_conv3_tc_bn: bad arguments");
+  const ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
+  float *wB = upload_tc_weights(w_host, cin, split), *bias = nullptr, *ep = nullptr, *wb = nullptr, *ac = nullptr;
+  double *part = nullptr, *stats = nullptr;
+  auto release = [&]() {
+    for (void* p : {(void*)wB, (void*)bias, (void*)ep, (void*)wb, (void*)ac, (void*)part, (void*)stats})
+      if (p) cudaFree(p);
+  };
+  if (!wB || cudaMalloc((void**)&bias, 8 * 4) != cudaSuccess || cudaMalloc((void**)&ep, 16 * 4) != cudaSuccess ||
+      cudaMalloc((void**)&wb, 16 * 4) != cudaSuccess || cudaMalloc((void**)&ac, 16 * 4) != cudaSuccess ||
+      cudaMalloc((void**)&part, sizeof(double) * 2 * (kBnBlocks + 1) * 8) != cudaSuccess ||
+      cudaMalloc((void**)&stats, sizeof(double) * 16) != cudaSuccess) {
+    release();
+    return fail(ctx, "debug_conv3_tc_bn: cudaMalloc failed");
+  }
+  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
+  if (ep_ac_host) cudaMemcpy(ep, ep_ac_host, 16 * 4, cudaMemcpyHostToDevice);
+  if (bn_w_host) cudaMemcpy(wb, bn_w_host, 8 * 4, cudaMemcpyHostToDevice);
+  if (bn_b_host) cudaMemcpy(wb + 8, bn_b_host, 8 * 4, cudaMemcpyHostToDevice);
+  TcEpi e;
+  e.relu6 = relu6 ? 1 : 0;
+  e.ac = ep_ac_host ? ep : nullptr;
+  launch_conv3_tc(in, out, nullptr, wB, bias, nullptr, cin == 3 ? 1 : 2, 0, split, g, ctx->stream, e);
+  if (batch) {
+    launch_tc_bn_stats(out, g, part, ctx->stream);
+    launch_bn_finalize(part, 8, (long long)nb * nz * ny * nx, bn_w_host ? wb : nullptr, bn_b_host ? wb + 8 : nullptr,
+                       eps, ac, stats, ctx->stream);
+    launch_tc_bn_apply(out, g, ac, ctx->stream);
+  }
+  int rc = finish_debug(ctx, "debug_conv3_tc_bn");
+  if (!rc && batch &&
+      (cudaMemcpy(stats_host, stats, sizeof(double) * 16, cudaMemcpyDeviceToHost) != cudaSuccess ||
+       cudaMemcpy(ac_host, ac, 16 * 4, cudaMemcpyDeviceToHost) != cudaSuccess))
+    rc = fail(ctx, "debug_conv3_tc_bn: copy failed");
+  release();
+  return rc;
 }
 
 // tfl_debug_conv3_tc_dilated: one tensor-core 3x3x3 layer (not the final one) dilated by 2^sh the way a dilated bank
@@ -895,6 +1085,42 @@ int tfl_debug_bank_join(tfl_ctx* ctx, const float* const* banks, int nbanks, flo
   return finish_debug(ctx, "debug_bank_join");
 }
 
+// tfl_debug_bn: batch normalization with batch statistics (launch_bn_stats, _finalize, _apply) in place on device x
+// [nb][c][n] whose batch entries lie bstride floats apart; w_host / b_host [c] (may be NULL: 1 / 0).  stats_host
+// ([c][2] doubles: mean, biased variance) and ac_host ([2][c] floats: a, c of y = a x + c) receive what the finalize
+// computed.  Nothing but the nb c n values is written.
+int tfl_debug_bn(tfl_ctx* ctx, float* x, int nb, int c, int64_t n, int64_t bstride, const float* w_host,
+                 const float* b_host, float eps, double* stats_host, float* ac_host) {
+  DeviceGuard guard_(ctx);
+  if (!ctx) return 1;
+  if (!x || !stats_host || !ac_host) return fail(ctx, "debug_bn: nil argument");
+  if (nb < 1 || c < 1 || n < 1 || bstride < (int64_t)c * n || !(eps >= 0.0f)) return fail(ctx, "debug_bn: bad arguments");
+  float *wb = nullptr, *ac = nullptr;
+  double *part = nullptr, *stats = nullptr;
+  auto release = [&]() {
+    for (void* p : {(void*)wb, (void*)ac, (void*)part, (void*)stats})
+      if (p) cudaFree(p);
+  };
+  if (cudaMalloc((void**)&wb, 2 * c * 4) != cudaSuccess || cudaMalloc((void**)&ac, 2 * c * 4) != cudaSuccess ||
+      cudaMalloc((void**)&part, sizeof(double) * 2 * (kBnBlocks + 1) * c) != cudaSuccess ||
+      cudaMalloc((void**)&stats, sizeof(double) * 2 * c) != cudaSuccess) {
+    release();
+    return fail(ctx, "debug_bn: cudaMalloc failed");
+  }
+  if (w_host) cudaMemcpy(wb, w_host, c * 4, cudaMemcpyHostToDevice);
+  if (b_host) cudaMemcpy(wb + c, b_host, c * 4, cudaMemcpyHostToDevice);
+  launch_bn_stats(x, nb, c, n, bstride, part, ctx->stream);
+  launch_bn_finalize(part, c, (long long)nb * n, w_host ? wb : nullptr, b_host ? wb + c : nullptr, eps, ac, stats,
+                     ctx->stream);
+  launch_bn_apply(x, nb, c, n, bstride, ac, ctx->stream);
+  int rc = finish_debug(ctx, "debug_bn");
+  if (!rc && (cudaMemcpy(stats_host, stats, sizeof(double) * 2 * c, cudaMemcpyDeviceToHost) != cudaSuccess ||
+              cudaMemcpy(ac_host, ac, 2 * c * 4, cudaMemcpyDeviceToHost) != cudaSuccess))
+    rc = fail(ctx, "debug_bn: copy failed");
+  release();
+  return rc;
+}
+
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
@@ -911,6 +1137,10 @@ void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
   }
   for (float* p : m->bact) cudaFree(p);
   if (m->part) cudaFree(m->part);
+  for (float* p : m->bn_wb) cudaFree(p);
+  for (float* p : m->bn_ac) cudaFree(p);
+  if (m->bn_part) cudaFree(m->bn_part);
+  if (m->bn_tcac) cudaFree(m->bn_tcac);
   delete m;
 }
 
@@ -938,6 +1168,9 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
   float* actA = (float*)take(cells * 4 * m->max_c);      // max_c covers max_rel (set at creation)
   float* actB = (float*)take(cells * 4 * m->max_c);
   float* scale = (float*)take(sizeof(float) * g.nb);
+  // batch statistics: the partial sums and (a, c) of one BN module at a time (cnn_scratch_bytes)
+  double* bn_part = (double*)take(sizeof(double) * 2 * (kBnBlocks + 1) * m->bn_max_c);
+  float* bn_ac = (float*)take(sizeof(float) * 2 * m->bn_max_c);
   double* sums = ctx->dscratch + 64;
   cudaStream_t st = ctx->stream;
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
@@ -1045,6 +1278,19 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
       }
       gl.n = (long long)gl.nx * gl.ny * gl.nz;
       gl.gnz = gl.nz; gl.zlo = 0; gl.zhi = gl.nz;
+      if (m->bn && l < m->n_layers - 1) {     // lib/model.lua:343-350: BN closes every stage but the last
+        float* x = (float*)cur;               // one of this call's buffers, or a slot of one
+        const long long bs = out_bstride > 0 ? out_bstride : (long long)chans * gl.n;
+        const float* ac = m->bn_batch ? bn_ac : m->bn_ac[ci];
+        if (m->bn_batch) {
+          launch_bn_stats(x, gl.nb, chans, gl.n, bs, bn_part, st);
+          launch_bn_finalize(bn_part, chans, (long long)gl.nb * gl.n, m->bn_wb[ci], m->bn_wb[ci] + chans,
+                             m->bn_eps[ci], bn_ac, nullptr, st);
+          ctx->launches += 2;
+        }
+        launch_bn_apply(x, gl.nb, chans, gl.n, bs, ac, st);
+        ctx->launches += 1;
+      }
       *result = cur;
       return 0;
     };
@@ -1139,6 +1385,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
 static size_t cnn_scratch_bytes(const tfl_cnn* m, const Geo& g) {
   const size_t cells = (size_t)g.n * g.nb;
   size_t bytes = cells * 4 * (g.nc + m->in_ch + 2 * (size_t)m->max_c) + 4 * g.nb + 8 * 256;
+  bytes += (sizeof(double) * 2 * (kBnBlocks + 1) + sizeof(float) * 2) * (size_t)m->bn_max_c + 2 * 256;
   if (!m->plain) bytes += (size_t)((double)cells * m->max_rel + 64) * 4 + 256;     // third rotating buffer
   for (int i = 1; i < m->nbanks; i++) bytes += cnn_bank_nbufs(m) * (cnn_bank_buf_bytes(m, g, i) + 256);
   return bytes;
@@ -1204,6 +1451,7 @@ int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!m) return fail(ctx, "cnn is nil");
+  if (m->bn) return fail(ctx, "cnn_project_from_sums: %s", kSlabBatchNorm);
   if (m->bank_dilate) return fail(ctx, "cnn_project_from_sums: %s", kSlabDilate);
   if (!m->default_inputs) return fail(ctx, "cnn_project_from_sums: %s", kSlabDefaultInputs);
   if (!m->tc_ok || m->mode == 0) return fail(ctx, "cnn_project_from_sums: %s", kSlabTcOnly);

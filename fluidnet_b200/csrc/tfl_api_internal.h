@@ -95,7 +95,17 @@ struct tfl_cnn {
   // pooling of size `pool` follows the non-linearity.  plain = every pool / up is 1 and the non-linearity is ReLU.
   std::vector<int> pool, up;
   int pool_is_max = 0;
-  int nonlin = 1;            // 1 ReLU, 2 sigmoid (activation codes of tfl_cnn.cu)
+  int nonlin = 1;            // 1 ReLU, 2 sigmoid, 3 ReLU6 (activation codes of tfl_cnn.cu)
+  // batch normalization (tfl_cnn_norm) after every convolution but the last, on its stage's output: per convolution,
+  // bn_wb [2][c] (weight, bias) and eps for batch statistics, or bn_ac [2][c] (a, c of y = a x + c, computed at
+  // creation from the running statistics).  bn_max_c: the most channels of one BN module (sizes the scratch).
+  bool bn = false, bn_batch = false;
+  std::vector<float*> bn_wb, bn_ac;
+  std::vector<float> bn_eps;
+  int bn_max_c = 0;
+  // batch statistics on the tensor cores (run_conv_stack): the partials of one module and the (a, c) of BN1..BN4
+  double* bn_part = nullptr;
+  float* bn_tcac = nullptr;
   bool plain = true;
   double max_rel = 0.0;      // largest channels x (cells relative to the input grid) of any stage
   double bank_rel = 0.0;     // the same over one bank's activations in the banked stages (conv output, pooled)

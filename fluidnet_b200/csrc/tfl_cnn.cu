@@ -7,13 +7,16 @@
 // implementation and the parity anchor for the tensor-core path (tfl_cnn_tc.cu).
 #include "tfl_device.cuh"
 #include "tfl_kernels.h"
+#include "tfl_cnn_tc.h"
 
 namespace tfl {
 
-// Non-linearity between layers (torch.addNonlinearity, lib/model_utils.lua): 0 none, 1 ReLU, 2 sigmoid.
+// Non-linearity between layers (torch.addNonlinearity, lib/model_utils.lua): 0 none, 1 ReLU, 2 sigmoid, 3 ReLU6
+// (nn.ReLU6, min(max(x, 0), 6)).
 __device__ __forceinline__ float activate(float r, int act) {
   if (act == 1) return r < 0.0f ? 0.0f : r;
   if (act == 2) return 1.0f / (1.0f + expf(-r));
+  if (act == 3) return r < 0.0f ? 0.0f : (r > 6.0f ? 6.0f : r);
   return r;
 }
 
@@ -195,6 +198,237 @@ __global__ void k_bank_join(BankPtrs banks, int nbanks, float* __restrict__ out,
   }
 }
 
+// Batch normalization of x [nb][c][n] whose batch entries lie bstride floats apart (a stage's output written in
+// place into its 'concat' slot has bstride > c n).  Batch statistics: block (blk, ch) of k_bn_stats owns the fixed
+// contiguous range blk of channel ch's nb n values and writes its (sum d, sum d^2), d = x - K, in fp64 to slot
+// ch (gridDim.x + 1) + blk; K, the channel's first value, goes to slot ch (gridDim.x + 1) + gridDim.x, so a constant
+// channel has a variance of exactly 0.  k_bn_finalize sums a channel's slots in a fixed order.  No atomics: the
+// result is the same bits on every run.
+constexpr int kBnThreads = 256;
+
+// (s, q) summed over the block in a fixed order; the total is valid in thread 0.
+__device__ __forceinline__ void bn_block_sum(double& s, double& q, double* sh) {
+  for (int o = 16; o > 0; o >>= 1) {
+    s += __shfl_down_sync(0xffffffffu, s, o);
+    q += __shfl_down_sync(0xffffffffu, q, o);
+  }
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  if (lane == 0) {
+    sh[2 * wid] = s;
+    sh[2 * wid + 1] = q;
+  }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    s = 0.0;
+    q = 0.0;
+    for (int w = 0; w < (int)(blockDim.x >> 5); w++) {
+      s += sh[2 * w];
+      q += sh[2 * w + 1];
+    }
+  }
+}
+
+__global__ void __launch_bounds__(kBnThreads)
+k_bn_stats(const float* __restrict__ x, long long n, int nb, long long bstride, double* __restrict__ part) {
+  __shared__ double sh[2 * kBnThreads / 32];
+  const int ch = blockIdx.y;
+  const long long total = (long long)nb * n, chunk = (total + gridDim.x - 1) / gridDim.x;
+  const long long lo = (long long)blockIdx.x * chunk, hi = min(total, lo + chunk);
+  const double K = __ldg(x + ch * n);
+  double s = 0.0, q = 0.0;
+  for (long long b = lo / n; b * n < hi; b++) {        // the block's range, one batch entry at a time
+    const float* xb = x + b * bstride + ch * n;
+    const long long i1 = min(hi, (b + 1) * n) - b * n;
+    for (long long i = max(lo, b * n) - b * n + threadIdx.x; i < i1; i += blockDim.x) {
+      const double d = (double)__ldg(xb + i) - K;
+      s += d;
+      q = fma(d, d, q);
+    }
+  }
+  bn_block_sum(s, q, sh);
+  if (threadIdx.x == 0) {
+    double* slot = part + 2 * ((long long)ch * (gridDim.x + 1) + blockIdx.x);
+    slot[0] = s;
+    slot[1] = q;
+    if (blockIdx.x == 0) {
+      slot[2 * gridDim.x] = K;
+      slot[2 * gridDim.x + 1] = 0.0;
+    }
+  }
+}
+
+// One block per channel: mean and biased variance over `count` values, invstd = 1 / sqrt(var + eps) (0 when
+// var + eps == 0, as THNN), ac[ch] = a = w invstd, ac[c + ch] = b - mean a.  w / b may be null (1 / 0); stats (may be
+// null) gets (mean, var) per channel.  part: [c][nslots + 1][2] as k_bn_stats writes it.
+__global__ void __launch_bounds__(kBnThreads)
+k_bn_finalize(const double* __restrict__ part, int nslots, int c, long long count, const float* __restrict__ w,
+              const float* __restrict__ b, float eps, float* __restrict__ ac, double* __restrict__ stats) {
+  __shared__ double sh[2 * kBnThreads / 32];
+  const int ch = blockIdx.x;
+  const double* pc = part + 2 * (long long)ch * (nslots + 1);
+  double s = 0.0, q = 0.0;
+  for (int i = threadIdx.x; i < nslots; i += blockDim.x) {
+    s += pc[2 * i];
+    q += pc[2 * i + 1];
+  }
+  bn_block_sum(s, q, sh);
+  if (threadIdx.x != 0) return;
+  const double md = s / (double)count;
+  const double mean = pc[2 * nslots] + md;
+  const double var = fmax(q / (double)count - md * md, 0.0);
+  const double ve = var + (double)eps;
+  const double invstd = ve == 0.0 ? 0.0 : 1.0 / sqrt(ve);
+  const double a = (w ? (double)w[ch] : 1.0) * invstd;
+  ac[ch] = (float)a;
+  ac[c + ch] = (float)((b ? (double)b[ch] : 0.0) - mean * a);
+  if (stats) {
+    stats[2 * ch] = mean;
+    stats[2 * ch + 1] = var;
+  }
+}
+
+// y = a x + c in place, per channel.
+__global__ void k_bn_apply(float* __restrict__ x, int c, long long n, long long bstride, const float* __restrict__ ac,
+                           long long total) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const long long cn = (long long)c * n, b = t / cn, r = t - b * cn;
+  const int ch = (int)(r / n);
+  float* p = x + b * bstride + r;
+  *p = fmaf(__ldg(ac + ch), *p, __ldg(ac + c + ch));
+}
+
+
+// ---- batch statistics on the tensor-core path's padded channels-last layout (tfl_cnn_tc.h) ----
+// Block blk owns the fixed contiguous range blk of the nb nz ny interior rows and sums its 8 channels (two float4
+// planes) in fp64, shifted by the values of the first interior voxel, as k_bn_stats does; the slots are those of
+// k_bn_stats, so k_bn_finalize reads them.
+struct TcRows {
+  long long plane, batch;     // float4 per padded plane / batch entry
+  long long rows;             // nb nz ny
+};
+__device__ __forceinline__ TcRows tc_rows(const ConvTcGeo& g) {
+  TcRows r;
+  r.plane = (long long)(g.nz + 2) * g.py * g.px;
+  r.batch = 2 * r.plane;
+  r.rows = (long long)g.nb * g.nz * g.ny;
+  return r;
+}
+// float4 index of row `row`'s voxel x = 0 (first plane)
+__device__ __forceinline__ long long tc_row_base(const ConvTcGeo& g, const TcRows& r, long long row) {
+  const long long b = row / ((long long)g.nz * g.ny), zy = row - b * g.nz * g.ny;
+  const int z = (int)(zy / g.ny), y = (int)(zy - (long long)z * g.ny);
+  return b * r.batch + ((long long)(z + 1) * g.py + (y + 1)) * g.px + 1;
+}
+__device__ __forceinline__ void tc_load8(const float4* buf, const TcRows& r, long long i, float (&v)[8]) {
+  const float4 a = __ldg(buf + i), b = __ldg(buf + i + r.plane);
+  v[0] = a.x; v[1] = a.y; v[2] = a.z; v[3] = a.w; v[4] = b.x; v[5] = b.y; v[6] = b.z; v[7] = b.w;
+}
+// The tail's hidden layer: h4 = act(w4 (a3 h3 + c3) + b4), sTail = w4[64] b4[8] w5[8] b5, ac3 [2][8].
+__device__ __forceinline__ void tc_tail_h4(const float (&h3)[8], const float* sW, const float* sAc3, int relu6,
+                                           float (&h4)[8]) {
+  float x[8];
+#pragma unroll
+  for (int c = 0; c < 8; c++) x[c] = fmaf(sAc3[c], h3[c], sAc3[8 + c]);
+#pragma unroll
+  for (int o = 0; o < 8; o++) {
+    float a = sW[64 + o];
+#pragma unroll
+    for (int c = 0; c < 8; c++) a = fmaf(x[c], sW[o * 8 + c], a);
+    a = a > 0.0f ? a : 0.0f;
+    h4[o] = relu6 && a > 6.0f ? 6.0f : a;
+  }
+}
+// Fixed-order block sums of the 8 channels' (s, q) into part's slot blk, and the shift into the last slot.
+__device__ __forceinline__ void tc_bn_write(double (&s)[8], double (&q)[8], const float (&K)[8], double* sh,
+                                            double* part) {
+#pragma unroll
+  for (int ch = 0; ch < 8; ch++) {
+    __syncthreads();
+    bn_block_sum(s[ch], q[ch], sh);
+    if (threadIdx.x == 0) {
+      double* slot = part + 2 * ((long long)ch * (gridDim.x + 1) + blockIdx.x);
+      slot[0] = s[ch];
+      slot[1] = q[ch];
+      if (blockIdx.x == 0) {
+        slot[2 * gridDim.x] = K[ch];
+        slot[2 * gridDim.x + 1] = 0.0;
+      }
+    }
+  }
+}
+
+// TAIL = false: statistics of buf's 8 channels; TAIL = true: of the tail's h4 (pass A) or, with pass_b, p_net.
+template <bool TAIL>
+__global__ void __launch_bounds__(kBnThreads)
+k_tc_bn_rows(const float4* __restrict__ buf, ConvTcGeo g, const float* __restrict__ ac3, const float* __restrict__ tail,
+             int relu6, int pass_b, double* __restrict__ part, const float* __restrict__ ac4, float* __restrict__ p_net) {
+  __shared__ double sh[2 * kBnThreads / 32];
+  __shared__ float sW[64 + 8 + 8 + 1], sAc[32];
+  if (TAIL) {
+    for (int i = threadIdx.x; i < 81; i += blockDim.x) sW[i] = tail[i];
+    for (int i = threadIdx.x; i < 16; i += blockDim.x) {
+      sAc[i] = ac3[i];
+      if (pass_b) sAc[16 + i] = ac4[i];
+    }
+    __syncthreads();
+  }
+  const TcRows r = tc_rows(g);
+  const long long chunk = (r.rows + gridDim.x - 1) / gridDim.x;
+  const long long lo = (long long)blockIdx.x * chunk, hi = min(r.rows, lo + chunk);
+  float K[8];
+  {
+    float v[8];
+    tc_load8(buf, r, tc_row_base(g, r, 0), v);
+    if (TAIL) tc_tail_h4(v, sW, sAc, relu6, K);
+    else
+#pragma unroll
+      for (int c = 0; c < 8; c++) K[c] = v[c];
+  }
+  double s[8] = {}, q[8] = {};
+  for (long long row = lo; row < hi; row++) {
+    const long long base = tc_row_base(g, r, row);
+    for (int x = threadIdx.x; x < g.nx; x += blockDim.x) {
+      float v[8], h[8];
+      tc_load8(buf, r, base + x, v);
+      if (TAIL) tc_tail_h4(v, sW, sAc, relu6, h);
+      else
+#pragma unroll
+        for (int c = 0; c < 8; c++) h[c] = v[c];
+      if (TAIL && pass_b) {
+        float p = sW[80];
+#pragma unroll
+        for (int o = 0; o < 8; o++) p = fmaf(sW[72 + o], fmaf(sAc[16 + o], h[o], sAc[24 + o]), p);
+        p_net[row * g.nx + x] = p;
+        continue;
+      }
+#pragma unroll
+      for (int c = 0; c < 8; c++) {
+        const double d = (double)h[c] - (double)K[c];
+        s[c] += d;
+        q[c] = fma(d, d, q[c]);
+      }
+    }
+  }
+  if (TAIL && pass_b) return;       // uniform over the launch
+  tc_bn_write(s, q, K, sh, part);
+}
+
+__global__ void k_tc_bn_apply(float4* __restrict__ buf, ConvTcGeo g, const float* __restrict__ ac, long long total) {
+  const long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= total) return;
+  const TcRows r = tc_rows(g);
+  const long long row = t / g.nx;
+  const long long i = tc_row_base(g, r, row) + (t - row * g.nx);
+  float4 a = buf[i], b = buf[i + r.plane];
+  a = make_float4(fmaf(__ldg(ac + 0), a.x, __ldg(ac + 8)), fmaf(__ldg(ac + 1), a.y, __ldg(ac + 9)),
+                  fmaf(__ldg(ac + 2), a.z, __ldg(ac + 10)), fmaf(__ldg(ac + 3), a.w, __ldg(ac + 11)));
+  b = make_float4(fmaf(__ldg(ac + 4), b.x, __ldg(ac + 12)), fmaf(__ldg(ac + 5), b.y, __ldg(ac + 13)),
+                  fmaf(__ldg(ac + 6), b.z, __ldg(ac + 14)), fmaf(__ldg(ac + 7), b.w, __ldg(ac + 15)));
+  buf[i] = a;
+  buf[i + r.plane] = b;
+}
+
 template <int COUT, int KS, bool IS3D, bool DIL>
 static bool conv_launch(const float* in, float* out, const float* w, const float* b, int cin, int act,
                         const Geo& g, int dil, cudaStream_t st) {
@@ -272,6 +506,31 @@ int launch_bank_join(const float* const* banks, int nbanks, float* out, int nb, 
   else
     k_bank_join<false><<<(unsigned)((total + 255) / 256), 256, 0, st>>>(bp, nbanks, out, c, nz, ny, nx, is3d, add, total);
   return 1;
+}
+
+void launch_bn_stats(const float* x, int nb, int c, long long n, long long bstride, double* part, cudaStream_t st) {
+  k_bn_stats<<<dim3(kBnBlocks, c), kBnThreads, 0, st>>>(x, n, nb, bstride, part);
+}
+void launch_bn_finalize(const double* part, int c, long long count, const float* w, const float* b, float eps,
+                        float* ac, double* stats, cudaStream_t st) {
+  k_bn_finalize<<<c, kBnThreads, 0, st>>>(part, kBnBlocks, c, count, w, b, eps, ac, stats);
+}
+void launch_tc_bn_stats(const float* buf, const ConvTcGeo& g, double* part, cudaStream_t st) {
+  k_tc_bn_rows<false><<<kBnBlocks, kBnThreads, 0, st>>>((const float4*)buf, g, nullptr, nullptr, 0, 0, part, nullptr,
+                                                         nullptr);
+}
+void launch_tc_bn_apply(float* buf, const ConvTcGeo& g, const float* ac, cudaStream_t st) {
+  const long long total = (long long)g.nb * g.nz * g.ny * g.nx;
+  k_tc_bn_apply<<<(unsigned)((total + 255) / 256), 256, 0, st>>>((float4*)buf, g, ac, total);
+}
+void launch_tc_bn_tail(const float* buf, const ConvTcGeo& g, const float* ac3, const float* tail, int relu6,
+                       int pass_b, double* part, const float* ac4, float* p_net, cudaStream_t st) {
+  k_tc_bn_rows<true><<<kBnBlocks, kBnThreads, 0, st>>>((const float4*)buf, g, ac3, tail, relu6, pass_b, part, ac4,
+                                                        p_net);
+}
+void launch_bn_apply(float* x, int nb, int c, long long n, long long bstride, const float* ac, cudaStream_t st) {
+  const long long total = (long long)nb * c * n;
+  k_bn_apply<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(x, c, n, bstride, ac, total);
 }
 
 }  // namespace tfl

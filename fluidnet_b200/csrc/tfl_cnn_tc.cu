@@ -181,14 +181,25 @@ __device__ __forceinline__ float4 tf32_hi(float4 v) {
 
 __device__ long long* g_tc_dbg = nullptr;   // optional phase timestamps (tests/dbg only)
 
+// The non-linearity of the epilogues: ReLU, or nn.ReLU6 (min(max(x, 0), 6)).
+__device__ __forceinline__ float tc_act(float v, int relu6) {
+  v = v > 0.0f ? v : 0.0f;
+  return relu6 && v > 6.0f ? 6.0f : v;
+}
+
 // Bias, ReLU and (FINAL) the two 1x1x1 layers of one position's 4 channels (4 * half ..), as the two threads of a
 // position share them; writes the next layer's padded plane or the pressure when `valid`.
 template <bool FINAL>
 __device__ __forceinline__ void conv_epilogue(float (&h)[4], bool valid, int half, const float* sTail, float4* out,
-                                              float* p_net, long long out_idx, long long plane_g, long long p_idx) {
+                                              float* p_net, long long out_idx, long long plane_g, long long p_idx,
+                                              const TcEpi& ep) {
 #pragma unroll
-  for (int o = 0; o < 4; o++) h[o] = h[o] > 0.0f ? h[o] : 0.0f;
+  for (int o = 0; o < 4; o++) h[o] = tc_act(h[o], ep.relu6);
   if constexpr (!FINAL) {
+    if (ep.ac) {                                  // running-statistics BN after the activation (valid voxels only)
+#pragma unroll
+      for (int o = 0; o < 4; o++) h[o] = fmaf(sTail[8 + 4 * half + o], h[o], sTail[16 + 4 * half + o]);
+    }
     if (valid) out[out_idx + half * plane_g] = make_float4(h[0], h[1], h[2], h[3]);
   } else {
     float hh[8];
@@ -209,7 +220,7 @@ __device__ __forceinline__ void conv_epilogue(float (&h)[4], bool valid, int hal
       float a = b4[o];
 #pragma unroll
       for (int c = 0; c < 8; c++) a = fmaf(hh[c], w4[o * 8 + c], a);
-      a = a > 0.0f ? a : 0.0f;
+      a = tc_act(a, ep.relu6);
       part = fmaf(a, w5[o], part);
     }
     const float pacc = b5 + (part + __shfl_xor_sync(0xffffffffu, part, 1));
@@ -222,7 +233,7 @@ template <int IN_PLANES, bool FINAL, bool SPLIT>
 __global__ void __launch_bounds__(kZThreads, 1)
 k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __restrict__ p_net,
              const float* __restrict__ wB, const float* __restrict__ bias, const float* __restrict__ tail,
-             ConvTcGeo g, ZSched s) {
+             ConvTcGeo g, ZSched s, TcEpi ep) {
   extern __shared__ __align__(1024) uint8_t smem[];
   using L = ZLayout<IN_PLANES, SPLIT>;
   constexpr int TY = L::TY, PY = L::PY;
@@ -244,6 +255,7 @@ k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __r
   for (int i = tid; i < L::B_BYTES / 16; i += kZThreads) ((float4*)sB)[i] = __ldg((const float4*)wB + i);
   const int n_tail = FINAL ? (8 + 64 + 8 + 8 + 1) : 8;
   for (int i = tid; i < n_tail; i += kZThreads) sTail[i] = (i < 8) ? bias[i] : tail[i - 8];
+  if (!FINAL && ep.ac && tid < 16) sTail[8 + tid] = ep.ac[tid];
 
   const long long plane_g = (long long)(g.nz + 2) * g.py * g.px;            // float4 per global plane
   const long long batch_g = plane_g * 2;
@@ -379,7 +391,7 @@ k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __r
           h[3] = (dm.w + d0.w) + dp.w + bs[3];
           conv_epilogue<FINAL>(h, xp <= g.nx, half, sTail, out, p_net,
                                b * batch_g + ((long long)(z + 1) * g.py + (yg + 1)) * g.px + xp, plane_g,
-                               (long long)b * g.nz * g.ny * g.nx + ((long long)z * g.ny + yg) * g.nx + (xp - 1));
+                               (long long)b * g.nz * g.ny * g.nx + ((long long)z * g.ny + yg) * g.nx + (xp - 1), ep);
         }
         wg_barrier(1 + wg);                        // myD is rewritten by the next row
       }
@@ -405,7 +417,7 @@ template <int IN_PLANES, bool FINAL, bool SPLIT, bool JOIN = false>
 __global__ void __launch_bounds__(kThreads, 2)
 k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __restrict__ p_net,
            const float* __restrict__ wB, const float* __restrict__ bias, const float* __restrict__ tail,
-           ConvTcGeo g, TcJoinSrc js) {
+           ConvTcGeo g, TcJoinSrc js, TcEpi ep) {
   static_assert(!JOIN || (FINAL && IN_PLANES == 2), "the join is the last 3x3x3 layer");
   extern __shared__ __align__(1024) uint8_t smem[];
   using T = Tile<SPLIT>;
@@ -528,6 +540,7 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
   for (int i = tid; i < L::B_BYTES / 16; i += kThreads) cp_async16(smem_u32(sB + i * 16), (const float4*)wB + i);
   const int n_tail = FINAL ? (8 + 64 + 8 + 8 + 1) : 8;
   for (int i = tid; i < n_tail; i += kThreads) sTail[i] = (i < 8) ? bias[i] : tail[i - 8];
+  if (!FINAL && ep.ac && tid < 16) sTail[8 + tid] = ep.ac[tid];
   asm volatile("cp.async.commit_group;" ::: "memory");
   asm volatile("cp.async.wait_group 0;" ::: "memory");
   // generic-proxy writes (st.shared, cp.async) -> visible to the wgmma (async proxy) reads
@@ -629,8 +642,12 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
       h[3] = (dm.w + d0.w) + dp.w + bs[3];
     }
 #pragma unroll
-    for (int o = 0; o < 4; o++) h[o] = h[o] > 0.0f ? h[o] : 0.0f;
+    for (int o = 0; o < 4; o++) h[o] = tc_act(h[o], ep.relu6);
     if (!FINAL) {
+      if (ep.ac) {                                      // running-statistics BN after the activation
+#pragma unroll
+        for (int o = 0; o < 4; o++) h[o] = fmaf(sTail[8 + 4 * half + o], h[o], sTail[16 + 4 * half + o]);
+      }
       if (valid) {
         const long long o = b * batch_g + ((long long)(zg + 1) * g.py + (yg + 1)) * g.px + (xg + 1);
         out[o + half * plane_g] = make_float4(h[0], h[1], h[2], h[3]);
@@ -654,7 +671,7 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
         float a = b4[o];
 #pragma unroll
         for (int c = 0; c < 8; c++) a = fmaf(hh[c], w4[o * 8 + c], a);
-        a = a > 0.0f ? a : 0.0f;
+        a = tc_act(a, ep.relu6);
         part = fmaf(a, w5[o], part);
       }
       const float pacc = b5 + (part + __shfl_xor_sync(0xffffffffu, part, 1));
@@ -670,7 +687,7 @@ k_conv3_tc(const float4* __restrict__ in, float4* __restrict__ out, float* __res
 
 template <int IN_PLANES, bool FINAL, bool SPLIT, bool JOIN = false>
 void launch_one(const float4* in, float4* out, float* p_net, const float* wB, const float* bias,
-                const float* tail, const ConvTcGeo& g, cudaStream_t st, const TcJoinSrc& js = TcJoinSrc{}) {
+                const float* tail, const ConvTcGeo& g, cudaStream_t st, const TcJoinSrc& js, const TcEpi& ep) {
   using T = Tile<SPLIT>;
   const size_t smem = Layout<IN_PLANES, SPLIT>::BYTES;
   auto kern = k_conv3_tc<IN_PLANES, FINAL, SPLIT, JOIN>;
@@ -686,7 +703,7 @@ void launch_one(const float4* in, float4* out, float* p_net, const float* wB, co
   gg.ntz = ntz;
   gg.nty = (g.ny + T::TY - 1) / T::TY;
   dim3 grid(g.ntx, gg.nty, ntz * g.nb);
-  kern<<<grid, kThreads, smem, st>>>(in, out, p_net, wB, bias, tail, gg, js);
+  kern<<<grid, kThreads, smem, st>>>(in, out, p_net, wB, bias, tail, gg, js, ep);
 }
 
 // Work items of one k_conv3_tc_z launch on `nsm` SMs.  ZC (output planes per item) minimises the rounds of the
@@ -717,7 +734,7 @@ ZSched z_schedule(const ConvTcGeo& g, int ty, int nsm) {
 
 template <int IN_PLANES, bool FINAL, bool SPLIT>
 void launch_z(const float4* in, float4* out, float* p_net, const float* wB, const float* bias, const float* tail,
-              const ConvTcGeo& g, cudaStream_t st) {
+              const ConvTcGeo& g, cudaStream_t st, const TcEpi& ep) {
   using L = ZLayout<IN_PLANES, SPLIT>;
   if (g.z_hi <= g.z_lo || g.nb < 1 || g.ny < 1 || g.nx < 1) return;     // nothing to compute
   auto kern = k_conv3_tc_z<IN_PLANES, FINAL, SPLIT>;
@@ -731,7 +748,7 @@ void launch_z(const float4* in, float4* out, float* p_net, const float* wB, cons
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const ZSched s = z_schedule(g, L::TY, nsm);
   const int grid = s.items < nsm ? s.items : nsm;
-  kern<<<grid, kZThreads, L::bytes(s.ww), st>>>(in, out, p_net, wB, bias, tail, g, s);
+  kern<<<grid, kZThreads, L::bytes(s.ww), st>>>(in, out, p_net, wB, bias, tail, g, s, ep);
 }
 
 // 2x2x2 average of the first float4 plane (k_pool's summation order), zero fourth channel; output planes
@@ -893,10 +910,10 @@ void conv_tc_pack_weights(const float* w, int cin, int split, float* out) {
 }
 
 int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, const float* bias, const float* tail,
-                         int split, const ConvTcGeo& g, cudaStream_t st) {
+                         int split, const ConvTcGeo& g, cudaStream_t st, const TcEpi& ep) {
   if (src.n < 1 || src.n > kTcMaxBanks) return -1;
-  if (split) launch_one<2, true, true, true>(nullptr, nullptr, p_net, wB, bias, tail, g, st, src);
-  else launch_one<2, true, false, true>(nullptr, nullptr, p_net, wB, bias, tail, g, st, src);
+  if (split) launch_one<2, true, true, true>(nullptr, nullptr, p_net, wB, bias, tail, g, st, src, ep);
+  else launch_one<2, true, false, true>(nullptr, nullptr, p_net, wB, bias, tail, g, st, src, ep);
   return 1;
 }
 
@@ -910,7 +927,7 @@ void launch_tc_pyramid(const float* in, const ConvTcGeo& gin, float* out, const 
 
 int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, const float* bias,
                     const float* tail, int in_planes, int final_layer, int split, const ConvTcGeo& g,
-                    cudaStream_t st) {
+                    cudaStream_t st, const TcEpi& ep) {
   const float4* i4 = (const float4*)in;
   float4* o4 = (float4*)out;
   // Rows up to kWWMax positions stream along z without an x halo; wider rows would need overlapping row windows
@@ -918,8 +935,8 @@ int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, 
   // per row against 288), so they keep the one-shot box.
 #define TFL_TC_CASE(P, F, S)                                                   \
   if (in_planes == P && (final_layer != 0) == F && (split != 0) == S) {        \
-    if (g.nx <= kWWMax) launch_z<P, F, S>(i4, o4, p_net, wB, bias, tail, g, st); \
-    else launch_one<P, F, S>(i4, o4, p_net, wB, bias, tail, g, st);            \
+    if (g.nx <= kWWMax) launch_z<P, F, S>(i4, o4, p_net, wB, bias, tail, g, st, ep); \
+    else launch_one<P, F, S>(i4, o4, p_net, wB, bias, tail, g, st, TcJoinSrc{}, ep); \
     return 1;                                                                  \
   }
   TFL_TC_CASE(1, false, false) TFL_TC_CASE(2, false, false) TFL_TC_CASE(2, true, false)

@@ -18,11 +18,19 @@ size_t conv_tc_act_bytes(const ConvTcGeo& g);
 int conv_tc_b_floats(int split);
 void conv_tc_set_debug(long long* dev_buf);   // nullptr disables
 void conv_tc_pack_weights(const float* w /*[8][cin][3][3][3]*/, int cin, int split, float* out);
+// The epilogue's options: relu6 = 1 clamps every non-linearity of the layer (and of the fused 1x1x1 tail) at 6
+// (nn.ReLU6); ac (device, [2][8]: a then c; non-final layers only, may be null) applies y = a h + c per channel after
+// the non-linearity -- batch normalization with running statistics -- to the voxels written, so the zero border stays
+// zero.
+struct TcEpi {
+  const float* ac = nullptr;
+  int relu6 = 0;
+};
 // in/out: padded channels-last activations; p_net: plain [b][z][y][x] (final layer only);
 // tail (final layer): w4[8][8] (o, c), b4[8], w5[8], b5[1] on the device.
 int launch_conv3_tc(const float* in, float* out, float* p_net, const float* wB, const float* bias,
                     const float* tail, int in_planes, int final_layer, int split, const ConvTcGeo& g,
-                    cudaStream_t st);
+                    cudaStream_t st, const TcEpi& ep = TcEpi());
 
 // Join layer of the multi-resolution banks (lib/model.lua:292-318) on the tensor cores: the last 3x3x3 layer
 // reads its 8 input channels as the sum over src[0..n) of bank src[k] upsampled nearest by 2^shift[k], staged
@@ -46,7 +54,20 @@ struct TcJoinSrc {
   float* partial;
 };
 int launch_conv3_tc_join(const TcJoinSrc& src, float* p_net, const float* wB, const float* bias, const float* tail,
-                         int split, const ConvTcGeo& g, cudaStream_t st);
+                         int split, const ConvTcGeo& g, cudaStream_t st, const TcEpi& ep = TcEpi());
+
+// Batch normalization with batch statistics on the padded layout (tfl_cnn.cu), all 8 channels of a 3x3x3 layer's
+// output over its interior (nb nz ny nx voxels; the border is neither read nor written).  Partials as
+// launch_bn_stats writes them (part [8][kBnBlocks + 1][2], fp64, fixed order), turned into ac [2][8] by
+// launch_bn_finalize; launch_tc_bn_apply: x = a x + c in place on the interior.
+void launch_tc_bn_stats(const float* buf, const ConvTcGeo& g, double* part, cudaStream_t st);
+void launch_tc_bn_apply(float* buf, const ConvTcGeo& g, const float* ac, cudaStream_t st);
+// The 1x1x1 tail of the 3-D 'default' graph with batch statistics, on layer 3's output `buf` (padded layout, already
+// through its non-linearity): h4 = act(w4 (a3 h3 + c3) + b4) with ac3 = BN3's (a, c).  pass_b = 0 (pass A): only the
+// per-channel partials of h4 into part, as launch_tc_bn_stats; pass_b = 1 (pass B): p_net = w5 (a4 h4 + c4) + b5 with
+// ac4 = BN4's (a, c).  h4 is recomputed in pass B rather than stored.  tail: w4[8][8], b4[8], w5[8], b5[1] (device).
+void launch_tc_bn_tail(const float* buf, const ConvTcGeo& g, const float* ac3, const float* tail, int relu6,
+                       int pass_b, double* part, const float* ac4, float* p_net, cudaStream_t st);
 // Bank pyramid on the padded channels-last layout: out's plane z = 2x2x2 average of in's planes 2 z + z_phase and
 // 2 z + z_phase + 1 (interior, first float4 plane only: the 3 input channels and a zero fourth), for the output
 // planes [gout.z_lo, gout.z_hi).  z_phase (0 or 1) aligns the pooling to the global grid on a z-slab whose

@@ -120,7 +120,7 @@ void launch_cnn_finish_fused(const float* p_net, float* U, const unsigned char* 
 // ---- tfl_cnn.cu ----
 // Generic direct convolution (fp32 FMA): in [b][cin][z][y][x] -> out [b][cout][z][y][x].
 // wdev: device weights re-laid out as [cin][tap][cout_pad], bias [cout].
-// act: 0 none, 1 ReLU, 2 sigmoid.
+// act: 0 none, 1 ReLU, 2 sigmoid, 3 ReLU6.
 // dil > 1: dilated convolution (nn.{Spatial,Volumetric}DilatedConvolution with dilation dil on every axis, stride 1,
 // padding dil (k-1)/2: same grid out as in); dil = 1 runs the undilated kernels.
 // Returns the kernel that ran: kConvDirect (k_conv_direct, a specialised (cout, k) whose weights fit shared
@@ -142,6 +142,17 @@ void launch_pixel_shuffle(const float* in, float* out, int nb, int n_out, int nz
 constexpr int kMaxBankPtrs = 8;
 int launch_bank_join(const float* const* banks, int nbanks, float* out, int nb, int c, int nz, int ny, int nx,
                      int is3d, int add, cudaStream_t st, int full = 0);
+// Batch normalization of x [nb][c][n] with batch entries bstride floats apart (>= c n).  launch_bn_stats: per-channel
+// fp64 partials of (sum d, sum d^2), d = x - K with K the channel's first value, into part [c][kBnBlocks + 1][2] (the
+// last slot holds K), one slot per block of a fixed range, no atomics.  launch_bn_finalize: mean and biased variance
+// over count = nb n values per channel, ac [2][c] = (w invstd, b - mean w invstd) with invstd = 1 / sqrt(var + eps), 0
+// when var + eps == 0 (a constant channel has var exactly 0) (w / b null: 1 / 0); stats (may be null) [c][2] gets
+// (mean, var).  launch_bn_apply: x = a x + c in place.
+constexpr int kBnBlocks = 128;
+void launch_bn_stats(const float* x, int nb, int c, long long n, long long bstride, double* part, cudaStream_t st);
+void launch_bn_finalize(const double* part, int c, long long count, const float* w, const float* b, float eps,
+                        float* ac, double* stats, cudaStream_t st);
+void launch_bn_apply(float* x, int nb, int c, long long n, long long bstride, const float* ac, cudaStream_t st);
 
 // ---- tfl_pcg.cu: matrix-free PCG pressure solve ----
 struct PcgScratch {            // owned by the context, grow-only

@@ -36,10 +36,10 @@ def default_layers(is3D):
 class ProjectionModel:
     def __init__(self, layers, is3D, device=None, normalizeInputThreshold=1e-5, pool=None, up=None,
                  poolType="avg", nonlinType="relu", banks=None, inputChannels=None, normalizeInput=True,
-                 normalizeInputFunc="std", normalizeInputChan="UDiv", addPressureSkip=False):
+                 normalizeInputFunc="std", normalizeInputChan="UDiv", addPressureSkip=False, batchNorm=None):
         """layers: [(weight ndarray [cout * up^d][cin][kz][ky][kx], bias ndarray [cout * up^d]), ...]
         pool / up: per-layer pooling and ConvolutionUpsample sizes of the 'tog' graph (lib/model.lua:164-226),
-        None = all 1 ('default', 'yang'); poolType 'avg' | 'max'; nonlinType 'relu' | 'sigmoid'.
+        None = all 1 ('default', 'yang'); poolType 'avg' | 'max'; nonlinType 'relu' | 'sigmoid' | 'relu6'.
         banks: banks of convolutions (lib/model.lua:252-361), {"num": banksNum, "split_stage": banksSplitStage,
         "join_stage": banksJoinStage, "aggregate": 'concat' | 'add', "type": 'mres' | 'dilate'} (stages numbered
         from 1; a missing "type" is banksType 'mres', multi-resolution banks; 'dilate' dilates bank i's convolutions by
@@ -48,7 +48,12 @@ class ProjectionModel:
         inputChannels ({"pDiv", "UDiv", "div", "flags"} -> bool, missing keys at their defaults pDiv, div, flags),
         normalizeInput, normalizeInputFunc ('std' | 'norm'), normalizeInputChan ('UDiv' | 'pDiv' | 'div') and
         addPressureSkip are the mconf keys of lib/model.lua:27-150, :357-387; layers[0] takes the selected channels and
-        with the skip the last layer takes one more, pDiv.  The library refuses what the reference cannot build."""
+        with the skip the last layer takes one more, pDiv.  The library refuses what the reference cannot build.
+        batchNorm: addBatchNorm (lib/model.lua:343-350), {"train": bool, "layers": [...]}: "layers" mirrors
+        layers[:-1] (a banked stage holds a list with one entry per bank), each entry {"weight", "bias" (None for a
+        module without batchNormAffine), "running_mean", "running_var", "eps"}.  train = True (the saved module's
+        `train` field, true unless the model was put in evaluate mode) normalises with the statistics of the batch,
+        False with the running statistics.  Such models run on the fp32 path, as do 'relu6' models."""
         ch = dict(DEFAULT_INPUTS, **(inputChannels or {}))
         if not ch["flags"]:
             raise TflError("Are you sure you dont want flags on input?")          # lib/model.lua:39-43
@@ -65,7 +70,7 @@ class ProjectionModel:
         pool = [1] * n if pool is None else [int(v) for v in pool]
         up = [1] * n if up is None else [int(v) for v in up]
         assert len(pool) == n and len(up) == n
-        assert poolType in ("avg", "max") and nonlinType in ("relu", "sigmoid")
+        assert poolType in ("avg", "max") and nonlinType in ("relu", "sigmoid", "relu6")
         self.banks = dict(banks) if banks is not None else None
         if banks is not None:
             assert banks["aggregate"] in ("concat", "add"), "banksAggregateMethod must be 'concat' or 'add'"
@@ -105,6 +110,35 @@ class ProjectionModel:
             self._keep += [w, b]
             wp[i] = w.ctypes.data_as(C.POINTER(C.c_float))
             bp[i] = b.ctypes.data_as(C.POINTER(C.c_float))
+        norm = None
+        if nonlinType == "relu6" or batchNorm is not None:
+            norm = _lib.CnnNorm(int(nonlinType == "relu6"), int(batchNorm is not None),
+                                int(bool(batchNorm is not None and batchNorm["train"])), None, None)
+        if batchNorm is not None:
+            entries = []        # conv order, as `convs` (the last convolution has no BN)
+            assert len(batchNorm["layers"]) == n - 1, "batchNorm['layers'] mirrors layers[:-1]"
+            for l, e in enumerate(batchNorm["layers"]):
+                per_bank = list(e) if isinstance(e, (tuple, list)) else [e]
+                fan = up[l] ** (3 if is3D else 2)
+                nconv = len(layers[l]) if isinstance(layers[l][0], (tuple, list)) else 1
+                assert len(per_bank) == nconv, "stage %d: one batch normalization per bank" % (l + 1)
+                for bk in per_bank:
+                    c = np.asarray(bk["running_mean"]).shape[0]
+                    w = np.ones(c, np.float32) if bk.get("weight") is None else bk["weight"]
+                    b = np.zeros(c, np.float32) if bk.get("bias") is None else bk["bias"]
+                    arr = np.ascontiguousarray(np.stack([np.asarray(v, np.float32).reshape(c) for v in
+                                                         (w, b, bk["running_mean"], bk["running_var"])]))
+                    assert c * fan == convs[len(entries)][0].shape[0], \
+                        "stage %d: batch normalization over %d channels, the stage has %d" % (l + 1, c, cout[l])
+                    entries.append((arr, float(bk["eps"])))
+            bnp = (C.POINTER(C.c_float) * len(entries))()
+            eps = (C.c_float * len(entries))(*[e for _, e in entries])
+            for i, (arr, _) in enumerate(entries):
+                self._keep.append(arr)
+                bnp[i] = arr.ctypes.data_as(C.POINTER(C.c_float))
+            self._keep += [bnp, eps]
+            norm.bn = bnp
+            norm.eps = eps
         h = C.c_void_p()
         args = (self.ctx.h, 1 if is3D else 0, n, cin, cout, ks, cpool, cup, 1 if poolType == "max" else 0,
                 1 if nonlinType == "sigmoid" else 0)
@@ -112,8 +146,9 @@ class ProjectionModel:
         if banks is not None:
             cb = _lib.CnnBanksEx(int(banks["num"]), int(banks["split_stage"]), int(banks["join_stage"]),
                                  1 if banks["aggregate"] == "add" else 0, 1 if banks.get("type") == "dilate" else 0)
-        self.ctx.check(self.ctx.lib.tfl_cnn_create_model_ex(*args, C.byref(cb) if cb is not None else None,
-                                                            C.byref(cin_), wp, bp, C.byref(h)))
+        self.ctx.check(self.ctx.lib.tfl_cnn_create_model_norm(*args, C.byref(cb) if cb is not None else None,
+                                                              C.byref(cin_), C.byref(norm) if norm is not None else None,
+                                                              wp, bp, C.byref(h)))
         self.h = h
         self.last_scale = None
 
@@ -126,8 +161,10 @@ class ProjectionModel:
         architecture.  Options and modules the library does not compute raise ValueError naming them."""
         from . import torch7
         ref = torch7.load_reference_model(model_path, mconf_path)
-        opts = torch7.model_options(ref["mconf"], inputs=True, dilate=True)
-        stages = torch7.graph_stages(ref["model"], dilate=opts.get("banks", {}).get("type") == "dilate")
+        bn = torch7.batch_norm_layers(ref["model"]) if ref["mconf"].get("addBatchNorm") else None
+        opts = torch7.model_options(ref["mconf"], inputs=True, dilate=True, batchnorm=True, relu6=True, bn=bn)
+        stages = torch7.graph_stages(ref["model"], dilate=opts.get("banks", {}).get("type") == "dilate",
+                                     batchnorm=bn is not None)
         torch7.check_stages(stages, ref["mconf"], opts)
         return cls(stages, ref["is3D"], device=device, **opts), ref["mconf"]
 

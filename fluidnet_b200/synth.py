@@ -81,7 +81,7 @@ def make_density(flags, seed=1235):
     return np.ascontiguousarray(d)
 
 
-def make_model(is3d=True, seed=4321, model_type="default", banks=None, inputs=None):
+def make_model(is3d=True, seed=4321, model_type="default", banks=None, inputs=None, batch_norm=None):
     """Random-init weights of a reference architecture (torch/lib/model.lua:164-226: 'default', 'tog',
     'yang'), Torch `reset` convention uniform +-1/sqrt(fan_in).  Inputs: pDiv, div, occupancy
     (lib/default_conf.lua:76-81).  'tog' layers carry pooling / ConvolutionUpsample sizes: the weights of
@@ -90,7 +90,11 @@ def make_model(is3d=True, seed=4321, model_type="default", banks=None, inputs=No
     entry in "layers" is then a list of num (weight, bias) pairs, and a 'concat' join stage takes num x the channels.
     "type" ('mres' or 'dilate') is carried through; both types draw the same weights.
     inputs: the input-block keywords of model.ProjectionModel (inputChannels, normalizeInput*, addPressureSkip),
-    kept under "inputs"; the first layer takes the selected channels, the last one more with addPressureSkip."""
+    kept under "inputs"; the first layer takes the selected channels, the last one more with addPressureSkip.
+    batch_norm: {"train": bool[, "affine": bool (default True), "eps": float (default 1e-4)]} adds "batchNorm" in the
+    form of model.ProjectionModel's keyword: per stage but the last (per bank of a banked stage) a weight in
+    [0.5, 1.5) and a bias in [-0.5, 0.5) (None without affine), a running mean in [-0.5, 0.5) and a running variance
+    in [0.05, 1.05), drawn after the weights from their own stream."""
     rs = np.random.RandomState(seed)
     extra = {}
     if model_type == "default":
@@ -138,4 +142,18 @@ def make_model(is3d=True, seed=4321, model_type="default", banks=None, inputs=No
         out["banks"] = dict(banks)
     if inputs is not None:
         out["inputs"] = dict(inputs)
+    if batch_norm is not None:
+        rb = np.random.RandomState(seed + 1)
+        affine = batch_norm.get("affine", True)
+        eps = float(batch_norm.get("eps", 1e-4))
+
+        def entry(c):
+            w = (0.5 + rb.rand(c)).astype(np.float32) if affine else None
+            b = (rb.rand(c) - 0.5).astype(np.float32) if affine else None
+            return {"weight": w, "bias": b, "running_mean": (rb.rand(c) - 0.5).astype(np.float32),
+                    "running_var": (0.05 + rb.rand(c)).astype(np.float32), "eps": eps}
+        bn_layers = []
+        for cout, layer in zip(osize[:-1], layers[:-1]):
+            bn_layers.append([entry(cout) for _ in layer] if isinstance(layer, list) else entry(cout))
+        out["batchNorm"] = {"train": bool(batch_norm["train"]), "layers": bn_layers}
     return out

@@ -223,7 +223,7 @@ _ALLOWED = {
     "nn.Identity", "nn.SelectTable", "nn.Select", "nn.Unsqueeze", "nn.JoinTable", "nn.CAddTable", "nn.ApplyScale",
     "nn.Sequential", "tfluids.SetWallBcs", "tfluids.VelocityDivergence", "tfluids.FlagsToOccupancy",
     "tfluids.VelocityUpdate", "tfluids.VolumetricUpSamplingNearest", "nn.SpatialUpSamplingNearest",
-    "nn.ReLU", "cudnn.ReLU", "nn.Sigmoid", "cudnn.Sigmoid",
+    "nn.ReLU", "cudnn.ReLU", "nn.Sigmoid", "cudnn.Sigmoid", "nn.ReLU6",
     "nn.SpatialConvolution", "nn.VolumetricConvolution", "cudnn.SpatialConvolution", "cudnn.VolumetricConvolution",
     "nn.SpatialConvolutionUpsample", "nn.VolumetricConvolutionUpsample",
     "nn.SpatialAveragePooling", "nn.VolumetricAveragePooling", "cudnn.SpatialAveragePooling",
@@ -233,6 +233,15 @@ _ALLOWED = {
 
 # The convolutions of banks 2..N of a banksType 'dilate' model (lib/model_utils.lua:122-146).
 _DILATED = {"nn.SpatialDilatedConvolution", "nn.VolumetricDilatedConvolution"}
+
+# torch.addBN (lib/model_utils.lua:36-62): cudnn.* with batchNormAffine, nn.* (no weight / bias) without.
+_BATCH_NORM = {"nn.SpatialBatchNormalization", "nn.VolumetricBatchNormalization", "cudnn.SpatialBatchNormalization",
+               "cudnn.VolumetricBatchNormalization"}
+# The nodes between a stage's convolution and its batch normalization (lib/model.lua:337-350).
+_NONLIN_POOL = {"nn.ReLU", "cudnn.ReLU", "nn.Sigmoid", "cudnn.Sigmoid", "nn.ReLU6",
+                "nn.SpatialAveragePooling", "nn.VolumetricAveragePooling", "cudnn.SpatialAveragePooling",
+                "cudnn.VolumetricAveragePooling", "nn.SpatialMaxPooling", "nn.VolumetricMaxPooling",
+                "cudnn.SpatialMaxPooling", "cudnn.VolumetricMaxPooling"}
 
 
 def _check_dilation(conv, cls, bank):
@@ -283,13 +292,14 @@ def _node_modules(model):
     return out
 
 
-def graph_stages(model, dilate=False):
+def graph_stages(model, dilate=False, batchnorm=False):
     """The convolutions of a reference gModule grouped by stage: [[(weight, bias) of bank 1, bank 2, ...], ...].
     Each convolution is assigned from its node's annotation "Bank i: conv stage l" (lib/model.lua:337); the final
     convolution has none.  Raises ValueError, naming it, for a module outside the graphs the library computes
     (batch normalisation, gated convolutions, low-rank convolution Sequentials, ...).  Dilated convolutions are such a
     module unless dilate=True, which reads a banksType 'dilate' model: bank i >= 2's convolutions must then be dilated
-    by 2^(i-1) (see _check_dilation) and all others undilated."""
+    by 2^(i-1) (see _check_dilation) and all others undilated.  Batch normalization modules are accepted with
+    batchnorm=True only (batch_norm_layers reads them)."""
     mods = _node_modules(model)
     if not mods:
         raise ValueError("torch7 model: not an nngraph gModule (no forwardnodes)")
@@ -297,7 +307,7 @@ def graph_stages(model, dilate=False):
     final = []
     for mod, name in mods:
         cls = mod.cls if isinstance(mod, T7Object) else type(mod).__name__
-        if cls not in _ALLOWED and not (dilate and cls in _DILATED):
+        if cls not in _ALLOWED and not (dilate and cls in _DILATED) and not (batchnorm and cls in _BATCH_NORM):
             raise ValueError("torch7 model: module %s is not supported by this library" % cls)
         convs = []
         _walk(mod, set(), convs)
@@ -335,6 +345,97 @@ def graph_stages(model, dilate=False):
         stages.append(convs if len(convs) > 1 else convs[0])
     stages.append(final[0])
     return stages
+
+
+def _cls(obj):
+    return obj.cls if isinstance(obj, T7Object) else type(obj).__name__
+
+
+def batch_norm_layers(model):
+    """The batch normalization of an addBatchNorm gModule (lib/model.lua:343-350) as ProjectionModel's batchNorm:
+    {"train": bool, "layers": [...]} with "layers" mirroring graph_stages(model)[:-1] (a list per banked stage, bank
+    order), each entry {"weight", "bias" (None without affine parameters), "running_mean", "running_var", "eps",
+    "cls"}.  BN nodes carry no annotation, so each is assigned to the convolution whose node reaches it through the
+    graph's edges (`children`) across non-linearity and pooling nodes only.  Raises ValueError, naming it, for a BN
+    module reached from no stage convolution, a stage convolution without one, a channel count other than the
+    convolution's, modules whose `train` flags differ, and an old-format module (running_std without running_var)."""
+    nodes = model.get("forwardnodes") if isinstance(model, T7Object) else None
+    if not nodes:
+        raise ValueError("torch7 model: not an nngraph gModule (no forwardnodes)")
+    order = [nodes[i] for i in sorted(nodes) if isinstance(nodes[i], T7Object)]
+
+    def data(node):
+        d = node.get("data")
+        return d if isinstance(d, dict) else {}
+
+    def children(node):
+        ch = node.get("children")
+        return [ch[k] for k in sorted(k for k in ch if isinstance(k, int))] if isinstance(ch, dict) else []
+
+    assigned = {}       # id(BN node) -> (stage, bank)
+    stage_conv = {}     # (stage, bank) -> conv module
+    for node in order:
+        d = data(node)
+        ann = d.get("annotations")
+        m = _CONV_STAGE.match((ann.get("name") if isinstance(ann, dict) else None) or "")
+        if not m or d.get("module") is None:
+            continue
+        key = (int(m.group(2)), int(m.group(1)))
+        stage_conv[key] = d["module"]
+        todo, seen = list(children(node)), set()
+        while todo:
+            nd = todo.pop()
+            if id(nd) in seen:
+                continue
+            seen.add(id(nd))
+            cls = _cls(data(nd).get("module"))
+            if cls in _BATCH_NORM:
+                if id(nd) in assigned and assigned[id(nd)] != key:
+                    raise ValueError("torch7 model: a %s is reached from two stage convolutions" % cls)
+                assigned[id(nd)] = key
+            elif cls in _NONLIN_POOL:
+                todo += children(nd)
+    found = {}
+    trains = set()
+    for node in order:
+        mod = data(node).get("module")
+        cls = _cls(mod)
+        if cls not in _BATCH_NORM:
+            continue
+        if id(node) not in assigned:
+            raise ValueError("torch7 model: %s is not placed after a stage's convolution, non-linearity and pooling "
+                             "(lib/model.lua:343-350)" % cls)
+        key = assigned[id(node)]
+        if key in found:
+            raise ValueError("torch7 model: stage %d bank %d has two batch normalizations (%s)" % (key + (cls,)))
+        if mod.get("running_var") is None:
+            if mod.get("running_std") is not None:
+                raise ValueError("torch7 model: %s carries running_std without running_var (an old nn format this "
+                                 "library does not read)" % cls)
+            raise ValueError("torch7 model: %s has no running_var" % cls)
+        mean = np.asarray(mod["running_mean"], np.float32).reshape(-1)
+        var = np.asarray(mod["running_var"], np.float32).reshape(-1)
+        conv = stage_conv[key]
+        c = conv.get("nOutputPlane") if isinstance(conv, T7Object) else None
+        if c is not None and mean.shape[0] != int(c):
+            raise ValueError("torch7 model: %s of stage %d bank %d has %d channels, its convolution %d"
+                             % (cls, key[0], key[1], mean.shape[0], int(c)))
+        w, b = mod.get("weight"), mod.get("bias")
+        trains.add(bool(mod.get("train", True)))
+        found[key] = {"weight": None if w is None else np.asarray(w, np.float32).reshape(-1),
+                      "bias": None if b is None else np.asarray(b, np.float32).reshape(-1),
+                      "running_mean": mean, "running_var": var, "eps": float(mod.get("eps", 1e-5)), "cls": cls}
+    if len(trains) > 1:
+        raise ValueError("torch7 model: the batch normalization modules differ in their train flag")
+    layers = []
+    for s in range(1, max([k[0] for k in stage_conv] + [0]) + 1):
+        banks = sorted(b for st, b in stage_conv if st == s)
+        missing = [b for b in banks if (s, b) not in found]
+        if missing:
+            raise ValueError("torch7 model: stage %d bank %d has no batch normalization" % (s, missing[0]))
+        entries = [found[(s, b)] for b in banks]
+        layers.append(entries if len(entries) > 1 else entries[0])
+    return {"train": trains.pop() if trains else True, "layers": layers}
 
 
 def input_options(mconf):
@@ -390,21 +491,23 @@ def input_options(mconf):
             "normalizeInputChan": chan, "addPressureSkip": skip}
 
 
-def model_options(mconf, n_stages=None, inputs=False, dilate=False):
+def model_options(mconf, n_stages=None, inputs=False, dilate=False, batchnorm=False, relu6=False, bn=None):
     """ProjectionModel keyword arguments for a reference mconf (lib/default_conf.lua, lib/model.lua:27-401):
     pool / up from modelType, poolType, nonlinType, banks, normalizeInputThreshold, and with inputs=True the input
     block (input_options).  Raises ValueError, naming the option, for anything the library does not compute.  Without
     inputs=True a non-default input block is refused too: a caller that drops those keys would build another model.
     Likewise banksType 'dilate' is accepted with dilate=True only (banks["type"] = 'dilate'; the file's convolutions
-    then come from graph_stages(model, dilate=True))."""
+    then come from graph_stages(model, dilate=True)), addBatchNorm with batchnorm=True only and nonlinType 'relu6'
+    with relu6=True only.  bn (batch_norm_layers of the file) is checked against batchNormAffine (modules with or
+    without weight and bias), batchNormEps and the channel count osize of each stage, and returned as "batchNorm"."""
     def opt(key, default=None):
         return mconf.get(key, default)
 
     def refuse(what):
         raise ValueError("mconf: %s is not supported by this library" % what)
 
-    if opt("addBatchNorm"):
-        refuse("addBatchNorm = true")
+    if opt("addBatchNorm") and not batchnorm:
+        refuse("addBatchNorm = true (model_options(mconf, batchnorm=True) builds it)")
     if not inputs:
         if opt("addPressureSkip"):
             refuse("addPressureSkip = true (model_options(mconf, inputs=True) builds it)")
@@ -421,7 +524,9 @@ def model_options(mconf, n_stages=None, inputs=False, dilate=False):
             refuse("normalizeInputChan = %r (model_options(mconf, inputs=True) builds 'pDiv', 'div')"
                    % opt("normalizeInputChan"))
     nonlin = opt("nonlinType", "relu")
-    if nonlin not in ("relu", "sigmoid"):
+    if nonlin == "relu6" and not relu6:
+        refuse("nonlinType = 'relu6' (model_options(mconf, relu6=True) builds it)")
+    if nonlin not in ("relu", "sigmoid", "relu6"):
         refuse("nonlinType = %r" % nonlin)
     pool_type = opt("poolType", "avg")
     if pool_type not in ("avg", "max"):
@@ -453,7 +558,31 @@ def model_options(mconf, n_stages=None, inputs=False, dilate=False):
                 raise ValueError("mconf: banksType = 'dilate': upsampling not supported for dilated convolutions.")
     if inputs:
         out.update(input_options(mconf))
+    if opt("addBatchNorm"):
+        if bn is None:
+            raise ValueError("mconf: addBatchNorm = true needs the file's batch normalization (bn=batch_norm_layers)")
+        _check_batch_norm(bn, mconf, _ARCH[key][0])
+        out["batchNorm"] = {"train": bn["train"], "layers": bn["layers"]}
     return out
+
+
+def _check_batch_norm(bn, mconf, osize):
+    """batchNormAffine (default true), batchNormEps (default 1e-4) and osize against the modules (model_utils.lua:36-62)."""
+    affine = bool(mconf.get("batchNormAffine", True))
+    eps = float(mconf.get("batchNormEps", 1e-4))
+    if len(bn["layers"]) != len(osize) - 1:
+        raise ValueError("torch7 model: batch normalization in %d stages, the mconf gives %d"
+                         % (len(bn["layers"]), len(osize) - 1))
+    for s, layer in enumerate(bn["layers"], start=1):
+        for e in (layer if isinstance(layer, list) else [layer]):
+            if (e["weight"] is not None) != affine or e["cls"].startswith("cudnn.") != affine:
+                raise ValueError("mconf: batchNormAffine = %s, but stage %d holds %s %s weight and bias"
+                                 % (str(affine).lower(), s, e["cls"], "with" if e["weight"] is not None else "without"))
+            if e["eps"] != eps:
+                raise ValueError("mconf: batchNormEps = %g, but stage %d's %s has eps %g" % (eps, s, e["cls"], e["eps"]))
+            if e["running_mean"].shape[0] != osize[s - 1]:
+                raise ValueError("torch7 model: stage %d's batch normalization has %d channels, osize is %d"
+                                 % (s, e["running_mean"].shape[0], osize[s - 1]))
 
 
 def check_stages(stages, mconf, options):

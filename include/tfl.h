@@ -270,11 +270,45 @@ int tfl_cnn_create_model_ex(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t
                             const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
                             int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
                             const float* const* weights, const float* const* biases, tfl_cnn** out);
+/* The non-linearity 'relu6' and batch normalization (lib/model.lua:316-350, lib/model_utils.lua:22-62).
+ * relu6: nonlinType 'relu6', nn.ReLU6 = min(max(x, 0), 6) after every convolution but the last (nonlin_sigmoid must
+ * be 0).  batch_norm: addBatchNorm; every stage but the last, and every bank of a banked stage, ends with
+ * {Spatial,Volumetric}BatchNormalization over its osize channels: convolution -> non-linearity -> pooling -> BN, after
+ * the pixel shuffle of an upsampling stage, at the stage's output resolution (a multi-resolution bank at its own
+ * resolution, before the join).  bn[i] (HOST) belongs to convolution i in the order of `weights`, every one but the
+ * last: [4][c] floats = weight, bias (1 and 0 for a module built without batchNormAffine), running_mean, running_var;
+ * eps[i] its eps (batchNormEps, default 1e-4).
+ * batch_stats = 1 for modules saved with train = true, the nn.Module default: the reference's simulators never call
+ * evaluate(), so such a module normalises with the statistics of the batch it is given -- per channel, the mean and
+ * the biased variance over all batch entries and voxels, y = (x - mean) / sqrt(var + eps) w + b, with 1 / sqrt taken
+ * as 0 where var + eps == 0.  The entries of a batch are then coupled: entry 0's output depends on entry 1's input.
+ * Batch statistics are summed in fp64 in a fixed order, so a result is the same bits on every run.  A training-mode
+ * forward of the reference also updates the running averages; no output reads them, and the library does not update
+ * them.  batch_stats = 0 (train = false): y = (x - running_mean) / sqrt(running_var + eps) w + b.
+ * These models run on whole grids (tfl_cnn_project, tfl_simulate_step, step graphs, tfl_host_sim_step): on the fp32
+ * path for every graph and, for the 3-D 'default' graph, on the tensor cores (3xTF32 by default, TF32; relu6 also with
+ * banks split 1 / join 3, batch normalization single-bank only), where running statistics apply in the layers'
+ * epilogues and fold into the 1x1x1 tail, and batch statistics take passes of their own over each layer's output
+ * (also inside the fused step).  tfl_cnn_set_mode refuses the tensor-core modes for banked models with batch
+ * normalization, and the z-slab entry points refuse every model with batch normalization.  norm == NULL, or all its fields 0: exactly tfl_cnn_create_model_ex.  Refused by name:
+ * relu6 with nonlin_sigmoid, a missing bn / eps array or entry where batch_norm is set, a negative eps. */
+typedef struct tfl_cnn_norm {
+  int32_t relu6;
+  int32_t batch_norm;
+  int32_t batch_stats;            /* 1: batch statistics (train = true); 0: running statistics */
+  const float* const* bn;         /* one per convolution but the last: [4][c] weight, bias, running_mean, running_var */
+  const float* eps;               /* one per BN module */
+} tfl_cnn_norm;
+int tfl_cnn_create_model_norm(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                              int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                              const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
+                              tfl_cnn** out);
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* cnn);
 /* Arithmetic of the convolution stack: 0 = fp32 FMA on the CUDA cores; 1 = TF32 tensor cores
  * (wgmma, fp32 accumulate); 2 = 3xTF32 tensor cores (error-compensated split, fp32-class
  * accuracy; the default where available).  Modes 1 and 2 cover the 3-D 'default' architecture, single-bank
- * or with banks split at stage 1 and joined at stage 3. */
+ * or with banks split at stage 1 and joined at stage 3 (with batch normalization: single-bank only). */
 int tfl_cnn_set_mode(tfl_ctx* ctx, tfl_cnn* cnn, int mode);
 int tfl_cnn_get_mode(const tfl_cnn* cnn);
 /* model:forward({pDiv, UDiv, flags}) -> {p, U} (lib/model.lua:421-450).  threshold is
