@@ -270,6 +270,8 @@ int tfl_sync(tfl_ctx* ctx) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (conv_tc_take_z_fault(ctx->stream))
+    return fail(ctx, "internal error, the z-streaming tensor-core convolution's pipeline stalled (a bounded wait ran out)");
   return 0;
 }
 int64_t tfl_launch_count(const tfl_ctx* ctx) { return ctx ? ctx->launches : 0; }

@@ -15,6 +15,8 @@ constexpr char kSlabDilate[] =
     "the z-slab projection does not run banksType 'dilate' (dilated banks run on whole grids only)";
 constexpr char kSlabBatchNorm[] =
     "the z-slab projection does not run batch normalization (addBatchNorm models run on whole grids only)";
+constexpr char kConvZStalled[] =
+    "internal error, the z-streaming tensor-core convolution's pipeline stalled (a bounded wait ran out)";
 constexpr char kSlabDefaultInputs[] =
     "the z-slab projection takes the default input block only (inputChannels pDiv, div, flags; normalizeInput with "
     "'std' of UDiv; no addPressureSkip)";
@@ -141,6 +143,7 @@ int finish_debug(tfl_ctx* ctx, const char* what) {
   const cudaError_t se = cudaStreamSynchronize(ctx->stream);
   if (rc) return rc;
   if (se != cudaSuccess) return fail(ctx, "%s: %s", what, cudaGetErrorString(se));
+  if (conv_tc_take_z_fault(ctx->stream)) return fail(ctx, "%s: %s", what, kConvZStalled);
   return 0;
 }
 
@@ -743,6 +746,14 @@ int tfl_debug_conv3_tc(tfl_ctx* ctx, const float* in, float* out, float* p_net, 
   release();
   if (rc) return rc;
   if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc: %s", cudaGetErrorString(se));
+  if (conv_tc_take_z_fault(ctx->stream)) return fail(ctx, "debug_conv3_tc: %s", kConvZStalled);
+  return 0;
+}
+
+// Undocumented test hook (not in tfl.h): caps the persistent grid of the z-streaming tensor-core convolution at
+// `ctas` CTAs (0: one per SM), so that every CTA runs several work items back to back.
+int tfl_debug_conv_tc_z_grid(int ctas) {
+  conv_tc_set_z_grid(ctas);
   return 0;
 }
 

@@ -29,13 +29,15 @@
 // the other's math (the boxes are sized so that two fit the SM's 228 KB of shared memory).  The
 // box kernel k_conv3_tc runs the join layer of banked models and layers 1-3 at nx > kWWMax.
 //
-// Layers 1-3 at nx <= kWWMax (k_conv3_tc_z): a persistent CTA (one per SM, four warpgroups) takes
-// work items of TY output rows x the whole row x ZC output planes x one batch entry and streams
-// along z through a ring of three staged planes.  A staged row is padded x = 1 .. ww (ww = 64 or
-// kWWMax), so no x halo is staged or computed: D of the zero border voxels x = 0 and x = nx + 1 is
-// zero and the epilogue uses 0 for it, and at nx = 128 a row is exactly two M tiles of 64.  The
-// next plane is loaded into registers while the current plane's MMAs run and is split and stored
-// after them, between two __syncthreads per plane.
+// Layers 1-3 at nx <= kWWMax (k_conv3_tc_z): a persistent CTA (one per SM, four consumer warpgroups
+// and one producer warpgroup) takes work items of TY output rows x the whole row x ZC output planes x
+// one batch entry and streams along z through a ring of three staged planes.  A staged row is padded
+// x = 1 .. ww (ww = 64 or kWWMax), so no x halo is staged or computed: D of the zero border voxels
+// x = 0 and x = nx + 1 is zero and the epilogue uses 0 for it, and at nx = 128 a row is exactly two M
+// tiles of 64.  The producer loads the next plane into registers, splits and stores it as soon as the
+// consumers have released its slot (mbarrier `empty`) and hands it over (mbarrier `full`); the
+// consumers release a slot as soon as their MMAs on it have completed, so that their epilogues overlap
+// the producer's stores and the other warpgroups' MMAs.
 #include <cuda_runtime.h>
 #include <stdint.h>
 
@@ -82,10 +84,26 @@ template <int IN_PLANES, bool SPLIT> struct Layout {
   static constexpr int BYTES = A_BYTES + B_BYTES + 2 * 64 * kDPitch * 4 + 4 * 96;
 };
 
-// Layers 1-3 at nx <= kWWMax: four warpgroups; a staged row holds ww = 64 or kWWMax positions.
-constexpr int kZWarpGroups = 4;
-constexpr int kZThreads = 128 * kZWarpGroups;
+// Layers 1-3 at nx <= kWWMax: four consumer warpgroups (the MMAs and the epilogues) and one producer warpgroup
+// (loads, hi / lo split and stores of the staged planes); a staged row holds ww = 64 or kWWMax positions.
+constexpr int kZWarpGroups = 4;                             // consumers
+constexpr int kZThreads = 128 * (kZWarpGroups + 1);
 constexpr int kWWMax = 128;
+// Registers per thread: 640 threads launch with 96 (65536 / 640, rounded down to the allocation unit of 8), then
+// setmaxnreg moves them between the warpgroups.  3xTF32: the producer holds one plane (6 positions x 2 float4 per
+// thread) in 64, the consumers get 104 (128 x 64 + 512 x 104 = 640 x 96).  TF32 stages 10 rows per plane (10 positions
+// x 2 float4 per producer thread), so there the producer takes 128 and the consumers, with one accumulator set of 12,
+// keep 88.
+constexpr int kZLaunchRegs = 96;
+template <bool SPLIT> struct ZRegs {
+  static constexpr int PRODUCER = SPLIT ? 64 : 128;
+  static constexpr int CONSUMER = SPLIT ? 104 : 88;
+  static_assert(128 * PRODUCER + 128 * kZWarpGroups * CONSUMER <= kZThreads * kZLaunchRegs, "register file");
+};
+// Bounded mbarrier waits: a wait that has not completed after this many clock cycles (about a second) records a fault
+// in g_tc_z_fault, and every later wait of the CTA returns at once, so a pipeline bug ends the kernel with an error
+// instead of hanging the device.
+constexpr long long kZSpinCycles = 1ll << 31;
 
 // Shared memory of k_conv3_tc_z for staged rows of ww positions:
 //   ring   3 slots; a slot is one staged padded plane, PY rows x ww positions, as two 16-byte K chunks
@@ -97,7 +115,8 @@ constexpr int kWWMax = 128;
 //          rows (dz, dy) = (1, -1) / (1, 0) of chunk 0 (LBO = one row), group 4 is the single tap (1, 1)
 //          whose chunk 1 reads 64 zero positions (its B rows are zero too, but 0 * NaN would not be);
 //   zeros  (layer 1) 64 positions;
-//   B      the weight groups; D: one row buffer of ww x kDPitch floats per warpgroup; then bias / tail.
+//   B      the weight groups; D: one row buffer of ww x kDPitch floats per consumer warpgroup; then bias / tail;
+//   bars   mbarriers full[3], empty[3] of the ring slots and the CTA's abort flag (64 bytes).
 template <int IN_PLANES, bool SPLIT> struct ZLayout {
   static constexpr int TY = SPLIT ? 4 : 8;      // output rows of a work item
   static constexpr int PY = TY + 2;
@@ -109,7 +128,7 @@ template <int IN_PLANES, bool SPLIT> struct ZLayout {
   static constexpr int SLOT_CHUNKS = SPLIT ? 4 : 2;
   static constexpr size_t bytes(int ww) {
     return (size_t)3 * SLOT_CHUNKS * PY * ww * 16 + ZERO_BYTES + B_BYTES + (size_t)kZWarpGroups * ww * kDPitch * 4 +
-           4 * 96;
+           4 * 96 + 64;
   }
 };
 
@@ -170,6 +189,40 @@ __device__ __forceinline__ void wgmma_n48(float (&d)[24], uint64_t da, uint64_t 
 __device__ __forceinline__ void wg_barrier(int id) {
   asm volatile("bar.sync %0, 128;" ::"r"(id) : "memory");
 }
+__device__ __forceinline__ void mbar_init(uint32_t bar, int count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint32_t bar) {
+  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.shared::cta.b64 st, [%0];\n\t}" ::"r"(bar) : "memory");
+}
+__device__ __forceinline__ bool mbar_try_wait(uint32_t bar, uint32_t parity) {
+  uint32_t done;
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
+      "selp.u32 %0, 1, 0, p;\n\t}"
+      : "=r"(done)
+      : "r"(bar), "r"(parity)
+      : "memory");
+  return done != 0;
+}
+
+__device__ unsigned int g_tc_z_fault = 0;   // k_conv3_tc_z: 1 once a wait of its pipeline ran out (kZSpinCycles)
+
+// Waits for the completion of phase `parity` of the mbarrier at `bar`, for at most kZSpinCycles.  A wait that runs
+// out records the fault and raises the CTA's abort flag; once it is raised, every wait returns at once.
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity, volatile int* abort) {
+  if (mbar_try_wait(bar, parity)) return;
+  const long long t0 = clock64();
+  while (!mbar_try_wait(bar, parity)) {
+    if (*abort) return;
+    if (clock64() - t0 > kZSpinCycles) {
+      *abort = 1;
+      atomicOr(&g_tc_z_fault, 1u);
+      return;
+    }
+  }
+}
 __device__ __forceinline__ float4 tf32_hi(float4 v) {
   float4 h;
   h.x = __uint_as_float(__float_as_uint(v.x) & 0xFFFFE000u);
@@ -229,6 +282,15 @@ __device__ __forceinline__ void conv_epilogue(float (&h)[4], bool valid, int hal
 }
 
 // Layers 1-3 (see the file comment and ZLayout).
+//
+// Pipeline.  The CTA numbers the planes it stages across all of its work items, q = 0, 1, ...; plane q lives in
+// ring slot q % 3.  full[s] completes (one arrival, the producer's) when the slot holds its plane; empty[s]
+// completes (four arrivals, one per consumer warpgroup) when every consumer is done with it.  Both count their
+// phases per slot, across planes and work items: use k = q / 3 of slot q % 3 waits for phase k & 1 of full and,
+// before the producer overwrites the slot, for phase (k - 1) & 1 of empty.  An item with output planes [za, zb)
+// stages the padded planes za .. zb + 1; output plane z reads planes z, z + 1, z + 2 and a consumer releases plane z
+// when the MMAs of output plane z have completed (planes zb, zb + 1 after the item's last output plane), so every
+// consumer warpgroup arrives on every staged plane exactly once and only after it has waited for that plane.
 template <int IN_PLANES, bool FINAL, bool SPLIT>
 __global__ void __launch_bounds__(kZThreads, 1)
 k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __restrict__ p_net,
@@ -236,6 +298,7 @@ k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __r
              ConvTcGeo g, ZSched s, TcEpi ep) {
   extern __shared__ __align__(1024) uint8_t smem[];
   using L = ZLayout<IN_PLANES, SPLIT>;
+  using R = ZRegs<SPLIT>;
   constexpr int TY = L::TY, PY = L::PY;
   const int ww = s.ww, ntile = ww >> 6;
   const int gbytes = PY * ww * 16;                    // one K chunk of a slot
@@ -246,40 +309,61 @@ k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __r
   uint8_t* sB = sZero + L::ZERO_BYTES;
   float* sD = (float*)(sB + L::B_BYTES);              // [kZWarpGroups][ww][kDPitch]
   float* sTail = sD + kZWarpGroups * ww * kDPitch;    // bias[8] (+ w4[64] b4[8] w5[8] b5[1] when FINAL)
+  uint64_t* sBar = (uint64_t*)(sTail + 96);           // full[3], empty[3]
+  volatile int* sAbort = (volatile int*)(sBar + 6);
 
   const int tid = threadIdx.x, warp = tid >> 5, lane = tid & 31;
-  long long* dbg = g_tc_dbg;
-  if (dbg && tid == 0) dbg[blockIdx.x * 8 + 0] = clock64();
 
-  for (int i = tid; i < L::ZERO_BYTES / 16; i += kZThreads) ((float4*)sZero)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
-  for (int i = tid; i < L::B_BYTES / 16; i += kZThreads) ((float4*)sB)[i] = __ldg((const float4*)wB + i);
-  const int n_tail = FINAL ? (8 + 64 + 8 + 8 + 1) : 8;
-  for (int i = tid; i < n_tail; i += kZThreads) sTail[i] = (i < 8) ? bias[i] : tail[i - 8];
-  if (!FINAL && ep.ac && tid < 16) sTail[8 + tid] = ep.ac[tid];
+  const uint32_t bar_u = smem_u32(sBar);              // full[k] at bar_u + 8 k, empty[k] at bar_u + 24 + 8 k
+  // Zeros, B, bias / tail and the mbarriers, by all threads.  Each role calls this after its setmaxnreg, so that
+  // nothing is live across the register hand-over.
+  auto setup = [&]() {
+    for (int i = tid; i < L::ZERO_BYTES / 16; i += kZThreads) ((float4*)sZero)[i] = make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll 1
+    for (int i = tid; i < L::B_BYTES / 16; i += kZThreads) ((float4*)sB)[i] = __ldg((const float4*)wB + i);
+    const int n_tail = FINAL ? (8 + 64 + 8 + 8 + 1) : 8;
+    for (int i = tid; i < n_tail; i += kZThreads) sTail[i] = (i < 8) ? bias[i] : tail[i - 8];
+    if (!FINAL && ep.ac && tid < 16) sTail[8 + tid] = ep.ac[tid];
+    if (tid == 0) {
+      for (int k = 0; k < 3; k++) {
+        mbar_init(bar_u + 8 * k, 1);
+        mbar_init(bar_u + 24 + 8 * k, kZWarpGroups);
+      }
+      *sAbort = 0;
+    }
+    // generic-proxy writes (st.shared: zeros, B) -> visible to the wgmma (async proxy) reads
+    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+    __syncthreads();
+  };
 
   const long long plane_g = (long long)(g.nz + 2) * g.py * g.px;            // float4 per global plane
   const long long batch_g = plane_g * 2;
   const int npos = PY * ww;                                                 // staged positions of a plane
-  constexpr int PER = (PY * kWWMax + kZThreads - 1) / kZThreads;
-  float4 v[PER][IN_PLANES];
-
   const int wg = warp >> 2, wq = warp & 3;
-  const uint32_t sRing_u = smem_u32(sRing), sB_u = smem_u32(sB), sZero_u = smem_u32(sZero);
-  float* myD = sD + wg * ww * kDPitch;
-  const int tw = tid & 127, half = tw & 1;
-  const float* bs = sTail + 4 * half;
+  const int tw = tid & 127;
+  // work item -> first padded row y0, output planes [za, zb), batch entry b
+  auto item_geo = [&](int item, int& y0, int& za, int& zb, int& b) {
+    const int ty = item % s.nty, zc = (item / s.nty) % s.nzc;
+    b = item / s.nty / s.nzc;
+    y0 = ty * TY;
+    za = g.z_lo + zc * s.zc;
+    zb = min(za + s.zc, g.z_hi);
+  };
 
-  for (int item = blockIdx.x; item < s.items; item += gridDim.x) {
-    const int ty = item % s.nty, zc = (item / s.nty) % s.nzc, b = item / s.nty / s.nzc;
-    const int y0 = ty * TY;                                             // padded row of staged row 0
-    const int za = g.z_lo + zc * s.zc, zb = min(za + s.zc, g.z_hi);     // output planes [za, zb)
-    const float4* inb = in + b * batch_g;
-
-    // padded plane pz -> registers (positions outside the buffer read the zero border voxel (0, 0, 0))
-    auto load = [&](int pz) {
+  if (wg == kZWarpGroups) {
+    // ---- producer ------------------------------------------------------------------------------------------
+    if constexpr (R::PRODUCER < kZLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R::PRODUCER));
+    if constexpr (R::PRODUCER > kZLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R::PRODUCER));
+    setup();
+    constexpr int PER = (PY * kWWMax + 127) / 128;
+    float4 v[PER][IN_PLANES];
+    // padded plane pz of the item at (y0, b) -> registers (positions outside the buffer read the zero border voxel
+    // (0, 0, 0))
+    auto load = [&](int y0, int b, int pz) {
+      const float4* inb = in + b * batch_g;
 #pragma unroll
       for (int it = 0; it < PER; it++) {
-        const int idx = tid + it * kZThreads;
+        const int idx = tw + it * 128;
         const int row = idx / ww, gx = 1 + idx - row * ww, gy = y0 + row;
         const bool inside = idx < npos && gx < g.px && gy < g.py;
         const long long go = inside ? ((long long)pz * g.py + gy) * g.px + gx : 0;
@@ -287,18 +371,21 @@ k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __r
         for (int h = 0; h < IN_PLANES; h++) v[it][h] = __ldg(inb + h * plane_g + go);
       }
     };
-    // registers -> slot pz % 3 (layer 1: also chunk 1 of plane pz - 1's slot), split into hi / lo when SPLIT
-    auto store = [&](int pz) {
-      uint8_t* slot = sRing + (pz % 3) * slot_bytes;
-      uint8_t* prev = sRing + ((pz + 2) % 3) * slot_bytes;
+    int item = blockIdx.x, y0, za, zb, b;
+    if (item < s.items) {
+      item_geo(item, y0, za, zb, b);
+      load(y0, b, za);
+    }
+    for (int q = 0, pz = za; item < s.items; q++) {
+      const int slot = q % 3;
+      // registers -> K chunk c of a slot, split into hi / lo when SPLIT
+      auto put = [&](uint8_t* slot_p, int c) {
 #pragma unroll
-      for (int it = 0; it < PER; it++) {
-        const int idx = tid + it * kZThreads;
-        if (idx < npos) {
-#pragma unroll
-          for (int c = 0; c < 2; c++) {
+        for (int it = 0; it < PER; it++) {
+          const int idx = tw + it * 128;
+          if (idx < npos) {
             const float4 w = v[it][IN_PLANES == 2 ? c : 0];
-            uint8_t* dst = (IN_PLANES == 1 && c == 1 ? prev : slot) + c * gbytes + idx * 16;
+            uint8_t* dst = slot_p + c * gbytes + idx * 16;
             if constexpr (SPLIT) {
               const float4 hi = tf32_hi(w);
               *(float4*)dst = hi;
@@ -308,106 +395,160 @@ k_conv3_tc_z(const float4* __restrict__ in, float4* __restrict__ out, float* __r
             }
           }
         }
+      };
+      // Layer 1 also writes the plane as K chunk 1 of the previous plane's slot (q - 1) % 3, before this plane's own
+      // slot is free (not for an item's first plane: no output plane reads it with its predecessor).  Chunk 1 of
+      // that slot was last read for output plane pz - 4, whose MMAs completed before the previous plane was stored;
+      // it is read next for output plane pz - 1, after this plane's `full`.  Its chunk 0 (plane pz - 1) may still be
+      // in use as base[2] of output plane pz - 3 while this runs, which is safe only because groups 3 and 4 never read
+      // K chunk 1 of base[2]: group 3's second chunk is one row further inside chunk 0 and group 4's is the zero
+      // block.  Keep it so.
+      if (IN_PLANES == 1 && pz > za) put(sRing + ((q + 2) % 3) * slot_bytes, 1);
+      if (q >= 3) mbar_wait(bar_u + 24 + 8 * slot, ((q / 3) - 1) & 1, sAbort);
+      put(sRing + slot * slot_bytes, 0);
+      if (IN_PLANES == 2) put(sRing + slot * slot_bytes, 1);
+      // generic-proxy writes (st.shared) -> visible to the wgmma (async proxy) reads; then one arrival for all
+      asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
+      wg_barrier(1 + kZWarpGroups);
+      if (tw == 0) mbar_arrive(bar_u + 8 * slot);
+      // the next plane (of this item, else of the next one) is in flight while the consumers work
+      if (++pz > zb + 1) {
+        item += gridDim.x;
+        if (item >= s.items) break;
+        item_geo(item, y0, za, zb, b);
+        pz = za;
       }
+      load(y0, b, pz);
+    }
+  } else {
+    // ---- consumers ------------------------------------------------------------------------------------------
+    if constexpr (R::CONSUMER > kZLaunchRegs) asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(R::CONSUMER));
+    if constexpr (R::CONSUMER < kZLaunchRegs) asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(R::CONSUMER));
+    long long* dbg = g_tc_dbg;
+    if (dbg && tid == 0) dbg[blockIdx.x * 8 + 0] = clock64();
+    setup();
+    const uint32_t sRing_u = smem_u32(sRing), sB_u = smem_u32(sB), sZero_u = smem_u32(sZero);
+    float* myD = sD + wg * ww * kDPitch;
+    const int half = tw & 1;
+    const float* bs = sTail + 4 * half;
+    int qa = 0;                 // sequence number of the item's first staged plane
+    int waited = 0;             // planes q < waited are known to be in their slots
+    auto wait_plane = [&](int q) {
+      for (; waited <= q; waited++) mbar_wait(bar_u + 8 * (waited % 3), (waited / 3) & 1, sAbort);
     };
+    auto release_plane = [&](int q) {
+      if (tw == 0) mbar_arrive(bar_u + 24 + 8 * (q % 3));
+    };
+    for (int item = blockIdx.x; item < s.items; item += gridDim.x) {
+      int y0, za, zb, b;
+      item_geo(item, y0, za, zb, b);
+      const bool has_rows = y0 + wg < g.ny;   // warpgroup wg takes rows wg, wg + 4, ...
 
-    // output plane z reads padded planes z, z + 1, z + 2
-    for (int k = 0; k < 3; k++) {
-      load(za + k);
-      store(za + k);
-    }
-    // generic-proxy writes (st.shared) -> visible to the wgmma (async proxy) reads
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-    __syncthreads();
-    if (dbg && tid == 0 && item == blockIdx.x) dbg[blockIdx.x * 8 + 1] = clock64();
+      for (int z = za; z < zb; z++) {
+        const int qz = qa + (z - za);            // padded plane z; the output plane reads qz .. qz + 2
+        uint32_t base[3];                        // slot of padded plane z + 1 + dz
+#pragma unroll
+        for (int d = 0; d < 3; d++) base[d] = sRing_u + (uint32_t)(((qz + d) % 3) * slot_bytes);
+        wait_plane(qz + 1);
+        if (dbg && tid == 0 && item == blockIdx.x && z == za) dbg[blockIdx.x * 8 + 1] = clock64();
+        if (!has_rows) {
+          wait_plane(qz + 2);
+          release_plane(qz);
+          continue;
+        }
 
-    for (int z = za; z < zb; z++) {
-      const bool more = z + 1 < zb;
-      if (more) load(z + 3);                       // in flight during this plane's MMAs
-      uint32_t base[3];                            // slot of padded plane z + 1 + dz
+        // a row is ntile M tiles of 64 positions
+        for (int r = wg; r < TY && y0 + r < g.ny; r += kZWarpGroups) {
+          const bool last_row = r + kZWarpGroups >= TY || y0 + r + kZWarpGroups >= g.ny;
+          for (int t = 0; t < ntile; t++) {
+            const uint32_t row_off = (uint32_t)(((r + 1) * ww + 64 * t) * 16);
+            float acc[SPLIT ? 24 : 12] = {}, acl[12] = {};
+            asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
 #pragma unroll
-      for (int d = 0; d < 3; d++) base[d] = sRing_u + (uint32_t)(((z + d) % 3) * slot_bytes);
-
-      // warpgroup wg takes rows wg, wg + 4, ...; a row is ntile M tiles of 64 positions
-      for (int r = wg; r < TY && y0 + r < g.ny; r += kZWarpGroups) {
-        for (int t = 0; t < ntile; t++) {
-          const uint32_t row_off = (uint32_t)(((r + 1) * ww + 64 * t) * 16);
-          float acc[SPLIT ? 24 : 12] = {}, acl[12] = {};
-          asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
-#pragma unroll
-          for (int gi = 0; gi < L::GROUPS; gi++) {
-            const int dz = IN_PLANES == 1 ? layer1_dz(gi) : gi / 3 - 1;
-            const int dy = IN_PLANES == 1 ? layer1_dy(gi) : gi % 3 - 1;
-            const uint32_t a = base[1 + dz] + row_off + (uint32_t)(dy * ww * 16);
-            const bool zero_k1 = IN_PLANES == 1 && gi == 4;
-            const uint32_t lbo = IN_PLANES == 1 && gi == 3 ? (uint32_t)(ww * 16) : zero_k1 ? sZero_u - a : (uint32_t)gbytes;
-            const uint64_t da = make_desc(a, lbo, 128);
-            const uint64_t db = make_desc(sB_u + gi * L::B_GROUP_BYTES, L::NB * 16, 128);
-            if constexpr (SPLIT) {
-              const uint32_t al = a + (uint32_t)lo_off;
-              wgmma_n48(acc, da, db, gi > 0 ? 1u : 0u);
-              wgmma_n24(acl, make_desc(al, zero_k1 ? sZero_u - al : lbo, 128), db, gi > 0 ? 1u : 0u);
-            } else {
-              wgmma_n24(acc, da, db, gi > 0 ? 1u : 0u);
-            }
-          }
-          asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
-          asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
-          if (dbg && tid == 0 && item == blockIdx.x && z == za && t == 0) dbg[blockIdx.x * 8 + 2] = clock64();
-
-          // accumulator fragment: element (row 16 wq + lane / 4 + 8 i, column 8 k + 2 (lane % 4) + j) is acc[4 k + 2 i + j]
-          float* tD = myD + 64 * t * kDPitch;
-#pragma unroll
-          for (int k = 0; k < 3; k++)
-#pragma unroll
-            for (int i = 0; i < 2; i++) {
-              const int row = 16 * wq + (lane >> 2) + 8 * i, col = 8 * k + 2 * (lane & 3);
-              float2 d2;
-              if constexpr (SPLIT) {
-                d2.x = acc[4 * k + 2 * i] + (acc[12 + 4 * k + 2 * i] + acl[4 * k + 2 * i]);
-                d2.y = acc[4 * k + 2 * i + 1] + (acc[12 + 4 * k + 2 * i + 1] + acl[4 * k + 2 * i + 1]);
-              } else {
-                d2.x = acc[4 * k + 2 * i];
-                d2.y = acc[4 * k + 2 * i + 1];
+            for (int gi = 0; gi < L::GROUPS; gi++) {
+              // The groups of padded plane z + 2 (dz = +1) wait until that plane is in its slot, so that the groups
+              // of planes z and z + 1 run while the producer stores it.  The groups before are committed first:
+              // ptxas serialises every wgmma of the sequence when uncommitted ones are in flight across the wait.
+              if (gi == (IN_PLANES == 1 ? 3 : 6)) {
+                asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+                wait_plane(qz + 2);
+                asm volatile("wgmma.fence.sync.aligned;" ::: "memory");
               }
-              *(float2*)(tD + row * kDPitch + col) = d2;
+              const int dz = IN_PLANES == 1 ? layer1_dz(gi) : gi / 3 - 1;
+              const int dy = IN_PLANES == 1 ? layer1_dy(gi) : gi % 3 - 1;
+              const uint32_t a = base[1 + dz] + row_off + (uint32_t)(dy * ww * 16);
+              const bool zero_k1 = IN_PLANES == 1 && gi == 4;
+              const uint32_t lbo = IN_PLANES == 1 && gi == 3 ? (uint32_t)(ww * 16) : zero_k1 ? sZero_u - a : (uint32_t)gbytes;
+              const uint64_t da = make_desc(a, lbo, 128);
+              const uint64_t db = make_desc(sB_u + gi * L::B_GROUP_BYTES, L::NB * 16, 128);
+              if constexpr (SPLIT) {
+                const uint32_t al = a + (uint32_t)lo_off;
+                wgmma_n48(acc, da, db, gi > 0 ? 1u : 0u);
+                wgmma_n24(acl, make_desc(al, zero_k1 ? sZero_u - al : lbo, 128), db, gi > 0 ? 1u : 0u);
+              } else {
+                wgmma_n24(acc, da, db, gi > 0 ? 1u : 0u);
+              }
             }
-        }
-        wg_barrier(1 + wg);
+            asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory");
+            asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory");
+            if (dbg && tid == 0 && item == blockIdx.x && z == za && t == 0) dbg[blockIdx.x * 8 + 2] = clock64();
+            // this warpgroup's last MMAs on padded plane z: its slot may be refilled while D goes out
+            if (last_row && t == ntile - 1) release_plane(qz);
 
-        // epilogue: staged position i (padded x = i + 1), channels 4 half .. 4 half + 3; D of the zero border
-        // voxels x = 0 and x = nx + 1 is 0
-        const int yg = y0 + r;
-        for (int j = 0; j < ntile; j++) {
-          const int i = (tw >> 1) + 64 * j, xp = i + 1;
-          const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-          const float4 dm = i >= 1 ? *(const float4*)(myD + (i - 1) * kDPitch + 4 * half) : zero4;
-          const float4 d0 = *(const float4*)(myD + i * kDPitch + 8 + 4 * half);
-          const float4 dp = xp < g.nx ? *(const float4*)(myD + (i + 1) * kDPitch + 16 + 4 * half) : zero4;
-          float h[4];
-          h[0] = (dm.x + d0.x) + dp.x + bs[0];
-          h[1] = (dm.y + d0.y) + dp.y + bs[1];
-          h[2] = (dm.z + d0.z) + dp.z + bs[2];
-          h[3] = (dm.w + d0.w) + dp.w + bs[3];
-          conv_epilogue<FINAL>(h, xp <= g.nx, half, sTail, out, p_net,
-                               b * batch_g + ((long long)(z + 1) * g.py + (yg + 1)) * g.px + xp, plane_g,
-                               (long long)b * g.nz * g.ny * g.nx + ((long long)z * g.ny + yg) * g.nx + (xp - 1), ep);
+            // accumulator fragment: element (row 16 wq + lane / 4 + 8 i, column 8 k + 2 (lane % 4) + j) is acc[4 k + 2 i + j]
+            float* tD = myD + 64 * t * kDPitch;
+#pragma unroll
+            for (int k = 0; k < 3; k++)
+#pragma unroll
+              for (int i = 0; i < 2; i++) {
+                const int row = 16 * wq + (lane >> 2) + 8 * i, col = 8 * k + 2 * (lane & 3);
+                float2 d2;
+                if constexpr (SPLIT) {
+                  d2.x = acc[4 * k + 2 * i] + (acc[12 + 4 * k + 2 * i] + acl[4 * k + 2 * i]);
+                  d2.y = acc[4 * k + 2 * i + 1] + (acc[12 + 4 * k + 2 * i + 1] + acl[4 * k + 2 * i + 1]);
+                } else {
+                  d2.x = acc[4 * k + 2 * i];
+                  d2.y = acc[4 * k + 2 * i + 1];
+                }
+                *(float2*)(tD + row * kDPitch + col) = d2;
+              }
+          }
+          wg_barrier(1 + wg);
+
+          // epilogue: staged position i (padded x = i + 1), channels 4 half .. 4 half + 3; D of the zero border
+          // voxels x = 0 and x = nx + 1 is 0
+          const int yg = y0 + r;
+          for (int j = 0; j < ntile; j++) {
+            const int i = (tw >> 1) + 64 * j, xp = i + 1;
+            const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
+            const float4 dm = i >= 1 ? *(const float4*)(myD + (i - 1) * kDPitch + 4 * half) : zero4;
+            const float4 d0 = *(const float4*)(myD + i * kDPitch + 8 + 4 * half);
+            const float4 dp = xp < g.nx ? *(const float4*)(myD + (i + 1) * kDPitch + 16 + 4 * half) : zero4;
+            float h[4];
+            h[0] = (dm.x + d0.x) + dp.x + bs[0];
+            h[1] = (dm.y + d0.y) + dp.y + bs[1];
+            h[2] = (dm.z + d0.z) + dp.z + bs[2];
+            h[3] = (dm.w + d0.w) + dp.w + bs[3];
+            conv_epilogue<FINAL>(h, xp <= g.nx, half, sTail, out, p_net,
+                                 b * batch_g + ((long long)(z + 1) * g.py + (yg + 1)) * g.px + xp, plane_g,
+                                 (long long)b * g.nz * g.ny * g.nx + ((long long)z * g.ny + yg) * g.nx + (xp - 1), ep);
+          }
+          wg_barrier(1 + wg);                    // myD is rewritten by the next row
         }
-        wg_barrier(1 + wg);                        // myD is rewritten by the next row
       }
-      __syncthreads();                             // every warpgroup is done with padded plane z's slot
-      if (more) {
-        store(z + 3);
-        asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-      }
-      __syncthreads();
+      // padded planes zb, zb + 1 are read by no later output plane of the item
+      const int qb = qa + (zb - za);
+      wait_plane(qb + 1);
+      release_plane(qb);
+      release_plane(qb + 1);
+      qa = qb + 2;
     }
-  }
-  if (dbg && tid == 0) {
-    dbg[blockIdx.x * 8 + 5] = clock64();
-    unsigned smid;
-    asm("mov.u32 %0, %%smid;" : "=r"(smid));
-    dbg[blockIdx.x * 8 + 7] = smid;
+    if (dbg && tid == 0) {
+      dbg[blockIdx.x * 8 + 5] = clock64();
+      unsigned smid;
+      asm("mov.u32 %0, %%smid;" : "=r"(smid));
+      dbg[blockIdx.x * 8 + 7] = smid;
+    }
   }
 }
 
@@ -732,6 +873,8 @@ ZSched z_schedule(const ConvTcGeo& g, int ty, int nsm) {
   return s;
 }
 
+int g_z_grid_cap = 0;           // test hook: at most this many CTAs in a k_conv3_tc_z grid (0: one per SM)
+
 template <int IN_PLANES, bool FINAL, bool SPLIT>
 void launch_z(const float4* in, float4* out, float* p_net, const float* wB, const float* bias, const float* tail,
               const ConvTcGeo& g, cudaStream_t st, const TcEpi& ep) {
@@ -747,7 +890,8 @@ void launch_z(const float4* in, float4* out, float* p_net, const float* wB, cons
   }
   cudaDeviceGetAttribute(&nsm, cudaDevAttrMultiProcessorCount, dev);
   const ZSched s = z_schedule(g, L::TY, nsm);
-  const int grid = s.items < nsm ? s.items : nsm;
+  int grid = s.items < nsm ? s.items : nsm;
+  if (g_z_grid_cap > 0 && grid > g_z_grid_cap) grid = g_z_grid_cap;
   kern<<<grid, kZThreads, L::bytes(s.ww), st>>>(in, out, p_net, wB, bias, tail, g, s, ep);
 }
 
@@ -873,6 +1017,19 @@ size_t conv_tc_act_bytes(const ConvTcGeo& g) {
   return (size_t)g.nb * 2 * (g.nz + 2) * g.py * g.px * 16;
 }
 void conv_tc_set_debug(long long* dev_buf) { cudaMemcpyToSymbol(g_tc_dbg, &dev_buf, sizeof(dev_buf)); }
+void conv_tc_set_z_grid(int ctas) { g_z_grid_cap = ctas > 0 ? ctas : 0; }
+int conv_tc_take_z_fault(cudaStream_t st) {
+  unsigned int v = 0;
+  if (cudaMemcpyFromSymbolAsync(&v, g_tc_z_fault, sizeof(v), 0, cudaMemcpyDeviceToHost, st) != cudaSuccess ||
+      cudaStreamSynchronize(st) != cudaSuccess)
+    return 0;                        // a CUDA error is reported by the caller's own checks
+  if (v) {
+    const unsigned int zero = 0;
+    cudaMemcpyToSymbolAsync(g_tc_z_fault, &zero, sizeof(zero), 0, cudaMemcpyHostToDevice, st);
+    cudaStreamSynchronize(st);
+  }
+  return v ? 1 : 0;
+}
 
 int conv_tc_b_floats(int split) { return kGroups * 2 * (split ? 48 : 32) * 4; }
 

@@ -17,6 +17,12 @@ ConvTcGeo make_conv_tc_geo(int nb, int nz, int ny, int nx);
 size_t conv_tc_act_bytes(const ConvTcGeo& g);
 int conv_tc_b_floats(int split);
 void conv_tc_set_debug(long long* dev_buf);   // nullptr disables
+// Test hook: caps the persistent grid of the z-streaming kernel at `ctas` CTAs (0: one per SM), so that every CTA
+// runs several work items.
+void conv_tc_set_z_grid(int ctas);
+// 1 if a z-streaming launch on this device recorded a stalled pipeline (a bounded mbarrier wait ran out) since the
+// last call, 0 otherwise; clears the record.  Synchronises `st`.
+int conv_tc_take_z_fault(cudaStream_t st);
 void conv_tc_pack_weights(const float* w /*[8][cin][3][3][3]*/, int cin, int split, float* out);
 // The epilogue's options: relu6 = 1 clamps every non-linearity of the layer (and of the fused 1x1x1 tail) at 6
 // (nn.ReLU6); ac (device, [2][8]: a then c; non-final layers only, may be null) applies y = a h + c per channel after
