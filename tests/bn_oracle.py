@@ -85,27 +85,47 @@ def _shuffle(x, s_, is3d):
     return np.ascontiguousarray(x).reshape(b_, no, z_, y_ * s_, x_ * s_)
 
 
-def stage(model, li, w, b, x, d=1, bn=None):
+def _rep(a, r, is3d):
+    """Nearest up-sampling by r (the join of an 'mres' bank)."""
+    return np.repeat(np.repeat(np.repeat(a, r, 2), r, 3), r, 4) if is3d else np.repeat(np.repeat(a, r, 3), r, 4)
+
+
+class F64:
+    """The float64 operations `stage` and `network` compose.  tests/network_bound.py substitutes operations on
+    (value, error bound) pairs and a float32 emulation of the library with the same signatures; `li` is the stage
+    index (0-based) of the convolution or BN it belongs to."""
+    lift = staticmethod(lambda x: np.asarray(x, np.float64))
+    conv = staticmethod(lambda x, w, b, is3d, d, li: conv64(x, w, b, is3d, d))
+    shuffle = staticmethod(_shuffle)
+    nonlin = staticmethod(nonlin)
+    pool = staticmethod(_pool)
+    bn = staticmethod(lambda x, e, train, li: batch_norm(x, e, train))
+    up = staticmethod(_rep)
+    concat = staticmethod(lambda hs: np.concatenate(hs, axis=1))
+    add = staticmethod(lambda hs: sum(hs[1:], hs[0]))
+
+
+def stage(model, li, w, b, x, d=1, bn=None, ops=F64):
     """One stage of model.lua:320-350: convolution (dilated by d) -> shuffle -> non-linearity -> pooling -> BN."""
     is3d = model["is3D"]
     nl = len(model["layers"])
     pool = model.get("pool") or [1] * nl
     up = model.get("up") or [1] * nl
-    x = conv64(x, w, b, is3d, d)
+    x = ops.conv(x, w, b, is3d, d, li)
     if up[li] > 1:
-        x = _shuffle(x, up[li], is3d)
+        x = ops.shuffle(x, up[li], is3d)
     if li < nl - 1:
-        x = nonlin(x, model.get("nonlinType", "relu"))
+        x = ops.nonlin(x, model.get("nonlinType", "relu"))
     if pool[li] > 1:
-        x = _pool(x, pool[li], is3d, model.get("poolType", "avg"))
+        x = ops.pool(x, pool[li], is3d, model.get("poolType", "avg"))
     if bn is not None:
-        x = batch_norm(x, bn, model["batchNorm"]["train"])
+        x = ops.bn(x, bn, model["batchNorm"]["train"], li)
     return x
 
 
-def network(model, x, hidden=False):
+def network(model, x, hidden=False, ops=F64):
     """The stages on the network input x -> p_net [b][1][z][y][x] (float64); hidden=True stops before the last
-    convolution and returns its input."""
+    convolution and returns its input.  `ops` (default F64) supplies the operations."""
     is3d = model["is3D"]
     banks = model.get("banks")
     n = banks["num"] if banks else 1
@@ -113,20 +133,16 @@ def network(model, x, hidden=False):
     dil = bool(banks) and banks.get("type") == "dilate"
     bnl = (model.get("batchNorm") or {}).get("layers")
     nl = len(model["layers"])
-    hl = [np.asarray(x, np.float64)]
+    hl = [ops.lift(x)]
     for li, layer in enumerate(model["layers"]):
         lid = li + 1
         if n > 1 and lid == s:
             hl = [hl[0]] * n if dil else [hl[0]]
             for i in range(1, n if not dil else 1):
-                hl.append(_pool(hl[i - 1], 2, is3d, "avg"))
+                hl.append(ops.pool(hl[i - 1], 2, is3d, "avg"))
         if n > 1 and lid == j:
-            ups = hl
-            if not dil:
-                rep = lambda a, r: np.repeat(np.repeat(np.repeat(a, r, 2), r, 3), r, 4) if is3d else \
-                    np.repeat(np.repeat(a, r, 3), r, 4)
-                ups = [hl[0]] + [rep(hl[i], 2 ** i) for i in range(1, n)]
-            hl = [np.concatenate(ups, axis=1)] if banks["aggregate"] == "concat" else [sum(ups[1:], ups[0])]
+            ups = hl if dil else [hl[0]] + [ops.up(hl[i], 2 ** i, is3d) for i in range(1, n)]
+            hl = [ops.concat(ups)] if banks["aggregate"] == "concat" else [ops.add(ups)]
         if hidden and li == nl - 1:
             return hl[0]
         convs = layer if isinstance(layer[0], (tuple, list)) else [layer]
@@ -134,7 +150,7 @@ def network(model, x, hidden=False):
         if bnl is not None and li < nl - 1:
             bns = bnl[li] if isinstance(bnl[li], (tuple, list)) else [bnl[li]]
         assert len(convs) == len(hl) == len(bns)
-        hl = [stage(model, li, w, b, h, 2 ** i if dil else 1, e)
+        hl = [stage(model, li, w, b, h, 2 ** i if dil else 1, e, ops)
               for i, ((w, b), h, e) in enumerate(zip(convs, hl, bns))]
     assert len(hl) == 1
     return hl[0]
