@@ -270,8 +270,7 @@ int tfl_sync(tfl_ctx* ctx) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (conv_tc_take_z_fault(ctx->stream))
-    return fail(ctx, "internal error, the z-streaming tensor-core convolution's pipeline stalled (a bounded wait ran out)");
+  if (conv_tc_take_z_fault(ctx->stream)) return fail(ctx, "%s", kConvZStalled);
   return 0;
 }
 int64_t tfl_launch_count(const tfl_ctx* ctx) { return ctx ? ctx->launches : 0; }
@@ -947,7 +946,7 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
                       u_bc ? s->U_bc.data : nullptr, qmask, 1, sums, g, st);
   const ConvTcGeo& tg = m->act_geo;
   if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in, 0));          // pDiv is first read here
-  launch_cnn_inputs_fused(s->p.data, s->U.data, fl8, sums, mc->normalize_input_threshold, scale, m->act[0],
+  launch_cnn_inputs_fused(s->p.data, s->U.data, fl8, sums, mc->normalize_input_threshold, scale, m->act[0].get(),
                           tg.px, tg.py, g, st);
   run_conv_stack(m, p_net, st);
   launch_cnn_finish_fused(p_net, s->U.data, fl8, scale, s->p.data, u_bc ? s->U_bc_inv_mask.data : nullptr,

@@ -15,23 +15,49 @@ constexpr char kSlabDilate[] =
     "the z-slab projection does not run banksType 'dilate' (dilated banks run on whole grids only)";
 constexpr char kSlabBatchNorm[] =
     "the z-slab projection does not run batch normalization (addBatchNorm models run on whole grids only)";
-constexpr char kConvZStalled[] =
-    "internal error, the z-streaming tensor-core convolution's pipeline stalled (a bounded wait ran out)";
 constexpr char kSlabDefaultInputs[] =
     "the z-slab projection takes the default input block only (inputChannels pDiv, div, flags; normalizeInput with "
     "'std' of UDiv; no addPressureSkip)";
 
+constexpr int kTailFloats = 64 + 8 + 8 + 1;     // the fused 1x1x1 tail: w4[8][8], b4[8], w5[8], b5[1]
+
 namespace {
 
-// Packs a [8][cin][3][3][3] weight for launch_conv3_tc / launch_conv3_tc_join and uploads it; nullptr if the
-// allocation fails.
-float* upload_tc_weights(const float* w, int cin, int split) {
+// n device values, uninitialised; empty if cudaMalloc fails.
+template <typename T>
+DevPtr<T> dev_alloc(size_t n) {
+  T* p = nullptr;
+  if (cudaMalloc((void**)&p, n * sizeof(T)) != cudaSuccess) return DevPtr<T>();
+  return DevPtr<T>(p);
+}
+// n device values set to zero; empty if cudaMalloc or cudaMemset fails.
+template <typename T>
+DevPtr<T> dev_zeros(size_t n) {
+  DevPtr<T> d = dev_alloc<T>(n);
+  if (d && cudaMemset(d.get(), 0, n * sizeof(T)) != cudaSuccess) d.reset();
+  return d;
+}
+// A device copy of host[0, n); empty if cudaMalloc or cudaMemcpy fails.
+template <typename T>
+DevPtr<T> upload(const T* host, size_t n) {
+  DevPtr<T> d = dev_alloc<T>(n);
+  if (d && cudaMemcpy(d.get(), host, n * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) d.reset();
+  return d;
+}
+template <typename T>
+DevPtr<T> upload(const std::vector<T>& host) { return upload(host.data(), host.size()); }
+// Appends p to v; false (and v unchanged) if p is empty, its upload having failed.
+bool keep(std::vector<DevPtr<float>>& v, DevPtr<float> p) {
+  if (!p) return false;
+  v.push_back(std::move(p));
+  return true;
+}
+
+// Packs a [8][cin][3][3][3] weight for launch_conv3_tc / launch_conv3_tc_join and uploads it.
+DevPtr<float> upload_tc_weights(const float* w, int cin, int split) {
   std::vector<float> packed(conv_tc_b_floats(split));
   conv_tc_pack_weights(w, cin, split, packed.data());
-  float* d = nullptr;
-  if (cudaMalloc((void**)&d, packed.size() * 4) != cudaSuccess) return nullptr;
-  cudaMemcpy(d, packed.data(), packed.size() * 4, cudaMemcpyHostToDevice);
-  return d;
+  return upload(packed);
 }
 
 // A convolution weight in Torch layout [cout][cin][taps] re-laid out as the [cin][tap][cout] that
@@ -55,25 +81,17 @@ void bn_running_affine(const tfl_cnn_norm* norm, int wi, int c, double* a, doubl
     cc[ch] = (double)p[c + ch] - (double)p[2 * c + ch] * a[ch];
   }
 }
-int cnn_upload_bn(tfl_ctx* ctx, tfl_cnn* m, const tfl_cnn_norm* norm, int wi, int c) {
+// What the model keeps on the device of convolution wi's batch normalization: bn_wb or bn_ac [2][c].
+DevPtr<float> upload_bn(const tfl_cnn_norm* norm, bool batch, int wi, int c) {
   const float* p = norm->bn[wi];
-  if (!p) return fail(ctx, "cnn: addBatchNorm: the batch normalization parameters of convolution %d are missing", wi + 1);
-  const float eps = norm->eps[wi];
-  if (!(eps >= 0.0f)) return fail(ctx, "cnn: batch normalization eps of convolution %d must be >= 0 (got %g)", wi + 1, eps);
   std::vector<float> h(2 * c);
   std::vector<double> a(c), cc(c);
-  if (!m->bn_batch) bn_running_affine(norm, wi, c, a.data(), cc.data());
+  if (!batch) bn_running_affine(norm, wi, c, a.data(), cc.data());
   for (int ch = 0; ch < c; ch++) {
-    h[ch] = m->bn_batch ? p[ch] : (float)a[ch];
-    h[c + ch] = m->bn_batch ? p[c + ch] : (float)cc[ch];
+    h[ch] = batch ? p[ch] : (float)a[ch];
+    h[c + ch] = batch ? p[c + ch] : (float)cc[ch];
   }
-  float* d = nullptr;
-  if (cudaMalloc((void**)&d, 2 * c * 4) != cudaSuccess) return fail(ctx, "cnn: cudaMalloc failed");
-  cudaMemcpy(d, h.data(), 2 * c * 4, cudaMemcpyHostToDevice);
-  (m->bn_batch ? m->bn_wb : m->bn_ac).push_back(d);
-  m->bn_eps.push_back(eps);
-  m->bn_max_c = std::max(m->bn_max_c, c);
-  return 0;
+  return upload(h);
 }
 
 // A layer-1 weight [8][cin][3][3][3] zero-padded to [8][8][3][3][3] (the two-plane input of a set with UDiv).
@@ -100,8 +118,9 @@ std::vector<float> concat_slice(const float* w, int nbanks, int i) {
 // bank: no partial sum).  phases: banks 2..N are dilated banks held as phase sub-grids (geo[i] =
 // make_conv_tc_phase_geo(.., i)) rather than multi-resolution banks.
 void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org, int zoff, int nbanks, bool add,
-                    float* part, float* p_net, float* const* wj, const float* bias, const float* tail, int split,
-                    const ConvTcGeo& g, cudaStream_t st, bool phases = false, const TcEpi& ep = TcEpi()) {
+                    float* part, float* p_net, const std::vector<DevPtr<float>>& wj, const float* bias,
+                    const float* tail, int split, const ConvTcGeo& g, cudaStream_t st, bool phases = false,
+                    const TcEpi& ep = TcEpi()) {
   auto src_of = [&](int first, int n, int mode) {
     TcJoinSrc js = {};
     for (int k = 0; k < n; k++) {
@@ -117,11 +136,11 @@ void launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org
     return js;
   };
   if (add) {
-    launch_conv3_tc_join(src_of(0, nbanks, 0), p_net, wj[0], bias, tail, split, g, st, ep);
+    launch_conv3_tc_join(src_of(0, nbanks, 0), p_net, wj[0].get(), bias, tail, split, g, st, ep);
   } else {
     for (int i = nbanks - 1; i >= 0; i--)
-      launch_conv3_tc_join(src_of(i, 1, nbanks == 1 ? 0 : (i == nbanks - 1 ? 1 : (i > 0 ? 2 : 3))), p_net, wj[i], bias,
-                           tail, split, g, st, ep);
+      launch_conv3_tc_join(src_of(i, 1, nbanks == 1 ? 0 : (i == nbanks - 1 ? 1 : (i > 0 ? 2 : 3))), p_net, wj[i].get(),
+                           bias, tail, split, g, st, ep);
   }
 }
 
@@ -147,6 +166,15 @@ int finish_debug(tfl_ctx* ctx, const char* what) {
   return 0;
 }
 
+// Why the z-slab entry points refuse the model, or null if they run it.
+const char* cnn_slab_refusal(const tfl_cnn* m) {
+  if (m->bn) return kSlabBatchNorm;
+  if (m->bank_dilate) return kSlabDilate;
+  if (!m->default_inputs) return kSlabDefaultInputs;
+  if (!m->tc_ok || m->mode == 0) return kSlabTcOnly;
+  return nullptr;
+}
+
 }  // namespace
 
 // The reach of a banked model, with s = 2^(banksNum-1) the coarsest bank's scale: p on the planes the velocity
@@ -157,10 +185,7 @@ int finish_debug(tfl_ctx* ctx, const char* what) {
 // planes short of the local end), which a halo of 2 margin + 2 provides from margin = 3 s / 2 on.
 int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, int nx, int zoff, int nz, int own_lo,
                    int own_hi) {
-  if (m->bn) return fail(ctx, "slab: %s", kSlabBatchNorm);
-  if (m->bank_dilate) return fail(ctx, "slab: %s", kSlabDilate);
-  if (!m->default_inputs) return fail(ctx, "slab: %s", kSlabDefaultInputs);
-  if (!m->tc_ok || m->mode == 0) return fail(ctx, "slab: %s", kSlabTcOnly);
+  if (const char* why = cnn_slab_refusal(m)) return fail(ctx, "slab: %s", why);
   if (m->nbanks == 1) return 0;
   const int need = tfl_slab_cnn_margin(m->nbanks), s = 1 << (m->nbanks - 1), depth = 3 * s + 2;
   if (margin < need)
@@ -198,35 +223,28 @@ int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g) {
   }
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   m->act_gen++;
-  m->act_geo = make_conv_tc_geo(g.nb, g.nz, g.ny, g.nx);
-  m->act_zoff = g.zoff;
-  for (int i = 0; i < 3; i++) {
-    if (m->act[i]) cudaFree(m->act[i]);
-    m->act[i] = nullptr;
-    TFL_CUDA(ctx, cudaMalloc((void**)&m->act[i], conv_tc_act_bytes(m->act_geo)));
-    TFL_CUDA(ctx, cudaMemset(m->act[i], 0, conv_tc_act_bytes(m->act_geo)));
-  }
-  for (float* p : m->bact) cudaFree(p);
+  m->act_geo = ConvTcGeo{};     // matches no grid until every buffer of the new one is in place
+  for (DevPtr<float>& a : m->act) a.reset();
   m->bact.clear();
   m->bgeo.clear();
   m->borg.clear();
-  if (m->part) cudaFree(m->part);
-  m->part = nullptr;
+  m->part.reset();
+  const ConvTcGeo ag = make_conv_tc_geo(g.nb, g.nz, g.ny, g.nx);
+  for (DevPtr<float>& a : m->act)
+    if (!(a = dev_zeros<float>(conv_tc_act_bytes(ag) / 4))) return fail(ctx, "cnn: cudaMalloc failed");
   for (int i = 1, org = g.zoff; i < m->nbanks; i++) {
     org = m->bank_dilate ? 0 : (org + 1) >> 1;     // dilated banks: whole grids only (cnn_slab_check)
     const ConvTcGeo bg = m->bank_dilate ? make_conv_tc_phase_geo(g.nb, g.nz, g.ny, g.nx, i)
                                         : make_conv_tc_geo(g.nb, ((g.zoff + g.nz) >> i) - org, g.ny >> i, g.nx >> i);
     m->bgeo.push_back(bg);
     m->borg.push_back(org);
-    for (int q = 0; q < 3; q++) {
-      float* p = nullptr;
-      TFL_CUDA(ctx, cudaMalloc((void**)&p, conv_tc_act_bytes(bg)));
-      m->bact.push_back(p);
-      TFL_CUDA(ctx, cudaMemset(p, 0, conv_tc_act_bytes(bg)));
-    }
+    for (int q = 0; q < 3; q++)
+      if (!keep(m->bact, dev_zeros<float>(conv_tc_act_bytes(bg) / 4))) return fail(ctx, "cnn: cudaMalloc failed");
   }
-  if (m->nbanks > 1 && !m->bank_add)
-    TFL_CUDA(ctx, cudaMalloc((void**)&m->part, (size_t)g.nb * g.nz * g.ny * g.nx * 8 * 4));
+  if (m->nbanks > 1 && !m->bank_add && !(m->part = dev_alloc<float>((size_t)g.nb * g.nz * g.ny * g.nx * 8)))
+    return fail(ctx, "cnn: cudaMalloc failed");
+  m->act_geo = ag;
+  m->act_zoff = g.zoff;
   return 0;
 }
 
@@ -246,13 +264,13 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
   const float* l2[kTcMaxBanks];
   ConvTcGeo geo[kTcMaxBanks];
   int org[kTcMaxBanks];
-  in[0] = m->act[0];
+  in[0] = m->act[0].get();
   geo[0] = tg;
   org[0] = zoff;
   for (int i = 1; i < nbk; i++) {
     geo[i] = m->bgeo[i - 1];
     org[i] = m->borg[i - 1];
-    float* dst = m->bact[3 * (i - 1)];
+    float* dst = m->bact[3 * (i - 1)].get();
     if (m->bank_dilate) {
       // dilated bank i: the network input laid out as its 8^i phase sub-grids
       launch_tc_phase_copy(in[0], tg, dst, geo[i], i, m->tc_planes, st);
@@ -263,8 +281,8 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
     in[i] = dst;
   }
   for (int i = 0; i < nbk; i++) {
-    float* o1 = i == 0 ? m->act[1] : m->bact[3 * (i - 1) + 1];
-    float* o2 = i == 0 ? m->act[2] : m->bact[3 * (i - 1) + 2];
+    float* o1 = i == 0 ? m->act[1].get() : m->bact[3 * (i - 1) + 1].get();
+    float* o2 = i == 0 ? m->act[2].get() : m->bact[3 * (i - 1) + 2].get();
     ConvTcGeo g1 = geo[i], g2 = geo[i];
     if (!m->bank_dilate) {
       // the join reads bank i at the coarse planes of the full-resolution planes [p_lo - 1, p_hi]
@@ -272,20 +290,20 @@ static void run_conv_stack_banked(tfl_cnn* m, float* p_net, cudaStream_t st, int
       g2.z_lo = std::max(0, c_lo);     g2.z_hi = std::min(geo[i].nz, c_hi);
       g1.z_lo = std::max(0, c_lo - 1); g1.z_hi = std::min(geo[i].nz, c_hi + 1);
     }
-    launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i], m->b[m->conv0[0] + i], nullptr, m->tc_planes, 0, split,
-                    g1, st, act);
+    launch_conv3_tc(in[i], o1, nullptr, m->wBk[split][2 * i].get(), m->b[m->conv0[0] + i].get(), nullptr,
+                    m->tc_planes, 0, split, g1, st, act);
     // a phase shorter than the sub-grid (d does not divide an axis): its extra voxels are padding for layer 2
     if (m->bank_dilate && i > 0 && ((tg.nx | tg.ny | tg.nz) & ((1 << i) - 1)))
       launch_tc_phase_zero(o1, geo[i], i, tg, st);
-    launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1], m->b[m->conv0[1] + i], nullptr, 2, 0, split, g2, st,
-                    act);
+    launch_conv3_tc(o1, o2, nullptr, m->wBk[split][2 * i + 1].get(), m->b[m->conv0[1] + i].get(), nullptr, 2, 0,
+                    split, g2, st, act);
     l2[i] = o2;
   }
   ConvTcGeo g3 = tg;
   g3.z_lo = std::max(0, p_lo);
   g3.z_hi = std::min(tg.nz, p_hi);
-  launch_tc_join(l2, geo, org, zoff, nbk, m->bank_add, m->part, p_net, m->wBj[split].data(), m->b[m->conv0[2]],
-                 m->tail, split, g3, st, m->bank_dilate != 0, act);
+  launch_tc_join(l2, geo, org, zoff, nbk, m->bank_add, m->part.get(), p_net, m->wBj[split], m->b[m->conv0[2]].get(),
+                 m->tail.get(), split, g3, st, m->bank_dilate != 0, act);
 }
 
 // The three 3x3x3 layers (+ fused 1x1x1 tail) on tensor cores: act[0] -> act[1] -> act[2] -> p_net.
@@ -308,148 +326,85 @@ void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo, int p_h
   if (m->bn && !m->bn_batch) {
     // running statistics: BN1 / BN2 in the producing epilogues (after the activation, valid voxels only: the zero
     // padding of the next layer lies after BN), BN3 / BN4 folded into the tail at creation
-    e1.ac = m->bn_ac[0];
-    e2.ac = m->bn_ac[1];
+    e1.ac = m->bn_ac[0].get();
+    e2.ac = m->bn_ac[1].get();
   }
+  float *a0 = m->act[0].get(), *a1 = m->act[1].get(), *a2 = m->act[2].get(), *tail = m->tail.get();
+  const float *w1 = m->wBk[split][0].get(), *w2 = m->wBk[split][1].get(), *w3 = m->wBj[split][0].get();
   if (!m->bn_batch) {
-    launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, m->tc_planes, 0, split, g1, st, e1);
-    launch_conv3_tc(m->act[1], m->act[2], nullptr, m->wBk[split][1], m->b[1], nullptr, 2, 0, split, g2, st, e2);
-    launch_conv3_tc(m->act[2], nullptr, p_net, m->wBj[split][0], m->b[2], m->tail, 2, 1, split, g3, st, e3);
+    launch_conv3_tc(a0, a1, nullptr, w1, m->b[0].get(), nullptr, m->tc_planes, 0, split, g1, st, e1);
+    launch_conv3_tc(a1, a2, nullptr, w2, m->b[1].get(), nullptr, 2, 0, split, g2, st, e2);
+    launch_conv3_tc(a2, nullptr, p_net, w3, m->b[2].get(), tail, 2, 1, split, g3, st, e3);
     return;
   }
   // Batch statistics (whole grids only): each BN needs its layer's whole output first.  Layers 1 and 2: statistics
   // of the interior, then y = a x + c in place on it; layer 3 writes its output to act[1] (free again), and the tail
   // runs as two passes over it -- pass A accumulates BN4's statistics of h4 = act(w4 BN3(h3) + b4), pass B
   // recomputes h4 and writes p_net = w5 BN4(h4) + b5.
-  double* part = m->bn_part;
-  float* ac = m->bn_tcac;                     // [4][2][8]
+  double* part = m->bn_part.get();
+  float* ac = m->bn_tcac.get();               // [4][2][8]
   const long long count = (long long)tg.nb * tg.nz * tg.ny * tg.nx;
   auto stats = [&](const float* buf, int l) {
     launch_tc_bn_stats(buf, tg, part, st);
-    launch_bn_finalize(part, 8, count, m->bn_wb[l], m->bn_wb[l] + 8, m->bn_eps[l], ac + 16 * l, nullptr, st);
+    const float* wb = m->bn_wb[l].get();
+    launch_bn_finalize(part, 8, count, wb, wb + 8, m->bn_eps[l], ac + 16 * l, nullptr, st);
   };
-  launch_conv3_tc(m->act[0], m->act[1], nullptr, m->wBk[split][0], m->b[0], nullptr, m->tc_planes, 0, split, tg, st, e1);
-  stats(m->act[1], 0);
-  launch_tc_bn_apply(m->act[1], tg, ac, st);
-  launch_conv3_tc(m->act[1], m->act[2], nullptr, m->wBk[split][1], m->b[1], nullptr, 2, 0, split, tg, st, e2);
-  stats(m->act[2], 1);
-  launch_tc_bn_apply(m->act[2], tg, ac + 16, st);
-  launch_conv3_tc(m->act[2], m->act[1], nullptr, m->wBj[split][0], m->b[2], nullptr, 2, 0, split, tg, st, e3);
-  stats(m->act[1], 2);
-  launch_tc_bn_tail(m->act[1], tg, ac + 32, m->tail, e3.relu6, 0, part, nullptr, nullptr, st);
-  launch_bn_finalize(part, 8, count, m->bn_wb[3], m->bn_wb[3] + 8, m->bn_eps[3], ac + 48, nullptr, st);
-  launch_tc_bn_tail(m->act[1], tg, ac + 32, m->tail, e3.relu6, 1, nullptr, ac + 48, p_net, st);
+  launch_conv3_tc(a0, a1, nullptr, w1, m->b[0].get(), nullptr, m->tc_planes, 0, split, tg, st, e1);
+  stats(a1, 0);
+  launch_tc_bn_apply(a1, tg, ac, st);
+  launch_conv3_tc(a1, a2, nullptr, w2, m->b[1].get(), nullptr, 2, 0, split, tg, st, e2);
+  stats(a2, 1);
+  launch_tc_bn_apply(a2, tg, ac + 16, st);
+  launch_conv3_tc(a2, a1, nullptr, w3, m->b[2].get(), nullptr, 2, 0, split, tg, st, e3);
+  stats(a1, 2);
+  launch_tc_bn_tail(a1, tg, ac + 32, tail, e3.relu6, 0, part, nullptr, nullptr, st);
+  launch_bn_finalize(part, 8, count, m->bn_wb[3].get(), m->bn_wb[3].get() + 8, m->bn_eps[3], ac + 48, nullptr, st);
+  launch_tc_bn_tail(a1, tg, ac + 32, tail, e3.relu6, 1, nullptr, ac + 48, p_net, st);
 }
 
-extern "C" {
-
-// ---------------------------------------------------------------------------------------
-// CNN projection
-// ---------------------------------------------------------------------------------------
-int tfl_cnn_create(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                   const int32_t* ksize, const float* const* weights, const float* const* biases,
-                   tfl_cnn** out) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  return tfl_cnn_create_graph(ctx, is_3d, n_layers, cin, cout, ksize, nullptr, nullptr, 0, 0, weights, biases, out);
-}
-
-static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
-                           const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                           int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate, const tfl_cnn_inputs* inputs,
-                           const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
-                           tfl_cnn** out);
-static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                              int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                              const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
-                              const float* const* biases, tfl_cnn** out);
-static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                                 const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                                 int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                                 const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
-                                 const float* const* biases, tfl_cnn** out);
-static int cnn_create_model_ex_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                                    const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                                    int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
-                                    const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
-                                    tfl_cnn** out);
 static const tfl_cnn_inputs kDefaultInputs = {1, 0, 1, 1, 0, 0, 0};
 
-int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
-                         const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                         int nonlin_sigmoid, const float* const* weights, const float* const* biases,
-                         tfl_cnn** out) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  return cnn_create_impl(ctx, is_3d, n_layers, cin, cout_logical, ksize, pool, up, pool_is_max, nonlin_sigmoid,
-                         nullptr, 0, &kDefaultInputs, nullptr, weights, biases, out);
+namespace {
+
+// A model as the arguments of tfl_cnn_create_model_norm describe it, whichever creator it came through.
+struct CnnSpec {
+  int is_3d, n_layers;
+  const int32_t *cin, *cout, *ksize, *pool, *up;     // pool / up may be null (all 1)
+  int pool_is_max, nonlin_sigmoid;
+  const float* const* weights;
+  const float* const* biases;
+  tfl_cnn_banks_ex banks = {1, 0, 0, 0, 0};          // num = 1: no banks
+  bool banks_given = false;                           // the bank assertions of lib/model.lua hold whatever num is
+  tfl_cnn_inputs inputs = kDefaultInputs;
+  const tfl_cnn_norm* norm = nullptr;
+};
+
+void set_banks(CnnSpec& s, const tfl_cnn_banks_ex* banks) {
+  if (!banks) return;
+  s.banks = *banks;
+  s.banks_given = true;
+}
+void set_banks(CnnSpec& s, const tfl_cnn_banks* banks) {
+  if (!banks) return;
+  const tfl_cnn_banks_ex ex = {banks->num, banks->split_stage, banks->join_stage, banks->aggregate_add, 0};
+  set_banks(s, &ex);
 }
 
-int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                          const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                          int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
-                          const float* const* biases, tfl_cnn** out) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, 0,
-                            &kDefaultInputs, nullptr, weights, biases, out);
-}
+// Convolutions of stage l: one per bank in the banked stages.
+int stage_convs(const tfl_cnn* m, int l) { return (m->nbanks > 1 && l >= m->split && l < m->join) ? m->nbanks : 1; }
 
-int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                         const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                         int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
-                         const float* const* weights, const float* const* biases, tfl_cnn** out) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  return cnn_create_model_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks, 0,
-                               inputs, nullptr, weights, biases, out);
-}
-
-int tfl_cnn_create_model_ex(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                            int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
-                            const float* const* weights, const float* const* biases, tfl_cnn** out) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  return cnn_create_model_ex_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                                  inputs, nullptr, weights, biases, out);
-}
-
-int tfl_cnn_create_model_norm(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                              int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
-                              const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
-                              tfl_cnn** out) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  if (norm && norm->relu6 && nonlin_sigmoid)
+// Checks a spec, in one order whichever creator it came through, and fills in m's host-side description of the
+// model.  Makes no CUDA call.
+int cnn_validate(tfl_ctx* ctx, const CnnSpec& s, tfl_cnn** out, tfl_cnn* m) {
+  const tfl_cnn_norm* norm = s.norm;
+  if (norm && norm->relu6 && s.nonlin_sigmoid)
     return fail(ctx, "cnn: nonlinType is either 'relu6' or 'sigmoid', not both");
   if (norm && norm->batch_norm && (!norm->bn || !norm->eps))
     return fail(ctx, "cnn: addBatchNorm needs the batch normalization parameters (bn) and eps of every module");
-  return cnn_create_model_ex_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                                  inputs, norm, weights, biases, out);
-}
-
-static int cnn_create_model_ex_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                                    const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                                    int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
-                                    const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
-                                    tfl_cnn** out) {
-  if (banks && banks->dilate != 0 && banks->dilate != 1)
-    return fail(ctx, "cnn: banks dilate must be 0 ('mres') or 1 ('dilate') (got %d)", banks->dilate);
-  tfl_cnn_banks b = {};
-  if (banks) b = {banks->num, banks->split_stage, banks->join_stage, banks->aggregate_add};
-  return cnn_create_model_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid,
-                               banks ? &b : nullptr, banks ? banks->dilate : 0, inputs, norm, weights, biases, out);
-}
-
-static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                                 const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                                 int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                                 const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
-                                 const float* const* biases, tfl_cnn** out) {
-  const tfl_cnn_inputs in = inputs ? *inputs : kDefaultInputs;
+  const tfl_cnn_banks_ex& banks = s.banks;
+  if (banks.dilate != 0 && banks.dilate != 1)
+    return fail(ctx, "cnn: banks dilate must be 0 ('mres') or 1 ('dilate') (got %d)", banks.dilate);
+  const tfl_cnn_inputs& in = s.inputs;
   // lib/model.lua:27-150 and :357-361; checkYangSettings, lib/model_utils.lua:211-227.
   if (!in.p_div && !in.u_div && !in.div) return fail(ctx, "Are you sure you dont want any (U, div or p) fields?");
   if (!in.u_div && !in.div)
@@ -459,12 +414,16 @@ static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const in
   if (in.normalize && (in.norm_chan < 0 || in.norm_chan > 2)) return fail(ctx, "Incorrect normalize input channel.");
   if (in.normalize && in.norm_chan == 2 && !in.div)
     return fail(ctx, "cnn: normalizeInputChan 'div' needs inputChannels.div (lib/model.lua:108-116)");
-  if (!out || n_layers < 1 || !cin || !cout || !ksize) return fail(ctx, "cnn: bad arguments");
+  const int is_3d = s.is_3d, n_layers = s.n_layers;
+  const int32_t *cin = s.cin, *cout_logical = s.cout, *ksize = s.ksize, *pool = s.pool, *up = s.up;
+  if (!out || n_layers < 1 || !cin || !cout_logical || !ksize || !s.weights || !s.biases)
+    return fail(ctx, "cnn: bad arguments");
   bool unit_sizes = true;     // no pooling, no upsampling
   for (int l = 0; l < n_layers; l++) unit_sizes = unit_sizes && (!pool || pool[l] == 1) && (!up || up[l] == 1);
   // 'yang' (lib/model.lua:228-239): osize {6, 6, 6, 1}, ksize {3, 1, 1, 1}
-  const bool yang = n_layers == 4 && unit_sizes && cout[0] == 6 && cout[1] == 6 && cout[2] == 6 && cout[3] == 1 &&
-                    ksize[0] == 3 && ksize[1] == 1 && ksize[2] == 1 && ksize[3] == 1;
+  const bool yang = n_layers == 4 && unit_sizes && cout_logical[0] == 6 && cout_logical[1] == 6 &&
+                    cout_logical[2] == 6 && cout_logical[3] == 1 && ksize[0] == 3 && ksize[1] == 1 && ksize[2] == 1 &&
+                    ksize[3] == 1;
   if (yang && !in.p_div) return fail(ctx, "ERROR: yang model must have pDiv input");
   if (yang && !in.div) return fail(ctx, "ERROR: yang model must have div input");
   if (yang && in.u_div) return fail(ctx, "ERROR: yang model must not have UDiv input");
@@ -472,51 +431,29 @@ static int cnn_create_model_impl(tfl_ctx* ctx, int is_3d, int n_layers, const in
     return fail(ctx, "cnn: addPressureSkip joins pDiv to the hidden layer before the last convolution at full "
                      "resolution, which needs a 1x1 last convolution without upsampling (lib/model.lua:357-361; "
                      "not 'tog')");
-  return cnn_create_checked(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                            dilate, &in, norm, weights, biases, out);
-}
-
-static int cnn_create_checked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
-                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                              int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate,
-                              const tfl_cnn_inputs* inputs, const tfl_cnn_norm* norm, const float* const* weights,
-                              const float* const* biases, tfl_cnn** out) {
-  if (banks) {     // the assertions of lib/model.lua:246-252 (checked whatever banksNum is)
-    if (banks->num < 1) return fail(ctx, "cnn: banksNum >= 1 failed (got %d)", banks->num);
-    if (!(banks->split_stage < banks->join_stage))
-      return fail(ctx, "cnn: banksSplitStage < banksJoinStage failed (%d, %d)", banks->split_stage, banks->join_stage);
-    if (banks->split_stage < 1 || banks->split_stage >= n_layers)
+  if (s.banks_given) {     // the assertions of lib/model.lua:246-252 (checked whatever banksNum is)
+    if (banks.num < 1) return fail(ctx, "cnn: banksNum >= 1 failed (got %d)", banks.num);
+    if (!(banks.split_stage < banks.join_stage))
+      return fail(ctx, "cnn: banksSplitStage < banksJoinStage failed (%d, %d)", banks.split_stage, banks.join_stage);
+    if (banks.split_stage < 1 || banks.split_stage >= n_layers)
       return fail(ctx, "cnn: banksSplitStage >= 1 and banksSplitStage < #osize failed (%d, %d stages)",
-                  banks->split_stage, n_layers);
-    if (banks->join_stage < 1 || banks->join_stage >= n_layers)
+                  banks.split_stage, n_layers);
+    if (banks.join_stage < 1 || banks.join_stage >= n_layers)
       return fail(ctx, "cnn: banksJoinStage >= 1 and banksJoinStage < #osize failed (%d, %d stages)",
-                  banks->join_stage, n_layers);
-    if (banks->num > kMaxBanks) return fail(ctx, "cnn: at most %d banks are supported (got %d)", kMaxBanks, banks->num);
+                  banks.join_stage, n_layers);
+    if (banks.num > kMaxBanks) return fail(ctx, "cnn: at most %d banks are supported (got %d)", kMaxBanks, banks.num);
     // getConvLayer's assertion for banks 2..N, dilated by 2^(i-1) (lib/model_utils.lua:125)
-    for (int l = banks->split_stage - 1; dilate && banks->num > 1 && up && l < banks->join_stage - 1; l++)
+    for (int l = banks.split_stage - 1; banks.dilate && banks.num > 1 && up && l < banks.join_stage - 1; l++)
       if (up[l] > 1) return fail(ctx, "upsampling not supported for dilated convolutions. (stage %d)", l + 1);
-    if (banks->num == 1) banks = nullptr;
   }
-  return cnn_create_impl(ctx, is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, banks,
-                         banks ? dilate : 0, inputs, norm, weights, biases, out);
-}
-
-static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout_logical,
-                           const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
-                           int nonlin_sigmoid, const tfl_cnn_banks* banks, int dilate, const tfl_cnn_inputs* inputs,
-                           const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
-                           tfl_cnn** out) {
-  if (!out || n_layers < 1) return fail(ctx, "cnn: bad arguments");
-  const tfl_cnn_inputs& in = *inputs;
+  const int nbanks = banks.num;
+  const int bsplit = nbanks > 1 ? banks.split_stage - 1 : 0, bjoin = nbanks > 1 ? banks.join_stage - 1 : 0;
   const int in_sel = (in.p_div ? kCnnInPDiv : 0) | (in.u_div ? kCnnInUDiv : 0) | (in.div ? kCnnInDiv : 0);
   const int in_ch = (in.p_div ? 1 : 0) + (in.u_div ? (is_3d ? 3 : 2) : 0) + (in.div ? 1 : 0) + 1;
   const bool skip = in.pressure_skip != 0;
-  const int nbanks = banks ? banks->num : 1;
-  const int bsplit = banks ? banks->split_stage - 1 : 0, bjoin = banks ? banks->join_stage - 1 : 0;
-  auto convs_of = [&](int l) { return (nbanks > 1 && l >= bsplit && l < bjoin) ? nbanks : 1; };
   // Channels the convolution of layer l really emits: cout * up^d (ConvolutionUpsample, model_utils.lua:74-76).
   std::vector<int32_t> cout_conv(n_layers);
-  bool plain = !nonlin_sigmoid;
+  bool plain = !s.nonlin_sigmoid;
   for (int l = 0; l < n_layers; l++) {
     const int u = up ? up[l] : 1, pl = pool ? pool[l] : 1;
     if (u < 1 || pl < 1) return fail(ctx, "cnn: pooling / upsampling sizes must be >= 1");
@@ -544,7 +481,6 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
   if (nbanks > 1) plain = false;
   const bool relu6 = norm && norm->relu6, bn = norm && norm->batch_norm;
   if (relu6 || bn) plain = false;     // the stage loop applies BN; relu6 is activation code 3
-  tfl_cnn* m = new tfl_cnn();
   m->bn = bn;
   m->bn_batch = bn && norm->batch_stats;
   m->in_sel = in_sel;
@@ -557,52 +493,43 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
                       !skip;
   m->tc_planes = (in_sel & kCnnInUDiv) ? 2 : 1;
   m->plain = plain;
-  m->pool_is_max = pool_is_max ? 1 : 0;
-  m->nonlin = nonlin_sigmoid ? 2 : (relu6 ? 3 : 1);
+  m->pool_is_max = s.pool_is_max ? 1 : 0;
+  m->nonlin = s.nonlin_sigmoid ? 2 : (relu6 ? 3 : 1);
   m->is3d = is_3d ? 1 : 0;
   m->n_layers = n_layers;
   m->nbanks = nbanks;
   m->split = bsplit;
   m->join = bjoin;
-  m->bank_add = banks && banks->aggregate_add ? 1 : 0;
-  m->bank_dilate = nbanks > 1 && dilate ? 1 : 0;
+  m->bank_add = nbanks > 1 && banks.aggregate_add ? 1 : 0;
+  m->bank_dilate = nbanks > 1 && banks.dilate ? 1 : 0;
   int wi = 0;     // index into weights / biases
   for (int l = 0; l < n_layers; l++) {
-    if (l > 0 && nbanks > 1 && l == bjoin && !m->bank_add && cin[l] != nbanks * cout_logical[l - 1]) {
-      delete m;
+    if (l > 0 && nbanks > 1 && l == bjoin && !m->bank_add && cin[l] != nbanks * cout_logical[l - 1])
       return fail(ctx, "cnn: stage %d concatenates %d banks of %d channels, so it needs cin = %d (got %d)", l + 1,
                   nbanks, cout_logical[l - 1], nbanks * cout_logical[l - 1], cin[l]);
-    }
-    if (l > 0 && !(nbanks > 1 && l == bjoin && !m->bank_add) && cin[l] != cout_logical[l - 1]) {
-      delete m;
+    if (l > 0 && !(nbanks > 1 && l == bjoin && !m->bank_add) && cin[l] != cout_logical[l - 1])
       return fail(ctx, "cnn: channel mismatch at layer %d", l);
-    }
+    if (ksize[l] % 2 != 1) return fail(ctx, "convolution size must be odd");     // model_utils.lua:70
     m->pool.push_back(pool ? pool[l] : 1);
     m->up.push_back(up ? up[l] : 1);
     m->conv0.push_back(wi);
-    if (ksize[l] % 2 != 1) { delete m; return fail(ctx, "convolution size must be odd"); }   // model_utils.lua:70
-    const int kz = is_3d ? ksize[l] : 1;
-    const int taps = kz * ksize[l] * ksize[l];
-    for (int bk = 0; bk < convs_of(l); bk++, wi++) {
-      // the skip's layer is 1x1 with one output: its hidden channels' weights come first, pDiv's last
-      if (skip && l == n_layers - 1) m->w_skip = weights[wi][cin[l]];
-      const std::vector<float> relaid = relayout_conv_weights(weights[wi], cin[l], cout[l], taps);
-      float *dw = nullptr, *db = nullptr;
-      if (cudaMalloc((void**)&dw, relaid.size() * 4) != cudaSuccess ||
-          cudaMalloc((void**)&db, cout[l] * 4) != cudaSuccess) { tfl_cnn_destroy(ctx, m); return fail(ctx, "cnn: cudaMalloc failed"); }
-      cudaMemcpy(dw, relaid.data(), relaid.size() * 4, cudaMemcpyHostToDevice);
-      cudaMemcpy(db, biases[wi], cout[l] * 4, cudaMemcpyHostToDevice);
+    for (int k = 0; k < stage_convs(m, l); k++, wi++) {
       m->cin.push_back(cin[l]); m->cout.push_back(cout[l]); m->ks.push_back(ksize[l]);
-      m->w.push_back(dw); m->b.push_back(db);
-      if (bn && l < n_layers - 1 && cnn_upload_bn(ctx, m, norm, wi, cout_logical[l])) {
-        tfl_cnn_destroy(ctx, m);
-        return 1;
+      if (bn && l < n_layers - 1) {
+        if (!norm->bn[wi])
+          return fail(ctx, "cnn: addBatchNorm: the batch normalization parameters of convolution %d are missing",
+                      wi + 1);
+        const float eps = norm->eps[wi];
+        if (!(eps >= 0.0f))
+          return fail(ctx, "cnn: batch normalization eps of convolution %d must be >= 0 (got %g)", wi + 1, eps);
+        m->bn_eps.push_back(eps);
+        m->bn_max_c = std::max(m->bn_max_c, (int)cout_logical[l]);
       }
     }
     if (cout[l] > m->max_c) m->max_c = cout[l];
   }
   {   // largest activation of the graph, in channels x cells-of-the-input-grid (banks 2..N have buffers of their
-      // own, cnn_bank_buf_bytes; the joined banks are counted here)
+      // own, cnn_scratch; the joined banks are counted here)
     double rel = 1.0;
     m->max_rel = in_ch;      // the network input (pooled into, or shared by, the banks at stage 1)
     for (int l = 0; l < n_layers; l++) {
@@ -615,67 +542,169 @@ static int cnn_create_impl(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t*
       m->max_rel = std::max(m->max_rel, rel * cout_logical[l]);                  // after the pixel shuffle
       rel /= (double)pl * pl * (is_3d ? pl : 1);
     }
-    if (rel != 1.0) { tfl_cnn_destroy(ctx, m); return fail(ctx, "cnn: pooling and upsampling do not return to the input resolution"); }
+    if (rel != 1.0) return fail(ctx, "cnn: pooling and upsampling do not return to the input resolution");
     if ((double)m->max_c < m->max_rel) m->max_c = (int)std::ceil(m->max_rel);
   }
   // Tensor-core eligibility: the 3-D 'default' graph (lib/model.lua:219-226), single-bank or with banks (either type)
   // split before stage 1 and joined before stage 3.
   static const int want[5][3] = {{0, 8, 3}, {8, 8, 3}, {8, 8, 3}, {8, 8, 1}, {8, 1, 1}};   // cin[0]: any input set
-  m->tc_ok = is_3d && n_layers == 5 && !nonlin_sigmoid && !(bn && nbanks > 1) &&
+  m->tc_ok = is_3d && n_layers == 5 && !s.nonlin_sigmoid && !(bn && nbanks > 1) &&
              (nbanks == 1 || (bsplit == 0 && bjoin == 2 && nbanks <= kTcMaxBanks));
   for (int l = 0; m->tc_ok && l < 5; l++) {
     const int want_cin = l == 0 ? in_ch : (l == 2 && !m->bank_add) ? 8 * nbanks : want[l][0];
     m->tc_ok = m->pool[l] == 1 && m->up[l] == 1 && cin[l] == want_cin && cout[l] == want[l][1] && ksize[l] == want[l][2];
   }
-  if (m->tc_ok) {
-    const int j0 = m->conv0[2], nj = m->bank_add ? 1 : nbanks;
-    for (int split = 0; split < 2; split++) {
-      for (int i = 0; i < nbanks; i++) {                 // layers 1 and 2 of bank i
-        // layer 1: the input set on one float4 plane, or (with UDiv) on two with zero weights past in_ch
-        m->wBk[split].push_back(m->tc_planes == 1 ? upload_tc_weights(weights[m->conv0[0] + i], in_ch, split)
-                                                  : upload_tc_weights(pad_cin8(weights[m->conv0[0] + i], in_ch).data(),
-                                                                      8, split));
-        m->wBk[split].push_back(upload_tc_weights(weights[m->conv0[1] + i], 8, split));
-      }
-      for (int i = 0; i < nj; i++)
-        m->wBj[split].push_back(upload_tc_weights(concat_slice(weights[j0], nj, i).data(), 8, split));
-    }
-    std::vector<float> tail(64 + 8 + 8 + 1);
-    memcpy(tail.data(), weights[m->conv0[3]], 64 * 4);
-    memcpy(tail.data() + 64, biases[m->conv0[3]], 8 * 4);
-    memcpy(tail.data() + 72, weights[m->conv0[4]], 8 * 4);
-    tail[80] = biases[m->conv0[4]][0];
-    if (bn && !m->bn_batch) {
-      // running statistics: BN3 (after layer 3's activation) into w4 / b4, BN4 (after layer 4's) into w5 / b5, exact in
-      // real arithmetic: w4 (a3 h + c3) + b4 = (w4 a3) h + (b4 + w4 c3), w5 (a4 h + c4) + b5 = (w5 a4) h + (b5 + w5 c4)
-      double a3[8], c3[8], a4[8], c4[8];
-      bn_running_affine(norm, 2, 8, a3, c3);
-      bn_running_affine(norm, 3, 8, a4, c4);
-      double b5 = tail[80];
-      for (int o = 0; o < 8; o++) {
-        double b4 = tail[64 + o];
-        for (int c = 0; c < 8; c++) {
-          b4 += (double)tail[o * 8 + c] * c3[c];
-          tail[o * 8 + c] = (float)((double)tail[o * 8 + c] * a3[c]);
-        }
-        tail[64 + o] = (float)b4;
-        b5 += (double)tail[72 + o] * c4[o];
-        tail[72 + o] = (float)((double)tail[72 + o] * a4[o]);
-      }
-      tail[80] = (float)b5;
-    }
-    if (bn && m->bn_batch &&
-        (cudaMalloc((void**)&m->bn_part, sizeof(double) * 2 * (kBnBlocks + 1) * 8) != cudaSuccess ||
-         cudaMalloc((void**)&m->bn_tcac, sizeof(float) * 4 * 16) != cudaSuccess)) {
-      tfl_cnn_destroy(ctx, m);
-      return fail(ctx, "cnn: cudaMalloc failed");
-    }
-    cudaMalloc((void**)&m->tail, tail.size() * 4);
-    cudaMemcpy(m->tail, tail.data(), tail.size() * 4, cudaMemcpyHostToDevice);
-    m->mode = 2;
-  }
-  *out = m;
   return 0;
+}
+
+// Puts the parameters of a model cnn_validate has described on the device: every convolution's weights, bias and
+// batch normalization, and for the tensor cores the packed weights and the tail.  1 if a cudaMalloc or cudaMemcpy
+// fails.
+int cnn_upload(const CnnSpec& s, tfl_cnn* m) {
+  const float* const* weights = s.weights;
+  const float* const* biases = s.biases;
+  const int n_layers = s.n_layers;
+  for (int l = 0, wi = 0; l < n_layers; l++) {
+    const int taps = (s.is_3d ? s.ksize[l] : 1) * s.ksize[l] * s.ksize[l];
+    for (int k = 0; k < stage_convs(m, l); k++, wi++) {
+      // the skip's layer is 1x1 with one output: its hidden channels' weights come first, pDiv's last
+      if (m->skip && l == n_layers - 1) m->w_skip = weights[wi][m->cin[wi]];
+      if (!keep(m->w, upload(relayout_conv_weights(weights[wi], m->cin[wi], m->cout[wi], taps))) ||
+          !keep(m->b, upload(biases[wi], m->cout[wi])))
+        return 1;
+      if (m->bn && l < n_layers - 1 &&
+          !keep(m->bn_batch ? m->bn_wb : m->bn_ac, upload_bn(s.norm, m->bn_batch, wi, s.cout[l])))
+        return 1;
+    }
+  }
+  if (!m->tc_ok) return 0;
+  const int nbanks = m->nbanks, in_ch = m->in_ch, j0 = m->conv0[2], nj = m->bank_add ? 1 : nbanks;
+  for (int split = 0; split < 2; split++) {
+    for (int i = 0; i < nbanks; i++) {                 // layers 1 and 2 of bank i
+      // layer 1: the input set on one float4 plane, or (with UDiv) on two with zero weights past in_ch
+      const float* w1 = weights[m->conv0[0] + i];
+      if (!keep(m->wBk[split], m->tc_planes == 1 ? upload_tc_weights(w1, in_ch, split)
+                                                 : upload_tc_weights(pad_cin8(w1, in_ch).data(), 8, split)) ||
+          !keep(m->wBk[split], upload_tc_weights(weights[m->conv0[1] + i], 8, split)))
+        return 1;
+    }
+    for (int i = 0; i < nj; i++)
+      if (!keep(m->wBj[split], upload_tc_weights(concat_slice(weights[j0], nj, i).data(), 8, split))) return 1;
+  }
+  std::vector<float> tail(kTailFloats);
+  memcpy(tail.data(), weights[m->conv0[3]], 64 * 4);
+  memcpy(tail.data() + 64, biases[m->conv0[3]], 8 * 4);
+  memcpy(tail.data() + 72, weights[m->conv0[4]], 8 * 4);
+  tail[80] = biases[m->conv0[4]][0];
+  if (m->bn && !m->bn_batch) {
+    // running statistics: BN3 (after layer 3's activation) into w4 / b4, BN4 (after layer 4's) into w5 / b5, exact in
+    // real arithmetic: w4 (a3 h + c3) + b4 = (w4 a3) h + (b4 + w4 c3), w5 (a4 h + c4) + b5 = (w5 a4) h + (b5 + w5 c4)
+    double a3[8], c3[8], a4[8], c4[8];
+    bn_running_affine(s.norm, 2, 8, a3, c3);
+    bn_running_affine(s.norm, 3, 8, a4, c4);
+    double b5 = tail[80];
+    for (int o = 0; o < 8; o++) {
+      double b4 = tail[64 + o];
+      for (int c = 0; c < 8; c++) {
+        b4 += (double)tail[o * 8 + c] * c3[c];
+        tail[o * 8 + c] = (float)((double)tail[o * 8 + c] * a3[c]);
+      }
+      tail[64 + o] = (float)b4;
+      b5 += (double)tail[72 + o] * c4[o];
+      tail[72 + o] = (float)((double)tail[72 + o] * a4[o]);
+    }
+    tail[80] = (float)b5;
+  }
+  if (m->bn_batch && (!(m->bn_part = dev_alloc<double>(2 * (kBnBlocks + 1) * 8)) ||
+                      !(m->bn_tcac = dev_alloc<float>(4 * 16))))
+    return 1;
+  if (!(m->tail = upload(tail))) return 1;
+  m->mode = 2;
+  return 0;
+}
+
+// The one path of every creator: nothing reaches the device unless the spec is valid, and a failed upload frees what
+// was uploaded before it.
+int cnn_create(tfl_ctx* ctx, const CnnSpec& s, tfl_cnn** out) {
+  std::unique_ptr<tfl_cnn> m(new tfl_cnn());
+  if (cnn_validate(ctx, s, out, m.get())) return 1;
+  if (cnn_upload(s, m.get())) return fail(ctx, "cnn: cudaMalloc failed");
+  *out = m.release();
+  return 0;
+}
+
+}  // namespace
+
+extern "C" {
+
+// ---------------------------------------------------------------------------------------
+// CNN projection
+// ---------------------------------------------------------------------------------------
+int tfl_cnn_create(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                   const int32_t* ksize, const float* const* weights, const float* const* biases,
+                   tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  return cnn_create(ctx, {is_3d, n_layers, cin, cout, ksize, nullptr, nullptr, 0, 0, weights, biases}, out);
+}
+
+int tfl_cnn_create_graph(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                         const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                         int nonlin_sigmoid, const float* const* weights, const float* const* biases,
+                         tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  return cnn_create(ctx, {is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, weights, biases},
+                    out);
+}
+
+int tfl_cnn_create_banked(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                          const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                          int nonlin_sigmoid, const tfl_cnn_banks* banks, const float* const* weights,
+                          const float* const* biases, tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  CnnSpec s = {is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, weights, biases};
+  set_banks(s, banks);
+  return cnn_create(ctx, s, out);
+}
+
+int tfl_cnn_create_model(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                         const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                         int nonlin_sigmoid, const tfl_cnn_banks* banks, const tfl_cnn_inputs* inputs,
+                         const float* const* weights, const float* const* biases, tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  CnnSpec s = {is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, weights, biases};
+  set_banks(s, banks);
+  if (inputs) s.inputs = *inputs;
+  return cnn_create(ctx, s, out);
+}
+
+int tfl_cnn_create_model_ex(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                            const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                            int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                            const float* const* weights, const float* const* biases, tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  CnnSpec s = {is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, weights, biases};
+  set_banks(s, banks);
+  if (inputs) s.inputs = *inputs;
+  return cnn_create(ctx, s, out);
+}
+
+int tfl_cnn_create_model_norm(tfl_ctx* ctx, int is_3d, int n_layers, const int32_t* cin, const int32_t* cout,
+                              const int32_t* ksize, const int32_t* pool, const int32_t* up, int pool_is_max,
+                              int nonlin_sigmoid, const tfl_cnn_banks_ex* banks, const tfl_cnn_inputs* inputs,
+                              const tfl_cnn_norm* norm, const float* const* weights, const float* const* biases,
+                              tfl_cnn** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  CnnSpec s = {is_3d, n_layers, cin, cout, ksize, pool, up, pool_is_max, nonlin_sigmoid, weights, biases};
+  set_banks(s, banks);
+  if (inputs) s.inputs = *inputs;
+  s.norm = norm;
+  return cnn_create(ctx, s, out);
 }
 
 int tfl_cnn_set_mode(tfl_ctx* ctx, tfl_cnn* m, int mode) {
@@ -726,28 +755,12 @@ int tfl_debug_conv3_tc(tfl_ctx* ctx, const float* in, float* out, float* p_net, 
   ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
   g.z_lo = z_lo;
   g.z_hi = z_hi;
-  float *wB = upload_tc_weights(w_host, cin, split), *bias = nullptr, *tail = nullptr;
-  auto release = [&]() {
-    if (wB) cudaFree(wB);
-    if (bias) cudaFree(bias);
-    if (tail) cudaFree(tail);
-  };
-  const int n_tail = 64 + 8 + 8 + 1;
-  if (!wB || cudaMalloc((void**)&bias, 8 * 4) != cudaSuccess ||
-      (final_layer && cudaMalloc((void**)&tail, n_tail * 4) != cudaSuccess)) {
-    release();
-    return fail(ctx, "debug_conv3_tc: cudaMalloc failed");
-  }
-  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
-  if (final_layer) cudaMemcpy(tail, tail_host, n_tail * 4, cudaMemcpyHostToDevice);
-  launch_conv3_tc(in, out, p_net, wB, bias, tail, cin == 3 ? 1 : 2, final_layer, split, g, ctx->stream);
-  const int rc = check_launch(ctx, "debug_conv3_tc");
-  const cudaError_t se = cudaStreamSynchronize(ctx->stream);
-  release();
-  if (rc) return rc;
-  if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc: %s", cudaGetErrorString(se));
-  if (conv_tc_take_z_fault(ctx->stream)) return fail(ctx, "debug_conv3_tc: %s", kConvZStalled);
-  return 0;
+  const DevPtr<float> wB = upload_tc_weights(w_host, cin, split), bias = upload(bias_host, 8),
+                      tail = final_layer ? upload(tail_host, kTailFloats) : DevPtr<float>();
+  if (!wB || !bias || (final_layer && !tail)) return fail(ctx, "debug_conv3_tc: cudaMalloc failed");
+  launch_conv3_tc(in, out, p_net, wB.get(), bias.get(), tail.get(), cin == 3 ? 1 : 2, final_layer, split, g,
+                  ctx->stream);
+  return finish_debug(ctx, "debug_conv3_tc");
 }
 
 // Undocumented test hook (not in tfl.h): caps the persistent grid of the z-streaming tensor-core convolution at
@@ -774,40 +787,28 @@ int tfl_debug_conv3_tc_bn(tfl_ctx* ctx, const float* in, float* out, const float
     return fail(ctx, "debug_conv3_tc_bn: nil argument");
   if (bad_grid(nb, nz, ny, nx, 1) || !(eps >= 0.0f)) return fail(ctx, "debug_conv3_tc_bn: bad arguments");
   const ConvTcGeo g = make_conv_tc_geo(nb, nz, ny, nx);
-  float *wB = upload_tc_weights(w_host, cin, split), *bias = nullptr, *ep = nullptr, *wb = nullptr, *ac = nullptr;
-  double *part = nullptr, *stats = nullptr;
-  auto release = [&]() {
-    for (void* p : {(void*)wB, (void*)bias, (void*)ep, (void*)wb, (void*)ac, (void*)part, (void*)stats})
-      if (p) cudaFree(p);
-  };
-  if (!wB || cudaMalloc((void**)&bias, 8 * 4) != cudaSuccess || cudaMalloc((void**)&ep, 16 * 4) != cudaSuccess ||
-      cudaMalloc((void**)&wb, 16 * 4) != cudaSuccess || cudaMalloc((void**)&ac, 16 * 4) != cudaSuccess ||
-      cudaMalloc((void**)&part, sizeof(double) * 2 * (kBnBlocks + 1) * 8) != cudaSuccess ||
-      cudaMalloc((void**)&stats, sizeof(double) * 16) != cudaSuccess) {
-    release();
+  const DevPtr<float> wB = upload_tc_weights(w_host, cin, split), bias = upload(bias_host, 8),
+                      ep = ep_ac_host ? upload(ep_ac_host, 16) : DevPtr<float>(),
+                      bw = bn_w_host ? upload(bn_w_host, 8) : DevPtr<float>(),
+                      bb = bn_b_host ? upload(bn_b_host, 8) : DevPtr<float>(), ac = dev_alloc<float>(16);
+  const DevPtr<double> part = dev_alloc<double>(2 * (kBnBlocks + 1) * 8), stats = dev_alloc<double>(16);
+  if (!wB || !bias || (ep_ac_host && !ep) || (bn_w_host && !bw) || (bn_b_host && !bb) || !ac || !part || !stats)
     return fail(ctx, "debug_conv3_tc_bn: cudaMalloc failed");
-  }
-  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
-  if (ep_ac_host) cudaMemcpy(ep, ep_ac_host, 16 * 4, cudaMemcpyHostToDevice);
-  if (bn_w_host) cudaMemcpy(wb, bn_w_host, 8 * 4, cudaMemcpyHostToDevice);
-  if (bn_b_host) cudaMemcpy(wb + 8, bn_b_host, 8 * 4, cudaMemcpyHostToDevice);
   TcEpi e;
   e.relu6 = relu6 ? 1 : 0;
-  e.ac = ep_ac_host ? ep : nullptr;
-  launch_conv3_tc(in, out, nullptr, wB, bias, nullptr, cin == 3 ? 1 : 2, 0, split, g, ctx->stream, e);
+  e.ac = ep.get();
+  launch_conv3_tc(in, out, nullptr, wB.get(), bias.get(), nullptr, cin == 3 ? 1 : 2, 0, split, g, ctx->stream, e);
   if (batch) {
-    launch_tc_bn_stats(out, g, part, ctx->stream);
-    launch_bn_finalize(part, 8, (long long)nb * nz * ny * nx, bn_w_host ? wb : nullptr, bn_b_host ? wb + 8 : nullptr,
-                       eps, ac, stats, ctx->stream);
-    launch_tc_bn_apply(out, g, ac, ctx->stream);
+    launch_tc_bn_stats(out, g, part.get(), ctx->stream);
+    launch_bn_finalize(part.get(), 8, (long long)nb * nz * ny * nx, bw.get(), bb.get(), eps, ac.get(), stats.get(),
+                       ctx->stream);
+    launch_tc_bn_apply(out, g, ac.get(), ctx->stream);
   }
-  int rc = finish_debug(ctx, "debug_conv3_tc_bn");
-  if (!rc && batch &&
-      (cudaMemcpy(stats_host, stats, sizeof(double) * 16, cudaMemcpyDeviceToHost) != cudaSuccess ||
-       cudaMemcpy(ac_host, ac, 16 * 4, cudaMemcpyDeviceToHost) != cudaSuccess))
-    rc = fail(ctx, "debug_conv3_tc_bn: copy failed");
-  release();
-  return rc;
+  if (const int rc = finish_debug(ctx, "debug_conv3_tc_bn")) return rc;
+  if (batch && (cudaMemcpy(stats_host, stats.get(), sizeof(double) * 16, cudaMemcpyDeviceToHost) != cudaSuccess ||
+                cudaMemcpy(ac_host, ac.get(), 16 * 4, cudaMemcpyDeviceToHost) != cudaSuccess))
+    return fail(ctx, "debug_conv3_tc_bn: copy failed");
+  return 0;
 }
 
 // tfl_debug_conv3_tc_dilated: one tensor-core 3x3x3 layer (not the final one) dilated by 2^sh the way a dilated bank
@@ -823,28 +824,16 @@ int tfl_debug_conv3_tc_dilated(tfl_ctx* ctx, const float* in, float* out, const 
   if (sh < 0 || sh > 7 || bad_grid(nb, nz, ny, nx, 1))
     return fail(ctx, "debug_conv3_tc_dilated: bad grid %dx%dx%dx%d or dilation 2^%d", nb, nz, ny, nx, sh);
   const ConvTcGeo gf = make_conv_tc_geo(nb, nz, ny, nx), gs = make_conv_tc_phase_geo(nb, nz, ny, nx, sh);
-  float *wB = upload_tc_weights(w_host, cin, split), *bias = nullptr, *sin = nullptr, *sout = nullptr;
-  auto release = [&]() {
-    for (float* p : {wB, bias, sin, sout})
-      if (p) cudaFree(p);
-  };
-  if (!wB || cudaMalloc((void**)&bias, 8 * 4) != cudaSuccess ||
-      cudaMalloc((void**)&sin, conv_tc_act_bytes(gs)) != cudaSuccess ||
-      cudaMalloc((void**)&sout, conv_tc_act_bytes(gs)) != cudaSuccess) {
-    release();
-    return fail(ctx, "debug_conv3_tc_dilated: cudaMalloc failed");
-  }
-  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
-  cudaMemset(sin, 0, conv_tc_act_bytes(gs));
-  cudaMemset(sout, 0, conv_tc_act_bytes(gs));
+  const DevPtr<float> wB = upload_tc_weights(w_host, cin, split), bias = upload(bias_host, 8),
+                      sin = dev_zeros<float>(conv_tc_act_bytes(gs) / 4),
+                      sout = dev_zeros<float>(conv_tc_act_bytes(gs) / 4);
+  if (!wB || !bias || !sin || !sout) return fail(ctx, "debug_conv3_tc_dilated: cudaMalloc failed");
   const int planes = cin == 3 ? 1 : 2;
-  launch_tc_phase_copy(in, gf, sin, gs, sh, planes, ctx->stream);
-  launch_conv3_tc(sin, sout, nullptr, wB, bias, nullptr, planes, 0, split, gs, ctx->stream);
-  launch_tc_phase_zero(sout, gs, sh, gf, ctx->stream);
-  launch_tc_phase_gather(sout, gs, out, gf, sh, ctx->stream);
-  const int rc = finish_debug(ctx, "debug_conv3_tc_dilated");
-  release();
-  return rc;
+  launch_tc_phase_copy(in, gf, sin.get(), gs, sh, planes, ctx->stream);
+  launch_conv3_tc(sin.get(), sout.get(), nullptr, wB.get(), bias.get(), nullptr, planes, 0, split, gs, ctx->stream);
+  launch_tc_phase_zero(sout.get(), gs, sh, gf, ctx->stream);
+  launch_tc_phase_gather(sout.get(), gs, out, gf, sh, ctx->stream);
+  return finish_debug(ctx, "debug_conv3_tc_dilated");
 }
 
 // tfl_debug_conv3_tc_join: the join layer of a banked model (split 1, join 3) on caller-owned bank buffers.
@@ -911,37 +900,22 @@ static int debug_join_impl(tfl_ctx* ctx, const float* const* banks, int nbanks, 
   g.z_lo = z_lo;
   g.z_hi = z_hi;
   const int cin = add ? 8 : 8 * nbanks, nw = add ? 1 : nbanks;
-  std::vector<float*> wj(nw, nullptr);
-  float *bias = nullptr, *tail = nullptr, *part = nullptr;
-  auto release = [&]() {
-    for (float* p : wj) if (p) cudaFree(p);
-    if (bias) cudaFree(bias);
-    if (tail) cudaFree(tail);
-    if (part) cudaFree(part);
-  };
-  bool ok = cudaMalloc((void**)&bias, 8 * 4) == cudaSuccess && cudaMalloc((void**)&tail, 81 * 4) == cudaSuccess &&
-            (add || cudaMalloc((void**)&part, (size_t)nb * nz * ny * nx * 8 * 4) == cudaSuccess);
+  const DevPtr<float> bias = upload(bias_host, 8), tail = upload(tail_host, kTailFloats),
+                      part = add ? DevPtr<float>() : dev_alloc<float>((size_t)nb * nz * ny * nx * 8);
+  std::vector<DevPtr<float>> wj;
+  bool ok = bias && tail && (add || part);
   for (int i = 0; ok && i < nw; i++)
-    ok = (wj[i] = upload_tc_weights(concat_slice(w_host, cin / 8, i).data(), 8, split)) != nullptr;
-  if (!ok) {
-    release();
-    return fail(ctx, "debug_conv3_tc_join: cudaMalloc failed");
-  }
-  cudaMemcpy(bias, bias_host, 8 * 4, cudaMemcpyHostToDevice);
-  cudaMemcpy(tail, tail_host, 81 * 4, cudaMemcpyHostToDevice);
+    ok = keep(wj, upload_tc_weights(concat_slice(w_host, cin / 8, i).data(), 8, split));
+  if (!ok) return fail(ctx, "debug_conv3_tc_join: cudaMalloc failed");
   ConvTcGeo geo[kTcMaxBanks];
   int org[kTcMaxBanks];
   for (int i = 0; i < nbanks; i++) {
     geo[i] = make_conv_tc_geo(nb, bank_nz[i], ny >> i, nx >> i);
     org[i] = bank_org[i];
   }
-  launch_tc_join(banks, geo, org, zoff, nbanks, add, part, p_net, wj.data(), bias, tail, split, g, ctx->stream);
-  const int rc = check_launch(ctx, "debug_conv3_tc_join");
-  const cudaError_t se = cudaStreamSynchronize(ctx->stream);
-  release();
-  if (rc) return rc;
-  if (se != cudaSuccess) return fail(ctx, "debug_conv3_tc_join: %s", cudaGetErrorString(se));
-  return 0;
+  launch_tc_join(banks, geo, org, zoff, nbanks, add, part.get(), p_net, wj, bias.get(), tail.get(), split, g,
+                 ctx->stream);
+  return finish_debug(ctx, "debug_conv3_tc_join");
 }
 
 // tfl_debug_tc_pyramid: one level of the bank pyramid on caller-owned padded buffers: in is
@@ -958,9 +932,7 @@ static int debug_tc_pyramid_impl(tfl_ctx* ctx, const float* in, float* out, int 
   go.z_lo = z_lo;
   go.z_hi = z_hi;
   launch_tc_pyramid(in, make_conv_tc_geo(nb, nz_in, ny, nx), out, go, z_phase, ctx->stream, planes);
-  if (check_launch(ctx, "debug_tc_pyramid")) return 1;
-  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  return 0;
+  return finish_debug(ctx, "debug_tc_pyramid");
 }
 int tfl_debug_tc_pyramid(tfl_ctx* ctx, const float* in, float* out, int nb, int nz_in, int ny, int nx, int nz_out,
                          int z_phase, int z_lo, int z_hi) {
@@ -985,15 +957,12 @@ int tfl_debug_cnn_inputs_padded(tfl_ctx* ctx, const tfl_cnn* m, const float* p_d
   if (!ctx) return 1;
   if (!m || !p_div || !U1 || !flags || !scale_host || !out) return fail(ctx, "debug_cnn_inputs_padded: nil argument");
   if (!m->is3d || bad_grid(nb, nz, ny, nx, 1)) return fail(ctx, "debug_cnn_inputs_padded: bad grid or 2-D model");
-  float* scale = nullptr;
-  TFL_CUDA(ctx, cudaMalloc((void**)&scale, 4 * nb));
-  cudaMemcpy(scale, scale_host, 4 * nb, cudaMemcpyHostToDevice);
+  const DevPtr<float> scale = upload(scale_host, nb);
+  if (!scale) return fail(ctx, "debug_cnn_inputs_padded: cudaMalloc failed");
   const ConvTcGeo tg = make_conv_tc_geo(nb, nz, ny, nx);
-  launch_cnn_inputs_padded(p_div, U1, flags, scale, out, tg.px, tg.py, whole_grid(ctx, nb, nz, ny, nx, 1),
+  launch_cnn_inputs_padded(p_div, U1, flags, scale.get(), out, tg.px, tg.py, whole_grid(ctx, nb, nz, ny, nx, 1),
                            ctx->stream, m->in_sel, m->tc_planes);
-  const int rc = finish_debug(ctx, "debug_cnn_inputs_padded");
-  cudaFree(scale);
-  return rc;
+  return finish_debug(ctx, "debug_cnn_inputs_padded");
 }
 
 // Undocumented test hooks (not in tfl.h): the fp32 path's kernels (tfl_cnn.cu) on caller-owned device buffers, on
@@ -1031,21 +1000,12 @@ static int debug_conv_fp32_impl(tfl_ctx* ctx, const float* in, float* out, const
     return fail(ctx, "debug_conv_fp32: bad layer cin=%d cout=%d k=%d act=%d generic=%d", cin, cout, ks, act, generic);
   if (bad_grid(nb, nz, ny, nx, is3d)) return fail(ctx, "debug_conv_fp32: bad grid %dx%dx%dx%d", nb, nz, ny, nx);
   const int taps = (is3d ? ks : 1) * ks * ks;
-  const std::vector<float> relaid = relayout_conv_weights(w_host, cin, cout, taps);
-  float *dw = nullptr, *db = nullptr;
-  if (cudaMalloc((void**)&dw, relaid.size() * 4) != cudaSuccess || cudaMalloc((void**)&db, cout * 4) != cudaSuccess) {
-    if (dw) cudaFree(dw);
-    return fail(ctx, "debug_conv_fp32: cudaMalloc failed");
-  }
-  cudaMemcpy(dw, relaid.data(), relaid.size() * 4, cudaMemcpyHostToDevice);
-  cudaMemcpy(db, bias_host, cout * 4, cudaMemcpyHostToDevice);
+  const DevPtr<float> dw = upload(relayout_conv_weights(w_host, cin, cout, taps)), db = upload(bias_host, cout);
+  if (!dw || !db) return fail(ctx, "debug_conv_fp32: cudaMalloc failed");
   const Geo g = whole_grid(ctx, nb, nz, ny, nx, is3d);
-  const int ran = generic ? launch_conv_any(in, out, dw, db, cin, cout, ks, act, g, ctx->stream, dil)
-                          : launch_conv_direct(in, out, dw, db, cin, cout, ks, act, g, ctx->stream, dil);
-  const int rc = finish_debug(ctx, "debug_conv_fp32");
-  cudaFree(dw);
-  cudaFree(db);
-  if (rc) return rc;
+  const int ran = generic ? launch_conv_any(in, out, dw.get(), db.get(), cin, cout, ks, act, g, ctx->stream, dil)
+                          : launch_conv_direct(in, out, dw.get(), db.get(), cin, cout, ks, act, g, ctx->stream, dil);
+  if (const int rc = finish_debug(ctx, "debug_conv_fp32")) return rc;
   if (ran < 0) return fail(ctx, "debug_conv_fp32: no kernel for cout=%d k=%d", cout, ks);
   *kernel = ran;
   return 0;
@@ -1106,30 +1066,18 @@ int tfl_debug_bn(tfl_ctx* ctx, float* x, int nb, int c, int64_t n, int64_t bstri
   if (!ctx) return 1;
   if (!x || !stats_host || !ac_host) return fail(ctx, "debug_bn: nil argument");
   if (nb < 1 || c < 1 || n < 1 || bstride < (int64_t)c * n || !(eps >= 0.0f)) return fail(ctx, "debug_bn: bad arguments");
-  float *wb = nullptr, *ac = nullptr;
-  double *part = nullptr, *stats = nullptr;
-  auto release = [&]() {
-    for (void* p : {(void*)wb, (void*)ac, (void*)part, (void*)stats})
-      if (p) cudaFree(p);
-  };
-  if (cudaMalloc((void**)&wb, 2 * c * 4) != cudaSuccess || cudaMalloc((void**)&ac, 2 * c * 4) != cudaSuccess ||
-      cudaMalloc((void**)&part, sizeof(double) * 2 * (kBnBlocks + 1) * c) != cudaSuccess ||
-      cudaMalloc((void**)&stats, sizeof(double) * 2 * c) != cudaSuccess) {
-    release();
-    return fail(ctx, "debug_bn: cudaMalloc failed");
-  }
-  if (w_host) cudaMemcpy(wb, w_host, c * 4, cudaMemcpyHostToDevice);
-  if (b_host) cudaMemcpy(wb + c, b_host, c * 4, cudaMemcpyHostToDevice);
-  launch_bn_stats(x, nb, c, n, bstride, part, ctx->stream);
-  launch_bn_finalize(part, c, (long long)nb * n, w_host ? wb : nullptr, b_host ? wb + c : nullptr, eps, ac, stats,
-                     ctx->stream);
-  launch_bn_apply(x, nb, c, n, bstride, ac, ctx->stream);
-  int rc = finish_debug(ctx, "debug_bn");
-  if (!rc && (cudaMemcpy(stats_host, stats, sizeof(double) * 2 * c, cudaMemcpyDeviceToHost) != cudaSuccess ||
-              cudaMemcpy(ac_host, ac, 2 * c * 4, cudaMemcpyDeviceToHost) != cudaSuccess))
-    rc = fail(ctx, "debug_bn: copy failed");
-  release();
-  return rc;
+  const DevPtr<float> w = w_host ? upload(w_host, c) : DevPtr<float>(),
+                      b = b_host ? upload(b_host, c) : DevPtr<float>(), ac = dev_alloc<float>(2 * c);
+  const DevPtr<double> part = dev_alloc<double>(2 * (kBnBlocks + 1) * c), stats = dev_alloc<double>(2 * c);
+  if ((w_host && !w) || (b_host && !b) || !ac || !part || !stats) return fail(ctx, "debug_bn: cudaMalloc failed");
+  launch_bn_stats(x, nb, c, n, bstride, part.get(), ctx->stream);
+  launch_bn_finalize(part.get(), c, (long long)nb * n, w.get(), b.get(), eps, ac.get(), stats.get(), ctx->stream);
+  launch_bn_apply(x, nb, c, n, bstride, ac.get(), ctx->stream);
+  if (const int rc = finish_debug(ctx, "debug_bn")) return rc;
+  if (cudaMemcpy(stats_host, stats.get(), sizeof(double) * 2 * c, cudaMemcpyDeviceToHost) != cudaSuccess ||
+      cudaMemcpy(ac_host, ac.get(), 2 * c * 4, cudaMemcpyDeviceToHost) != cudaSuccess)
+    return fail(ctx, "debug_bn: copy failed");
+  return 0;
 }
 
 void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
@@ -1137,51 +1085,59 @@ void tfl_cnn_destroy(tfl_ctx* ctx, tfl_cnn* m) {
   NvtxRange range_(__func__);
   if (!m) return;
   if (ctx) cudaStreamSynchronize(ctx->stream);
-  for (float* p : m->w) cudaFree(p);
-  for (float* p : m->b) cudaFree(p);
-  if (m->tail) cudaFree(m->tail);
-  for (float* p : m->act)
-    if (p) cudaFree(p);
-  for (int sp = 0; sp < 2; sp++) {
-    for (float* p : m->wBk[sp]) cudaFree(p);
-    for (float* p : m->wBj[sp]) cudaFree(p);
-  }
-  for (float* p : m->bact) cudaFree(p);
-  if (m->part) cudaFree(m->part);
-  for (float* p : m->bn_wb) cudaFree(p);
-  for (float* p : m->bn_ac) cudaFree(p);
-  if (m->bn_part) cudaFree(m->bn_part);
-  if (m->bn_tcac) cudaFree(m->bn_tcac);
   delete m;
 }
 
-// One rotating buffer of bank i (0-based, i >= 1): a multi-resolution bank holds 2^-d i of bank 1's cells, and every
-// activation of bank 1 fits max_rel; a dilated bank has bank 1's resolution and needs its own largest activation,
-// bank_rel (the joined banks live in bank 1's buffers).
-static size_t cnn_bank_buf_bytes(const tfl_cnn* m, const Geo& g, int i) {
-  const double cells = (double)g.n * g.nb;
-  if (m->bank_dilate) return (size_t)(cells * m->bank_rel + 64) * 4;
-  return (size_t)(cells * m->max_rel / (double)(1LL << ((m->is3d ? 3 : 2) * i)) + 64) * 4;
+// The fp32 path's scratch in the arena, in pieces aligned to 256 bytes from `base`.  Over a null base only `bytes` is
+// meaningful: what arena_reserve needs, 256 bytes beyond each piece (at least its alignment) and 768 more.
+struct CnnScratch {
+  float *U1, *x0, *actA, *actB, *scale;
+  double* bn_part;     // batch statistics: the partial sums and (a, c) of one BN module at a time
+  float* bn_ac;
+  float* actC;         // the third rotating buffer of the graphs that are not plain
+  float* bank[kMaxBanks][3];
+  size_t bytes;
+};
+static CnnScratch cnn_scratch(const tfl_cnn* m, const Geo& g, char* base) {
+  CnnScratch s = {};
+  s.bytes = 3 * 256;
+  size_t off = 0;
+  auto take = [&](size_t bytes) {
+    char* p = base ? base + off : nullptr;
+    off = (off + bytes + 255) & ~(size_t)255;
+    s.bytes += bytes + 256;
+    return p;
+  };
+  const size_t cells = (size_t)g.n * g.nb;
+  s.U1 = (float*)take(cells * 4 * g.nc);
+  s.x0 = (float*)take(cells * 4 * m->in_ch);
+  s.actA = (float*)take(cells * 4 * m->max_c);      // max_c covers max_rel (set at creation)
+  s.actB = (float*)take(cells * 4 * m->max_c);
+  s.scale = (float*)take(sizeof(float) * g.nb);
+  s.bn_part = (double*)take(sizeof(double) * 2 * (kBnBlocks + 1) * m->bn_max_c);
+  s.bn_ac = (float*)take(sizeof(float) * 2 * m->bn_max_c);
+  if (m->plain) return s;
+  s.actC = (float*)take((size_t)((double)cells * m->max_rel + 64) * 4);
+  // Banks 2..N rotate through buffers of their own.  A multi-resolution bank i (0-based) holds 2^-d i of bank 1's
+  // cells, and every activation of bank 1 fits max_rel; a dilated bank has bank 1's resolution and needs its own
+  // largest activation, bank_rel (the joined banks live in bank 1's buffers).  A dilated stage is convolution ->
+  // non-linearity -> pooling (no pixel shuffle), so its result can go back to the buffer its input came from, and two
+  // buffers suffice: run_stage alternates them.
+  for (int i = 1; i < m->nbanks; i++) {
+    const double rel = m->bank_dilate ? m->bank_rel : m->max_rel / (double)(1LL << ((m->is3d ? 3 : 2) * i));
+    for (int q = 0; q < (m->bank_dilate ? 2 : 3); q++)
+      s.bank[i][q] = (float*)take((size_t)((double)cells * rel + 64) * 4);
+    if (m->bank_dilate) s.bank[i][2] = s.bank[i][0];
+  }
+  return s;
 }
-// Rotating buffers of each of banks 2..N: a dilated stage is convolution -> non-linearity -> pooling (no pixel
-// shuffle), so its result can go back to the buffer its input came from, and two suffice.
-static int cnn_bank_nbufs(const tfl_cnn* m) { return m->bank_dilate ? 2 : 3; }
 
 static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const float* U_div,
                             const float* flags, float* p_out, float* U_out, float threshold, const Geo& g,
-                            char* scratch, float** scale_dev_out) {
-  // scratch layout (caller reserved): U1 [nc], x0 [cin[0]], actA [max_c], actB [max_c], scale [nb]
-  const size_t cells = (size_t)g.n * g.nb;
-  size_t off = 0;
-  auto take = [&](size_t bytes) { char* p = scratch + off; off = (off + bytes + 255) & ~(size_t)255; return p; };
-  float* U1 = (float*)take(cells * 4 * g.nc);
-  float* x0 = (float*)take(cells * 4 * m->in_ch);
-  float* actA = (float*)take(cells * 4 * m->max_c);      // max_c covers max_rel (set at creation)
-  float* actB = (float*)take(cells * 4 * m->max_c);
-  float* scale = (float*)take(sizeof(float) * g.nb);
-  // batch statistics: the partial sums and (a, c) of one BN module at a time (cnn_scratch_bytes)
-  double* bn_part = (double*)take(sizeof(double) * 2 * (kBnBlocks + 1) * m->bn_max_c);
-  float* bn_ac = (float*)take(sizeof(float) * 2 * m->bn_max_c);
+                            const CnnScratch& scr, float** scale_dev_out) {
+  float *U1 = scr.U1, *x0 = scr.x0, *actA = scr.actA, *actB = scr.actB, *scale = scr.scale;
+  double* bn_part = scr.bn_part;
+  float* bn_ac = scr.bn_ac;
   double* sums = ctx->dscratch + 64;
   cudaStream_t st = ctx->stream;
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
@@ -1195,7 +1151,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
   if (m->mode > 0 && m->tc_ok && !ctx->slab) {
     if (cnn_ensure_act(ctx, m, g)) return 1;
     const ConvTcGeo& tg = m->act_geo;
-    launch_cnn_inputs_padded(p_div, U1, flags, scale, m->act[0], tg.px, tg.py, g, st, m->in_sel, m->tc_planes);
+    launch_cnn_inputs_padded(p_div, U1, flags, scale, m->act[0].get(), tg.px, tg.py, g, st, m->in_sel, m->tc_planes);
     float* p_net = actA;      // plain [b][z][y][x]
     run_conv_stack(m, p_net, st);
     if (m->skip) {
@@ -1215,7 +1171,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
     for (int l = 0; l < m->n_layers; l++) {
       float* o = bufs[l & 1];
       const int act = (l < m->n_layers - 1) ? 1 : 0;
-      if (launch_conv_direct(in, o, m->w[l], m->b[l], m->cin[l], m->cout[l], m->ks[l], act, g, st) < 0)
+      if (launch_conv_direct(in, o, m->w[l].get(), m->b[l].get(), m->cin[l], m->cout[l], m->ks[l], act, g, st) < 0)
         return fail(ctx, "cnn: unsupported layer shape cout=%d k=%d", m->cout[l], m->ks[l]);
       ctx->launches += 1;
       in = o;
@@ -1224,14 +1180,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
     // 'tog' / 'yang' graphs: conv (+ pixel shuffle) -> non-linearity -> pooling, layer by layer, on grids
     // whose resolution follows the pooling / upsampling sizes (lib/model.lua:262-340, single bank).
     if (ctx->slab) return fail(ctx, "cnn: pooled / upsampled graphs run on whole grids only");
-    float* bufs[3] = {actA, actB, (float*)take((size_t)((double)cells * m->max_rel + 64) * 4)};
-    // Banks 2..N rotate through three buffers of their own (a multi-resolution bank i is 2^-d(i-1) the size of
-    // bank 1, a dilated one the same size).
-    float* bank_bufs[kMaxBanks][3] = {};
-    for (int i = 1; i < m->nbanks; i++) {
-      for (int q = 0; q < cnn_bank_nbufs(m); q++) bank_bufs[i][q] = (float*)take(cnn_bank_buf_bytes(m, g, i));
-      if (cnn_bank_nbufs(m) == 2) bank_bufs[i][2] = bank_bufs[i][0];     // run_stage alternates the two
-    }
+    float* bufs[3] = {actA, actB, scr.actC};
     // One stage of one bank: convolution ci (dilated by dil) (+ pixel shuffle) -> non-linearity -> pooling, on grid
     // gl, through the rotating buffers bb, never writing `keep` (an input other banks still read).  out_bstride > 0:
     // the stage's result is written with that batch stride (floats), so that it lands in place in a concatenation
@@ -1253,8 +1202,8 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
         if (nloop_conv > 1) gb.nb = 1;
         const long long ioff = nloop_conv > 1 ? (long long)b * m->cin[ci] * gl.n : 0;
         const long long ooff = nloop_conv > 1 ? (long long)b * out_bstride : 0;
-        if (launch_conv_direct(src + ioff, o + ooff, m->w[ci], m->b[ci], m->cin[ci], m->cout[ci], m->ks[ci], act, gb, st,
-                               dil) < 0)
+        if (launch_conv_direct(src + ioff, o + ooff, m->w[ci].get(), m->b[ci].get(), m->cin[ci], m->cout[ci],
+                               m->ks[ci], act, gb, st, dil) < 0)
           return fail(ctx, "cnn: unsupported layer shape cout=%d k=%d", m->cout[ci], m->ks[ci]);
         ctx->launches += 1;
       }
@@ -1292,10 +1241,10 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
       if (m->bn && l < m->n_layers - 1) {     // lib/model.lua:343-350: BN closes every stage but the last
         float* x = (float*)cur;               // one of this call's buffers, or a slot of one
         const long long bs = out_bstride > 0 ? out_bstride : (long long)chans * gl.n;
-        const float* ac = m->bn_batch ? bn_ac : m->bn_ac[ci];
+        const float* ac = m->bn_batch ? bn_ac : m->bn_ac[ci].get();
         if (m->bn_batch) {
           launch_bn_stats(x, gl.nb, chans, gl.n, bs, bn_part, st);
-          launch_bn_finalize(bn_part, chans, (long long)gl.nb * gl.n, m->bn_wb[ci], m->bn_wb[ci] + chans,
+          launch_bn_finalize(bn_part, chans, (long long)gl.nb * gl.n, m->bn_wb[ci].get(), m->bn_wb[ci].get() + chans,
                              m->bn_eps[ci], bn_ac, nullptr, st);
           ctx->launches += 2;
         }
@@ -1326,13 +1275,13 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
         bank_g[0] = gl;
         for (int i = 1; i < nbk; i++) {
           Geo gi = bank_g[i - 1];
-          launch_pool(bank_in[i - 1], bank_bufs[i][0], gi.nb * m->cin[m->conv0[l]], gi.nz, gi.ny, gi.nx, 2, gi.is3d, 0, st);
+          launch_pool(bank_in[i - 1], scr.bank[i][0], gi.nb * m->cin[m->conv0[l]], gi.nz, gi.ny, gi.nx, 2, gi.is3d, 0, st);
           ctx->launches += 1;
           gi.nx /= 2; gi.ny /= 2; if (gi.is3d) gi.nz /= 2;
           gi.n = (long long)gi.nx * gi.ny * gi.nz;
           gi.gnz = gi.nz; gi.zlo = 0; gi.zhi = gi.nz;
           bank_g[i] = gi;
-          bank_in[i] = bank_bufs[i][0];
+          bank_in[i] = scr.bank[i][0];
         }
       }
       if (nbk > 1 && l >= m->split && l < m->join) {
@@ -1351,7 +1300,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
           const long long bstride = (last && (i == 0 || in_slot) && !m->bank_add && g.nb > 1)
                                         ? (long long)nbk * c_out * n_join : 0;
           float* dst = (in_slot && i > 0) ? (float*)bank_in[0] + (long long)i * c_out * n_join : nullptr;
-          if (run_stage(m->conv0[l] + i, l, bank_in[i], i == 0 ? bufs : bank_bufs[i], bank_g[i], bstride, &bank_in[i],
+          if (run_stage(m->conv0[l] + i, l, bank_in[i], i == 0 ? bufs : scr.bank[i], bank_g[i], bstride, &bank_in[i],
                         m->bank_dilate ? 1 << i : 1, shared, dst))
             return 1;
         }
@@ -1393,15 +1342,6 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
   return check_launch(ctx, "cnn_project");
 }
 
-static size_t cnn_scratch_bytes(const tfl_cnn* m, const Geo& g) {
-  const size_t cells = (size_t)g.n * g.nb;
-  size_t bytes = cells * 4 * (g.nc + m->in_ch + 2 * (size_t)m->max_c) + 4 * g.nb + 8 * 256;
-  bytes += (sizeof(double) * 2 * (kBnBlocks + 1) + sizeof(float) * 2) * (size_t)m->bn_max_c + 2 * 256;
-  if (!m->plain) bytes += (size_t)((double)cells * m->max_rel + 64) * 4 + 256;     // third rotating buffer
-  for (int i = 1; i < m->nbanks; i++) bytes += cnn_bank_nbufs(m) * (cnn_bank_buf_bytes(m, g, i) + 256);
-  return bytes;
-}
-
 int tfl_cnn_project(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, const tfl_grid* U_div,
                     const tfl_grid* flags, const tfl_grid* p_out, const tfl_grid* U_out, float threshold,
                     float* scale_out) {
@@ -1417,10 +1357,10 @@ int tfl_cnn_project(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, const tfl_g
   if (ctx->slab) return fail(ctx, "cnn_project on a z-slab goes through the multi-GPU driver");
   Geo g;
   if (make_geo(ctx, flags, m->is3d, &g)) return 1;
-  if (arena_reserve(ctx, cnn_scratch_bytes(m, g))) return 1;
+  if (arena_reserve(ctx, cnn_scratch(m, g, nullptr).bytes)) return 1;
   float* scale_dev = nullptr;
   if (cnn_project_impl(ctx, m, p_div->data, U_div->data, flags->data, p_out->data, U_out->data, threshold, g,
-                       ctx->arena, &scale_dev))
+                       cnn_scratch(m, g, ctx->arena), &scale_dev))
     return 1;
   if (scale_out) {
     TFL_CUDA(ctx, cudaMemcpyAsync(scale_out, scale_dev, sizeof(float) * g.nb, cudaMemcpyDeviceToHost, ctx->stream));
@@ -1462,10 +1402,7 @@ int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, c
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!m) return fail(ctx, "cnn is nil");
-  if (m->bn) return fail(ctx, "cnn_project_from_sums: %s", kSlabBatchNorm);
-  if (m->bank_dilate) return fail(ctx, "cnn_project_from_sums: %s", kSlabDilate);
-  if (!m->default_inputs) return fail(ctx, "cnn_project_from_sums: %s", kSlabDefaultInputs);
-  if (!m->tc_ok || m->mode == 0) return fail(ctx, "cnn_project_from_sums: %s", kSlabTcOnly);
+  if (const char* why = cnn_slab_refusal(m)) return fail(ctx, "cnn_project_from_sums: %s", why);
   if (!dev_sums) return fail(ctx, "cnn_project_from_sums: nil sums");
   if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, p_div, "pDiv") || check_vel(ctx, U1, flags) ||
       check_scalar(ctx, p_out, "p") || check_vel(ctx, U_out, flags))
@@ -1490,7 +1427,7 @@ int tfl_cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, c
     gi.zhi = (g.zoff + g.nz == g.gnz) ? g.nz : g.nz - 2;
   }
   const ConvTcGeo& tg = m->act_geo;
-  launch_cnn_inputs_padded(p_div->data, U1->data, flags->data, scale, m->act[0], tg.px, tg.py, gi, st);
+  launch_cnn_inputs_padded(p_div->data, U1->data, flags->data, scale, m->act[0].get(), tg.px, tg.py, gi, st);
   // the velocity update of the computed planes [zlo, zhi) reads p on [zlo - 1, zhi)
   if (ctx->slab) run_conv_stack(m, p_net, st, g.zlo - 1, g.zhi);
   else run_conv_stack(m, p_net, st);

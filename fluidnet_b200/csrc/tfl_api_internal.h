@@ -7,6 +7,7 @@
 #include <nvtx3/nvToolsExt.h>
 #include <nccl.h>      // types and prototypes only: libnccl is loaded on demand (dlopen), see tfl_api_slab.cu
 #include <initializer_list>
+#include <memory>
 #include <string>
 #include <vector>
 
@@ -14,6 +15,16 @@
 #include "tfl_cnn_tc.h"
 
 using namespace tfl;
+
+// Device memory held by std::unique_ptr: cudaFree runs when the holder goes.
+struct CudaFree {
+  void operator()(void* p) const { cudaFree(p); }
+};
+template <typename T>
+using DevPtr = std::unique_ptr<T, CudaFree>;
+
+constexpr char kConvZStalled[] =
+    "internal error, the z-streaming tensor-core convolution's pipeline stalled (a bounded wait ran out)";
 
 struct tfl_ctx {
   int device = 0;
@@ -79,8 +90,8 @@ struct tfl_cnn {
   int is3d = 1;
   int n_layers = 0;
   std::vector<int> cin, cout, ks;   // per convolution (= per stage unless banked)
-  std::vector<float*> w;     // device, [cin][tap][cout]
-  std::vector<float*> b;     // device, [cout]
+  std::vector<DevPtr<float>> w;     // device, [cin][tap][cout]
+  std::vector<DevPtr<float>> b;     // device, [cout]
   // multi-resolution banks (lib/model.lua:252-361): stages [split, join) (0-based here) hold one convolution
   // per bank; conv0[l] is the index of stage l's first convolution.  nbanks == 1: single bank.
   int nbanks = 1, split = 0, join = 0, bank_add = 0;
@@ -100,12 +111,12 @@ struct tfl_cnn {
   // bn_wb [2][c] (weight, bias) and eps for batch statistics, or bn_ac [2][c] (a, c of y = a x + c, computed at
   // creation from the running statistics).  bn_max_c: the most channels of one BN module (sizes the scratch).
   bool bn = false, bn_batch = false;
-  std::vector<float*> bn_wb, bn_ac;
+  std::vector<DevPtr<float>> bn_wb, bn_ac;
   std::vector<float> bn_eps;
   int bn_max_c = 0;
   // batch statistics on the tensor cores (run_conv_stack): the partials of one module and the (a, c) of BN1..BN4
-  double* bn_part = nullptr;
-  float* bn_tcac = nullptr;
+  DevPtr<double> bn_part;
+  DevPtr<float> bn_tcac;
   bool plain = true;
   double max_rel = 0.0;      // largest channels x (cells relative to the input grid) of any stage
   double bank_rel = 0.0;     // the same over one bank's activations in the banked stages (conv output, pooled)
@@ -121,8 +132,8 @@ struct tfl_cnn {
   // tensor-core path (3-D 'default' architecture, single-bank or with banks split at stage 1 and joined at stage 3)
   int mode = 0;              // 0 fp32 FMA, 1 TF32 tensor cores, 2 3xTF32 tensor cores
   bool tc_ok = false;
-  float* tail = nullptr;     // w4[8][8], b4[8], w5[8], b5[1]
-  float* act[3] = {nullptr, nullptr, nullptr};   // padded channels-last activation buffers
+  DevPtr<float> tail;        // w4[8][8], b4[8], w5[8], b5[1]
+  DevPtr<float> act[3];      // padded channels-last activation buffers
   ConvTcGeo act_geo = {0, 0, 0, 0, 0, 0, 0, 0, 0, 0, 0};
   int act_zoff = 0;          // global plane of act's local plane 0 (z-slab; 0 on whole grids)
   unsigned long long act_gen = 0;   // bumped whenever act / bact / part are reallocated (see tfl_ctx::arena_gen)
@@ -131,11 +142,11 @@ struct tfl_cnn {
   // own three padded buffers each (pyramid input, layer 1, layer 2) at their resolution; 'concat' with N > 1 adds
   // an fp32 partial sum.  On a z-slab, bank i's local plane 0 is its global coarse plane borg[i - 1] =
   // ceil(act_zoff / 2^i), and it holds the coarse planes whose 2^i fine planes all lie in the local slab.
-  std::vector<float*> wBk[2], wBj[2];
-  std::vector<float*> bact;
+  std::vector<DevPtr<float>> wBk[2], wBj[2];
+  std::vector<DevPtr<float>> bact;
   std::vector<ConvTcGeo> bgeo;
   std::vector<int> borg;
-  float* part = nullptr;
+  DevPtr<float> part;
 };
 
 // Every entry point runs on the context's device whatever the caller's current device is, and leaves the

@@ -1,7 +1,7 @@
 """The input block of the projection network (lib/model.lua:27-150, :357-387: inputChannels, normalizeInput,
 normalizeInputFunc, normalizeInputChan, addPressureSkip) on the GPU: model:forward against the CPU restatement
 (tests/inputs_oracle.py, pinned on torch.nn.functional by tests/test_oracle_model_inputs.py), the returned scale,
-the default block against tfl_cnn_create_banked bit for bit, layer 1 and the bank pyramid on the two-plane
+the default block built by every creator bit for bit, layer 1 and the bank pyramid on the two-plane
 tensor-core input, the step and its graph, and the z-slab refusal.
 
 Tolerances as tests/test_gpu_cnn_banks.py: p and U within 2e-5 (fp32, 3xTF32) or 3e-3 (TF32) of each entry's max,
@@ -130,20 +130,36 @@ def test_scale(func, chan):
             assert np.all(np.abs(gm.last_scale - want) <= 1e-6 * want), (gm.last_scale, want)
 
 
-def banked_twin(mnp):
-    """The model of tfl_cnn_create_banked (banks NULL) for mnp's single-bank layers, in a ProjectionModel shell."""
-    gm = make_gpu(mnp)
+# The six creators, with the arguments between ksize and weights: all NULL or 0 (the single-bank graph, the default
+# input block, no normalization).
+CREATORS = {"tfl_cnn_create": [], "tfl_cnn_create_graph": [None, None, 0, 0],
+            "tfl_cnn_create_banked": [None, None, 0, 0, None],
+            "tfl_cnn_create_model": [None, None, 0, 0, None, None],
+            "tfl_cnn_create_model_ex": [None, None, 0, 0, None, None],
+            "tfl_cnn_create_model_norm": [None, None, 0, 0, None, None, None]}
+
+
+def create_via(gm, creator, mnp, cin="layers"):
+    """(rc, handle) of `creator` on mnp's single-bank layers in gm's context; cin: a list, None (NULL), or the
+    layers' input channels."""
     layers = mnp["layers"]
     n = len(layers)
     arr = lambda v: (C.c_int32 * n)(*v)
+    cin = [w.shape[1] for w, _ in layers] if cin == "layers" else cin
     wp = (C.POINTER(C.c_float) * n)(*[w.ctypes.data_as(C.POINTER(C.c_float)) for w, _ in layers])
     bp = (C.POINTER(C.c_float) * n)(*[b.ctypes.data_as(C.POINTER(C.c_float)) for _, b in layers])
     h = C.c_void_p()
-    gm.ctx.check(gm.ctx.lib.tfl_cnn_create_banked(gm.ctx.h, 1 if mnp["is3D"] else 0, n,
-                                                  arr([w.shape[1] for w, _ in layers]),
-                                                  arr([w.shape[0] for w, _ in layers]),
-                                                  arr([w.shape[4] for w, _ in layers]), None, None, 0, 0, None, wp, bp,
-                                                  C.byref(h)))
+    rc = getattr(gm.ctx.lib, creator)(gm.ctx.h, 1 if mnp["is3D"] else 0, n, None if cin is None else arr(cin),
+                                      arr([w.shape[0] for w, _ in layers]), arr([w.shape[4] for w, _ in layers]),
+                                      *CREATORS[creator], wp, bp, C.byref(h))
+    return rc, h
+
+
+def twin(mnp, creator):
+    """The model `creator` builds for mnp's single-bank layers, in a ProjectionModel shell."""
+    gm = make_gpu(mnp)
+    rc, h = create_via(gm, creator, mnp)
+    gm.ctx.check(rc)
     gm.ctx.lib.tfl_cnn_destroy(gm.ctx.h, gm.h)
     gm.h = h
     return gm
@@ -151,17 +167,26 @@ def banked_twin(mnp):
 
 @pytest.mark.parametrize("is3d", [True, False], ids=["3d", "2d"])
 def test_default_block_is_the_banked_model(is3d):
-    """tfl_cnn_create_model with the default block gives the bits of tfl_cnn_create_banked's model in every mode."""
+    """Every creator builds the model of tfl_cnn_create_model with the default block: the same bits in every mode.
+    Each refuses a channel mismatch with the same message, and a NULL cin as a bad argument."""
     shape = (8, 12, 16) if is3d else (1, 24, 20)
     batch = make_batch(shape, is3d, nb=2)
     mnp = synth.make_model(is3d, inputs=ins())
     _, inp = inputs_of(batch)
-    a, b = make_gpu(mnp), banked_twin(mnp)
-    for mode in (["tf32x3", "tf32", "fp32"] if is3d else ["fp32"]):
-        a.set_mode(mode)
-        b.set_mode(mode)
-        for x, y in zip(a.forward(inp), b.forward(inp)):
-            assert torch.equal(x.view(torch.int32), y.view(torch.int32)), mode
+    a = make_gpu(mnp)
+    cin = [w.shape[1] for w, _ in mnp["layers"]]
+    cin[2] += 1
+    for creator in CREATORS:
+        b = twin(mnp, creator)
+        for mode in (["tf32x3", "tf32", "fp32"] if is3d else ["fp32"]):
+            a.set_mode(mode)
+            b.set_mode(mode)
+            for x, y in zip(a.forward(inp), b.forward(inp)):
+                assert torch.equal(x.view(torch.int32), y.view(torch.int32)), (creator, mode)
+        for bad, msg in ((cin, "cnn: channel mismatch at layer 2"), (None, "cnn: bad arguments")):
+            rc, h = create_via(a, creator, mnp, cin=bad)
+            assert rc != 0 and not h.value, creator
+            assert a.ctx.lib.tfl_last_error(a.ctx.h).decode() == msg, creator
 
 
 @pytest.mark.parametrize("split", [1, 0], ids=["tf32x3", "tf32"])
