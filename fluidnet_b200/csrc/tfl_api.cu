@@ -29,25 +29,23 @@ void widen_for_forward_pass(const tfl_ctx* ctx, const Geo& g, Geo* gf) {
 int flag_cache_ensure(tfl_ctx* ctx, const Geo& g) {
   auto& fc = ctx->fcache;
   const size_t cells = (size_t)g.n * g.nb;
+  void* p = nullptr;
   if (!fc.changed) {
-    void* p = nullptr;
     TFL_CUDA(ctx, cudaMalloc(&p, sizeof(int)));
-    fc.changed = (int*)p;
+    fc.changed.reset((int*)p);
   }
   if (fc.bytes && fc.cells == cells && fc.nb == g.nb && fc.nz == g.nz && fc.ny == g.ny && fc.nx == g.nx) {
-    TFL_CUDA(ctx, cudaMemsetAsync(fc.changed, 0, sizeof(int), ctx->stream));
+    TFL_CUDA(ctx, cudaMemsetAsync(fc.changed.get(), 0, sizeof(int), ctx->stream));
     return 0;
   }
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (fc.bytes) cudaFree(fc.bytes);
-  fc.bytes = nullptr;
+  fc.bytes.reset();                         // before the new one is allocated
   fc.gen++;
-  void* p = nullptr;
   TFL_CUDA(ctx, cudaMalloc(&p, 3 * cells + 64));
-  fc.bytes = (unsigned char*)p;
+  fc.bytes.reset((unsigned char*)p);
   fc.cells = cells; fc.nb = g.nb; fc.nz = g.nz; fc.ny = g.ny; fc.nx = g.nx;
-  TFL_CUDA(ctx, cudaMemsetAsync(fc.bytes, 0, 3 * cells + 64, ctx->stream));
-  TFL_CUDA(ctx, cudaMemsetAsync(fc.changed, 1, sizeof(int), ctx->stream));     // non-zero: rebuild
+  TFL_CUDA(ctx, cudaMemsetAsync(fc.bytes.get(), 0, 3 * cells + 64, ctx->stream));
+  TFL_CUDA(ctx, cudaMemsetAsync(fc.changed.get(), 1, sizeof(int), ctx->stream));     // non-zero: rebuild
   return 0;
 }
 
@@ -57,15 +55,15 @@ int prepare_flags(tfl_ctx* ctx, const float* flags, const Geo& g, unsigned char*
   const size_t cells = (size_t)g.n * g.nb;
   auto& fc = ctx->fcache;
   if (fc.fresh_for == flags && fc.bytes && fc.cells == cells && fc.nz == g.nz && fc.ny == g.ny && fc.nx == g.nx) {
-    *fl8 = fc.bytes;                        // refreshed earlier in this (slab) step: nothing wrote the flags since
-    *clear = fc.bytes + cells;
+    *fl8 = fc.bytes.get();                  // refreshed earlier in this (slab) step: nothing wrote the flags since
+    *clear = fc.bytes.get() + cells;
     return 0;
   }
   if (flag_cache_ensure(ctx, g)) return 1;
-  *fl8 = ctx->fcache.bytes;
-  *clear = ctx->fcache.bytes + cells;
-  launch_flags_to_u8(flags, *fl8, (long long)cells, ctx->fcache.changed, ctx->stream);
-  ctx->launches += 1 + launch_clearance(*fl8, *clear, *clear + cells, g, ctx->fcache.changed, ctx->stream);
+  *fl8 = fc.bytes.get();
+  *clear = fc.bytes.get() + cells;
+  launch_flags_to_u8(flags, *fl8, (long long)cells, fc.changed.get(), ctx->stream);
+  ctx->launches += 1 + launch_clearance(*fl8, *clear, *clear + cells, g, fc.changed.get(), ctx->stream);
   if (ctx->in_slab_step) fc.fresh_for = flags;
   return 0;
 }
@@ -76,7 +74,7 @@ int tile_halo_choice(tfl_ctx* ctx, bool probe) {
   auto& tl = ctx->tile;
   if (tl.mode >= 0) return tl.mode;
   float longest = 0.0f;
-  if (tl.host) { const unsigned int bits = *(volatile unsigned int*)tl.host; memcpy(&longest, &bits, 4); }
+  if (tl.host) { const unsigned int bits = *(volatile unsigned int*)tl.host.get(); memcpy(&longest, &bits, 4); }
   int hf = longest < 0.45f ? 1 : (longest < 1.4f ? 2 : 0);
   // beyond the wide halo the per-pass kernels are faster; the velocity kernel looks again every 16th call
   if (hf == 0 && probe && ++tl.calls_since_probe >= 16) { hf = 2; tl.calls_since_probe = 0; }
@@ -92,19 +90,19 @@ int advect_vel_dispatch(tfl_ctx* ctx, float dt, const float* U, const FT* flags,
   const bool ours = method == TFL_ADVECT_MACCORMACK_OURS || method == TFL_ADVECT_RK2_OURS || method == TFL_ADVECT_RK3_OURS;
   auto& tl = ctx->tile;
   if (ours && fl8 && clear && tl.mode != 0) {
-    if (!tl.dev) {
-      void* p = nullptr;
-      if (cudaMalloc(&p, sizeof(unsigned int)) == cudaSuccess) tl.dev = (unsigned int*)p;
-      if (cudaHostAlloc(&p, sizeof(unsigned int), cudaHostAllocDefault) == cudaSuccess) { tl.host = (unsigned int*)p; *tl.host = 0; }
+    if (!tl.dev || !tl.host) {
+      if (!tl.dev) tl.dev = dev_alloc<unsigned int>(1);
+      if (!tl.host && (tl.host = pinned_alloc<unsigned int>(1))) *tl.host = 0;
+      if (!tl.dev || !tl.host) cudaGetLastError();    // no telemetry: the two-kernel version runs, nothing fails
     }
     const int hf = tile_halo_choice(ctx, true);
     if (hf > 0 && tl.dev && tl.host) {
-      cudaMemsetAsync(tl.dev, 0, sizeof(unsigned int), st);
-      if (tl.timed) cudaEventRecord(tl.ev0, st);
-      const bool launched = launch_advect_vel_tile(dt, U, fl8, clear, strength, dst, g, hf, tl.variant, tl.dev, st);
-      if (tl.timed) cudaEventRecord(tl.ev1, st);
+      cudaMemsetAsync(tl.dev.get(), 0, sizeof(unsigned int), st);
+      if (tl.timed) cudaEventRecord(tl.ev0.get(), st);
+      const bool launched = launch_advect_vel_tile(dt, U, fl8, clear, strength, dst, g, hf, tl.variant, tl.dev.get(), st);
+      if (tl.timed) cudaEventRecord(tl.ev1.get(), st);
       if (launched) {
-        cudaMemcpyAsync(tl.host, tl.dev, sizeof(unsigned int), cudaMemcpyDeviceToHost, st);
+        cudaMemcpyAsync(tl.host.get(), tl.dev.get(), sizeof(unsigned int), cudaMemcpyDeviceToHost, st);
         return 1;
       }
     }
@@ -201,23 +199,17 @@ int tfl_create(tfl_ctx** out, int device) {
   cudaGetDevice(&prev_dev);
   struct Restore { int d; ~Restore() { cudaSetDevice(d); } } restore_{prev_dev};   // caller's device stays current
   if (cudaSetDevice(device) != cudaSuccess) return 1;
-  tfl_ctx* c = new tfl_ctx();
+  // Declared after restore_: on a failure below, what was made is released while `device` is still current.
+  std::unique_ptr<tfl_ctx> c(new tfl_ctx());
   c->device = device;
-  if (cudaStreamCreate(&c->stream) != cudaSuccess) { delete c; return 1; }
-  void* p = nullptr;
-  if (cudaMalloc(&p, 16 * sizeof(unsigned long long)) != cudaSuccess) { delete c; return 1; }
-  c->counters = (unsigned long long*)p;
-  cudaMemset(c->counters, 0, 16 * sizeof(unsigned long long));
-  if (cudaMalloc(&p, 256 * sizeof(double)) != cudaSuccess) { delete c; return 1; }
-  c->dscratch = (double*)p;
-  cudaStreamCreateWithFlags(&c->side_stream, cudaStreamNonBlocking);
-  cudaEventCreateWithFlags(&c->ev_fork, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&c->ev_join, cudaEventDisableTiming);
-  cudaStreamCreateWithFlags(&c->copy_in, cudaStreamNonBlocking);
-  cudaStreamCreateWithFlags(&c->copy_out, cudaStreamNonBlocking);
-  for (cudaEvent_t* e : {&c->ev_u_in, &c->ev_d_in, &c->ev_p_in, &c->ev_d_ready, &c->ev_d_out})
-    cudaEventCreateWithFlags(e, cudaEventDisableTiming);
-  *out = c;
+  if (!(c->own_stream = new_stream(cudaStreamDefault))) return 1;
+  c->stream = c->own_stream.get();
+  if (!(c->counters = dev_zeros<unsigned long long>(16)) || !(c->dscratch = dev_alloc<double>(256))) return 1;
+  for (StreamPtr* q : {&c->side_stream, &c->copy_in, &c->copy_out})
+    if (!(*q = new_stream(cudaStreamNonBlocking))) return 1;
+  for (EventPtr* e : {&c->ev_fork, &c->ev_join, &c->ev_u_in, &c->ev_d_in, &c->ev_p_in, &c->ev_d_ready, &c->ev_d_out})
+    if (!(*e = new_event(cudaEventDisableTiming))) return 1;
+  *out = c.release();
   return 0;
 }
 
@@ -225,24 +217,9 @@ void tfl_destroy(tfl_ctx* ctx) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!ctx) return;
-  cudaSetDevice(ctx->device);
-  cudaStreamSynchronize(ctx->stream);
-  if (ctx->arena) cudaFree(ctx->arena);
-  if (ctx->counters) cudaFree(ctx->counters);
-  if (ctx->dscratch) cudaFree(ctx->dscratch);
-  pcg_release(ctx->pcg);
-  if (ctx->fcache.bytes) cudaFree(ctx->fcache.bytes);
-  if (ctx->fcache.changed) cudaFree(ctx->fcache.changed);
-  if (ctx->tile.dev) cudaFree(ctx->tile.dev);
-  if (ctx->tile.host) cudaFreeHost(ctx->tile.host);
-  if (ctx->tile.ev0) { cudaEventDestroy(ctx->tile.ev0); cudaEventDestroy(ctx->tile.ev1); }
+  for (cudaStream_t q : {ctx->stream, ctx->side_stream.get(), ctx->copy_in.get(), ctx->copy_out.get()})
+    cudaStreamSynchronize(q);
   tfl_comm_destroy(ctx);
-  if (ctx->side_stream) { cudaStreamSynchronize(ctx->side_stream); cudaStreamDestroy(ctx->side_stream); }
-  if (ctx->ev_fork) cudaEventDestroy(ctx->ev_fork);
-  if (ctx->ev_join) cudaEventDestroy(ctx->ev_join);
-  for (cudaStream_t q : {ctx->copy_in, ctx->copy_out}) if (q) { cudaStreamSynchronize(q); cudaStreamDestroy(q); }
-  for (cudaEvent_t e : {ctx->ev_u_in, ctx->ev_d_in, ctx->ev_p_in, ctx->ev_d_ready, ctx->ev_d_out}) if (e) cudaEventDestroy(e);
-  if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
   delete ctx;
 }
 
@@ -255,14 +232,16 @@ int tfl_set_stream(tfl_ctx* ctx, void* s) {
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (s == nullptr) {
     if (!ctx->own_stream) {
-      TFL_CUDA(ctx, cudaStreamCreate(&ctx->stream));
-      ctx->own_stream = true;
+      cudaStream_t q = nullptr;
+      TFL_CUDA(ctx, cudaStreamCreate(&q));
+      ctx->own_stream.reset(q);
+      ctx->stream = q;
     }
     return 0;
   }
-  if (ctx->own_stream && ctx->stream) cudaStreamDestroy(ctx->stream);
+  if ((cudaStream_t)s == ctx->own_stream.get()) return 0;
+  ctx->own_stream.reset();                  // an adopted stream is the caller's: never destroyed here
   ctx->stream = (cudaStream_t)s;
-  ctx->own_stream = false;
   return 0;
 }
 void* tfl_get_stream(tfl_ctx* ctx) { return ctx ? (void*)ctx->stream : nullptr; }
@@ -279,10 +258,10 @@ int tfl_trace_faults(tfl_ctx* ctx, int64_t* count, int reset) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   unsigned long long v = 0;
-  TFL_CUDA(ctx, cudaMemcpyAsync(&v, ctx->counters, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+  TFL_CUDA(ctx, cudaMemcpyAsync(&v, ctx->counters.get(), sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   if (count) *count = (int64_t)v;
-  if (reset) TFL_CUDA(ctx, cudaMemsetAsync(ctx->counters, 0, sizeof(v), ctx->stream));
+  if (reset) TFL_CUDA(ctx, cudaMemsetAsync(ctx->counters.get(), 0, sizeof(v), ctx->stream));
   return 0;
 }
 
@@ -369,13 +348,13 @@ int tfl_flags_to_occupancy(tfl_ctx* ctx, const tfl_grid* flags, const tfl_grid* 
   if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, occ, "occupancy")) return 1;
   if (!same_spatial(flags, occ)) return fail(ctx, "Size mismatch");
   const long long n = (long long)flags->nb * flags->nz * flags->ny * flags->nx;
-  TFL_CUDA(ctx, cudaMemsetAsync(ctx->counters + 1, 0, sizeof(unsigned long long), ctx->stream));
-  launch_flags_to_occupancy(flags->data, occ->data, n, ctx->counters + 1, ctx->stream);
+  TFL_CUDA(ctx, cudaMemsetAsync(ctx->counters.get() + 1, 0, sizeof(unsigned long long), ctx->stream));
+  launch_flags_to_occupancy(flags->data, occ->data, n, ctx->counters.get() + 1, ctx->stream);
   ctx->launches += 1;
   if (check_launch(ctx, "flagsToOccupancy")) return 1;
   if (bad) {
     unsigned long long v = 0;
-    TFL_CUDA(ctx, cudaMemcpyAsync(&v, ctx->counters + 1, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
+    TFL_CUDA(ctx, cudaMemcpyAsync(&v, ctx->counters.get() + 1, sizeof(v), cudaMemcpyDeviceToHost, ctx->stream));
     TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
     *bad = (int64_t)v;
   }
@@ -572,10 +551,10 @@ int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_gr
     ctx->launches += 1;
     const bool last = (iter + 1 >= max_iter);
     if (need_every || (last && residual)) {
-      TFL_CUDA(ctx, cudaMemsetAsync(ctx->dscratch, 0, sizeof(double) * g.nb, st));
-      launch_sqdiff(p->data, p_prev, g.n, g.nb, ctx->dscratch, st);
+      TFL_CUDA(ctx, cudaMemsetAsync(ctx->dscratch.get(), 0, sizeof(double) * g.nb, st));
+      launch_sqdiff(p->data, p_prev, g.n, g.nb, ctx->dscratch.get(), st);
       ctx->launches += 1;
-      TFL_CUDA(ctx, cudaMemcpyAsync(h.data(), ctx->dscratch, sizeof(double) * g.nb, cudaMemcpyDeviceToHost, st));
+      TFL_CUDA(ctx, cudaMemcpyAsync(h.data(), ctx->dscratch.get(), sizeof(double) * g.nb, cudaMemcpyDeviceToHost, st));
       TFL_CUDA(ctx, cudaStreamSynchronize(st));
       double worst = 0.0;
       for (int b = 0; b < g.nb; b++) { const double nr = sqrt(h[b]); if (nr > worst) worst = nr; }
@@ -627,7 +606,7 @@ int tfl_solve_linear_system_pcg(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid*
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (pcg_check_args(ctx, p, "p", flags, div, "div", is_3d, precond)) return 1;
-  const int rc = pcg_solve(ctx->pcg, ctx->arena, p->data, flags->data, div->data, flags->nb, flags->nz, flags->ny,
+  const int rc = pcg_solve(ctx->pcg, ctx->arena.get(), p->data, flags->data, div->data, flags->nb, flags->nz, flags->ny,
                            flags->nx, is_3d, precond, tol, max_iter, residual, iterations, &ctx->launches,
                            ctx->stream);
   return pcg_report(ctx, rc, "solveLinearSystemPCG");
@@ -642,7 +621,7 @@ int tfl_normalize_pressure_mean(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid*
   if (ctx->slab) return fail(ctx, "normalizePressureMean: single GPU only (connected components span the slabs)");
   if ((long long)flags->nb * flags->nz * flags->ny * flags->nx >= (1ll << 31)) return fail(ctx, "grid too large");
   if (arena_reserve(ctx, pcg_workspace_bytes(flags->nb, flags->nz, flags->ny, flags->nx))) return 1;
-  if (normalize_pressure_mean(ctx->arena, p->data, flags->data, flags->nb, flags->nz, flags->ny, flags->nx, is_3d,
+  if (normalize_pressure_mean(ctx->arena.get(), p->data, flags->data, flags->nb, flags->nz, flags->ny, flags->nx, is_3d,
                               &ctx->launches, ctx->stream))
     return fail(ctx, "normalizePressureMean: %s", cudaGetErrorString(cudaGetLastError()));
   return check_launch(ctx, "normalizePressureMean");
@@ -762,7 +741,7 @@ extern "C" int tfl_debug_pcg_precond(tfl_ctx* ctx, const tfl_grid* z, const tfl_
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (pcg_check_args(ctx, z, "z", flags, r, "r", is_3d, precond)) return 1;
-  const int rc = pcg_precond(ctx->pcg, ctx->arena, z->data, flags->data, r->data, flags->nb, flags->nz, flags->ny,
+  const int rc = pcg_precond(ctx->pcg, ctx->arena.get(), z->data, flags->data, r->data, flags->nb, flags->nz, flags->ny,
                              flags->nx, is_3d, precond, geometry, &ctx->launches, ctx->stream);
   return pcg_report(ctx, rc, "pcg precond");
 }
@@ -816,15 +795,20 @@ int tfl_debug_time_advect_kernel(tfl_ctx* ctx, int on) {
   if (!ctx) return 1;
   DeviceGuard guard_(ctx);
   auto& tl = ctx->tile;
-  if (on && !tl.ev0) { cudaEventCreate(&tl.ev0); cudaEventCreate(&tl.ev1); }
+  if (on && !(tl.ev0 && tl.ev1)) {
+    tl.ev0 = new_event(cudaEventDefault);
+    tl.ev1 = new_event(cudaEventDefault);
+    if (!tl.ev0 || !tl.ev1) cudaGetLastError();     // untimed: the getter reports -1, nothing else fails
+  }
   tl.timed = on != 0 && tl.ev0 && tl.ev1;
   return 0;
 }
 float tfl_debug_last_advect_kernel_ms(tfl_ctx* ctx) {
-  if (!ctx || !ctx->tile.ev0) return -1.0f;
+  if (!ctx || !ctx->tile.ev0 || !ctx->tile.ev1) return -1.0f;
   DeviceGuard guard_(ctx);
   float ms = -1.0f;
-  if (cudaEventSynchronize(ctx->tile.ev1) != cudaSuccess || cudaEventElapsedTime(&ms, ctx->tile.ev0, ctx->tile.ev1) != cudaSuccess) {
+  cudaEvent_t e0 = ctx->tile.ev0.get(), e1 = ctx->tile.ev1.get();
+  if (cudaEventSynchronize(e1) != cudaSuccess || cudaEventElapsedTime(&ms, e0, e1) != cudaSuccess) {
     cudaGetLastError();
     return -1.0f;
   }
@@ -870,7 +854,7 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
   unsigned char *fl8 = nullptr, *clear = nullptr;
   if (prepare_flags(ctx, s->flags.data, g, &fl8, &clear)) return 1;
   const bool ov = ctx->ov.active;
-  if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_u_in, 0));          // U has arrived from the host
+  if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_u_in.get(), 0));          // U has arrived from the host
   // Which quads of the BC arrays are the identity pair (the point-wise stages then skip their loads): rebuilt
   // every step from the arrays, beside the advection (on the side stream when there is one).
   const unsigned char* qmask = nullptr;
@@ -880,21 +864,21 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
   if (has_density) {
     // Density and velocity advection are independent (both read the old U): run the density
     // kernels on a side stream so the two latency-bound kernel pairs overlap.
-    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_fork, st));
-    TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->side_stream, ctx->ev_fork, 0));
+    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_fork.get(), st));
+    TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->side_stream.get(), ctx->ev_fork.get(), 0));
     if (launch_bc_quad_mask(u_bc0 ? s->U_bc_inv_mask.data : nullptr, u_bc0 ? s->U_bc.data : nullptr,
                             d_bc0 ? s->density_bc_inv_mask.data : nullptr, d_bc0 ? s->density_bc.data : nullptr,
-                            qmask_buf, g, ctx->side_stream)) {
+                            qmask_buf, g, ctx->side_stream.get())) {
       qmask = qmask_buf;
       qmask_on_side = true;
       ctx->launches += 1;
     }
-    if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->side_stream, ctx->ev_d_in, 0));
+    if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->side_stream.get(), ctx->ev_d_in.get(), 0));
     const int nl = advect_scalar_dispatch(ctx, mc->dt, s->density.data, s->U.data, fl8, fl8, clear, mc->advection_method,
-                                          0, mc->maccormack_strength, tmp_s, fwd_s, fwd_pos, g, g, ctx->side_stream);
+                                          0, mc->maccormack_strength, tmp_s, fwd_s, fwd_pos, g, g, ctx->side_stream.get());
     if (nl < 0) return fail(ctx, "advectScalar: bad method");
     ctx->launches += nl;
-    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_join, ctx->side_stream));
+    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_join.get(), ctx->side_stream.get()));
   }
   {
     const int nl = advect_vel_dispatch(ctx, mc->dt, s->U.data, fl8, fl8, clear, mc->advection_method,
@@ -902,7 +886,7 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
     if (nl < 0) return fail(ctx, "advectVel: bad method");
     ctx->launches += nl;
   }
-  if (has_density) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_join, 0));
+  if (has_density) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_join.get(), 0));
   if (!qmask_on_side && launch_bc_quad_mask(u_bc0 ? s->U_bc_inv_mask.data : nullptr, u_bc0 ? s->U_bc.data : nullptr, nullptr,
                                             nullptr, qmask_buf, g, st)) {
     qmask = qmask_buf;
@@ -924,11 +908,11 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
   if (ov && has_density && ctx->ov.density_host) {
     // The density is final here (nothing later in the step writes it): send it home while the
     // vorticity / projection kernels run.
-    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_d_ready, st));
-    TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_out, ctx->ev_d_ready, 0));
+    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_d_ready.get(), st));
+    TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_out.get(), ctx->ev_d_ready.get(), 0));
     TFL_CUDA(ctx, cudaMemcpyAsync(ctx->ov.density_host, s->density.data, ctx->ov.density_bytes, cudaMemcpyDeviceToHost,
-                                  ctx->copy_out));
-    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_d_out, ctx->copy_out));
+                                  ctx->copy_out.get()));
+    TFL_CUDA(ctx, cudaEventRecord(ctx->ev_d_out.get(), ctx->copy_out.get()));
     ctx->ov.density_sent = true;
   }
   if (fo.gravity) {
@@ -940,12 +924,12 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
     launch_vort_curl(s->U.data, curl, cnorm, force, fo.vort_amp, g, st);
     ctx->launches += 2;
   }
-  double* sums = ctx->dscratch + 64;
+  double* sums = ctx->dscratch.get() + 64;
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
   launch_vort_bc_mask(s->U.data, fl8, force, fo.vorticity, u_bc ? s->U_bc_inv_mask.data : nullptr,
                       u_bc ? s->U_bc.data : nullptr, qmask, 1, sums, g, st);
   const ConvTcGeo& tg = m->act_geo;
-  if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in, 0));          // pDiv is first read here
+  if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in.get(), 0));          // pDiv is first read here
   launch_cnn_inputs_fused(s->p.data, s->U.data, fl8, sums, mc->normalize_input_threshold, scale, m->act[0].get(),
                           tg.px, tg.py, g, st);
   run_conv_stack(m, p_net, st);
@@ -1021,8 +1005,8 @@ int tfl_simulate_step(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, tfl
 // Host-buffer driver for the same step.
 // ---------------------------------------------------------------------------------------
 struct tfl_host_sim {
-  tfl_state st;
-  std::vector<void*> owned;
+  tfl_state st;                     // views of the buffers below
+  DevPtr<float> flags, p, U, density, div, U_bc, U_bc_inv, d_bc, d_bc_inv;
   size_t cells = 0;
   int nc = 3;
 };
@@ -1033,39 +1017,35 @@ int tfl_host_sim_create(tfl_ctx* ctx, int32_t nb, int32_t nz, int32_t ny, int32_
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!out || !flags) return fail(ctx, "host_sim: bad arguments");
-  tfl_host_sim* hs = new tfl_host_sim();
+  *out = nullptr;
+  if (nb < 1 || nz < 1 || ny < 1 || nx < 1) return fail(ctx, "host_sim: every grid extent must be >= 1");
+  if (!is_3d && nz != 1) return fail(ctx, "host_sim: 2D grid must have zsize == 1");
+  if (grid_too_large((long long)nz * ny * nx, nb)) return fail(ctx, "host_sim: grid too large");
+  std::unique_ptr<tfl_host_sim> hs(new tfl_host_sim());
   memset(&hs->st, 0, sizeof(hs->st));
   hs->nc = is_3d ? 3 : 2;
   hs->cells = (size_t)nb * nz * ny * nx;
-  auto mk = [&](tfl_grid* g, int nc, const float* host) -> int {
-    g->nb = nb; g->nc = nc; g->nz = nz; g->ny = ny; g->nx = nx;
-    void* p = nullptr;
-    if (cudaMalloc(&p, hs->cells * nc * 4) != cudaSuccess) return 1;
-    hs->owned.push_back(p);
-    g->data = (float*)p;
-    if (host) cudaMemcpy(p, host, hs->cells * nc * 4, cudaMemcpyHostToDevice);
-    else cudaMemset(p, 0, hs->cells * nc * 4);
-    return 0;
+  // d <- a device copy of host (zeros without one) of nc channels; g views it
+  auto mk = [&](DevPtr<float>& d, tfl_grid* g, int nc, const float* host) {
+    d = host ? upload(host, hs->cells * nc) : dev_zeros<float>(hs->cells * nc);
+    *g = {d.get(), nb, nc, nz, ny, nx};
+    return d != nullptr;
   };
-  int bad = 0;
-  bad |= mk(&hs->st.flags, 1, flags);
-  bad |= mk(&hs->st.p, 1, nullptr);
-  bad |= mk(&hs->st.U, hs->nc, nullptr);
-  bad |= mk(&hs->st.density, 1, nullptr);
-  bad |= mk(&hs->st.div, 1, nullptr);
-  if (U_bc && U_bc_inv) { bad |= mk(&hs->st.U_bc, hs->nc, U_bc); bad |= mk(&hs->st.U_bc_inv_mask, hs->nc, U_bc_inv); }
-  if (d_bc && d_bc_inv) { bad |= mk(&hs->st.density_bc, 1, d_bc); bad |= mk(&hs->st.density_bc_inv_mask, 1, d_bc_inv); }
-  if (bad) { tfl_host_sim_destroy(ctx, hs); return fail(ctx, "host_sim: cudaMalloc failed"); }
-  *out = hs;
+  tfl_state& st = hs->st;
+  const int nc = hs->nc;
+  if (!mk(hs->flags, &st.flags, 1, flags) || !mk(hs->p, &st.p, 1, nullptr) || !mk(hs->U, &st.U, nc, nullptr) ||
+      !mk(hs->density, &st.density, 1, nullptr) || !mk(hs->div, &st.div, 1, nullptr) ||
+      (U_bc && U_bc_inv && (!mk(hs->U_bc, &st.U_bc, nc, U_bc) || !mk(hs->U_bc_inv, &st.U_bc_inv_mask, nc, U_bc_inv))) ||
+      (d_bc && d_bc_inv && (!mk(hs->d_bc, &st.density_bc, 1, d_bc) || !mk(hs->d_bc_inv, &st.density_bc_inv_mask, 1, d_bc_inv))))
+    return fail(ctx, "host_sim: cudaMalloc failed");
+  *out = hs.release();
   return 0;
 }
 
 void tfl_host_sim_destroy(tfl_ctx* ctx, tfl_host_sim* hs) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
-  if (!hs) return;
-  if (ctx) cudaStreamSynchronize(ctx->stream);
-  for (void* p : hs->owned) cudaFree(p);
+  if (hs && ctx) cudaStreamSynchronize(ctx->stream);
   delete hs;
 }
 
@@ -1079,31 +1059,31 @@ int tfl_host_sim_step(tfl_ctx* ctx, tfl_host_sim* hs, float* p, float* U, float*
   if (!density) s.density.data = nullptr;
   // Inputs in the order the step reads them: U (both advections), density (density advection), pDiv
   // (network input, much later).  One copy stream keeps them in that order on the PCIe link.
-  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_fork, st));                      // earlier work on the step stream
-  TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_in, ctx->ev_fork, 0));
-  TFL_CUDA(ctx, cudaMemcpyAsync(s.U.data, U, hs->cells * 4 * hs->nc, cudaMemcpyHostToDevice, ctx->copy_in));
-  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_u_in, ctx->copy_in));
-  if (density) TFL_CUDA(ctx, cudaMemcpyAsync(s.density.data, density, hs->cells * 4, cudaMemcpyHostToDevice, ctx->copy_in));
-  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_d_in, ctx->copy_in));
-  TFL_CUDA(ctx, cudaMemcpyAsync(s.p.data, p, hs->cells * 4, cudaMemcpyHostToDevice, ctx->copy_in));
-  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_p_in, ctx->copy_in));
+  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_fork.get(), st));                      // earlier work on the step stream
+  TFL_CUDA(ctx, cudaStreamWaitEvent(ctx->copy_in.get(), ctx->ev_fork.get(), 0));
+  TFL_CUDA(ctx, cudaMemcpyAsync(s.U.data, U, hs->cells * 4 * hs->nc, cudaMemcpyHostToDevice, ctx->copy_in.get()));
+  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_u_in.get(), ctx->copy_in.get()));
+  if (density) TFL_CUDA(ctx, cudaMemcpyAsync(s.density.data, density, hs->cells * 4, cudaMemcpyHostToDevice, ctx->copy_in.get()));
+  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_d_in.get(), ctx->copy_in.get()));
+  TFL_CUDA(ctx, cudaMemcpyAsync(s.p.data, p, hs->cells * 4, cudaMemcpyHostToDevice, ctx->copy_in.get()));
+  TFL_CUDA(ctx, cudaEventRecord(ctx->ev_p_in.get(), ctx->copy_in.get()));
   const bool fused = fused_step_applies(ctx, &s, mc, cnn);
   ctx->ov.active = fused;
   ctx->ov.density_host = density;
   ctx->ov.density_bytes = hs->cells * 4;
   ctx->ov.density_sent = false;
   if (!fused) {                                                           // operator-by-operator path: no overlap
-    TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in, 0));
+    TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in.get(), 0));
   }
   const int rc = tfl_simulate_step(ctx, &s, mc, cnn);
   const bool density_sent = ctx->ov.density_sent;
   ctx->ov.active = false;
-  if (rc) { cudaStreamSynchronize(ctx->copy_in); cudaStreamSynchronize(ctx->copy_out); return 1; }
+  if (rc) { cudaStreamSynchronize(ctx->copy_in.get()); cudaStreamSynchronize(ctx->copy_out.get()); return 1; }
   TFL_CUDA(ctx, cudaMemcpyAsync(U, s.U.data, hs->cells * 4 * hs->nc, cudaMemcpyDeviceToHost, st));
   TFL_CUDA(ctx, cudaMemcpyAsync(p, s.p.data, hs->cells * 4, cudaMemcpyDeviceToHost, st));
   if (density && !density_sent)
     TFL_CUDA(ctx, cudaMemcpyAsync(density, s.density.data, hs->cells * 4, cudaMemcpyDeviceToHost, st));
-  if (density_sent) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_d_out, 0));
+  if (density_sent) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_d_out.get(), 0));
   TFL_CUDA(ctx, cudaStreamSynchronize(st));
   return 0;
 }
@@ -1120,8 +1100,8 @@ int tfl_host_sim_step(tfl_ctx* ctx, tfl_host_sim* hs, float* p, float* U, float*
 // is refused (the replay would read and write freed memory).
 // ---------------------------------------------------------------------------------------
 struct tfl_step_graph {
-  cudaGraph_t graph = nullptr;
-  cudaGraphExec_t exec = nullptr;
+  GraphPtr graph;
+  GraphExecPtr exec;
   long long launches = 0;       // kernels in one replay
   unsigned long long arena_gen = 0, fcache_gen = 0, act_gen = 0;   // generations of the captured buffers
   tfl_cnn* cnn = nullptr;       // the captured model (its act_gen is checked), or null
@@ -1131,10 +1111,7 @@ extern "C" {
 
 void tfl_step_graph_destroy(tfl_ctx* ctx, tfl_step_graph* g) {
   DeviceGuard guard_(ctx);
-  if (!g) return;
-  if (ctx) cudaStreamSynchronize(ctx->stream);
-  if (g->exec) cudaGraphExecDestroy(g->exec);
-  if (g->graph) cudaGraphDestroy(g->graph);
+  if (g && ctx) cudaStreamSynchronize(ctx->stream);
   delete g;
 }
 
@@ -1155,26 +1132,28 @@ int tfl_step_graph_create(tfl_ctx* ctx, const tfl_state* state, const tfl_mconf*
     return fail(ctx, "step_graph: cudaStreamBeginCapture failed");
   }
   const int rc = tfl_simulate_step(ctx, state, mc, cnn);
-  tfl_step_graph* g = new tfl_step_graph();
-  const cudaError_t e = cudaStreamEndCapture(st, &g->graph);
-  if (rc != 0 || e != cudaSuccess || !g->graph) {
+  std::unique_ptr<tfl_step_graph> g(new tfl_step_graph());
+  cudaGraph_t graph = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(st, &graph);
+  g->graph.reset(graph);
+  if (rc != 0 || e != cudaSuccess || !graph) {
     cudaGetLastError();
     const std::string why = rc != 0 ? ctx->err : std::string(cudaGetErrorString(e));
-    tfl_step_graph_destroy(ctx, g);
     return fail(ctx, "step_graph: capture failed (%s); run tfl_simulate_step once before capturing", why.c_str());
   }
   g->launches = ctx->launches - l0;
   ctx->launches = l0;
-  if (cudaGraphInstantiate(&g->exec, g->graph, 0) != cudaSuccess) {
+  cudaGraphExec_t exec = nullptr;
+  if (cudaGraphInstantiate(&exec, graph, 0) != cudaSuccess) {
     cudaGetLastError();
-    tfl_step_graph_destroy(ctx, g);
     return fail(ctx, "step_graph: cudaGraphInstantiate failed");
   }
+  g->exec.reset(exec);
   g->arena_gen = ctx->arena_gen;
   g->fcache_gen = ctx->fcache.gen;
   g->cnn = cnn;
   g->act_gen = cnn ? cnn->act_gen : 0;
-  *out = g;
+  *out = g.release();
   return 0;
 }
 
@@ -1189,7 +1168,7 @@ int tfl_step_graph_launch(tfl_ctx* ctx, tfl_step_graph* g) {
   if (stale)
     return fail(ctx, "step_graph: stale graph: %s reallocated since the capture (a call on another grid shape or a "
                      "larger grid); replaying would touch freed memory: capture the step again", stale);
-  TFL_CUDA(ctx, cudaGraphLaunch(g->exec, ctx->stream));
+  TFL_CUDA(ctx, cudaGraphLaunch(g->exec.get(), ctx->stream));
   ctx->launches += g->launches;
   return 0;
 }

@@ -23,29 +23,6 @@ constexpr int kTailFloats = 64 + 8 + 8 + 1;     // the fused 1x1x1 tail: w4[8][8
 
 namespace {
 
-// n device values, uninitialised; empty if cudaMalloc fails.
-template <typename T>
-DevPtr<T> dev_alloc(size_t n) {
-  T* p = nullptr;
-  if (cudaMalloc((void**)&p, n * sizeof(T)) != cudaSuccess) return DevPtr<T>();
-  return DevPtr<T>(p);
-}
-// n device values set to zero; empty if cudaMalloc or cudaMemset fails.
-template <typename T>
-DevPtr<T> dev_zeros(size_t n) {
-  DevPtr<T> d = dev_alloc<T>(n);
-  if (d && cudaMemset(d.get(), 0, n * sizeof(T)) != cudaSuccess) d.reset();
-  return d;
-}
-// A device copy of host[0, n); empty if cudaMalloc or cudaMemcpy fails.
-template <typename T>
-DevPtr<T> upload(const T* host, size_t n) {
-  DevPtr<T> d = dev_alloc<T>(n);
-  if (d && cudaMemcpy(d.get(), host, n * sizeof(T), cudaMemcpyHostToDevice) != cudaSuccess) d.reset();
-  return d;
-}
-template <typename T>
-DevPtr<T> upload(const std::vector<T>& host) { return upload(host.data(), host.size()); }
 // Appends p to v; false (and v unchanged) if p is empty, its upload having failed.
 bool keep(std::vector<DevPtr<float>>& v, DevPtr<float> p) {
   if (!p) return false;
@@ -151,7 +128,7 @@ Geo whole_grid(tfl_ctx* ctx, int nb, int nz, int ny, int nx, int is3d) {
   g.is3d = is3d ? 1 : 0;
   g.nc = is3d ? 3 : 2;
   g.n = (long long)nx * ny * nz;
-  g.faults = ctx->counters;
+  g.faults = ctx->counters.get();
   return g;
 }
 bool bad_grid(int nb, int nz, int ny, int nx, int is3d) {
@@ -1138,7 +1115,7 @@ static int cnn_project_impl(tfl_ctx* ctx, tfl_cnn* m, const float* p_div, const 
   float *U1 = scr.U1, *x0 = scr.x0, *actA = scr.actA, *actB = scr.actB, *scale = scr.scale;
   double* bn_part = scr.bn_part;
   float* bn_ac = scr.bn_ac;
-  double* sums = ctx->dscratch + 64;
+  double* sums = ctx->dscratch.get() + 64;
   cudaStream_t st = ctx->stream;
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
   launch_cnn_mask_stats(U_div, flags, U1, sums, g.zlo, g.zhi, g, st, m->norm_chan, p_div);
@@ -1360,7 +1337,7 @@ int tfl_cnn_project(tfl_ctx* ctx, tfl_cnn* m, const tfl_grid* p_div, const tfl_g
   if (arena_reserve(ctx, cnn_scratch(m, g, nullptr).bytes)) return 1;
   float* scale_dev = nullptr;
   if (cnn_project_impl(ctx, m, p_div->data, U_div->data, flags->data, p_out->data, U_out->data, threshold, g,
-                       cnn_scratch(m, g, ctx->arena), &scale_dev))
+                       cnn_scratch(m, g, ctx->arena.get()), &scale_dev))
     return 1;
   if (scale_out) {
     TFL_CUDA(ctx, cudaMemcpyAsync(scale_out, scale_dev, sizeof(float) * g.nb, cudaMemcpyDeviceToHost, ctx->stream));

@@ -16,39 +16,32 @@
 
 using namespace tfl;
 
-// Device memory held by std::unique_ptr: cudaFree runs when the holder goes.
-struct CudaFree {
-  void operator()(void* p) const { cudaFree(p); }
-};
-template <typename T>
-using DevPtr = std::unique_ptr<T, CudaFree>;
-
 constexpr char kConvZStalled[] =
     "internal error, the z-streaming tensor-core convolution's pipeline stalled (a bounded wait ran out)";
 
 struct tfl_ctx {
   int device = 0;
-  cudaStream_t stream = nullptr;
-  bool own_stream = true;
+  cudaStream_t stream = nullptr;            // where work is enqueued: own_stream, or a stream the caller adopted
+  StreamPtr own_stream;                     // the stream the context made (empty while an adopted one is current)
   std::string err;
-  char* arena = nullptr;
+  DevPtr<char> arena;
   size_t arena_bytes = 0;
   size_t arena_used = 0;
   // Generation counters of the buffers a step graph captures: bumped whenever the buffer is freed and allocated
   // again, so that tfl_step_graph_launch can refuse a graph that would replay freed memory.
   unsigned long long arena_gen = 0;
-  unsigned long long* counters = nullptr;   // [0] trace faults, [1] bad occupancy cells
-  double* dscratch = nullptr;               // small double scratch (reductions), 256 entries
+  DevPtr<unsigned long long> counters;      // [0] trace faults, [1] bad occupancy cells
+  DevPtr<double> dscratch;                  // small double scratch (reductions), 256 entries
   long long launches = 0;
   bool slab = false;
   int zoff = 0, gnz = 0, zlo = 0, zhi = 0;
   int slab_margin = 2;                      // extra planes on which forward passes are evaluated
-  cudaStream_t side_stream = nullptr;       // density advection runs beside velocity advection
-  cudaEvent_t ev_fork = nullptr, ev_join = nullptr;
+  StreamPtr side_stream;                    // density advection runs beside velocity advection
+  EventPtr ev_fork, ev_join;
   // Host-buffer step (tfl_host_sim_step): copies run on their own streams and the step waits for each
   // input only where it is first read / hands each output over as soon as it is final.
-  cudaStream_t copy_in = nullptr, copy_out = nullptr;
-  cudaEvent_t ev_u_in = nullptr, ev_d_in = nullptr, ev_p_in = nullptr, ev_d_ready = nullptr, ev_d_out = nullptr;
+  StreamPtr copy_in, copy_out;
+  EventPtr ev_u_in, ev_d_in, ev_p_in, ev_d_ready, ev_d_out;
   struct {
     bool active = false;
     float* density_host = nullptr;          // where the advected density goes once it is final
@@ -60,10 +53,10 @@ struct tfl_ctx {
   // each step re-derives the bytes, compares them with the copy on the device and rebuilds the
   // clearance only if something changed (no host round trip).
   struct {
-    unsigned char* bytes = nullptr;         // [3][cells]: flags, clearance, scratch
+    DevPtr<unsigned char> bytes;            // [3][cells]: flags, clearance, scratch
     size_t cells = 0;
     int nb = 0, nz = 0, ny = 0, nx = 0;
-    int* changed = nullptr;                 // device word
+    DevPtr<int> changed;                    // device word
     const float* fresh_for = nullptr;       // set inside a slab step: the cache already mirrors these flags
     unsigned long long gen = 0;             // bumped on every reallocation of `bytes` (see arena_gen)
   } fcache;
@@ -71,14 +64,14 @@ struct tfl_ctx {
   // into a device word that is copied, asynchronously, into a pinned host word; the NEXT calls pick the tile
   // halo from it (stale by a step or two -- it only selects a code path, never a result).
   struct {
-    unsigned int* dev = nullptr;
-    unsigned int* host = nullptr;           // pinned
+    DevPtr<unsigned int> dev;
+    PinnedPtr<unsigned int> host;
     int mode = -1;                          // -1 automatic, 0 two-kernel version, 1 / 2 forced halo
     int variant = 0;                        // tile shape (tuning)
     int calls_since_probe = 0;
     // bench.py's roofline: CUDA events right around the tile kernel's launch (off unless asked for)
     bool timed = false;
-    cudaEvent_t ev0 = nullptr, ev1 = nullptr;
+    EventPtr ev0, ev1;
   } tile;
   // z-slab decomposition over several GPUs (tfl_comm_init / tfl_slab_sim_*): the communicator lives here
   ncclComm_t comm = nullptr;
@@ -195,13 +188,12 @@ inline int check_launch(tfl_ctx* ctx, const char* what) {
 inline int arena_reserve(tfl_ctx* ctx, size_t bytes) {
   if (bytes <= ctx->arena_bytes) return 0;
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-  if (ctx->arena) cudaFree(ctx->arena);
-  ctx->arena = nullptr;
+  ctx->arena.reset();                       // before the larger one is allocated
   ctx->arena_bytes = 0;
   ctx->arena_gen++;
   void* p = nullptr;
   TFL_CUDA(ctx, cudaMalloc(&p, bytes));
-  ctx->arena = (char*)p;
+  ctx->arena.reset((char*)p);
   ctx->arena_bytes = bytes;
   return 0;
 }
@@ -213,7 +205,7 @@ struct Carver {
   T* take(size_t count) {
     const size_t a = (off + 255) & ~(size_t)255;
     off = a + count * sizeof(T);
-    return (T*)(ctx->arena + a);
+    return (T*)(ctx->arena.get() + a);
   }
 };
 inline size_t carve_bytes(std::initializer_list<size_t> sizes) {
@@ -241,12 +233,16 @@ inline int check_vel(tfl_ctx* ctx, const tfl_grid* U, const tfl_grid* flags) {
   return 0;
 }
 
+// cell() (tfl_device.cuh) indexes one (batch, channel) block of n cells in 32 bits; the second bound keeps the whole
+// velocity field within 2^33 cells.
+inline bool grid_too_large(long long n, int nb) { return n >= (1LL << 31) || n * (long long)nb * 3 >= (1LL << 31) * 4; }
+
 inline int make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is3d, Geo* g) {
   g->nx = flags->nx; g->ny = flags->ny; g->nz = flags->nz; g->nb = flags->nb;
   g->is3d = is3d ? 1 : 0;
   g->nc = is3d ? 3 : 2;
   g->n = (long long)flags->nx * flags->ny * flags->nz;
-  g->faults = ctx->counters;
+  g->faults = ctx->counters.get();
   if (ctx->slab) {
     if (!is3d) return fail(ctx, "slab decomposition needs a 3D grid");
     g->zoff = ctx->zoff; g->gnz = ctx->gnz; g->zlo = ctx->zlo; g->zhi = ctx->zhi;
@@ -256,9 +252,7 @@ inline int make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is3d, Geo* g) {
     g->zoff = 0; g->gnz = flags->nz; g->zlo = 0; g->zhi = flags->nz;
   }
   if (!is3d && flags->nz != 1) return fail(ctx, "2D grid must have zsize == 1");
-  // cell() (tfl_device.cuh) indexes one (batch, channel) block in 32 bits; the second bound keeps the whole
-  // velocity field within 2^33 cells.
-  if (g->n >= (1LL << 31) || g->n * (long long)g->nb * 3 >= (1LL << 31) * 4) return fail(ctx, "grid too large");
+  if (grid_too_large(g->n, g->nb)) return fail(ctx, "grid too large");
   return 0;
 }
 

@@ -75,34 +75,35 @@ struct tfl_slab_sim {
   int rank = 0, world = 1;
   int z0 = 0, z1 = 0, lo_halo = 0, hi_halo = 0, zoff = 0, nz = 0, own_lo = 0, own_hi = 0;
   size_t cells = 0, plane = 0;      // local cells / cells per plane
-  tfl_state st;
-  float* U1 = nullptr;
-  double* sums = nullptr;
-  float* xbuf = nullptr;            // [send down | send up | recv from below | recv from above], xbuf_side floats each
+  tfl_state st;                     // views of the field buffers below
+  DevPtr<float> flags, p, U, density, U_bc, U_bc_inv, d_bc, d_bc_inv;
+  DevPtr<float> U1;
+  DevPtr<double> sums;
+  DevPtr<float> xbuf;               // [send down | send up | recv from below | recv from above], xbuf_side floats each
   size_t xbuf_side = 0;
   // Peer-memory halo exchange (CUDA IPC over NVLink, tfl_slab_sim_ipc_*): this rank's inbox -- per phase and side a
   // receive buffer of xbuf_side floats that the neighbour's push kernel fills with remote stores, and a step counter
   // it raises afterwards -- and the neighbours' inboxes mapped into this process.
-  float* inbox = nullptr;           // cudaMalloc'ed, exported: [3 phases][2 sides][xbuf_side] floats, then 64 counters
-  float* peer_inbox[2] = {nullptr, nullptr};   // lower / upper neighbour's inbox (cudaIpcOpenMemHandle)
+  DevPtr<float> inbox;              // exported: [3 phases][2 sides][xbuf_side] floats, then 64 counters
+  std::vector<IpcPtr<float>> mapped;           // the other ranks' inboxes (cudaIpcOpenMemHandle), empty at [rank]
+  float* peer_inbox[2] = {nullptr, nullptr};   // lower / upper neighbour's inbox
   std::vector<float*> all_inbox;               // every rank's inbox (own pointer at [rank]): the all-reduce's targets
-  float** all_inbox_dev = nullptr;             // the same table on the device
-  unsigned int* push_done = nullptr;           // CTAs of the running push kernel that finished their stores
+  DevPtr<float*> all_inbox_dev;                // the same table on the device
+  DevPtr<unsigned int> push_done;              // CTAs of the running push kernel that finished their stores
   bool peer_ok = false;
   unsigned int step_no = 0;
-  std::vector<void*> owned;
-  cudaEvent_t ev[4][2] = {{nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}, {nullptr, nullptr}};
+  EventPtr ev[4][2];
   size_t bytes_sent[3] = {0, 0, 0};
   // Jacobi projection (simMethod 'jacobi'): divergence, second p buffer and mask of the local slab; the p exchanges
   // land in their own inbox area behind the all-reduce's -- [2 parities][2 sides][p_side] floats, then
   // [2 parities][2 sides] counters -- and carry the monotone sequence number jseq instead of step_no.
-  float* div = nullptr;
-  float* p2 = nullptr;
-  unsigned char* mask = nullptr;
+  DevPtr<float> div;
+  DevPtr<float> p2;
+  DevPtr<unsigned char> mask;
   size_t p_side = 0;                // halo planes of one channel
   unsigned int jseq = 0;
   std::vector<int32_t> jsched;
-  std::vector<cudaEvent_t> jev;     // [2 * exchange] begin / end of the last step's p exchanges
+  std::vector<EventPtr> jev;        // [2 * exchange] begin / end of the last step's p exchanges
   int jx = 0;                       // p exchanges of the last step
   size_t jbytes = 0;
 };
@@ -151,12 +152,7 @@ int tfl_comm_destroy(tfl_ctx* ctx) {
 void tfl_slab_sim_destroy(tfl_ctx* ctx, tfl_slab_sim* s) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
-  if (!s) return;
-  if (ctx) cudaStreamSynchronize(ctx->stream);
-  for (int r = 0; r < (int)s->all_inbox.size(); r++) if (r != s->rank && s->all_inbox[r]) cudaIpcCloseMemHandle(s->all_inbox[r]);
-  for (void* p : s->owned) cudaFree(p);
-  for (auto& pr : s->ev) for (cudaEvent_t e : pr) if (e) cudaEventDestroy(e);
-  for (cudaEvent_t e : s->jev) if (e) cudaEventDestroy(e);
+  if (s && ctx) cudaStreamSynchronize(ctx->stream);
   delete s;
 }
 
@@ -167,12 +163,12 @@ int tfl_slab_sim_create(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!out || !flags || gnz < 3 || ny < 3 || nx < 3 || margin < 2) return fail(ctx, "slab_sim: bad arguments (margin >= 2)");
-  tfl_slab_sim* s = new tfl_slab_sim();
+  std::unique_ptr<tfl_slab_sim> s(new tfl_slab_sim());
   memset(&s->st, 0, sizeof(s->st));
   s->gnz = gnz; s->ny = ny; s->nx = nx; s->margin = margin; s->halo = 2 * margin + 2;
   s->rank = ctx->comm_rank; s->world = ctx->comm_world;
   const int base = gnz / s->world, rem = gnz % s->world;
-  if (s->world > 1 && base < s->halo) { delete s; return fail(ctx, "slab_sim: slabs of %d planes are thinner than the halo (%d)", base, s->halo); }
+  if (s->world > 1 && base < s->halo) return fail(ctx, "slab_sim: slabs of %d planes are thinner than the halo (%d)", base, s->halo);
   s->z0 = s->rank * base + std::min(s->rank, rem);
   s->z1 = s->z0 + base + (s->rank < rem ? 1 : 0);
   s->lo_halo = std::min(s->halo, s->z0);
@@ -184,51 +180,37 @@ int tfl_slab_sim_create(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32
   s->plane = (size_t)ny * nx;
   s->cells = s->plane * s->nz;
   const size_t gcells = s->plane * gnz;
-  auto mk = [&](tfl_grid* g, int nc, const float* host) -> int {
-    g->nb = 1; g->nc = nc; g->nz = s->nz; g->ny = ny; g->nx = nx;
-    void* p = nullptr;
-    if (cudaMalloc(&p, s->cells * nc * 4) != cudaSuccess) return 1;
-    s->owned.push_back(p);
-    g->data = (float*)p;
-    if (!host) return cudaMemset(p, 0, s->cells * nc * 4) != cudaSuccess;
-    for (int c = 0; c < nc; c++)
-      if (cudaMemcpy((float*)p + c * s->cells, host + c * gcells + (size_t)s->zoff * s->plane, s->cells * 4,
-                     cudaMemcpyHostToDevice) != cudaSuccess)
-        return 1;
-    return 0;
-  };
-  int bad = 0;
-  bad |= mk(&s->st.flags, 1, flags);
-  bad |= mk(&s->st.p, 1, nullptr);
-  bad |= mk(&s->st.U, 3, nullptr);
-  bad |= mk(&s->st.density, 1, nullptr);
-  if (U_bc && U_bc_inv) { bad |= mk(&s->st.U_bc, 3, U_bc); bad |= mk(&s->st.U_bc_inv_mask, 3, U_bc_inv); }
-  if (d_bc && d_bc_inv) { bad |= mk(&s->st.density_bc, 1, d_bc); bad |= mk(&s->st.density_bc_inv_mask, 1, d_bc_inv); }
-  void* p = nullptr;
-  bad |= cudaMalloc(&p, s->cells * 3 * 4) != cudaSuccess;
-  if (!bad) { s->owned.push_back(p); s->U1 = (float*)p; }
-  bad |= cudaMalloc(&p, 2 * sizeof(double)) != cudaSuccess;
-  if (!bad) { s->owned.push_back(p); s->sums = (double*)p; }
   s->xbuf_side = (size_t)s->halo * s->plane * 4;          // the widest exchange: halo planes of 4 channels
-  bad |= cudaMalloc(&p, 4 * s->xbuf_side * sizeof(float)) != cudaSuccess;
-  if (!bad) { s->owned.push_back(p); s->xbuf = (float*)p; }
-  bad |= cudaMalloc(&p, s->cells * 4) != cudaSuccess;
-  if (!bad) { s->owned.push_back(p); s->div = (float*)p; }
-  bad |= cudaMalloc(&p, s->cells * 4) != cudaSuccess;
-  if (!bad) { s->owned.push_back(p); s->p2 = (float*)p; }
-  bad |= cudaMalloc(&p, s->cells) != cudaSuccess;
-  if (!bad) { s->owned.push_back(p); s->mask = (unsigned char*)p; }
   s->p_side = (size_t)s->halo * s->plane;
-  if (s->world > 1) {
-    const size_t inbox_bytes = (6 * s->xbuf_side + 64 + kSumAreaFloats + 4 * s->p_side + 64) * sizeof(float);
-    bad |= cudaMalloc(&p, inbox_bytes) != cudaSuccess;
-    if (!bad) { s->owned.push_back(p); s->inbox = (float*)p; bad |= cudaMemset(p, 0, inbox_bytes) != cudaSuccess; }
-    bad |= cudaMalloc(&p, sizeof(unsigned int)) != cudaSuccess;
-    if (!bad) { s->owned.push_back(p); s->push_done = (unsigned int*)p; bad |= cudaMemset(p, 0, sizeof(unsigned int)) != cudaSuccess; }
-  }
-  for (auto& pr : s->ev) for (cudaEvent_t& e : pr) bad |= cudaEventCreate(&e) != cudaSuccess;
-  if (bad) { tfl_slab_sim_destroy(ctx, s); return fail(ctx, "slab_sim: allocation failed"); }
-  *out = s;
+  // d <- this rank's planes of the GLOBAL host field (zeros without one) of nc channels; g views it
+  auto mk = [&](DevPtr<float>& d, tfl_grid* g, int nc, const float* host) {
+    d = host ? dev_alloc<float>(s->cells * nc) : dev_zeros<float>(s->cells * nc);
+    for (int c = 0; host && d && c < nc; c++)
+      if (cudaMemcpy(d.get() + c * s->cells, host + c * gcells + (size_t)s->zoff * s->plane, s->cells * 4,
+                     cudaMemcpyHostToDevice) != cudaSuccess)
+        d.reset();
+    *g = {d.get(), 1, nc, s->nz, ny, nx};
+    return d != nullptr;
+  };
+  tfl_state& st = s->st;
+  constexpr char kFailed[] = "slab_sim: allocation failed";
+  if (!mk(s->flags, &st.flags, 1, flags) || !mk(s->p, &st.p, 1, nullptr) || !mk(s->U, &st.U, 3, nullptr) ||
+      !mk(s->density, &st.density, 1, nullptr) ||
+      (U_bc && U_bc_inv && (!mk(s->U_bc, &st.U_bc, 3, U_bc) || !mk(s->U_bc_inv, &st.U_bc_inv_mask, 3, U_bc_inv))) ||
+      (d_bc && d_bc_inv && (!mk(s->d_bc, &st.density_bc, 1, d_bc) || !mk(s->d_bc_inv, &st.density_bc_inv_mask, 1, d_bc_inv))))
+    return fail(ctx, kFailed);
+  if (!(s->U1 = dev_alloc<float>(s->cells * 3)) || !(s->sums = dev_alloc<double>(2)) ||
+      !(s->xbuf = dev_alloc<float>(4 * s->xbuf_side)) || !(s->div = dev_alloc<float>(s->cells)) ||
+      !(s->p2 = dev_alloc<float>(s->cells)) || !(s->mask = dev_alloc<unsigned char>(s->cells)))
+    return fail(ctx, kFailed);
+  if (s->world > 1 &&
+      (!(s->inbox = dev_zeros<float>(6 * s->xbuf_side + 64 + kSumAreaFloats + 4 * s->p_side + 64)) ||
+       !(s->push_done = dev_zeros<unsigned int>(1))))
+    return fail(ctx, kFailed);
+  for (auto& pr : s->ev)
+    for (EventPtr& e : pr)
+      if (!(e = new_event(cudaEventDefault))) return fail(ctx, kFailed);
+  *out = s.release();
   return 0;
 }
 
@@ -425,7 +407,7 @@ int run_jacobi_block(tfl_ctx* ctx, const unsigned char* mask, const float* div, 
 int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl_grid*> fields, int width, int phase) {
   const bool pph = phase == kPhaseP;
   if (!pph) {
-    TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][0], ctx->stream));
+    TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][0].get(), ctx->stream));
     s->bytes_sent[phase] = 0;
   }
   if (s->world > 1 && width > 0 && (ctx->comm || s->peer_ok)) {
@@ -435,9 +417,9 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
       while ((int)s->jev.size() < 2 * (s->jx + 1)) {
         cudaEvent_t e = nullptr;
         TFL_CUDA(ctx, cudaEventCreate(&e));
-        s->jev.push_back(e);
+        s->jev.emplace_back(e);
       }
-      TFL_CUDA(ctx, cudaEventRecord(s->jev[2 * s->jx], ctx->stream));
+      TFL_CUDA(ctx, cudaEventRecord(s->jev[2 * s->jx].get(), ctx->stream));
     }
     SlabPack d;
     d.nchan = 0;
@@ -469,18 +451,20 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
       // my first owned planes land in the lower neighbour's "from above" slot, my last ones in the upper neighbour's "from below"
       k_slab_push<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(s->peer_inbox[0], 1) : nullptr, hi ? buf(s->peer_inbox[1], 0) : nullptr,
                                                    lo ? flag(s->peer_inbox[0], 1) : nullptr, hi ? flag(s->peer_inbox[1], 0) : nullptr,
-                                                   seq, s->push_done);
-      k_slab_pull<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(s->inbox, 0) : nullptr, hi ? buf(s->inbox, 1) : nullptr,
-                                                   lo ? flag(s->inbox, 0) : nullptr, hi ? flag(s->inbox, 1) : nullptr,
-                                                   seq, ctx->counters);
+                                                   seq, s->push_done.get());
+      float* inbox = s->inbox.get();
+      k_slab_pull<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(inbox, 0) : nullptr, hi ? buf(inbox, 1) : nullptr,
+                                                   lo ? flag(inbox, 0) : nullptr, hi ? flag(inbox, 1) : nullptr,
+                                                   seq, ctx->counters.get());
       sent = (size_t)(lo + hi) * side * 4;
       ctx->launches += 2;
     } else {
       NcclApi* nc = nccl_api();
-      d.send_lo = lo ? s->xbuf : nullptr;
-      d.send_hi = hi ? s->xbuf + s->xbuf_side : nullptr;
-      d.recv_lo = lo ? s->xbuf + 2 * s->xbuf_side : nullptr;
-      d.recv_hi = hi ? s->xbuf + 3 * s->xbuf_side : nullptr;
+      float* xbuf = s->xbuf.get();
+      d.send_lo = lo ? xbuf : nullptr;
+      d.send_hi = hi ? xbuf + s->xbuf_side : nullptr;
+      d.recv_lo = lo ? xbuf + 2 * s->xbuf_side : nullptr;
+      d.recv_hi = hi ? xbuf + 3 * s->xbuf_side : nullptr;
       k_slab_pack<false><<<blocks, 256, 0, ctx->stream>>>(d);
       TFL_NCCL(ctx, nc->GroupStart());
       if (lo) {                                       // lower neighbour: my first owned planes go down
@@ -498,14 +482,14 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
       ctx->launches += 2;
     }
     if (pph) {
-      TFL_CUDA(ctx, cudaEventRecord(s->jev[2 * s->jx + 1], ctx->stream));
+      TFL_CUDA(ctx, cudaEventRecord(s->jev[2 * s->jx + 1].get(), ctx->stream));
       s->jx += 1;
       s->jbytes += sent;
       return 0;
     }
     s->bytes_sent[phase] = sent;
   }
-  if (!pph) TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][1], ctx->stream));
+  if (!pph) TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][1].get(), ctx->stream));
   return 0;
 }
 
@@ -528,21 +512,21 @@ int slab_jacobi_projection(tfl_ctx* ctx, tfl_slab_sim* s, int iters) {
   s->jsched.resize((size_t)nblk * TFL_JACOBI_BLOCK_INTS);
   tfl_slab_jacobi_schedule(s->gnz, s->world, s->rank, s->margin, iters, planes, s->jsched.data(), nblk);
   if (slab_exchange(ctx, s, {&st.U}, planes[2], 2)) return 1;
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0], ctx->stream));          // no all-reduce on this path
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][1], ctx->stream));
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0].get(), ctx->stream));          // no all-reduce on this path
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][1].get(), ctx->stream));
   tfl_grid dv = st.p;
-  dv.data = s->div;
+  dv.data = s->div.get();
   Geo g;
   {
     SlabScope scope(ctx, s, planes[0], planes[1]);
     if (tfl_velocity_divergence_forward(ctx, &st.U, &st.flags, &dv)) return 1;
     if (make_geo(ctx, &st.flags, 1, &g)) return 1;
-    launch_jacobi_mask(st.flags.data, s->mask, g, ctx->stream);
+    launch_jacobi_mask(st.flags.data, s->mask.get(), g, ctx->stream);
     ctx->launches += 1;
   }
   TFL_CUDA(ctx, cudaMemsetAsync(st.p.data, 0, s->cells * 4, ctx->stream));   // generic/tfluids.cu:1854-1855
-  TFL_CUDA(ctx, cudaMemsetAsync(s->p2, 0, s->cells * 4, ctx->stream));
-  float* buf[2] = {st.p.data, s->p2};
+  TFL_CUDA(ctx, cudaMemsetAsync(s->p2.get(), 0, s->cells * 4, ctx->stream));
+  float* buf[2] = {st.p.data, s->p2.get()};
   int done = 0;
   s->jx = 0;
   s->jbytes = 0;
@@ -553,11 +537,11 @@ int slab_jacobi_projection(tfl_ctx* ctx, tfl_slab_sim* s, int iters) {
       pc.data = buf[done & 1];
       if (slab_exchange(ctx, s, {&pc}, o[1], kPhaseP)) return 1;
     }
-    if (run_jacobi_block(ctx, s->mask, s->div, buf[done & 1], buf[(done + 1) & 1], g, o[2], o[3], o[4], o[5], o[0], -1) < 0)
+    if (run_jacobi_block(ctx, s->mask.get(), s->div.get(), buf[done & 1], buf[(done + 1) & 1], g, o[2], o[3], o[4], o[5], o[0], -1) < 0)
       return 1;
     done += o[0];
   }
-  if (done & 1) TFL_CUDA(ctx, cudaMemcpyAsync(st.p.data, s->p2, s->cells * 4, cudaMemcpyDeviceToDevice, ctx->stream));
+  if (done & 1) TFL_CUDA(ctx, cudaMemcpyAsync(st.p.data, s->p2.get(), s->cells * 4, cudaMemcpyDeviceToDevice, ctx->stream));
   if (check_launch(ctx, "slab_sim_step (jacobi)")) return 1;
   SlabScope scope(ctx, s, s->own_lo, s->own_hi);
   return tfl_velocity_update_forward(ctx, &st.U, &st.flags, &st.p);
@@ -738,23 +722,24 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
   // the network input's reach across the cut (5 planes for a single bank)
   if (slab_exchange(ctx, s, {&st.U, &st.p}, 2 * tfl_slab_cnn_margin(cnn->nbanks) + 1, 2)) return 1;
   tfl_grid u1 = st.U;
-  u1.data = s->U1;
+  u1.data = s->U1.get();
+  double* sums = s->sums.get();
   {
     SlabScope scope(ctx, s, s->own_lo, s->own_hi);
-    if (tfl_cnn_stats(ctx, &st.U, &st.flags, &u1, s->sums)) return 1;
+    if (tfl_cnn_stats(ctx, &st.U, &st.flags, &u1, sums)) return 1;
   }
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0], ctx->stream));
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0].get(), ctx->stream));
   if (s->world > 1 && s->peer_ok && s->all_inbox_dev) {
-    k_sum_push<<<1, 64, 0, ctx->stream>>>(s->sums, s->all_inbox_dev, s->xbuf_side, s->rank, s->world, s->step_no);
-    k_sum_pull<<<1, 64, 0, ctx->stream>>>(s->sums, s->inbox, s->xbuf_side, s->world, s->step_no, ctx->counters);
+    k_sum_push<<<1, 64, 0, ctx->stream>>>(sums, s->all_inbox_dev.get(), s->xbuf_side, s->rank, s->world, s->step_no);
+    k_sum_pull<<<1, 64, 0, ctx->stream>>>(sums, s->inbox.get(), s->xbuf_side, s->world, s->step_no, ctx->counters.get());
     ctx->launches += 2;
   } else if (s->world > 1 && ctx->comm) {
-    TFL_NCCL(ctx, nccl_api()->AllReduce(s->sums, s->sums, 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
+    TFL_NCCL(ctx, nccl_api()->AllReduce(sums, sums, 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
   }
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][1], ctx->stream));
+  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][1].get(), ctx->stream));
   {
     SlabScope scope(ctx, s, s->own_lo, s->own_hi);
-    if (tfl_cnn_project_from_sums(ctx, cnn, &st.p, &u1, &st.flags, s->sums, &st.p, &st.U, mc->normalize_input_threshold)) return 1;
+    if (tfl_cnn_project_from_sums(ctx, cnn, &st.p, &u1, &st.flags, sums, &st.p, &st.U, mc->normalize_input_threshold)) return 1;
   }
   if (bcs()) return 1;
   SlabScope scope(ctx, s, s->own_lo, s->own_hi);
@@ -769,7 +754,7 @@ int tfl_slab_sim_ipc_export(tfl_ctx* ctx, tfl_slab_sim* s, char* handle_out) {
   if (!s->inbox) return fail(ctx, "slab_sim_ipc_export: a single rank has no neighbours");
   static_assert(sizeof(cudaIpcMemHandle_t) <= TFL_IPC_HANDLE_BYTES, "IPC handle fits the ABI buffer");
   cudaIpcMemHandle_t h;
-  TFL_CUDA(ctx, cudaIpcGetMemHandle(&h, s->inbox));
+  TFL_CUDA(ctx, cudaIpcGetMemHandle(&h, s->inbox.get()));
   memset(handle_out, 0, TFL_IPC_HANDLE_BYTES);
   memcpy(handle_out, &h, sizeof(h));
   return 0;
@@ -784,8 +769,7 @@ int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* s, const char* handles)
   NvtxRange range_(__func__);
   if (!s || !s->inbox) return fail(ctx, "slab_sim_ipc_connect: nil argument");
   auto drop = [&]() {
-    for (int r = 0; r < (int)s->all_inbox.size(); r++)
-      if (r != s->rank && s->all_inbox[r]) cudaIpcCloseMemHandle(s->all_inbox[r]);
+    s->mapped.clear();
     s->all_inbox.clear();
     s->peer_inbox[0] = s->peer_inbox[1] = nullptr;
     s->peer_ok = false;
@@ -794,8 +778,9 @@ int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* s, const char* handles)
   drop();
   if (!handles) return 0;                          // back to NCCL (e.g. another rank could not map its peers)
   if (s->world > 64) return fail(ctx, "slab_sim_ipc_connect: more than 64 ranks");
+  s->mapped.resize(s->world);
   s->all_inbox.assign(s->world, nullptr);
-  s->all_inbox[s->rank] = s->inbox;
+  s->all_inbox[s->rank] = s->inbox.get();
   for (int r = 0; r < s->world; r++) {
     if (r == s->rank) continue;
     cudaIpcMemHandle_t h;
@@ -807,15 +792,15 @@ int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* s, const char* handles)
       drop();
       return fail(ctx, "slab_sim_ipc_connect: cudaIpcOpenMemHandle(rank %d): %s (the exchanges stay on NCCL)", r, cudaGetErrorString(e));
     }
+    s->mapped[r].reset((float*)q);
     s->all_inbox[r] = (float*)q;
   }
   if (!s->all_inbox_dev) {
     void* p = nullptr;
     TFL_CUDA(ctx, cudaMalloc(&p, 64 * sizeof(float*)));
-    s->owned.push_back(p);
-    s->all_inbox_dev = (float**)p;
+    s->all_inbox_dev.reset((float**)p);
   }
-  TFL_CUDA(ctx, cudaMemcpy(s->all_inbox_dev, s->all_inbox.data(), s->world * sizeof(float*), cudaMemcpyHostToDevice));
+  TFL_CUDA(ctx, cudaMemcpy(s->all_inbox_dev.get(), s->all_inbox.data(), s->world * sizeof(float*), cudaMemcpyHostToDevice));
   if (s->rank > 0) s->peer_inbox[0] = s->all_inbox[s->rank - 1];
   if (s->rank < s->world - 1) s->peer_inbox[1] = s->all_inbox[s->rank + 1];
   s->peer_ok = true;
@@ -831,7 +816,7 @@ int tfl_slab_sim_exchange_stats(tfl_ctx* ctx, tfl_slab_sim* s, float ms[4], int6
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   for (int i = 0; i < 4; i++) {
     ms[i] = 0.0f;
-    if (cudaEventElapsedTime(&ms[i], s->ev[i][0], s->ev[i][1]) != cudaSuccess) { cudaGetLastError(); ms[i] = -1.0f; }
+    if (cudaEventElapsedTime(&ms[i], s->ev[i][0].get(), s->ev[i][1].get()) != cudaSuccess) { cudaGetLastError(); ms[i] = -1.0f; }
   }
   for (int i = 0; i < 3; i++) bytes[i] = (int64_t)s->bytes_sent[i];
   return 0;
@@ -847,7 +832,7 @@ int tfl_slab_sim_jacobi_stats(tfl_ctx* ctx, tfl_slab_sim* s, int32_t* exchanges,
   float total = 0.0f;
   for (int i = 0; i < s->jx; i++) {
     float t = 0.0f;
-    TFL_CUDA(ctx, cudaEventElapsedTime(&t, s->jev[2 * i], s->jev[2 * i + 1]));
+    TFL_CUDA(ctx, cudaEventElapsedTime(&t, s->jev[2 * i].get(), s->jev[2 * i + 1].get()));
     total += t;
   }
   if (exchanges) *exchanges = s->jx;

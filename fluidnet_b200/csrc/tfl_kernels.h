@@ -4,6 +4,7 @@
 #include <cuda_runtime.h>
 #include "../../include/tfl.h"
 #include "tfl_device.cuh"
+#include "tfl_holders.h"
 
 namespace tfl {
 
@@ -156,13 +157,13 @@ void launch_bn_apply(float* x, int nb, int c, long long n, long long bstride, co
 
 // ---- tfl_pcg.cu: matrix-free PCG pressure solve ----
 struct PcgScratch {            // owned by the context, grow-only
-  void* comp_buf = nullptr;    // per-component CG scalars
+  DevPtr<char> comp_buf;       // per-component CG scalars
   size_t comp_cap = 0;
-  unsigned long long* prog = nullptr;   // progress words of the triangular-sweep pipeline
+  DevPtr<unsigned long long> prog;   // progress words of the triangular-sweep pipeline
   size_t prog_cap = 0;
   unsigned long long epoch = 0;
-  int* host = nullptr;         // pinned read-back words
-  int sm_count = 0;
+  PinnedPtr<int> host;         // pinned read-back words
+  int sm_count = 0;            // set once the one-time setup (host words, kernel attributes) has succeeded
   void* debug_timing = nullptr;   // debug: device buffer [chunks][4] of sweep timestamps
   int groups_override = 0;     // debug: planes per CTA of the sweep kernel (0 = as many as fit)
 };
@@ -177,7 +178,6 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
 // chunks, cooperative grid of the sweeps.  Synchronises `st`.
 int pcg_precond(PcgScratch& sc, void* workspace, float* z, const float* flags, const float* r, int nb, int nz, int ny,
                 int nx, int is3d, int precond, int* geometry, long long* launches, cudaStream_t st);
-void pcg_release(PcgScratch& sc);
 int normalize_pressure_mean(void* workspace, float* p, const float* flags, int nb, int nz, int ny, int nx, int is3d,
                             long long* launches, cudaStream_t st);
 

@@ -675,12 +675,13 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
   const long long cells = g.n * nb;
 
   if (!sc.sm_count) {
-    int dev = 0;
+    int dev = 0, sms = 0;
     PCG_CUDA(cudaGetDevice(&dev));
-    PCG_CUDA(cudaDeviceGetAttribute(&sc.sm_count, cudaDevAttrMultiProcessorCount, dev));
-    PCG_CUDA(cudaMallocHost((void**)&sc.host, 64));
+    PCG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+    if (!(sc.host = pinned_alloc<int>(16))) return 3;
     PCG_CUDA(cudaFuncSetAttribute(k_sweep<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
     PCG_CUDA(cudaFuncSetAttribute(k_sweep<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+    sc.sm_count = sms;
   }
   s.sweep_threads = g.GP * g.NYP + 64;
   s.sweep_smem = (size_t)g.GP * 2 * (g.NYP + 2) * sizeof(float);
@@ -714,23 +715,24 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
   k_label_flatten<<<blocks_for(cells), 256, 0, st>>>(s.parent, s.csize, g);
   k_label_assign<<<blocks_for(cells), 256, 0, st>>>(s.parent, s.csize, s.cid, g, s.header + 3);
   *launches += 4;
-  PCG_CUDA(cudaMemcpyAsync(sc.host, s.header, 32, cudaMemcpyDeviceToHost, st));
+  PCG_CUDA(cudaMemcpyAsync(sc.host.get(), s.header, 32, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
-  if (sc.host[4]) return 1;
-  const int ncomp = s.ncomp = sc.host[3];
+  if (sc.host.get()[4]) return 1;
+  const int ncomp = s.ncomp = sc.host.get()[3];
   PCG_CUDA(cudaMemsetAsync(out, 0, cells * 4, st));                     // :1337
   if (ncomp == 0) return 0;
-  // per-component scalars
+  // per-component scalars; a capacity is recorded once its buffer exists
   const size_t per = 6 * 8 + 3 * 4;
   if ((size_t)ncomp * per + 256 > sc.comp_cap) {
-    if (sc.comp_buf) cudaFree(sc.comp_buf);
-    sc.comp_cap = (size_t)ncomp * per * 2 + 4096;
-    PCG_CUDA(cudaMalloc(&sc.comp_buf, sc.comp_cap));
+    const size_t cap = (size_t)ncomp * per * 2 + 4096;
+    sc.comp_buf = dev_alloc<char>(cap);
+    sc.comp_cap = sc.comp_buf ? cap : 0;
+    if (!sc.comp_buf) return 3;
   }
-  PCG_CUDA(cudaMemsetAsync(sc.comp_buf, 0, (size_t)ncomp * per + 256, st));
+  PCG_CUDA(cudaMemsetAsync(sc.comp_buf.get(), 0, (size_t)ncomp * per + 256, st));
   CompScalars& cs = s.cs;
   {
-    double* d = (double*)sc.comp_buf;
+    double* d = (double*)sc.comp_buf.get();
     cs.rz_new = d; cs.rz_old = d + ncomp; cs.pw = d + 2 * (size_t)ncomp; cs.rr_new = d + 3 * (size_t)ncomp;
     cs.rr_cur = d + 4 * (size_t)ncomp; cs.xsum = d + 5 * (size_t)ncomp;
     int* q = (int*)(d + 6 * (size_t)ncomp);
@@ -738,10 +740,12 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
     cs.header = s.header;
   }
   if ((size_t)g.chunks * 2 > sc.prog_cap) {
-    if (sc.prog) cudaFree(sc.prog);
-    sc.prog_cap = (size_t)g.chunks * 2 + 64;
-    PCG_CUDA(cudaMalloc((void**)&sc.prog, sc.prog_cap * 8));
-    PCG_CUDA(cudaMemsetAsync(sc.prog, 0, sc.prog_cap * 8, st));
+    const size_t cap = (size_t)g.chunks * 2 + 64;
+    sc.prog = dev_alloc<unsigned long long>(cap);
+    sc.prog_cap = 0;
+    if (!sc.prog) return 3;
+    PCG_CUDA(cudaMemsetAsync(sc.prog.get(), 0, cap * 8, st));
+    sc.prog_cap = cap;
     sc.epoch = 0;
   }
   // system arrays
@@ -754,7 +758,7 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
 
   SweepArgs& sa = s.sa;
   sa.cf = s.cf; sa.comp = s.comp; sa.r = s.r; sa.z = s.z; sa.pre = s.pre;
-  sa.prog_f = sc.prog; sa.prog_b = sc.prog + g.chunks;
+  sa.prog_f = sc.prog.get(); sa.prog_b = sc.prog.get() + g.chunks;
   sa.rz = cs.rz_new; sa.faults = s.header + 2;
   sa.timing = (unsigned long long*)sc.debug_timing;
   return 0;
@@ -788,6 +792,7 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   const int ncomp = s.ncomp;
   const CompScalars& cs = s.cs;
   int* header = s.header;
+  int* const host = sc.host.get();
   const unsigned ew_blocks = s.ew_blocks;
   const int no_precond = precond == 0;
   if (!no_precond) PCG_CUDA(launch_sweep(sc, s, true, launches, st));
@@ -795,14 +800,14 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   const double tol2 = (double)tol * (double)tol;
   k_scalars<<<(ncomp + 255) / 256, 256, 0, st>>>(cs, ncomp, tol2, max_iter, 1, no_precond);
   *launches += 2;
-  PCG_CUDA(cudaMemcpyAsync(sc.host, header, 16, cudaMemcpyDeviceToHost, st));
+  PCG_CUDA(cudaMemcpyAsync(host, header, 16, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
   float* p_old = s.p0;
   float* p_new = s.p1;
   // The host only needs to learn when every component has terminated; termination itself (tolerance or
   // iteration cap) is decided per component on the device, so reading back every 4th iteration changes
   // nothing in the result -- iterations past a component's end are no-ops for it.
-  while (sc.host[0] > 0 && !sc.host[1] && !sc.host[2]) {
+  while (host[0] > 0 && !host[1] && !host[2]) {
     for (int rep = 0; rep < 4; rep++) {
       PCG_CUDA(cudaMemsetAsync(header, 0, 4, st));
       if (!no_precond) PCG_CUDA(launch_sweep(sc, s, false, launches, st));
@@ -813,11 +818,11 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
       *launches += 3;
       float* tswap = p_old; p_old = p_new; p_new = tswap;
     }
-    PCG_CUDA(cudaMemcpyAsync(sc.host, header, 16, cudaMemcpyDeviceToHost, st));
+    PCG_CUDA(cudaMemcpyAsync(host, header, 16, cudaMemcpyDeviceToHost, st));
     PCG_CUDA(cudaStreamSynchronize(st));
   }
-  if (sc.host[2]) return 5;
-  if (sc.host[1]) return 2;
+  if (host[2]) return 5;
+  if (host[1]) return 2;
   k_xsum<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, s.x, cs, g.slots);
   k_writeback<<<blocks_for(cells), 256, 0, st>>>(p, s.parent, s.csize, s.cid, s.x, cs, g, 1);
   *launches += 2;
@@ -851,9 +856,9 @@ int pcg_precond(PcgScratch& sc, void* workspace, float* z, const float* flags, c
   if (s.ncomp == 0) return 0;
   PCG_CUDA(launch_sweep(sc, s, true, launches, st));
   PCG_CUDA(launch_sweep(sc, s, false, launches, st));
-  PCG_CUDA(cudaMemcpyAsync(sc.host, s.header, 16, cudaMemcpyDeviceToHost, st));
+  PCG_CUDA(cudaMemcpyAsync(sc.host.get(), s.header, 16, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
-  if (sc.host[2]) return 5;
+  if (sc.host.get()[2]) return 5;
   k_writeback<<<blocks_for(s.g.n * nb), 256, 0, st>>>(z, s.parent, s.csize, s.cid, s.z, s.cs, s.g, 0);
   *launches += 1;
   return cudaPeekAtLastError() == cudaSuccess ? 0 : 3;
@@ -890,13 +895,6 @@ int normalize_pressure_mean(void* workspace, float* p, const float* flags, int n
   k_npm_subtract<<<blocks_for(cells), 256, 0, st>>>(p, parent, csize, sums, cells);
   *launches += 5;
   return cudaGetLastError() == cudaSuccess ? 0 : 3;
-}
-
-void pcg_release(PcgScratch& sc) {
-  if (sc.comp_buf) cudaFree(sc.comp_buf);
-  if (sc.prog) cudaFree(sc.prog);
-  if (sc.host) cudaFreeHost(sc.host);
-  sc = PcgScratch();
 }
 
 }  // namespace tfl

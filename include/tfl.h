@@ -360,7 +360,9 @@ int tfl_simulate_step(tfl_ctx* ctx, const tfl_state* state, const tfl_mconf* mco
 /* Same step through HOST buffers (what a host application holding CPU tensors calls):
  * copies p, U, density in (pinned staging inside the context), runs the step, copies
  * p, U, density back, and synchronises.  flags / BC arrays are uploaded by
- * tfl_host_state_create once.  Used for the end-to-end number in bench.py. */
+ * tfl_host_state_create once.  Used for the end-to-end number in bench.py.  tfl_host_sim_create refuses, before
+ * it allocates and with *out left NULL, a grid with an extent < 1, is_3d = 0 with nz != 1, and a grid too large for
+ * the operators. */
 typedef struct tfl_host_sim tfl_host_sim;
 int tfl_host_sim_create(tfl_ctx* ctx, int32_t nb, int32_t nz, int32_t ny, int32_t nx, int is_3d,
                         const float* flags, const float* U_bc, const float* U_bc_inv_mask,
