@@ -827,8 +827,8 @@ static int set_const_vals(tfl_ctx* ctx, const tfl_state* s) {       // lib/simul
   return 0;
 }
 
-// Fused pipeline for the convnet path with the tensor-core conv stack: 12 launches, every
-// field crosses memory once per stage.  Bit-identical to the operator sequence below.
+// Fused pipeline for the convnet path with the tensor-core conv stack: 12 launches with a single-bank
+// stack, every field crosses memory once per stage.  Bit-identical to the operator sequence below.
 static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, tfl_cnn* m, const Geo& g) {
   const size_t cells = (size_t)g.n * g.nb;
   const bool has_density = s->density.data != nullptr;
@@ -932,10 +932,10 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
   if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in.get(), 0));          // pDiv is first read here
   launch_cnn_inputs_fused(s->p.data, s->U.data, fl8, sums, mc->normalize_input_threshold, scale, m->act[0].get(),
                           tg.px, tg.py, g, st);
-  run_conv_stack(m, p_net, st);
+  const int stack = run_conv_stack(m, p_net, st);
   launch_cnn_finish_fused(p_net, s->U.data, fl8, scale, s->p.data, u_bc ? s->U_bc_inv_mask.data : nullptr,
                           u_bc ? s->U_bc.data : nullptr, qmask, -1e6f, 1e6f, g, st);
-  ctx->launches += 6;
+  ctx->launches += 3 + stack;     // launch_vort_bc_mask, the fused input and finish, and the stack's own
   return check_launch(ctx, "simulate_step (fused)");
 }
 

@@ -1,5 +1,6 @@
-// Internal interface of the C ABI units: tfl_api.cu (context, memory, operators, step drivers),
-// tfl_api_cnn.cu (projection network) and tfl_api_slab.cu (z-slab driver).
+// Internal interface of the C ABI units: tfl_api.cu (context, memory, operators, step drivers), tfl_api_cnn.cu
+// (projection network: creation and entry points), tfl_cnn_forward.cu (its forward drivers), tfl_api_cnn_debug.cu (its
+// test hooks) and tfl_api_slab.cu (z-slab driver).
 #pragma once
 #include <cuda_runtime.h>
 #include <stdarg.h>
@@ -266,9 +267,57 @@ struct StepForces {
 };
 StepForces step_forces(const tfl_mconf* mc, int nx, int ny, int gnz);
 
-// Tensor-core path of the projection network (tfl_api_cnn.cu).
+constexpr int kMaxBanks = kMaxBankPtrs;     // banks a join kernel takes
+constexpr int kTailFloats = 64 + 8 + 8 + 1;     // the fused 1x1x1 tail: w4[8][8], b4[8], w5[8], b5[1]
+
+// Appends p to v; false (and v unchanged) if p is empty, its upload having failed.
+inline bool keep(std::vector<DevPtr<float>>& v, DevPtr<float> p) {
+  if (!p) return false;
+  v.push_back(std::move(p));
+  return true;
+}
+
+// Weight layouts of the projection network (tfl_api_cnn.cu).
+// Packs a [8][cin][3][3][3] weight for launch_conv3_tc / launch_conv3_tc_join and uploads it.
+DevPtr<float> upload_tc_weights(const float* w, int cin, int split);
+// A convolution weight in Torch layout [cout][cin][taps] re-laid out as the [cin][tap][cout] that
+// launch_conv_direct and launch_conv_any read.
+std::vector<float> relayout_conv_weights(const float* w, int cin, int cout, int taps);
+// Bank i's 8-channel slice of a 'concat' join weight [8][8 nbanks][3][3][3] (one bank: the whole weight).
+std::vector<float> concat_slice(const float* w, int nbanks, int i);
+
+// The projection network's forward pass (tfl_cnn_forward.cu).  What enqueues kernels returns how many it enqueued.
+// Tensor-core path: padded channels-last activations owned by the model (their zero borders
+// must survive between calls, so they do not live in the shared arena).
+// z-slab (g.zoff, g.gnz): bank i holds the global coarse planes [ceil(zoff / 2^i), floor((zoff + nz) / 2^i)).
+// Dilated banks: bank i's buffers hold its 8^i phase sub-grids per batch entry (make_conv_tc_phase_geo).
 int cnn_ensure_act(tfl_ctx* ctx, tfl_cnn* m, const Geo& g);
-void run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo = 0, int p_hi = -1);
+// The three 3x3x3 layers (+ fused 1x1x1 tail) on tensor cores: act[0] -> act[1] -> act[2] -> p_net.
+// p_lo / p_hi: planes on which p_net is wanted (default all).  Layer l then only has to produce the planes the
+// later layers' 3x3x3 stencils reach from there; on a z-slab that spares most of the ghost planes.
+int run_conv_stack(tfl_cnn* m, float* p_net, cudaStream_t st, int p_lo = 0, int p_hi = -1);
+// The join layer of a banked stack (split 1, join 3) -> p_net on the output planes [g.z_lo, g.z_hi), reading bank
+// i's layer-2 output l2[i] (geometry geo[i], 2^-i of bank 1's resolution) with nearest indexing.  z-slab: local
+// full-resolution plane 0 is global plane zoff, bank i's local plane 0 its global coarse plane org[i] (whole grids:
+// all 0).  'add': one launch summing the banks, weights wj[0]; 'concat': one launch per bank with its slice wj[i],
+// banks N..2 writing / adding the fp32 partial sum `part`, bank 1 last adding it before the bias, ReLU and tail (one
+// bank: no partial sum).  phases: banks 2..N are dilated banks held as phase sub-grids (geo[i] =
+// make_conv_tc_phase_geo(.., i)) rather than multi-resolution banks.
+int launch_tc_join(const float* const* l2, const ConvTcGeo* geo, const int* org, int zoff, int nbanks, bool add,
+                   float* part, float* p_net, const std::vector<DevPtr<float>>& wj, const float* bias,
+                   const float* tail, int split, const ConvTcGeo& g, cudaStream_t st, bool phases = false,
+                   const TcEpi& ep = TcEpi());
+// Device fields of one forward: pDiv, the velocity (UDiv, or on a z-slab the wall-masked U1 of tfl_cnn_stats), the
+// flags, and the p and U the forward writes.
+struct CnnFields {
+  const float *p_div, *U, *flags;
+  float *p_out, *U_out;
+};
+// model:forward on the whole grid g; scale_out (host, may be null) receives the input scale of every batch entry.
+int cnn_project(tfl_ctx* ctx, tfl_cnn* m, const CnnFields& f, float threshold, const Geo& g, float* scale_out);
+// Everything after the one global reduction, from the reduced sums of tfl_cnn_stats (tensor-core path only).
+int cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const CnnFields& f, const double* dev_sums, float threshold,
+                          const Geo& g);
 // Whether the model runs on a z-slab of a [gnz][ny][nx] domain with this margin whose local planes [0, nz) start at
 // global plane zoff and own [own_lo, own_hi): the tensor-core path, and for banked models the margin of
 // tfl_slab_cnn_margin, ghost planes that deep and a global grid divisible by 2^(banksNum-1).  Fails naming the

@@ -1,8 +1,8 @@
 """Layer-level parity of the fp32 projection-network kernels (fluidnet_b200/csrc/tfl_cnn.cu): the direct convolution
 k_conv_direct at every (cout, k) it is specialised for, the generic k_conv_any, k_pool, k_pixel_shuffle and
 k_bank_join, one launch at a time through the test hooks tfl_debug_conv_fp32, tfl_debug_pool,
-tfl_debug_pixel_shuffle and tfl_debug_bank_join (tfl_api_cnn.cu); and the graph executor (cnn_project_impl), which
-must keep the entries of a batch apart.
+tfl_debug_pixel_shuffle and tfl_debug_bank_join (tfl_api_cnn_debug.cu); and the graph executor (tfl_cnn_forward.cu),
+which must keep the entries of a batch apart.
 
 Convolution reference: conv3d in float64 (conv2d for 2-D, as a conv3d with kz = 1), zero padding (k - 1) / 2, plus
 the bias, then the activation.  S = conv(|x|, |w|) + |b|, n = cin * taps + 1 terms.

@@ -1,6 +1,6 @@
 """Layer-level parity of the tensor-core 3x3x3 convolution (k_conv3_tc, fluidnet_b200/csrc/tfl_cnn_tc.cu).
 
-One layer at a time runs through the test hook tfl_debug_conv3_tc (tfl_api_cnn.cu): the weights are packed by
+One layer at a time runs through the test hook tfl_debug_conv3_tc (tfl_api_cnn_debug.cu): the weights are packed by
 conv_tc_pack_weights, the activations live in the padded channels-last layout [nb][2 planes][nz+2][py][px][4]
 (channels 0-3, 4-7), and the result is compared with torch.nn.functional.conv3d in float64 on the CPU
 (padding 1, + bias, ReLU; for the last 3x3x3 layer then the 8->8 1x1x1 layer, ReLU and the 8->1 layer).
