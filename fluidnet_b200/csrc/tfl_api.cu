@@ -538,9 +538,10 @@ int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_gr
   std::vector<double> h(g.nb);
   // A fixed number of sweeps on an L2-resident grid: all but the last inside one cooperative kernel (sweep 0
   // reads p_prev and writes p, as the loop below does); the loop then runs the last sweep and the residual.
-  if (!need_every && max_iter > 2) {
+  // Larger grids are bandwidth-bound per sweep and do not fit the SMs.
+  if (!need_every && max_iter > 2 && g.is3d && g.nz >= 4 && g.n * g.nb <= (3LL << 20)) {
     const int fused = max_iter - 1;
-    if (launch_jacobi_sweeps(mask, div->data, p_prev, p->data, g, fused, st)) {
+    if (launch_jacobi_block(mask, div->data, p_prev, p->data, g, 0, g.nz, 0, 0, fused, /*deep=*/false, st)) {
       ctx->launches += 1;
       iter = fused;
       if (fused & 1) { cur = p_prev; prev = p->data; }        // the last fused sweep wrote p

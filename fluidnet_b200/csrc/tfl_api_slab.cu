@@ -400,8 +400,6 @@ __global__ void k_sum_pull(double* __restrict__ out, float* inbox, size_t xbuf_s
 // may push exchange e + 1 while its neighbour still scatters exchange e; it cannot push e + 2 before the neighbour
 // has pushed e + 1, which that neighbour does after scattering e).
 constexpr int kPhaseP = 4;
-int run_jacobi_block(tfl_ctx* ctx, const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,
-                     int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int path);
 
 // Refresh `width` ghost planes on both sides of the listed fields from the neighbours' owned planes.
 int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl_grid*> fields, int width, int phase) {
@@ -501,6 +499,25 @@ struct SlabScope {       // slab placement of the context for the enclosed calls
   ~SlabScope() { ctx->slab = false; ctx->slab_margin = 2; }
 };
 
+// One block of sweeps on a prepared mask: the cooperative block kernel or one launch per sweep (path -1: automatic,
+// 0: per sweep, 1: one launch, refused when it does not apply).  Returns the path taken, -1 on refusal.
+// The automatic path takes the one-launch kernel only with 4-plane blocks (ranges up to 2.16M cells on an H100):
+// measured on an H100 at 400 W, 34 / 100 sweeps of 128^3 run at 8.4 / 7.3 us per sweep in one launch against
+// 8.9 / 8.2 per launch, but a 6-sweep block on an 8-rank slab of 256^3 (256^2 x 42 planes, 6-plane blocks) takes
+// 154 us against 94 us in per-sweep launches.
+int run_jacobi_block(tfl_ctx* ctx, const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,
+                     int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int path) {
+  if (sweeps < 1) return 0;
+  if (path != 0 && launch_jacobi_block(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, path == 1, ctx->stream)) {
+    ctx->launches += 1;
+    return 1;
+  }
+  if (path == 1) return -1;
+  launch_jacobi_range_sweeps(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, ctx->stream);
+  ctx->launches += sweeps;
+  return 0;
+}
+
 // lib/simulate.lua:275-303 with pTol = 0 on this rank's slab: divergence, `iters` Jacobi sweeps from p = 0 in the
 // blocks of tfl_slab_jacobi_schedule, velocity update on the owned planes.  Every cell sees the single-GPU sweep's
 // operands, so p and U are bit-identical to tfl_simulate_step's.
@@ -598,33 +615,6 @@ int tfl_slab_cnn_margin(int32_t banks_num) {
   if (banks_num > kTcMaxBanks) return -1;
   return std::max(2, (3 * (1 << (banks_num - 1)) + 1) / 2);
 }
-
-}  // extern "C"
-
-namespace {
-
-// One block of sweeps on a prepared mask: the cooperative block kernel or one launch per sweep (path -1: automatic,
-// 0: per sweep, 1: one launch, refused when it does not apply).  Returns the path taken, -1 on refusal.
-// The automatic path takes the one-launch kernel only with 4-plane blocks (ranges up to 2.16M cells on an H100):
-// measured on an H100 at 400 W, 34 / 100 sweeps of 128^3 run at 8.4 / 7.3 us per sweep in one launch against
-// 8.9 / 8.2 per launch, but a 6-sweep block on an 8-rank slab of 256^3 (256^2 x 42 planes, 6-plane blocks) takes
-// 154 us against 94 us in per-sweep launches.
-int run_jacobi_block(tfl_ctx* ctx, const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,
-                     int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int path) {
-  if (sweeps < 1) return 0;
-  if (path != 0 && launch_jacobi_block(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, path == 1, ctx->stream)) {
-    ctx->launches += 1;
-    return 1;
-  }
-  if (path == 1) return -1;
-  launch_jacobi_range_sweeps(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, ctx->stream);
-  ctx->launches += sweeps;
-  return 0;
-}
-
-}  // namespace
-
-extern "C" {
 
 int tfl_jacobi_slab_block(tfl_ctx* ctx, const tfl_grid* pa, const tfl_grid* pb, const tfl_grid* flags,
                           const tfl_grid* div, int is_3d, int32_t z_lo, int32_t z_hi, int32_t shrink_lo,

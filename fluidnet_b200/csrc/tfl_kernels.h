@@ -55,12 +55,11 @@ template <typename FT>
 void launch_jacobi_mask(const FT* flags, unsigned char* mask, const Geo& g, cudaStream_t st);
 void launch_jacobi_iter(const unsigned char* mask, const float* div, const float* prev, float* cur,
                         const Geo& g, cudaStream_t st);
-bool launch_jacobi_sweeps(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int sweeps,
-                          cudaStream_t st);
 // One block of `sweeps` sweeps on local planes [z_lo, z_hi) that shrink by shr_lo / shr_hi planes per sweep
 // (sweep s reads pa and writes pb for even s, the reverse for odd s).  launch_jacobi_block runs them in one
 // cooperative launch and returns its block depth in planes (4, or 6 with `deep`), or 0 when the shape / device does
-// not qualify or the range does not fit co-resident; launch_jacobi_range_sweeps launches one kernel per sweep.
+// not qualify or the range does not fit co-resident; it serves the z-slab blocks and, with [0, nz) and no shrink,
+// the whole-grid solve.  launch_jacobi_range_sweeps launches one kernel per sweep.
 int launch_jacobi_block(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo,
                         int z_hi, int shr_lo, int shr_hi, int sweeps, bool deep, cudaStream_t st);
 void launch_jacobi_range_sweeps(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,

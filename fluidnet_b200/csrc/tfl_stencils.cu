@@ -712,6 +712,36 @@ __global__ void k_jacobi_iter(const unsigned char* __restrict__ mask, const floa
   cur[c] = (p1 + p2 + p3 + p4 + p5 + p6 + __ldg(div + c)) / denom;
 }
 
+// The update of k_jacobi_iter on 4 consecutive x cells: m4 holds their 4 mask bytes, ctr / dv their p and div,
+// left / right the x neighbours of the first and last cell, ym .. zp the neighbouring rows.  Writes the live cells
+// of `out` and leaves the masked ones (the caller zeroes it).  Every kernel below computes its cells here, so they all
+// give the same bits.  The caller-owned array, rather than a returned float4, keeps k_jacobi_iter4 at 40 registers.
+template <bool IS3D>
+__device__ __forceinline__ void jacobi_update4(unsigned m4, float4 ctr, float left, float right, float4 ym, float4 yp,
+                                                 float4 zm, float4 zp, float4 dv, float (&out)[4]) {
+  const float pcv[4] = {ctr.x, ctr.y, ctr.z, ctr.w};
+  const float xm[4] = {left, ctr.x, ctr.y, ctr.z};
+  const float xp[4] = {ctr.y, ctr.z, ctr.w, right};
+  const float ymv[4] = {ym.x, ym.y, ym.z, ym.w}, ypv[4] = {yp.x, yp.y, yp.z, yp.w};
+  const float zmv[4] = {zm.x, zm.y, zm.z, zm.w}, zpv[4] = {zp.x, zp.y, zp.z, zp.w};
+  const float dvv[4] = {dv.x, dv.y, dv.z, dv.w};
+#pragma unroll
+  for (int q = 0; q < 4; q++) {
+    const unsigned m = (m4 >> (8 * q)) & 0xFFu;
+    if (m & 1) continue;
+    const float p1 = (m & 2) ? pcv[q] : xm[q];
+    const float p2 = (m & 4) ? pcv[q] : xp[q];
+    const float p3 = (m & 8) ? pcv[q] : ymv[q];
+    const float p4 = (m & 16) ? pcv[q] : ypv[q];
+    float p5 = 0.0f, p6 = 0.0f;
+    if (IS3D) {
+      p5 = (m & 32) ? pcv[q] : zmv[q];
+      p6 = (m & 64) ? pcv[q] : zpv[q];
+    }
+    out[q] = (p1 + p2 + p3 + p4 + p5 + p6 + dvv[q]) / (IS3D ? 6.0f : 4.0f);
+  }
+}
+
 // Same update, 4 consecutive x cells per thread (float4 rows, one 32-bit load for the 4 mask
 // bytes): 8 memory instructions per 4 cells instead of 40.  Requires nx % 4 == 0.
 template <bool IS3D, typename FT>
@@ -742,28 +772,7 @@ k_jacobi_iter4(const unsigned char* __restrict__ mask, const float* __restrict__
     }
     const float left = i0 > 0 ? __ldg(prev + c - 1) : 0.0f;
     const float right = i0 + 4 < g.nx ? __ldg(prev + c + 4) : 0.0f;
-    const float pcv[4] = {pc.x, pc.y, pc.z, pc.w};
-    const float xm[4] = {left, pc.x, pc.y, pc.z};
-    const float xp[4] = {pc.y, pc.z, pc.w, right};
-    const float ymv[4] = {ym.x, ym.y, ym.z, ym.w}, ypv[4] = {yp.x, yp.y, yp.z, yp.w};
-    const float zmv[4] = {zm.x, zm.y, zm.z, zm.w}, zpv[4] = {zp.x, zp.y, zp.z, zp.w};
-    const float dvv[4] = {dv.x, dv.y, dv.z, dv.w};
-    const float denom = g.is3d ? 6.0f : 4.0f;
-#pragma unroll
-    for (int q = 0; q < 4; q++) {
-      const unsigned m = (m4 >> (8 * q)) & 0xFFu;
-      if (m & 1) continue;
-      const float p1 = (m & 2) ? pcv[q] : xm[q];
-      const float p2 = (m & 4) ? pcv[q] : xp[q];
-      const float p3 = (m & 8) ? pcv[q] : ymv[q];
-      const float p4 = (m & 16) ? pcv[q] : ypv[q];
-      float p5 = 0.0f, p6 = 0.0f;
-      if (g.is3d) {
-        p5 = (m & 32) ? pcv[q] : zmv[q];
-        p6 = (m & 64) ? pcv[q] : zpv[q];
-      }
-      out[q] = (p1 + p2 + p3 + p4 + p5 + p6 + dvv[q]) / denom;
-    }
+    jacobi_update4<IS3D>(m4, pc, left, right, ym, yp, zm, zp, dv, out);
   }
   *(float4*)(cur + c) = make_float4(out[0], out[1], out[2], out[3]);
 }
@@ -819,28 +828,8 @@ k_jacobi_march(const unsigned char* __restrict__ mask, const float* __restrict__
     __syncthreads();
     const float4 ym = ty > 0 ? rows[buf][ty - 1][tx] : in.ym;
     const float4 yp = ty < kJY - 1 ? rows[buf][ty + 1][tx] : in.yp;
-    const unsigned m4 = in.m4;
     float out[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-    if ((m4 & 0x01010101u) != 0x01010101u) {
-      const float pcv[4] = {pc.x, pc.y, pc.z, pc.w};
-      const float xm[4] = {left, pc.x, pc.y, pc.z};
-      const float xp[4] = {pc.y, pc.z, pc.w, right};
-      const float ymv[4] = {ym.x, ym.y, ym.z, ym.w}, ypv[4] = {yp.x, yp.y, yp.z, yp.w};
-      const float zmv[4] = {pm.x, pm.y, pm.z, pm.w}, zpv[4] = {pp.x, pp.y, pp.z, pp.w};
-      const float dvv[4] = {in.dv.x, in.dv.y, in.dv.z, in.dv.w};
-#pragma unroll
-      for (int q = 0; q < 4; q++) {
-        const unsigned m = (m4 >> (8 * q)) & 0xFFu;
-        if (m & 1) continue;
-        const float p1 = (m & 2) ? pcv[q] : xm[q];
-        const float p2 = (m & 4) ? pcv[q] : xp[q];
-        const float p3 = (m & 8) ? pcv[q] : ymv[q];
-        const float p4 = (m & 16) ? pcv[q] : ypv[q];
-        const float p5 = (m & 32) ? pcv[q] : zmv[q];
-        const float p6 = (m & 64) ? pcv[q] : zpv[q];
-        out[q] = (p1 + p2 + p3 + p4 + p5 + p6 + dvv[q]) / 6.0f;
-      }
-    }
+    if ((in.m4 & 0x01010101u) != 0x01010101u) jacobi_update4<true>(in.m4, pc, left, right, ym, yp, pm, pp, in.dv, out);
     *(float4*)(cur + c) = make_float4(out[0], out[1], out[2], out[3]);
     pm = pc;
     pc = pp;
@@ -849,126 +838,31 @@ k_jacobi_march(const unsigned char* __restrict__ mask, const float* __restrict__
   }
 }
 
-// All sweeps in ONE kernel with the CTA's cells resident on the SM.  A CTA owns a 128 x 8 x kJZ block for the
-// whole solve (cooperative launch: every CTA stays resident): its p values live in registers from sweep to
-// sweep, div and the block's y-rows in shared memory, and per sweep only the block's halo (two z planes, two
-// y rows per plane, the x neighbours of wider grids) is read from L2 -- written there by the neighbouring CTAs
-// before the grid-wide barrier that separates the sweeps.  For grids whose fields sit in L2 (128^3: 8 MB per
-// field) the one-kernel-per-sweep version spent most of a sweep on the launch boundary and on L2 latency in
-// its plane-by-plane march; here a sweep is one halo round trip, ~500 instructions per thread and the barrier.
-// p is read with ld.global.cg (L1 is not coherent across CTAs).  Same per-cell expression (bit-identical).
-constexpr int kJZ = 4;
-constexpr int kJG = 4;        // blocks per CTA: fewer, fatter CTAs make the grid-wide barrier (one atomic per CTA) cheaper
-__global__ void __launch_bounds__(256 * kJG, 1)
-k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb, Geo g,
-                  int sweeps, int nblocks) {
-  cooperative_groups::grid_group grid = cooperative_groups::this_grid();
-  extern __shared__ float4 jsm[];
-  // thread group threadIdx.z of the CTA owns block blockIdx.x * kJG + threadIdx.z (x tile fastest, then y, then z chunk)
-  constexpr int kGroupF4 = kJZ * (kJY + 2) * 32 + kJZ * kJY * 32;
-  float4* gsm = jsm + threadIdx.z * kGroupF4;
-  float4 (*rows)[kJY + 2][32] = reinterpret_cast<float4 (*)[kJY + 2][32]>(gsm);               // [kJZ][kJY + 2][32]
-  float4 (*dvs)[kJY][32] = reinterpret_cast<float4 (*)[kJY][32]>(gsm + kJZ * (kJY + 2) * 32);   // [kJZ][kJY][32]
-  const int tx = threadIdx.x, ty = threadIdx.y;
-  const int blk = blockIdx.x * kJG + threadIdx.z;
-  const bool live = blk < nblocks;                         // a group without a block only takes part in the barriers
-  const int nxt = g.nx / 128, nyt = g.ny / kJY;
-  const int bx = blk % nxt, by = (blk / nxt) % nyt, bz = blk / (nxt * nyt);
-  const int i0 = (bx * 32 + tx) * 4;
-  const int j = by * kJY + ty;
-  const int nchunks = (g.nz + kJZ - 1) / kJZ;
-  const int b = live ? bz / nchunks : 0;
-  const int k0 = live ? (bz % nchunks) * kJZ : 0;
-  const int np = live ? min(kJZ, g.nz - k0) : 0;           // planes of this block
-  const int sy = g.nx, sz = g.nx * g.ny;
-  const long long base = live ? b * g.n + (long long)k0 * sz + (long long)j * sy + i0 : 0;
-  const float4 zero4 = make_float4(0.f, 0.f, 0.f, 0.f);
-  const bool has_left = tx == 0 && i0 > 0, has_right = tx == 31 && i0 + 4 < g.nx;
-  unsigned m4[kJZ];
-  float4 pc[kJZ];
-#pragma unroll
-  for (int k = 0; k < kJZ; k++) {
-    const bool in = k < np;
-    m4[k] = in ? __ldg((const unsigned*)(mask + base + (long long)k * sz)) : 0x01010101u;
-    dvs[k][ty][tx] = in ? __ldg((const float4*)(div + base + (long long)k * sz)) : zero4;
-    pc[k] = in ? __ldcg((const float4*)(pa + base + (long long)k * sz)) : zero4;
-  }
-  for (int s = 0; s < sweeps; s++) {
-    const float* prev = (s & 1) ? pb : pa;                 // sweep 0 reads pa and writes pb
-    float* cur = (s & 1) ? pa : pb;
-    // halo of the block, all requests in flight together
-    const float4 zlo = (live && k0 > 0) ? __ldcg((const float4*)(prev + base - sz)) : zero4;
-    const float4 zhi = (live && k0 + np < g.nz) ? __ldcg((const float4*)(prev + base + (long long)np * sz)) : zero4;
-    float left[kJZ], right[kJZ];
-#pragma unroll
-    for (int k = 0; k < kJZ; k++) {
-      const long long c = base + (long long)k * sz;
-      const bool in = k < np;
-      if (ty == 0) rows[k][0][tx] = (in && j > 0) ? __ldcg((const float4*)(prev + c - sy)) : zero4;
-      if (ty == kJY - 1) rows[k][kJY + 1][tx] = (in && j + 1 < g.ny) ? __ldcg((const float4*)(prev + c + sy)) : zero4;
-      left[k] = (in && has_left) ? __ldcg(prev + c - 1) : 0.0f;
-      right[k] = (in && has_right) ? __ldcg(prev + c + 4) : 0.0f;
-      rows[k][ty + 1][tx] = pc[k];
-    }
-    asm volatile("bar.sync %0, 256;" ::"r"(1 + (int)threadIdx.z) : "memory");      // this group's rows are in place
-    float4 below = zlo;
-#pragma unroll
-    for (int k = 0; k < kJZ; k++) {
-      const float4 ctr = pc[k];
-      const float4 above = k + 1 < kJZ ? (k + 1 < np ? pc[k + 1] : zhi) : zhi;
-      float out[4] = {0.0f, 0.0f, 0.0f, 0.0f};
-      const unsigned mm = m4[k];
-      float lf = __shfl_up_sync(0xffffffffu, ctr.w, 1);        // every lane takes part, whatever its mask
-      float rt = __shfl_down_sync(0xffffffffu, ctr.x, 1);
-      if (tx == 0) lf = left[k];
-      if (tx == 31) rt = right[k];
-      if ((mm & 0x01010101u) != 0x01010101u) {
-        const float4 ym = rows[k][ty][tx], yp = rows[k][ty + 2][tx], dv = dvs[k][ty][tx];
-        const float pcv[4] = {ctr.x, ctr.y, ctr.z, ctr.w};
-        const float xm[4] = {lf, ctr.x, ctr.y, ctr.z};
-        const float xp[4] = {ctr.y, ctr.z, ctr.w, rt};
-        const float ymv[4] = {ym.x, ym.y, ym.z, ym.w}, ypv[4] = {yp.x, yp.y, yp.z, yp.w};
-        const float zmv[4] = {below.x, below.y, below.z, below.w}, zpv[4] = {above.x, above.y, above.z, above.w};
-        const float dvv[4] = {dv.x, dv.y, dv.z, dv.w};
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-          const unsigned m = (mm >> (8 * q)) & 0xFFu;
-          if (m & 1) continue;
-          const float p1 = (m & 2) ? pcv[q] : xm[q];
-          const float p2 = (m & 4) ? pcv[q] : xp[q];
-          const float p3 = (m & 8) ? pcv[q] : ymv[q];
-          const float p4 = (m & 16) ? pcv[q] : ypv[q];
-          const float p5 = (m & 32) ? pcv[q] : zmv[q];
-          const float p6 = (m & 64) ? pcv[q] : zpv[q];
-          out[q] = (p1 + p2 + p3 + p4 + p5 + p6 + dvv[q]) / 6.0f;
-        }
-      }
-      const float4 o4 = make_float4(out[0], out[1], out[2], out[3]);
-      if (k < np) *(float4*)(cur + base + (long long)k * sz) = o4;
-      pc[k] = o4;
-      below = ctr;
-    }
-    grid.sync();                                           // also orders the shared rows against the next sweep
-  }
-}
-
-// One block of Jacobi sweeps on a plane range of a z-slab in ONE cooperative launch (the Jacobi path of
-// tfl_slab_sim_step).  Same residency as k_jacobi_resident -- a thread group owns a 128 x 8 x KZ block for the whole
-// launch, p in registers, div and the block's y rows in shared memory, a grid-wide barrier between sweeps -- but the
-// blocks tile the local planes [z_lo, z_hi) only, and sweep s computes [z_lo + s * shr_lo, z_hi - s * shr_hi): the
-// range loses one plane per sweep on each side whose ghost planes came from a neighbour.  Cells outside a sweep's
-// range keep their value and are not stored; no cell of a later, narrower range reads them.  Same per-cell
-// expression (bit-identical to one k_jacobi_iter4 launch per sweep on the same ranges and buffers).
+// Jacobi sweeps in ONE cooperative launch with the CTA's cells resident on the SM: the whole-grid solve of
+// tfl_solve_linear_system_jacobi (planes [0, nz), no shrink) and the sweep blocks of the z-slab step (tfl_slab_sim_step).
+// A 256-thread group owns a 128 x 8 x KZ block for the whole launch (every CTA stays resident): its p values live in
+// registers from sweep to sweep, div, the block's y rows and its x halo in shared memory, and per sweep only the
+// block's halo (two z planes, two y rows per plane, the x neighbours of wider grids) is read from L2 -- written there
+// by the neighbouring CTAs before the grid-wide barrier that separates the sweeps.  For grids whose fields sit in L2
+// (128^3: 8 MB per field) one kernel per sweep spends most of a sweep on the launch boundary and on L2 latency in its
+// plane-by-plane march; here a sweep is one halo round trip and the barrier.  p is read with ld.global.cg (L1 is not
+// coherent across CTAs).
+// The blocks tile the local planes [z_lo, z_hi), and sweep s computes [z_lo + s * shr_lo, z_hi - s * shr_hi): on a slab
+// the range loses one plane per sweep on each side whose ghost planes came from a neighbour.  Cells outside a sweep's
+// range keep their value and are not stored; no cell of a later, narrower range reads them.  Bit-identical to one
+// k_jacobi_iter4 launch per sweep on the same ranges and buffers.
 // Co-residency: one 1024-thread CTA per SM (64 registers per thread), kJG blocks of 128 x 8 x KZ cells per CTA, so
 // at most 132 * 4 * 4096 * KZ / 4 cells on an H100: 2.16M with KZ = 4, 3.24M with KZ = 6 -- the deepest block whose
 // shared memory (kJG x KZ x (18 rows of 32 float4 + the x halo)) fits one SM: 217.5 KiB.  The dispatcher takes the
 // shallowest KZ that fits.  The x halo goes through shared memory to spare registers.
+constexpr int kJG = 4;        // blocks per CTA: fewer, fatter CTAs make the grid-wide barrier (one atomic per CTA) cheaper
 template <int KZ>
 __global__ void __launch_bounds__(256 * kJG, 1)
-k_jacobi_block(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb, Geo g,
-               int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks) {
+k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb, Geo g,
+                  int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks) {
   cooperative_groups::grid_group grid = cooperative_groups::this_grid();
   extern __shared__ float4 jsm[];
+  // thread group threadIdx.z of the CTA owns block blockIdx.x * kJG + threadIdx.z (x tile fastest, then y, then z chunk)
   constexpr int kGroupF4 = KZ * (kJY + 2) * 32 + KZ * kJY * 32 + KZ * kJY * 2 / 4;
   float4* gsm = jsm + threadIdx.z * kGroupF4;
   float4 (*rows)[kJY + 2][32] = reinterpret_cast<float4 (*)[kJY + 2][32]>(gsm);               // [KZ][kJY + 2][32]
@@ -1030,27 +924,8 @@ k_jacobi_block(const unsigned char* __restrict__ mask, const float* __restrict__
       float rt = __shfl_down_sync(0xffffffffu, ctr.x, 1);
       if (tx == 0) lf = xh[k][ty][0];
       if (tx == 31) rt = xh[k][ty][1];
-      if (in && (mm & 0x01010101u) != 0x01010101u) {
-        const float4 ym = rows[k][ty][tx], yp = rows[k][ty + 2][tx], dv = dvs[k][ty][tx];
-        const float pcv[4] = {ctr.x, ctr.y, ctr.z, ctr.w};
-        const float xm[4] = {lf, ctr.x, ctr.y, ctr.z};
-        const float xp[4] = {ctr.y, ctr.z, ctr.w, rt};
-        const float ymv[4] = {ym.x, ym.y, ym.z, ym.w}, ypv[4] = {yp.x, yp.y, yp.z, yp.w};
-        const float zmv[4] = {below.x, below.y, below.z, below.w}, zpv[4] = {above.x, above.y, above.z, above.w};
-        const float dvv[4] = {dv.x, dv.y, dv.z, dv.w};
-#pragma unroll
-        for (int q = 0; q < 4; q++) {
-          const unsigned m = (mm >> (8 * q)) & 0xFFu;
-          if (m & 1) continue;
-          const float p1 = (m & 2) ? pcv[q] : xm[q];
-          const float p2 = (m & 4) ? pcv[q] : xp[q];
-          const float p3 = (m & 8) ? pcv[q] : ymv[q];
-          const float p4 = (m & 16) ? pcv[q] : ypv[q];
-          const float p5 = (m & 32) ? pcv[q] : zmv[q];
-          const float p6 = (m & 64) ? pcv[q] : zpv[q];
-          out[q] = (p1 + p2 + p3 + p4 + p5 + p6 + dvv[q]) / 6.0f;
-        }
-      }
+      if (in && (mm & 0x01010101u) != 0x01010101u)
+        jacobi_update4<true>(mm, ctr, lf, rt, rows[k][ty][tx], rows[k][ty + 2][tx], below, above, dvs[k][ty][tx], out);
       if (in) {
         const float4 o4 = make_float4(out[0], out[1], out[2], out[3]);
         *(float4*)(cp + k * sz) = o4;
@@ -1229,10 +1104,15 @@ template <typename FT>
 void launch_jacobi_mask(const FT* flags, unsigned char* mask, const Geo& g, cudaStream_t st) {
   TFL_LAUNCH3(k_jacobi_mask, FT, g, st, flags, mask, g);
 }
+namespace {
+// The 4-cell Jacobi kernels load the 4 mask bytes as one word and div and p as float4.
+bool jacobi_aligned(const unsigned char* mask, const float* div, const float* pa, const float* pb) {
+  return (uintptr_t)mask % 4 == 0 && (uintptr_t)div % 16 == 0 && (uintptr_t)pa % 16 == 0 && (uintptr_t)pb % 16 == 0;
+}
+}  // namespace
 void launch_jacobi_iter(const unsigned char* mask, const float* div, const float* prev, float* cur,
                         const Geo& g, cudaStream_t st) {
-  const bool aligned = ((uintptr_t)mask % 4 == 0) && ((uintptr_t)div % 16 == 0) && ((uintptr_t)prev % 16 == 0) &&
-                       ((uintptr_t)cur % 16 == 0);
+  const bool aligned = jacobi_aligned(mask, div, prev, cur);
   // The marching kernel pays off once the fields no longer fit L2 (>= 4M cells); smaller grids keep
   // more CTAs in flight with the flat float4 kernel.  (Tests force it through nx == 128 / 256 shapes
   // with few planes, where both kernels are selected by shape alone.)
@@ -1261,48 +1141,8 @@ void launch_jacobi_iter(const unsigned char* mask, const float* div, const float
   }
   TFL_LAUNCH3(k_jacobi_iter, float, g, st, mask, div, prev, cur, g);
 }
-// `sweeps` Jacobi sweeps in ONE cooperative launch: sweep 0 reads pa and writes pb, sweep 1 the other way, ...
-// (the result is in pb for an odd count).  Returns false when the shape / device does not qualify (the caller
-// then launches one kernel per sweep).
-bool launch_jacobi_sweeps(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int sweeps,
-                          cudaStream_t st) {
-  const bool aligned = ((uintptr_t)mask % 4 == 0) && ((uintptr_t)div % 16 == 0) && ((uintptr_t)pa % 16 == 0) &&
-                       ((uintptr_t)pb % 16 == 0);
-  // fields that sit in L2; larger grids are bandwidth-bound per sweep and do not fit the SMs
-  if (!g.is3d || !aligned || g.nx % 128 != 0 || g.ny % kJY != 0 || g.nz < 4 || g.zlo != 0 || g.zhi != g.nz ||
-      g.n * g.nb > (3LL << 20) || sweeps < 2)
-    return false;
-  const int smem = kJG * (kJZ * (kJY + 2) * 32 + kJZ * kJY * 32) * (int)sizeof(float4);
-  static int capacities[64];         // resident CTAs of this kernel, per device (0: not asked yet, -1: cannot)
-  int dev = 0;
-  cudaGetDevice(&dev);
-  int& capacity = capacities[dev & 63];
-  if (capacity == 0) {
-    int sms = 0, per_sm = 0, coop = 0;
-    cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
-    cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
-    capacity = -1;
-    if (coop && cudaFuncSetAttribute(k_jacobi_resident, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_jacobi_resident, 256 * kJG, smem) == cudaSuccess &&
-        sms * per_sm > 0)
-      capacity = sms * per_sm;
-    cudaGetLastError();
-  }
-  const int nch = (g.nz + kJZ - 1) / kJZ;
-  int nblocks = (g.nx / 128) * (g.ny / kJY) * nch * g.nb;
-  const int ctas = (nblocks + kJG - 1) / kJG;
-  if (ctas > capacity) return false;
-  dim3 block(32, kJY, kJG), grid(ctas, 1, 1);
-  Geo gg = g;
-  void* args[] = {(void*)&mask, (void*)&div, (void*)&pa, (void*)&pb, (void*)&gg, (void*)&sweeps, (void*)&nblocks};
-  if (cudaLaunchCooperativeKernel((const void*)k_jacobi_resident, grid, block, args, smem, st) != cudaSuccess) {
-    cudaGetLastError();
-    return false;
-  }
-  return true;
-}
 namespace {
-// Resident CTAs of k_jacobi_block<KZ> on the current device (0 when it cannot be launched cooperatively).
+// Resident CTAs of k_jacobi_resident<KZ> on the current device (0 when it cannot be launched cooperatively).
 template <int KZ>
 int jacobi_block_capacity(int smem) {
   static int capacities[64];         // per device (0: not asked yet, -1: cannot)
@@ -1314,8 +1154,8 @@ int jacobi_block_capacity(int smem) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
     capacity = -1;
-    if (coop && cudaFuncSetAttribute(k_jacobi_block<KZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_jacobi_block<KZ>, 256 * kJG, smem) == cudaSuccess &&
+    if (coop && cudaFuncSetAttribute(k_jacobi_resident<KZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_jacobi_resident<KZ>, 256 * kJG, smem) == cudaSuccess &&
         sms * per_sm > 0)
       capacity = sms * per_sm;
     cudaGetLastError();
@@ -1333,7 +1173,7 @@ int try_jacobi_block(const unsigned char* mask, const float* div, float* pa, flo
   Geo gg = g;
   void* args[] = {(void*)&mask, (void*)&div, (void*)&pa, (void*)&pb, (void*)&gg, (void*)&z_lo, (void*)&z_hi,
                   (void*)&shr_lo, (void*)&shr_hi, (void*)&sweeps, (void*)&nblocks};
-  if (cudaLaunchCooperativeKernel((const void*)k_jacobi_block<KZ>, grid, block, args, smem, st) != cudaSuccess) {
+  if (cudaLaunchCooperativeKernel((const void*)k_jacobi_resident<KZ>, grid, block, args, smem, st) != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
@@ -1342,9 +1182,8 @@ int try_jacobi_block(const unsigned char* mask, const float* div, float* pa, flo
 }  // namespace
 int launch_jacobi_block(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo,
                         int z_hi, int shr_lo, int shr_hi, int sweeps, bool deep, cudaStream_t st) {
-  const bool aligned = ((uintptr_t)mask % 4 == 0) && ((uintptr_t)div % 16 == 0) && ((uintptr_t)pa % 16 == 0) &&
-                       ((uintptr_t)pb % 16 == 0);
-  if (!g.is3d || !aligned || g.nx % 128 != 0 || g.ny % kJY != 0 || sweeps < 1 || z_lo >= z_hi) return 0;
+  if (!g.is3d || !jacobi_aligned(mask, div, pa, pb) || g.nx % 128 != 0 || g.ny % kJY != 0 || sweeps < 1 || z_lo >= z_hi)
+    return 0;
   // the shallowest block that fits: more, thinner CTAs spread a small range over more SMs
   const int kz = try_jacobi_block<4>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);
   return kz || !deep ? kz : try_jacobi_block<6>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);

@@ -1,6 +1,7 @@
 """Timing of simMethod 'jacobi' on z-slabs at one rank (one GPU): the slab step against tfl_simulate_step, and one block
-of sweeps in the one-launch kernel (k_jacobi_block) against one launch per sweep and the single-GPU solve
-(k_jacobi_resident / k_jacobi_march).  CUDA events, median of --reps after --warmup.  Prints one JSON line per row.
+of sweeps in the one-launch kernel (k_jacobi_resident<KZ>) against one launch per sweep and the single-GPU solve
+(the same kernel for maxIter - 1 sweeps plus one k_jacobi_iter4, or k_jacobi_march).  CUDA events, median of --reps
+after --warmup.  Prints one JSON line per row.
 
     python tests/dbg_slab_jacobi.py [--reps 20] [--warmup 5]
 """

@@ -52,10 +52,10 @@ ROWS = {
     (1028, 3, 3): "long row: 9 quad blocks of bx = 32, the last one partial; 33 x tiles",
     (4, 300, 3): "tall (getDx from y): 38 y tiles",
     (4, 3, 300): "deep (getDx from z): 38 z tiles; the step with quad bx = 1 and 150 z blocks",
-    (128, 8, 4): "k_jacobi_resident with 1 block: three of the CTA's four groups idle",
-    (128, 8, 5): "k_jacobi_resident with 2 blocks, the second a partial z chunk",
-    (128, 24, 4): "k_jacobi_resident with 3 blocks",
-    (256, 8, 4): "k_jacobi_resident with 2 x blocks",
+    (128, 8, 4): "k_jacobi_resident<4> with 1 block: three of the CTA's four groups idle",
+    (128, 8, 5): "k_jacobi_resident<4> with 2 blocks, the second a partial z chunk",
+    (128, 24, 4): "k_jacobi_resident<4> with 3 blocks",
+    (256, 8, 4): "k_jacobi_resident<4> with 2 x blocks",
     (128, 8, 8): "k_jacobi_march at its smallest depth (1 and 2 sweeps; more run resident)",
     (3, 3, 1): "2-D per-voxel kernels, one interior cell",
     (5, 3, 1): "2-D: a 3-cell line (PCG without preconditioner)",
@@ -79,8 +79,8 @@ def tile_kernel(shape, nb):
 
 
 def resident_blocks(shape, nb):
-    """Blocks (128 x 8 x 4 cells) of k_jacobi_resident under launch_jacobi_sweeps, 0 where it refuses the grid.
-    It runs for pTol == 0 and maxIter > 2 (tfl_solve_linear_system_jacobi)."""
+    """Blocks (128 x 8 x 4 cells) of k_jacobi_resident<4> in the whole-grid solve, 0 where it refuses the grid.
+    It runs for pTol == 0 and maxIter > 2 (tfl_solve_linear_system_jacobi, through launch_jacobi_block)."""
     nx, ny, nz = shape
     if nz == 1 or nx % 128 or ny % 8 or nz < 4 or nx * ny * nz * nb > (3 << 20):
         return 0
