@@ -68,6 +68,7 @@ SYMBOLS = [
     "tfl_slab_sim_layout", "tfl_slab_sim_upload", "tfl_slab_sim_download", "tfl_slab_sim_step",
     "tfl_slab_sim_exchange_stats", "tfl_slab_sim_ipc_export", "tfl_slab_sim_ipc_connect",
     "tfl_slab_sim_jacobi_stats", "tfl_slab_jacobi_schedule", "tfl_jacobi_slab_block", "tfl_slab_cnn_margin",
+    "tfl_recorder_create", "tfl_recorder_destroy", "tfl_recorder_capture", "tfl_recorder_take", "tfl_recorder_release",
 ]
 JACOBI_BLOCK_INTS = 6
 COMM_ID_BYTES = 128
@@ -191,5 +192,11 @@ def load():
                                           C.c_int32, C.c_int32, C.POINTER(C.c_int32)]
     lib.tfl_alloc_host.argtypes = [C.c_void_p, C.c_size_t, C.POINTER(C.c_void_p)]
     lib.tfl_free_host.argtypes = [C.c_void_p, C.c_void_p]
+    lib.tfl_recorder_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+    lib.tfl_recorder_destroy.argtypes = [C.c_void_p, C.c_void_p]
+    lib.tfl_recorder_capture.argtypes = [C.c_void_p, C.c_void_p, G, C.POINTER(C.c_int64)]
+    lib.tfl_recorder_take.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_float)),
+                                      C.POINTER(C.c_int64)]
+    lib.tfl_recorder_release.argtypes = [C.c_void_p, C.c_void_p]
     _lib = lib
     return lib

@@ -71,6 +71,12 @@ class VboxWriter:
         assert a.shape == self.shape, (a.shape, self.shape)
         np.ascontiguousarray(a.transpose(2, 1, 0)).tofile(self.f)      # permute(3, 2, 1): x slowest
 
+    def write_packed(self, frame):
+        """One frame already in file order, [x][y][z] (a record.FrameRecorder frame)."""
+        a = np.asarray(frame)
+        assert a.dtype == np.float32 and a.shape == self.shape[::-1], (a.dtype, a.shape, self.shape[::-1])
+        np.ascontiguousarray(a).tofile(self.f)
+
     def close(self):
         self.f.close()
 
@@ -133,3 +139,72 @@ def load_binvox(path):
     vol = data[:count_total].reshape(dims[0], dims[1], dims[2]).transpose(0, 2, 1)
     return {"dims": dims, "translation": translation, "scale": scale,
             "data": np.ascontiguousarray(vol, np.float32)}
+
+
+# ---- placing a voxelised obstacle in a domain (torch/lib/voxel_utils.lua), restated literally: the demo's scenes
+# (torch/fluid_net_3d_sim.lua:92-132) are built with these.  Volumes are 3-D arrays indexed [d1][d2][d3] like the
+# Torch tensors (Lua's dims 1, 2, 3); the demo's padded volume is [z][y][x] of the grid.
+
+def calculate_bounding_box(voxels):
+    """tfluids.calculateBoundingBox (voxel_utils.lua:20-50): {'min': [m1, m2, m3], 'max': [M1, M2, M3]}, per axis the
+    first and last 1-based index whose slab (the sum over the other two axes) is non-zero.  An empty volume fails the
+    reference's assertion."""
+    v = np.asarray(voxels)
+    assert v.ndim == 3
+
+    def first_last_nonzero(data):
+        nz = np.flatnonzero(data != 0)
+        return (int(nz[0]) + 1, int(nz[-1]) + 1) if nz.size else (None, None)
+
+    # the reference's xmin / ymin / zmin are Lua dims 1 / 2 / 3 (voxels:sum(2):sum(3), :sum(1):sum(3), :sum(1):sum(2))
+    s = v.astype(np.float64)
+    mins, maxs = [], []
+    for axis in range(3):
+        lo, hi = first_last_nonzero(s.sum(axis=tuple(a for a in range(3) if a != axis)))
+        mins.append(lo)
+        maxs.append(hi)
+    assert s.sum() > 0                       # make sure the volume wasn't empty
+    return {"min": mins, "max": maxs}
+
+
+def pad_voxels_to_dims(width, height, depth, voxels, offsetX, offsetY, offsetZ):
+    """tfluids.padVoxelsToDims (voxel_utils.lua:176-203): the volume trimmed to its bounding box and pasted into a
+    zeroed [depth][height][width] grid, before-padding max(floor((extent - size) / 2 + offset), 1) per axis (x: width,
+    Lua dim 3; y: height, dim 2; z: depth, dim 1).  Offsets may be negative or fractional; the clamp keeps at least one
+    empty plane before the volume.  A paste that would reach past the grid fails (the reference's tensor indexing
+    does); the reference's closing check that no voxel was lost is kept."""
+    v = np.asarray(voxels)
+    assert v.ndim == 3
+    assert v.shape[0] <= depth and v.shape[1] <= height and v.shape[2] <= width
+    bbox = calculate_bounding_box(v)
+    (a1, a2, a3), (b1, b2, b3) = bbox["min"], bbox["max"]
+    v = np.ascontiguousarray(v[a1 - 1:b1, a2 - 1:b2, a3 - 1:b3])
+    pad_lft = max(int(np.floor((width - v.shape[2]) / 2 + offsetX)), 1)
+    pad_bot = max(int(np.floor((height - v.shape[1]) / 2 + offsetY)), 1)
+    pad_bck = max(int(np.floor((depth - v.shape[0]) / 2 + offsetZ)), 1)
+    for pad, size, extent, name in ((pad_bck, v.shape[0], depth, "depth"), (pad_bot, v.shape[1], height, "height"),
+                                    (pad_lft, v.shape[2], width, "width")):
+        if pad + size > extent:
+            raise IndexError("padVoxelsToDims: the volume (%d cells after %d of padding) does not fit the %s %d"
+                             % (size, pad, name, extent))
+    ret = np.zeros((depth, height, width), v.dtype)
+    ret[pad_bck:pad_bck + v.shape[0], pad_bot:pad_bot + v.shape[1], pad_lft:pad_lft + v.shape[2]] = v
+    assert ret.sum(dtype=np.float64) == v.sum(dtype=np.float64), "Lost some voxels."
+    return ret
+
+
+def flip_diagonal(voxels, axis):
+    """tfluids.flipDiagonal (voxel_utils.lua:225-277), in place: axis 0 swaps Lua dims 2 and 3 (needs them equal),
+    axis 1 dims 1 and 3, axis 2 dims 1 and 2.  Returns `voxels`."""
+    dims = voxels.shape
+    assert len(dims) == 3
+    assert 0 <= axis <= 2
+    if axis == 0:
+        assert dims[1] == dims[2]
+    elif axis == 1:
+        assert dims[0] == dims[2]
+    else:
+        assert dims[0] == dims[1]
+    perm = {0: (0, 2, 1), 1: (2, 1, 0), 2: (1, 0, 2)}[axis]
+    voxels[...] = np.ascontiguousarray(voxels.transpose(perm))
+    return voxels

@@ -114,6 +114,12 @@ int tfl_slab_cnn_margin(int32_t banks_num);
 int tfl_jacobi_slab_block(tfl_ctx*, const tfl_grid* pa, const tfl_grid* pb, const tfl_grid* flags,
                           const tfl_grid* div, int is_3d, int32_t z_lo, int32_t z_hi, int32_t shrink_lo,
                           int32_t shrink_hi, int32_t sweeps, int32_t path, int32_t* path_out);
+typedef struct tfl_recorder tfl_recorder;
+int tfl_recorder_create(tfl_ctx*, int32_t nz, int32_t ny, int32_t nx, int32_t slots, tfl_recorder** out);
+void tfl_recorder_destroy(tfl_ctx*, tfl_recorder* rec);
+int tfl_recorder_capture(tfl_ctx*, tfl_recorder* rec, const tfl_grid* field, int64_t* frame_out);
+int tfl_recorder_take(tfl_ctx*, tfl_recorder* rec, int wait, const float** host_out, int64_t* frame_out);
+int tfl_recorder_release(tfl_ctx*, tfl_recorder* rec);
 ]]
 
 local lib = ffi.load('tfl')          -- libtfl.so on the library path
@@ -367,6 +373,27 @@ function tfluids.slabCnnMargin(banksNum)             -- smallest slab margin of 
   assert(m > 0, 'slabCnnMargin: banksNum above 8')
   return m
 end
+
+-- ---- density frames to the host behind the running step (the demo's save branch, fluid_net_3d_sim.lua:266-291) ----
+-- A frame is nx * ny * nz floats in .vbox order (x slowest); the pointer stays valid until recorderRelease.
+function tfluids.recorderCreate(nz, ny, nx, slots)
+  local r = ffi.new('tfl_recorder*[1]')
+  check(lib.tfl_recorder_create(ctx, nz, ny, nx, slots or 3, r))
+  return r[0]
+end
+function tfluids.recorderCapture(rec, field)       -- enqueued on the context's stream; never waits
+  local idx = ffi.new('int64_t[1]')
+  check(lib.tfl_recorder_capture(ctx, rec, field.c, idx))
+  return tonumber(idx[0])
+end
+function tfluids.recorderTake(rec, wait)           -- -> frame index, const float* (nil, nil: not landed yet)
+  local ptr, idx = ffi.new('const float*[1]'), ffi.new('int64_t[1]')
+  check(lib.tfl_recorder_take(ctx, rec, (wait == nil or wait) and 1 or 0, ptr, idx))
+  if idx[0] < 0 then return nil, nil end
+  return tonumber(idx[0]), ptr[0]
+end
+function tfluids.recorderRelease(rec) check(lib.tfl_recorder_release(ctx, rec)) end
+function tfluids.recorderDestroy(rec) lib.tfl_recorder_destroy(ctx, rec) end
 
 function tfluids.synchronize() check(lib.tfl_sync(ctx)) end
 

@@ -467,6 +467,29 @@ int tfl_jacobi_slab_block(tfl_ctx* ctx, const tfl_grid* pa, const tfl_grid* pb, 
 #define TFL_IPC_HANDLE_BYTES 64
 int tfl_slab_sim_ipc_export(tfl_ctx* ctx, tfl_slab_sim* sim, char* handle_out /* TFL_IPC_HANDLE_BYTES */);
 int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* sim, const char* handles);
+
+/* ---- frame output behind the running step (the save branch of fluid_net_3d_sim.lua:266-291) ------------------------
+ * A recorder moves a scalar grid [1][1][nz][ny][nx] to the host in `.vbox` order -- the value at (x, y, z) at index
+ * (x * ny + y) * nz + z, the demo's permute(3, 2, 1) -- without stalling the context's stream.
+ * tfl_recorder_create: one device staging frame, `slots` >= 1 pinned host frames, a copy stream and its events; on
+ *   failure *out stays NULL and nothing is kept.
+ * tfl_recorder_capture: enqueues the pack (k_pack_vbox, a bit copy) on the context's current stream, so it sees `field`
+ *   as the stream leaves it; the copy stream then moves the staging frame into the next free slot.  The next pack waits
+ *   on the device for that copy out of the staging frame.  Never synchronises.  *frame_out = the frame's index (0, 1,
+ *   ... per recorder).  Refused before anything is enqueued: every slot holds a frame not yet released, a field that is
+ *   not [1][1][nz][ny][nx] of the recorder (nb > 1, nc > 1 by name), a stream being captured into a graph.
+ * tfl_recorder_take: the oldest captured frame not yet taken.  wait = 1 blocks on that frame's copy only; wait = 0 sets
+ *   *frame_out = -1 and *host_out = NULL if the copy has not landed.  Fails at once, without waiting, when no captured
+ *   frame is left.  *host_out (pinned, nx * ny * nz floats) stays valid until the frame is released.
+ * tfl_recorder_release: gives back the oldest taken frame's slot (strictly first in, first out); fails if none is taken.
+ * tfl_recorder_destroy: waits for the copies in flight, then frees everything.
+ * Cost: k_pack_vbox moves 8 bytes per cell; the copy runs beside the following steps (DESIGN.md section 6a). */
+typedef struct tfl_recorder tfl_recorder;
+int tfl_recorder_create(tfl_ctx* ctx, int32_t nz, int32_t ny, int32_t nx, int32_t slots, tfl_recorder** out);
+void tfl_recorder_destroy(tfl_ctx* ctx, tfl_recorder* rec);
+int tfl_recorder_capture(tfl_ctx* ctx, tfl_recorder* rec, const tfl_grid* field, int64_t* frame_out);
+int tfl_recorder_take(tfl_ctx* ctx, tfl_recorder* rec, int wait, const float** host_out, int64_t* frame_out);
+int tfl_recorder_release(tfl_ctx* ctx, tfl_recorder* rec);
 #ifdef __cplusplus
 }
 #endif
