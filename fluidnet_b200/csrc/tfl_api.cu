@@ -89,6 +89,7 @@ int advect_vel_dispatch(tfl_ctx* ctx, float dt, const float* U, const FT* flags,
                         const Geo& gf, cudaStream_t st) {
   const bool ours = method == TFL_ADVECT_MACCORMACK_OURS || method == TFL_ADVECT_RK2_OURS || method == TFL_ADVECT_RK3_OURS;
   auto& tl = ctx->tile;
+  tl.last_vel_halo = 0;
   if (ours && fl8 && clear && tl.mode != 0) {
     if (!tl.dev || !tl.host) {
       if (!tl.dev) tl.dev = dev_alloc<unsigned int>(1);
@@ -103,6 +104,7 @@ int advect_vel_dispatch(tfl_ctx* ctx, float dt, const float* U, const FT* flags,
       if (tl.timed) cudaEventRecord(tl.ev1.get(), st);
       if (launched) {
         cudaMemcpyAsync(tl.host.get(), tl.dev.get(), sizeof(unsigned int), cudaMemcpyDeviceToHost, st);
+        tl.last_vel_halo = hf;
         return 1;
       }
     }
@@ -114,10 +116,13 @@ template <typename FT>
 int advect_scalar_dispatch(tfl_ctx* ctx, float dt, const float* s, const float* U, const FT* flags,
                            const unsigned char* fl8, const unsigned char* clear, int method, int outside, float strength,
                            float* dst, float* fwd, float* fwd_pos, const Geo& g, const Geo& gf, cudaStream_t st) {
+  ctx->tile.last_scalar_halo = 0;
   if (method == TFL_ADVECT_MACCORMACK_OURS && fl8 && clear && ctx->tile.mode != 0) {
     const int hf = tile_halo_choice(ctx, false);
-    if (hf > 0 && launch_advect_scalar_tile(dt, s, U, fl8, clear, outside, strength, dst, g, hf, ctx->tile.variant, st))
+    if (hf > 0 && launch_advect_scalar_tile(dt, s, U, fl8, clear, outside, strength, dst, g, hf, ctx->tile.variant, st)) {
+      ctx->tile.last_scalar_halo = hf;
       return 1;
+    }
   }
   return launch_advect_scalar(dt, s, U, flags, clear, method, outside, strength, dst, fwd, fwd_pos, g, gf, st);
 }
@@ -787,6 +792,21 @@ int tfl_debug_advect_tile(tfl_ctx* ctx, int mode, int variant) {
   if (!ctx) return 1;
   ctx->tile.mode = mode;
   ctx->tile.variant = variant;
+  return 0;
+}
+
+// Undocumented debugging hook, read-only: the tile halo the last advectVel and advectScalar dispatches launched
+// (0: the per-pass kernels ran) and the longest trace in the pinned telemetry word, which the next automatic choice
+// reads (synchronise first for the last call's value).  Launches nothing.
+int tfl_debug_advect_tile_used(tfl_ctx* ctx, int32_t* vel_halo, int32_t* scalar_halo, float* longest) {
+  if (!ctx || !vel_halo || !scalar_halo || !longest) return 1;
+  *vel_halo = ctx->tile.last_vel_halo;
+  *scalar_halo = ctx->tile.last_scalar_halo;
+  *longest = 0.0f;
+  if (ctx->tile.host) {
+    const unsigned int bits = *(volatile unsigned int*)ctx->tile.host.get();
+    memcpy(longest, &bits, 4);
+  }
   return 0;
 }
 

@@ -31,6 +31,10 @@ struct Geo {
   int nc;                // velocity channels (3 or 2)
   long long n;           // cells per (batch, channel) = nx*ny*nz
   unsigned long long* faults;   // device counter (trace faults / slab overruns)
+  // Local planes out of reach at the low / high end, on top of the storage bounds: an access there is a fault.
+  // Non-zero only for the backward pass of a z-slab's MacCormack advection, whose forward field holds just the
+  // planes the forward pass computed (the slab margin around the owned ones).
+  int skip_lo = 0, skip_hi = 0;
 };
 
 struct V3 { float x, y, z; };
@@ -78,13 +82,20 @@ __device__ __forceinline__ int clamp_i(int x, int lo, int hi) {
 __device__ __forceinline__ void note_fault(const Geo& g) {
   if (g.faults) atomicAdd(g.faults, 1ULL);
 }
-// Local plane of a global z index; records a fault (and clamps) if the slab halo is
-// too small for the access.
+// Local plane of a global z index; records a fault (and clamps) if the slab halo, or the
+// planes in reach (skip_lo / skip_hi), are too small for the access.
+// Clearance of a cell on local plane k, capped at its distance to the planes out of reach as the clearance field
+// is capped at the ends of the local storage: the fast path of a cell with clearance never reads past them.
+__device__ __forceinline__ int clear_in_reach(const Geo& g, int clr, int k) {
+  if ((g.skip_lo | g.skip_hi) == 0) return clr;
+  const int lo = k - g.skip_lo, hi = g.nz - 1 - g.skip_hi - k;
+  return clr < lo ? (clr < hi ? clr : hi) : (lo < hi ? lo : hi);
+}
 __device__ __forceinline__ int local_z(const Geo& g, int kg) {
   int k = kg - g.zoff;
-  if (k < 0 || k >= g.nz) {
+  if (k < g.skip_lo || k >= g.nz - g.skip_hi) {
     note_fault(g);
-    k = k < 0 ? 0 : g.nz - 1;
+    k = k < g.skip_lo ? g.skip_lo : g.nz - g.skip_hi - 1;
   }
   return k;
 }
@@ -121,7 +132,10 @@ __device__ __forceinline__ Lerp build_index(const Geo& g, V3 pos) {
 __device__ __forceinline__ int corner(const Geo& g, const Lerp& q) {
   int kl = q.zi - g.zoff;
   if (g.is3d) {
-    if (kl < 0 || kl + 1 >= g.nz) { note_fault(g); kl = kl < 0 ? 0 : g.nz - 2; }
+    if (kl < g.skip_lo || kl + 1 >= g.nz - g.skip_hi) {
+      note_fault(g);
+      kl = kl < g.skip_lo ? g.skip_lo : g.nz - g.skip_hi - 2;
+    }
   } else {
     kl = 0;
   }

@@ -370,7 +370,7 @@ __global__ void k_advect_scalar_pass2_ours(const float* __restrict__ s, const fl
   const float* sb = s + b * g.n;
   const float* fb = fwd + b * g.n;
   const float fw = __ldg(fb + c);
-  const int clr = cl ? (int)__ldg(cl + c) : 0;
+  const int clr = cl ? clear_in_reach(g, (int)__ldg(cl + c), k) : 0;
   const bool border = clr > 0 ? false : on_border(g, k, j, i);
   float bw = 0.0f;
   if (clr > 0)
@@ -593,7 +593,7 @@ __global__ void __launch_bounds__(256, TFL_ADVECT_MINB2) k_advect_vel_pass2(cons
   const float* ub = U + (long long)b * g.nc * g.n;
   const float* fb = fwd + (long long)b * g.nc * g.n;
   float* db = dst + (long long)b * g.nc * g.n + c;
-  const int clr = (OURS && clear) ? (int)__ldg(clear + b * g.n + c) : 0;
+  const int clr = (OURS && clear) ? clear_in_reach(g, (int)__ldg(clear + b * g.n + c), k) : 0;
   if (clr > 0) {
     // Fluid cell of the interior.  clr >= 2: its 26 neighbours are fluid, no face is skipped by the
     // correction; clr == 1: the three lower neighbours decide.
@@ -1048,10 +1048,20 @@ int launch_vorticity(float* U, const FT* flags, float strength, float* curl, flo
   return 3;
 }
 
+// Geometry of a MacCormack backward pass: the planes the forward pass (g_fwd) did not compute are out of reach, so a
+// trace longer than the z-slab margin counts a fault instead of reading a forward value that was never written.
+static Geo backward_geo(const Geo& g, const Geo& g_fwd) {
+  Geo gb = g;
+  gb.skip_lo = g_fwd.zlo;
+  gb.skip_hi = g.nz - g_fwd.zhi;
+  return gb;
+}
+
 template <typename FT>
 int launch_advect_scalar(float dt, const float* s, const float* U, const FT* flags, const unsigned char* clear,
                          int method, int outside, float strength, float* dst, float* fwd, float* fwd_pos,
                          const Geo& g, const Geo& g_fwd, cudaStream_t st) {
+  const Geo gb = backward_geo(g, g_fwd);
   switch (method) {
     case TFL_ADVECT_EULER:
       TFL_LAUNCH3X(k_advect_scalar_pass1, FT, TFL_ADVECT_EULER, g, st, s, U, flags, clear, dst, nullptr, dt, outside, g);
@@ -1067,11 +1077,11 @@ int launch_advect_scalar(float dt, const float* s, const float* U, const FT* fla
       return 1;
     case TFL_ADVECT_MACCORMACK:
       TFL_LAUNCH3X(k_advect_scalar_pass1, FT, TFL_ADVECT_MACCORMACK, g_fwd, st, s, U, flags, clear, fwd, nullptr, dt, outside, g_fwd);
-      TFL_LAUNCH3(k_advect_scalar_pass2_manta, FT, g, st, s, fwd, U, flags, dst, dt, strength, g);
+      TFL_LAUNCH3(k_advect_scalar_pass2_manta, FT, gb, st, s, fwd, U, flags, dst, dt, strength, gb);
       return 2;
     case TFL_ADVECT_MACCORMACK_OURS:
       TFL_LAUNCH3X(k_advect_scalar_pass1, FT, TFL_ADVECT_MACCORMACK_OURS, g_fwd, st, s, U, flags, clear, fwd, fwd_pos, dt, outside, g_fwd);
-      TFL_LAUNCH3(k_advect_scalar_pass2_ours, FT, g, st, s, fwd, fwd_pos, U, flags, clear, dst, dt, strength, outside, g);
+      TFL_LAUNCH3(k_advect_scalar_pass2_ours, FT, gb, st, s, fwd, fwd_pos, U, flags, clear, dst, dt, strength, outside, gb);
       return 2;
   }
   return -1;
@@ -1081,6 +1091,7 @@ template <typename FT>
 int launch_advect_vel(float dt, const float* U, const FT* flags, const unsigned char* clear, int method,
                       float strength, float* dst, float* fwd, const Geo& g, const Geo& g_fwd, cudaStream_t st) {
   if (method == TFL_ADVECT_RK2_OURS || method == TFL_ADVECT_RK3_OURS) method = TFL_ADVECT_MACCORMACK_OURS;
+  const Geo gb = backward_geo(g, g_fwd);
   switch (method) {
     case TFL_ADVECT_EULER:
       TFL_LAUNCH3X(k_advect_vel_pass1, FT, false, g, st, U, flags, clear, dst, dt, g);
@@ -1090,11 +1101,11 @@ int launch_advect_vel(float dt, const float* U, const FT* flags, const unsigned 
       return 1;
     case TFL_ADVECT_MACCORMACK:
       TFL_LAUNCH3X(k_advect_vel_pass1, FT, false, g_fwd, st, U, flags, clear, fwd, dt, g_fwd);
-      TFL_LAUNCH3X(k_advect_vel_pass2, FT, false, g, st, U, fwd, flags, clear, dst, dt, strength, g);
+      TFL_LAUNCH3X(k_advect_vel_pass2, FT, false, gb, st, U, fwd, flags, clear, dst, dt, strength, gb);
       return 2;
     case TFL_ADVECT_MACCORMACK_OURS:
       TFL_LAUNCH3X(k_advect_vel_pass1, FT, true, g_fwd, st, U, flags, clear, fwd, dt, g_fwd);
-      TFL_LAUNCH3X(k_advect_vel_pass2, FT, true, g, st, U, fwd, flags, clear, dst, dt, strength, g);
+      TFL_LAUNCH3X(k_advect_vel_pass2, FT, true, gb, st, U, fwd, flags, clear, dst, dt, strength, gb);
       return 2;
   }
   return -1;
