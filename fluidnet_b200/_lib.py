@@ -63,7 +63,7 @@ SYMBOLS = [
     "tfl_velocity_update_backward", "tfl_volumetric_up_sampling_nearest_backward", "tfl_empty_domain", "tfl_flags_to_occupancy", "tfl_apply_bc",
     "tfl_clamp", "tfl_cnn_create", "tfl_cnn_create_graph", "tfl_cnn_create_banked", "tfl_cnn_create_model", "tfl_cnn_create_model_ex", "tfl_cnn_create_model_norm", "tfl_cnn_destroy", "tfl_cnn_set_mode", "tfl_cnn_get_mode", "tfl_cnn_project", "tfl_simulate_step",
     "tfl_host_sim_create", "tfl_host_sim_destroy", "tfl_host_sim_step",
-    "tfl_step_graph_create", "tfl_step_graph_launch", "tfl_step_graph_destroy",
+    "tfl_step_graph_create", "tfl_step_graph_launch", "tfl_step_graph_pcg_status", "tfl_step_graph_destroy",
     "tfl_comm_unique_id", "tfl_comm_init", "tfl_comm_destroy", "tfl_slab_sim_create", "tfl_slab_sim_destroy",
     "tfl_slab_sim_layout", "tfl_slab_sim_upload", "tfl_slab_sim_download", "tfl_slab_sim_step",
     "tfl_slab_sim_exchange_stats", "tfl_slab_sim_ipc_export", "tfl_slab_sim_ipc_connect",
@@ -169,6 +169,7 @@ def load():
                                       C.POINTER(MConf), C.c_void_p]
     lib.tfl_step_graph_create.argtypes = [C.c_void_p, C.POINTER(State), C.POINTER(MConf), C.c_void_p, C.POINTER(C.c_void_p)]
     lib.tfl_step_graph_launch.argtypes = [C.c_void_p, C.c_void_p]
+    lib.tfl_step_graph_pcg_status.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
     lib.tfl_step_graph_destroy.argtypes = [C.c_void_p, C.c_void_p]
     lib.tfl_comm_unique_id.argtypes = [C.c_void_p, C.c_char_p]
     lib.tfl_comm_init.argtypes = [C.c_void_p, C.c_char_p, C.c_int32, C.c_int32]

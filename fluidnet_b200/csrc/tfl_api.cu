@@ -612,9 +612,12 @@ int tfl_solve_linear_system_pcg(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid*
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (pcg_check_args(ctx, p, "p", flags, div, "div", is_3d, precond)) return 1;
-  const int rc = pcg_solve(ctx->pcg, ctx->arena.get(), p->data, flags->data, div->data, flags->nb, flags->nz, flags->ny,
-                           flags->nx, is_3d, precond, tol, max_iter, residual, iterations, &ctx->launches,
-                           ctx->stream);
+  const int rc =
+      ctx->pcg_graph
+          ? pcg_solve_graph(*ctx->pcg_graph, ctx->pcg, ctx->arena.get(), p->data, flags->data, div->data, flags->nb,
+                            flags->nz, flags->ny, flags->nx, is_3d, precond, tol, max_iter, &ctx->launches, ctx->stream)
+          : pcg_solve(ctx->pcg, ctx->arena.get(), p->data, flags->data, div->data, flags->nb, flags->nz, flags->ny,
+                      flags->nx, is_3d, precond, tol, max_iter, residual, iterations, &ctx->launches, ctx->stream);
   return pcg_report(ctx, rc, "solveLinearSystemPCG");
 }
 
@@ -1119,11 +1122,15 @@ int tfl_host_sim_step(tfl_ctx* ctx, tfl_host_sim* hs, float* p, float* U, float*
 // The graph also holds pointers into buffers the library owns: the context's scratch arena and flag cache, and
 // the model's activation buffers.  Each carries a generation counter; a launch after any of them was reallocated
 // is refused (the replay would read and write freed memory).
+// A PCG step's solve is captured by pcg_solve_graph: its iteration loop is a conditional node the device re-arms,
+// and its per-component scalars, progress words and result words are the graph's own (PcgGraphScratch), allocated
+// before the capture for the most components the grid can hold.
 // ---------------------------------------------------------------------------------------
 struct tfl_step_graph {
+  PcgGraphScratch pcg;          // declared first: released after the executable graph that uses it
   GraphPtr graph;
   GraphExecPtr exec;
-  long long launches = 0;       // kernels in one replay
+  long long launches = 0;       // kernels in one replay outside the PCG loop
   unsigned long long arena_gen = 0, fcache_gen = 0, act_gen = 0;   // generations of the captured buffers
   tfl_cnn* cnn = nullptr;       // the captured model (its act_gen is checked), or null
 };
@@ -1146,14 +1153,25 @@ int tfl_step_graph_create(tfl_ctx* ctx, const tfl_state* state, const tfl_mconf*
   cudaStream_t st = ctx->stream;
   if (st == nullptr || st == cudaStreamLegacy || st == cudaStreamPerThread)
     return fail(ctx, "step_graph: the default stream cannot be captured; give the context a stream (tfl_set_stream)");
+  std::unique_ptr<tfl_step_graph> g(new tfl_step_graph());
+  const bool pcg = mc->sim_method == TFL_SIM_PCG;
+  if (pcg) {              // the limits of the direct solve, by name, before anything is allocated or captured
+    if (check_scalar(ctx, &state->flags, "flags")) return 1;
+    if (ctx->slab) return fail(ctx, "step_graph: PCG does not shard (triangular solves): single GPU only");
+    const tfl_grid& f = state->flags;
+    const int prc = pcg_graph_alloc(g->pcg, ctx->pcg, f.nb, f.nz, f.ny, f.nx, state->U.nc == 3);
+    if (prc == 4) return fail(ctx, "step_graph: %s", pcg_status_string(prc));
+    if (prc) return fail(ctx, "step_graph: PCG buffers: %s", cudaGetErrorString(cudaGetLastError()));
+  }
   TFL_CUDA(ctx, cudaStreamSynchronize(st));
   const long long l0 = ctx->launches;
   if (cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
     cudaGetLastError();
     return fail(ctx, "step_graph: cudaStreamBeginCapture failed");
   }
+  ctx->pcg_graph = pcg ? &g->pcg : nullptr;
   const int rc = tfl_simulate_step(ctx, state, mc, cnn);
-  std::unique_ptr<tfl_step_graph> g(new tfl_step_graph());
+  ctx->pcg_graph = nullptr;
   cudaGraph_t graph = nullptr;
   const cudaError_t e = cudaStreamEndCapture(st, &graph);
   g->graph.reset(graph);
@@ -1191,6 +1209,32 @@ int tfl_step_graph_launch(tfl_ctx* ctx, tfl_step_graph* g) {
                      "larger grid); replaying would touch freed memory: capture the step again", stale);
   TFL_CUDA(ctx, cudaGraphLaunch(g->exec.get(), ctx->stream));
   ctx->launches += g->launches;
+  return 0;
+}
+
+int tfl_step_graph_pcg_status(tfl_ctx* ctx, tfl_step_graph* g, float* residual, int32_t* iterations) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!g || !g->exec) return fail(ctx, "step_graph is nil");
+  if (!g->pcg.captured) {
+    if (iterations) *iterations = -1;
+    return 0;
+  }
+  int w[8];
+  cudaStream_t st = ctx->stream;
+  TFL_CUDA(ctx, cudaMemcpyAsync(w, g->pcg.words.get(), sizeof(w), cudaMemcpyDeviceToHost, st));
+  // the error has been read and the passes counted: both start again from here
+  TFL_CUDA(ctx, cudaMemsetAsync(g->pcg.words.get(), 0, sizeof(int), st));
+  TFL_CUDA(ctx, cudaMemsetAsync(g->pcg.words.get() + 4, 0, sizeof(unsigned long long), st));
+  TFL_CUDA(ctx, cudaStreamSynchronize(st));
+  unsigned long long passes = 0;
+  memcpy(&passes, w + 4, sizeof(passes));
+  ctx->launches += (long long)passes * g->pcg.body_launches;
+  if (w[0]) return fail(ctx, "%s", pcg_status_string(w[0]));
+  float res;
+  memcpy(&res, w + 2, sizeof(res));
+  if (residual) *residual = res;
+  if (iterations) *iterations = w[1];
   return 0;
 }
 

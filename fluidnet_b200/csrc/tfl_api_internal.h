@@ -50,6 +50,7 @@ struct tfl_ctx {
     bool density_sent = false;
   } ov;
   PcgScratch pcg;                           // grow-only buffers of the PCG solve
+  PcgGraphScratch* pcg_graph = nullptr;     // set while tfl_step_graph_create captures: PCG solves are captured there
   // Byte copy of the step's flags and their clearance field (advection fast path), kept between steps:
   // each step re-derives the bytes, compares them with the copy on the device and rebuilds the
   // clearance only if something changed (no host round trip).

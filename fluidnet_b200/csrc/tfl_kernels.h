@@ -166,12 +166,35 @@ struct PcgScratch {            // owned by the context, grow-only
   void* debug_timing = nullptr;   // debug: device buffer [chunks][4] of sweep timestamps
   int groups_override = 0;     // debug: planes per CTA of the sweep kernel (0 = as many as fit)
 };
+// What a PCG solve captured into a step graph uses besides the arena (pcg_solve_graph): owned by the graph and sized
+// for the worst case before the capture, so replays never allocate and share no per-component scalars or progress
+// words with direct solves or with other graphs.
+struct PcgGraphScratch {
+  DevPtr<char> comp_buf;       // per-component CG scalars of up to comp_cap components
+  long long comp_cap = 0;      // floor(cells / 2): every component of the system has at least two cells
+  DevPtr<unsigned long long> prog;   // progress words of the captured sweeps, [2][chunks]
+  long long prog_words = 0;
+  // [0] status of the first failed solve since the last read (pcg_status_string, sticky), [1] iterations and [2]
+  // residual (float bits) of the last solve, [4..5] passes of the loop body since the last read (u64)
+  DevPtr<int> words;
+  StreamPtr body_stream;       // captures the loop body
+  long long body_launches = 0; // kernels in one pass of the loop body
+  bool captured = false;       // a solve was captured
+};
 size_t pcg_workspace_bytes(int nb, int nz, int ny, int nx);
 const char* pcg_status_string(int rc);
 // precond: 0 none, 1 ilu0, 2 ic0.  Returns 0 or a status for pcg_status_string.  Synchronises `st`.
 int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, const float* div, int nb, int nz, int ny,
               int nx, int is3d, int precond, float tol, int max_iter, float* residual, int* iterations,
               long long* launches, cudaStream_t st);
+// Allocates gs for solves on this grid (before a capture: status 4 for ny > 960, 3 for a CUDA failure).
+int pcg_graph_alloc(PcgGraphScratch& gs, PcgScratch& sc, int nb, int nz, int ny, int nx, int is3d);
+// pcg_solve for a stream being captured: the same kernels per iteration, no host read.  The iteration loop is a
+// conditional WHILE node whose body the device re-arms; the result goes to gs.words.  `launches` gets the kernels
+// outside the loop, gs.body_launches those of one pass of the body.
+int pcg_solve_graph(PcgGraphScratch& gs, PcgScratch& sc, void* workspace, float* p, const float* flags,
+                    const float* div, int nb, int nz, int ny, int nx, int is3d, int precond, float tol, int max_iter,
+                    long long* launches, cudaStream_t st);
 // Debug: the preconditioner alone.  Same labelling, system and sweeps as pcg_solve; z = M^-1 r in the
 // natural layout (0 outside every system of two or more cells); geometry = NYP, planes per CTA,
 // chunks, cooperative grid of the sweeps.  Synchronises `st`.

@@ -264,24 +264,74 @@ __global__ void k_update(const unsigned short* __restrict__ cf, const int* __res
   warp_comp_add(sc.rr_new, a.comp, a.v);
 }
 
-// End of an iteration (or, with `start`, before the first): termination test per component.
-__global__ void k_scalars(CompScalars sc, int ncomp, double tol2, int max_iter, int start, int no_precond) {
-  const int id = blockIdx.x * blockDim.x + threadIdx.x;
-  if (id >= ncomp) return;
-  if (!sc.done[id]) {
-    if (!start) {
-      sc.rz_old[id] = no_precond ? sc.rr_cur[id] : sc.rz_new[id];
-      sc.rr_cur[id] = sc.rr_new[id];
-      sc.iters[id] += 1;
+// End of an iteration (or, with `start`, before the first): termination test per component.  The component count
+// is `ncomp`, or *ncomp_dev when that is given (captured solves, which never read it back to the host).
+__global__ void k_scalars(CompScalars sc, const int* __restrict__ ncomp_dev, int ncomp, double tol2, int max_iter,
+                          int start, int no_precond) {
+  const int n = ncomp_dev ? *ncomp_dev : ncomp;
+  for (int id = blockIdx.x * blockDim.x + threadIdx.x; id < n; id += gridDim.x * blockDim.x) {
+    if (!sc.done[id]) {
+      if (!start) {
+        sc.rz_old[id] = no_precond ? sc.rr_cur[id] : sc.rz_new[id];
+        sc.rr_cur[id] = sc.rr_new[id];
+        sc.iters[id] += 1;
+      }
+      const double rr = sc.rr_cur[id];
+      if (rr != rr) atomicOr(sc.header + 1, 1);
+      if (!(rr > tol2) || sc.iters[id] > max_iter) sc.done[id] = 1;     // while (rr > tol^2 && iter <= maxIter)
+      else atomicAdd(sc.header, 1);
     }
-    const double rr = sc.rr_cur[id];
-    if (rr != rr) atomicOr(sc.header + 1, 1);
-    if (!(rr > tol2) || sc.iters[id] > max_iter) sc.done[id] = 1;     // while (rr > tol^2 && iter <= maxIter)
-    else atomicAdd(sc.header, 1);
+    sc.rz_new[id] = 0.0;
+    sc.pw[id] = 0.0;
+    sc.rr_new[id] = 0.0;
   }
-  sc.rz_new[id] = 0.0;
-  sc.pw[id] = 0.0;
-  sc.rr_new[id] = 0.0;
+}
+
+// ---- the captured solve's own kernels ---------------------------------------------------------
+// Zeroes the scalars of the header[3] components labelling found (a direct solve memsets them, knowing the count).
+__global__ void k_comp_clear(CompScalars sc) {
+  const int n = sc.header[3];
+  for (int id = blockIdx.x * blockDim.x + threadIdx.x; id < n; id += gridDim.x * blockDim.x) {
+    sc.rz_new[id] = 0.0; sc.rz_old[id] = 0.0; sc.pw[id] = 0.0; sc.rr_new[id] = 0.0; sc.rr_cur[id] = 0.0;
+    sc.xsum[id] = 0.0;
+    sc.cnt[id] = 0; sc.done[id] = 0; sc.iters[id] = 0;
+  }
+}
+
+// Sets the WHILE node's condition: another pass while a component is active and no NaN, sweep fault or border cell
+// was seen (what pcg_solve's host loop tests).  `passes` (or null) counts the passes of the body.
+__global__ void k_pcg_continue(const int* __restrict__ header, cudaGraphConditionalHandle loop,
+                               unsigned long long* __restrict__ passes) {
+  const bool more = header[0] > 0 && !header[1] && !header[2] && !header[4];
+  cudaGraphSetConditional(loop, more ? 1u : 0u);
+  if (passes) *passes += 1;
+}
+
+// What pcg_solve reports, into the graph's words: the status (border, then sweep fault, then NaN, as pcg_solve tests
+// them) is kept if no earlier solve's is pending; residual = max over components of (float)sqrt(r.r), -inf without
+// components; iterations = the longest component's.  One block.
+__global__ void k_pcg_finish(CompScalars sc, int* __restrict__ words) {
+  __shared__ float s_res[32];
+  __shared__ int s_it[32];
+  const int n = sc.header[3];
+  float worst = -INFINITY;
+  int worst_it = 0;
+  for (int id = threadIdx.x; id < n; id += blockDim.x) {
+    worst = fmaxf(worst, (float)sqrt(sc.rr_cur[id]));
+    worst_it = max(worst_it, sc.iters[id]);
+  }
+  for (int o = 16; o > 0; o >>= 1) {
+    worst = fmaxf(worst, __shfl_down_sync(0xffffffffu, worst, o));
+    worst_it = max(worst_it, __shfl_down_sync(0xffffffffu, worst_it, o));
+  }
+  if ((threadIdx.x & 31) == 0) { s_res[threadIdx.x >> 5] = worst; s_it[threadIdx.x >> 5] = worst_it; }
+  __syncthreads();
+  if (threadIdx.x != 0) return;
+  for (int w = 1; w < (int)(blockDim.x >> 5); w++) { worst = fmaxf(worst, s_res[w]); worst_it = max(worst_it, s_it[w]); }
+  const int status = sc.header[4] ? 1 : sc.header[2] ? 5 : sc.header[1] ? 2 : 0;
+  if (status && words[0] == 0) words[0] = status;
+  words[1] = worst_it;
+  words[2] = __float_as_int(worst);
 }
 
 __global__ void k_xsum(const unsigned short* __restrict__ cf, const int* __restrict__ comp,
@@ -653,12 +703,8 @@ struct PcgSystem {
 
 #define PCG_CUDA(call) do { if ((call) != cudaSuccess) return 3; } while (0)
 
-// Geometry and launch shape of the sweeps, labelling, and (when there is a system of two or more
-// cells, s.ncomp > 0) the per-component scalars, the progress words and the system arrays.  `out`
-// is zeroed: cells outside every system keep that 0.  Returns 0 or a status for pcg_status_string.
-int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, const float* div, int nb, int nz,
-              int ny, int nx, int is3d, int precond, long long* launches, cudaStream_t st, PcgSystem& s) {
-  PcgGeo& g = s.g;
+// Geometry of the skewed layout and the sweeps' plane chunks.  Returns 0 or 4 (rows too long for a CTA).
+int pcg_geometry(const PcgScratch& sc, int nb, int nz, int ny, int nx, int is3d, PcgGeo& g) {
   g.nx = nx; g.ny = ny; g.nz = nz; g.nb = nb; g.is3d = is3d ? 1 : 0;
   g.S = nx + ny - 1;
   g.NYP = (ny + 31) / 32 * 32;
@@ -672,17 +718,31 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
   if (sc.groups_override > 0 && sc.groups_override < g.GP) g.GP = sc.groups_override;
   if (g.GP > g.P) g.GP = g.P;
   g.chunks = (g.P + g.GP - 1) / g.GP;
-  const long long cells = g.n * nb;
+  return 0;
+}
 
-  if (!sc.sm_count) {
-    int dev = 0, sms = 0;
-    PCG_CUDA(cudaGetDevice(&dev));
-    PCG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
-    if (!(sc.host = pinned_alloc<int>(16))) return 3;
-    PCG_CUDA(cudaFuncSetAttribute(k_sweep<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    PCG_CUDA(cudaFuncSetAttribute(k_sweep<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
-    sc.sm_count = sms;
-  }
+// One-time setup of the scratch: host words, the sweeps' shared-memory limit, the SM count.
+int pcg_init_once(PcgScratch& sc) {
+  if (sc.sm_count) return 0;
+  int dev = 0, sms = 0;
+  PCG_CUDA(cudaGetDevice(&dev));
+  PCG_CUDA(cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev));
+  if (!(sc.host = pinned_alloc<int>(16))) return 3;
+  PCG_CUDA(cudaFuncSetAttribute(k_sweep<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+  PCG_CUDA(cudaFuncSetAttribute(k_sweep<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 160 * 1024));
+  sc.sm_count = sms;
+  return 0;
+}
+
+// What both drivers do first: geometry and launch shape of the sweeps, the workspace carved, and the labelling
+// enqueued (header[3] = components of two or more cells, header[4] = a fluid cell on the border; with one, the union
+// pass does nothing, so every component has one cell and no system is built).
+int pcg_label(PcgScratch& sc, void* workspace, const float* flags, int nb, int nz, int ny, int nx, int is3d,
+              long long* launches, cudaStream_t st, PcgSystem& s) {
+  PcgGeo& g = s.g;
+  if (pcg_geometry(sc, nb, nz, ny, nx, is3d, g)) return 4;
+  const long long cells = g.n * nb;
+  if (pcg_init_once(sc)) return 3;
   s.sweep_threads = g.GP * g.NYP + 64;
   s.sweep_smem = (size_t)g.GP * 2 * (g.NYP + 2) * sizeof(float);
   int occ = 0;
@@ -715,6 +775,52 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
   k_label_flatten<<<blocks_for(cells), 256, 0, st>>>(s.parent, s.csize, g);
   k_label_assign<<<blocks_for(cells), 256, 0, st>>>(s.parent, s.csize, s.cid, g, s.header + 3);
   *launches += 4;
+  return 0;
+}
+
+// The per-component scalars in `buf`, `stride` entries per array.
+CompScalars comp_scalars(char* buf, size_t stride, int* header) {
+  CompScalars cs;
+  double* d = (double*)buf;
+  cs.rz_new = d; cs.rz_old = d + stride; cs.pw = d + 2 * stride; cs.rr_new = d + 3 * stride;
+  cs.rr_cur = d + 4 * stride; cs.xsum = d + 5 * stride;
+  int* q = (int*)(d + 6 * stride);
+  cs.cnt = q; cs.done = q + stride; cs.iters = q + 2 * stride;
+  cs.header = header;
+  return cs;
+}
+constexpr size_t kCompBytes = 6 * 8 + 3 * 4;     // scalars of one component
+
+// The system arrays (cleared, then k_build) and the sweeps' arguments over the progress words `prog` ([2][chunks]);
+// s.cs must be set.
+int pcg_build(PcgScratch& sc, PcgSystem& s, const float* flags, const float* div, int precond,
+              unsigned long long* prog, long long* launches, cudaStream_t st) {
+  const PcgGeo& g = s.g;
+  PCG_CUDA(cudaMemsetAsync(s.cf, 0, g.slots * 2, st));
+  PCG_CUDA(cudaMemsetAsync(s.comp, 0xff, g.slots * 4, st));
+  for (float* v : {s.r, s.z, s.pre, s.p0, s.p1, s.w, s.x}) PCG_CUDA(cudaMemsetAsync(v, 0, g.slots * 4, st));
+  k_build<<<blocks_for(g.n * g.nb), 256, 0, st>>>(flags, div, s.parent, s.csize, s.cid, s.cf, s.comp, s.r, s.cs.cnt,
+                                                  g, precond);
+  *launches += 1;
+
+  SweepArgs& sa = s.sa;
+  sa.cf = s.cf; sa.comp = s.comp; sa.r = s.r; sa.z = s.z; sa.pre = s.pre;
+  sa.prog_f = prog; sa.prog_b = prog + g.chunks;
+  sa.base = 0;
+  sa.rz = s.cs.rz_new; sa.faults = s.header + 2;
+  sa.timing = (unsigned long long*)sc.debug_timing;
+  return 0;
+}
+
+// Labelling, and (when there is a system of two or more cells, s.ncomp > 0) the per-component scalars, the progress
+// words and the system arrays.  `out` is zeroed: cells outside every system keep that 0.  Returns 0 or a status for
+// pcg_status_string.
+int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, const float* div, int nb, int nz,
+              int ny, int nx, int is3d, int precond, long long* launches, cudaStream_t st, PcgSystem& s) {
+  const int rc = pcg_label(sc, workspace, flags, nb, nz, ny, nx, is3d, launches, st, s);
+  if (rc) return rc;
+  const PcgGeo& g = s.g;
+  const long long cells = g.n * nb;
   PCG_CUDA(cudaMemcpyAsync(sc.host.get(), s.header, 32, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
   if (sc.host.get()[4]) return 1;
@@ -722,23 +828,14 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
   PCG_CUDA(cudaMemsetAsync(out, 0, cells * 4, st));                     // :1337
   if (ncomp == 0) return 0;
   // per-component scalars; a capacity is recorded once its buffer exists
-  const size_t per = 6 * 8 + 3 * 4;
-  if ((size_t)ncomp * per + 256 > sc.comp_cap) {
-    const size_t cap = (size_t)ncomp * per * 2 + 4096;
+  if ((size_t)ncomp * kCompBytes + 256 > sc.comp_cap) {
+    const size_t cap = (size_t)ncomp * kCompBytes * 2 + 4096;
     sc.comp_buf = dev_alloc<char>(cap);
     sc.comp_cap = sc.comp_buf ? cap : 0;
     if (!sc.comp_buf) return 3;
   }
-  PCG_CUDA(cudaMemsetAsync(sc.comp_buf.get(), 0, (size_t)ncomp * per + 256, st));
-  CompScalars& cs = s.cs;
-  {
-    double* d = (double*)sc.comp_buf.get();
-    cs.rz_new = d; cs.rz_old = d + ncomp; cs.pw = d + 2 * (size_t)ncomp; cs.rr_new = d + 3 * (size_t)ncomp;
-    cs.rr_cur = d + 4 * (size_t)ncomp; cs.xsum = d + 5 * (size_t)ncomp;
-    int* q = (int*)(d + 6 * (size_t)ncomp);
-    cs.cnt = q; cs.done = q + ncomp; cs.iters = q + 2 * (size_t)ncomp;
-    cs.header = s.header;
-  }
+  PCG_CUDA(cudaMemsetAsync(sc.comp_buf.get(), 0, (size_t)ncomp * kCompBytes + 256, st));
+  s.cs = comp_scalars(sc.comp_buf.get(), (size_t)ncomp, s.header);
   if ((size_t)g.chunks * 2 > sc.prog_cap) {
     const size_t cap = (size_t)g.chunks * 2 + 64;
     sc.prog = dev_alloc<unsigned long long>(cap);
@@ -748,30 +845,22 @@ int pcg_setup(PcgScratch& sc, void* workspace, float* out, const float* flags, c
     sc.prog_cap = cap;
     sc.epoch = 0;
   }
-  // system arrays
-  PCG_CUDA(cudaMemsetAsync(s.cf, 0, g.slots * 2, st));
-  PCG_CUDA(cudaMemsetAsync(s.comp, 0xff, g.slots * 4, st));
-  for (float* v : {s.r, s.z, s.pre, s.p0, s.p1, s.w, s.x}) PCG_CUDA(cudaMemsetAsync(v, 0, g.slots * 4, st));
-  k_build<<<blocks_for(cells), 256, 0, st>>>(flags, div, s.parent, s.csize, s.cid, s.cf, s.comp, s.r, cs.cnt, g,
-                                             precond);
-  *launches += 1;
-
-  SweepArgs& sa = s.sa;
-  sa.cf = s.cf; sa.comp = s.comp; sa.r = s.r; sa.z = s.z; sa.pre = s.pre;
-  sa.prog_f = sc.prog.get(); sa.prog_b = sc.prog.get() + g.chunks;
-  sa.rz = cs.rz_new; sa.faults = s.header + 2;
-  sa.timing = (unsigned long long*)sc.debug_timing;
-  return 0;
+  return pcg_build(sc, s, flags, div, precond, sc.prog.get(), launches, st);
 }
 
-// One cooperative launch of the sweep pipeline: the IC(0) factor (pre) or one solve z = M^-1 r.
-cudaError_t launch_sweep(PcgScratch& sc, PcgSystem& s, bool factor, long long* launches, cudaStream_t st) {
-  s.sa.base = sc.epoch;
-  sc.epoch += (unsigned long long)s.g.S + 1;
+// One cooperative launch of the sweep pipeline: the IC(0) factor (pre) or one solve z = M^-1 r, with s.sa.base set.
+cudaError_t launch_sweep_at(PcgSystem& s, bool factor, long long* launches, cudaStream_t st) {
   void* args[] = {(void*)&s.sa, (void*)&s.g};
   *launches += 1;
   return cudaLaunchCooperativeKernel(factor ? (void*)k_sweep<true> : (void*)k_sweep<false>, dim3(s.sweep_grid),
                                      dim3(s.sweep_threads), args, s.sweep_smem, st);
+}
+// Direct solves: every launch gets the next epoch of the scratch's progress words, so no wait is satisfied by
+// progress an earlier launch left there.
+cudaError_t launch_sweep(PcgScratch& sc, PcgSystem& s, bool factor, long long* launches, cudaStream_t st) {
+  s.sa.base = sc.epoch;
+  sc.epoch += (unsigned long long)s.g.S + 1;
+  return launch_sweep_at(s, factor, launches, st);
 }
 
 }  // namespace
@@ -798,7 +887,7 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   if (!no_precond) PCG_CUDA(launch_sweep(sc, s, true, launches, st));
   k_rr_init<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, s.r, cs, g.slots);
   const double tol2 = (double)tol * (double)tol;
-  k_scalars<<<(ncomp + 255) / 256, 256, 0, st>>>(cs, ncomp, tol2, max_iter, 1, no_precond);
+  k_scalars<<<(ncomp + 255) / 256, 256, 0, st>>>(cs, nullptr, ncomp, tol2, max_iter, 1, no_precond);
   *launches += 2;
   PCG_CUDA(cudaMemcpyAsync(host, header, 16, cudaMemcpyDeviceToHost, st));
   PCG_CUDA(cudaStreamSynchronize(st));
@@ -814,7 +903,7 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
       k_direction_spmv<<<ew_blocks, g.NYP, 0, st>>>(s.cf, s.comp, no_precond ? s.r : s.z, p_old, p_new, s.w, cs, g,
                                                     no_precond);
       k_update<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, p_new, s.w, s.x, s.r, cs, g.slots, no_precond);
-      k_scalars<<<(ncomp + 255) / 256, 256, 0, st>>>(cs, ncomp, tol2, max_iter, 0, no_precond);
+      k_scalars<<<(ncomp + 255) / 256, 256, 0, st>>>(cs, nullptr, ncomp, tol2, max_iter, 0, no_precond);
       *launches += 3;
       float* tswap = p_old; p_old = p_new; p_new = tswap;
     }
@@ -843,6 +932,113 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   if (residual) *residual = worst;
   if (iterations) *iterations = worst_it;
   return 0;
+}
+
+int pcg_graph_alloc(PcgGraphScratch& gs, PcgScratch& sc, int nb, int nz, int ny, int nx, int is3d) {
+  PcgGeo g;
+  if (pcg_geometry(sc, nb, nz, ny, nx, is3d, g)) return 4;
+  if (pcg_init_once(sc)) return 3;
+  // A component in the system has at least two cells, so there are at most cells / 2 of them, whatever the flags
+  // hold at a replay.
+  const long long cap = std::max(1ll, g.n * nb / 2);
+  if (!(gs.comp_buf = dev_alloc<char>((size_t)cap * kCompBytes))) return 3;
+  gs.comp_cap = cap;
+  gs.prog_words = 2ll * g.chunks;
+  if (!(gs.prog = dev_zeros<unsigned long long>((size_t)gs.prog_words))) return 3;
+  if (!(gs.words = dev_zeros<int>(8))) return 3;
+  if (!(gs.body_stream = new_stream(cudaStreamNonBlocking))) return 3;
+  return 0;
+}
+
+// The loop runs two iterations per pass, so p_old / p_new swap as pointers (the body's launches are fixed) and a
+// replay runs at most one iteration more than the longest component needs, where pcg_solve's reads every 4th
+// iteration allow up to three; the extra ones are no-ops for finished components, so the results are pcg_solve's.
+//
+// Progress words: k_sweep's cross-CTA waits accept a progress value above the launch's base.  A base taken from a
+// host counter would be frozen by the capture, and the second sweep of a replay would find the words already past it
+// and read z values not yet written.  So each captured sweep is preceded by a memset node that zeroes the graph's own
+// words, and runs with base 0: the nodes of one replay run in stream order, a replay of an executable graph never
+// overlaps another of the same graph, and no other solve writes these words, so every value a sweep reads was
+// published by that sweep.
+int pcg_solve_graph(PcgGraphScratch& gs, PcgScratch& sc, void* workspace, float* p, const float* flags,
+                    const float* div, int nb, int nz, int ny, int nx, int is3d, int precond, float tol, int max_iter,
+                    long long* launches, cudaStream_t st) {
+  PcgSystem s;
+  int rc = pcg_label(sc, workspace, flags, nb, nz, ny, nx, is3d, launches, st, s);
+  if (rc) return rc;
+  const PcgGeo& g = s.g;
+  if (!gs.comp_buf || gs.comp_cap < std::max(1ll, g.n * nb / 2) || gs.prog_words < 2ll * g.chunks) return 3;
+  s.cs = comp_scalars(gs.comp_buf.get(), (size_t)gs.comp_cap, s.header);
+  const CompScalars& cs = s.cs;
+  const unsigned comp_blocks = (unsigned)sc.sm_count;     // loops over the device's component count
+  k_comp_clear<<<comp_blocks, 256, 0, st>>>(cs);
+  *launches += 1;
+  if ((rc = pcg_build(sc, s, flags, div, precond, gs.prog.get(), launches, st))) return rc;
+  const int no_precond = precond == 0;
+  const double tol2 = (double)tol * (double)tol;
+  const unsigned ew_blocks = s.ew_blocks;
+  auto sweep = [&](bool factor, long long* n, cudaStream_t q) {
+    const cudaError_t e = cudaMemsetAsync(gs.prog.get(), 0, (size_t)gs.prog_words * 8, q);
+    return e != cudaSuccess ? e : launch_sweep_at(s, factor, n, q);
+  };
+  if (!no_precond) PCG_CUDA(sweep(true, launches, st));
+  k_rr_init<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, s.r, cs, g.slots);
+  k_scalars<<<comp_blocks, 256, 0, st>>>(cs, s.header + 3, 0, tol2, max_iter, 1, no_precond);
+  *launches += 2;
+
+  // the WHILE node after what is captured so far; the first test arms it
+  cudaStreamCaptureStatus cap_status;
+  cudaGraph_t graph = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t ndeps = 0;
+  PCG_CUDA(cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, &deps, &ndeps));
+  if (cap_status != cudaStreamCaptureStatusActive) return 3;
+  cudaGraphConditionalHandle loop;
+  PCG_CUDA(cudaGraphConditionalHandleCreate(&loop, graph, 0, cudaGraphCondAssignDefault));
+  k_pcg_continue<<<1, 1, 0, st>>>(s.header, loop, nullptr);
+  *launches += 1;
+  PCG_CUDA(cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, &deps, &ndeps));
+  cudaGraphNodeParams np = {};
+  np.type = cudaGraphNodeTypeConditional;
+  np.conditional.handle = loop;
+  np.conditional.type = cudaGraphCondTypeWhile;
+  np.conditional.size = 1;
+  cudaGraphNode_t node;
+  PCG_CUDA(cudaGraphAddNode(&node, graph, deps, ndeps, &np));
+  PCG_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
+
+  // the body, captured on the graph's own stream into the node's body graph
+  cudaStream_t bs = gs.body_stream.get();
+  PCG_CUDA(cudaStreamBeginCaptureToGraph(bs, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                         cudaStreamCaptureModeRelaxed));
+  long long body = 0;
+  cudaError_t be = cudaSuccess;
+  float* p_old = s.p0;
+  float* p_new = s.p1;
+  for (int rep = 0; rep < 2 && be == cudaSuccess; rep++) {
+    be = cudaMemsetAsync(s.header, 0, 4, bs);
+    if (be == cudaSuccess && !no_precond) be = sweep(false, &body, bs);
+    if (be != cudaSuccess) break;
+    k_direction_spmv<<<ew_blocks, g.NYP, 0, bs>>>(s.cf, s.comp, no_precond ? s.r : s.z, p_old, p_new, s.w, cs, g,
+                                                  no_precond);
+    k_update<<<ew_blocks, 256, 0, bs>>>(s.cf, s.comp, p_new, s.w, s.x, s.r, cs, g.slots, no_precond);
+    k_scalars<<<comp_blocks, 256, 0, bs>>>(cs, s.header + 3, 0, tol2, max_iter, 0, no_precond);
+    body += 3;
+    float* tswap = p_old; p_old = p_new; p_new = tswap;
+  }
+  k_pcg_continue<<<1, 1, 0, bs>>>(s.header, loop, (unsigned long long*)(gs.words.get() + 4));
+  body += 1;
+  cudaGraph_t body_graph = nullptr;
+  const cudaError_t ee = cudaStreamEndCapture(bs, &body_graph);     // ends the body's capture on every path
+  if (be != cudaSuccess || ee != cudaSuccess) return 3;
+  gs.body_launches = body;
+
+  k_xsum<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, s.x, cs, g.slots);
+  k_writeback<<<blocks_for(g.n * nb), 256, 0, st>>>(p, s.parent, s.csize, s.cid, s.x, cs, g, 1);
+  k_pcg_finish<<<1, 256, 0, st>>>(cs, gs.words.get());
+  *launches += 3;
+  gs.captured = true;
+  return cudaPeekAtLastError() == cudaSuccess ? 0 : 3;
 }
 
 int pcg_precond(PcgScratch& sc, void* workspace, float* z, const float* flags, const float* r, int nb, int nz, int ny,

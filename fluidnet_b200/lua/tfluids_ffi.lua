@@ -94,6 +94,7 @@ typedef struct tfl_slab_sim tfl_slab_sim;
 int tfl_set_stream(tfl_ctx* ctx, void* cuda_stream);
 int tfl_step_graph_create(tfl_ctx*, const tfl_state* state, const tfl_mconf* mconf, tfl_cnn* cnn, tfl_step_graph** out);
 int tfl_step_graph_launch(tfl_ctx*, tfl_step_graph* graph);
+int tfl_step_graph_pcg_status(tfl_ctx*, tfl_step_graph* graph, float* residual, int32_t* iterations);
 void tfl_step_graph_destroy(tfl_ctx*, tfl_step_graph* graph);
 int tfl_comm_unique_id(tfl_ctx*, char* id_out);
 int tfl_comm_init(tfl_ctx*, const char* id_bytes, int32_t rank, int32_t world);
@@ -327,6 +328,13 @@ function tfluids.captureStep(cstate, cmconf, model)          -- after one tfluid
   return g[0]
 end
 function tfluids.launchStep(graph) check(lib.tfl_step_graph_launch(ctx, graph)) end
+-- residual, iterations of the last replay's PCG solve (iterations -1 without one); raises the reference's error
+-- string for the first failed solve since the previous call.  Synchronises.
+function tfluids.stepPcgStatus(graph)
+  local res, it = ffi.new('float[1]'), ffi.new('int32_t[1]')
+  check(lib.tfl_step_graph_pcg_status(ctx, graph, res, it))
+  return res[0], it[0]
+end
 function tfluids.commUniqueId()
   local id = ffi.new('char[128]')
   check(lib.tfl_comm_unique_id(ctx, id))

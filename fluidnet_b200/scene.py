@@ -167,8 +167,7 @@ def run(res=128, scene="plume", sim_method="convnet", model=None, model_mconf=No
                             w.write(occ)
                         with formats.VboxWriter(paths["geom_blender"], res, 1) as w:
                             w.write(blender_geometry(occ))
-                        if sim_method == "convnet":   # PCG polls a host word and cannot be captured
-                            graph = simulate.StepGraph(mconf, batch, model)
+                        graph = simulate.StepGraph(mconf, batch, model)
                     if i % output_decimation == 0:
                         rec.record(batch["density"], dens)
                         written += 1
@@ -176,6 +175,8 @@ def run(res=128, scene="plume", sim_method="convnet", model=None, model_mconf=No
                 rec.drain(dens, wait=True)
             stream.synchronize()
             t1 = time.perf_counter()
+            if graph is not None and sim_method == "pcg":
+                graph.pcg_status()        # raises what the reference's solve would have (a NaN residual, ...)
         finally:
             rec.close()
             if graph is not None:

@@ -204,6 +204,15 @@ class StepGraph:
         self.ctx.use_current_stream()
         self.ctx.check(self.ctx.lib.tfl_step_graph_launch(self.ctx.h, self.h))
 
+    def pcg_status(self):
+        """(residual, iterations) of the last replay's PCG solve, as solveLinearSystemPCG returns them (-inf, 0
+        without a component to solve); iterations is -1 for a step without a PCG solve.  Synchronises.  Raises
+        TflError with the direct solve's message for the first replay since the previous call whose solve failed."""
+        self.ctx.use_current_stream()
+        res, it = C.c_float(0.0), C.c_int32(0)
+        self.ctx.check(self.ctx.lib.tfl_step_graph_pcg_status(self.ctx.h, self.h, C.byref(res), C.byref(it)))
+        return res.value, it.value
+
     def close(self):
         if self.h:
             self.ctx.lib.tfl_step_graph_destroy(self.ctx.h, self.h)

@@ -74,7 +74,9 @@ int tfl_sync(tfl_ctx* ctx);
  * treats as a hard error (generic/calc_line_trace.cc THError sites) or that left the
  * local z-slab (halo too small).  Synchronises. */
 int tfl_trace_faults(tfl_ctx* ctx, int64_t* count, int reset);
-/* Kernels launched by this context since creation (bench.py's gpu_launches). */
+/* Kernels launched by this context since creation (bench.py's gpu_launches).  A step graph's replay adds the kernels
+ * it runs outside a PCG solve's iteration loop; the loop's kernels, whose number only the device knows, are added by
+ * the next tfl_step_graph_pcg_status of that graph (loop passes counted on the device times the body's kernels). */
 int64_t tfl_launch_count(const tfl_ctx* ctx);
 
 /* z-slab placement of subsequent grids: local plane 0 is global plane `z_offset` of a
@@ -382,11 +384,21 @@ int tfl_host_sim_step(tfl_ctx* ctx, tfl_host_sim* hs, float* p, float* U, float*
  *     another shape, smaller ones included (the context's flag cache);
  *   - tfl_cnn_project or a step with the captured model on another grid (the model's activation buffers).
  * After any of them tfl_step_graph_launch fails, naming the buffer, and replays nothing: capture again (after one
- * tfl_simulate_step).  Destroying the model or the context while a graph that uses them exists is a caller error. */
+ * tfl_simulate_step).  Destroying the model or the context while a graph that uses them exists is a caller error.
+ * Every simMethod is captured.  With 'pcg' the solve's iteration loop is a conditional node: the device decides after
+ * every second iteration whether any component still runs, so a replay never waits for the host, follows flags
+ * changed in place (the graph owns per-component scalars for cells / 2 components, about 30 bytes per cell) and runs
+ * at most one iteration past the longest component.  The direct solve's limits are refused at creation by name
+ * (ny > 960, z-slabs).  A replay cannot fail on the device: tfl_step_graph_pcg_status synchronises the context's
+ * stream and gives the last replay's residual and iterations as tfl_solve_linear_system_pcg returns them (-inf and
+ * 0 when no component was solved), or fails with the direct call's message for the first replay since the previous
+ * call whose solve failed (a fluid cell on the border, a NaN residual, a stalled sweep pipeline); that error stays
+ * until this call reads it.  *iterations = -1 for a graph without a PCG solve. */
 typedef struct tfl_step_graph tfl_step_graph;
 int tfl_step_graph_create(tfl_ctx* ctx, const tfl_state* state, const tfl_mconf* mconf, tfl_cnn* cnn,
                           tfl_step_graph** out);
 int tfl_step_graph_launch(tfl_ctx* ctx, tfl_step_graph* graph);
+int tfl_step_graph_pcg_status(tfl_ctx* ctx, tfl_step_graph* graph, float* residual, int32_t* iterations);
 void tfl_step_graph_destroy(tfl_ctx* ctx, tfl_step_graph* graph);
 /* ---- one domain in z-slabs over the GPUs of a node (no counterpart in the reference, which is single-GPU;
  * SURVEY.md section 8e).  One process and one context per GPU.  The context owns the NCCL communicator
