@@ -69,10 +69,12 @@ SYMBOLS = [
     "tfl_slab_sim_exchange_stats", "tfl_slab_sim_ipc_export", "tfl_slab_sim_ipc_connect",
     "tfl_slab_sim_jacobi_stats", "tfl_slab_jacobi_schedule", "tfl_jacobi_slab_block", "tfl_slab_cnn_margin",
     "tfl_recorder_create", "tfl_recorder_destroy", "tfl_recorder_capture", "tfl_recorder_take", "tfl_recorder_release",
+    "tfl_recorder_create_slab", "tfl_recorder_ipc_export", "tfl_recorder_ipc_connect", "tfl_recorder_capture_slab",
 ]
 JACOBI_BLOCK_INTS = 6
 COMM_ID_BYTES = 128
 IPC_HANDLE_BYTES = 64
+RECORDER_HANDLE_BYTES = 128
 
 _lib = None
 
@@ -199,5 +201,10 @@ def load():
     lib.tfl_recorder_take.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.POINTER(C.c_float)),
                                       C.POINTER(C.c_int64)]
     lib.tfl_recorder_release.argtypes = [C.c_void_p, C.c_void_p]
+    lib.tfl_recorder_create_slab.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
+                                             C.POINTER(C.c_void_p)]
+    lib.tfl_recorder_ipc_export.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p]
+    lib.tfl_recorder_ipc_connect.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p]
+    lib.tfl_recorder_capture_slab.argtypes = [C.c_void_p, C.c_void_p, G, C.c_int32, C.POINTER(C.c_int64)]
     _lib = lib
     return lib

@@ -240,6 +240,14 @@ inline int check_vel(tfl_ctx* ctx, const tfl_grid* U, const tfl_grid* flags) {
 // velocity field within 2^33 cells.
 inline bool grid_too_large(long long n, int nb) { return n >= (1LL << 31) || n * (long long)nb * 3 >= (1LL << 31) * 4; }
 
+// The global planes [*z0, *z1) z-slab rank `rank` of `world` owns in a domain of gnz planes: gnz / world each, one more
+// for the first gnz % world ranks.  The slab simulator, its Jacobi schedule and the slab recorder all use this rule.
+inline void slab_planes(int gnz, int world, int rank, int* z0, int* z1) {
+  const int base = gnz / world, rem = gnz % world;
+  *z0 = rank * base + (rank < rem ? rank : rem);
+  *z1 = *z0 + base + (rank < rem ? 1 : 0);
+}
+
 inline int make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is3d, Geo* g) {
   g->nx = flags->nx; g->ny = flags->ny; g->nz = flags->nz; g->nb = flags->nb;
   g->is3d = is3d ? 1 : 0;

@@ -167,10 +167,9 @@ int tfl_slab_sim_create(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32
   memset(&s->st, 0, sizeof(s->st));
   s->gnz = gnz; s->ny = ny; s->nx = nx; s->margin = margin; s->halo = 2 * margin + 2;
   s->rank = ctx->comm_rank; s->world = ctx->comm_world;
-  const int base = gnz / s->world, rem = gnz % s->world;
+  const int base = gnz / s->world;
   if (s->world > 1 && base < s->halo) return fail(ctx, "slab_sim: slabs of %d planes are thinner than the halo (%d)", base, s->halo);
-  s->z0 = s->rank * base + std::min(s->rank, rem);
-  s->z1 = s->z0 + base + (s->rank < rem ? 1 : 0);
+  slab_planes(gnz, s->world, s->rank, &s->z0, &s->z1);
   s->lo_halo = std::min(s->halo, s->z0);
   s->hi_halo = std::min(s->halo, gnz - s->z1);
   s->zoff = s->z0 - s->lo_halo;
@@ -576,9 +575,10 @@ extern "C" {
 int tfl_slab_jacobi_schedule(int32_t gnz, int32_t world, int32_t rank, int32_t margin, int32_t max_iter,
                              int32_t planes[3], int32_t* blocks, int32_t cap) {
   if (gnz < 3 || world < 1 || rank < 0 || rank >= world || margin < 2 || max_iter < 1) return -1;
-  const int halo = 2 * margin + 2, base = gnz / world, rem = gnz % world;
-  if (world > 1 && base < halo) return -1;
-  const int z0 = rank * base + std::min(rank, rem), z1 = z0 + base + (rank < rem ? 1 : 0);
+  const int halo = 2 * margin + 2;
+  if (world > 1 && gnz / world < halo) return -1;
+  int z0, z1;
+  slab_planes(gnz, world, rank, &z0, &z1);
   const int lo_halo = std::min(halo, z0), hi_halo = std::min(halo, gnz - z1);
   const int nz = (z1 - z0) + lo_halo + hi_halo, own_lo = lo_halo, own_hi = lo_halo + (z1 - z0);
   const bool lo = rank > 0, hi = rank < world - 1;     // sides with a neighbour: the ranges shrink there

@@ -121,6 +121,11 @@ void tfl_recorder_destroy(tfl_ctx*, tfl_recorder* rec);
 int tfl_recorder_capture(tfl_ctx*, tfl_recorder* rec, const tfl_grid* field, int64_t* frame_out);
 int tfl_recorder_take(tfl_ctx*, tfl_recorder* rec, int wait, const float** host_out, int64_t* frame_out);
 int tfl_recorder_release(tfl_ctx*, tfl_recorder* rec);
+int tfl_recorder_create_slab(tfl_ctx*, int32_t gnz, int32_t ny, int32_t nx, int32_t rank, int32_t world, int32_t slots,
+                             tfl_recorder** out);
+int tfl_recorder_ipc_export(tfl_ctx*, tfl_recorder* rec, char* handle_out);
+int tfl_recorder_ipc_connect(tfl_ctx*, tfl_recorder* rec, const char* handle);
+int tfl_recorder_capture_slab(tfl_ctx*, tfl_recorder* rec, const tfl_grid* field, int32_t z_offset, int64_t* frame_out);
 ]]
 
 local lib = ffi.load('tfl')          -- libtfl.so on the library path
@@ -402,6 +407,25 @@ function tfluids.recorderTake(rec, wait)           -- -> frame index, const floa
 end
 function tfluids.recorderRelease(rec) check(lib.tfl_recorder_release(ctx, rec)) end
 function tfluids.recorderDestroy(rec) lib.tfl_recorder_destroy(ctx, rec) end
+-- z-slab runs: one frame gathered on rank 0 from every rank's owned planes (collective captures, rank 0 takes).
+-- Rank 0 passes recorderIpcHandle's 128 bytes to the other ranks, which recorderIpcConnect; then a barrier, then
+-- captures.  Destroy on the other ranks first, then a barrier, then on rank 0.
+function tfluids.recorderCreateSlab(gnz, ny, nx, rank, world, slots)
+  local r = ffi.new('tfl_recorder*[1]')
+  check(lib.tfl_recorder_create_slab(ctx, gnz, ny, nx, rank, world, slots or 3, r))
+  return r[0]
+end
+function tfluids.recorderIpcHandle(rec)
+  local h = ffi.new('char[128]')
+  check(lib.tfl_recorder_ipc_export(ctx, rec, h))
+  return ffi.string(h, 128)
+end
+function tfluids.recorderIpcConnect(rec, handle) check(lib.tfl_recorder_ipc_connect(ctx, rec, handle)) end
+function tfluids.recorderCaptureSlab(rec, field, zOffset)   -- field: the rank's local slab, plane 0 = global zOffset
+  local idx = ffi.new('int64_t[1]')
+  check(lib.tfl_recorder_capture_slab(ctx, rec, field.c, zOffset, idx))
+  return tonumber(idx[0])
+end
 
 function tfluids.synchronize() check(lib.tfl_sync(ctx)) end
 

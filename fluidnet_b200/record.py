@@ -19,7 +19,7 @@ import ctypes as C
 
 import numpy as np
 
-from . import tfluids
+from . import _lib, tfluids
 from ._lib import TflError
 
 
@@ -64,7 +64,11 @@ class FrameRecorder:
         grid), valid until `release`: copy it to keep it."""
         ptr = C.POINTER(C.c_float)()
         idx = C.c_int64(-1)
-        self.ctx.check(self.ctx.lib.tfl_recorder_take(self.ctx.h, self.h, 1 if wait else 0, C.byref(ptr), C.byref(idx)))
+        rc = self.ctx.lib.tfl_recorder_take(self.ctx.h, self.h, 1 if wait else 0, C.byref(ptr), C.byref(idx))
+        if rc != 0 and idx.value >= 0:       # a z-slab frame whose planes did not all arrive: taken, to be released
+            self.captured -= 1
+            self.taken += 1
+        self.ctx.check(rc)
         if idx.value < 0:
             return None
         self.captured -= 1
@@ -115,3 +119,124 @@ class FrameRecorder:
 
     def __exit__(self, *exc):
         self.close()
+
+
+class SlabFrameRecorder(FrameRecorder):
+    """One `.vbox` frame gathered from every rank of a z-slab run (tfl_recorder_create_slab, DESIGN.md section 6a).
+
+    Every rank packs the global planes it owns (SlabDecomposition's z0 .. z1) straight into rank 0's staging frame;
+    rank 0 is the writer and alone takes, releases, drains and records frames -- on the other ranks `record` is a
+    capture and `drain` writes nothing.  Captures are collective: every rank captures the same number of times, in
+    step order.  The constructor is collective too: rank 0's handle goes to the other ranks with `share` (by default
+    torch.distributed over `group`) and it ends with `barrier`, so no rank captures before every rank is connected.
+    `close` is collective as well: the other ranks free their recorders before rank 0 frees the frame they write into.
+
+        rec = SlabFrameRecorder((gnz, ny, nx), rank, world)
+        rec.record(local_density, z_offset, writer if rank == 0 else None)
+    """
+
+    def __init__(self, shape, rank, world, slots=3, device=None, group=None, share=None, barrier=None):
+        """shape: the GLOBAL (gnz, ny, nx).  share(handle bytes on rank 0, None elsewhere) -> rank 0's bytes on every
+        rank and barrier() replace torch.distributed (e.g. processes that share one GPU without a process group).
+        Raises TflError on every rank if any rank could not map rank 0's frame (there is no other transport)."""
+        import torch.distributed as dist
+        shape = tuple(int(v) for v in shape)
+        if len(shape) != 3:
+            raise TflError("SlabFrameRecorder: shape must be the global (gnz, ny, nx), got %r" % (shape,))
+        self.shape, self.rank, self.world, self.slots = shape, int(rank), int(world), int(slots)
+        self.group = group
+        self.ctx = tfluids.context(device)
+        self.captured = 0
+        self.taken = 0
+        h = C.c_void_p()
+        self.ctx.check(self.ctx.lib.tfl_recorder_create_slab(self.ctx.h, shape[0], shape[1], shape[2], self.rank,
+                                                             self.world, self.slots, C.byref(h)))
+        self.h = h
+        if self.world == 1:
+            return
+        if share is None:
+            def share(b):
+                obj = [b]
+                dist.broadcast_object_list(obj, src=0, group=group)
+                return obj[0]
+        self._custom = barrier is not None
+        self._barrier = barrier or (lambda: dist.barrier(group=group))
+        lib, error = self.ctx.lib, None
+        if self.rank == 0:
+            buf = C.create_string_buffer(_lib.RECORDER_HANDLE_BYTES)
+            if lib.tfl_recorder_ipc_export(self.ctx.h, self.h, buf) != 0:
+                error = lib.tfl_last_error(self.ctx.h).decode()
+            handle = share(None if error else buf.raw)
+        else:
+            handle = share(None)
+            if handle is None:
+                error = "rank 0 could not export its frame"
+            elif lib.tfl_recorder_ipc_connect(self.ctx.h, self.h, handle) != 0:
+                error = lib.tfl_last_error(self.ctx.h).decode()
+        if self._custom:                      # the barrier before the first capture; each rank reports its own error
+            self._barrier()
+            failed = [(self.rank, error)] if error else []
+        else:                                 # every rank learns every rank's error (also the barrier)
+            errs = [None] * self.world
+            dist.all_gather_object(errs, error, group=group)
+            failed = [(r, e) for r, e in enumerate(errs) if e]
+        if failed:                            # nothing was captured: no rank writes into rank 0's frame
+            self.ctx.lib.tfl_recorder_destroy(self.ctx.h, self.h)
+            self.h = None
+            raise TflError("SlabFrameRecorder: peer memory refused (%s); frames cannot be gathered asynchronously"
+                           % "; ".join("rank %d: %s" % rf for rf in failed))
+
+    def capture(self, tensor, z_offset):
+        """Enqueue the pack of this rank's planes of `tensor` (its local [1][1][nz][ny][nx] CUDA float32 slab, whose
+        plane 0 is global plane z_offset) on the current stream; returns the frame's index.  Never waits on the
+        host."""
+        c = tfluids._ctx_for(tensor)
+        if c is not self.ctx:
+            raise TflError("SlabFrameRecorder: the tensor lives on another device than the recorder")
+        assert tensor.dim() == 5 and tensor.is_contiguous(), "SlabFrameRecorder: a contiguous 5-D tensor is needed"
+        self.ctx.use_current_stream()
+        return self.capture_grid(tfluids._grid(tensor), z_offset)
+
+    def capture_grid(self, grid, z_offset):
+        """capture of a tfl_grid (e.g. a field of tfl_slab_sim_layout) on the context's stream."""
+        idx = C.c_int64(-1)
+        self.ctx.check(self.ctx.lib.tfl_recorder_capture_slab(self.ctx.h, self.h, C.byref(grid), int(z_offset),
+                                                              C.byref(idx)))
+        if self.rank == 0:
+            self.captured += 1
+        return idx.value
+
+    def drain(self, writer, wait=False):
+        return super().drain(writer, wait) if self.rank == 0 else 0
+
+    def _make_room(self, writer):
+        if self.rank == 0 and self.full and self.captured:
+            idx, frame = self.take(True)
+            writer.write_packed(frame)
+            self.release()
+
+    def record(self, tensor, z_offset, writer):
+        """capture on every rank; on rank 0 first writes the oldest frame to `writer` if every slot is in use."""
+        self._make_room(writer)
+        return self.capture(tensor, z_offset)
+
+    def record_grid(self, grid, z_offset, writer):
+        self._make_room(writer)
+        return self.capture_grid(grid, z_offset)
+
+    def close(self):
+        """Free the recorder.  Collective for world > 1: the other ranks drain their packs and unmap, then (after a
+        barrier) rank 0 waits for its copies and frees the frame."""
+        if not getattr(self, "h", None):
+            return
+        if self.world > 1 and self.rank > 0:
+            self.ctx.lib.tfl_recorder_destroy(self.ctx.h, self.h)
+            self.h = None
+        if self.world > 1 and getattr(self, "_barrier", None) is not None:
+            self._barrier()
+        if self.h:
+            self.ctx.lib.tfl_recorder_destroy(self.ctx.h, self.h)
+            self.h = None
+
+    def __del__(self):
+        pass          # close() is collective: never from the garbage collector

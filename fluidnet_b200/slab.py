@@ -328,8 +328,9 @@ class NativeSlabSimulator:
     other ranks (any transport would do) and, in `gather`, by the tests."""
 
     def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=None, group=None,
-                 peer_halos=True, banks=None, conv_mode=None):
-        """Arguments as SlabSimulator's (margin=None: the model's smallest, cnn_margin)."""
+                 peer_halos=True, banks=None, conv_mode=None, model=None):
+        """Arguments as SlabSimulator's (margin=None: the model's smallest, cnn_margin).  model: an existing
+        ProjectionModel on `device` to run instead of one built from model_layers / banks."""
         import numpy as np
         from . import tfluids, model as fmodel, simulate, _lib
         self.group = group
@@ -337,6 +338,8 @@ class NativeSlabSimulator:
         self.world = dist.get_world_size(group) if world is None else world
         self.mconf = dict(mconf)
         method, _ = _sim_method(self.mconf)
+        if model is not None:
+            banks = model.banks
         margin = _resolve_margin(margin, None if method == "jacobi" else banks)
         self.device = torch.device(device)
         self.ctx = tfluids.context(self.device)
@@ -350,9 +353,13 @@ class NativeSlabSimulator:
             dist.broadcast_object_list(ident, src=0, group=group)
         self.ctx.check(lib.tfl_comm_init(self.ctx.h, ident[0] if ident[0] else b"\0" * _lib.COMM_ID_BYTES, self.rank, self.world))
         self.mc = simulate.make_mconf(self.mconf)
-        self.model = None if method == "jacobi" else fmodel.ProjectionModel(
-            model_layers, True, device=self.device, banks=banks,
-            normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
+        if method == "jacobi":
+            self.model = None
+        elif model is not None:
+            self.model = model
+        else:
+            self.model = fmodel.ProjectionModel(model_layers, True, device=self.device, banks=banks,
+                                                normalizeInputThreshold=self.mconf.get("normalizeInputThreshold", 1e-5))
         if self.model is not None and conv_mode is not None:
             self.model.set_mode(conv_mode)
 
@@ -360,6 +367,7 @@ class NativeSlabSimulator:
             t = batch.get(key)
             return None if t is None else np.ascontiguousarray(t.numpy() if isinstance(t, torch.Tensor) else t, np.float32)
 
+        self.margin = margin
         self._shape = tuple(batch["flags"].shape)
         gnz, ny, nx = self._shape[2:]
         arrs = [host(k) for k in ("flags", "UBC", "UBCInvMask", "densityBC", "densityBCInvMask")]
@@ -434,6 +442,24 @@ class NativeSlabSimulator:
             dist.all_reduce(t, group=self.group)          # owned planes are disjoint, the rest is zero
             mine = t.cpu()
         return mine
+
+    def frame_recorder(self, slots=3, share=None, barrier=None):
+        """A record.SlabFrameRecorder for this decomposition's global grid (collective; see there)."""
+        from .record import SlabFrameRecorder
+        return SlabFrameRecorder(self._shape[2:], self.rank, self.world, slots, self.device, self.group, share, barrier)
+
+    def field(self, key):
+        """The tfl_grid of this rank's local slab of `key` ('density' or 'pDiv'; owned and ghost planes, local plane 0
+        at global plane self.zoff)."""
+        st = _lib.State()
+        self.ctx.check(self.ctx.lib.tfl_slab_sim_layout(self.h, C.byref(st), None))
+        return getattr(st, {"density": "density", "pDiv": "p"}[key])
+
+    def record(self, rec, writer, key="density"):
+        """Collective: capture this rank's planes of `key` into `rec` (a frame_recorder) on the current stream, behind
+        the steps enqueued so far; rank 0 writes the oldest frame to `writer` first if its ring is full."""
+        self.ctx.use_current_stream()
+        return rec.record_grid(self.field(key), self.zoff, writer)
 
     def close(self):
         if self.h:

@@ -495,13 +495,48 @@ int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* sim, const char* handle
  *   frame is left.  *host_out (pinned, nx * ny * nz floats) stays valid until the frame is released.
  * tfl_recorder_release: gives back the oldest taken frame's slot (strictly first in, first out); fails if none is taken.
  * tfl_recorder_destroy: waits for the copies in flight, then frees everything.
- * Cost: k_pack_vbox moves 8 bytes per cell; the copy runs beside the following steps (DESIGN.md section 6a). */
+ * Cost: k_pack_vbox moves 8 bytes per cell; the copy runs beside the following steps (DESIGN.md section 6a).
+ *
+ * Z-slab runs (one frame gathered from every rank of a decomposed domain, DESIGN.md section 6a):
+ * tfl_recorder_create_slab: the recorder of rank `rank` of `world` (1 .. 64) for a [gnz][ny][nx] domain.  The rank
+ *   owns global planes [z0, z1) by the slab simulator's rule (gnz / world planes each, one more for the first
+ *   gnz % world ranks).  Rank 0 is the writer: its recorder is the one above with nz = gnz and `slots` host frames;
+ *   `slots` is ignored on the other ranks.  Refused before anything is allocated when a slab would be empty.
+ *   With world = 1 it is a whole-grid recorder that captures with tfl_recorder_capture_slab.
+ * tfl_recorder_ipc_export (rank 0): TFL_RECORDER_HANDLE_BYTES naming rank 0's staging frame and counters (a CUDA IPC
+ *   handle) and the recorder's gnz, ny, nx and world.  The host application hands these bytes to every other rank.
+ * tfl_recorder_ipc_connect (every other rank): maps rank 0's frame; refuses a handle of another shape or world, and
+ *   fails by name where the mapping is refused (there is no NCCL path for frames).  Every rank must export or
+ *   connect before any rank captures (a host-side barrier).
+ * tfl_recorder_capture_slab: collective -- every rank calls it the same number of times, in step order.  `field`
+ *   holds this rank's planes, its local plane 0 being global plane z_offset (tfl_slab_sim_layout's info[0]).  Rank
+ *   r > 0 waits on the device (bounded, ~2 s) until rank 0's copy of its previous frame is done, then packs its planes
+ *   into rank 0's staging frame with remote stores and raises its arrival counter.  Rank 0 packs its own planes like
+ *   tfl_recorder_capture; its copy stream, not the context's stream, waits (bounded) for every rank's arrival before
+ *   the copy to the host.  A wait that times out writes nothing and raises tfl_trace_faults.  Refused with nothing
+ *   enqueued: a field that does not hold the rank's planes, wrong ny / nx, nb or nc != 1, a stream being captured, a
+ *   world > 1 recorder not exported / connected, and on rank 0 a full ring (retry after a release: the frame index
+ *   does not advance).  *frame_out counts the captures on every rank.
+ * tfl_recorder_take / tfl_recorder_release: rank 0 only (refused by name elsewhere).  A frame whose ranks did not all
+ *   arrive within the wait bound is not handed out: take fails naming the frame and the missing ranks, sets
+ *   *frame_out to the frame (host_out stays NULL) and counts it as taken, so release it to go on.
+ * tfl_recorder_destroy: on a rank r > 0 it drains the context's stream and unmaps rank 0's frame.  Caller contract, as
+ *   for the slab simulator: rank 0 destroys its recorder only after every other rank has destroyed its own (a
+ *   host-side barrier), since their packs write into rank 0's memory.
+ * tfl_recorder_capture refuses a recorder of world > 1. */
 typedef struct tfl_recorder tfl_recorder;
 int tfl_recorder_create(tfl_ctx* ctx, int32_t nz, int32_t ny, int32_t nx, int32_t slots, tfl_recorder** out);
 void tfl_recorder_destroy(tfl_ctx* ctx, tfl_recorder* rec);
 int tfl_recorder_capture(tfl_ctx* ctx, tfl_recorder* rec, const tfl_grid* field, int64_t* frame_out);
 int tfl_recorder_take(tfl_ctx* ctx, tfl_recorder* rec, int wait, const float** host_out, int64_t* frame_out);
 int tfl_recorder_release(tfl_ctx* ctx, tfl_recorder* rec);
+#define TFL_RECORDER_HANDLE_BYTES 128
+int tfl_recorder_create_slab(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32_t rank, int32_t world,
+                             int32_t slots, tfl_recorder** out);
+int tfl_recorder_ipc_export(tfl_ctx* ctx, tfl_recorder* rec, char* handle_out /* TFL_RECORDER_HANDLE_BYTES */);
+int tfl_recorder_ipc_connect(tfl_ctx* ctx, tfl_recorder* rec, const char* handle);
+int tfl_recorder_capture_slab(tfl_ctx* ctx, tfl_recorder* rec, const tfl_grid* field, int32_t z_offset,
+                              int64_t* frame_out);
 #ifdef __cplusplus
 }
 #endif
