@@ -325,14 +325,28 @@ class NativeSlabSimulator:
     """The same decomposition with everything inside libtfl.so (tfl_slab_sim_*): the context owns the NCCL
     communicator, the halo exchanges are ncclSend / ncclRecv straight on the field arrays, one C call per step.
     This is what a LuaJIT host would drive; torch.distributed is used here only to hand rank 0's NCCL id to the
-    other ranks (any transport would do) and, in `gather`, by the tests."""
+    other ranks (any transport would do) and, in `gather`, by the tests.
+
+    Without torch.distributed (`allgather` and `barrier` given, e.g. processes that share one GPU): no NCCL
+    communicator, the IPC handles go through `allgather`, and peer memory is the only transport -- the constructor
+    raises on every rank if any rank cannot map its neighbours' inboxes."""
 
     def __init__(self, batch, mconf, model_layers, device, rank=None, world=None, margin=None, group=None,
-                 peer_halos=True, banks=None, conv_mode=None, model=None):
+                 peer_halos=True, banks=None, conv_mode=None, model=None, allgather=None, barrier=None):
         """Arguments as SlabSimulator's (margin=None: the model's smallest, cnn_margin).  model: an existing
-        ProjectionModel on `device` to run instead of one built from model_layers / banks."""
+        ProjectionModel on `device` to run instead of one built from model_layers / banks.
+        allgather(bytes or None) -> list over the ranks in rank order, and barrier(): replace torch.distributed (both
+        or neither; rank and world must then be given)."""
         import numpy as np
         from . import tfluids, model as fmodel, simulate, _lib
+        if (allgather is None) != (barrier is None):
+            raise ValueError("NativeSlabSimulator: give allgather and barrier together")
+        self._allgather, self._barrier = allgather, barrier
+        if allgather is not None and (rank is None or world is None):
+            raise ValueError("NativeSlabSimulator: without torch.distributed, rank and world must be given")
+        if allgather is not None and world > 1 and not peer_halos:
+            raise ValueError("NativeSlabSimulator: without torch.distributed there is no NCCL communicator; "
+                             "the halos need peer memory (peer_halos=True)")
         self.group = group
         self.rank = dist.get_rank(group) if rank is None else rank
         self.world = dist.get_world_size(group) if world is None else world
@@ -344,14 +358,14 @@ class NativeSlabSimulator:
         self.device = torch.device(device)
         self.ctx = tfluids.context(self.device)
         lib = self.ctx.lib
-        ident = [None]
-        if self.world > 1:
+        ident = [None]                        # NULL id: the context takes rank and world but makes no communicator
+        if self.world > 1 and allgather is None:
             if self.rank == 0:
                 buf = C.create_string_buffer(_lib.COMM_ID_BYTES)
                 self.ctx.check(lib.tfl_comm_unique_id(self.ctx.h, buf))
                 ident = [buf.raw]
             dist.broadcast_object_list(ident, src=0, group=group)
-        self.ctx.check(lib.tfl_comm_init(self.ctx.h, ident[0] if ident[0] else b"\0" * _lib.COMM_ID_BYTES, self.rank, self.world))
+        self.ctx.check(lib.tfl_comm_init(self.ctx.h, ident[0], self.rank, self.world))
         self.mc = simulate.make_mconf(self.mconf)
         if method == "jacobi":
             self.model = None
@@ -383,7 +397,9 @@ class NativeSlabSimulator:
         self.zoff, self.nz, self.own_lo, self.own_hi, self.z0, self.z1 = list(info)
         # Halos over peer memory (CUDA IPC + NVLink) when every rank can map its neighbours; otherwise NCCL.
         self.halo_transport = "nccl"
-        if self.world > 1 and peer_halos:
+        if self.world > 1 and allgather is not None:
+            self._connect_without_dist()
+        elif self.world > 1 and peer_halos:
             buf = C.create_string_buffer(_lib.IPC_HANDLE_BYTES)
             ok = lib.tfl_slab_sim_ipc_export(self.ctx.h, self.h, buf) == 0
             handles = [None] * self.world
@@ -398,6 +414,29 @@ class NativeSlabSimulator:
                 self.halo_transport = "peer memory (CUDA IPC over NVLink)"
             elif ok:                                          # every rank must use the same transport
                 self.ctx.check(lib.tfl_slab_sim_ipc_connect(self.ctx.h, self.h, None))
+
+    def _connect_without_dist(self):
+        """Peer memory with the handles moved by `allgather`.  There is no communicator to fall back on: an unconnected
+        tfl_slab_sim_step would exchange nothing and reduce nothing, so every rank raises if any rank fails."""
+        from ._lib import TflError
+        lib = self.ctx.lib
+        buf = C.create_string_buffer(_lib.IPC_HANDLE_BYTES)
+        error = None
+        if lib.tfl_slab_sim_ipc_export(self.ctx.h, self.h, buf) != 0:
+            error = lib.tfl_last_error(self.ctx.h).decode()
+        handles = self._allgather(None if error else buf.raw)
+        failed = [(r, "no inbox handle") for r, h in enumerate(handles) if h is None]
+        if not failed:                        # every rank learns every rank's error (the same list everywhere)
+            if lib.tfl_slab_sim_ipc_connect(self.ctx.h, self.h, b"".join(handles)) != 0:
+                error = lib.tfl_last_error(self.ctx.h).decode()
+            failed = [(r, e) for r, e in enumerate(self._allgather(error)) if e]
+        if failed:
+            self.close()
+            raise TflError("NativeSlabSimulator: peer memory refused (%s); without torch.distributed there is no "
+                           "NCCL fallback, the halo exchanges would move nothing"
+                           % "; ".join("rank %d: %s" % rf for rf in failed))
+        self._barrier()                       # every rank is connected before any rank steps
+        self.halo_transport = "peer memory (CUDA IPC)"
 
     def step(self):
         self.ctx.use_current_stream()
@@ -417,8 +456,10 @@ class NativeSlabSimulator:
         return n.value, ms.value, by.value
 
     def check(self):
+        """Raises if any stencil / trace left the local slab since the last check: on any rank, or without
+        torch.distributed on this one."""
         f = torch.tensor([self.ctx.trace_faults()], dtype=torch.float64, device=self.device)
-        if self.world > 1:
+        if self.world > 1 and self._allgather is None:
             dist.all_reduce(f, group=self.group)
         if f.item() != 0:
             raise RuntimeError("z-slab halo too small for the current velocities (%d faults): raise `margin`"
@@ -436,6 +477,9 @@ class NativeSlabSimulator:
 
     def gather(self, key):
         """Global tensor assembled from every rank's owned planes (on every rank, CPU)."""
+        if self.world > 1 and self._allgather is not None:
+            raise RuntimeError("NativeSlabSimulator.gather needs torch.distributed; without it each rank download()s "
+                               "its owned planes and the host application assembles them")
         mine = torch.from_numpy(self.download()[key])
         if self.world > 1:
             t = mine.to(self.device)
@@ -444,8 +488,12 @@ class NativeSlabSimulator:
         return mine
 
     def frame_recorder(self, slots=3, share=None, barrier=None):
-        """A record.SlabFrameRecorder for this decomposition's global grid (collective; see there)."""
+        """A record.SlabFrameRecorder for this decomposition's global grid (collective; see there).  Without
+        torch.distributed, share and barrier default to the simulator's allgather and barrier."""
         from .record import SlabFrameRecorder
+        if self._allgather is not None:
+            share = share or (lambda b: self._allgather(b)[0])
+            barrier = barrier or self._barrier
         return SlabFrameRecorder(self._shape[2:], self.rank, self.world, slots, self.device, self.group, share, barrier)
 
     def field(self, key):
@@ -462,9 +510,18 @@ class NativeSlabSimulator:
         return rec.record_grid(self.field(key), self.zoff, writer)
 
     def close(self):
+        """Free the slab and the communicator.  Without torch.distributed (world > 1) this is collective: every rank
+        finishes its queued work and passes `barrier` before any rank frees its inbox (a neighbour's push may still be
+        landing in it), and passes it again before going on (e.g. to map the inboxes of a new simulator)."""
         if self.h:
+            collective = self._barrier is not None and self.world > 1
+            if collective:
+                torch.cuda.synchronize(self.device)
+                self._barrier()
             self.ctx.lib.tfl_slab_sim_destroy(self.ctx.h, self.h)
             self.h = None
+            if collective:
+                self._barrier()
         self.ctx.lib.tfl_comm_destroy(self.ctx.h)
 
 

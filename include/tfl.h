@@ -403,10 +403,14 @@ void tfl_step_graph_destroy(tfl_ctx* ctx, tfl_step_graph* graph);
 /* ---- one domain in z-slabs over the GPUs of a node (no counterpart in the reference, which is single-GPU;
  * SURVEY.md section 8e).  One process and one context per GPU.  The context owns the NCCL communicator
  * (libnccl.so.2 is loaded on demand); rank 0 makes an id, the host application distributes its
- * TFL_COMM_ID_BYTES bytes to every rank by its own means, every rank calls tfl_comm_init. */
+ * TFL_COMM_ID_BYTES bytes to every rank by its own means, every rank calls tfl_comm_init.
+ * world 1: no NCCL.  A NULL id_bytes with world > 1 sets the context's rank and world without a communicator: the
+ * slab step then exchanges halos and reduces its sums only over peer memory (tfl_slab_sim_ipc_connect on every
+ * rank before any rank steps; ranks may also be processes sharing one GPU).  Unconnected, its exchanges move
+ * nothing and the all-reduce is skipped -- one rank's workload alone, for profiling. */
 #define TFL_COMM_ID_BYTES 128
 int tfl_comm_unique_id(tfl_ctx* ctx, char* id_out /* TFL_COMM_ID_BYTES */);
-int tfl_comm_init(tfl_ctx* ctx, const char* id_bytes, int32_t rank, int32_t world);   /* world 1: no NCCL */
+int tfl_comm_init(tfl_ctx* ctx, const char* id_bytes, int32_t rank, int32_t world);
 int tfl_comm_destroy(tfl_ctx* ctx);
 /* Rank r keeps planes [z0, z1) of a [gnz][ny][nx] domain plus 2 * margin + 2 ghost planes per interior side
  * (margin = planes a backward trace may reach = ceil(max|u| dt) + 1, >= 2).  The host arrays are GLOBAL

@@ -51,6 +51,8 @@ EMU += [
     (4, 24, 16, 27, 2, 100, (False, False, False)),            # no forces, uneven
     (2, 128, 16, 13, 2, 34, (True, False, True)),              # one-launch block kernel
     (3, 128, 16, 20, 2, 100, (True, True, True)),
+    # rank 0 owns 9 planes: the last advection z tile runs past them, and counted faults there (DESIGN.md section 1)
+    (3, 128, 16, 26, 3, "k+1", (True, True, False)),
 ]
 
 
