@@ -100,7 +100,7 @@ int advect_vel_dispatch(tfl_ctx* ctx, float dt, const float* U, const FT* flags,
     if (hf > 0 && tl.dev && tl.host) {
       cudaMemsetAsync(tl.dev.get(), 0, sizeof(unsigned int), st);
       if (tl.timed) cudaEventRecord(tl.ev0.get(), st);
-      const bool launched = launch_advect_vel_tile(dt, U, fl8, clear, strength, dst, g, hf, tl.variant, tl.dev.get(), st);
+      const bool launched = launch_advect_vel_tile(dt, U, fl8, clear, strength, dst, g, hf, tl.dev.get(), st);
       if (tl.timed) cudaEventRecord(tl.ev1.get(), st);
       if (launched) {
         cudaMemcpyAsync(tl.host.get(), tl.dev.get(), sizeof(unsigned int), cudaMemcpyDeviceToHost, st);
@@ -119,7 +119,7 @@ int advect_scalar_dispatch(tfl_ctx* ctx, float dt, const float* s, const float* 
   ctx->tile.last_scalar_halo = 0;
   if (method == TFL_ADVECT_MACCORMACK_OURS && fl8 && clear && ctx->tile.mode != 0) {
     const int hf = tile_halo_choice(ctx, false);
-    if (hf > 0 && launch_advect_scalar_tile(dt, s, U, fl8, clear, outside, strength, dst, g, hf, ctx->tile.variant, st)) {
+    if (hf > 0 && launch_advect_scalar_tile(dt, s, U, fl8, clear, outside, strength, dst, g, hf, st)) {
       ctx->tile.last_scalar_halo = hf;
       return 1;
     }
@@ -790,11 +790,10 @@ int tfl_debug_make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is_3d) {
 }
 
 // Undocumented debugging hook.
-// mode: -1 automatic, 0 two-kernel advectVel, 1 / 2 tile kernel with that halo; variant: tile shape.
-int tfl_debug_advect_tile(tfl_ctx* ctx, int mode, int variant) {
+// mode: -1 automatic, 0 two-kernel advectVel, 1 / 2 tile kernel with that halo.
+int tfl_debug_advect_tile(tfl_ctx* ctx, int mode) {
   if (!ctx) return 1;
   ctx->tile.mode = mode;
-  ctx->tile.variant = variant;
   return 0;
 }
 
@@ -964,9 +963,10 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
 }
 
 // Whether tfl_simulate_step takes the fused pipeline for this state, configuration and model.
+// Its point-wise stages are 3-D kernels: the tensor-core stack (tc_ok) serves 3-D models only.
 static bool fused_step_applies(const tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, const tfl_cnn* cnn) {
   return mc->sim_method == TFL_SIM_CONVNET && cnn && cnn->tc_ok && cnn->mode > 0 && cnn->default_inputs && !ctx->slab &&
-         s->flags.nb == 1 &&
+         s->U.nc == 3 && s->flags.nb == 1 &&
          !s->p_bc.data && mc->advection_method >= 0 && mc->advection_method <= 5;
 }
 

@@ -69,7 +69,6 @@ struct tfl_ctx {
     DevPtr<unsigned int> dev;
     PinnedPtr<unsigned int> host;
     int mode = -1;                          // -1 automatic, 0 two-kernel version, 1 / 2 forced halo
-    int variant = 0;                        // tile shape (tuning)
     int calls_since_probe = 0;
     int last_vel_halo = 0, last_scalar_halo = 0;   // halo of the last dispatches' tile kernels (0: none ran)
     // bench.py's roofline: CUDA events right around the tile kernel's launch (off unless asked for)

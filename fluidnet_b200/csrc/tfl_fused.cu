@@ -3,7 +3,8 @@
 // SAME floating-point order, what a run of separate operators / cutorch calls does in the
 // reference loop, so results are bit-identical to the operator-by-operator sequence while
 // the velocity / density fields cross HBM once instead of once per operator.
-// Compiled with -fmad=false.
+// Compiled with -fmad=false.  The fused step runs the 3-D tensor-core stack only, so these stages are
+// 3-D kernels on the step's byte flags; the curl / force quads also serve the 2-D vorticity confinement.
 //
 //   k_post_advect        s:copy(tmp) ; U:copy(tmp)            (tfluids/init.lua:145-148, :215-218)
 //                        setConstVals (U, density)            (lib/simulate.lua:202, :130-160)
@@ -42,12 +43,11 @@ __device__ __forceinline__ float bc_apply(float x, const float* __restrict__ inv
 }
 
 // density = BC(tmp_s); U = BC(tmp_U) (+ buoyancy with the NEW density).
-template <bool IS3D, typename FT>
 __global__ void k_post_advect(const float* __restrict__ tmp_s, const float* __restrict__ tmp_u,
-                              const FT* __restrict__ flags, float* __restrict__ density,
+                              const unsigned char* __restrict__ flags, float* __restrict__ density,
                               float* __restrict__ U, BcPtrs bc, int do_buoy, float sx, float sy_, float sz_,
                               Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   const int c = cell(g, k, j, i);
@@ -63,7 +63,7 @@ __global__ void k_post_advect(const float* __restrict__ tmp_s, const float* __re
   float u[3];
   for (int a = 0; a < g.nc; a++) u[a] = bc_apply(__ldg(tmp_u + ub + a * g.n + c), bc.u_inv, bc.u_bc, ub + a * g.n + c);
   if (do_buoy && density && !on_border(g, k, j, i)) {
-    const FT* fl = flags + sb;
+    const unsigned char* fl = flags + sb;
     if (flag_i(fl, g, k, j, i) & kFluid) {
       const int st[3] = {1, g.nx, g.nx * g.ny};
       const float str[3] = {sx, sy_, sz_};
@@ -84,18 +84,17 @@ __global__ void k_post_advect(const float* __restrict__ tmp_s, const float* __re
 
 // U += confinement force; U = BC(U); then (mask_mode 1) U *= wall mask and accumulate the
 // sums for the input scale.
-template <bool IS3D, typename FT>
-__global__ void k_vort_bc_mask(float* __restrict__ U, const FT* __restrict__ flags,
+__global__ void k_vort_bc_mask(float* __restrict__ U, const unsigned char* __restrict__ flags,
                                const float* __restrict__ force, int do_vort, BcPtrs bc, int mask_mode,
                                double* __restrict__ sums, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i;
   const bool live = thread_cell(g, b, k, j, i);
   double s = 0.0, ss = 0.0;
   if (live) {
     const int c = cell(g, k, j, i);
     const long long ub = (long long)b * g.nc * g.n;
-    const FT* fl = flags + b * g.n;
+    const unsigned char* fl = flags + b * g.n;
     float u[3];
     for (int a = 0; a < g.nc; a++) u[a] = U[ub + a * g.n + c];
     if (do_vort && !on_border(g, k, j, i)) {
@@ -135,12 +134,11 @@ __global__ void k_vort_bc_mask(float* __restrict__ U, const FT* __restrict__ fla
 
 // First channels-last plane of the conv input: (pDiv/s, div(U1)/s, occupancy, 0); U1 is the
 // already masked velocity left in U by k_vort_bc_mask.
-template <bool IS3D, typename FT>
 __global__ void k_cnn_inputs_fused(const float* __restrict__ p_div, const float* __restrict__ U1,
-                                   const FT* __restrict__ flags, const double* __restrict__ sums,
+                                   const unsigned char* __restrict__ flags, const double* __restrict__ sums,
                                    float threshold, float* __restrict__ scale_out, float4* __restrict__ x0,
                                    int px, int py, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   const int c = cell(g, k, j, i);
@@ -160,16 +158,15 @@ __global__ void k_cnn_inputs_fused(const float* __restrict__ p_div, const float*
 }
 
 // U = clamp(BC(setWallBcs(velocityUpdate(U1 / s, p_net) * s)));  p = p_net * s.  In place on U.
-template <bool IS3D, typename FT>
 __global__ void k_cnn_finish_fused(const float* __restrict__ p_net, float* __restrict__ U,
-                                   const FT* __restrict__ flags, const float* __restrict__ scale,
+                                   const unsigned char* __restrict__ flags, const float* __restrict__ scale,
                                    float* __restrict__ p_out, BcPtrs bc, float lo, float hi, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   const int c = cell(g, k, j, i);
   const float sc = __ldg(scale + b);
-  const FT* fl = flags + b * g.n;
+  const unsigned char* fl = flags + b * g.n;
   const float* pb = p_net + b * g.n;
   const long long ub = (long long)b * g.nc * g.n;
   const float pc = __ldg(pb + c);
@@ -236,9 +233,9 @@ __device__ __forceinline__ void st4(float* p, const float (&v)[4]) {
 }
 __device__ __forceinline__ void zero4(float (&o)[4]) { o[0] = o[1] = o[2] = o[3] = 0.0f; }
 
-// wall_bc_zero_mask (tfl_device.cuh) on flag values; a neighbour outside the grid is passed as 0.
+// wall_bc_zero_mask (tfl_device.cuh) on flag values of a 3-D grid; a neighbour outside the grid is passed as 0.
 __device__ __forceinline__ void wall_mask_from_flags(int fc, int fxm, int fxp, int fym, int fyp, int fzm, int fzp,
-                                                     bool is3d, bool z[3]) {
+                                                     bool z[3]) {
   z[0] = z[1] = z[2] = false;
   const bool cf = fc & kFluid, co = fc & kObstacle;
   if (!cf && !co) return;
@@ -246,9 +243,9 @@ __device__ __forceinline__ void wall_mask_from_flags(int fc, int fxm, int fxp, i
   if ((fym & kObstacle) || (co && (fym & kFluid))) z[1] = true;
   if ((fzm & kObstacle) || (co && (fzm & kFluid))) z[2] = true;
   if (cf) {
-    if ((fxm & kStick) || (fxp & kStick)) { z[1] = true; if (is3d) z[2] = true; }
-    if ((fym & kStick) || (fyp & kStick)) { z[0] = true; if (is3d) z[2] = true; }
-    if (is3d && ((fzm & kStick) || (fzp & kStick))) { z[0] = true; z[1] = true; }
+    if ((fxm & kStick) || (fxp & kStick)) { z[1] = true; z[2] = true; }
+    if ((fym & kStick) || (fyp & kStick)) { z[0] = true; z[2] = true; }
+    if ((fzm & kStick) || (fzp & kStick)) { z[0] = true; z[1] = true; }
   }
 }
 
@@ -262,14 +259,13 @@ __device__ __forceinline__ bool thread_cell4(const Geo& g, int& b, int& k, int& 
   return i0 < g.nx && j < g.ny && b < g.nb;
 }
 
-// The flag values around a quad: centre row, the scalars left / right of it, and the four rows around.
+// The flag values around a quad of a 3-D grid: centre row, the scalars left / right of it, and the four rows around.
 struct QuadFlags {
   Flags4 c, ym, yp, zm, zp;
   int left, right;
   __device__ __forceinline__ int xm(int v) const { return v == 0 ? left : c.c[v - 1]; }
   __device__ __forceinline__ int xp(int v) const { return v == 3 ? right : c.c[v + 1]; }
 };
-template <bool IS3D>
 __device__ __forceinline__ QuadFlags quad_flags(const unsigned char* __restrict__ fl, const Geo& g, int c0, int k, int j,
                                                 int i0, bool need_plus) {
   QuadFlags q;
@@ -277,19 +273,18 @@ __device__ __forceinline__ QuadFlags quad_flags(const unsigned char* __restrict_
   q.c = flags4(fl + c0, true);
   q.left = i0 > 0 ? (int)__ldg(fl + c0 - 1) : 0;
   q.ym = flags4(fl + c0 - sy, j > 0);
-  q.zm = flags4(fl + c0 - sz, IS3D && k > 0);
+  q.zm = flags4(fl + c0 - sz, k > 0);
   q.right = (need_plus && i0 + 4 < g.nx) ? (int)__ldg(fl + c0 + 4) : 0;
   q.yp = flags4(fl + c0 + sy, need_plus && j < g.ny - 1);
-  q.zp = flags4(fl + c0 + sz, need_plus && IS3D && k < g.nz - 1);
+  q.zp = flags4(fl + c0 + sz, need_plus && k < g.nz - 1);
   return q;
 }
 
-template <bool IS3D>
 __global__ void __launch_bounds__(256) k_post_advect4(const float* __restrict__ tmp_s, const float* __restrict__ tmp_u,
                                                       const unsigned char* __restrict__ flags, float* __restrict__ density,
                                                       float* __restrict__ U, BcPtrs bc, int do_buoy, float sx, float sy_,
                                                       float sz_, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i0;
   if (!thread_cell4(g, b, k, j, i0)) return;
   const int c0 = cell(g, k, j, i0);
@@ -356,7 +351,7 @@ __global__ void __launch_bounds__(256) k_post_advect4(const float* __restrict__ 
     }
   }
   if (do_buoy && density) {
-    const QuadFlags q = quad_flags<IS3D>(flags + sb, g, c0, k, j, i0, false);
+    const QuadFlags q = quad_flags(flags + sb, g, c0, k, j, i0, false);
     // density (after its BC) of the -x / -y / -z neighbours
     float rl = 0.0f, ry[4], rz[4];
     zero4(ry); zero4(rz);
@@ -368,24 +363,23 @@ __global__ void __launch_bounds__(256) k_post_advect4(const float* __restrict__ 
       }
     }
     if (j > 0) dens_bc(sb + c0 - sy, ry);
-    if (IS3D && k > 0) dens_bc(sb + c0 - sz, rz);
+    if (k > 0) dens_bc(sb + c0 - sz, rz);
 #pragma unroll
     for (int v = 0; v < 4; v++) {
       if (on_border(g, k, j, i0 + v) || !(q.c.c[v] & kFluid)) continue;
       if (q.xm(v) & kFluid) u[0][v] += (0.5f * sx * (rc[v] + (v == 0 ? rl : rc[v - 1])));
       if (q.ym.c[v] & kFluid) u[1][v] += (0.5f * sy_ * (rc[v] + ry[v]));
-      if (IS3D && (q.zm.c[v] & kFluid)) u[2][v] += (0.5f * sz_ * (rc[v] + rz[v]));
+      if (q.zm.c[v] & kFluid) u[2][v] += (0.5f * sz_ * (rc[v] + rz[v]));
     }
   }
 #pragma unroll
   for (int a = 0; a < 3; a++) if (a < g.nc) st4(U + ub + a * g.n + c0, u[a]);
 }
 
-template <bool IS3D>
 __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, const unsigned char* __restrict__ flags,
                                                        const float* __restrict__ force, int do_vort, BcPtrs bc,
                                                        int mask_mode, double* __restrict__ sums, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i0;
   const bool live = thread_cell4(g, b, k, j, i0);
   double s = 0.0, ss = 0.0;
@@ -393,7 +387,7 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
     const int c0 = cell(g, k, j, i0);
     const int sy = g.nx, sz = g.nx * g.ny;
     const long long ub = (long long)b * g.nc * g.n;
-    const QuadFlags q = quad_flags<IS3D>(flags + b * g.n, g, c0, k, j, i0, mask_mode != 0);
+    const QuadFlags q = quad_flags(flags + b * g.n, g, c0, k, j, i0, mask_mode != 0);
     float u[3][4];
 #pragma unroll
     for (int a = 0; a < 3; a++) if (a < g.nc) ld4_rw(U + ub + a * g.n + c0, u[a]);
@@ -405,10 +399,8 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
       ld4(fb + g.n + c0, fy);
       zero4(fyl); zero4(fz); zero4(fzl);
       if (j > 0) ld4(fb + g.n + c0 - sy, fyl);
-      if (IS3D) {
-        ld4(fb + 2 * g.n + c0, fz);
-        if (k > 0) ld4(fb + 2 * g.n + c0 - sz, fzl);
-      }
+      ld4(fb + 2 * g.n + c0, fz);
+      if (k > 0) ld4(fb + 2 * g.n + c0 - sz, fzl);
 #pragma unroll
       for (int v = 0; v < 4; v++) {
         if (on_border(g, k, j, i0 + v)) continue;
@@ -419,10 +411,8 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
         if ((f & kFluid) || (cf && (f & kEmpty))) u[0][v] += (0.5f * ((v == 0 ? fxl : fx[v - 1]) + fx[v]));
         f = q.ym.c[v];
         if ((f & kFluid) || (cf && (f & kEmpty))) u[1][v] += (0.5f * (fyl[v] + fy[v]));
-        if (IS3D) {
-          f = q.zm.c[v];
-          if ((f & kFluid) || (cf && (f & kEmpty))) u[2][v] += (0.5f * (fzl[v] + fz[v]));
-        }
+        f = q.zm.c[v];
+        if ((f & kFluid) || (cf && (f & kEmpty))) u[2][v] += (0.5f * (fzl[v] + fz[v]));
       }
     }
     if (bc.u_inv) {
@@ -447,7 +437,7 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
 #pragma unroll
       for (int v = 0; v < 4; v++) {
         bool z[3];
-        wall_mask_from_flags(q.c.c[v], q.xm(v), q.xp(v), q.ym.c[v], q.yp.c[v], q.zm.c[v], q.zp.c[v], IS3D, z);
+        wall_mask_from_flags(q.c.c[v], q.xm(v), q.xp(v), q.ym.c[v], q.yp.c[v], q.zm.c[v], q.zp.c[v], z);
 #pragma unroll
         for (int a = 0; a < 3; a++) {
           if (a < g.nc) {
@@ -465,13 +455,12 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
   if (mask_mode) block_accumulate(s, ss, sums + 2 * (live ? b : 0));
 }
 
-template <bool IS3D>
 __global__ void __launch_bounds__(256) k_cnn_inputs_fused4(const float* __restrict__ p_div, const float* __restrict__ U1,
                                                            const unsigned char* __restrict__ flags,
                                                            const double* __restrict__ sums, float threshold,
                                                            float* __restrict__ scale_out, float4* __restrict__ x0, int px,
                                                            int py, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i0;
   if (!thread_cell4(g, b, k, j, i0)) return;
   const int c0 = cell(g, k, j, i0);
@@ -486,10 +475,8 @@ __global__ void __launch_bounds__(256) k_cnn_inputs_fused4(const float* __restri
   ld4(ub + g.n + c0, uy);
   zero4(uyp); zero4(uz); zero4(uzp);
   if (j < g.ny - 1) ld4(ub + g.n + c0 + sy, uyp);
-  if (IS3D) {
-    ld4(ub + 2 * g.n + c0, uz);
-    if (k < g.nz - 1) ld4(ub + 2 * g.n + c0 + sz, uzp);
-  }
+  ld4(ub + 2 * g.n + c0, uz);
+  if (k < g.nz - 1) ld4(ub + 2 * g.n + c0 + sz, uzp);
   ld4(p_div + b * g.n + c0, pd);
   const long long plane = (long long)(g.nz + 2) * py * px;
   const long long o = (long long)b * 2 * plane + ((long long)(k + 1) * py + (j + 1)) * px + (i0 + 1);
@@ -499,18 +486,17 @@ __global__ void __launch_bounds__(256) k_cnn_inputs_fused4(const float* __restri
     float dv = 0.0f;
     if (!on_border(g, k, j, i0 + v) && (f & kFluid)) {
       dv = ux[v] - (v == 3 ? uxr : ux[v + 1]) + uy[v] - uyp[v];
-      if (IS3D) dv += (uz[v] - uzp[v]);
+      dv += (uz[v] - uzp[v]);
     }
     x0[o + v] = make_float4(pd[v] / sc, dv / sc, (f == kFluid) ? 0.0f : ((f == kObstacle) ? 1.0f : -1.0f), 0.0f);
   }
 }
 
-template <bool IS3D>
 __global__ void __launch_bounds__(256) k_cnn_finish_fused4(const float* __restrict__ p_net, float* __restrict__ U,
                                                            const unsigned char* __restrict__ flags,
                                                            const float* __restrict__ scale, float* __restrict__ p_out,
                                                            BcPtrs bc, float lo, float hi, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i0;
   if (!thread_cell4(g, b, k, j, i0)) return;
   const int c0 = cell(g, k, j, i0);
@@ -518,13 +504,13 @@ __global__ void __launch_bounds__(256) k_cnn_finish_fused4(const float* __restri
   const float sc = __ldg(scale + b);
   const float* pb = p_net + b * g.n;
   const long long ub = (long long)b * g.nc * g.n;
-  const QuadFlags q = quad_flags<IS3D>(flags + b * g.n, g, c0, k, j, i0, true);
+  const QuadFlags q = quad_flags(flags + b * g.n, g, c0, k, j, i0, true);
   float pc[4], py_[4], pz[4];
   ld4(pb + c0, pc);
   const float pl = i0 > 0 ? __ldg(pb + c0 - 1) : 0.0f;
   zero4(py_); zero4(pz);
   if (j > 0) ld4(pb + c0 - sy, py_);
-  if (IS3D && k > 0) ld4(pb + c0 - sz, pz);
+  if (k > 0) ld4(pb + c0 - sz, pz);
   float u[3][4];
 #pragma unroll
   for (int a = 0; a < 3; a++) {
@@ -538,7 +524,7 @@ __global__ void __launch_bounds__(256) k_cnn_finish_fused4(const float* __restri
   for (int v = 0; v < 4; v++) {
     if (on_border(g, k, j, i0 + v)) continue;
     const int fc = q.c.c[v];
-    const int fn[3] = {q.xm(v), q.ym.c[v], IS3D ? q.zm.c[v] : 0};
+    const int fn[3] = {q.xm(v), q.ym.c[v], q.zm.c[v]};
     const float pn[3] = {v == 0 ? pl : pc[v - 1], py_[v], pz[v]};
     if (fc & kFluid) {
 #pragma unroll
@@ -561,7 +547,7 @@ __global__ void __launch_bounds__(256) k_cnn_finish_fused4(const float* __restri
   bool z[4][3];
 #pragma unroll
   for (int v = 0; v < 4; v++)
-    wall_mask_from_flags(q.c.c[v], q.xm(v), q.xp(v), q.ym.c[v], q.yp.c[v], q.zm.c[v], q.zp.c[v], IS3D, z[v]);
+    wall_mask_from_flags(q.c.c[v], q.xm(v), q.xp(v), q.ym.c[v], q.yp.c[v], q.zm.c[v], q.zp.c[v], z[v]);
   const bool bc_identity_quad = bc.qmask && (__ldg(bc.qmask + ((b * g.n + c0) >> 2)) & 1);
 #pragma unroll
   for (int a = 0; a < 3; a++) {
@@ -718,11 +704,10 @@ __global__ void __launch_bounds__(256) k_vort_force4(const float* __restrict__ c
 }
 
 // One byte per quad: which BCs are the identity pair there (see BcPtrs::qmask).
-template <bool IS3D>
 __global__ void __launch_bounds__(256) k_bc_quad_mask(const float* __restrict__ u_inv, const float* __restrict__ u_bc,
                                                       const float* __restrict__ d_inv, const float* __restrict__ d_bc,
                                                       unsigned char* __restrict__ qmask, Geo gin) {
-  const Geo g = static_geo<IS3D>(gin);
+  const Geo g = static_geo<true>(gin);
   int b, k, j, i0;
   if (!thread_cell4(g, b, k, j, i0)) return;
   const long long o = b * g.n + cell(g, k, j, i0);
@@ -765,27 +750,18 @@ static inline bool aligned16(std::initializer_list<const void*> ptrs) {
     if (((uintptr_t)p & 15u) != 0) return false;
   return true;
 }
-#define TFL_LAUNCH4F(kernel, g, grid_, block_, st, ...)                            \
-  do {                                                                              \
-    if ((g).is3d) kernel<true><<<grid_, block_, 0, st>>>(__VA_ARGS__);              \
-    else kernel<false><<<grid_, block_, 0, st>>>(__VA_ARGS__);                      \
-  } while (0)
-
-#define TFL_LAUNCH3F(kernel, g, st, ...)                                                \
-  do {                                                                                  \
-    dim3 grid_, block_;                                                                 \
-    launch_dims(g, grid_, block_);                                                      \
-    if ((g).is3d) kernel<true, unsigned char><<<grid_, block_, 0, st>>>(__VA_ARGS__);   \
-    else kernel<false, unsigned char><<<grid_, block_, 0, st>>>(__VA_ARGS__);           \
-  } while (0)
-
 // Quad versions of curl + force over the whole grid; false if the shape does not fit (caller falls back).
 bool launch_vort_curl_quad(const float* U, float* curl, float* cnorm, float* force, float strength, const Geo& g,
                            cudaStream_t st) {
   dim3 qg, qb;
   if (!quad_dims(g, qg, qb) || !aligned16({U, curl, cnorm, force})) return false;
-  TFL_LAUNCH4F(k_vort_curl4, g, qg, qb, st, U, curl, cnorm, g);
-  TFL_LAUNCH4F(k_vort_force4, g, qg, qb, st, curl, cnorm, force, strength, g);
+  if (g.is3d) {
+    k_vort_curl4<true><<<qg, qb, 0, st>>>(U, curl, cnorm, g);
+    k_vort_force4<true><<<qg, qb, 0, st>>>(curl, cnorm, force, strength, g);
+  } else {
+    k_vort_curl4<false><<<qg, qb, 0, st>>>(U, curl, cnorm, g);
+    k_vort_force4<false><<<qg, qb, 0, st>>>(curl, cnorm, force, strength, g);
+  }
   return true;
 }
 
@@ -794,7 +770,7 @@ bool launch_bc_quad_mask(const float* u_inv, const float* u_bc, const float* d_i
                          unsigned char* qmask, const Geo& g, cudaStream_t st) {
   dim3 qg, qb;
   if (!quad_dims(g, qg, qb) || !aligned16({u_inv, u_bc, d_inv, d_bc}) || (!u_inv && !d_inv)) return false;
-  TFL_LAUNCH4F(k_bc_quad_mask, g, qg, qb, st, u_inv, u_bc, d_inv, d_bc, qmask, g);
+  k_bc_quad_mask<<<qg, qb, 0, st>>>(u_inv, u_bc, d_inv, d_bc, qmask, g);
   return true;
 }
 
@@ -802,44 +778,48 @@ void launch_post_advect(const float* tmp_s, const float* tmp_u, const unsigned c
                         const float* u_inv, const float* u_bc, const float* d_inv, const float* d_bc,
                         const unsigned char* qmask, int do_buoy, const float s[3], const Geo& g, cudaStream_t st) {
   BcPtrs bc{u_inv, u_bc, d_inv, d_bc, qmask};
-  dim3 qg, qb;
-  if (quad_dims(g, qg, qb) && aligned16({tmp_s, tmp_u, flags, density, U, u_inv, u_bc, d_inv, d_bc})) {
-    TFL_LAUNCH4F(k_post_advect4, g, qg, qb, st, tmp_s, tmp_u, flags, density, U, bc, do_buoy, s[0], s[1], s[2], g);
+  dim3 grid, block;
+  if (quad_dims(g, grid, block) && aligned16({tmp_s, tmp_u, flags, density, U, u_inv, u_bc, d_inv, d_bc})) {
+    k_post_advect4<<<grid, block, 0, st>>>(tmp_s, tmp_u, flags, density, U, bc, do_buoy, s[0], s[1], s[2], g);
     return;
   }
-  TFL_LAUNCH3F(k_post_advect, g, st, tmp_s, tmp_u, flags, density, U, bc, do_buoy, s[0], s[1], s[2], g);
+  launch_dims(g, grid, block);
+  k_post_advect<<<grid, block, 0, st>>>(tmp_s, tmp_u, flags, density, U, bc, do_buoy, s[0], s[1], s[2], g);
 }
 void launch_vort_bc_mask(float* U, const unsigned char* flags, const float* force, int do_vort,
                          const float* u_inv, const float* u_bc, const unsigned char* qmask, int mask_mode, double* sums,
                          const Geo& g, cudaStream_t st) {
   BcPtrs bc{u_inv, u_bc, nullptr, nullptr, qmask};
-  dim3 qg, qb;
-  if (quad_dims(g, qg, qb) && aligned16({U, flags, force, u_inv, u_bc})) {
-    TFL_LAUNCH4F(k_vort_bc_mask4, g, qg, qb, st, U, flags, force, do_vort, bc, mask_mode, sums, g);
+  dim3 grid, block;
+  if (quad_dims(g, grid, block) && aligned16({U, flags, force, u_inv, u_bc})) {
+    k_vort_bc_mask4<<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
     return;
   }
-  TFL_LAUNCH3F(k_vort_bc_mask, g, st, U, flags, force, do_vort, bc, mask_mode, sums, g);
+  launch_dims(g, grid, block);
+  k_vort_bc_mask<<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
 }
 void launch_cnn_inputs_fused(const float* p_div, const float* U1, const unsigned char* flags, const double* sums,
                              float threshold, float* scale_out, float* x0, int px, int py, const Geo& g,
                              cudaStream_t st) {
-  dim3 qg, qb;
-  if (quad_dims(g, qg, qb) && aligned16({p_div, U1, flags, x0})) {
-    TFL_LAUNCH4F(k_cnn_inputs_fused4, g, qg, qb, st, p_div, U1, flags, sums, threshold, scale_out, (float4*)x0, px, py, g);
+  dim3 grid, block;
+  if (quad_dims(g, grid, block) && aligned16({p_div, U1, flags, x0})) {
+    k_cnn_inputs_fused4<<<grid, block, 0, st>>>(p_div, U1, flags, sums, threshold, scale_out, (float4*)x0, px, py, g);
     return;
   }
-  TFL_LAUNCH3F(k_cnn_inputs_fused, g, st, p_div, U1, flags, sums, threshold, scale_out, (float4*)x0, px, py, g);
+  launch_dims(g, grid, block);
+  k_cnn_inputs_fused<<<grid, block, 0, st>>>(p_div, U1, flags, sums, threshold, scale_out, (float4*)x0, px, py, g);
 }
 void launch_cnn_finish_fused(const float* p_net, float* U, const unsigned char* flags, const float* scale, float* p_out,
                              const float* u_inv, const float* u_bc, const unsigned char* qmask, float lo, float hi,
                              const Geo& g, cudaStream_t st) {
   BcPtrs bc{u_inv, u_bc, nullptr, nullptr, qmask};
-  dim3 qg, qb;
-  if (quad_dims(g, qg, qb) && aligned16({p_net, U, flags, p_out, u_inv, u_bc})) {
-    TFL_LAUNCH4F(k_cnn_finish_fused4, g, qg, qb, st, p_net, U, flags, scale, p_out, bc, lo, hi, g);
+  dim3 grid, block;
+  if (quad_dims(g, grid, block) && aligned16({p_net, U, flags, p_out, u_inv, u_bc})) {
+    k_cnn_finish_fused4<<<grid, block, 0, st>>>(p_net, U, flags, scale, p_out, bc, lo, hi, g);
     return;
   }
-  TFL_LAUNCH3F(k_cnn_finish_fused, g, st, p_net, U, flags, scale, p_out, bc, lo, hi, g);
+  launch_dims(g, grid, block);
+  k_cnn_finish_fused<<<grid, block, 0, st>>>(p_net, U, flags, scale, p_out, bc, lo, hi, g);
 }
 
 }  // namespace tfl

@@ -12,20 +12,16 @@ namespace tfl {
 void launch_empty_domain(float* flags, const Geo& g, int bnd, cudaStream_t st);
 void launch_flags_to_occupancy(const float* flags, float* occ, long long n, unsigned long long* bad,
                                cudaStream_t st);
-template <typename FT>
-void launch_set_wall_bcs(float* U, const FT* flags, const Geo& g, int as_mask, cudaStream_t st);
-template <typename FT>
-void launch_divergence(const float* U, const FT* flags, float* div, const Geo& g, cudaStream_t st);
-template <typename FT>
-void launch_velocity_update(float* U, const FT* flags, const float* p, const Geo& g, cudaStream_t st);
-template <typename FT>
-void launch_add_buoyancy(float* U, const FT* flags, const float* rho, const float s[3], const Geo& g,
+void launch_set_wall_bcs(float* U, const float* flags, const Geo& g, int as_mask, cudaStream_t st);
+void launch_divergence(const float* U, const float* flags, float* div, const Geo& g, cudaStream_t st);
+void launch_velocity_update(float* U, const float* flags, const float* p, const Geo& g, cudaStream_t st);
+void launch_add_buoyancy(float* U, const float* flags, const float* rho, const float s[3], const Geo& g,
                          cudaStream_t st);
+int launch_vorticity(float* U, const float* flags, float strength, float* curl, float* cnorm, float* force,
+                     const Geo& g, cudaStream_t st);
+// Gravity and advection take the operators' float flags or the fused step's byte flags (FT float or unsigned char).
 template <typename FT>
 void launch_add_gravity(float* U, const FT* flags, const float f[3], const Geo& g, cudaStream_t st);
-template <typename FT>
-int launch_vorticity(float* U, const FT* flags, float strength, float* curl, float* cnorm, float* force,
-                     const Geo& g, cudaStream_t st);
 // g: range of the result; g_fwd: (wider, in slab mode) range of the forward pass.
 // clear: clearance field of the same grid (launch_clearance) or nullptr (general code everywhere).
 template <typename FT>
@@ -40,19 +36,16 @@ int launch_advect_vel(float dt, const float* U, const FT* flags, const unsigned 
 // take the general code).  longest: optional device word, atomicMax of the longest trace (float bits).
 // Returns false when the grid does not qualify (2-D, batch, slab, nx % 4 != 0): run launch_advect_vel then.
 bool launch_advect_vel_tile(float dt, const float* U, const unsigned char* flags, const unsigned char* clear,
-                            float strength, float* dst, const Geo& g, int hf, int variant, unsigned int* longest,
-                            cudaStream_t st);
+                            float strength, float* dst, const Geo& g, int hf, unsigned int* longest, cudaStream_t st);
 // advectScalar('maccormackOurs') on the same tiles.
 bool launch_advect_scalar_tile(float dt, const float* src, const float* U, const unsigned char* flags,
                                const unsigned char* clear, int outside, float strength, float* dst, const Geo& g, int hf,
-                               int variant, cudaStream_t st);
-// Clearance of every cell of the local storage (advection fast path, tfl_device.cuh); tmp: scratch of the
-// same size; gate: optional device word, the kernels do nothing when it is 0.  Returns the launch count.
-template <typename FT>
-int launch_clearance(const FT* flags, unsigned char* clear, unsigned char* tmp, const Geo& g, const int* gate,
+                               cudaStream_t st);
+// Clearance of every cell of the local storage (advection fast path, tfl_device.cuh) from the byte flags; tmp:
+// scratch of the same size; gate: optional device word, the kernels do nothing when it is 0.  Returns the launch count.
+int launch_clearance(const unsigned char* flags, unsigned char* clear, unsigned char* tmp, const Geo& g, const int* gate,
                      cudaStream_t st);
-template <typename FT>
-void launch_jacobi_mask(const FT* flags, unsigned char* mask, const Geo& g, cudaStream_t st);
+void launch_jacobi_mask(const float* flags, unsigned char* mask, const Geo& g, cudaStream_t st);
 void launch_jacobi_iter(const unsigned char* mask, const float* div, const float* prev, float* cur,
                         const Geo& g, cudaStream_t st);
 // One block of `sweeps` sweeps on local planes [z_lo, z_hi) that shrink by shr_lo / shr_hi planes per sweep
@@ -98,6 +91,8 @@ void launch_cnn_finish(const float* p_net, const float* U1, const float* flags, 
                        float* p_out, float* U_out, const Geo& g, cudaStream_t st);
 
 // ---- tfl_fused.cu (-fmad=false): fused point-wise stages of the convnet step ----
+// The stages other than launch_vort_curl(_quad), which the 2-D vorticity confinement shares, run on 3-D grids with
+// byte flags only: the fused step requires them (fused_step_applies, tfl_api.cu).
 // qmask (may be null): BcPtrs::qmask of tfl_fused.cu, filled by launch_bc_quad_mask for the same step.
 bool launch_bc_quad_mask(const float* u_inv, const float* u_bc, const float* d_inv, const float* d_bc,
                          unsigned char* qmask, const Geo& g, cudaStream_t st);

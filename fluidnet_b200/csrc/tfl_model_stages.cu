@@ -26,8 +26,8 @@ __device__ __forceinline__ void add_entry_sums(double s, double ss, double* __re
 
 // U1 = U * wallmask; sums[b] += (sum f, sum f^2) over the owned planes (double), f = U1 (kCnnStatU) or pDiv
 // (kCnnStatPDiv, normalizeInputChan 'pDiv'); kCnnStatDiv leaves the sums to k_cnn_div_stats.
-template <bool IS3D, typename FT>
-__global__ void k_cnn_mask_stats(const float* __restrict__ U, const FT* __restrict__ flags,
+template <bool IS3D>
+__global__ void k_cnn_mask_stats(const float* __restrict__ U, const float* __restrict__ flags,
                                  float* __restrict__ U1, double* __restrict__ sums, int own_lo, int own_hi, int stat,
                                  const float* __restrict__ p_div, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
@@ -60,8 +60,7 @@ __global__ void k_cnn_mask_stats(const float* __restrict__ U, const FT* __restri
 }
 
 // tfluids.VelocityDivergence of the masked velocity at cell c (lib/model.lua:86-89).
-template <typename FT>
-__device__ __forceinline__ float cnn_div(const float* __restrict__ ub, const FT* __restrict__ fb, const Geo& g, int k,
+__device__ __forceinline__ float cnn_div(const float* __restrict__ ub, const float* __restrict__ fb, const Geo& g, int k,
                                          int j, int i, int c, int* flag) {
   const int f = flag_i(fb, g, k, j, i);
   *flag = f;
@@ -74,8 +73,8 @@ __device__ __forceinline__ float cnn_div(const float* __restrict__ ub, const FT*
 }
 
 // normalizeInputChan 'div': sums[b] += (sum div, sum div^2) over the owned planes, once U1 is complete.
-template <bool IS3D, typename FT>
-__global__ void k_cnn_div_stats(const float* __restrict__ U1, const FT* __restrict__ flags, double* __restrict__ sums,
+template <bool IS3D>
+__global__ void k_cnn_div_stats(const float* __restrict__ U1, const float* __restrict__ flags, double* __restrict__ sums,
                                 int own_lo, int own_hi, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
@@ -117,9 +116,8 @@ __device__ __forceinline__ void put_channel(float (&v)[8], int& n, float x) {
 
 // The network input at one cell (nn.JoinTable(2), lib/model.lua:133-150): pDiv / s, U1 / s (nc), div / s,
 // occupancy(flags), the channels of `sel` only, then zeros up to 8.  Returns the channel count.
-template <typename FT>
 __device__ __forceinline__ int cnn_input_channels(const float* __restrict__ p_div, const float* __restrict__ ub,
-                                                  const FT* __restrict__ fb, float sc, int sel, const Geo& g, int b,
+                                                  const float* __restrict__ fb, float sc, int sel, const Geo& g, int b,
                                                   int k, int j, int i, int c, float (&v)[8]) {
   int f;
   const float dv = cnn_div(ub, fb, g, k, j, i, c, &f);
@@ -135,9 +133,9 @@ __device__ __forceinline__ int cnn_input_channels(const float* __restrict__ p_di
 }
 
 // x0 [b][cin][n] = the input channels of `sel` (default: pDiv / s, div(U1) / s, occupancy(flags)).
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_cnn_inputs(const float* __restrict__ p_div, const float* __restrict__ U1,
-                             const FT* __restrict__ flags, const float* __restrict__ scale,
+                             const float* __restrict__ flags, const float* __restrict__ scale,
                              float* __restrict__ x0, int sel, int cin, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
@@ -155,9 +153,9 @@ __global__ void k_cnn_inputs(const float* __restrict__ p_div, const float* __res
 // Same input channels written channels-last into the padded activation layout the tensor-core convolution reads
 // (tfl_cnn_tc.cu): the first float4 plane (planes = 1: up to 3 channels, zero fourth) or both planes (planes = 2:
 // channels 0-3 and 4-7, zero-padded), e.g. the default set as (pDiv/s, div/s, occ, 0).
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_cnn_inputs_padded(const float* __restrict__ p_div, const float* __restrict__ U1,
-                                    const FT* __restrict__ flags, const float* __restrict__ scale,
+                                    const float* __restrict__ flags, const float* __restrict__ scale,
                                     float4* __restrict__ x0, int sel, int planes, int px, int py, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
@@ -175,7 +173,7 @@ __global__ void k_cnn_inputs_padded(const float* __restrict__ p_div, const float
 // addPressureSkip (lib/model.lua:357-361): the last convolution is 1x1, so its pDiv input channel adds
 // w_skip * pDiv_scaled to p_net.  A pass of its own because the velocity update reads p at the neighbours while
 // p_out, which may alias pDiv, is written.
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_cnn_skip(float* __restrict__ p_net, const float* __restrict__ p_div, const float* __restrict__ scale,
                            float w_skip, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
@@ -186,16 +184,16 @@ __global__ void k_cnn_skip(float* __restrict__ p_net, const float* __restrict__ 
 }
 
 // U = setWallBcs(velocityUpdate(U1 / scale, p_net) * scale);  p = p_net * scale.
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_cnn_finish(const float* __restrict__ p_net, const float* __restrict__ U1,
-                             const FT* __restrict__ flags, const float* __restrict__ scale,
+                             const float* __restrict__ flags, const float* __restrict__ scale,
                              float* __restrict__ p_out, float* __restrict__ U_out, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   const int c = cell(g, k, j, i);
   const float sc = __ldg(scale + b);
-  const FT* fl = flags + b * g.n;
+  const float* fl = flags + b * g.n;
   const float* pb = p_net + b * g.n;
   const float* ub = U1 + (long long)b * g.nc * g.n;
   const float pc = __ldg(pb + c);
@@ -235,8 +233,8 @@ __global__ void k_cnn_finish(const float* __restrict__ p_net, const float* __res
   do {                                                                          \
     dim3 grid_, block_;                                                         \
     launch_dims(g, grid_, block_);                                              \
-    if ((g).is3d) kernel<true, float><<<grid_, block_, 0, st>>>(__VA_ARGS__);   \
-    else kernel<false, float><<<grid_, block_, 0, st>>>(__VA_ARGS__);           \
+    if ((g).is3d) kernel<true><<<grid_, block_, 0, st>>>(__VA_ARGS__);          \
+    else kernel<false><<<grid_, block_, 0, st>>>(__VA_ARGS__);                  \
   } while (0)
 
 void launch_cnn_mask_stats(const float* U, const float* flags, float* U1, double* sums, int own_lo, int own_hi,

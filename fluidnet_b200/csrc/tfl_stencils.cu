@@ -22,7 +22,7 @@ namespace tfl {
 // ---------------------------------------------------------------------------------------
 // emptyDomain / flagsToOccupancy
 // ---------------------------------------------------------------------------------------
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_empty_domain(float* __restrict__ flags, Geo gin, int bnd) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
@@ -48,8 +48,8 @@ __global__ void k_flags_to_occupancy(const float* __restrict__ flags, float* __r
 // ---------------------------------------------------------------------------------------
 // setWallBcsForward
 // ---------------------------------------------------------------------------------------
-template <bool IS3D, typename FT>
-__global__ void k_set_wall_bcs(float* __restrict__ U, const FT* __restrict__ flags, Geo gin,
+template <bool IS3D>
+__global__ void k_set_wall_bcs(float* __restrict__ U, const float* __restrict__ flags, Geo gin,
                                int as_mask) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
@@ -64,8 +64,8 @@ __global__ void k_set_wall_bcs(float* __restrict__ U, const FT* __restrict__ fla
 // ---------------------------------------------------------------------------------------
 // velocityDivergenceForward  (returns u(i)-u(i+1)+..., i.e. minus the divergence)
 // ---------------------------------------------------------------------------------------
-template <bool IS3D, typename FT>
-__global__ void k_divergence(const float* __restrict__ U, const FT* __restrict__ flags,
+template <bool IS3D>
+__global__ void k_divergence(const float* __restrict__ U, const float* __restrict__ flags,
                              float* __restrict__ div, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
@@ -83,14 +83,14 @@ __global__ void k_divergence(const float* __restrict__ U, const FT* __restrict__
 // ---------------------------------------------------------------------------------------
 // velocityUpdateForward
 // ---------------------------------------------------------------------------------------
-template <bool IS3D, typename FT>
-__global__ void k_velocity_update(float* __restrict__ U, const FT* __restrict__ flags,
+template <bool IS3D>
+__global__ void k_velocity_update(float* __restrict__ U, const float* __restrict__ flags,
                                   const float* __restrict__ p, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   if (on_border(g, k, j, i)) return;
-  const FT* fl = flags + b * g.n;
+  const float* fl = flags + b * g.n;
   const float* pb = p + b * g.n;
   float* ub = U + (long long)b * g.nc * g.n;
   const int c = cell(g, k, j, i);
@@ -121,14 +121,14 @@ __global__ void k_velocity_update(float* __restrict__ U, const FT* __restrict__ 
 // ---------------------------------------------------------------------------------------
 // addBuoyancy / addGravity
 // ---------------------------------------------------------------------------------------
-template <bool IS3D, typename FT>
-__global__ void k_add_buoyancy(float* __restrict__ U, const FT* __restrict__ flags,
+template <bool IS3D>
+__global__ void k_add_buoyancy(float* __restrict__ U, const float* __restrict__ flags,
                                const float* __restrict__ rho, float sx, float sy_, float sz_, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   if (on_border(g, k, j, i)) return;
-  const FT* fl = flags + b * g.n;
+  const float* fl = flags + b * g.n;
   if (!(flag_i(fl, g, k, j, i) & kFluid)) return;
   const float* rb = rho + b * g.n;
   float* ub = U + (long long)b * g.nc * g.n;
@@ -175,7 +175,7 @@ __device__ __forceinline__ V3 centered_or_zero(const float* __restrict__ Ub, con
   return mac_centered(Ub, g, k, j, i);
 }
 
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_vort_curl(const float* __restrict__ U, float* __restrict__ curl,
                             float* __restrict__ cnorm, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
@@ -202,7 +202,7 @@ __global__ void k_vort_curl(const float* __restrict__ U, float* __restrict__ cur
 }
 
 // Confinement force per cell (zero on the border), third_party/tfluids.cc:1411-1439.
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_vort_force(const float* __restrict__ curl, const float* __restrict__ cnorm,
                              float* __restrict__ force, float strength, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
@@ -214,14 +214,14 @@ __global__ void k_vort_force(const float* __restrict__ curl, const float* __rest
 }
 
 // AddForceField, third_party/tfluids.cc:1312-1339 (CPU caller guards the border, :1443-1451).
-template <bool IS3D, typename FT>
-__global__ void k_vort_apply(float* __restrict__ U, const FT* __restrict__ flags,
+template <bool IS3D>
+__global__ void k_vort_apply(float* __restrict__ U, const float* __restrict__ flags,
                              const float* __restrict__ force, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   if (on_border(g, k, j, i)) return;
-  const FT* fl = flags + b * g.n;
+  const float* fl = flags + b * g.n;
   const int fc = flag_i(fl, g, k, j, i);
   const bool cf = fc & kFluid, ce = fc & kEmpty;
   if (!cf && !ce) return;
@@ -522,15 +522,10 @@ __device__ __forceinline__ V3 advect_mac_cell_clear(const FT* __restrict__ fl, c
   return r;
 }
 // Resident CTAs per SM the advectVel kernels are compiled for (register budget 65536 / 256 / N).
-#ifndef TFL_ADVECT_MINB1
-#define TFL_ADVECT_MINB1 4
-#endif
-#ifndef TFL_ADVECT_MINB2
-#define TFL_ADVECT_MINB2 4
-#endif
+constexpr int kAdvectVelMinBlocks = 4;
 
 template <bool IS3D, typename FT, bool OURS>
-__global__ void __launch_bounds__(256, TFL_ADVECT_MINB1) k_advect_vel_pass1(const float* __restrict__ U, const FT* __restrict__ flags,
+__global__ void __launch_bounds__(256, kAdvectVelMinBlocks) k_advect_vel_pass1(const float* __restrict__ U, const FT* __restrict__ flags,
                                    const unsigned char* __restrict__ clear, float* __restrict__ out, float dt, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
@@ -582,7 +577,7 @@ __device__ __forceinline__ float clamp_component_mac_clear(const float* __restri
 // Backward pass on the forward field + MacCormackCorrectMAC + MacCormackClampMAC, fused
 // (third_party/tfluids.cc:859-915, 660-774).
 template <bool IS3D, typename FT, bool OURS>
-__global__ void __launch_bounds__(256, TFL_ADVECT_MINB2) k_advect_vel_pass2(const float* __restrict__ U, const float* __restrict__ fwd,
+__global__ void __launch_bounds__(256, kAdvectVelMinBlocks) k_advect_vel_pass2(const float* __restrict__ U, const float* __restrict__ fwd,
                                    const FT* __restrict__ flags, const unsigned char* __restrict__ clear,
                                    float* __restrict__ dst, float dt, float strength, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
@@ -666,12 +661,12 @@ __global__ void __launch_bounds__(256, TFL_ADVECT_MINB2) k_advect_vel_pass2(cons
 // generic/tfluids.cu:1765-1821 in IEEE arithmetic.
 //   bit0: cell is border-or-obstacle (p = 0); bits1..6: neighbour -x,+x,-y,+y,-z,+z is obstacle.
 // ---------------------------------------------------------------------------------------
-template <bool IS3D, typename FT>
-__global__ void k_jacobi_mask(const FT* __restrict__ flags, unsigned char* __restrict__ mask, Geo gin) {
+template <bool IS3D>
+__global__ void k_jacobi_mask(const float* __restrict__ flags, unsigned char* __restrict__ mask, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
-  const FT* fl = flags + b * g.n;
+  const float* fl = flags + b * g.n;
   unsigned m = 0;
   if (on_border(g, k, j, i) || (flag_i(fl, g, k, j, i) & kObstacle)) {
     m = 1;
@@ -688,7 +683,7 @@ __global__ void k_jacobi_mask(const FT* __restrict__ flags, unsigned char* __res
   mask[b * g.n + cell(g, k, j, i)] = (unsigned char)m;
 }
 
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void k_jacobi_iter(const unsigned char* __restrict__ mask, const float* __restrict__ div,
                               const float* __restrict__ prev, float* __restrict__ cur, Geo gin) {
   const Geo g = static_geo<IS3D>(gin);
@@ -744,7 +739,7 @@ __device__ __forceinline__ void jacobi_update4(unsigned m4, float4 ctr, float le
 
 // Same update, 4 consecutive x cells per thread (float4 rows, one 32-bit load for the 4 mask
 // bytes): 8 memory instructions per 4 cells instead of 40.  Requires nx % 4 == 0.
-template <bool IS3D, typename FT>
+template <bool IS3D>
 __global__ void __launch_bounds__(256)
 k_jacobi_iter4(const unsigned char* __restrict__ mask, const float* __restrict__ div,
                const float* __restrict__ prev, float* __restrict__ cur, Geo gin) {
@@ -981,8 +976,15 @@ __global__ void k_clamp(float* __restrict__ x, float lo, float hi, long long n) 
 // ---------------------------------------------------------------------------------------
 // Launchers
 // ---------------------------------------------------------------------------------------
-// Launch `kernel<IS3D, FT, extra...>` with IS3D picked from the geometry.
-#define TFL_LAUNCH3(kernel, FT, g, st, ...)                      \
+// Launch `kernel<IS3D>`, `kernel<IS3D, FT>` or `kernel<IS3D, FT, X>` with IS3D picked from the geometry.
+#define TFL_LAUNCH3(kernel, g, st, ...)                          \
+  do {                                                           \
+    dim3 grid_, block_;                                          \
+    launch_dims(g, grid_, block_);                               \
+    if ((g).is3d) kernel<true><<<grid_, block_, 0, st>>>(__VA_ARGS__);   \
+    else kernel<false><<<grid_, block_, 0, st>>>(__VA_ARGS__);           \
+  } while (0)
+#define TFL_LAUNCH3T(kernel, FT, g, st, ...)                     \
   do {                                                           \
     dim3 grid_, block_;                                          \
     launch_dims(g, grid_, block_);                               \
@@ -998,32 +1000,28 @@ __global__ void k_clamp(float* __restrict__ x, float lo, float hi, long long n) 
   } while (0)
 
 void launch_empty_domain(float* flags, const Geo& g, int bnd, cudaStream_t st) {
-  TFL_LAUNCH3(k_empty_domain, float, g, st, flags, g, bnd);
+  TFL_LAUNCH3(k_empty_domain, g, st, flags, g, bnd);
 }
 void launch_flags_to_occupancy(const float* flags, float* occ, long long n, unsigned long long* bad,
                                cudaStream_t st) {
   k_flags_to_occupancy<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(flags, occ, n, bad);
 }
-template <typename FT>
-void launch_set_wall_bcs(float* U, const FT* flags, const Geo& g, int as_mask, cudaStream_t st) {
-  TFL_LAUNCH3(k_set_wall_bcs, FT, g, st, U, flags, g, as_mask);
+void launch_set_wall_bcs(float* U, const float* flags, const Geo& g, int as_mask, cudaStream_t st) {
+  TFL_LAUNCH3(k_set_wall_bcs, g, st, U, flags, g, as_mask);
 }
-template <typename FT>
-void launch_divergence(const float* U, const FT* flags, float* div, const Geo& g, cudaStream_t st) {
-  TFL_LAUNCH3(k_divergence, FT, g, st, U, flags, div, g);
+void launch_divergence(const float* U, const float* flags, float* div, const Geo& g, cudaStream_t st) {
+  TFL_LAUNCH3(k_divergence, g, st, U, flags, div, g);
 }
-template <typename FT>
-void launch_velocity_update(float* U, const FT* flags, const float* p, const Geo& g, cudaStream_t st) {
-  TFL_LAUNCH3(k_velocity_update, FT, g, st, U, flags, p, g);
+void launch_velocity_update(float* U, const float* flags, const float* p, const Geo& g, cudaStream_t st) {
+  TFL_LAUNCH3(k_velocity_update, g, st, U, flags, p, g);
 }
-template <typename FT>
-void launch_add_buoyancy(float* U, const FT* flags, const float* rho, const float s[3], const Geo& g,
+void launch_add_buoyancy(float* U, const float* flags, const float* rho, const float s[3], const Geo& g,
                          cudaStream_t st) {
-  TFL_LAUNCH3(k_add_buoyancy, FT, g, st, U, flags, rho, s[0], s[1], s[2], g);
+  TFL_LAUNCH3(k_add_buoyancy, g, st, U, flags, rho, s[0], s[1], s[2], g);
 }
 template <typename FT>
 void launch_add_gravity(float* U, const FT* flags, const float f[3], const Geo& g, cudaStream_t st) {
-  TFL_LAUNCH3(k_add_gravity, FT, g, st, U, flags, f[0], f[1], f[2], g);
+  TFL_LAUNCH3T(k_add_gravity, FT, g, st, U, flags, f[0], f[1], f[2], g);
 }
 // curl + |curl| on [zlo-2, zhi+1), then the force on [zlo-1, zhi) (what AddForceField on
 // [zlo, zhi) reads).  force always has 3 channels.
@@ -1035,16 +1033,15 @@ void launch_vort_curl(const float* U, float* curl, float* cnorm, float* force, f
   Geo g1 = g;
   g1.zlo = g.zlo - 2 < 0 ? 0 : g.zlo - 2;
   g1.zhi = g.zhi + 1 > g.nz ? g.nz : g.zhi + 1;
-  TFL_LAUNCH3(k_vort_curl, float, g1, st, U, curl, cnorm, g1);
+  TFL_LAUNCH3(k_vort_curl, g1, st, U, curl, cnorm, g1);
   Geo g2 = g;
   g2.zlo = g.zlo - 1 < 0 ? 0 : g.zlo - 1;
-  TFL_LAUNCH3(k_vort_force, float, g2, st, curl, cnorm, force, strength, g2);
+  TFL_LAUNCH3(k_vort_force, g2, st, curl, cnorm, force, strength, g2);
 }
-template <typename FT>
-int launch_vorticity(float* U, const FT* flags, float strength, float* curl, float* cnorm, float* force,
+int launch_vorticity(float* U, const float* flags, float strength, float* curl, float* cnorm, float* force,
                      const Geo& g, cudaStream_t st) {
   launch_vort_curl(U, curl, cnorm, force, strength, g, st);
-  TFL_LAUNCH3(k_vort_apply, FT, g, st, U, flags, force, g);
+  TFL_LAUNCH3(k_vort_apply, g, st, U, flags, force, g);
   return 3;
 }
 
@@ -1077,11 +1074,11 @@ int launch_advect_scalar(float dt, const float* s, const float* U, const FT* fla
       return 1;
     case TFL_ADVECT_MACCORMACK:
       TFL_LAUNCH3X(k_advect_scalar_pass1, FT, TFL_ADVECT_MACCORMACK, g_fwd, st, s, U, flags, clear, fwd, nullptr, dt, outside, g_fwd);
-      TFL_LAUNCH3(k_advect_scalar_pass2_manta, FT, gb, st, s, fwd, U, flags, dst, dt, strength, gb);
+      TFL_LAUNCH3T(k_advect_scalar_pass2_manta, FT, gb, st, s, fwd, U, flags, dst, dt, strength, gb);
       return 2;
     case TFL_ADVECT_MACCORMACK_OURS:
       TFL_LAUNCH3X(k_advect_scalar_pass1, FT, TFL_ADVECT_MACCORMACK_OURS, g_fwd, st, s, U, flags, clear, fwd, fwd_pos, dt, outside, g_fwd);
-      TFL_LAUNCH3(k_advect_scalar_pass2_ours, FT, gb, st, s, fwd, fwd_pos, U, flags, clear, dst, dt, strength, outside, gb);
+      TFL_LAUNCH3T(k_advect_scalar_pass2_ours, FT, gb, st, s, fwd, fwd_pos, U, flags, clear, dst, dt, strength, outside, gb);
       return 2;
   }
   return -1;
@@ -1111,9 +1108,8 @@ int launch_advect_vel(float dt, const float* U, const FT* flags, const unsigned 
   return -1;
 }
 
-template <typename FT>
-void launch_jacobi_mask(const FT* flags, unsigned char* mask, const Geo& g, cudaStream_t st) {
-  TFL_LAUNCH3(k_jacobi_mask, FT, g, st, flags, mask, g);
+void launch_jacobi_mask(const float* flags, unsigned char* mask, const Geo& g, cudaStream_t st) {
+  TFL_LAUNCH3(k_jacobi_mask, g, st, flags, mask, g);
 }
 namespace {
 // The 4-cell Jacobi kernels load the 4 mask bytes as one word and div and p as float4.
@@ -1146,11 +1142,11 @@ void launch_jacobi_iter(const unsigned char* mask, const float* div, const float
     block.z = g.nz == 1 ? 1 : 2;
     dim3 grid((qx + block.x - 1) / block.x, (g.ny + block.y - 1) / block.y,
               ((long long)g.nb * nzr + block.z - 1) / block.z);
-    if (g.is3d) k_jacobi_iter4<true, float><<<grid, block, 0, st>>>(mask, div, prev, cur, g);
-    else k_jacobi_iter4<false, float><<<grid, block, 0, st>>>(mask, div, prev, cur, g);
+    if (g.is3d) k_jacobi_iter4<true><<<grid, block, 0, st>>>(mask, div, prev, cur, g);
+    else k_jacobi_iter4<false><<<grid, block, 0, st>>>(mask, div, prev, cur, g);
     return;
   }
-  TFL_LAUNCH3(k_jacobi_iter, float, g, st, mask, div, prev, cur, g);
+  TFL_LAUNCH3(k_jacobi_iter, g, st, mask, div, prev, cur, g);
 }
 namespace {
 // Resident CTAs of k_jacobi_resident<KZ> on the current device (0 when it cannot be launched cooperatively).
@@ -1221,22 +1217,18 @@ void launch_clamp(float* x, float lo, float hi, long long n, cudaStream_t st) {
 }
 
 
-// Explicit instantiations: float flags (operator-level API) and byte flags (fused step).
-#define TFL_INSTANTIATE(FT)                                                                                   \
-  template void launch_set_wall_bcs<FT>(float*, const FT*, const Geo&, int, cudaStream_t);                    \
-  template void launch_divergence<FT>(const float*, const FT*, float*, const Geo&, cudaStream_t);            \
-  template void launch_velocity_update<FT>(float*, const FT*, const float*, const Geo&, cudaStream_t);       \
-  template void launch_add_buoyancy<FT>(float*, const FT*, const float*, const float*, const Geo&, cudaStream_t); \
-  template void launch_add_gravity<FT>(float*, const FT*, const float*, const Geo&, cudaStream_t);           \
-  template int launch_vorticity<FT>(float*, const FT*, float, float*, float*, float*, const Geo&, cudaStream_t); \
-  template int launch_advect_scalar<FT>(float, const float*, const float*, const FT*, const unsigned char*, int, int, \
-                                        float, float*, float*, float*, const Geo&, const Geo&, cudaStream_t);  \
-  template int launch_advect_vel<FT>(float, const float*, const FT*, const unsigned char*, int, float, float*, \
-                                     float*, const Geo&, const Geo&, cudaStream_t);                          \
-  template void launch_jacobi_mask<FT>(const FT*, unsigned char*, const Geo&, cudaStream_t);
-TFL_INSTANTIATE(float)
-TFL_INSTANTIATE(unsigned char)
-#undef TFL_INSTANTIATE
+// Float flags come from the operator-level API, byte flags from the fused step (gravity and advection only).
+template void launch_add_gravity<float>(float*, const float*, const float*, const Geo&, cudaStream_t);
+template void launch_add_gravity<unsigned char>(float*, const unsigned char*, const float*, const Geo&, cudaStream_t);
+template int launch_advect_scalar<float>(float, const float*, const float*, const float*, const unsigned char*, int,
+                                         int, float, float*, float*, float*, const Geo&, const Geo&, cudaStream_t);
+template int launch_advect_scalar<unsigned char>(float, const float*, const float*, const unsigned char*,
+                                                 const unsigned char*, int, int, float, float*, float*, float*,
+                                                 const Geo&, const Geo&, cudaStream_t);
+template int launch_advect_vel<float>(float, const float*, const float*, const unsigned char*, int, float, float*,
+                                      float*, const Geo&, const Geo&, cudaStream_t);
+template int launch_advect_vel<unsigned char>(float, const float*, const unsigned char*, const unsigned char*, int,
+                                              float, float*, float*, const Geo&, const Geo&, cudaStream_t);
 
 // ---------------------------------------------------------------------------------------
 // Clearance field of the advection fast path (tfl_device.cuh): three separable passes over the LOCAL
@@ -1255,14 +1247,13 @@ __device__ __forceinline__ bool clear_cell(const Geo& g, long long t, int& b, in
   i = r - j * g.nx;
   return true;
 }
-template <typename FT>
-__global__ void k_clear_x(const FT* __restrict__ flags, unsigned char* __restrict__ out, Geo g,
+__global__ void k_clear_x(const unsigned char* __restrict__ flags, unsigned char* __restrict__ out, Geo g,
                           const int* __restrict__ gate) {
   if (gate && *gate == 0) return;          // flags unchanged since the cached field was built
   for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x;; t += (long long)gridDim.x * blockDim.x) {
     int b, k, j, i;
     if (!clear_cell(g, t, b, k, j, i)) return;
-    const FT* row = flags + b * g.n + cell(g, k, j, 0);
+    const unsigned char* row = flags + b * g.n + cell(g, k, j, 0);
     // usable = fluid and not on an end of the storage (whole row if j / k sit on one)
     const bool row_ok = j > 0 && j < g.ny - 1 && (!g.is3d || (k > 0 && k < g.nz - 1));
     int r = -1;
@@ -1307,25 +1298,21 @@ __global__ void k_clear_axis(const unsigned char* __restrict__ in, unsigned char
     out[t] = (unsigned char)r;
   }
 }
-template <typename FT>
-int launch_clearance(const FT* flags, unsigned char* clear, unsigned char* tmp, const Geo& g, const int* gate,
+int launch_clearance(const unsigned char* flags, unsigned char* clear, unsigned char* tmp, const Geo& g, const int* gate,
                      cudaStream_t st) {
   const long long total = g.n * g.nb;
   const int block = 256;
   const int grid = (int)std::min<long long>((total + block - 1) / block, 132 * 8);
   if (g.is3d) {                            // (a 3-D grid with fewer than 3 planes gets clearance 0)
-    k_clear_x<FT><<<grid, block, 0, st>>>(flags, clear, g, gate);
+    k_clear_x<<<grid, block, 0, st>>>(flags, clear, g, gate);
     k_clear_axis<1, false><<<grid, block, 0, st>>>(clear, tmp, g, gate);
     k_clear_axis<2, true><<<grid, block, 0, st>>>(tmp, clear, g, gate);
     return 3;
   }
-  k_clear_x<FT><<<grid, block, 0, st>>>(flags, tmp, g, gate);
+  k_clear_x<<<grid, block, 0, st>>>(flags, tmp, g, gate);
   k_clear_axis<1, true><<<grid, block, 0, st>>>(tmp, clear, g, gate);
   return 2;
 }
-template int launch_clearance<float>(const float*, unsigned char*, unsigned char*, const Geo&, const int*, cudaStream_t);
-template int launch_clearance<unsigned char>(const unsigned char*, unsigned char*, unsigned char*, const Geo&, const int*,
-                                             cudaStream_t);
 
 // float flags -> byte flags (once per fused step).  With `changed` the kernel also reports whether any
 // byte differs from what the destination held (the step keeps its byte copy and the clearance field

@@ -44,27 +44,27 @@ def timed(fn):
 
 import ctypes as C
 ctx = tfluids.context()
-ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int, C.c_int]
+ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int]
 ref = None
-for mode, variant in [(0, 0), (1, 0), (1, 1), (1, 2), (1, 3), (1, 4), (2, 0), (2, 1)]:
-    if len(sys.argv) > 4 and (mode, variant) != tuple(int(x) for x in sys.argv[4].split(",")):
+for mode in (0, 1, 2):
+    if len(sys.argv) > 4 and mode != int(sys.argv[4]):
         continue
-    ctx.lib.tfl_debug_advect_tile(ctx.h, mode, variant)
+    ctx.lib.tfl_debug_advect_tile(ctx.h, mode)
     t = timed(lambda: tfluids.advectVel(0.1, U, fl, "maccormackOurs", Ud, 0.6))
     if ref is None:
         ref = Ud.clone()
     same = torch.equal(ref.view(torch.int32), Ud.view(torch.int32))
-    print("advectVel mode %d variant %d: %.1f us  %s" % (mode, variant, t, "== first" if same else "DIFFERS"), flush=True)
-ctx.lib.tfl_debug_advect_tile(ctx.h, -1, 0)
+    print("advectVel mode %d: %.1f us  %s" % (mode, t, "== first" if same else "DIFFERS"), flush=True)
+ctx.lib.tfl_debug_advect_tile(ctx.h, -1)
 ref = None
-for mode, variant in [(0, 0), (1, 0), (1, 1), (2, 0)]:
-    ctx.lib.tfl_debug_advect_tile(ctx.h, mode, variant)
+for mode in (0, 1, 2):
+    ctx.lib.tfl_debug_advect_tile(ctx.h, mode)
     t = timed(lambda: tfluids.advectScalar(0.1, rho, U, fl, "maccormackOurs", rd, False, 0.6))
     if ref is None:
         ref = rd.clone()
     same = torch.equal(ref.view(torch.int32), rd.view(torch.int32))
-    print("advectScalar mode %d variant %d: %.1f us  %s" % (mode, variant, t, "== first" if same else "DIFFERS"), flush=True)
-ctx.lib.tfl_debug_advect_tile(ctx.h, -1, 0)
+    print("advectScalar mode %d: %.1f us  %s" % (mode, t, "== first" if same else "DIFFERS"), flush=True)
+ctx.lib.tfl_debug_advect_tile(ctx.h, -1)
 t_v = timed(lambda: tfluids.advectVel(0.1, U, fl, "maccormackOurs", Ud, 0.6))
 t_s = timed(lambda: tfluids.advectScalar(0.1, rho, U, fl, "maccormackOurs", rd, False, 0.6))
 print("advectVel %.1f us   advectScalar %.1f us   (%d^3, %s velocity, L2 flushed)" % (t_v, t_s, n, velocity), flush=True)

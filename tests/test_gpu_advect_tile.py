@@ -1,6 +1,6 @@
 """advectVel('maccormackOurs') over shared-memory tiles (tfl_advect_tile.cu) against the CPU oracle, bit for
 bit, in every configuration the dispatcher can choose: the two-kernel version (mode 0), the tile kernel with
-a forward halo of 1 and of 2 cells, every tile shape, and velocities whose traces stay inside the halo
+a forward halo of 1 and of 2 cells, and velocities whose traces stay inside the halo
 (amp 2: 0.2 cell), leave halo 1 (amp 8), and leave every halo (amp 25: the backward pass re-evaluates the
 forward values it needs).  Grids: not multiples of the tile, with solids (sphere + slab), with the exotic
 flag mix (empty / outflow / stick cells), and one plane thinner than a tile."""
@@ -21,11 +21,11 @@ def gpu():
     return GpuBackend()
 
 
-def set_tile(mode, variant=0):
+def set_tile(mode):
     from fluidnet_b200 import tfluids
     ctx = tfluids.context()
-    ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    assert ctx.lib.tfl_debug_advect_tile(ctx.h, mode, variant) == 0
+    ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int]
+    assert ctx.lib.tfl_debug_advect_tile(ctx.h, mode) == 0
 
 
 GRIDS = [((40, 24, 20), True, False), ((36, 20, 12), True, True), ((64, 16, 5), False, False)]
@@ -40,14 +40,14 @@ def test_tile_modes_match_oracle(orc, gpu, dims, geom, exotic, amp):
     orc.setWallBcsForward(U, flags)
     want = orc.advectVel(0.1, U, flags, "maccormackOurs", 0.6)
     try:
-        for mode, variant in [(0, 0), (1, 0), (1, 1), (1, 2), (1, 3), (1, 4), (2, 0), (2, 1), (-1, 0)]:
-            set_tile(mode, variant)
+        for mode in (0, 1, 2, -1):
+            set_tile(mode)
             got = gpu.advectVel(0.1, U, flags, "maccormackOurs", 0.6)
-            assert bits_equal(got, want), "mode %d variant %d: %s" % (mode, variant, describe_diff(got, want))
+            assert bits_equal(got, want), "mode %d: %s" % (mode, describe_diff(got, want))
             got = gpu.advectVel(0.1, U, flags, "maccormackOurs", 0.6, in_place=True)
-            assert bits_equal(got, want), "in place, mode %d variant %d: %s" % (mode, variant, describe_diff(got, want))
+            assert bits_equal(got, want), "in place, mode %d: %s" % (mode, describe_diff(got, want))
     finally:
-        set_tile(-1, 0)
+        set_tile(-1)
     assert gpu.trace_faults() == 0
 
 
@@ -64,15 +64,14 @@ def test_scalar_tile_modes_match_oracle(orc, gpu, dims, geom, exotic, amp):
     try:
         for outside in (False, True):
             want = orc.advectScalar(0.1, rho, U, flags, "maccormackOurs", outside, 0.6)
-            for mode, variant in [(0, 0), (1, 0), (1, 1), (2, 0), (-1, 0)]:
-                set_tile(mode, variant)
+            for mode in (0, 1, 2, -1):
+                set_tile(mode)
                 got = gpu.advectScalar(0.1, rho, U, flags, "maccormackOurs", outside, 0.6)
-                assert bits_equal(got, want), "outside %s mode %d variant %d: %s" % (outside, mode, variant,
-                                                                                      describe_diff(got, want))
+                assert bits_equal(got, want), "outside %s mode %d: %s" % (outside, mode, describe_diff(got, want))
             got = gpu.advectScalar(0.1, rho, U, flags, "maccormackOurs", outside, 0.6, in_place=True)
             assert bits_equal(got, want), "in place: " + describe_diff(got, want)
     finally:
-        set_tile(-1, 0)
+        set_tile(-1)
     assert gpu.trace_faults() == 0
 
 
@@ -89,11 +88,11 @@ def test_zero_bounds_keep_their_sign(orc, gpu):
     want = orc.advectVel(0.1, U, flags, "maccormackOurs", 0.6)
     try:
         for mode in (1, 2):
-            set_tile(mode, 0)
+            set_tile(mode)
             got = gpu.advectVel(0.1, U, flags, "maccormackOurs", 0.6)
             assert bits_equal(got, want), "mode %d: %s" % (mode, describe_diff(got, want))
     finally:
-        set_tile(-1, 0)
+        set_tile(-1)
 
 
 def test_halo_choice_follows_the_velocities(gpu):
@@ -108,14 +107,14 @@ def test_halo_choice_follows_the_velocities(gpu):
         for amp in (2.0, 9.0, 30.0, 2.0):
             U = torch.from_numpy(synth.make_velocity(flags, True, amp=amp)).cuda()
             tfluids.setWallBcsForward(U, tf)
-            set_tile(0, 0)
+            set_tile(0)
             ref = torch.empty_like(U)
             tfluids.advectVel(0.1, U, tf, "maccormackOurs", ref, 0.6)
-            set_tile(-1, 0)
+            set_tile(-1)
             for _ in range(3):                   # the choice may change between these calls
                 out = torch.empty_like(U)
                 tfluids.advectVel(0.1, U, tf, "maccormackOurs", out, 0.6)
                 torch.cuda.synchronize()
                 assert torch.equal(out.view(torch.int32), ref.view(torch.int32)), "amp %g" % amp
     finally:
-        set_tile(-1, 0)
+        set_tile(-1)

@@ -206,8 +206,8 @@ def run(what, plane, fn, *arrays):
 
 def set_tile_mode(mode):
     c = ctx()
-    c.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    assert c.lib.tfl_debug_advect_tile(c.h, -1 if mode is None else mode, 0) == 0
+    c.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int]
+    assert c.lib.tfl_debug_advect_tile(c.h, -1 if mode is None else mode) == 0
 
 
 def plane_of(fl):

@@ -77,8 +77,8 @@ def expect(gb, want, step, what):
 
 
 def set_tile_mode(ctx, mode):
-    ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    assert ctx.lib.tfl_debug_advect_tile(ctx.h, mode, 0) == 0
+    ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int]
+    assert ctx.lib.tfl_debug_advect_tile(ctx.h, mode) == 0
 
 
 def tile_used(ctx):

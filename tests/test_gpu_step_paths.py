@@ -276,8 +276,8 @@ def to_gpu(batch, unaligned=False):
 def set_tile_mode(mode):
     from fluidnet_b200 import tfluids
     ctx = tfluids.context()
-    ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int, C.c_int]
-    assert ctx.lib.tfl_debug_advect_tile(ctx.h, -1 if mode is None else mode, 0) == 0
+    ctx.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int]
+    assert ctx.lib.tfl_debug_advect_tile(ctx.h, -1 if mode is None else mode) == 0
 
 
 def host(batch):
