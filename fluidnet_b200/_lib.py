@@ -70,6 +70,7 @@ SYMBOLS = [
     "tfl_slab_sim_jacobi_stats", "tfl_slab_jacobi_schedule", "tfl_jacobi_slab_block", "tfl_slab_cnn_margin",
     "tfl_recorder_create", "tfl_recorder_destroy", "tfl_recorder_capture", "tfl_recorder_take", "tfl_recorder_release",
     "tfl_recorder_create_slab", "tfl_recorder_ipc_export", "tfl_recorder_ipc_connect", "tfl_recorder_capture_slab",
+    "tfl_monitor_create", "tfl_monitor_destroy", "tfl_monitor_record", "tfl_monitor_take", "tfl_slab_sim_monitor_record",
 ]
 JACOBI_BLOCK_INTS = 6
 COMM_ID_BYTES = 128
@@ -206,5 +207,11 @@ def load():
     lib.tfl_recorder_ipc_export.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p]
     lib.tfl_recorder_ipc_connect.argtypes = [C.c_void_p, C.c_void_p, C.c_char_p]
     lib.tfl_recorder_capture_slab.argtypes = [C.c_void_p, C.c_void_p, G, C.c_int32, C.POINTER(C.c_int64)]
+    lib.tfl_monitor_create.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.POINTER(C.c_void_p)]
+    lib.tfl_monitor_destroy.argtypes = [C.c_void_p, C.c_void_p]
+    lib.tfl_monitor_record.argtypes = [C.c_void_p, C.c_void_p, G, G, C.POINTER(C.c_int64)]
+    lib.tfl_monitor_take.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.POINTER(C.c_int64), C.POINTER(C.c_double),
+                                     C.POINTER(C.c_int32), C.POINTER(C.c_int32)]
+    lib.tfl_slab_sim_monitor_record.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.POINTER(C.c_int64)]
     _lib = lib
     return lib

@@ -333,3 +333,6 @@ int cnn_project_from_sums(tfl_ctx* ctx, tfl_cnn* m, const CnnFields& f, const do
 // z-slab; launches nothing.
 int cnn_slab_check(tfl_ctx* ctx, const tfl_cnn* m, int margin, int gnz, int ny, int nx, int zoff, int nz, int own_lo,
                    int own_hi);
+
+// The step monitor's refusals that do not need the grid (tfl_monitor.cu): a full ring, another nb or gnz.
+int monitor_precheck(tfl_ctx* ctx, const tfl_monitor* m, int nb, int gnz);

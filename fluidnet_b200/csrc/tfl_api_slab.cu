@@ -736,6 +736,33 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
   return tfl_clamp(ctx, &st.U, -1e6f, 1e6f);
 }
 
+// The step leaves the ghost planes stale; the divergence on the last owned plane reads U_z one plane above it.  So one
+// plane of U_z is exchanged first -- on the p exchange's inbox area and sequence, which every rank advances alike as
+// long as every rank records -- without counting in the last step's Jacobi statistics.
+int tfl_slab_sim_monitor_record(tfl_ctx* ctx, tfl_slab_sim* s, tfl_monitor* mon, int64_t* index_out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!ctx) return 1;
+  if (index_out) *index_out = -1;
+  if (!s || !mon) return fail(ctx, "slab_sim_monitor_record: nil argument");
+  if (s->world != ctx->comm_world || s->rank != ctx->comm_rank) return fail(ctx, "slab_sim_monitor_record: communicator changed");
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  TFL_CUDA(ctx, cudaStreamIsCapturing(ctx->stream, &cs));
+  if (cs != cudaStreamCaptureStatusNone)        // before the exchange: a refusal enqueues nothing
+    return fail(ctx, "monitor_record: the context's stream is being captured into a graph; record after the graph's launch");
+  if (monitor_precheck(ctx, mon, 1, s->gnz)) return 1;
+  tfl_grid uz = s->st.U;
+  uz.nc = 1;
+  uz.data = s->st.U.data + 2 * s->cells;
+  const int jx = s->jx;
+  const size_t jbytes = s->jbytes;
+  if (slab_exchange(ctx, s, {&uz}, 1, kPhaseP)) return 1;
+  s->jx = jx;
+  s->jbytes = jbytes;
+  SlabScope scope(ctx, s, s->own_lo, s->own_hi);
+  return tfl_monitor_record(ctx, mon, &s->st.U, &s->st.flags, index_out);
+}
+
 // Peer-memory halos: export this rank's inbox (64-byte CUDA IPC handle) ...
 int tfl_slab_sim_ipc_export(tfl_ctx* ctx, tfl_slab_sim* s, char* handle_out) {
   DeviceGuard guard_(ctx);

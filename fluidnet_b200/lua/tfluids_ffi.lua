@@ -126,6 +126,12 @@ int tfl_recorder_create_slab(tfl_ctx*, int32_t gnz, int32_t ny, int32_t nx, int3
 int tfl_recorder_ipc_export(tfl_ctx*, tfl_recorder* rec, char* handle_out);
 int tfl_recorder_ipc_connect(tfl_ctx*, tfl_recorder* rec, const char* handle);
 int tfl_recorder_capture_slab(tfl_ctx*, tfl_recorder* rec, const tfl_grid* field, int32_t z_offset, int64_t* frame_out);
+typedef struct tfl_monitor tfl_monitor;
+int tfl_monitor_create(tfl_ctx*, int32_t nb, int32_t gnz, int32_t capacity, tfl_monitor** out);
+void tfl_monitor_destroy(tfl_ctx*, tfl_monitor* mon);
+int tfl_monitor_record(tfl_ctx*, tfl_monitor* mon, const tfl_grid* U, const tfl_grid* flags, int64_t* index_out);
+int tfl_monitor_take(tfl_ctx*, tfl_monitor* mon, int wait, int64_t* index_out, double* values_out, int32_t* z0_out,
+                     int32_t* planes_out);
 ]]
 
 local lib = ffi.load('tfl')          -- libtfl.so on the library path
@@ -426,6 +432,31 @@ function tfluids.recorderCaptureSlab(rec, field, zOffset)   -- field: the rank's
   check(lib.tfl_recorder_capture_slab(ctx, rec, field.c, zOffset, idx))
   return tonumber(idx[0])
 end
+
+-- ---- divergence statistics after every step (lib/calc_stats.lua:81-123), behind the running step ----
+-- monitorTake -> record index and a table of nb entries {divNorm, divMax, uMax} (nil, nil: not landed yet).
+function tfluids.monitorCreate(nb, gnz, capacity)
+  local m = ffi.new('tfl_monitor*[1]')
+  check(lib.tfl_monitor_create(ctx, nb, gnz, capacity or 64, m))
+  return {c = m[0], nb = nb, buf = ffi.new('double[?]', nb * gnz * 3)}
+end
+function tfluids.monitorRecord(mon, U, flags)        -- enqueued on the context's stream; never waits
+  local idx = ffi.new('int64_t[1]')
+  check(lib.tfl_monitor_record(ctx, mon.c, U.c, flags.c, idx))
+  return tonumber(idx[0])
+end
+function tfluids.monitorTake(mon, wait)
+  local idx, z0, planes = ffi.new('int64_t[1]'), ffi.new('int32_t[1]'), ffi.new('int32_t[1]')
+  check(lib.tfl_monitor_take(ctx, mon.c, (wait == nil or wait) and 1 or 0, idx, mon.buf, z0, planes))
+  if idx[0] < 0 then return nil, nil end
+  assert(planes[0] == 0, 'monitorTake: a z-slab record holds plane partials')
+  local out = {}
+  for b = 0, mon.nb - 1 do
+    out[b + 1] = {divNorm = mon.buf[3 * b], divMax = mon.buf[3 * b + 1], uMax = mon.buf[3 * b + 2]}
+  end
+  return tonumber(idx[0]), out
+end
+function tfluids.monitorDestroy(mon) lib.tfl_monitor_destroy(ctx, mon.c) end
 
 function tfluids.synchronize() check(lib.tfl_sync(ctx)) end
 

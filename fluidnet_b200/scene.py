@@ -16,6 +16,11 @@ Files, as the demo writes them (into --out-dir, by default the demo's render fol
   * geom_output.vbox: the occupancy after frame 1 (tfluids.flagsToOccupancy), one frame;
   * geom_output_blender.vbox: the same with the six border planes zeroed, so the renderer can see inside.
 
+With --stats FILE every frame is followed by the library's step monitor (monitor.StepMonitor; DESIGN.md section 6b),
+which reduces U and the flags on the device behind the running step, and FILE gets one CSV row per frame: the frame,
+div_norm (the reference's `div:norm()`, lib/calc_stats.lua:99-115), div_max (max |div|) and u_max_dt (max |U| dt, the
+longest trace in cells).  The log gives the run's largest u_max_dt, next to --margin on z-slabs.
+
 With --slabs the domain is split into z-slabs, one rank per process (the library's slab step, tfl_slab_sim_step), and
 every rank packs its planes of each recorded frame into rank 0's staging frame over peer memory
 (record.SlabFrameRecorder); rank 0 writes the same files.  Under torchrun with more than one process --slabs is implied:
@@ -29,7 +34,7 @@ import time
 
 import numpy as np
 
-from . import formats
+from . import formats, monitor
 from .tfluids import CellType
 
 SCENES = {"plume": "mushroom_cloud_render", "arch": "arch_render", "bunny": "bunny_render"}   # the demo's outDir
@@ -167,12 +172,42 @@ def write_geometry(paths, res, flags):
         w.write(blender_geometry(occ))
 
 
+STATS_COLUMNS = ("frame", "div_norm", "div_max", "u_max_dt")
+STATS_CAPACITY = 64       # records in the monitor's ring: the oldest is taken when it is full, long after it landed
+
+
+def write_stats(path, rows):
+    """rows: (frame, div_norm, div_max, u_max_dt) -> a CSV file with a header; floats as the shortest repr that reads
+    back to the same double."""
+    os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
+    with open(path, "w") as f:
+        f.write(",".join(STATS_COLUMNS) + "\n")
+        for frame, dn, dm, ud in rows:
+            f.write("%d,%r,%r,%r\n" % (int(frame), float(dn), float(dm), float(ud)))
+
+
+def read_stats(path):
+    """The rows of a --stats file as (frame, div_norm, div_max, u_max_dt) tuples."""
+    with open(path) as f:
+        head = f.readline().strip().split(",")
+        if tuple(head) != STATS_COLUMNS:
+            raise ValueError("%s is not a --stats file (header %r)" % (path, head))
+        return [(int(r[0]), float(r[1]), float(r[2]), float(r[3])) for r in (ln.strip().split(",") for ln in f) if r[0]]
+
+
+def stats_rows(records, dt):
+    """Monitor records [(index, [1][3] values), ...] of frames 1, 2, ... -> CSV rows (u_max scaled by dt)."""
+    return [(idx + 1, v[0][0], v[0][1], v[0][2] * dt) for idx, v in records]
+
+
 def run(res=128, scene="plume", sim_method="convnet", model=None, model_mconf=None, model_name="model",
         out_dir=None, binvox=None, num_frames=NUM_FRAMES, output_decimation=OUTPUT_DECIMATION, slots=3,
-        density_file=None, log=print, slabs=False, margin=None, world=None, rank=None):
+        density_file=None, log=print, slabs=False, margin=None, world=None, rank=None, stats=None):
     """Simulate the scene and write its files; returns {'density', 'geom', 'geom_blender': paths,
-    'ms_per_frame': host time per frame excluding frame 1 (None for a single frame), 'frames_written': n}.
-    slabs: run on z-slabs (run_slabs), one rank per process; implied when the launcher's WORLD_SIZE > 1."""
+    'ms_per_frame': host time per frame excluding frame 1 (None for a single frame), 'frames_written': n,
+    'max_u_dt': the run's largest max |U| dt (None without stats)}.
+    slabs: run on z-slabs (run_slabs), one rank per process; implied when the launcher's WORLD_SIZE > 1.
+    stats: a path for the per-frame divergence statistics (CSV), taken by the step monitor after every frame."""
     if not RES_RANGE[0] <= res <= RES_RANGE[1]:
         raise ValueError("res must lie in [%d, %d] (the demo's range), got %d" % (RES_RANGE + (res,)))
     if sim_method == "convnet" and model is None:
@@ -193,9 +228,9 @@ def run(res=128, scene="plume", sim_method="convnet", model=None, model_mconf=No
             % (res, scene, sim_method, num_frames, output_decimation))
     if slabs or world > 1:
         return run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation, slots, margin, rank, world,
-                         log)
+                         log, stats)
     import torch
-    from . import record, simulate, tfluids
+    from . import monitor, record, simulate, tfluids
 
     stream = torch.cuda.Stream()          # a step graph cannot be captured on the legacy default stream
     with torch.cuda.stream(stream):
@@ -204,6 +239,8 @@ def run(res=128, scene="plume", sim_method="convnet", model=None, model_mconf=No
         batch = {"pDiv": zeros(1), "UDiv": zeros(3), "flags": torch.from_numpy(flags_np).cuda(), "density": zeros(1)}
         simulate.createPlumeBCs(batch, DENSITY_VAL, 1.0 * (res / 128), PLUME_RAD)
         rec = record.FrameRecorder((res, res, res), slots)
+        mon = monitor.StepMonitor(None, batch, STATS_CAPACITY) if stats else None
+        records = []
         graph = None
         t0 = None
         written = 0
@@ -217,6 +254,11 @@ def run(res=128, scene="plume", sim_method="convnet", model=None, model_mconf=No
                         graph.launch()
                     else:
                         simulate.simulate_fused(None, mconf, batch, model)
+                    if mon is not None:
+                        if mon.full:
+                            records.append(mon.take())
+                        mon.record(batch)
+                        records += mon.drain()
                     if i == 1:
                         write_geometry(paths, res, batch["flags"])
                         graph = simulate.StepGraph(mconf, batch, model)
@@ -229,18 +271,38 @@ def run(res=128, scene="plume", sim_method="convnet", model=None, model_mconf=No
             t1 = time.perf_counter()
             if graph is not None and sim_method == "pcg":
                 graph.pcg_status()        # raises what the reference's solve would have (a NaN residual, ...)
+            if mon is not None:
+                records += mon.drain(wait=True)
         finally:
             rec.close()
+            if mon is not None:
+                mon.close()
             if graph is not None:
                 graph.close()
     ms = None if t0 is None else 1000.0 * (t1 - t0) / (num_frames - 1)
+    max_u_dt = _write_run_stats(stats, records, mconf["dt"], None, log)
     log("All done!")
     if ms is not None:
         log("Processing time: %.4f ms per frame" % ms)
-    return dict(paths, ms_per_frame=ms, frames_written=int(written))
+    return dict(paths, ms_per_frame=ms, frames_written=int(written), max_u_dt=max_u_dt)
 
 
-def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation, slots, margin, rank, world, log):
+def _write_run_stats(stats, records, dt, margin, log):
+    """Writes the --stats file and logs the run's largest max |U| dt; returns it (None without stats)."""
+    if not stats:
+        return None
+    rows = stats_rows(records, dt)
+    write_stats(stats, rows)
+    top = 0.0
+    for r in rows:                        # a NaN row (a run that blew up) makes the peak NaN
+        top = monitor._nanmax(top, r[3])
+    at = "" if margin is None else " (--margin %d: traces up to %d cells)" % (margin, margin - 1)
+    log("divergence statistics of %d frames in %s; largest max|U| dt: %.4f cells%s" % (len(rows), stats, top, at))
+    return top
+
+
+def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation, slots, margin, rank, world, log,
+              stats=None):
     """run() on z-slabs: rank `rank` of `world` steps its slab with the library's slab step (NativeSlabSimulator) and
     captures every `output_decimation`-th density frame into a SlabFrameRecorder; rank 0 writes the files.  Every rank
     holds the global flags and BCs.  Without peer memory the frames are gathered synchronously (and the log says so).
@@ -260,10 +322,12 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
     batch = {"pDiv": zeros(1), "UDiv": zeros(3), "flags": torch.from_numpy(flags_np), "density": zeros(1)}
     simulate.createPlumeBCs(batch, DENSITY_VAL, 1.0 * (res / 128), PLUME_RAD)     # on the host, as the whole-grid scene
     stream = torch.cuda.Stream(device)
-    written, t0, rec, dens = 0, None, None, None
+    written, t0, rec, dens, mon, max_u_dt = 0, None, None, None, None, None
     with torch.cuda.stream(stream):
         sim = NativeSlabSimulator(batch, mconf, None, device, rank, world, margin, model=model)
         try:
+            if stats:
+                mon = sim.monitor(STATS_CAPACITY)
             try:
                 rec = sim.frame_recorder(slots)
                 transport = "peer memory" if world > 1 else "one rank"
@@ -278,6 +342,8 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
                     stream.synchronize()      # frame 1 is not timed
                     t0 = time.perf_counter()
                 sim.step()
+                if mon is not None:
+                    mon.record_frame()        # no collective: a rank keeps its own records until the run ends
                 if i == 1 and rank == 0:
                     write_geometry(paths, res, batch["flags"].to(device))
                 if i % output_decimation == 0:
@@ -294,7 +360,9 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
                 rec.drain(dens, wait=True)
             stream.synchronize()
             t1 = time.perf_counter()
-            try:
+            if mon is not None:           # one gather of every rank's records, then the file and the log line --
+                max_u_dt = _write_run_stats(stats if rank == 0 else None, mon.collect(), mconf["dt"], margin, log)
+            try:                          # -- also for a run that outgrew its margin and raises below
                 sim.check()
             except RuntimeError as e:
                 raise RuntimeError("%s (the scene's --margin, now %d)" % (e, margin)) from None
@@ -303,13 +371,15 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
                 dens.close()
             if rec is not None:
                 rec.close()
+            if mon is not None:
+                mon.close()
             sim.close()
     ms = None if t0 is None else 1000.0 * (t1 - t0) / (num_frames - 1)
     if rank == 0:
         log("All done!")
         if ms is not None:
             log("Processing time: %.4f ms per frame" % ms)
-    return dict(paths, ms_per_frame=ms, frames_written=int(written))
+    return dict(paths, ms_per_frame=ms, frames_written=int(written), max_u_dt=max_u_dt)
 
 
 def main(argv=None):
@@ -330,6 +400,8 @@ def main(argv=None):
     ap.add_argument("--margin", type=int, default=None,
                     help="z-slab margin: planes a backward trace may reach (default %d, from the measured plume)"
                          % SLAB_MARGIN)
+    ap.add_argument("--stats", metavar="FILE",
+                    help="write the divergence statistics of every frame (frame, div_norm, div_max, u_max_dt) as CSV")
     args = ap.parse_args(argv)
     rank, world, local = launcher_world()
     if args.slabs or world > 1:
@@ -349,7 +421,7 @@ def main(argv=None):
         name = "synthetic"
     run(args.res, args.scene, args.sim_method, model, model_mconf, name, args.out_dir, args.binvox, args.frames,
         args.decimation, args.slots, args.density_filename, print if rank == 0 else (lambda *a: None), args.slabs,
-        args.margin)
+        args.margin, stats=args.stats)
 
 
 if __name__ == "__main__":

@@ -496,6 +496,12 @@ class NativeSlabSimulator:
             barrier = barrier or self._barrier
         return SlabFrameRecorder(self._shape[2:], self.rank, self.world, slots, self.device, self.group, share, barrier)
 
+    def monitor(self, capacity=64):
+        """A monitor.SlabStepMonitor of this decomposition: each rank reduces its owned planes after a step, and the
+        ranks' plane partials combine into the whole grid's divergence statistics (every rank records alike)."""
+        from .monitor import SlabStepMonitor
+        return SlabStepMonitor(self, capacity)
+
     def field(self, key):
         """The tfl_grid of this rank's local slab of `key` ('density' or 'pDiv'; owned and ghost planes, local plane 0
         at global plane self.zoff)."""

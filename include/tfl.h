@@ -541,6 +541,41 @@ int tfl_recorder_ipc_export(tfl_ctx* ctx, tfl_recorder* rec, char* handle_out /*
 int tfl_recorder_ipc_connect(tfl_ctx* ctx, tfl_recorder* rec, const char* handle);
 int tfl_recorder_capture_slab(tfl_ctx* ctx, tfl_recorder* rec, const tfl_grid* field, int32_t z_offset,
                               int64_t* frame_out);
+
+/* ---- step monitor: the divergence statistics of torch/lib/calc_stats.lua:81-123 behind the running step ------------
+ * One record per call, per batch entry: div_norm = sqrt(sum d^2) over all cells, div_max = max |d|, u_max = max |U| over
+ * every face and component, where d is what tfl_velocity_divergence_forward writes (u(i) - u(i+1) + ..., 0 outside
+ * interior fluid cells).  Summed in fp64 in an order fixed by the field alone: one partial per (batch entry, global
+ * plane) from a fixed split of the plane into rows, then the planes in ascending global z, then the square root
+ * (DESIGN.md section 6b).  The same fields give the same bits on every run, whole grid or z-slabs.  The maxima
+ * propagate NaN: a NaN anywhere in U makes u_max NaN, one in d makes div_max (and div_norm) NaN.
+ * tfl_monitor_create: `capacity` >= 1 record slots in pinned, mapped host memory for grids of nb batch entries and gnz
+ *   global planes; on failure *out stays NULL.
+ * tfl_monitor_record: enqueues two kernels on the context's current stream, which read U and flags as the stream leaves
+ *   them; the second stores the record straight into its host slot and then, with release semantics, its sequence
+ *   number.  Never synchronises.  *index_out (may be NULL) = the record's index (0, 1, ... per monitor).  The first
+ *   record fixes the monitor's nc, ny and nx.  On a context with a slab placement (tfl_set_slab) it reduces the
+ *   placement's planes [z_lo, z_hi) only, and the record keeps their per-plane partials (sum d^2, max |d|, max |U|)
+ *   with the global index of the first; d on the placement's last plane reads U_z on the plane above it, which the
+ *   caller keeps current (tfl_slab_sim_monitor_record does).  Refused with nothing enqueued: a stream being captured
+ *   into a graph (record after tfl_step_graph_launch instead), a ring whose slots all hold records not yet taken, and a
+ *   grid whose nb, gnz or shape differs from the monitor's (the message names it).
+ * tfl_monitor_take: the oldest record not yet taken, first in, first out.  values_out receives nb x 3 doubles {div_norm,
+ *   div_max, u_max} and *planes_out = 0 for a whole-grid record, or nb x planes x 3 doubles {sum d^2, max |d|, max |U|}
+ *   for global planes [*z0_out, *z0_out + *planes_out) of a z-slab record (size it nb x gnz x 3).  wait = 0 returns at
+ *   once with *index_out = -1 if the record has not landed; wait = 1 polls its sequence word.  Fails at once when no
+ *   record is left.
+ * tfl_monitor_destroy: waits for the records in flight, then frees everything.
+ * tfl_slab_sim_monitor_record: collective over the ranks of a slab simulator, like a step: refreshes the ghost plane
+ *   of U_z above each rank's owned planes from its neighbour (the step leaves it stale), then tfl_monitor_record of the
+ *   owned planes.  Adding every rank's plane partials in ascending global z gives the whole grid's record bit for bit. */
+typedef struct tfl_monitor tfl_monitor;
+int tfl_monitor_create(tfl_ctx* ctx, int32_t nb, int32_t gnz, int32_t capacity, tfl_monitor** out);
+void tfl_monitor_destroy(tfl_ctx* ctx, tfl_monitor* mon);
+int tfl_monitor_record(tfl_ctx* ctx, tfl_monitor* mon, const tfl_grid* U, const tfl_grid* flags, int64_t* index_out);
+int tfl_monitor_take(tfl_ctx* ctx, tfl_monitor* mon, int wait, int64_t* index_out, double* values_out, int32_t* z0_out,
+                     int32_t* planes_out);
+int tfl_slab_sim_monitor_record(tfl_ctx* ctx, tfl_slab_sim* sim, tfl_monitor* mon, int64_t* index_out);
 #ifdef __cplusplus
 }
 #endif
