@@ -209,7 +209,7 @@ int tfl_create(tfl_ctx** out, int device) {
   c->device = device;
   if (!(c->own_stream = new_stream(cudaStreamDefault))) return 1;
   c->stream = c->own_stream.get();
-  if (!(c->counters = dev_zeros<unsigned long long>(16)) || !(c->dscratch = dev_alloc<double>(256))) return 1;
+  if (!(c->counters = dev_zeros<unsigned long long>(16))) return 1;
   for (StreamPtr* q : {&c->side_stream, &c->copy_in, &c->copy_out})
     if (!(*q = new_stream(cudaStreamNonBlocking))) return 1;
   for (EventPtr* e : {&c->ev_fork, &c->ev_join, &c->ev_u_in, &c->ev_d_in, &c->ev_p_in, &c->ev_d_ready, &c->ev_d_out})
@@ -525,10 +525,11 @@ int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_gr
   Geo g;
   if (make_geo(ctx, flags, is_3d, &g)) return 1;
   const size_t cells = (size_t)g.n * g.nb;
-  if (arena_reserve(ctx, carve_bytes({cells * 4, cells}))) return 1;
+  if (arena_reserve(ctx, carve_bytes({cells * 4, cells, sizeof(double) * g.nb}))) return 1;
   Carver cv(ctx);
   float* p_prev = cv.take<float>(cells);
   unsigned char* mask = cv.take<unsigned char>(cells);
+  double* sq = cv.take<double>(g.nb);          // per-entry sum of squared changes (the residual)
   cudaStream_t st = ctx->stream;
   launch_jacobi_mask(flags->data, mask, g, st);
   ctx->launches += 1;
@@ -557,10 +558,10 @@ int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_gr
     ctx->launches += 1;
     const bool last = (iter + 1 >= max_iter);
     if (need_every || (last && residual)) {
-      TFL_CUDA(ctx, cudaMemsetAsync(ctx->dscratch.get(), 0, sizeof(double) * g.nb, st));
-      launch_sqdiff(p->data, p_prev, g.n, g.nb, ctx->dscratch.get(), st);
+      TFL_CUDA(ctx, cudaMemsetAsync(sq, 0, sizeof(double) * g.nb, st));
+      launch_sqdiff(p->data, p_prev, g.n, g.nb, sq, st);
       ctx->launches += 1;
-      TFL_CUDA(ctx, cudaMemcpyAsync(h.data(), ctx->dscratch.get(), sizeof(double) * g.nb, cudaMemcpyDeviceToHost, st));
+      TFL_CUDA(ctx, cudaMemcpyAsync(h.data(), sq, sizeof(double) * g.nb, cudaMemcpyDeviceToHost, st));
       TFL_CUDA(ctx, cudaStreamSynchronize(st));
       double worst = 0.0;
       for (int b = 0; b < g.nb; b++) { const double nr = sqrt(h[b]); if (nr > worst) worst = nr; }
@@ -857,7 +858,8 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
   const bool has_density = s->density.data != nullptr;
   if (cnn_ensure_act(ctx, m, g)) return 1;
   if (arena_reserve(ctx, carve_bytes({cells * 4, cells * 4 * g.nc, cells * 4, cells * 4 * g.nc, cells * 4 * g.nc,
-                                      cells * 12, cells * 4, cells * 4, 4 * (size_t)g.nb, cells * 12, cells / 4 + 64})))
+                                      cells * 12, cells * 4, cells * 4, 4 * (size_t)g.nb, cells * 12, cells / 4 + 64,
+                                      16 * (size_t)g.nb})))
     return 1;
   Carver cv(ctx);
   float* fwd_s = cv.take<float>(cells);
@@ -871,6 +873,7 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
   float* scale = cv.take<float>(g.nb);
   float* force = cv.take<float>(cells * 3);
   unsigned char* qmask_buf = cv.take<unsigned char>(cells / 4 + 64);
+  double* sums = cv.take<double>(2 * (size_t)g.nb);      // (sum, sum of squares) of the masked U per entry
   cudaStream_t st = ctx->stream;
   // Byte copy of the flags for this step (every bit the kernels test is below 256) and, when a byte
   // differs from the previous step's copy, the clearance field of the advection fast path.
@@ -947,7 +950,6 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
     launch_vort_curl(s->U.data, curl, cnorm, force, fo.vort_amp, g, st);
     ctx->launches += 2;
   }
-  double* sums = ctx->dscratch.get() + 64;
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
   launch_vort_bc_mask(s->U.data, fl8, force, fo.vorticity, u_bc ? s->U_bc_inv_mask.data : nullptr,
                       u_bc ? s->U_bc.data : nullptr, qmask, 1, sums, g, st);
@@ -966,8 +968,7 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
 // Its point-wise stages are 3-D kernels: the tensor-core stack (tc_ok) serves 3-D models only.
 static bool fused_step_applies(const tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, const tfl_cnn* cnn) {
   return mc->sim_method == TFL_SIM_CONVNET && cnn && cnn->tc_ok && cnn->mode > 0 && cnn->default_inputs && !ctx->slab &&
-         s->U.nc == 3 && s->flags.nb == 1 &&
-         !s->p_bc.data && mc->advection_method >= 0 && mc->advection_method <= 5;
+         s->U.nc == 3 && !s->p_bc.data && mc->advection_method >= 0 && mc->advection_method <= 5;
 }
 
 int tfl_simulate_step(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, tfl_cnn* cnn) {
@@ -982,6 +983,11 @@ int tfl_simulate_step(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, tfl
   const bool has_density = s->density.data != nullptr;
   if (fused_step_applies(ctx, s, mc, cnn)) {
     if (has_density && (check_scalar(ctx, &s->density, "density") || !same_spatial(&s->density, &s->flags)))
+      return fail(ctx, "Size mismatch");
+    // the fused stages index p and the BC arrays per batch entry, as setConstVals' applyBC refuses other shapes
+    auto fits = [&](const tfl_grid& x, int nc) { return !x.data || (same_spatial(&x, &s->flags) && x.nc == nc); };
+    if (!fits(s->p, 1) || !fits(s->U_bc, 3) || !fits(s->U_bc_inv_mask, 3) || !fits(s->density_bc, 1) ||
+        !fits(s->density_bc_inv_mask, 1))
       return fail(ctx, "Size mismatch");
     return simulate_step_fused(ctx, s, mc, cnn, g);
   }

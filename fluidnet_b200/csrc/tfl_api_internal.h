@@ -32,7 +32,6 @@ struct tfl_ctx {
   // again, so that tfl_step_graph_launch can refuse a graph that would replay freed memory.
   unsigned long long arena_gen = 0;
   DevPtr<unsigned long long> counters;      // [0] trace faults, [1] bad occupancy cells
-  DevPtr<double> dscratch;                  // small double scratch (reductions), 256 entries
   long long launches = 0;
   bool slab = false;
   int zoff = 0, gnz = 0, zlo = 0, zhi = 0;

@@ -223,6 +223,7 @@ int cnn_forward_tc(tfl_ctx* ctx, tfl_cnn* m, const CnnFields& f, const Geo& g, c
 // meaningful: what arena_reserve needs, 256 bytes beyond each piece (at least its alignment) and 768 more.
 struct CnnScratch {
   float *U1, *x0, *actA, *actB, *scale;
+  double* sums;        // the input scale's (sum, sum of squares) per batch entry
   double* bn_part;     // batch statistics: the partial sums and (a, c) of one BN module at a time
   float* bn_ac;
   float* actC;         // the third rotating buffer of the graphs that are not plain
@@ -245,6 +246,7 @@ CnnScratch cnn_scratch(const tfl_cnn* m, const Geo& g, char* base) {
   s.actA = (float*)take(cells * 4 * m->max_c);      // max_c covers max_rel (set at creation)
   s.actB = (float*)take(cells * 4 * m->max_c);
   s.scale = (float*)take(sizeof(float) * g.nb);
+  s.sums = (double*)take(sizeof(double) * 2 * g.nb);
   s.bn_part = (double*)take(sizeof(double) * 2 * (kBnBlocks + 1) * m->bn_max_c);
   s.bn_ac = (float*)take(sizeof(float) * 2 * m->bn_max_c);
   if (m->plain) return s;
@@ -509,7 +511,7 @@ int cnn_project_fp32(tfl_ctx* ctx, const tfl_cnn* m, const CnnFields& f, const G
 int cnn_project(tfl_ctx* ctx, tfl_cnn* m, const CnnFields& f, float threshold, const Geo& g, float* scale_out) {
   if (arena_reserve(ctx, cnn_scratch(m, g, nullptr).bytes)) return 1;
   const CnnScratch scr = cnn_scratch(m, g, ctx->arena.get());
-  double* sums = ctx->dscratch.get() + 64;
+  double* sums = scr.sums;
   cudaStream_t st = ctx->stream;
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
   launch_cnn_mask_stats(f.U, f.flags, scr.U1, sums, g.zlo, g.zhi, g, st, m->norm_chan, f.p_div);

@@ -551,4 +551,19 @@ __device__ __forceinline__ void block_accumulate(double s, double ss, double* __
   }
 }
 
+// Adds (s, ss) to sums[2 b]: one block never straddles two batch entries unless nb > 1 and the z range is odd; in
+// that (rare) case fall back to per-thread atomics.  All threads of the block must call.
+__device__ __forceinline__ void add_entry_sums(double s, double ss, double* __restrict__ sums, bool live, int b,
+                                               const Geo& g) {
+  const int nzr = g.zhi - g.zlo;
+  const bool block_uniform = (g.nb == 1) || (nzr % (int)blockDim.z == 0);
+  if (block_uniform) {
+    const int zz0 = blockIdx.z * blockDim.z;
+    block_accumulate(s, ss, sums + 2 * (zz0 / nzr < g.nb ? zz0 / nzr : 0));
+  } else if (live) {
+    atomicAdd(sums + 2 * b, s);
+    atomicAdd(sums + 2 * b + 1, ss);
+  }
+}
+
 }  // namespace tfl

@@ -83,7 +83,9 @@ __global__ void k_post_advect(const float* __restrict__ tmp_s, const float* __re
 }
 
 // U += confinement force; U = BC(U); then (mask_mode 1) U *= wall mask and accumulate the
-// sums for the input scale.
+// sums for the input scale.  BATCH (nb > 1): the sums go to each thread's own entry (add_entry_sums); nb = 1 compiles
+// without that branch.
+template <bool BATCH>
 __global__ void k_vort_bc_mask(float* __restrict__ U, const unsigned char* __restrict__ flags,
                                const float* __restrict__ force, int do_vort, BcPtrs bc, int mask_mode,
                                double* __restrict__ sums, Geo gin) {
@@ -127,8 +129,8 @@ __global__ void k_vort_bc_mask(float* __restrict__ U, const unsigned char* __res
     for (int a = 0; a < g.nc; a++) U[ub + a * g.n + c] = u[a];
   }
   if (mask_mode) {
-    // nb == 1 in the fused step (one grid per context); a block never straddles batches then.
-    block_accumulate(s, ss, sums + 2 * (live ? b : 0));
+    if (BATCH) add_entry_sums(s, ss, sums, live, b, g);         // a block may straddle two entries
+    else block_accumulate(s, ss, sums + 2 * (live ? b : 0));
   }
 }
 
@@ -376,6 +378,7 @@ __global__ void __launch_bounds__(256) k_post_advect4(const float* __restrict__ 
   for (int a = 0; a < 3; a++) if (a < g.nc) st4(U + ub + a * g.n + c0, u[a]);
 }
 
+template <bool BATCH>
 __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, const unsigned char* __restrict__ flags,
                                                        const float* __restrict__ force, int do_vort, BcPtrs bc,
                                                        int mask_mode, double* __restrict__ sums, Geo gin) {
@@ -452,7 +455,10 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
 #pragma unroll
     for (int a = 0; a < 3; a++) if (a < g.nc) st4(U + ub + a * g.n + c0, u[a]);
   }
-  if (mask_mode) block_accumulate(s, ss, sums + 2 * (live ? b : 0));
+  if (mask_mode) {
+    if (BATCH) add_entry_sums(s, ss, sums, live, b, g);         // thread_cell4's z range is [0, nz), as thread_cell's
+    else block_accumulate(s, ss, sums + 2 * (live ? b : 0));
+  }
 }
 
 __global__ void __launch_bounds__(256) k_cnn_inputs_fused4(const float* __restrict__ p_div, const float* __restrict__ U1,
@@ -792,11 +798,13 @@ void launch_vort_bc_mask(float* U, const unsigned char* flags, const float* forc
   BcPtrs bc{u_inv, u_bc, nullptr, nullptr, qmask};
   dim3 grid, block;
   if (quad_dims(g, grid, block) && aligned16({U, flags, force, u_inv, u_bc})) {
-    k_vort_bc_mask4<<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
+    if (g.nb > 1) k_vort_bc_mask4<true><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
+    else k_vort_bc_mask4<false><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
     return;
   }
   launch_dims(g, grid, block);
-  k_vort_bc_mask<<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
+  if (g.nb > 1) k_vort_bc_mask<true><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
+  else k_vort_bc_mask<false><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
 }
 void launch_cnn_inputs_fused(const float* p_div, const float* U1, const unsigned char* flags, const double* sums,
                              float threshold, float* scale_out, float* x0, int px, int py, const Geo& g,

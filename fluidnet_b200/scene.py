@@ -176,14 +176,18 @@ STATS_COLUMNS = ("frame", "div_norm", "div_max", "u_max_dt")
 STATS_CAPACITY = 64       # records in the monitor's ring: the oldest is taken when it is full, long after it landed
 
 
+def csv_float(x):
+    """A float in a statistics CSV: the shortest repr that reads back to the same double."""
+    return repr(float(x))
+
+
 def write_stats(path, rows):
-    """rows: (frame, div_norm, div_max, u_max_dt) -> a CSV file with a header; floats as the shortest repr that reads
-    back to the same double."""
+    """rows: (frame, div_norm, div_max, u_max_dt) -> a CSV file with a header; floats as csv_float writes them."""
     os.makedirs(os.path.dirname(path) or ".", exist_ok=True)
     with open(path, "w") as f:
         f.write(",".join(STATS_COLUMNS) + "\n")
         for frame, dn, dm, ud in rows:
-            f.write("%d,%r,%r,%r\n" % (int(frame), float(dn), float(dm), float(ud)))
+            f.write("%d,%s,%s,%s\n" % (int(frame), csv_float(dn), csv_float(dm), csv_float(ud)))
 
 
 def read_stats(path):
