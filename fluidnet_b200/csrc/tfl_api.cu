@@ -789,6 +789,11 @@ int tfl_debug_make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is_3d) {
   Geo g;
   return make_geo(ctx, flags, is_3d, &g);
 }
+// Debug hook: whether check_launch_grid accepts an nb x nz x ny grid (1) or refuses it (0).  Host arithmetic only: it
+// needs no context and no device.
+int tfl_debug_launch_grid_ok(int32_t nb, int32_t nz, int32_t ny) {
+  return !check_launch_grid(nullptr, "", nb, nz, ny);
+}
 
 // Undocumented debugging hook.
 // mode: -1 automatic, 0 two-kernel advectVel, 1 / 2 tile kernel with that halo.
@@ -1051,6 +1056,7 @@ int tfl_host_sim_create(tfl_ctx* ctx, int32_t nb, int32_t nz, int32_t ny, int32_
   if (nb < 1 || nz < 1 || ny < 1 || nx < 1) return fail(ctx, "host_sim: every grid extent must be >= 1");
   if (!is_3d && nz != 1) return fail(ctx, "host_sim: 2D grid must have zsize == 1");
   if (grid_too_large((long long)nz * ny * nx, nb)) return fail(ctx, "host_sim: grid too large");
+  if (check_launch_grid(ctx, "host_sim", nb, nz, ny)) return 1;
   std::unique_ptr<tfl_host_sim> hs(new tfl_host_sim());
   memset(&hs->st, 0, sizeof(hs->st));
   hs->nc = is_3d ? 3 : 2;

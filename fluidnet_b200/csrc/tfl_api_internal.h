@@ -238,6 +238,30 @@ inline int check_vel(tfl_ctx* ctx, const tfl_grid* U, const tfl_grid* flags) {
 // velocity field within 2^33 cells.
 inline bool grid_too_large(long long n, int nb) { return n >= (1LL << 31) || n * (long long)nb * 3 >= (1LL << 31) * 4; }
 
+// CUDA launches at most 65535 blocks along gridDim.y and along gridDim.z, and the launchers put the batch's planes and
+// the rows there:
+//  * planes (z): launch_dims, quad_dims, conv_launch and k_jacobi_iter4 give a block two planes of a grid with nz > 1
+//    and one plane otherwise, over all nb entries: nb nz <= 2 x 65535 (nz > 1), nb <= 65535 (nz = 1).  The launchers
+//    that give a block more planes (the advection tiles 8, the box convolution 5 or 6, k_jacobi_march at least 4)
+//    stay below that, and so does nb <= 65535 for k_sqdiff (y) and k_monitor_chunks (z), one block per entry.
+//  * rows (y): launch_dims gives a block two rows of a grid with nz > 1 (rows of a multiple of 64 cells) and four
+//    otherwise; every other launcher more: ny <= 2 x 65535 (nz > 1), ny <= 4 x 65535 (nz = 1).
+// Two launchers go further: k_monitor_chunks puts one block per plane on y (tfl_monitor_create refuses gnz > 65535)
+// and the recorder's k_pack_vbox one per row on z (tfl_recorder_create refuses ny > 65535).
+constexpr long long kMaxGridYZ = 65535;
+inline long long max_batch_planes(int nz) { return nz > 1 ? 2 * kMaxGridYZ : kMaxGridYZ; }
+inline long long max_rows(int nz) { return nz > 1 ? 2 * kMaxGridYZ : 4 * kMaxGridYZ; }
+// 0 if every launcher a call on an nb x nz x ny grid can reach fits CUDA's grid, else fails naming the limit.
+inline int check_launch_grid(tfl_ctx* ctx, const char* who, int nb, int nz, int ny) {
+  if ((long long)nb * nz > max_batch_planes(nz))
+    return fail(ctx, "%s: grid too large for one launch: nb x nz = %lld planes, at most %lld (65535 blocks along "
+                     "gridDim.z, %d plane(s) each)", who, (long long)nb * nz, max_batch_planes(nz), nz > 1 ? 2 : 1);
+  if (ny > max_rows(nz))
+    return fail(ctx, "%s: grid too large for one launch: ny = %d rows, at most %lld (65535 blocks along gridDim.y, "
+                     "%d rows each)", who, ny, max_rows(nz), nz > 1 ? 2 : 4);
+  return 0;
+}
+
 // The global planes [*z0, *z1) z-slab rank `rank` of `world` owns in a domain of gnz planes: gnz / world each, one more
 // for the first gnz % world ranks.  The slab simulator, its Jacobi schedule and the slab recorder all use this rule.
 inline void slab_planes(int gnz, int world, int rank, int* z0, int* z1) {
@@ -262,7 +286,7 @@ inline int make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is3d, Geo* g) {
   }
   if (!is3d && flags->nz != 1) return fail(ctx, "2D grid must have zsize == 1");
   if (grid_too_large(g->n, g->nb)) return fail(ctx, "grid too large");
-  return 0;
+  return check_launch_grid(ctx, "grid", g->nb, g->nz, g->ny);
 }
 
 // The step's body forces (lib/simulate.lua:216-239) for a grid of global extent nx x ny x gnz: the vectors that

@@ -34,8 +34,8 @@ int launch_advect_vel(float dt, const float* U, const FT* flags, const unsigned 
 // ---- tfl_advect_tile.cu (-fmad=false): maccormackOurs advectVel as one kernel over shared-memory tiles ----
 // hf: halo of the forward field in cells (1: traces < ~0.5 cell are served from the tile, 2: < ~1.5; longer ones
 // take the general code).  longest: optional device word, atomicMax of the longest trace (float bits).
-// One launch covers every batch entry.  Returns false when the grid does not qualify (2-D, nx % 4 != 0, more
-// than 65535 z tiles over the batch): run launch_advect_vel then.
+// One launch covers every batch entry.  Returns false when the grid does not qualify (2-D, nx % 4 != 0, nz < 3,
+// unaligned U): run launch_advect_vel then.
 bool launch_advect_vel_tile(float dt, const float* U, const unsigned char* flags, const unsigned char* clear,
                             float strength, float* dst, const Geo& g, int hf, unsigned int* longest, cudaStream_t st);
 // advectScalar('maccormackOurs') on the same tiles.

@@ -166,6 +166,9 @@ int tfl_monitor_create(tfl_ctx* ctx, int32_t nb, int32_t gnz, int32_t capacity, 
   if (nb < 1 || gnz < 1) return fail(ctx, "monitor_create: nb and gnz must be >= 1 (got nb = %d, gnz = %d)", nb, gnz);
   if (capacity < 1) return fail(ctx, "monitor_create: capacity must be >= 1 (got %d)", capacity);
   if ((long long)nb * gnz * kMonChunks * 3 >= (1LL << 31)) return fail(ctx, "monitor_create: nb x gnz too large");
+  if (nb > kMaxGridYZ || gnz > kMaxGridYZ)      // k_monitor_chunks: one block per entry on z, per plane on y
+    return fail(ctx, "monitor_create: nb = %d and gnz = %d must each be at most %lld (blocks along gridDim.z and y)",
+                nb, gnz, kMaxGridYZ);
   std::unique_ptr<tfl_monitor> m(new tfl_monitor());
   m->nb = nb; m->gnz = gnz; m->capacity = capacity;
   m->slot_doubles = 1 + (size_t)nb * gnz * 3;

@@ -256,6 +256,7 @@ int tfl_recorder_create(tfl_ctx* ctx, int32_t nz, int32_t ny, int32_t nx, int32_
   if (nz < 1 || ny < 1 || nx < 1) return fail(ctx, "recorder_create: every grid extent must be >= 1 (got %d x %d x %d)", nz, ny, nx);
   if (slots < 1) return fail(ctx, "recorder_create: slots must be >= 1 (got %d)", slots);
   if (grid_too_large((long long)nz * ny * nx, 1)) return fail(ctx, "recorder_create: grid too large");
+  if (ny > kMaxGridYZ) return fail(ctx, "recorder_create: ny = %d, at most %lld (k_pack_vbox: one block per row along gridDim.z)", ny, kMaxGridYZ);
   return recorder_new(ctx, nz, ny, nx, 0, 1, slots, out);
 }
 
@@ -274,6 +275,7 @@ int tfl_recorder_create_slab(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, 
     return fail(ctx, "recorder_create_slab: %d planes over %d ranks leave empty slabs", gnz, world);
   if (rank == 0 && slots < 1) return fail(ctx, "recorder_create_slab: slots must be >= 1 on rank 0 (got %d)", slots);
   if (grid_too_large((long long)gnz * ny * nx, 1)) return fail(ctx, "recorder_create_slab: grid too large");
+  if (ny > kMaxGridYZ) return fail(ctx, "recorder_create_slab: ny = %d, at most %lld (k_pack_vbox: one block per row along gridDim.z)", ny, kMaxGridYZ);
   return recorder_new(ctx, gnz, ny, nx, rank, world, rank == 0 ? slots : 0, out);
 }
 

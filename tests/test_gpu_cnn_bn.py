@@ -22,8 +22,8 @@ banked), with batch statistics (modules saved with train = true) and running sta
     values past 6.  With batch
     statistics changing entry 1 changes entry 0; with running statistics it does not, bit for bit.  Running statistics
     with w = 1, b = 0, mean 0, var 1 - eps equal the model without BN.
-  * The step: a BN model in 3xTF32 at nb = 1 takes the fused step (fused_step_applies, restated as takes_fused_path
-    in tests/test_gpu_step_paths.py) and matches the operator sequence (1e-6) and oracle.simulate with the restated
+  * The step: a BN model in 3xTF32 takes the fused step at any nb (fused_step_applies, restated as takes_fused_path
+    in tests/test_gpu_step_paths.py; tests/test_gpu_batch_models.py steps BN models batched); here at nb = 1 it and matches the operator sequence (1e-6) and oracle.simulate with the restated
     network (2e-5); step-graph replay bit for bit; the host-buffer step.  The tensor-core modes refuse banked BN models
     and the z-slab entry points every BN model, by name; a BN reference file end to end."""
 import ctypes as C

@@ -9,7 +9,8 @@ case is labelled with the convolution kernel the host's predicate picks (nx <= 1
 the box kernel, restated as in test_gpu_conv_tc_zstream.py; nothing observes the launch itself).  The GPU's scale
 (return_scale) must lie in network_bound.scale_interval.
 
-The fused step (tfl_simulate_step, 64^3 and 128^3 in 3xTF32, direct and as a replayed step graph) and the emulated
+The fused step (tfl_simulate_step, 64^3 and 128^3 in 3xTF32 at nb = 1, direct and as a replayed step graph; batches of
+every tensor-core model in tests/test_gpu_batch_models.py) and the emulated
 z-slabs (world 2 and 3 on one GPU) do not return their scale: they are checked on the scale interval
 (forward_bound(scale=None)), against the float64 projection of the pre-projection state.  That state comes from the
 operator sequence (simulate.simulate(outputDiv=True) and setConstVals), which the step tests pin bit-exact; the

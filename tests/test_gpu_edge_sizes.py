@@ -3,13 +3,14 @@ test_oracle_edge_sizes.py pins on the compiled reference at exactly these inputs
 
 Every grid of edge_cases.CASES runs:
   * all six advection methods, scalar (both sampleOutsideFluid settings) and velocity, in place and out of place,
-    at traces of 0.2 to 20 cells; on 3-D grids at nb = 1 also under tile modes 0, 1, 2 and automatic: bit for bit;
+    at traces of 0.2 to 20 cells; on 3-D grids (nb = 1 and 2) also under tile modes 0, 1, 2 and automatic: bit for
+    bit;
   * every point-wise operator, emptyDomain, flagsToOccupancy, rectangularBlur, signedDistanceField, upsampling and
     the backward operators: bit for bit;
   * the Jacobi solve at pTol = 0 with 1, 2, 3, 7 and 40 sweeps and at pTol > 0: p bit for bit, same iterations;
   * the PCG solve with each preconditioner: the tolerances of test_gpu_pcg.py, size-1 components exactly 0.
-STEP_SHAPES also run the whole step (fused convnet, Jacobi, the operator path at nb = 2), 2-D grids the fp32-model
-step, and 4x3x3 a step-graph replay.
+STEP_SHAPES also run the whole step (the fused convnet step at nb = 1 and 2, the operator path at nb = 2, Jacobi), 2-D
+grids the fp32-model step, and 4x3x3 a step-graph replay.
 
 Every array the library reads or writes is a 16-byte-aligned view into a buffer with a guard band of at least one
 plane on each side, filled with a quiet-NaN sentinel: a kernel that reads past a small grid poisons its result, and
@@ -32,7 +33,8 @@ import oracle
 from cases import bits_equal, describe_diff
 from edge_cases import CASES, CASE_IDS, DT, STRENGTH
 from fluidnet_b200 import synth
-from test_gpu_step_paths import MODE_TOL, OPS_TOL, case, close_per_entry, make_batch, quad_dims, same_zero_bits
+from test_gpu_step_paths import (MODE_TOL, OPS_TOL, case, close_per_entry, make_batch, quad_dims, same_zero_bits,
+                                 takes_fused_path)
 
 METHODS = list(oracle.ADVECT_METHODS)
 OURS_VEL = {"maccormackOurs", "rk2Ours", "rk3Ours"}       # advectVel methods the tile kernel runs
@@ -42,8 +44,8 @@ STEP_SHAPES = [(3, 3, 3), (4, 3, 3), (36, 3, 3), (4, 3, 300), (1028, 3, 3)]
 # What each grid (nx, ny, nz) reaches, and why it cannot take a path it does not.
 ROWS = {
     (3, 3, 3): "per-voxel kernels only, one interior cell (size-1 PCG component); no tile, quad or iter4: nx % 4 != 0",
-    (4, 3, 3): "tile kernel smaller than one tile (nb = 1), quad bx = 1 with a 128-row y block on 3 rows; "
-               "per-pass advection at nb = 2 (the tile needs nb = 1)",
+    (4, 3, 3): "tile kernel smaller than one tile (nb = 1 and 2: the batch-wide tiles), quad bx = 1 with a 128-row y "
+               "block on 3 rows",
     (4, 3, 5): "tile with an odd nz; jacobi iter4",
     (33, 3, 3): "per-voxel kernels (nx % 4 != 0)",
     (3, 17, 4): "per-voxel kernels (nx % 4 != 0), ny odd",
@@ -73,9 +75,20 @@ SENTINEL = 0x7FC5A5A5          # a quiet NaN with a payload
 # ---------------------------------------------------------------------------------------------------------------
 def tile_kernel(shape, nb):
     """launch_advect_vel_tile / launch_advect_scalar_tile (tfl_advect_tile.cu) accept the grid (16-byte-aligned
-    views, whole grid on one GPU)."""
+    views, whole grid on one GPU), at any nb: the nb ceil(nz / 8) z tiles of a batch stay within CUDA's 65535 blocks
+    along gridDim.z wherever the grid check (check_launch_grid, nb nz <= 2 x 65535) lets the grid in."""
     nx, ny, nz = shape
-    return nz > 1 and nb == 1 and nx % 4 == 0 and nz >= 3
+    return nz > 1 and nx % 4 == 0 and nz >= 3
+
+
+def tile_modes(shape, nb):
+    """The tfl_debug_advect_tile modes test_advection forces (None: automatic): all of them on every 3-D grid."""
+    return (None, 0, 1, 2) if shape[2] > 1 else (None,)
+
+
+# (nb, conv mode) of test_step_fused_and_ops: the fused step alone and batched, and the operator path batched (an fp32
+# model: fused_step_applies needs a tensor-core mode).
+STEP_LEGS = ((1, "tf32x3"), (2, "tf32x3"), (2, "fp32"))
 
 
 def resident_blocks(shape, nb):
@@ -155,6 +168,11 @@ def test_table_reaches_every_branch():
     assert resident_blocks((128, 8, 8), 1) and jacobi_sweep_kernel((128, 8, 8), 1) == "march"
     assert quad_dims(1, 3, 3, 4)[1] == (1, 128, 2)            # bx = 1, 128 rows per block on a 3-row grid
     assert quad_dims(1, 3, 3, 1028)[0][0] == 9
+    # forced tile modes on the batch-wide tiles (nb = 2), and the step legs: fused at nb = 1 and 2, the operator path
+    # at nb = 2
+    assert any(nb == 2 and tile_kernel(s, nb) and {0, 1, 2} <= set(tile_modes(s, nb)) for s, nb in CASES)
+    legs = {(nb, takes_fused_path({"mode": m, "nb": nb, "pbc": False})) for nb, m in STEP_LEGS}
+    assert {(1, True), (2, True), (2, False)} <= legs, legs
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -226,7 +244,7 @@ def fill(shape, v=123.0):
 def test_advection(orc, shape, nb):
     from fluidnet_b200 import tfluids
     is3d = shape[2] > 1
-    modes = (None, 0, 1, 2) if is3d and nb == 1 else (None,)
+    modes = tile_modes(shape, nb)
     tile = tile_kernel(shape, nb)
     try:
         for trace in edge_cases.traces(shape):
@@ -427,17 +445,17 @@ def step_checks(gd, what):
 @pytest.mark.gpu
 @pytest.mark.parametrize("shape", STEP_SHAPES, ids=["%dx%dx%d" % s for s in STEP_SHAPES])
 def test_step_fused_and_ops(orc, shape):
-    """tfl_simulate_step on the fused convnet path (nb = 1) and on the operator path (nb = 2), two steps each,
-    against the oracle: density bit for bit, U and p within MODE_TOL; at nb = 1 also against the operator
-    sequence within OPS_TOL with the same zeros."""
+    """tfl_simulate_step on each of STEP_LEGS (the fused convnet path at nb = 1 and 2, the operator path at nb = 2),
+    two steps each, against the oracle (density bit for bit, U and p within MODE_TOL) and against the operator
+    sequence (within OPS_TOL with the same zeros)."""
     from fluidnet_b200 import simulate
     from gpu_backend import make_gpu_model
     nx, ny, nz = shape
     mnp = synth.make_model(True)
-    gm = make_gpu_model(mnp)
-    gm.set_mode("tf32x3")
-    for nb in (1, 2):
-        c = case((nz, ny, nx), nb=nb, flags="empty", state="density")
+    for nb, mode in STEP_LEGS:
+        gm = make_gpu_model(mnp)
+        gm.set_mode(mode)
+        c = case((nz, ny, nx), nb=nb, flags="empty", state="density", mode=mode)
         batch = make_batch(orc, c)
         gd = Guards(nx * ny)
         fused, ops = guarded_batch(batch, gd), guarded_batch(batch, gd)
@@ -448,18 +466,16 @@ def test_step_fused_and_ops(orc, shape):
                 ops[k].copy_(fused[k])
             oracle.simulate(orc, c["mconf"], ref, mnp)
             simulate.simulate_fused(None, c["mconf"], fused, gm)
-            if nb == 1:
-                simulate.simulate(None, c["mconf"], ops, gm)
-            what = "%s nb %d step %d" % (shape, nb, step)
+            simulate.simulate(None, c["mconf"], ops, gm)
+            what = "%s nb %d %s step %d" % (shape, nb, mode, step)
             step_checks(gd, what)
             got, opg = host(fused), host(ops)
             assert bits_equal(got["density"], ref["density"]), \
                 "%s density: %s" % (what, describe_diff(got["density"], ref["density"]))
             for k in ("UDiv", "pDiv"):
-                close_per_entry(got[k], ref[k], MODE_TOL["tf32x3"], "%s %s vs oracle" % (what, k))
-                if nb == 1:
-                    close_per_entry(got[k], opg[k], OPS_TOL, "%s %s vs ops" % (what, k))
-                    assert same_zero_bits(got[k], opg[k]), "%s %s zeros" % (what, k)
+                close_per_entry(got[k], ref[k], MODE_TOL[mode], "%s %s vs oracle" % (what, k))
+                close_per_entry(got[k], opg[k], OPS_TOL, "%s %s vs ops" % (what, k))
+                assert same_zero_bits(got[k], opg[k]), "%s %s zeros" % (what, k)
         assert orc.trace_faults() == 0
 
 

@@ -2,7 +2,7 @@
 
 Every row of CASES runs three steps three ways from one state:
   * tfl_simulate_step (simulate.simulate_fused): the fused kernels of tfl_fused.cu (4-voxel quad kernels or the
-    per-voxel ones), or the C operator sequence for an fp32 model, nb > 1 or a pressure BC;
+    per-voxel ones) at any nb, or the C operator sequence for an fp32 model or a pressure BC;
   * simulate.simulate: the operators called one by one from Python;
   * the oracle (oracle.simulate).
 Before each step the operator copy and the oracle are re-seeded with the GPU's current state, so every comparison
@@ -19,8 +19,13 @@ the advection method and tile halo, the trace length, the optional state (densit
 BCs with -0.0, unaligned views), the mconf (gravity, buoyancy, vorticity, strength, dt, a clamping input-scale
 threshold), the flags (geometry, empty box, an open border, Empty / Outflow / Stick cells) and the conv mode.
 test_case_table_reaches_every_branch (no GPU) keeps the table covering every branch of quad_dims
-(tfl_fused.cu) and both paths of tfl_simulate_step."""
+(tfl_fused.cu) and both paths of tfl_simulate_step, each at nb = 1 and nb > 1; test_case_paths_are_the_kernels_that_ran
+proves each row's path from the kernels torch.profiler saw, so the restated rule cannot drift from the library's."""
 import ctypes as C
+import json
+import os
+import subprocess
+import sys
 
 import numpy as np
 import pytest
@@ -86,10 +91,13 @@ CASES = {
     "q12x16x32-threshold-tf32": case((12, 16, 32), threshold=50.0, mode="tf32"),
     # caller-owned views that are only 4-byte aligned: the per-voxel kernels on a quad shape
     "q12x16x32-unaligned": case((12, 16, 32), state="unaligned", method="eulerOurs"),
-    # the C operator path: fp32 model, nb = 2 with per-entry BCs, a pressure BC
+    # the fused step at nb = 2 with per-entry BCs (odd nz: no block straddles; test_gpu_batch_models.py has those)
+    "q10x12x16-nb2": case((10, 12, 16), nb=2, method="maccormack"),
+    # the C operator path: fp32 model, a pressure BC, each at nb = 1 and nb = 2
     "ops12x16x20-fp32": case((12, 16, 20), mode="fp32", gravityScale=0.5, gravity=GRAVITY),
-    "ops10x12x16-nb2": case((10, 12, 16), nb=2, method="maccormack"),
     "ops16x16x16-pbc": case((16, 16, 16), pbc=True, method="rk2Ours"),
+    "ops9x12x20-fp32-nb2": case((9, 12, 20), nb=2, mode="fp32", method="rk3Ours"),
+    "ops8x12x16-pbc-nb2": case((8, 12, 16), nb=2, pbc=True, method="maccormack"),
 }
 
 
@@ -97,8 +105,9 @@ CASES = {
 # Which branch each case reaches (restated from tfl_simulate_step and quad_dims, tfl_fused.cu)
 # ---------------------------------------------------------------------------------------------------------------
 def takes_fused_path(c):
-    """tfl_simulate_step's test: convnet, a tensor-core mode, nb == 1, no pressure BC."""
-    return c["mode"] != "fp32" and c["nb"] == 1 and not c["pbc"]
+    """fused_step_applies (tfl_api.cu) for the 3-D convnet steps these tests run with the default input block: a
+    tensor-core mode and no pressure BC, at any nb."""
+    return c["mode"] != "fp32" and not c["pbc"]
 
 
 def quad_dims(nb, nz, ny, nx):
@@ -157,8 +166,11 @@ def test_case_table_reaches_every_branch():
     assert any(c["mconf"]["vorticityConfinementAmp"] == 0 for c in fused)
     assert any(c["mconf"]["buoyancyScale"] == 0 for c in fused)
     assert any(c["threshold"] > 1.0 for c in fused)
+    assert any(c["nb"] > 1 for c in fused)
     ops = [c for c in CASES.values() if not takes_fused_path(c)]
-    assert {"fp32"} <= {c["mode"] for c in ops} and any(c["nb"] > 1 for c in ops) and any(c["pbc"] for c in ops)
+    for nb in (1, 2):                          # the operator path with each of its two reasons, alone and batched
+        assert any(c["mode"] == "fp32" and c["nb"] == nb for c in ops), nb
+        assert any(c["pbc"] and c["nb"] == nb for c in ops), nb
     # the scalar per-voxel kernels with buoyancy (k_post_advect's neighbour sums)
     assert any("scalar" in branches(c) and c["mconf"]["buoyancyScale"] > 0 and c["state"] != "none"
                for c in fused)
@@ -338,6 +350,73 @@ def test_step_paths(orc, name):
         assert be.trace_faults() == 0, "the oracle traced out of the domain: the case is not a valid input"
     finally:
         set_tile_mode(None)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# Each row's path, from the kernels that ran
+# ---------------------------------------------------------------------------------------------------------------
+def step_path(kernels):
+    """'quad', 'scalar' (the fused step's 4-voxel or per-voxel kernels) or 'ops' (neither: the operator sequence),
+    from the names of the kernels one step ran."""
+    names = list(kernels)
+    quad = any("k_cnn_finish_fused4" in k for k in names)
+    scalar = any("k_cnn_finish_fused" in k and "k_cnn_finish_fused4" not in k for k in names)
+    assert not (quad and scalar), names
+    if quad or scalar:
+        assert any("k_vort_bc_mask" in k for k in names), names
+        return "quad" if quad else "scalar"
+    assert not any("k_vort_bc_mask" in k for k in names), names
+    return "ops"
+
+
+def expected_path(c):
+    b = branches(c)
+    return "ops" if "ops" in b else "scalar" if "scalar" in b else "quad"
+
+
+def run_in_child(module, expr, timeout=900):
+    """json.loads of what `expr` (evaluated after `import <module> as t`) returns in a fresh interpreter.  The profiler
+    runs there: on one H100 run, a profiler session opened in the test process left every capture of
+    test_gpu_launch_tally.py, later in the same process, without a kernel event."""
+    here = os.path.dirname(os.path.abspath(__file__))
+    env = dict(os.environ)
+    env["PYTHONPATH"] = os.pathsep.join(p for p in (here, os.path.dirname(here), env.get("PYTHONPATH")) if p)
+    code = "import json, %s as t; print(json.dumps(%s))" % (module, expr)
+    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=timeout)
+    assert r.returncode == 0, r.stderr[-4000:]
+    return json.loads(r.stdout.strip().splitlines()[-1])
+
+
+def case_kernels():
+    """{row: (launch tally, {kernel: count})} of one tfl_simulate_step per CASES row, under torch.profiler."""
+    from fluidnet_b200 import simulate, tfluids
+    from gpu_backend import make_gpu_model
+    from test_gpu_launch_tally import _tally_and_kernels
+    orc = oracle.Oracle()
+    out = {}
+    for name, c in CASES.items():
+        gm = make_gpu_model(synth.make_model(True), threshold=c["threshold"])
+        gm.set_mode(c["mode"])
+        st = to_gpu(make_batch(orc, c), c["state"] == "unaligned")
+        tally, kernels = _tally_and_kernels(tfluids.context(), lambda: simulate.simulate_fused(None, c["mconf"], st, gm),
+                                            attempts=6)
+        out[name] = (tally, dict(kernels))
+    return out
+
+
+@pytest.mark.gpu
+def test_case_paths_are_the_kernels_that_ran():
+    """Every row takes the path takes_fused_path and quad_dims restate (the fused step's quad or per-voxel kernels, or
+    the operator sequence), as the profiler sees it; on the fused path the library's launch tally counts exactly those
+    kernels."""
+    seen = run_in_child("test_gpu_step_paths", "t.case_kernels()")
+    assert set(seen) == set(CASES)
+    for name, (tally, kernels) in seen.items():
+        path = step_path(kernels)
+        print("step path %s: %s (nb %d, %d kernels)" % (name, path, CASES[name]["nb"], tally))
+        assert path == expected_path(CASES[name]), (name, path, sorted(kernels))
+        if path != "ops":
+            assert tally == sum(kernels.values()), (name, tally, kernels)
 
 
 # ---------------------------------------------------------------------------------------------------------------
