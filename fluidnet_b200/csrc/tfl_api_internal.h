@@ -270,6 +270,12 @@ inline void slab_planes(int gnz, int world, int rank, int* z0, int* z1) {
   *z1 = *z0 + base + (rank < rem ? 1 : 0);
 }
 
+// CUDA IPC for the peer-memory exchanges (tfl_api_slab.cu).  ipc_export: the handle of device allocation `dev` into an
+// ABI buffer of `bytes`, zero-filled behind the handle.  ipc_map: maps the allocation whose handle starts at `handle`
+// into *out; on failure it clears the CUDA error and fails as "<who>: <the CUDA call><which>: <error><tail>".
+int ipc_export(tfl_ctx* ctx, void* dev, char* out, size_t bytes);
+int ipc_map(tfl_ctx* ctx, const char* handle, IpcPtr<float>* out, const char* who, const char* which, const char* tail);
+
 inline int make_geo(tfl_ctx* ctx, const tfl_grid* flags, int is3d, Geo* g) {
   g->nx = flags->nx; g->ny = flags->ny; g->nz = flags->nz; g->nb = flags->nb;
   g->is3d = is3d ? 1 : 0;

@@ -6,6 +6,7 @@
 #include <vector>
 
 #include "tfl_api_internal.h"
+#include "tfl_peer.cuh"
 
 // ---------------------------------------------------------------------------------------
 // One domain split into z-slabs over the GPUs of a node (SURVEY.md 8e).  The reference is
@@ -66,9 +67,41 @@ NcclApi* nccl_api() {
 
 }  // namespace
 
-// floats reserved behind the halo counters of an inbox for the all-reduce: [2 parities][world <= 64][2] doubles, then
-// [2][64] step counters
-constexpr int kSumAreaFloats = 2 * 64 * 2 * 2 + 2 * 64;
+// A rank's inbox: the one allocation its peers store into over peer memory (exported as one CUDA IPC handle).  Every
+// rank's has this layout, in floats, with the counters written and waited on as tfl_peer.cuh describes:
+//   [3 phases][2 from][xbuf_side]        halo messages (from 0: the rank below, 1: the rank above)
+//   [64]                                  their counters, [phase][from], carrying step_no
+//   [2 parities][kMaxRanks][2] doubles    the all-reduce's pair from each rank, parity = step_no & 1
+//   [2 parities][kMaxRanks]               their counters, carrying step_no
+//   [2 parities][2 from][p_side]          the Jacobi p exchange's messages, parity = jseq & 1
+//   [64]                                  their counters, [parity][from], carrying jseq
+// Alternating parities let a rank push the next all-reduce or p exchange while its peer still reads the current one.
+struct SlabInbox {
+  size_t xbuf_side, p_side;             // floats of one halo message / one p message
+  static constexpr int kCounterFloats = 64;
+  static constexpr int kSumSlotFloats = 2 * kMaxRanks * 2 * 2;
+  static constexpr int kSumFloats = kSumSlotFloats + 2 * kMaxRanks;
+  __host__ __device__ float* halo(float* inbox, int phase, int from) const {
+    return inbox + ((size_t)phase * 2 + from) * xbuf_side;
+  }
+  __host__ __device__ unsigned int* halo_flag(float* inbox, int phase, int from) const {
+    return (unsigned int*)(inbox + 6 * xbuf_side) + phase * 2 + from;
+  }
+  __host__ __device__ double* sum_slot(float* inbox, int parity, int rank) const {
+    return reinterpret_cast<double*>(inbox + 6 * xbuf_side + kCounterFloats) + ((size_t)parity * kMaxRanks + rank) * 2;
+  }
+  __host__ __device__ unsigned int* sum_flag(float* inbox, int parity, int rank) const {
+    return reinterpret_cast<unsigned int*>(inbox + 6 * xbuf_side + kCounterFloats + kSumSlotFloats) + parity * kMaxRanks + rank;
+  }
+  __host__ __device__ float* p_area(float* inbox) const { return inbox + 6 * xbuf_side + kCounterFloats + kSumFloats; }
+  __host__ __device__ float* p_buf(float* inbox, int parity, int from) const {
+    return p_area(inbox) + ((size_t)parity * 2 + from) * p_side;
+  }
+  __host__ __device__ unsigned int* p_flag(float* inbox, int parity, int from) const {
+    return (unsigned int*)(p_area(inbox) + 4 * p_side) + parity * 2 + from;
+  }
+  size_t floats() const { return 6 * xbuf_side + kCounterFloats + kSumFloats + 4 * p_side + kCounterFloats; }
+};
 
 struct tfl_slab_sim {
   int gnz = 0, ny = 0, nx = 0, margin = 2, halo = 6;
@@ -81,11 +114,10 @@ struct tfl_slab_sim {
   DevPtr<double> sums;
   DevPtr<float> xbuf;               // [send down | send up | recv from below | recv from above], xbuf_side floats each
   size_t xbuf_side = 0;
-  // Peer-memory halo exchange (CUDA IPC over NVLink, tfl_slab_sim_ipc_*): this rank's inbox -- per phase and side a
-  // receive buffer of xbuf_side floats that the neighbour's push kernel fills with remote stores, and a step counter
-  // it raises afterwards -- and the neighbours' inboxes mapped into this process.
-  DevPtr<float> inbox;              // exported: [3 phases][2 sides][xbuf_side] floats, then 64 counters
-  std::vector<IpcPtr<float>> mapped;           // the other ranks' inboxes (cudaIpcOpenMemHandle), empty at [rank]
+  // Peer-memory exchanges (CUDA IPC over NVLink, tfl_slab_sim_ipc_*): this rank's inbox, which the peers' push kernels
+  // fill with remote stores, and the other ranks' inboxes mapped into this process.
+  DevPtr<float> inbox;              // exported, laid out as SlabInbox
+  std::vector<IpcPtr<float>> mapped;           // the other ranks' inboxes, empty at [rank]
   float* peer_inbox[2] = {nullptr, nullptr};   // lower / upper neighbour's inbox
   std::vector<float*> all_inbox;               // every rank's inbox (own pointer at [rank]): the all-reduce's targets
   DevPtr<float*> all_inbox_dev;                // the same table on the device
@@ -95,8 +127,7 @@ struct tfl_slab_sim {
   EventPtr ev[4][2];
   size_t bytes_sent[3] = {0, 0, 0};
   // Jacobi projection (simMethod 'jacobi'): divergence, second p buffer and mask of the local slab; the p exchanges
-  // land in their own inbox area behind the all-reduce's -- [2 parities][2 sides][p_side] floats, then
-  // [2 parities][2 sides] counters -- and carry the monotone sequence number jseq instead of step_no.
+  // land in their own inbox area and carry the monotone sequence number jseq instead of step_no.
   DevPtr<float> div;
   DevPtr<float> p2;
   DevPtr<unsigned char> mask;
@@ -106,7 +137,29 @@ struct tfl_slab_sim {
   std::vector<EventPtr> jev;        // [2 * exchange] begin / end of the last step's p exchanges
   int jx = 0;                       // p exchanges of the last step
   size_t jbytes = 0;
+  SlabInbox layout() const { return {xbuf_side, p_side}; }
 };
+
+int ipc_export(tfl_ctx* ctx, void* dev, char* out, size_t bytes) {
+  cudaIpcMemHandle_t h;
+  TFL_CUDA(ctx, cudaIpcGetMemHandle(&h, dev));
+  memset(out, 0, bytes);
+  memcpy(out, &h, sizeof(h));
+  return 0;
+}
+
+int ipc_map(tfl_ctx* ctx, const char* handle, IpcPtr<float>* out, const char* who, const char* which, const char* tail) {
+  cudaIpcMemHandle_t h;
+  memcpy(&h, handle, sizeof(h));
+  void* q = nullptr;
+  const cudaError_t e = cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess);
+  if (e != cudaSuccess) {
+    cudaGetLastError();
+    return fail(ctx, "%s: cudaIpcOpenMemHandle%s: %s%s", who, which, cudaGetErrorString(e), tail);
+  }
+  out->reset((float*)q);
+  return 0;
+}
 
 extern "C" {
 
@@ -203,7 +256,7 @@ int tfl_slab_sim_create(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32
       !(s->p2 = dev_alloc<float>(s->cells)) || !(s->mask = dev_alloc<unsigned char>(s->cells)))
     return fail(ctx, kFailed);
   if (s->world > 1 &&
-      (!(s->inbox = dev_zeros<float>(6 * s->xbuf_side + 64 + kSumAreaFloats + 4 * s->p_side + 64)) ||
+      (!(s->inbox = dev_zeros<float>(s->layout().floats())) ||
        !(s->push_done = dev_zeros<unsigned int>(1))))
     return fail(ctx, kFailed);
   for (auto& pr : s->ev)
@@ -264,54 +317,46 @@ struct SlabPack {
   long long src_lo, src_hi;         // float offset (within a channel) of the planes sent down / up
   long long dst_lo, dst_hi;         // ... of the ghost planes filled from below / above
   float* send_lo; float* send_hi; float* recv_lo; float* recv_hi;     // null: no neighbour on that side
+  // Grid-stride walk over both sides' messages: float r of side `side`'s message is float e of channel c's planes.
+  template <typename F> __device__ __forceinline__ void walk(F f) const {
+    const long long per_side = cnt * nchan;
+    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < 2 * per_side; t += (long long)gridDim.x * blockDim.x) {
+      const int side = t >= per_side;
+      const long long r = t - side * per_side;
+      const int c = (int)(r / cnt);
+      f(side, r, c, r - c * cnt);
+    }
+  }
+  // The planes sent down / up -> the messages to the lower / upper neighbour (null: none).
+  __device__ __forceinline__ void gather(float* lo, float* hi) const {
+    walk([&](int side, long long r, int c, long long e) {
+      float* buf = side ? hi : lo;
+      if (buf) buf[r] = chan[c][(side ? src_hi : src_lo) + e];
+    });
+  }
+  // The messages from below / above (null: none) -> the ghost planes; CG loads past L1 (a peer's remote stores).
+  template <bool CG> __device__ __forceinline__ void scatter(const float* lo, const float* hi) const {
+    walk([&](int side, long long r, int c, long long e) {
+      const float* buf = side ? hi : lo;
+      if (buf) chan[c][(side ? dst_hi : dst_lo) + e] = CG ? __ldcg(buf + r) : buf[r];
+    });
+  }
 };
 template <bool UNPACK>
 __global__ void k_slab_pack(SlabPack d) {
-  const long long per_side = d.cnt * d.nchan;
-  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < 2 * per_side; t += (long long)gridDim.x * blockDim.x) {
-    const int side = t >= per_side;
-    const long long r = t - side * per_side;
-    const int c = (int)(r / d.cnt);
-    const long long e = r - c * d.cnt;
-    if (!UNPACK) {
-      float* buf = side ? d.send_hi : d.send_lo;
-      if (buf) buf[r] = d.chan[c][(side ? d.src_hi : d.src_lo) + e];
-    } else {
-      const float* buf = side ? d.recv_hi : d.recv_lo;
-      if (buf) d.chan[c][(side ? d.dst_hi : d.dst_lo) + e] = buf[r];
-    }
-  }
+  if (!UNPACK) d.gather(d.send_lo, d.send_hi);
+  else d.scatter<false>(d.recv_lo, d.recv_hi);
 }
 
 // Peer-memory exchange, sending half: every channel's boundary planes are written straight into the neighbours'
-// inboxes (remote stores over NVLink), and when the last CTA has finished, the step number is stored (system
-// scope, after a system-wide fence) into the neighbours' counters.
+// inboxes (remote stores over NVLink), then the last CTA publishes the step number in the neighbours' counters.
 __global__ void k_slab_push(SlabPack d, float* peer_lo_buf, float* peer_hi_buf, unsigned int* peer_lo_flag,
                             unsigned int* peer_hi_flag, unsigned int step, unsigned int* done) {
-  const long long per_side = d.cnt * d.nchan;
-  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < 2 * per_side; t += (long long)gridDim.x * blockDim.x) {
-    const int side = t >= per_side;
-    const long long r = t - side * per_side;
-    const int c = (int)(r / d.cnt);
-    const long long e = r - c * d.cnt;
-    float* buf = side ? peer_hi_buf : peer_lo_buf;
-    if (buf) buf[r] = d.chan[c][(side ? d.src_hi : d.src_lo) + e];
-  }
-  __threadfence_system();
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    const unsigned int prev = atomicAdd(done, 1u);
-    if (prev == gridDim.x - 1) {               // every CTA's stores are fenced: publish
-      *done = 0u;
-      __threadfence_system();
-      if (peer_lo_flag) asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(peer_lo_flag), "r"(step) : "memory");
-      if (peer_hi_flag) asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(peer_hi_flag), "r"(step) : "memory");
-    }
-  }
+  d.gather(peer_lo_buf, peer_hi_buf);
+  last_cta_publish(done, gridDim.x, threadIdx.x == 0, peer_lo_flag, peer_hi_flag, step);
 }
 // ... receiving half: wait until the neighbours' counters have reached this step, then scatter the inbox into the
-// ghost planes.  The wait is bounded (a neighbour that never arrives raises the fault counter instead of hanging
-// the GPU).
+// ghost planes.  A neighbour that never arrives raises the fault counter, and nothing is scattered.
 __global__ void k_slab_pull(SlabPack d, const float* buf_lo, const float* buf_hi, const unsigned int* flag_lo,
                             const unsigned int* flag_hi, unsigned int step, unsigned long long* faults) {
   __shared__ int ok;
@@ -320,52 +365,29 @@ __global__ void k_slab_pull(SlabPack d, const float* buf_lo, const float* buf_hi
     const long long t0 = clock64();
     for (int sde = 0; sde < 2; sde++) {
       const unsigned int* f = sde ? flag_hi : flag_lo;
-      if (!f) continue;
-      for (;;) {
-        unsigned int v;
-        asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(f) : "memory");
-        if ((int)(v - step) >= 0) break;
-        if (clock64() - t0 > 4000000000LL) { ok = 0; break; }       // ~2 s
-        __nanosleep(200);
-      }
+      if (f && !wait_seq(f, step, t0, 200)) ok = 0;
     }
     if (!ok && blockIdx.x == 0 && faults) atomicAdd(faults, 1ULL);
   }
   __syncthreads();
   if (!ok) return;
-  const long long per_side = d.cnt * d.nchan;
-  for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < 2 * per_side; t += (long long)gridDim.x * blockDim.x) {
-    const int side = t >= per_side;
-    const long long r = t - side * per_side;
-    const int c = (int)(r / d.cnt);
-    const long long e = r - c * d.cnt;
-    const float* buf = side ? buf_hi : buf_lo;
-    if (buf) d.chan[c][(side ? d.dst_hi : d.dst_lo) + e] = __ldcg(buf + r);
-  }
+  d.scatter<true>(buf_lo, buf_hi);
 }
 
 // All-reduce of the two partial sums over peer memory: every rank stores its pair into slot [parity][rank] of every
 // rank's inbox and raises that rank's counter [parity][rank]; then waits for all counters of its own inbox and adds
 // the pairs in rank order (the same order on every rank: identical results everywhere, independent of timing).
-// Slots alternate with the step's parity: a rank that is still reading step s cannot be overwritten by step s + 1.
-__device__ __forceinline__ double* sum_slot(float* inbox, size_t xbuf_side, int parity, int r) {
-  return reinterpret_cast<double*>(inbox + 6 * xbuf_side + 64) + ((size_t)parity * 64 + r) * 2;
-}
-__device__ __forceinline__ unsigned int* sum_flag(float* inbox, size_t xbuf_side, int parity, int r) {
-  return reinterpret_cast<unsigned int*>(inbox + 6 * xbuf_side + 64 + 2 * 64 * 2 * 2) + parity * 64 + r;
-}
-__global__ void k_sum_push(const double* __restrict__ mine, float* const* __restrict__ inboxes, size_t xbuf_side, int rank,
+__global__ void k_sum_push(const double* __restrict__ mine, float* const* __restrict__ inboxes, SlabInbox box, int rank,
                            int world, unsigned int step) {
   const int t = threadIdx.x;
   if (t >= world) return;
   const int parity = step & 1;
-  double* slot = sum_slot(inboxes[t], xbuf_side, parity, rank);
+  double* slot = box.sum_slot(inboxes[t], parity, rank);
   slot[0] = mine[0];
   slot[1] = mine[1];
-  __threadfence_system();
-  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(sum_flag(inboxes[t], xbuf_side, parity, rank)), "r"(step) : "memory");
+  publish_seq(box.sum_flag(inboxes[t], parity, rank), step);
 }
-__global__ void k_sum_pull(double* __restrict__ out, float* inbox, size_t xbuf_side, int world, unsigned int step,
+__global__ void k_sum_pull(double* __restrict__ out, float* inbox, SlabInbox box, int world, unsigned int step,
                            unsigned long long* faults) {
   __shared__ int ok;
   const int t = threadIdx.x, parity = step & 1;
@@ -373,20 +395,14 @@ __global__ void k_sum_pull(double* __restrict__ out, float* inbox, size_t xbuf_s
   __syncthreads();
   if (t < world) {
     const long long t0 = clock64();
-    for (;;) {
-      unsigned int v;
-      asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(sum_flag(inbox, xbuf_side, parity, t)) : "memory");
-      if ((int)(v - step) >= 0) break;
-      if (clock64() - t0 > 4000000000LL) { ok = 0; break; }
-      __nanosleep(100);
-    }
+    if (!wait_seq(box.sum_flag(inbox, parity, t), step, t0, 100)) ok = 0;
   }
   __syncthreads();
   if (t == 0) {
     if (!ok) { if (faults) atomicAdd(faults, 1ULL); return; }
     double s0 = 0.0, s1 = 0.0;
     for (int r = 0; r < world; r++) {
-      const volatile double* slot = sum_slot(inbox, xbuf_side, parity, r);
+      const volatile double* slot = box.sum_slot(inbox, parity, r);
       s0 += slot[0];
       s1 += slot[1];
     }
@@ -433,17 +449,10 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
     const bool lo = s->rank > 0, hi = s->rank < s->world - 1;
     const int blocks = (int)std::min<size_t>((2 * side + 255) / 256, 132 * 4);
     if (s->peer_ok) {
-      // inbox layout: buffer (phase, from-below = 0 / from-above = 1) at ((phase * 2 + from) * xbuf_side), counters behind;
-      // the p exchange's (parity, from) buffers and counters behind the all-reduce area
-      const size_t p_area = 6 * s->xbuf_side + 64 + kSumAreaFloats;
+      const SlabInbox box = s->layout();
       const unsigned int seq = pph ? s->jseq : s->step_no, par = seq & 1u;
-      auto buf = [&](float* base, int from) {
-        return pph ? base + p_area + ((size_t)par * 2 + from) * s->p_side : base + ((size_t)phase * 2 + from) * s->xbuf_side;
-      };
-      auto flag = [&](float* base, int from) {
-        return pph ? (unsigned int*)(base + p_area + 4 * s->p_side) + par * 2 + from
-                   : (unsigned int*)(base + 6 * s->xbuf_side) + phase * 2 + from;
-      };
+      auto buf = [&](float* base, int from) { return pph ? box.p_buf(base, par, from) : box.halo(base, phase, from); };
+      auto flag = [&](float* base, int from) { return pph ? box.p_flag(base, par, from) : box.halo_flag(base, phase, from); };
       d.send_lo = d.send_hi = d.recv_lo = d.recv_hi = nullptr;
       // my first owned planes land in the lower neighbour's "from above" slot, my last ones in the upper neighbour's "from below"
       k_slab_push<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(s->peer_inbox[0], 1) : nullptr, hi ? buf(s->peer_inbox[1], 0) : nullptr,
@@ -720,8 +729,8 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
   }
   TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0].get(), ctx->stream));
   if (s->world > 1 && s->peer_ok && s->all_inbox_dev) {
-    k_sum_push<<<1, 64, 0, ctx->stream>>>(sums, s->all_inbox_dev.get(), s->xbuf_side, s->rank, s->world, s->step_no);
-    k_sum_pull<<<1, 64, 0, ctx->stream>>>(sums, s->inbox.get(), s->xbuf_side, s->world, s->step_no, ctx->counters.get());
+    k_sum_push<<<1, kMaxRanks, 0, ctx->stream>>>(sums, s->all_inbox_dev.get(), s->layout(), s->rank, s->world, s->step_no);
+    k_sum_pull<<<1, kMaxRanks, 0, ctx->stream>>>(sums, s->inbox.get(), s->layout(), s->world, s->step_no, ctx->counters.get());
     ctx->launches += 2;
   } else if (s->world > 1 && ctx->comm) {
     TFL_NCCL(ctx, nccl_api()->AllReduce(sums, sums, 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
@@ -770,11 +779,7 @@ int tfl_slab_sim_ipc_export(tfl_ctx* ctx, tfl_slab_sim* s, char* handle_out) {
   if (!s || !handle_out) return fail(ctx, "slab_sim_ipc_export: nil argument");
   if (!s->inbox) return fail(ctx, "slab_sim_ipc_export: a single rank has no neighbours");
   static_assert(sizeof(cudaIpcMemHandle_t) <= TFL_IPC_HANDLE_BYTES, "IPC handle fits the ABI buffer");
-  cudaIpcMemHandle_t h;
-  TFL_CUDA(ctx, cudaIpcGetMemHandle(&h, s->inbox.get()));
-  memset(handle_out, 0, TFL_IPC_HANDLE_BYTES);
-  memcpy(handle_out, &h, sizeof(h));
-  return 0;
+  return ipc_export(ctx, s->inbox.get(), handle_out, TFL_IPC_HANDLE_BYTES);
 }
 
 // ... and map every rank's (handles: world x TFL_IPC_HANDLE_BYTES in rank order; NULL switches back to NCCL).
@@ -794,27 +799,22 @@ int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* s, const char* handles)
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   drop();
   if (!handles) return 0;                          // back to NCCL (e.g. another rank could not map its peers)
-  if (s->world > 64) return fail(ctx, "slab_sim_ipc_connect: more than 64 ranks");
+  if (s->world > kMaxRanks) return fail(ctx, "slab_sim_ipc_connect: more than %d ranks", kMaxRanks);
   s->mapped.resize(s->world);
   s->all_inbox.assign(s->world, nullptr);
   s->all_inbox[s->rank] = s->inbox.get();
   for (int r = 0; r < s->world; r++) {
     if (r == s->rank) continue;
-    cudaIpcMemHandle_t h;
-    memcpy(&h, handles + (size_t)r * TFL_IPC_HANDLE_BYTES, sizeof(h));
-    void* q = nullptr;
-    const cudaError_t e = cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess);
-    if (e != cudaSuccess) {
-      cudaGetLastError();
+    if (ipc_map(ctx, handles + (size_t)r * TFL_IPC_HANDLE_BYTES, &s->mapped[r], "slab_sim_ipc_connect",
+                ("(rank " + std::to_string(r) + ")").c_str(), " (the exchanges stay on NCCL)")) {
       drop();
-      return fail(ctx, "slab_sim_ipc_connect: cudaIpcOpenMemHandle(rank %d): %s (the exchanges stay on NCCL)", r, cudaGetErrorString(e));
+      return 1;
     }
-    s->mapped[r].reset((float*)q);
-    s->all_inbox[r] = (float*)q;
+    s->all_inbox[r] = s->mapped[r].get();
   }
   if (!s->all_inbox_dev) {
     void* p = nullptr;
-    TFL_CUDA(ctx, cudaMalloc(&p, 64 * sizeof(float*)));
+    TFL_CUDA(ctx, cudaMalloc(&p, kMaxRanks * sizeof(float*)));
     s->all_inbox_dev.reset((float**)p);
   }
   TFL_CUDA(ctx, cudaMemcpy(s->all_inbox_dev.get(), s->all_inbox.data(), s->world * sizeof(float*), cudaMemcpyHostToDevice));

@@ -17,7 +17,7 @@ struct CudaIpcClose { void operator()(void* p) const { cudaIpcCloseMemHandle(p);
 
 template <typename T> using DevPtr = std::unique_ptr<T, CudaFree>;          // device memory
 template <typename T> using PinnedPtr = std::unique_ptr<T, CudaFreeHost>;   // pinned host memory
-template <typename T> using IpcPtr = std::unique_ptr<T, CudaIpcClose>;      // a peer's memory (cudaIpcOpenMemHandle)
+template <typename T> using IpcPtr = std::unique_ptr<T, CudaIpcClose>;      // a peer's memory (ipc_map)
 using StreamPtr = std::unique_ptr<CUstream_st, CudaStreamDestroy>;
 using EventPtr = std::unique_ptr<CUevent_st, CudaEventDestroy>;
 using GraphPtr = std::unique_ptr<CUgraph_st, CudaGraphDestroy>;

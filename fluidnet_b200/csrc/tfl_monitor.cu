@@ -15,8 +15,8 @@
 // host adding them in ascending z repeats the device's last step bit for bit.
 //
 // Records go straight into a ring of pinned, mapped host slots: the finishing CTA stores the record's doubles, fences
-// at system scope and stores the record's sequence number last with release semantics (the k_slab_push pattern).  The
-// host polls that word; there is no copy stream and no event per record.
+// at system scope and stores the record's sequence number last with release semantics (tfl_peer.cuh).  The host polls
+// that word; there is no copy stream and no event per record.
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <string.h>
@@ -24,6 +24,7 @@
 
 #include "tfl_device.cuh"
 #include "tfl_api_internal.h"
+#include "tfl_peer.cuh"
 #include "../../include/tfl.h"
 
 constexpr int kMonThreads = 256;
@@ -116,7 +117,7 @@ k_monitor_finish(const double* __restrict__ part, int nb, int nplanes, int nchun
   }
   __threadfence_system();
   __syncthreads();
-  if (threadIdx.x == 0) asm volatile("st.release.sys.global.u64 [%0], %1;" ::"l"(seq_word), "l"(seq) : "memory");
+  if (threadIdx.x == 0) store_release_sys(seq_word, seq);
 }
 
 // A ring of `capacity` mapped host slots; slot = [sequence word][nb x gnz x 3 doubles].  Records in flight or

@@ -16,14 +16,13 @@
 #include <string.h>
 
 #include "tfl_api_internal.h"
+#include "tfl_peer.cuh"
 #include "../../include/tfl.h"
 
 constexpr int kPackTile = 32;     // a 32 x 32 (z, x) tile per block
 constexpr int kPackRows = 8;      // 32 x 8 threads, 4 rows each
-constexpr int kMaxRanks = 64;
 // Behind the staging frame of a z-slab recorder: arrived[kMaxRanks], then freed (unsigned words, sequence numbers).
 constexpr int kCounterWords = kMaxRanks + 64;
-constexpr long long kWaitCycles = 4000000000LL;     // ~2 s at the H100's clock, as the slab exchanges' waits
 constexpr int32_t kHandleMagic = 0x52464c54;        // "TLFR"
 
 // Global planes [z0, z1) of in ([nz_local][ny][nx], x fastest; local plane 0 is global plane z_offset) -> out, a
@@ -34,8 +33,7 @@ constexpr int32_t kHandleMagic = 0x52464c54;        // "TLFR"
 // transposed read free of bank conflicts.  A bit copy (32-bit words, no arithmetic): -0.0, denormals and NaN payloads
 // arrive unchanged.  The whole grid is [0, nz), z_offset = 0, gnz = nz, with no gate and no arrival counter.
 // A z-slab rank other than the writer passes `gate` (the pack runs only if the wait before it stored `seq` there) and
-// `arrived`: after the last CTA's stores, fenced at system scope, `seq` is stored there with release semantics
-// (the k_slab_push pattern; `done` counts the finished CTAs and is reset by the last one).
+// `arrived`, where the last CTA publishes `seq` once every CTA's stores are done (`done` counts the CTAs).
 // Not in an anonymous namespace: the kernel keeps a stable name in traces and profiles.
 __global__ void __launch_bounds__(kPackTile * kPackRows)
 k_pack_vbox(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, int z0, int z1, int z_offset, int gnz, int ny,
@@ -59,16 +57,7 @@ k_pack_vbox(const uint32_t* __restrict__ in, uint32_t* __restrict__ out, int z0,
     if (xo < nx && z < z1) out[((long long)xo * ny + y) * gnz + z] = tile[tx][r];
   }
   if (!arrived) return;
-  __threadfence_system();
-  __syncthreads();
-  if (tx == 0 && ty == 0) {
-    const unsigned int blocks = gridDim.x * gridDim.y * gridDim.z;
-    if (atomicAdd(done, 1u) == blocks - 1) {        // every CTA's stores are fenced: publish
-      *done = 0u;
-      __threadfence_system();
-      asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(arrived), "r"(seq) : "memory");
-    }
-  }
+  last_cta_publish(done, gridDim.x * gridDim.y * gridDim.z, tx == 0 && ty == 0, arrived, nullptr, seq);
 }
 
 namespace {
@@ -77,14 +66,7 @@ namespace {
 // frame left the staging frame), then *gate = seq.  A wait that times out stores nothing and raises the fault counter.
 __global__ void k_rec_wait_freed(const unsigned int* freed, unsigned int seq, unsigned int* gate,
                                  unsigned long long* faults) {
-  const long long t0 = clock64();
-  for (;;) {
-    unsigned int v;
-    asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(freed) : "memory");
-    if ((int)(v - (seq - 1u)) >= 0) break;
-    if (clock64() - t0 > kWaitCycles) { if (faults) atomicAdd(faults, 1ULL); return; }
-    __nanosleep(200);
-  }
+  if (!wait_seq(freed, seq - 1u, clock64(), 200)) { if (faults) atomicAdd(faults, 1ULL); return; }
   *gate = seq;
 }
 
@@ -98,13 +80,7 @@ __global__ void k_rec_wait_arrived(const unsigned int* arrived, int world, unsig
   __syncthreads();
   if (t >= 1 && t < world) {
     const long long t0 = clock64();
-    for (;;) {
-      unsigned int v;
-      asm volatile("ld.acquire.sys.global.u32 %0, [%1];" : "=r"(v) : "l"(arrived + t) : "memory");
-      if ((int)(v - seq) >= 0) break;
-      if (clock64() - t0 > kWaitCycles) { atomicOr(&miss, 1ULL << t); break; }
-      __nanosleep(200);
-    }
+    if (!wait_seq(arrived + t, seq, t0, 200)) atomicOr(&miss, 1ULL << t);
   }
   __syncthreads();
   if (t == 0) {
@@ -114,10 +90,7 @@ __global__ void k_rec_wait_arrived(const unsigned int* arrived, int world, unsig
 }
 
 // ... and after it: freed = seq, so the other ranks may pack the next frame.
-__global__ void k_rec_publish_freed(unsigned int* freed, unsigned int seq) {
-  __threadfence_system();
-  asm volatile("st.release.sys.global.u32 [%0], %1;" ::"l"(freed), "r"(seq) : "memory");
-}
+__global__ void k_rec_publish_freed(unsigned int* freed, unsigned int seq) { publish_seq(freed, seq); }
 
 }  // namespace
 
@@ -296,12 +269,9 @@ int tfl_recorder_ipc_export(tfl_ctx* ctx, tfl_recorder* r, char* handle_out) {
   if (r->world == 1) return fail(ctx, "recorder_ipc_export: a recorder of one rank has nothing to share");
   if (r->rank != 0) return fail(ctx, "recorder_ipc_export: rank %d does not export; rank 0 (the writer) does", r->rank);
   static_assert(sizeof(cudaIpcMemHandle_t) + 5 * sizeof(int32_t) <= TFL_RECORDER_HANDLE_BYTES, "handle fits the ABI buffer");
-  cudaIpcMemHandle_t h;
-  TFL_CUDA(ctx, cudaIpcGetMemHandle(&h, r->stage.get()));
-  memset(handle_out, 0, TFL_RECORDER_HANDLE_BYTES);
-  memcpy(handle_out, &h, sizeof(h));
+  if (ipc_export(ctx, r->stage.get(), handle_out, TFL_RECORDER_HANDLE_BYTES)) return 1;
   const int32_t meta[5] = {kHandleMagic, r->nz, r->ny, r->nx, r->world};
-  memcpy(handle_out + sizeof(h), meta, sizeof(meta));
+  memcpy(handle_out + sizeof(cudaIpcMemHandle_t), meta, sizeof(meta));
   r->connected = true;
   return 0;
 }
@@ -313,22 +283,14 @@ int tfl_recorder_ipc_connect(tfl_ctx* ctx, tfl_recorder* r, const char* handle) 
   if (!r || !handle) return fail(ctx, "recorder_ipc_connect: nil argument");
   if (r->rank == 0) return fail(ctx, "recorder_ipc_connect: rank 0 (the writer) exports its frame, it does not connect");
   if (r->connected) return fail(ctx, "recorder_ipc_connect: rank %d is already connected", r->rank);
-  cudaIpcMemHandle_t h;
   int32_t meta[5];
-  memcpy(&h, handle, sizeof(h));
-  memcpy(meta, handle + sizeof(h), sizeof(meta));
+  memcpy(meta, handle + sizeof(cudaIpcMemHandle_t), sizeof(meta));
   if (meta[0] != kHandleMagic) return fail(ctx, "recorder_ipc_connect: the bytes are not a recorder's handle");
   if (meta[1] != r->nz || meta[2] != r->ny || meta[3] != r->nx || meta[4] != r->world)
     return fail(ctx, "recorder_ipc_connect: the handle is of a %d x %d x %d recorder over %d ranks, this one is "
                      "%d x %d x %d over %d ranks", meta[1], meta[2], meta[3], meta[4], r->nz, r->ny, r->nx, r->world);
-  void* q = nullptr;
-  const cudaError_t e = cudaIpcOpenMemHandle(&q, h, cudaIpcMemLazyEnablePeerAccess);
-  if (e != cudaSuccess) {
-    cudaGetLastError();
-    return fail(ctx, "recorder_ipc_connect: cudaIpcOpenMemHandle (rank 0's frame): %s", cudaGetErrorString(e));
-  }
-  r->mapped.reset((float*)q);
-  r->frame_dev = (float*)q;
+  if (ipc_map(ctx, handle, &r->mapped, "recorder_ipc_connect", " (rank 0's frame)", "")) return 1;
+  r->frame_dev = r->mapped.get();
   r->counters = reinterpret_cast<unsigned int*>(r->frame_dev + counter_offset((size_t)r->nz * r->ny * r->nx));
   r->connected = true;
   return 0;
