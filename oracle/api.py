@@ -6,6 +6,8 @@ import subprocess
 
 import numpy as np
 
+from .model import model_forward
+
 HERE = os.path.dirname(os.path.abspath(__file__))
 ORACLE_SO = os.path.join(HERE, "liboracle.so")
 REF_SO = os.path.join(HERE, "_ref", "libtfluids_ref.so")
@@ -506,8 +508,8 @@ class Reference(Oracle):
 
 
 # ----------------------------------------------------------------------------------------
-# The loop around the operators (torch/lib/simulate.lua) and the projection model
-# (torch/lib/model.lua), restated on top of a backend (Oracle or Reference).
+# The loop around the operators (torch/lib/simulate.lua), restated on top of a backend
+# (Oracle or Reference); the projection model (torch/lib/model.lua) is oracle/model.py.
 # ----------------------------------------------------------------------------------------
 def default_mconf(**over):
     """Keys the hot path reads (lib/simulate.lua:188-291; defaults lib/default_conf.lua)."""
@@ -562,70 +564,10 @@ def _set_const_vals(be, batch, p, U, flags, density):
         be.applyBC(density, batch["densityBCInvMask"], batch["densityBC"])
 
 
-def model_forward(be, model, pDiv, UDiv, flags, threshold=1e-5):
-    """lib/model.lua:27-401 for the 'default' graph (inputs pDiv, div, flags).
-
-    model: {"is3D": bool, "layers": [(weight, bias), ...]}; ReLU after every layer but
-    the last (lib/model.lua:262-364).  Returns (p, U, scale)."""
-    is3d = model["is3D"]
-    U1 = UDiv.copy()
-    be.setWallBcsForward(U1, flags, as_mask_multiply=True)              # model.lua:81-84
-    div = be.velocityDivergenceForward(U1, flags)                       # :86-89
-    b = U1.shape[0]
-    scales = np.empty(b, np.float32)
-    for ib in range(b):                                                 # :92-117
-        s = np.float32(be.sampleStd(U1[ib]))
-        scales[ib] = max(s, np.float32(threshold))
-    sc = scales.reshape(b, 1, 1, 1, 1)
-    pS = (pDiv / sc).astype(np.float32)                                 # :119-130 (CDivTable)
-    US = (U1 / sc).astype(np.float32)
-    divS = (div / sc).astype(np.float32)
-    occ = be.flagsToOccupancy(flags)                                    # :144-147
-    x = np.ascontiguousarray(np.concatenate([pS, divS, occ], axis=1))   # :134-150
-    nl = len(model["layers"])
-    pool = model.get("pool") or [1] * nl                                # 'tog' graphs, model.lua:164-226
-    up = model.get("up") or [1] * nl
-    sigmoid = model.get("nonlinType", "relu") == "sigmoid"
-    for li, (w, bias) in enumerate(model["layers"]):
-        plain = up[li] == 1 and pool[li] == 1 and not sigmoid
-        x = be.conv(x, w, bias, is3d, relu=(plain and li < nl - 1))
-        if plain:
-            continue
-        if up[li] > 1:                                                  # *_convolution_upsample.lua updateOutput
-            s_ = up[li]
-            b_, ct, z_, y_, x_ = x.shape
-            if is3d:
-                no = ct // s_ ** 3
-                x = x.reshape(b_, no, s_, s_, s_, z_, y_, x_).transpose(0, 1, 5, 2, 6, 3, 7, 4)
-                x = np.ascontiguousarray(x).reshape(b_, no, z_ * s_, y_ * s_, x_ * s_)
-            else:
-                no = ct // s_ ** 2
-                x = x.reshape(b_, no, s_, s_, z_, y_, x_).transpose(0, 1, 4, 5, 2, 6, 3)
-                x = np.ascontiguousarray(x).reshape(b_, no, z_, y_ * s_, x_ * s_)
-        if li < nl - 1:                                                 # addNonlinearity
-            x = (1.0 / (1.0 + np.exp(-x.astype(np.float64)))).astype(np.float32) if sigmoid else np.maximum(x, 0)
-        if pool[li] > 1:                                                # addPooling (cudnn avg / max)
-            q = pool[li]
-            b_, c_, z_, y_, x_ = x.shape
-            qz = q if is3d else 1
-            v = x.reshape(b_, c_, z_ // qz, qz, y_ // q, q, x_ // q, q)
-            if model.get("poolType", "avg") == "max":
-                x = v.max(axis=(3, 5, 7))
-            else:
-                x = (v.astype(np.float64).sum(axis=(3, 5, 7)) / (qz * q * q)).astype(np.float32)
-        x = np.ascontiguousarray(x, np.float32)
-    p = x
-    U2 = np.ascontiguousarray(US.copy())
-    be.velocityUpdateForward(U2, flags, p)                              # :380
-    p = (p * sc).astype(np.float32)                                     # :384-387 (CMulTable)
-    U2 = np.ascontiguousarray((U2 * sc).astype(np.float32))
-    be.setWallBcsForward(U2, flags, as_mask_multiply=True)              # :390
-    return p, U2, scales
-
-
-def simulate(be, mconf, batch, model=None):
+def simulate(be, mconf, batch, model=None, f64=False):
     """tfluids.simulate, lib/simulate.lua:175-327.  batch holds numpy arrays pDiv, UDiv,
-    flags, density (+ optional BC arrays) and is updated in place."""
+    flags, density (+ optional BC arrays) and is updated in place.  f64: the projection network
+    in float64 (model_forward)."""
     p, U, flags, density = batch["pDiv"], batch["UDiv"], batch["flags"], batch.get("density")
     dt = mconf["dt"]
     if density is not None:
@@ -653,8 +595,11 @@ def simulate(be, mconf, batch, model=None):
         be.setWallBcsForward(U, flags)
     _set_const_vals(be, batch, p, U, flags, density)
     if mconf["simMethod"] == "convnet":
-        pP, UP, _ = model_forward(be, model, p, U, flags,
-                                  mconf.get("normalizeInputThreshold", 1e-5))
+        # f64 only as a keyword, and only when asked for: a forward put in place of oracle.api.model_forward with
+        # the signature (be, model, pDiv, UDiv, flags, threshold) keeps running the float32 step.
+        threshold = mconf.get("normalizeInputThreshold", 1e-5)
+        pP, UP, _ = (model_forward(be, model, p, U, flags, threshold, f64=True) if f64 else
+                     model_forward(be, model, p, U, flags, threshold))
         p[...] = pP
         U[...] = UP
     else:

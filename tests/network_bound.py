@@ -2,7 +2,7 @@
 dispatches: the fp32 kernels, the tensor cores in 3xTF32 and TF32, with or without BN, banks, relu6, sigmoid, pooling,
 pixel shuffle, the input block and the pressure skip.
 
-The network is tests/bn_oracle.network, run on (value, bound) pairs by `Bound`, whose operations mirror F64's; `E` is a
+The network is oracle.model.network, run on (value, bound) pairs by `Bound`, whose operations mirror F64's; `E` is a
 float64 array beside each float64 activation with |gpu - value| <= E at every voxel.  u = 2^-24 (float32),
 gamma_n = n u / (1 - n u), S(m) = conv(m, |w|) + |b| with m >= |gpu input| (|x| + E), taken with the layer's dilation.
 
@@ -61,15 +61,14 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
-import bn_oracle
-from bn_oracle import network
+from oracle import model as om
+from oracle.model import DEFAULT_CHANNELS, model_inputs, network
 
 U32 = 2.0 ** -24
 U64 = 2.0 ** -53
 SIGMOID_ULPS = 2.0 ** -20
 KAPPA = {"tf32x3": 2.0 ** -16, "tf32": 2.0 ** -8}
 TAIL_ULPS = 2.0 ** -20
-DEFAULT_CHANNELS = {"pDiv": True, "UDiv": False, "div": True, "flags": True}
 
 
 def gamma(n):
@@ -77,7 +76,7 @@ def gamma(n):
 
 
 def conv_f64(x, w, b=None, d=1):
-    """bn_oracle.conv64 (zero padding d (k - 1) / 2, dilation d) through torch's conv3d in z chunks, float64."""
+    """oracle.model.conv64 (zero padding d (k - 1) / 2, dilation d) through torch's conv3d in z chunks, float64."""
     kz, k = w.shape[2], w.shape[4]
     pz, p = d * (kz - 1) // 2, d * (k - 1) // 2
     xt = F.pad(torch.from_numpy(np.ascontiguousarray(x, np.float64)), (0, 0, 0, 0, pz, pz))
@@ -102,7 +101,7 @@ def tc_covered(model):
 
 
 class Bound:
-    """bn_oracle.F64's operations on (value, E) pairs for one arithmetic path: mode 'fp32', 'tf32x3' or 'tf32'."""
+    """oracle.model.F64's operations on (value, E) pairs for one arithmetic path: mode 'fp32', 'tf32x3' or 'tf32'."""
 
     def __init__(self, model, mode):
         assert mode == "fp32" or tc_covered(model), "the tensor cores do not run this graph"
@@ -118,7 +117,7 @@ class Bound:
             return gamma(w[0].size + 1)
         return KAPPA[self.mode] if w.shape[-1] == 3 else max(TAIL_ULPS, gamma(w[0].size + 1))
 
-    def conv(self, x, w, b, is3d, d, li):
+    def conv(self, x, w, b, is3d, d, li, relu):
         v, E = x
         wa = np.abs(w)
         kappa = self.kappa(li, w)
@@ -126,16 +125,17 @@ class Bound:
         if self._fold_mag is not None:                       # a BN folded into these weights
             m, kappa = self._fold_mag, kappa + 2 * U32
             self._fold_mag = None
-        return conv_f64(v, w, b, d), kappa * conv_f64(m, wa, np.abs(b), d) + conv_f64(E, wa, None, d)
+        y = conv_f64(v, w, b, d), kappa * conv_f64(m, wa, np.abs(b), d) + conv_f64(E, wa, None, d)
+        return self.nonlin(y, "relu") if relu else y
 
     @staticmethod
     def shuffle(x, s, is3d):
-        return tuple(bn_oracle._shuffle(a, s, is3d) for a in x)
+        return tuple(om.shuffle(a, s, is3d) for a in x)
 
     @staticmethod
     def nonlin(x, kind):
         v, E = x
-        y = bn_oracle.nonlin(v, kind)
+        y = om.nonlin(v, kind)
         if kind == "sigmoid":
             return y, E / 4 + SIGMOID_ULPS * y
         lo = np.clip(v + E, 0.0, E)                          # v + E <= 0: both clamp to exactly 0
@@ -145,13 +145,13 @@ class Bound:
     def pool(x, q, is3d, kind):
         v, E = x
         if kind == "max":
-            return bn_oracle._pool(v, q, is3d, "max"), bn_oracle._pool(E, q, is3d, "max")
-        m = bn_oracle._pool(np.abs(v) + E, q, is3d, "avg")
-        return bn_oracle._pool(v, q, is3d, "avg"), bn_oracle._pool(E, q, is3d, "avg") + gamma(q ** (3 if is3d else 2)) * m
+            return om.pool(v, q, is3d, "max"), om.pool(E, q, is3d, "max")
+        m = om.pool(np.abs(v) + E, q, is3d, "avg")
+        return om.pool(v, q, is3d, "avg"), om.pool(E, q, is3d, "avg") + gamma(q ** (3 if is3d else 2)) * m
 
     @staticmethod
     def up(x, r, is3d):
-        return tuple(bn_oracle._rep(a, r, is3d) for a in x)
+        return tuple(om.upsample(a, r, is3d) for a in x)
 
     @staticmethod
     def concat(hs):
@@ -170,7 +170,7 @@ class Bound:
         w = np.ones(c_) if e.get("weight") is None else np.asarray(e["weight"], np.float64)
         b = np.zeros(c_) if e.get("bias") is None else np.asarray(e["bias"], np.float64)
         eps = float(np.float32(e["eps"]))
-        y = bn_oracle.batch_norm(v, e, train)
+        y = om.batch_norm(v, e, train)
         if not train:
             a = w / np.sqrt(np.asarray(e["running_var"], np.float64) + eps)
             c = b - np.asarray(e["running_mean"], np.float64) * a
@@ -310,14 +310,6 @@ def finish(be, U1, flags, pn, Epn, is3d, s_lo, s_hi, s_mid):
 # ---------------------------------------------------------------------------------------------------------------
 # The whole forward
 # ---------------------------------------------------------------------------------------------------------------
-def model_inputs(model):
-    """The input-block keywords of a synth.make_model dict, with their defaults."""
-    kw = dict(inputChannels=None, normalizeInput=True, normalizeInputFunc="std", normalizeInputChan="UDiv",
-              addPressureSkip=False)
-    kw.update(model.get("inputs") or {})
-    return kw
-
-
 def scale_intervals(fields, model, threshold=1e-5):
     """Per entry (lo, hi) of the input scale (1 without normalizeInput)."""
     kw = model_inputs(model)
@@ -334,10 +326,10 @@ def p_net_bound(model, x0, E0, mode, pS=None, rho=0.0):
     interval's relative width (pDiv / s_gpu is within rho |pS| of pS)."""
     ops = Bound(model, mode)
     if pS is None:
-        return network(model, (x0, E0), ops=ops)
-    hv, hE = network(model, (x0, E0), hidden=True, ops=ops)
+        return network(model, (x0, E0), ops)
+    hv, hE = network(model, (x0, E0), ops, hidden=True)
     w, b = model["layers"][-1]
-    body_v, body_E = ops.conv((hv, hE), w[:, :-1], b, model["is3D"], 1, len(model["layers"]) - 1)
+    body_v, body_E = ops.conv((hv, hE), w[:, :-1], b, model["is3D"], 1, len(model["layers"]) - 1, False)
     skip = float(w[0, -1].ravel()[0]) * pS
     rho = np.asarray(rho, np.float64).reshape(-1, 1, 1, 1, 1)
     return body_v + skip, body_E + gamma(3) * (np.abs(body_v) + body_E + np.abs(skip)) + rho * np.abs(skip)

@@ -14,7 +14,7 @@ Three steps per case, each re-seeded from the GPU's state (as tests/test_gpu_ste
       scale interval (projection_reference of tests/test_gpu_cnn_network_f64.py, batches included); the largest
       err / E of each case is printed;
   (2) the operator sequence (simulate.simulate): density bit for bit, U and p within OPS_TOL with the same zero bits;
-  (3) oracle.simulate with the restated network (bn_oracle): density bit for bit, U and p within MODE_TOL (TF32 with
+  (3) oracle.simulate with the network in float64: density bit for bit, U and p within MODE_TOL (TF32 with
       batch statistics: 1e-2, oracle_tol);
   (4) entries: for every model without batch statistics each entry equals its scene stepped alone (OPS_TOL, zero
       bits); with batch statistics changing entry 1 changes entry 0's p (and (2) holds for the coupled batch);
@@ -37,7 +37,6 @@ import torch
 
 import monitor_reference
 import oracle
-from bn_oracle import model_forward_of_model
 from cases import bits_equal, describe_diff
 from fluidnet_b200 import synth
 from network_bound import check, tc_covered
@@ -175,9 +174,8 @@ def make_model(mnp, mode):
 # ---------------------------------------------------------------------------------------------------------------
 @pytest.mark.gpu
 @pytest.mark.parametrize("scene,mode", CASES, ids=CASE_IDS)
-def test_batched_fused_step(orc, monkeypatch, scene, mode):
+def test_batched_fused_step(orc, scene, mode):
     from fluidnet_b200 import simulate, tfluids
-    monkeypatch.setattr(oracle.api, "model_forward", model_forward_of_model)
     model, shape, kinds, amps = SCENES[scene]
     nb = len(kinds)
     mnp = MODELS[model]()
@@ -191,7 +189,7 @@ def test_batched_fused_step(orc, monkeypatch, scene, mode):
         state = {k: v.clone() for k, v in fused.items()}
         ops = {k: v.clone() for k, v in fused.items()}
         bound = projection_reference(state, MCONF, gm, mnp)
-        oracle.simulate(orc, MCONF, ref, mnp)
+        oracle.simulate(orc, MCONF, ref, mnp, f64=True)
         simulate.simulate_fused(None, MCONF, fused, gm)
         simulate.simulate(None, MCONF, ops, gm)
         got, opg = host(fused), host(ops)

@@ -1,5 +1,5 @@
 """Multi-resolution banks of the projection network (lib/model.lua:252-361) on the GPU: model:forward against the
-CPU restatement (tests/bank_oracle.py, pinned on torch.nn.functional by tests/test_oracle_model_banks.py), the
+CPU restatement (oracle.model_forward, pinned on torch.nn.functional by tests/test_oracle_model_banks.py), the
 whole step, CUDA-graph replay, model reuse across grids, and the argument errors.
 
 The 3-D 'default' graph with banks split at stage 1 and joined at stage 3 also runs on the tensor cores (3xTF32 by
@@ -13,7 +13,6 @@ import pytest
 import torch
 
 import oracle
-from bank_oracle import model_forward_banked
 from fluidnet_b200 import synth
 from fluidnet_b200 import model as fmodel
 from fluidnet_b200._lib import TflError
@@ -88,7 +87,7 @@ def test_banked_forward(case, mode):
     batch = make_batch(shape, is3d, nb=nb)
     mnp = synth.make_model(is3d, model_type=model_type, banks=bk)
     p0, inp = inputs_of(batch)
-    wp, wU, wscale = model_forward_banked(orc, mnp, p0, batch["UDiv"], batch["flags"])
+    wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
     gm = make_gpu(mnp)
     assert gm.get_mode() == ("tf32x3" if covered else "fp32")
     if mode != "default":
@@ -136,11 +135,10 @@ def test_banked_model_across_shapes_and_modes(agg):
 
 
 @pytest.mark.parametrize("bk", [banks(2, "concat"), banks(3, "add")], ids=["n2-concat", "n3-add"])
-def test_banked_step(bk, monkeypatch):
+def test_banked_step(bk):
     """tfl_simulate_step with a banked model equals the operator sequence (1e-6) and oracle.simulate with the
     banked graph (2e-5, first step)."""
     from fluidnet_b200 import simulate
-    monkeypatch.setattr(oracle.api, "model_forward", model_forward_banked)
     orc = oracle.Oracle()
     n = 24
     batch = make_batch((n, n, n), True, plume=True)
@@ -253,7 +251,7 @@ def test_banked_reference_file_end_to_end(tmp_path, agg):
     assert mconf["banksNum"] == 2 and gm.banks == banks(2, agg) and gm.get_mode() == "tf32x3"
     batch = make_batch((8, 12, 16), True, nb=1)
     p0, inp = inputs_of(batch)
-    wp, wU, _ = model_forward_banked(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"])
+    wp, wU, _ = oracle.model_forward(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"])
     gp, gU = gm.forward(inp)
     close(gp.cpu().numpy(), wp, 2e-5, "p")
     close(gU.cpu().numpy(), wU, 2e-5, "U")

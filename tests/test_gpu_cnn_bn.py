@@ -17,8 +17,8 @@ banked), with batch statistics (modules saved with train = true) and running sta
     sums are what keeps a channel with |mean| / std ~ 1e3 within these bounds; float32 sums of x^2 would lose var.
     A second call gives the same bits; a dead channel with eps = 0 gives exactly b; nothing outside the nb c n values
     (the gaps of a batch stride) is written.
-  * model:forward against tests/bn_oracle.py (pinned on torch.nn.functional by tests/test_oracle_model_bn.py) within
-    2e-5 of each entry's max (fp32, 3xTF32; 3e-3 TF32), on every graph, in both BN modes, nb = 1 and 2, relu6 with
+  * model:forward against oracle.model_forward(f64=True) (pinned on torch.nn.functional by
+    tests/test_oracle_model_bn.py) within 2e-5 of each entry's max (fp32, 3xTF32; 3e-3 TF32), on every graph, in both BN modes, nb = 1 and 2, relu6 with
     values past 6.  With batch
     statistics changing entry 1 changes entry 0; with running statistics it does not, bit for bit.  Running statistics
     with w = 1, b = 0, mean 0, var 1 - eps equal the model without BN.
@@ -33,7 +33,6 @@ import pytest
 import torch
 
 import oracle
-from bn_oracle import model_forward_bn, model_forward_of_model
 from fluidnet_b200 import synth
 from fluidnet_b200 import model as fmodel
 from fluidnet_b200._lib import TflError
@@ -174,7 +173,7 @@ def test_bn_forward(case, variant, nb, mode):
     mnp = bn_model(is3d, model_type, bk, inputs, variant.startswith("batch"), relu6, "noaffine" not in variant)
     batch = make_batch(shape, is3d, nb=nb)
     p0, inp = inputs_of(batch)
-    wp, wU, wscale = model_forward_bn(orc, mnp, p0, batch["UDiv"], batch["flags"], **(inputs or {}))
+    wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"], f64=True)
     gm = make_gpu(mnp)
     assert gm.get_mode() == ("tf32x3" if covered else "fp32")
     if mode != "default":
@@ -197,7 +196,7 @@ def test_relu6_banked_on_tensor_cores(bk, mode):
     mnp["layers"][0][0][0][...] *= np.float32(30.0)
     batch = make_batch((8, 12, 16), True, nb=2)
     p0, inp = inputs_of(batch)
-    wp, wU, _ = model_forward_bn(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"])
+    wp, wU, _ = oracle.model_forward(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"], f64=True)
     gm = make_gpu(mnp)
     assert gm.get_mode() == "tf32x3"
     gm.set_mode(mode)
@@ -318,9 +317,8 @@ def step_mconf(n):
 
 
 @pytest.mark.parametrize("train", [True, False], ids=["batch", "running"])
-def test_bn_step(train, monkeypatch, contexts):
+def test_bn_step(train, contexts):
     from fluidnet_b200 import simulate
-    monkeypatch.setattr(oracle.api, "model_forward", model_forward_of_model)
     orc = oracle.Oracle()
     n = 20
     batch = make_batch((n, n, n), True, plume=True)
@@ -336,7 +334,7 @@ def test_bn_step(train, monkeypatch, contexts):
     g = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
     simulate.simulate(None, mconf, a, gm)
     simulate.simulate_fused(None, mconf, b, gm)
-    oracle.simulate(orc, mconf, batch, mnp)
+    oracle.simulate(orc, mconf, batch, mnp, f64=True)
     for k in ("density", "UDiv", "pDiv"):
         close(b[k].cpu().numpy(), a[k].cpu().numpy(), 1e-6, "step vs ops " + k)
         close(b[k].cpu().numpy(), batch[k], 2e-5, "step vs oracle " + k)
@@ -447,7 +445,7 @@ def test_bn_reference_file_end_to_end(tmp_path, train):
     assert mconf["addBatchNorm"] and gm.get_mode() == "fp32"          # banked: the fp32 path
     batch = make_batch((8, 12, 16), True, nb=2)
     p0, inp = inputs_of(batch)
-    wp, wU, _ = model_forward_bn(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"])
+    wp, wU, _ = oracle.model_forward(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"], f64=True)
     gp, gU = gm.forward(inp)
     close(gp.cpu().numpy(), wp, 2e-5, "p")
     close(gU.cpu().numpy(), wU, 2e-5, "U")

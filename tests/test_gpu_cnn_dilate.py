@@ -11,7 +11,7 @@ phase sub-grids.
     conv2d(dilation=d) in float64: per value within gamma_n S (the bound of tests/test_gpu_conv_fp32.py, whose
     argument does not depend on where the taps sit), exactly on the 2^-k 'exact' inputs, the generic kernel equal to
     the direct one bit for bit, nothing written outside the output.
-  * model:forward against the CPU restatement (tests/dilate_oracle.py, pinned on torch.nn.functional by
+  * model:forward against the CPU restatement (oracle.model_forward, pinned on torch.nn.functional by
     tests/test_oracle_model_dilate.py) within 2e-5 of each entry's max, on every graph; N = 1 'dilate' equals the
     single-bank model bit for bit; batch entries equal their own forward bit for bit.
   * The step against the operator sequence (1e-6) and oracle.simulate with the restated network (2e-5), step-graph
@@ -25,10 +25,10 @@ import torch
 import torch.nn.functional as F
 
 import oracle
-from dilate_oracle import model_forward_dilated
 from fluidnet_b200 import synth
 from fluidnet_b200 import model as fmodel
 from fluidnet_b200._lib import TflError
+from network_bound import conv_f64
 from test_gpu_cnn_banks import close, inputs_of, make_batch, write_mconf
 from test_gpu_step_paths import contexts  # noqa: F401  (fixture: library contexts of one test)
 from test_gpu_conv_fp32 import (DIRECT, GENERIC, SIGMOID_ULPS, activate, check_guards, gamma, guarded, make_conv,
@@ -50,14 +50,6 @@ def make_gpu(mnp, threshold=1e-5):
 # ---------------------------------------------------------------------------------------------------------------
 # One dilated convolution
 # ---------------------------------------------------------------------------------------------------------------
-def conv_f64(x, w, b, d):
-    kz, k = w.shape[2], w.shape[4]
-    pad = (d * (kz - 1) // 2, d * (k - 1) // 2, d * (k - 1) // 2)
-    dil = (d if kz > 1 else 1, d, d)
-    return F.conv3d(torch.from_numpy(x).double(), torch.from_numpy(w).double(), torch.from_numpy(b).double(),
-                    padding=pad, dilation=dil).numpy()
-
-
 def run_conv(x, w, b, act, is3d, generic, d, what):
     from fluidnet_b200 import tfluids
     lib = tfluids.context().lib
@@ -161,7 +153,7 @@ def test_dilated_forward(case, mode):
     batch = make_batch(shape, is3d, nb=nb)
     mnp = synth.make_model(is3d, model_type=model_type, banks=bk)
     p0, inp = inputs_of(batch)
-    wp, wU, wscale = model_forward_dilated(orc, mnp, p0, batch["UDiv"], batch["flags"])
+    wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
     gm = make_gpu(mnp)
     assert gm.get_mode() == ("tf32x3" if covered else "fp32")
     if mode != "default":
@@ -272,9 +264,8 @@ def step_mconf(n):
 
 
 @pytest.mark.parametrize("bk", [dilate(2, "concat"), dilate(3, "add")], ids=["n2-concat", "n3-add"])
-def test_dilated_step(bk, monkeypatch):
+def test_dilated_step(bk):
     from fluidnet_b200 import simulate
-    monkeypatch.setattr(oracle.api, "model_forward", model_forward_dilated)
     orc = oracle.Oracle()
     n = 20
     batch = make_batch((n, n, n), True, plume=True)
@@ -394,7 +385,7 @@ def test_dilated_reference_file_end_to_end(tmp_path, agg):
     assert mconf["banksType"] == "dilate" and gm.banks == dilate(3, agg) and gm.get_mode() == "tf32x3"
     batch = make_batch((8, 12, 16), True, nb=1)
     p0, inp = inputs_of(batch)
-    wp, wU, _ = model_forward_dilated(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"])
+    wp, wU, _ = oracle.model_forward(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"])
     gp, gU = gm.forward(inp)
     close(gp.cpu().numpy(), wp, 2e-5, "p")
     close(gU.cpu().numpy(), wU, 2e-5, "U")

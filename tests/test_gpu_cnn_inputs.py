@@ -1,6 +1,6 @@
 """The input block of the projection network (lib/model.lua:27-150, :357-387: inputChannels, normalizeInput,
 normalizeInputFunc, normalizeInputChan, addPressureSkip) on the GPU: model:forward against the CPU restatement
-(tests/inputs_oracle.py, pinned on torch.nn.functional by tests/test_oracle_model_inputs.py), the returned scale,
+(oracle.model_forward, pinned on torch.nn.functional by tests/test_oracle_model_inputs.py), the returned scale,
 the default block built by every creator bit for bit, layer 1 and the bank pyramid on the two-plane
 tensor-core input, the step and its graph, and the z-slab refusal.
 
@@ -15,7 +15,7 @@ import torch
 import oracle
 from fluidnet_b200 import model as fmodel
 from fluidnet_b200 import synth
-from inputs_oracle import model_forward_inputs, model_forward_of_model, model_input
+from oracle.model import model_input
 from test_gpu_cnn_banks import banks, close, inputs_of, make_batch
 from test_gpu_conv_tc import SENTINEL, check_layer, is_sentinel, layout, make_layer, pack, unpack
 from test_gpu_slab_banks import _problem, _refused
@@ -33,10 +33,6 @@ def make_gpu(mnp):
     return fmodel.ProjectionModel(mnp["layers"], mnp["is3D"], pool=mnp.get("pool"), up=mnp.get("up"),
                                   poolType=mnp.get("poolType", "avg"), nonlinType=mnp.get("nonlinType", "relu"),
                                   banks=mnp.get("banks"), **(mnp.get("inputs") or {}))
-
-
-def forward_ref(orc, mnp, p0, U, flags, threshold=1e-5):
-    return model_forward_inputs(orc, mnp, p0, U, flags, threshold, **(mnp.get("inputs") or {}))
 
 
 def ins(ch=None, **kw):
@@ -81,7 +77,7 @@ def run_forward(case, mode):
     batch = make_batch(shape, is3d, nb=nb)
     mnp = synth.make_model(is3d, model_type=model_type, banks=bk, inputs=inputs)
     p0, inp = inputs_of(batch)
-    wp, wU, wscale = forward_ref(orc, mnp, p0, batch["UDiv"], batch["flags"])
+    wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
     gm = make_gpu(mnp)
     if mode != "default":
         gm.set_mode(mode)
@@ -119,7 +115,7 @@ def test_scale(func, chan):
     inputs = ins(ALL, normalizeInputFunc=func, normalizeInputChan=chan or "UDiv", normalizeInput=chan is not None)
     mnp = synth.make_model(True, inputs=inputs)
     p0, inp = inputs_of(batch)
-    _, _, want = forward_ref(orc, mnp, p0, batch["UDiv"], batch["flags"])
+    _, _, want = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
     for mode in ("tf32x3", "fp32"):
         gm = make_gpu(mnp)
         gm.set_mode(mode)
@@ -218,7 +214,7 @@ def test_padded_input_is_the_oracle_input(ch):
     nb, shape = 2, (6, 9, 13)
     batch = make_batch(shape, True, nb=nb)
     p0, _ = inputs_of(batch)
-    x, _, _, _, scales = model_input(orc, p0, batch["UDiv"], batch["flags"], inputChannels=ch)
+    x, _, _, _, scales = model_input(orc, {"inputs": ins(ch)}, p0, batch["UDiv"], batch["flags"])
     U1 = batch["UDiv"].copy()
     orc.setWallBcsForward(U1, batch["flags"], as_mask_multiply=True)
     gm = make_gpu(synth.make_model(True, inputs=ins(ch)))
@@ -271,11 +267,10 @@ def test_two_plane_pyramid_on_a_plane_range(phase):
     assert np.array_equal(got.view(np.uint32), want.view(np.uint32))
 
 
-def test_step_and_its_graph(monkeypatch):
+def test_step_and_its_graph():
     """One tfl_simulate_step with a UDiv + skip model (the per-operator path) against oracle.simulate, and the step
     graph replaying it bit for bit."""
     from fluidnet_b200 import simulate
-    monkeypatch.setattr(oracle.api, "model_forward", model_forward_of_model)
     orc = oracle.Oracle()
     n = 24
     batch = make_batch((n, n, n), True, plume=True)

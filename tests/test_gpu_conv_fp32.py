@@ -54,6 +54,8 @@ import pytest
 import torch
 import torch.nn.functional as F
 
+from network_bound import conv_f64
+
 U_ROUND = 2.0 ** -24
 SIGMOID_ULPS = 2.0 ** -20
 SENTINEL = 0x7FC0BEEF                 # a NaN payload that no kernel produces from finite inputs
@@ -86,12 +88,6 @@ def make_conv(inputs, cin, cout, k, is3d, shape, nb, seed):
         w = rs.uniform(lo * bw, bw, ws)
         b = rs.uniform(lo * bw, bw, cout)
     return tuple(np.ascontiguousarray(a, np.float32) for a in (x, w, b))
-
-
-def conv_f64(x, w, b):
-    kz, k = w.shape[2], w.shape[4]
-    return F.conv3d(torch.from_numpy(x).double(), torch.from_numpy(w).double(), torch.from_numpy(b).double(),
-                    padding=((kz - 1) // 2, (k - 1) // 2, (k - 1) // 2)).numpy()
 
 
 def activate(v, act):

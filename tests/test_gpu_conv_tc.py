@@ -44,7 +44,8 @@ import zlib
 import numpy as np
 import pytest
 import torch
-import torch.nn.functional as F
+
+from network_bound import conv_f64
 
 KAPPA = {1: 2.0 ** -16, 0: 2.0 ** -8}            # split -> per-voxel bound factor
 TAIL_ULPS = 2.0 ** -20                            # fp32 rounding of the 1x1x1 tail, relative
@@ -78,20 +79,10 @@ def make_layer(inputs, cin, final, shape, nb, seed):
     return f32(x), f32(w), f32(b), f32(tail)
 
 
-def conv3d_f64(x, w, b):
-    """conv3d(x, w) + b in float64 (padding 1), in z chunks so that the CPU's im2col buffer stays small."""
-    xt = F.pad(torch.from_numpy(x).double(), (0, 0, 0, 0, 1, 1))
-    wt, bt = torch.from_numpy(w).double(), torch.from_numpy(b).double()
-    nz, ny, nx = x.shape[2:]
-    step = max(1, (1 << 24) // (ny * nx * w.shape[1] * 27))
-    out = [F.conv3d(xt[:, :, z0:min(nz, z0 + step) + 2], wt, bt, padding=(0, 1, 1)) for z0 in range(0, nz, step)]
-    return torch.cat(out, dim=2).numpy()
-
-
 def reference(x, w, b, tail, kappa):
     """(ref, bound): the float64 result of the layer and the per-voxel error bound (module docstring)."""
-    pre = conv3d_f64(x, w, b)
-    S = conv3d_f64(np.abs(x), np.abs(w), np.abs(b))
+    pre = conv_f64(x, w, b)
+    S = conv_f64(np.abs(x), np.abs(w), np.abs(b))
     h, Eh = np.maximum(pre, 0.0), kappa * S
     if tail is None:
         return h, Eh
@@ -259,12 +250,12 @@ def emulate(x, w, b, split, drop_lo_hi=False):
     """The kernel's operand rounding in float64 (exact accumulation): TF32 truncates both operands; 3xTF32
     sums hi*hi + hi*lo + lo*hi with the fp32 residual lo truncated to tf32 again."""
     if not split:
-        return conv3d_f64(tf32(x), tf32(w), b)
+        return conv_f64(tf32(x), tf32(w), b)
     xh, wh = tf32(x), tf32(w)
     xl, wl = tf32(x - xh), tf32(w - wh)
     zero = np.zeros_like(b)
-    y = conv3d_f64(xh, wh, b) + conv3d_f64(xh, wl, zero)
-    return y if drop_lo_hi else y + conv3d_f64(xl, wh, zero)
+    y = conv_f64(xh, wh, b) + conv_f64(xh, wl, zero)
+    return y if drop_lo_hi else y + conv_f64(xl, wh, zero)
 
 
 @pytest.mark.parametrize("inputs", INPUTS)
@@ -274,8 +265,8 @@ def test_error_model_emulation(inputs):
     non-negative data (as does single-pass TF32 against the 3xTF32 kappa)."""
     for cin in (3, 8):
         x, w, b, _ = make_layer(inputs, cin, 0, (7, 9, 31), 2, 3)
-        ref = conv3d_f64(x, w, b)
-        S = conv3d_f64(np.abs(x), np.abs(w), np.abs(b))
+        ref = conv_f64(x, w, b)
+        S = conv_f64(np.abs(x), np.abs(w), np.abs(b))
         for split in (0, 1):
             r = (np.abs(emulate(x, w, b, split) - ref) / S).max()
             assert r <= KAPPA[split], (cin, split, r)

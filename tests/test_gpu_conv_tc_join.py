@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_conv_tc import KAPPA, SENTINEL, TAIL_ULPS, conv3d_f64, is_sentinel, layout, pack
+from test_gpu_conv_tc import KAPPA, SENTINEL, TAIL_ULPS, conv_f64, is_sentinel, layout, pack
 
 pytestmark = pytest.mark.gpu
 
@@ -36,8 +36,8 @@ def reference(banks, agg, w, b, tail, kappa):
         x, xa = np.concatenate(ups, axis=1), np.abs(np.concatenate(ups, axis=1))
     else:
         x, xa = sum(ups[1:], ups[0]), sum((np.abs(u) for u in ups[1:]), np.abs(ups[0]))
-    pre = conv3d_f64(x, w, b)
-    S = conv3d_f64(xa, np.abs(w), np.abs(b))
+    pre = conv_f64(x, w, b)
+    S = conv_f64(xa, np.abs(w), np.abs(b))
     h, Eh = np.maximum(pre, 0.0), kappa * S
     t = tail.astype(np.float64)
     w4, b4, w5, b5 = t[:64].reshape(8, 8), t[64:72], t[72:80], t[80]

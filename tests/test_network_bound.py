@@ -2,7 +2,7 @@
 arithmetic, it fails for that emulation with one fault injected, and the batch-statistics BN rule holds for perturbed
 float64 inputs.
 
-`F32` is bn_oracle.F64's set of operations in float32 the way the fp32 kernels compute them: a convolution starts from
+`F32` is oracle.model.F64's set of operations in float32 the way the fp32 kernels compute them: a convolution starts from
 the bias and adds one fmaf per term in the order (c, dz, dy, dx) (one rounding per term: the float32 product is exact
 in float64), average pooling sums in order and divides, BN rounds a and c once and applies a fused multiply-add, a
 bank join 'add' sums in bank order.  The input block divides by the float32 scale, and the finish is the oracle's
@@ -22,7 +22,7 @@ import numpy as np
 import pytest
 
 import oracle
-from bn_oracle import F64, network
+from oracle.model import F64, batch_norm, network
 from fluidnet_b200 import synth
 from network_bound import (Bound, check, excess, forward_bound, input_fields, model_inputs, scale_intervals)
 
@@ -54,7 +54,7 @@ class F32:
 
     lift = staticmethod(lambda x: np.asarray(x, np.float32))
 
-    def conv(self, x, w, b, is3d, d, li):
+    def conv(self, x, w, b, is3d, d, li, relu):
         x, w, b = np.asarray(x, np.float32), np.asarray(w, np.float32), np.asarray(b, np.float32).copy()
         if self.fault == "plane" and li == 1:
             x = x.copy()
@@ -79,7 +79,7 @@ class F32:
                     for tx in range(k):
                         sl = xp[:, c, tz * d:tz * d + Z, ty * d:ty * d + Y, tx * d:tx * d + X].astype(np.float64)
                         acc = (acc + w64[:, c, tz, ty, tx][None, :, None, None, None] * sl[:, None]).astype(np.float32)
-        return acc
+        return self.nonlin(acc, "relu") if relu else acc
 
     shuffle = staticmethod(F64.shuffle)
 
@@ -151,12 +151,12 @@ def emulate(be, model, pDiv, UDiv, flags, fault=None):
     ops = F32(fault)
     if kw["addPressureSkip"]:
         w, b = model["layers"][-1]
-        h = network(model, x0, hidden=True, ops=ops)
-        body = ops.conv(h, w[:, :-1], b, model["is3D"], 1, len(model["layers"]) - 1)
+        h = network(model, x0, ops, hidden=True)
+        body = ops.conv(h, w[:, :-1], b, model["is3D"], 1, len(model["layers"]) - 1, False)
         pS = (fields["pDiv"] / sc).astype(np.float32)
         pn = (body + (np.float32(w[0, -1].ravel()[0]) * pS).astype(np.float32)).astype(np.float32)
     else:
-        pn = network(model, x0, ops=ops)
+        pn = network(model, x0, ops)
     U = np.ascontiguousarray((fields["U1"] / sc).astype(np.float32))
     be.velocityUpdateForward(U, flags, pn)
     U = np.ascontiguousarray((U * sc).astype(np.float32))
@@ -258,7 +258,6 @@ def test_tf32_operands_stay_within_their_own_bound(orc):
 def test_batch_statistics_rule(seed):
     """h' = h + r E with r in [-1, 1] (random, and at the signs +-1): BN with batch statistics of h' stays within
     the rule's bound of BN of h, in float64 (the float rounding terms only widen it)."""
-    import bn_oracle
     rs = np.random.RandomState(seed)
     c = 4
     h = rs.randn(2, c, 5, 6, 7) * np.array([1.0, 1e-2, 5.0, 1.0]).reshape(1, c, 1, 1, 1)
@@ -267,10 +266,10 @@ def test_batch_statistics_rule(seed):
     e = {"weight": (0.5 + rs.rand(c)).astype(np.float32), "bias": (rs.rand(c) - 0.5).astype(np.float32),
          "running_mean": np.zeros(c, np.float32), "running_var": np.ones(c, np.float32), "eps": 1e-4}
     y, Ey = Bound(synth.make_model(True), "fp32").bn((h, E), e, True, 0)
-    assert np.allclose(y, bn_oracle.batch_norm(h, e, True), rtol=0, atol=0)
+    assert np.allclose(y, batch_norm(h, e, True), rtol=0, atol=0)
     worst = 0.0
     for r in (rs.uniform(-1, 1, h.shape), np.sign(rs.randn(*h.shape)), np.ones(h.shape), -np.ones(h.shape)):
-        y2 = bn_oracle.batch_norm(h + r * E, e, True)
+        y2 = batch_norm(h + r * E, e, True)
         worst = max(worst, check("BN batch r", y2, y, Ey))
     print("batch-statistics BN: max err/E %.3f" % worst)
 

@@ -1,4 +1,4 @@
-"""The CPU restatement of the multi-resolution bank graph (tests/bank_oracle.py, lib/model.lua:252-361) against an
+"""The CPU restatement of the multi-resolution bank graph (oracle/model.py, lib/model.lua:252-361) against an
 independent float64 evaluation with torch.nn.functional: avg_pool for the pyramid, interpolate(mode='nearest') for
 the join's upsampling, cat / + for the aggregation.  The GPU path is then compared with the restatement."""
 import numpy as np
@@ -7,7 +7,6 @@ import torch
 import torch.nn.functional as F
 
 import oracle
-from bank_oracle import model_forward_banked
 from fluidnet_b200 import synth
 
 
@@ -88,7 +87,7 @@ def test_banked_graph_matches_torch(case):
     model = synth.make_model(is3d, model_type=model_type,
                              banks={"num": num, "split_stage": s, "join_stage": j, "aggregate": agg})
     p0 = (synth.make_density(flags, seed=5) - np.float32(0.5)) * np.float32(0.1)
-    p, U2, scale = model_forward_banked(orc, model, p0, U, flags)
+    p, U2, scale = oracle.model_forward(orc, model, p0, U, flags)
     U1 = U.copy()
     orc.setWallBcsForward(U1, flags, as_mask_multiply=True)
     sc = scale.reshape(-1, 1, 1, 1, 1)
@@ -100,7 +99,7 @@ def test_banked_graph_matches_torch(case):
 
 
 def test_single_bank_is_the_plain_graph():
-    """num = 1 draws the same weights as no banks, and the restatement then equals oracle.model_forward."""
+    """num = 1 draws the same weights as no banks, and the 1-bank graph then computes the plain graph's bits."""
     orc = oracle.Oracle()
     flags = synth.make_flags(8, 8, 8, True, nb=1, geometry=False)
     U = synth.make_smooth_velocity(flags, True, amp=1.0)
@@ -111,6 +110,6 @@ def test_single_bank_is_the_plain_graph():
         assert np.array_equal(w0, w1) and np.array_equal(b0, b1)
     p0 = np.zeros_like(flags)
     a = oracle.model_forward(orc, plain, p0, U, flags)
-    b = model_forward_banked(orc, one, p0, U, flags)
+    b = oracle.model_forward(orc, one, p0, U, flags)
     for u, v in zip(a, b):
         assert np.array_equal(u, v)

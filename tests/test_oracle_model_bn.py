@@ -1,4 +1,4 @@
-"""The CPU restatement of batch normalization and relu6 (tests/bn_oracle.py, lib/model.lua:316-350,
+"""The CPU restatement of batch normalization and relu6 (oracle/model.py, lib/model.lua:316-350,
 lib/model_utils.lua:20-62) against an independent float64 evaluation with torch.nn.functional: conv{2,3}d (dilated for
 'dilate' banks), the pixel shuffle, hardtanh(0, 6) / relu / sigmoid, avg / max pooling, batch_norm(training=True)
 for modules saved with train = true and batch_norm(training=False) with the running statistics otherwise, avg_pool
@@ -9,8 +9,7 @@ import torch
 import torch.nn.functional as F
 
 import oracle
-from bn_oracle import batch_norm, model_forward_bn, network
-from inputs_oracle import model_forward_inputs, model_input
+from oracle.model import F64, batch_norm, conv64, model_input, network
 from fluidnet_b200 import synth
 
 
@@ -132,7 +131,7 @@ def test_bn_network_matches_torch(graph, variant):
     relu6 = "relu6" in variant and model_type != "yang"
     model = bn_model(is3d, model_type, bk, train, affine="noaffine" not in variant, relu6=relu6)
     x = network_input(2, shape, is3d, 17)
-    got = network(model, x)
+    got = network(model, x, F64)
     want = torch_network(x, model)
     assert got.shape == (2, 1) + shape
     assert np.abs(got - want).max() <= 1e-10 * max(np.abs(want).max(), 1.0)
@@ -143,7 +142,6 @@ def test_relu6_clamps_in_the_restatement():
     exercises it)."""
     model = bn_model(True, "default", None, True, relu6=True)
     x = network_input(1, (6, 7, 9), True, 3)
-    from bn_oracle import conv64
     w, b = model["layers"][0]
     pre = conv64(x.astype(np.float64), w, b, True)
     assert pre.max() > 6.0 and pre.min() < 0.0
@@ -166,8 +164,8 @@ def test_batch_norm_dead_channel_and_train_coupling():
 
 @pytest.mark.parametrize("skip", [False, True])
 def test_identity_bn_is_the_model_without_bn(skip):
-    """Running statistics with w = 1, b = 0, mean 0, var 1 - eps is the identity: model_forward_bn then equals the
-    input-block restatement (float32 convolutions) to float32 rounding, with and without the pressure skip."""
+    """Running statistics with w = 1, b = 0, mean 0, var 1 - eps is the identity: the float64 forward then equals the
+    float32 forward of the model without BN to float32 rounding, with and without the pressure skip."""
     orc = oracle.Oracle()
     inputs = {"addPressureSkip": True} if skip else None
     model = synth.make_model(True, inputs=inputs, batch_norm={"train": False})
@@ -178,9 +176,8 @@ def test_identity_bn_is_the_model_without_bn(skip):
     U = synth.make_smooth_velocity(flags, True, amp=1.0)
     orc.setWallBcsForward(U, flags)
     p0 = (synth.make_density(flags, seed=5) - np.float32(0.5)) * np.float32(0.1)
-    kw = model.get("inputs") or {}
-    a = model_forward_bn(orc, model, p0, U, flags, **kw)
-    b = model_forward_inputs(orc, dict(model, batchNorm=None), p0, U, flags, **kw)
+    a = oracle.model_forward(orc, model, p0, U, flags, f64=True)
+    b = oracle.model_forward(orc, dict(model, batchNorm=None), p0, U, flags)
     for u, v in zip(a, b):
         assert np.abs(u - v).max() <= 1e-5 * max(np.abs(v).max(), 1e-3)
 
@@ -193,9 +190,9 @@ def test_pressure_skip_with_bn_matches_torch():
     U = synth.make_smooth_velocity(flags, True, amp=1.0)
     orc.setWallBcsForward(U, flags)
     p0 = (synth.make_density(flags, seed=5) - np.float32(0.5)) * np.float32(0.1)
-    p, _, scale = model_forward_bn(orc, model, p0, U, flags, addPressureSkip=True)
-    x, pS, _, sc, _ = model_input(orc, p0, U, flags)
-    hidden = torch.from_numpy(network(model, x, hidden=True))
+    p, _, scale = oracle.model_forward(orc, model, p0, U, flags, f64=True)
+    x, pS, _, sc, _ = model_input(orc, model, p0, U, flags)
+    hidden = torch.from_numpy(network(model, x, F64, hidden=True))
     w, b = model["layers"][-1]
     want = F.conv3d(torch.cat([hidden, torch.from_numpy(pS).double()], 1), torch.from_numpy(w).double(),
                     torch.from_numpy(b).double()).numpy() * sc

@@ -1,4 +1,4 @@
-"""The CPU restatement of the dilated-bank graph (tests/dilate_oracle.py, banksType 'dilate', lib/model.lua:252-361)
+"""The CPU restatement of the dilated-bank graph (oracle/model.py, banksType 'dilate', lib/model.lua:252-361)
 against an independent float64 evaluation with torch.nn.functional: conv{2,3}d(dilation=2^(i-1), padding
 2^(i-1) (k-1)/2) for bank i, cat / + for the aggregation, no upsampling.  The GPU path is then compared with the
 restatement.  Grids are chosen not divisible by the dilations, and some have an axis shorter than the largest one."""
@@ -8,7 +8,7 @@ import torch
 import torch.nn.functional as F
 
 import oracle
-from dilate_oracle import conv_dilated, model_forward_dilated
+from oracle.model import Float32Ops
 from fluidnet_b200 import synth
 from test_oracle_model_banks import torch_stage
 
@@ -95,7 +95,7 @@ def test_dilated_graph_matches_torch(case):
     model = synth.make_model(is3d, model_type=model_type, banks=bk)
     assert model["banks"]["type"] == "dilate"
     p0 = (synth.make_density(flags, seed=5) - np.float32(0.5)) * np.float32(0.1)
-    p, U2, scale = model_forward_dilated(orc, model, p0, U, flags)
+    p, U2, scale = oracle.model_forward(orc, model, p0, U, flags)
     x, sc = network_input(orc, model, flags, U, p0, scale)
     want = torch_dilated(x, model) * sc
     assert p.shape == flags.shape
@@ -105,14 +105,14 @@ def test_dilated_graph_matches_torch(case):
 @pytest.mark.parametrize("is3d", [True, False], ids=["3d", "2d"])
 @pytest.mark.parametrize("d", [1, 2, 4, 8])
 def test_dilated_convolution_matches_torch(is3d, d):
-    """conv_dilated alone, on a grid with an axis shorter than d and axes d does not divide."""
+    """The oracle's float32 convolution alone, on a grid with an axis shorter than d and axes d does not divide."""
     rs = np.random.RandomState(d)
     shape = (2, 3) + ((5, 7, 9) if is3d else (1, 7, 9))
     kz = 3 if is3d else 1
     x = rs.uniform(-1, 1, shape).astype(np.float32)
     w = rs.uniform(-1, 1, (4, 3, kz, 3, 3)).astype(np.float32)
     b = rs.uniform(-1, 1, 4).astype(np.float32)
-    got = conv_dilated(x, w, b, is3d, d)
+    got = Float32Ops(oracle.Oracle()).conv(x, w, b, is3d, d, 0, False)
     xt, wt, bt = (torch.from_numpy(a).double() for a in (x, w, b))
     if is3d:
         want = F.conv3d(xt, wt, bt, padding=d, dilation=d).numpy()
@@ -123,7 +123,8 @@ def test_dilated_convolution_matches_torch(is3d, d):
 
 
 def test_one_dilated_bank_is_the_plain_graph():
-    """num = 1 'dilate' draws the same weights as no banks, and the restatement then equals oracle.model_forward."""
+    """num = 1 'dilate' draws the same weights as no banks, and the 1-bank graph then computes the plain graph's
+    bits."""
     orc = oracle.Oracle()
     flags = synth.make_flags(8, 8, 8, True, nb=1, geometry=False)
     U = synth.make_smooth_velocity(flags, True, amp=1.0)
@@ -134,13 +135,13 @@ def test_one_dilated_bank_is_the_plain_graph():
         assert np.array_equal(w0, w1) and np.array_equal(b0, b1)
     p0 = np.zeros_like(flags)
     a = oracle.model_forward(orc, plain, p0, U, flags)
-    b = model_forward_dilated(orc, one, p0, U, flags)
+    b = oracle.model_forward(orc, one, p0, U, flags)
     for u, v in zip(a, b):
         assert np.array_equal(u, v)
 
 
 def test_dilate_and_mres_draw_the_same_weights():
-    """synth.make_model gives 'dilate' the weight shapes (and values) of 'mres'; the restatements differ."""
+    """synth.make_model gives 'dilate' the weight shapes (and values) of 'mres'; the graphs differ."""
     mres = synth.make_model(True, banks={"num": 2, "split_stage": 1, "join_stage": 3, "aggregate": "concat"})
     dil = synth.make_model(True, banks=dilate(2, "concat"))
     for a, b in zip(mres["layers"], dil["layers"]):

@@ -1,4 +1,4 @@
-"""The CPU restatement of the input block of torch/lib/model.lua:27-150 and :357-387 (tests/inputs_oracle.py:
+"""The CPU restatement of the input block of torch/lib/model.lua:27-150 and :357-387 (oracle/model.py:
 inputChannels, normalizeInput, normalizeInputFunc, normalizeInputChan, addPressureSkip) against an independent
 float64 evaluation: the divergence, the scale and the channel join restated here in numpy, the convolutions in
 torch.nn.functional.  This pins the semantics the GPU path is then compared with (tests/test_gpu_cnn_inputs.py)."""
@@ -11,7 +11,6 @@ import torch.nn.functional as F
 
 import oracle
 from fluidnet_b200 import synth
-from inputs_oracle import model_forward_inputs
 from test_oracle_model_graph import torch_stack
 
 # Every inputChannels set the reference can build: flags on, and UDiv or div (tfluids.VelocityUpdate needs UDiv).
@@ -87,7 +86,7 @@ def run_case(is3d, ch, normalize=True, func="std", chan="UDiv", skip=False, mode
     model = synth.make_model(is3d, model_type=model_type, inputs=inputs)
     assert model["layers"][0][0].shape[1] == ch["pDiv"] + (3 if is3d else 2) * ch["UDiv"] + ch["div"] + 1
     assert model["layers"][-1][0].shape[1] == model["layers"][-2][0].shape[0] + skip
-    p, U2, scale = model_forward_inputs(orc, model, p0, U, flags, **model["inputs"])
+    p, U2, scale = oracle.model_forward(orc, model, p0, U, flags)
     U1 = U.copy()
     orc.setWallBcsForward(U1, flags, as_mask_multiply=True)
     want, want_scale = reference_p(model, p0, U1, flags, ch, normalize, func, chan, skip)
@@ -131,16 +130,17 @@ def test_pressure_skip(is3d, model_type, ch):
 
 
 def test_defaults_are_the_default_graph():
-    """No keywords and the explicit defaults give the bits of oracle.model_forward (the 'default' input block)."""
+    """A model without input keywords and one with the explicit defaults give the same bits (the 'default' input
+    block)."""
     orc = oracle.Oracle()
     flags = synth.make_flags(8, 8, 8, True, nb=2)
     U = synth.make_smooth_velocity(flags, True)
     p0 = (synth.make_density(flags, seed=5) - np.float32(0.5)) * np.float32(0.2)
     model = synth.make_model(True)
+    kw = dict(inputChannels=dict(pDiv=True, UDiv=False, div=True, flags=True), normalizeInput=True,
+              normalizeInputFunc="std", normalizeInputChan="UDiv", addPressureSkip=False)
     want = oracle.model_forward(orc, model, p0, U, flags)
-    a = model_forward_inputs(orc, model, p0, U, flags)
-    b = model_forward_inputs(orc, model, p0, U, flags, inputChannels=dict(pDiv=True, UDiv=False, div=True, flags=True),
-                             normalizeInput=True, normalizeInputFunc="std", normalizeInputChan="UDiv",
-                             addPressureSkip=False)
+    a = oracle.model_forward(orc, dict(model, inputs={}), p0, U, flags)
+    b = oracle.model_forward(orc, dict(model, inputs=kw), p0, U, flags)
     for x, y, z in zip(want, a, b):
         assert np.array_equal(x, y) and np.array_equal(x, z)

@@ -5,7 +5,7 @@ plane that can change the projection's output on the owned planes, and the U / p
 rank's boundary to the coarsest bank's 2^(N-1) planes.
 
 The model is a float64 restatement of the step's projection on the 3-D 'default' graph with banks split at stage 1
-and joined at stage 3 (tests/bank_oracle.py's graph, lib/model.lua:252-361): wall mask, divergence and occupancy in
+and joined at stage 3 (oracle/model.py's 'mres' graph, lib/model.lua:252-361): wall mask, divergence and occupancy in
 front, the velocity update and wall mask behind.  Its dependency structure follows the kernels (the input at plane z
 reads U at z and z + 1 and the flags at z - 1 .. z + 1; the update at z reads p and the flags at z - 1).  The input
 scale is a global reduction the slab step all-reduces, not a halo matter: it is held fixed.  Weights are positive
