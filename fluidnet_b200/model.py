@@ -168,6 +168,21 @@ class ProjectionModel:
         torch7.check_stages(stages, ref["mconf"], opts)
         return cls(stages, ref["is3D"], device=device, **opts), ref["mconf"]
 
+    MODEL_KEYS = ("layers", "is3D", "pool", "up", "poolType", "nonlinType", "banks", "inputs", "batchNorm")
+
+    @classmethod
+    def from_model(cls, model, device=None, normalizeInputThreshold=1e-5):
+        """The model a model dict describes: the form of synth.make_model and oracle.model, {"layers", "is3D"[,
+        "pool", "up", "poolType", "nonlinType", "banks", "batchNorm"]} as the keywords of the constructor, and
+        "inputs" holding the input-block keywords.  A key outside these raises ValueError, so no part of the
+        description is left out of the network."""
+        unknown = sorted(set(model) - set(cls.MODEL_KEYS))
+        if unknown:
+            raise ValueError("model keys ProjectionModel does not take: %s" % ", ".join(unknown))
+        kw = {k: model[k] for k in ("pool", "up", "poolType", "nonlinType", "banks", "batchNorm") if k in model}
+        return cls(model["layers"], model["is3D"], device=device, normalizeInputThreshold=normalizeInputThreshold,
+                   **kw, **(model.get("inputs") or {}))
+
     MODES = {"fp32": 0, "tf32": 1, "tf32x3": 2}
 
     def set_mode(self, mode):

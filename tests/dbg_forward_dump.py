@@ -17,7 +17,8 @@ def main():
     import torch
     from fluidnet_b200 import simulate, synth
     from fluidnet_b200.slab import NativeSlabSimulator
-    from test_gpu_launch_tally import banks, _fields, _model, _step_problem
+    from fluidnet_b200.model import ProjectionModel
+    from scenes import banks, fields_with_random_p, plume_batch, step_mconf
 
     out = sys.argv[1]
     os.makedirs(out, exist_ok=True)
@@ -26,8 +27,9 @@ def main():
         np.save(os.path.join(out, name + ".npy"), t.cpu().numpy() if hasattr(t, "cpu") else t)
 
     skip = {"inputChannels": {"UDiv": True}, "addPressureSkip": True}
-    models = [("default", True, {}, (16, 16, 16)), ("mres3-concat", True, {"banks": banks(3, "concat")}, (16, 16, 16)),
-              ("mres3-add", True, {"banks": banks(3, "add")}, (16, 16, 16)),
+    models = [("default", True, {}, (16, 16, 16)), 
+              ("mres3-concat", True, {"banks": banks(3, "concat", "mres")}, (16, 16, 16)),
+              ("mres3-add", True, {"banks": banks(3, "add", "mres")}, (16, 16, 16)),
               ("dilate2", True, {"banks": banks(2, "concat", "dilate")}, (15, 16, 15)),
               ("bn-batch", True, {"batch_norm": {"train": True}}, (16, 16, 16)),
               ("bn-running", True, {"batch_norm": {"train": False}}, (16, 16, 16)),
@@ -35,27 +37,28 @@ def main():
               ("yang", True, {"model_type": "yang"}, (16, 16, 16)), ("default2d", False, {}, (1, 32, 32))]
     for name, is3d, kw, (nz, ny, nx) in models:
         mnp = synth.make_model(is3d, **kw)
-        f = {k: torch.from_numpy(v).cuda() for k, v in _fields(nz, ny, nx, is3d).items()}
+        f = {k: torch.from_numpy(v).cuda() for k, v in fields_with_random_p(nz, ny, nx, is3d).items()}
         for mode in ("fp32", "tf32", "tf32x3"):
             try:
-                gm = _model(mnp, mode)
+                gm = ProjectionModel.from_model(mnp)
+                gm.set_mode(mode)
             except Exception:       # the model does not take this mode
                 assert mode != "fp32"
                 continue
             p, U = gm.forward((f["pDiv"], f["UDiv"], f["flags"]))
             save("%s-%s-p" % (name, mode), p)
             save("%s-%s-U" % (name, mode), U)
-    for name, bk in (("default", None), ("mres2", banks(2, "concat")), ("mres3-add", banks(3, "add"))):
-        batch, mconf, mnp = _step_problem(32, bk)
-        gm = _model(mnp, "tf32x3")
+    for name, bk in (("default", None), ("mres2", banks(2, "concat", "mres")), ("mres3-add", banks(3, "add", "mres"))):
+        batch, mconf, mnp = plume_batch(32, inflow=32 / 128.0 * 4), step_mconf(32), synth.make_model(True, banks=bk)
+        gm = ProjectionModel.from_model(mnp)
+        gm.set_mode("tf32x3")
         gb = {k: torch.from_numpy(v).cuda() for k, v in batch.items()}
         for _ in range(3):
             simulate.simulate_fused(None, mconf, gb, gm)
         for k in ("pDiv", "UDiv", "density"):
             save("step-%s-%s" % (name, k), gb[k])
     bk = banks(2, "concat")
-    del bk["type"]
-    batch, mconf, mnp = _step_problem(32, bk)
+    batch, mconf, mnp = plume_batch(32, inflow=32 / 128.0 * 4), step_mconf(32), synth.make_model(True, banks=bk)
     tb = {k: torch.from_numpy(v) for k, v in batch.items()}
     sim = NativeSlabSimulator(tb, mconf, mnp["layers"], torch.device("cuda", 0), rank=0, world=1, banks=bk)
     for _ in range(3):

@@ -2,16 +2,16 @@ import os, sys, traceback
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 import torch, torch.multiprocessing as mp
-import test_gpu_slab as T
+from slab_cases import collect, free_port, slab_worker
 
 if __name__ == "__main__":
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = T._free_port()
-    procs = [ctx.Process(target=T._worker, args=(r, 2, port, 48, 2, q)) for r in range(2)]
+    port = free_port()
+    procs = [ctx.Process(target=slab_worker, args=(r, 2, port, 48, 2, q)) for r in range(2)]
     for p in procs:
         p.start()
-    res = T._collect(procs, q, 100)
+    res = collect(procs, q, 100)
     for r in res:
         print(r[0], r[1][-3000:])
     print("n results", len(res))

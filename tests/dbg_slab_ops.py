@@ -3,8 +3,8 @@ sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
 from fluidnet_b200 import tfluids
 from fluidnet_b200.slab import SlabDecomposition
-from test_gpu_slab import _problem
-batch, mconf, mnp = _problem(48)
+from slab_cases import convnet_problem
+batch, mconf, mnp = convnet_problem(48)
 tb = {k: torch.from_numpy(v).cuda() for k, v in batch.items()}
 ctx = tfluids.context()
 def cmp(name, got, want, d):

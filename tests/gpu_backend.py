@@ -3,7 +3,7 @@ numpy-level API as oracle.Oracle, so GPU parity tests read like the oracle tests
 import numpy as np
 import torch
 
-from fluidnet_b200 import tfluids, model as fmodel
+from fluidnet_b200 import tfluids
 
 
 def dev(a):
@@ -113,13 +113,3 @@ class GpuBackend:
         tfluids.clamp(t, lo, hi)
         x[...] = host(t)
 
-
-def make_gpu_model(model_np, threshold=1e-5):
-    return fmodel.ProjectionModel(model_np["layers"], model_np["is3D"], normalizeInputThreshold=threshold,
-                                  pool=model_np.get("pool"), up=model_np.get("up"),
-                                  poolType=model_np.get("poolType", "avg"),
-                                  nonlinType=model_np.get("nonlinType", "relu"))
-
-
-def batch_to_gpu(batch):
-    return {k: (dev(v) if isinstance(v, np.ndarray) else v) for k, v in batch.items()}

@@ -13,7 +13,7 @@ The 2-D run is the same scene on a 128^2 grid (no vorticity confinement, as in t
 import numpy as np
 
 import oracle
-from fluidnet_b200 import synth
+from scenes import plume_batch
 
 N = 100
 DT = 0.1
@@ -25,12 +25,7 @@ KEYS = ("pDiv", "UDiv", "density")
 def make_batch(is3d):
     """Initial state and BCs: [1][c][64][64][64] in 3-D, [1][c][1][128][128] in 2-D (numpy)."""
     n = 64 if is3d else 128
-    flags = synth.make_flags(n, n, n if is3d else 1, is3d, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, is3d, amp=2.0, seed=1234)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], n / 128.0 * 4, 0.15)
-    return batch
+    return plume_batch(n, is3d, amp=2.0, inflow=n / 128.0 * 4)
 
 
 def make_mconf(is3d, sim_method="jacobi"):

@@ -61,6 +61,7 @@ import numpy as np
 import torch
 import torch.nn.functional as F
 
+import oracle
 from oracle import model as om
 from oracle.model import DEFAULT_CHANNELS, model_inputs, network
 
@@ -370,3 +371,22 @@ def check(what, got, want, E):
     assert r <= 1.0, "%s: %d voxels over the bound; worst %s: err %.3e bound %.3e (err/E %.3g)" % (
         what, int((np.abs(np.asarray(got, np.float64) - want) > E).sum()), worst, err, bound, r)
     return r
+
+
+def projection_reference(state, mconf, gm, mnp):
+    """The float64 projection of one step from `state` (GPU tensors, left as they are) on the scale interval: the
+    operator sequence up to the projection and setConstVals, forward_bound, then the U BCs (x inv + bc: E |inv| plus
+    two roundings) and the +-1e6 clamp (1-Lipschitz)."""
+    from fluidnet_b200 import simulate
+    ob = {k: v.clone() for k, v in state.items()}
+    simulate.simulate(None, mconf, ob, gm, outputDiv=True)
+    p, U, flags, density = simulate.getPUFlagsDensityReference(ob)
+    simulate.setConstVals(ob, p, U, flags, density)
+    assert ob.get("pBC") is None, "a pressure BC takes the operator path, not these cases"
+    ref = forward_bound(oracle.Oracle(), mnp, p.cpu().numpy(), U.cpu().numpy(), flags.cpu().numpy(), gm.get_mode(),
+                        scale=None, threshold=gm.threshold)
+    inv, bc = ob["UBCInvMask"].cpu().numpy().astype(np.float64), ob["UBC"].cpu().numpy().astype(np.float64)
+    Ui = ref["U"] * inv
+    ref["EU"] = ref["EU"] * np.abs(inv) + gamma(2) * (np.abs(Ui) + ref["EU"] * np.abs(inv) + np.abs(bc))
+    ref["U"] = np.clip(Ui + bc, -1e6, 1e6)
+    return ref

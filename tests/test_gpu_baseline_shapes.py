@@ -19,28 +19,10 @@ import torch
 import oracle
 from cases import bits_equal, describe_diff
 from fluidnet_b200 import synth
+from scenes import close, plume_batch, step_mconf, to_gpu
+from step_cases import MODE_TOL
 
 pytestmark = pytest.mark.gpu
-
-
-def close(got, want, tol, what):
-    err = np.abs(got.astype(np.float64) - want.astype(np.float64)).max()
-    scale = max(np.abs(want).max(), 1e-6)
-    assert err <= tol * scale, "%s: max err %g vs scale %g" % (what, err, scale)
-
-
-def make_batch(n, plume=True, amp=3.0, smooth=True):
-    flags = synth.make_flags(n, n, n, True, nb=1, geometry=True)
-    U = (synth.make_smooth_velocity if smooth else synth.make_velocity)(flags, True, amp=amp)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    if plume:
-        oracle.create_plume_bcs(batch, [1.0], n / 128.0, 0.15)
-    return batch
-
-
-def to_gpu(batch):
-    return {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items() if v is not None}
 
 
 @pytest.fixture(scope="module")
@@ -49,18 +31,15 @@ def gpu():
     return GpuBackend()
 
 
-MODE_TOL = {"fp32": 2e-5, "tf32x3": 2e-5, "tf32": 3e-3}
-
-
 @pytest.mark.parametrize("mode", ["fp32", "tf32x3", "tf32"])
 def test_c2_model_forward_64(orc, mode):
     """BASELINE config 2: 3-D 64^3, CNN pressure projection forward."""
-    from gpu_backend import make_gpu_model
-    batch = make_batch(64, plume=False)
+    from fluidnet_b200.model import ProjectionModel
+    batch = plume_batch(64)
     mnp = synth.make_model(True)
     p0 = (synth.make_density(batch["flags"], seed=77) - np.float32(0.5)) * np.float32(0.1)
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
-    gm = make_gpu_model(mnp)
+    gm = ProjectionModel.from_model(mnp)
     gm.set_mode(mode)
     gp, gU = gm.forward((torch.from_numpy(p0).cuda(), torch.from_numpy(batch["UDiv"]).cuda(),
                          torch.from_numpy(batch["flags"]).cuda()), return_scale=True)
@@ -76,13 +55,12 @@ def test_c3_fused_step_vs_oracle(orc, n):
     single-call fused step against oracle.simulate.  The density leaves the step after the advection and
     the boundary conditions only -> bit-exact; U and p pass through the conv stack -> 2e-5 (3xTF32)."""
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
-    batch = make_batch(n)
+    from fluidnet_b200.model import ProjectionModel
+    batch = plume_batch(n, inflow=n / 128.0)
     mnp = synth.make_model(True)
-    gm = make_gpu_model(mnp)
+    gm = ProjectionModel.from_model(mnp)
     assert gm.get_mode() == "tf32x3"
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                 vorticityConfinementAmp=3.0, simMethod="convnet")
+    mconf = step_mconf(n)
     gb = to_gpu(batch)
     simulate.simulate_fused(None, mconf, gb, gm)
     torch.cuda.synchronize()
@@ -101,7 +79,7 @@ def test_advection_128_bit_exact(orc, gpu, amp, smooth):
     """advectVel / advectScalar (maccormackOurs) on the 128^3 grid with the sphere + slab geometry: the
     large clear interior takes the clear-space path, cells near the solids and (amp 25: 2.5-cell traces)
     fast cells the general one."""
-    b = make_batch(128, plume=False, amp=amp, smooth=smooth)
+    b = plume_batch(128, amp=amp, uniform=not smooth)
     U, fl, d = b["UDiv"], b["flags"], b["density"]
     want = orc.advectVel(0.1, U, fl, "maccormackOurs", 0.6)
     got = gpu.advectVel(0.1, U, fl, "maccormackOurs", 0.6)
@@ -118,7 +96,7 @@ def test_advection_128_bit_exact(orc, gpu, amp, smooth):
 
 def test_c4_jacobi_128_bit_exact(orc, gpu):
     """BASELINE config 4: divergence + 100 Jacobi sweeps + velocity update at 128^3."""
-    b = make_batch(128, plume=False)
+    b = plume_batch(128)
     U, fl = b["UDiv"], b["flags"]
     div_w = orc.velocityDivergenceForward(U, fl)
     div_g = gpu.velocityDivergenceForward(U, fl)
@@ -138,7 +116,7 @@ def test_c4_jacobi_128_bit_exact(orc, gpu):
 def test_jacobi_step_64_bit_exact(orc):
     """Whole step on the Jacobi path at 64^3 (every kernel a per-cell restatement): bit-exact."""
     from fluidnet_b200 import simulate
-    batch = make_batch(64)
+    batch = plume_batch(64, inflow=64 / 128.0)
     mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=1.0,
                                  vorticityConfinementAmp=3.0, simMethod="jacobi", maxIter=30, is3D=True)
     gb = to_gpu(batch)

@@ -26,8 +26,7 @@ import monitor_reference
 import oracle
 from cases import bits_equal, describe_diff
 from fluidnet_b200 import synth
-from test_gpu_edge_sizes import fill, plane_of, run, set_tile_mode
-from test_gpu_step_paths import MODE_TOL, OPS_TOL, close_per_entry, plume_bcs, same_zero_bits
+from step_cases import MODE_TOL, OPS_TOL, close_per_entry, fill, plane_of, plume_bcs, run, same_zero_bits, set_tile_mode
 
 pytestmark = pytest.mark.gpu
 
@@ -175,12 +174,12 @@ STEP_CASES = {
 @pytest.mark.parametrize("name", list(STEP_CASES))
 def test_convnet_entries_equal_alone(orc, name, mode):
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     shape, amps, kind = STEP_CASES[name]
     nb = len(amps)
     batch = step_batch(orc, shape, nb, amps, kind=kind)
     mnp = synth.make_model(True)
-    gm = make_gpu_model(mnp)
+    gm = ProjectionModel.from_model(mnp)
     gm.set_mode(mode)
     together = gpu(batch)
     ctx = tfluids.context()
@@ -211,10 +210,10 @@ def test_large_batches(orc):
     """nb = 100 tiny scenes through the fused step (z range 5: blocks straddle entries) and nb = 300 through a Jacobi
     solve with a tolerance (the per-entry residual sums): every per-entry buffer grows with nb."""
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     four = step_batch(orc, (5, 8, 8), 4, (3.0, 0.0, 8.0, 1.0), kind="open")
     many = {k: np.ascontiguousarray(np.concatenate([v[b % 4:b % 4 + 1] for b in range(100)])) for k, v in four.items()}
-    gm = make_gpu_model(synth.make_model(True))
+    gm = ProjectionModel.from_model(synth.make_model(True))
     gm.set_mode("tf32x3")
     together = gpu(many)
     alone = [gpu(entry(four, b)) for b in range(4)]
@@ -250,10 +249,10 @@ def test_large_batches(orc):
 @pytest.mark.parametrize("method", ["convnet", "jacobi"])
 def test_batched_graph_replays_equal_direct_steps(orc, method):
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     mconf = CONVNET if method == "convnet" else JACOBI
     batch = step_batch(orc, (8, 12, 32), 3, (3.0, 0.0, 8.0))
-    gm = make_gpu_model(synth.make_model(True)) if method == "convnet" else None
+    gm = ProjectionModel.from_model(synth.make_model(True)) if method == "convnet" else None
     if gm is not None:
         gm.set_mode("tf32x3")
     stream = torch.cuda.Stream()
@@ -280,10 +279,10 @@ def test_batched_graph_replays_equal_direct_steps(orc, method):
 
 def test_host_buffer_step_at_nb3(orc):
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     shape = (9, 12, 32)
     batch = step_batch(orc, shape, 3, (3.0, 0.0, 8.0))
-    gm = make_gpu_model(synth.make_model(True))
+    gm = ProjectionModel.from_model(synth.make_model(True))
     gm.set_mode("tf32x3")
     dev = gpu(batch)
     ctx = tfluids.context()
@@ -340,9 +339,9 @@ def _tally_and_kernels(ctx, call, attempts=3):
 def launch_census(nb):
     """{n: (tally, {kernel: count})} of one fused step at n = 1 and n = nb, under torch.profiler in this process."""
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     orc = oracle.Oracle()
-    gm = make_gpu_model(synth.make_model(True))
+    gm = ProjectionModel.from_model(synth.make_model(True))
     gm.set_mode("tf32x3")
     ctx = tfluids.context()
     out = {}
@@ -471,9 +470,9 @@ def test_calc_stats_convnet_batches(tmp_path):
     """The convnet table through the fused step: the start frame's row is exact, later rows stay close to the plain
     operator loop (the conv stack and the input scale's double atomics)."""
     from fluidnet_b200 import calc_stats
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     frames = calc_stats.synthetic_frames(5, 16, 9)
-    gm = make_gpu_model(synth.make_model(True))
+    gm = ProjectionModel.from_model(synth.make_model(True))
     gm.set_mode("tf32x3")
     mconf = calc_stats.eval_mconf(None, "convnet")
     rows = calc_stats.run(frames, mconf, gm, 4, 2, log=lambda *a: None)

@@ -39,11 +39,11 @@ import monitor_reference
 import oracle
 from cases import bits_equal, describe_diff
 from fluidnet_b200 import synth
-from network_bound import check, tc_covered
-from test_gpu_cnn_bn import make_gpu
-from test_gpu_cnn_network_f64 import banks, bn_model, projection_reference
-from test_gpu_step_paths import (MODE_TOL, OPS_TOL, close_per_entry, plume_bcs, quad_dims, run_in_child,
-                                 same_zero_bits, takes_fused_path)
+from fluidnet_b200.model import ProjectionModel
+from network_bound import check, projection_reference, tc_covered
+from scenes import banks, bn_model
+from step_cases import (MODE_TOL, OPS_TOL, close_per_entry, plume_bcs, quad_dims, run_in_child, same_zero_bits,
+                        takes_fused_path)
 
 MCONF = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=0.5, vorticityConfinementAmp=3.0,
                              simMethod="convnet")
@@ -53,14 +53,14 @@ JACOBI = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=0.5,
 
 MODELS = {
     "default": lambda: synth.make_model(True),
-    "mres-n2-concat": lambda: synth.make_model(True, banks=banks(2, "concat")),
-    "mres-n3-add": lambda: synth.make_model(True, banks=banks(3, "add")),
+    "mres-n2-concat": lambda: synth.make_model(True, banks=banks(2, "concat", "mres")),
+    "mres-n3-add": lambda: synth.make_model(True, banks=banks(3, "add", "mres")),
     "dilate-n2-concat": lambda: synth.make_model(True, banks=banks(2, "concat", "dilate")),
     "dilate-n3-add": lambda: synth.make_model(True, banks=banks(3, "add", "dilate")),
     "bn-batch": lambda: bn_model(True),
     "bn-running": lambda: bn_model(False),
     "bn-batch-relu6": lambda: bn_model(True, relu6=True),
-    "relu6-mres-n2-concat": lambda: bn_model(None, banks(2, "concat"), relu6=True),
+    "relu6-mres-n2-concat": lambda: bn_model(None, bk=banks(2, "concat", "mres"), relu6=True),
 }
 BATCH_STATS = {"bn-batch", "bn-batch-relu6"}
 
@@ -163,7 +163,7 @@ def oracle_tol(model, mode):
 
 
 def make_model(mnp, mode):
-    gm = make_gpu(mnp)
+    gm = ProjectionModel.from_model(mnp)
     assert gm.get_mode() == "tf32x3"
     gm.set_mode(mode)
     return gm
@@ -257,14 +257,14 @@ def test_batched_graph_replays_equal_direct_steps(orc, scene):
 def scene_kernels():
     """{case: (launch tally, {kernel: count})} of one fused step per case, under torch.profiler."""
     from fluidnet_b200 import simulate, tfluids
-    from test_gpu_launch_tally import _tally_and_kernels
+    from step_cases import tally_and_kernels
     orc = oracle.Oracle()
     out = {}
     for scene, mode in CASES:
         model, shape, kinds, amps = SCENES[scene]
         gm = make_model(MODELS[model](), mode)
         st = gpu(make_scene(orc, shape, kinds, amps))
-        tally, kernels = _tally_and_kernels(tfluids.context(), lambda: simulate.simulate_fused(None, MCONF, st, gm),
+        tally, kernels = tally_and_kernels(tfluids.context(), lambda: simulate.simulate_fused(None, MCONF, st, gm),
                                             attempts=6)
         out["%s-%s" % (scene, mode)] = (tally, dict(kernels))
     return out
@@ -272,7 +272,7 @@ def scene_kernels():
 
 @pytest.mark.gpu
 def test_fused_kernels_ran():
-    from test_gpu_step_paths import step_path
+    from step_cases import step_path
     seen = run_in_child("test_gpu_batch_models", "t.scene_kernels()")
     assert set(seen) == set(CASE_IDS)
     for (scene, mode), cid in zip(CASES, CASE_IDS):
@@ -419,14 +419,13 @@ LIMIT_GRIDS = {"2d-8x8": ((1, 8, 8), False), "3d-5x8x8": ((5, 8, 8), True)}
 def test_largest_batch_runs_and_one_more_is_refused(orc, grid):
     from fluidnet_b200 import monitor, simulate, tfluids
     from fluidnet_b200._lib import TflError
-    from gpu_backend import make_gpu_model
     shape, is3d = LIMIT_GRIDS[grid]
     nz = shape[0]
     nb = max_batch_planes(nz) // nz
     assert nb * nz == max_batch_planes(nz)
     protos = prototypes(orc, shape, is3d)
     mnp = synth.make_model(True)
-    gm = make_gpu_model(mnp) if is3d else None
+    gm = ProjectionModel.from_model(mnp) if is3d else None
     jac = dict(JACOBI, is3D=is3d)
     ctx = tfluids.context()
     ctx.trace_faults()

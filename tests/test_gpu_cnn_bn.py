@@ -36,18 +36,13 @@ import oracle
 from fluidnet_b200 import synth
 from fluidnet_b200 import model as fmodel
 from fluidnet_b200._lib import TflError
-from test_gpu_cnn_banks import close, inputs_of, make_batch, write_mconf
-from test_gpu_step_paths import contexts  # noqa: F401  (fixture: library contexts of one test)
+from scenes import banks, bn_model, close, inputs_of, plume_batch, step_mconf, to_gpu
+from step_cases import MODE_TOL, contexts
+from torch7_writer import write_mconf
 
 pytestmark = pytest.mark.gpu
 
 U32, U64 = 2.0 ** -24, 2.0 ** -53
-
-
-def make_gpu(mnp):
-    return fmodel.ProjectionModel(mnp["layers"], mnp["is3D"], pool=mnp.get("pool"), up=mnp.get("up"),
-                                  poolType=mnp.get("poolType", "avg"), nonlinType=mnp.get("nonlinType", "relu"),
-                                  banks=mnp.get("banks"), batchNorm=mnp.get("batchNorm"), **(mnp.get("inputs") or {}))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -119,10 +114,6 @@ def test_bn_kernels_against_float64(nb, n, gap):
 # ---------------------------------------------------------------------------------------------------------------
 # model:forward
 # ---------------------------------------------------------------------------------------------------------------
-def banks(num, agg, kind="mres", s=1, j=3):
-    return {"num": num, "split_stage": s, "join_stage": j, "aggregate": agg, "type": kind}
-
-
 # (is3d, model_type, banks, inputs, (nz, ny, nx))
 FORWARD = {
     "3d-default": (True, "default", None, None, (8, 10, 12)),
@@ -130,28 +121,15 @@ FORWARD = {
                              (7, 9, 11)),
     "3d-tog": (True, "tog", None, None, (16, 16, 24)),
     "3d-yang": (True, "yang", None, None, (6, 8, 10)),
-    "3d-mres-n2-concat": (True, "default", banks(2, "concat"), None, (8, 12, 16)),
-    "3d-mres-n3-add": (True, "default", banks(3, "add"), None, (8, 8, 12)),
+    "3d-mres-n2-concat": (True, "default", banks(2, "concat", "mres"), None, (8, 12, 16)),
+    "3d-mres-n3-add": (True, "default", banks(3, "add", "mres"), None, (8, 8, 12)),
     "3d-dilate-n2-concat": (True, "default", banks(2, "concat", "dilate"), None, (7, 10, 29)),
     "3d-dilate-n3-add-s2j4": (True, "default", banks(3, "add", "dilate", 2, 4), None, (6, 10, 12)),
     "2d-default": (False, "default", None, None, (1, 36, 51)),
     "2d-tog": (False, "tog", None, None, (1, 32, 48)),
-    "2d-mres-n2-add": (False, "default", banks(2, "add"), None, (1, 32, 24)),
+    "2d-mres-n2-add": (False, "default", banks(2, "add", "mres"), None, (1, 32, 24)),
     "2d-dilate-n3-concat": (False, "default", banks(3, "concat", "dilate"), None, (1, 41, 35)),
 }
-
-
-def bn_model(is3d, model_type, bk, inputs, train, relu6=False, affine=True):
-    m = synth.make_model(is3d, model_type=model_type, banks=bk, inputs=inputs,
-                         batch_norm={"train": train, "affine": affine})
-    if relu6:
-        m["nonlinType"] = "relu6"
-        first = m["layers"][0] if not isinstance(m["layers"][0], list) else m["layers"][0][0]
-        first[0][...] *= np.float32(30.0)          # the first stage's values cross 6
-    return m
-
-
-MODE_TOL = {"fp32": 2e-5, "tf32x3": 2e-5, "tf32": 3e-3}
 
 
 def tc_covered(is3d, model_type, bk):
@@ -170,11 +148,11 @@ def test_bn_forward(case, variant, nb, mode):
     if mode != "default" and not covered:
         pytest.skip("fp32 only: the default mode is the only mode")
     relu6 = "relu6" in variant and model_type != "yang"
-    mnp = bn_model(is3d, model_type, bk, inputs, variant.startswith("batch"), relu6, "noaffine" not in variant)
-    batch = make_batch(shape, is3d, nb=nb)
+    mnp = bn_model(variant.startswith("batch"), is3d, model_type, bk, inputs, relu6, "noaffine" not in variant)
+    batch = plume_batch(shape, is3d, nb=nb)
     p0, inp = inputs_of(batch)
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"], f64=True)
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     assert gm.get_mode() == ("tf32x3" if covered else "fp32")
     if mode != "default":
         gm.set_mode(mode)
@@ -188,16 +166,17 @@ def test_bn_forward(case, variant, nb, mode):
 
 
 @pytest.mark.parametrize("mode", ["tf32x3", "tf32"])
-@pytest.mark.parametrize("bk", [banks(2, "concat"), banks(3, "add", "dilate")], ids=["mres-n2-concat", "dilate-n3-add"])
+@pytest.mark.parametrize("bk", [banks(2, "concat", "mres"), banks(3, "add", "dilate")],
+                         ids=["mres-n2-concat", "dilate-n3-add"])
 def test_relu6_banked_on_tensor_cores(bk, mode):
     """relu6 without BN keeps the banked tensor-core path: the clamp is in the bank layers' and the join's epilogues."""
     mnp = synth.make_model(True, banks=bk)
     mnp["nonlinType"] = "relu6"
     mnp["layers"][0][0][0][...] *= np.float32(30.0)
-    batch = make_batch((8, 12, 16), True, nb=2)
+    batch = plume_batch((8, 12, 16), True, nb=2)
     p0, inp = inputs_of(batch)
     wp, wU, _ = oracle.model_forward(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"], f64=True)
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     assert gm.get_mode() == "tf32x3"
     gm.set_mode(mode)
     gp, gU = gm.forward(inp)
@@ -215,7 +194,7 @@ TC_BN_CASES = {"ragged": (2, (5, 7, 9)), "nx128": (1, (3, 5, 128)), "nx130": (1,
 def test_tc_bn_layer(case, relu6, split):
     import torch.nn.functional as F
     from fluidnet_b200 import tfluids
-    from test_gpu_conv_tc import KAPPA, SENTINEL, layout, make_layer, pack, unpack
+    from tc_conv import KAPPA, SENTINEL, layout, make_layer, pack, unpack
     nb, shape = TC_BN_CASES[case]
     nz, ny, nx = shape
     kappa = KAPPA[split]
@@ -277,12 +256,12 @@ def test_tc_bn_layer(case, relu6, split):
 @pytest.mark.parametrize("case", ["3d-default", "3d-mres-n2-concat", "3d-dilate-n2-concat", "2d-tog"])
 def test_batch_statistics_couple_the_entries(case):
     is3d, model_type, bk, inputs, shape = FORWARD[case]
-    batch = make_batch(shape, is3d, nb=2)
+    batch = plume_batch(shape, is3d, nb=2)
     p0, inp = inputs_of(batch)
     other = list(t.clone() for t in inp)
     other[1][1] *= 2.0                  # entry 1's velocity
     for train in (True, False):
-        gm = make_gpu(bn_model(is3d, model_type, bk, inputs, train))
+        gm = fmodel.ProjectionModel.from_model(bn_model(train, is3d, model_type, bk, inputs))
         a = gm.forward(tuple(inp))[0][0].cpu().numpy()
         b = gm.forward(tuple(other))[0][0].cpu().numpy()
         if train:
@@ -298,11 +277,11 @@ def test_identity_running_statistics_equal_the_model_without_bn(is3d):
         c = len(e["running_mean"])
         e.update(weight=np.ones(c, np.float32), bias=np.zeros(c, np.float32), running_mean=np.zeros(c, np.float32),
                  running_var=np.full(c, 1.0 - 1e-4, np.float32), eps=1e-4)
-    batch = make_batch((8, 10, 12) if is3d else (1, 30, 26), is3d, nb=2)
+    batch = plume_batch((8, 10, 12) if is3d else (1, 30, 26), is3d, nb=2)
     _, inp = inputs_of(batch)
-    plain = make_gpu(dict(mnp, batchNorm=None))
+    plain = fmodel.ProjectionModel.from_model(dict(mnp, batchNorm=None))
     plain.set_mode("fp32")
-    with_bn = make_gpu(mnp)
+    with_bn = fmodel.ProjectionModel.from_model(mnp)
     with_bn.set_mode("fp32")
     for x, y in zip(with_bn.forward(inp), plain.forward(inp)):
         close(x.cpu().numpy(), y.cpu().numpy(), 2e-5, "identity BN")
@@ -311,27 +290,22 @@ def test_identity_running_statistics_equal_the_model_without_bn(is3d):
 # ---------------------------------------------------------------------------------------------------------------
 # The step
 # ---------------------------------------------------------------------------------------------------------------
-def step_mconf(n):
-    return oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                vorticityConfinementAmp=3.0, simMethod="convnet")
-
-
 @pytest.mark.parametrize("train", [True, False], ids=["batch", "running"])
 def test_bn_step(train, contexts):
     from fluidnet_b200 import simulate
     orc = oracle.Oracle()
     n = 20
-    batch = make_batch((n, n, n), True, plume=True)
-    from test_gpu_step_paths import takes_fused_path
-    mnp = bn_model(True, "default", None, None, train, relu6=True)
+    batch = plume_batch((n, n, n), True, inflow=n / 128.0 * 4)
+    from step_cases import takes_fused_path
+    mnp = bn_model(train, relu6=True)
     contexts.use(contexts.new())
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     contexts.models.append(gm)
     assert gm.get_mode() == "tf32x3" and takes_fused_path({"mode": gm.get_mode(), "nb": 1, "pbc": False})
     mconf = step_mconf(n)
-    a = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
-    b = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
-    g = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
+    a = to_gpu(batch)
+    b = to_gpu(batch)
+    g = to_gpu(batch)
     simulate.simulate(None, mconf, a, gm)
     simulate.simulate_fused(None, mconf, b, gm)
     oracle.simulate(orc, mconf, batch, mnp, f64=True)
@@ -355,10 +329,10 @@ def test_bn_step(train, contexts):
 def test_bn_host_buffer_step():
     from fluidnet_b200 import simulate, tfluids
     n = 16
-    batch = make_batch((n, n, n), True, plume=True)
-    gm = make_gpu(bn_model(True, "default", None, None, True))
+    batch = plume_batch((n, n, n), True, inflow=n / 128.0 * 4)
+    gm = fmodel.ProjectionModel.from_model(bn_model(True))
     mconf = step_mconf(n)
-    dev_batch = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
+    dev_batch = to_gpu(batch)
     ctx = tfluids.context()
     lib = ctx.lib
     hs = C.c_void_p()
@@ -383,10 +357,10 @@ def test_bn_host_buffer_step():
 # ---------------------------------------------------------------------------------------------------------------
 def test_bn_refusals():
     from fluidnet_b200 import tfluids
-    gm = make_gpu(bn_model(True, "default", None, None, True))
+    gm = fmodel.ProjectionModel.from_model(bn_model(True))
     assert gm.get_mode() == "tf32x3"
-    for bk in (banks(2, "concat"), banks(2, "add", "dilate")):
-        banked = make_gpu(bn_model(True, "default", bk, None, False))
+    for bk in (banks(2, "concat", "mres"), banks(2, "add", "dilate")):
+        banked = fmodel.ProjectionModel.from_model(bn_model(False, bk=bk))
         assert banked.get_mode() == "fp32"
         with pytest.raises(TflError, match="batch normalization"):
             banked.set_mode("tf32")
@@ -397,11 +371,11 @@ def test_bn_refusals():
                                        C.c_void_p(0), tfluids._grid(g), tfluids._grid(torch.zeros_like(U)),
                                        C.c_float(1e-5))
     assert rc != 0 and b"batch normalization" in lib.tfl_last_error(ctx.h)
-    mnp = bn_model(True, "default", None, None, True)
+    mnp = bn_model(True)
     bad = dict(mnp["batchNorm"], layers=[dict(e) for e in mnp["batchNorm"]["layers"]])
     bad["layers"][2]["eps"] = -1e-4
     with pytest.raises(TflError, match="eps"):
-        make_gpu(dict(mnp, batchNorm=bad))
+        fmodel.ProjectionModel.from_model(dict(mnp, batchNorm=bad))
     sig = synth.make_model(True, model_type="yang")
     lib2 = gm.ctx.lib
     from fluidnet_b200 import _lib
@@ -423,27 +397,27 @@ def test_bn_refusals():
 def test_slab_step_refuses_bn():
     from fluidnet_b200 import simulate
     from fluidnet_b200.slab import NativeSlabSimulator
-    from test_gpu_slab_banks import _problem, _refused
+    from slab_cases import banked_problem, refused
     dev = torch.device("cuda", 0)
-    tb, mconf, _ = _problem(32, 16, 16, None)
+    tb, mconf, _ = banked_problem(32, 16, 16, None)
     sim = NativeSlabSimulator(tb, mconf, synth.make_model(True)["layers"], dev, rank=0, world=1, margin=6)
     ctx, mc = sim.ctx, simulate.make_mconf(mconf)
     for train in (True, False):
-        gm = make_gpu(bn_model(True, "default", None, None, train))
-        msg = _refused(ctx, lambda: ctx.lib.tfl_slab_sim_step(ctx.h, sim.h, C.byref(mc), gm.h))
+        gm = fmodel.ProjectionModel.from_model(bn_model(train))
+        msg = refused(ctx, lambda: ctx.lib.tfl_slab_sim_step(ctx.h, sim.h, C.byref(mc), gm.h))
         assert b"batch normalization" in msg, msg
 
 
 @pytest.mark.parametrize("train", [True, False])
 def test_bn_reference_file_end_to_end(tmp_path, train):
-    from test_torch7_bn import bn_graph, mconf_for, write_bn_graph
-    bk = banks(2, "concat")
-    mnp = bn_model(True, "default", {k: v for k, v in bk.items() if k != "type"}, None, train)
+    from torch7_writer import bn_graph, mconf_for, write_bn_graph
+    bk = banks(2, "concat", "mres")
+    mnp = bn_model(train, bk={k: v for k, v in bk.items() if k != "type"})
     write_bn_graph(tmp_path / "net", bn_graph(mnp, True, train=train, interleave=True), True)
     write_mconf(tmp_path / "net_mconf.bin", mconf_for(True, bk, True))
     gm, mconf = fmodel.ProjectionModel.from_reference_file(str(tmp_path / "net"))
     assert mconf["addBatchNorm"] and gm.get_mode() == "fp32"          # banked: the fp32 path
-    batch = make_batch((8, 12, 16), True, nb=2)
+    batch = plume_batch((8, 12, 16), True, nb=2)
     p0, inp = inputs_of(batch)
     wp, wU, _ = oracle.model_forward(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"], f64=True)
     gp, gU = gm.forward(inp)

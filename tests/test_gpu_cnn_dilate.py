@@ -28,23 +28,18 @@ import oracle
 from fluidnet_b200 import synth
 from fluidnet_b200 import model as fmodel
 from fluidnet_b200._lib import TflError
+from fp32_conv import (DIRECT, GENERIC, SIGMOID_ULPS, activate, check_guards, gamma, guarded, make_conv,
+                       quantised_batch, seed_of, shuffle_model)
 from network_bound import conv_f64
-from test_gpu_cnn_banks import close, inputs_of, make_batch, write_mconf
-from test_gpu_step_paths import contexts  # noqa: F401  (fixture: library contexts of one test)
-from test_gpu_conv_fp32 import (DIRECT, GENERIC, SIGMOID_ULPS, activate, check_guards, gamma, guarded, make_conv,
-                                quantised_batch, seed_of, shuffle_model)
+from scenes import close, inputs_of, plume_batch, step_mconf, to_gpu
+from step_cases import MODE_TOL, contexts
+from torch7_writer import write_mconf
 
 pytestmark = pytest.mark.gpu
 
 
 def dilate(num, agg, s=1, j=3):
     return {"num": num, "split_stage": s, "join_stage": j, "aggregate": agg, "type": "dilate"}
-
-
-def make_gpu(mnp, threshold=1e-5):
-    return fmodel.ProjectionModel(mnp["layers"], mnp["is3D"], normalizeInputThreshold=threshold, pool=mnp.get("pool"),
-                                  up=mnp.get("up"), poolType=mnp.get("poolType", "avg"),
-                                  nonlinType=mnp.get("nonlinType", "relu"), banks=mnp.get("banks"))
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -105,7 +100,7 @@ def test_dilated_convolution(case, d):
 
 def test_dilation_one_is_the_plain_kernel():
     """dil = 1 through the dilated hook gives the bits of tfl_debug_conv_fp32."""
-    from test_gpu_conv_fp32 import run_conv as run_plain
+    from fp32_conv import run_conv as run_plain
     x, w, b = make_conv("signed", 3, 8, 3, True, (5, 6, 9), 2, 11)
     for generic in (0, 1):
         a, _ = run_conv(x, w, b, 1, True, generic, 1, "d1")
@@ -135,9 +130,6 @@ FORWARD = {
 }
 
 
-MODE_TOL = {"fp32": 2e-5, "tf32x3": 2e-5, "tf32": 3e-3}
-
-
 def tc_covered(is3d, model_type, bk):
     return is3d and model_type == "default" and bk["split_stage"] == 1 and bk["join_stage"] == 3
 
@@ -150,11 +142,11 @@ def test_dilated_forward(case, mode):
     covered = tc_covered(is3d, model_type, bk)
     if mode != "default" and not covered:
         pytest.skip("fp32 only: the default mode is the only mode")
-    batch = make_batch(shape, is3d, nb=nb)
+    batch = plume_batch(shape, is3d, nb=nb)
     mnp = synth.make_model(is3d, model_type=model_type, banks=bk)
     p0, inp = inputs_of(batch)
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     assert gm.get_mode() == ("tf32x3" if covered else "fp32")
     if mode != "default":
         gm.set_mode(mode)
@@ -185,7 +177,7 @@ TC_LAYER_CASES = {
 @pytest.mark.parametrize("case", list(TC_LAYER_CASES))
 def test_dilated_tc_layer(case, layer, split):
     from fluidnet_b200 import tfluids
-    from test_gpu_conv_tc import KAPPA, SENTINEL, layout, make_layer, pack, unpack
+    from tc_conv import KAPPA, SENTINEL, layout, make_layer, pack, unpack
     nb, shape, sh = TC_LAYER_CASES[case]
     d = 1 << sh
     cin = 3 if layer == "l1" else 8
@@ -220,11 +212,11 @@ def test_dilated_tc_layer(case, layer, split):
 @pytest.mark.parametrize("is3d", [True, False], ids=["3d", "2d"])
 def test_one_dilated_bank_is_the_single_bank_graph(is3d):
     shape = (8, 12, 16) if is3d else (1, 24, 20)
-    batch = make_batch(shape, is3d, nb=2)
+    batch = plume_batch(shape, is3d, nb=2)
     plain = synth.make_model(is3d)
     one = dict(plain, banks=dilate(1, "concat"))
     _, inp = inputs_of(batch)
-    a, b = make_gpu(plain), make_gpu(one)
+    a, b = fmodel.ProjectionModel.from_model(plain), fmodel.ProjectionModel.from_model(one)
     assert a.get_mode() == b.get_mode()
     for x, y in zip(a.forward(inp), b.forward(inp)):
         assert torch.equal(x.view(torch.int32), y.view(torch.int32))
@@ -244,7 +236,7 @@ def test_batch_entries_are_independent(name):
     channel slots of the 'concat' join keep the entries apart."""
     is3d, model_type, bk, shape = BATCH_GRAPHS[name]
     mnp = synth.make_model(is3d, model_type=model_type, banks=bk)
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     arrays = quantised_batch(shape, is3d, 3, seed_of(name) % 10000)
     p3, U3 = (t.cpu().numpy() for t in gm.forward(tuple(torch.from_numpy(a).cuda() for a in arrays)))
     assert np.isfinite(p3).all() and np.abs(p3).max() > 0
@@ -258,22 +250,17 @@ def test_batch_entries_are_independent(name):
 # ---------------------------------------------------------------------------------------------------------------
 # The step
 # ---------------------------------------------------------------------------------------------------------------
-def step_mconf(n):
-    return oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                vorticityConfinementAmp=3.0, simMethod="convnet")
-
-
 @pytest.mark.parametrize("bk", [dilate(2, "concat"), dilate(3, "add")], ids=["n2-concat", "n3-add"])
 def test_dilated_step(bk):
     from fluidnet_b200 import simulate
     orc = oracle.Oracle()
     n = 20
-    batch = make_batch((n, n, n), True, plume=True)
+    batch = plume_batch((n, n, n), True, inflow=n / 128.0 * 4)
     mnp = synth.make_model(True, banks=bk)
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     mconf = step_mconf(n)
-    a = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
-    b = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
+    a = to_gpu(batch)
+    b = to_gpu(batch)
     simulate.simulate(None, mconf, a, gm)
     simulate.simulate_fused(None, mconf, b, gm)
     oracle.simulate(orc, mconf, batch, mnp)
@@ -288,13 +275,13 @@ def test_dilated_step_graph_replay_and_stale_refusal(contexts):
     arena starts at this step's size."""
     from fluidnet_b200 import simulate
     n = 24
-    batch = make_batch((n, n, n), True, plume=True)
+    batch = plume_batch((n, n, n), True, inflow=n / 128.0 * 4)
     contexts.use(contexts.new())
-    gm = make_gpu(synth.make_model(True, banks=dilate(2, "concat")))
+    gm = fmodel.ProjectionModel.from_model(synth.make_model(True, banks=dilate(2, "concat")))
     contexts.models.append(gm)
     mconf = step_mconf(n)
-    ga = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
-    gb = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
+    ga = to_gpu(batch)
+    gb = to_gpu(batch)
     stream = torch.cuda.Stream()
     torch.cuda.synchronize()
     with torch.cuda.stream(stream):
@@ -307,7 +294,7 @@ def test_dilated_step_graph_replay_and_stale_refusal(contexts):
         stream.synchronize()
         for k in ("density", "UDiv", "pDiv"):
             assert torch.equal(ga[k].view(torch.int32), gb[k].view(torch.int32)), k
-        big = make_batch((40, 40, 40), True)
+        big = plume_batch((40, 40, 40), True)
         _, inp = inputs_of(big)
         gm.forward(inp)
         with pytest.raises(TflError, match="stale graph"):
@@ -319,11 +306,11 @@ def test_dilated_step_graph_replay_and_stale_refusal(contexts):
 def test_dilated_host_buffer_step(mode):
     from fluidnet_b200 import simulate, tfluids
     n = 16
-    batch = make_batch((n, n, n), True, plume=True)
-    gm = make_gpu(synth.make_model(True, banks=dilate(2, "concat")))
+    batch = plume_batch((n, n, n), True, inflow=n / 128.0 * 4)
+    gm = fmodel.ProjectionModel.from_model(synth.make_model(True, banks=dilate(2, "concat")))
     gm.set_mode(mode)
     mconf = step_mconf(n)
-    dev_batch = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
+    dev_batch = to_gpu(batch)
     ctx = tfluids.context()
     lib = ctx.lib
     hs = C.c_void_p()
@@ -347,9 +334,9 @@ def test_dilated_host_buffer_step(mode):
 # Refusals and import
 # ---------------------------------------------------------------------------------------------------------------
 def test_dilated_refusals():
-    gm = make_gpu(synth.make_model(True, banks=dilate(2, "concat")))
+    gm = fmodel.ProjectionModel.from_model(synth.make_model(True, banks=dilate(2, "concat")))
     assert gm.get_mode() == "tf32x3"
-    other = make_gpu(synth.make_model(True, banks=dilate(2, "concat", 2, 4)))
+    other = fmodel.ProjectionModel.from_model(synth.make_model(True, banks=dilate(2, "concat", 2, 4)))
     assert other.get_mode() == "fp32"
     with pytest.raises(TflError, match="split at stage 1 and joined at stage 3"):
         other.set_mode("tf32x3")
@@ -376,14 +363,14 @@ def test_dilated_refusals():
 
 @pytest.mark.parametrize("agg", ["concat", "add"])
 def test_dilated_reference_file_end_to_end(tmp_path, agg):
-    from test_torch7_banks import mconf_of
-    from test_torch7_dilate import write_dilated
+    from torch7_writer import mconf_of
+    from torch7_writer import write_dilated
     mnp = synth.make_model(True, banks=dilate(3, agg))
     write_dilated(tmp_path / "net", mnp, True)
     write_mconf(tmp_path / "net_mconf.bin", mconf_of(True, banksNum=3, banksAggregateMethod=agg, banksType="dilate"))
     gm, mconf = fmodel.ProjectionModel.from_reference_file(str(tmp_path / "net"))
     assert mconf["banksType"] == "dilate" and gm.banks == dilate(3, agg) and gm.get_mode() == "tf32x3"
-    batch = make_batch((8, 12, 16), True, nb=1)
+    batch = plume_batch((8, 12, 16), True, nb=1)
     p0, inp = inputs_of(batch)
     wp, wU, _ = oracle.model_forward(oracle.Oracle(), mnp, p0, batch["UDiv"], batch["flags"])
     gp, gU = gm.forward(inp)
@@ -396,13 +383,13 @@ def test_slab_step_refuses_dilated_banks():
     launches anything."""
     from fluidnet_b200 import simulate
     from fluidnet_b200.slab import NativeSlabSimulator
-    from test_gpu_slab_banks import _problem, _refused
+    from slab_cases import banked_problem, refused
     dev = torch.device("cuda", 0)
-    tb, mconf, _ = _problem(32, 16, 16, None)
+    tb, mconf, _ = banked_problem(32, 16, 16, None)
     sim = NativeSlabSimulator(tb, mconf, synth.make_model(True)["layers"], dev, rank=0, world=1, margin=6)
     ctx, mc = sim.ctx, simulate.make_mconf(mconf)
     gm = fmodel.ProjectionModel(synth.make_model(True, banks=dilate(2, "add"))["layers"], True, banks=dilate(2, "add"))
     for mode in ("tf32x3", "fp32"):
         gm.set_mode(mode)
-        msg = _refused(ctx, lambda: ctx.lib.tfl_slab_sim_step(ctx.h, sim.h, C.byref(mc), gm.h))
+        msg = refused(ctx, lambda: ctx.lib.tfl_slab_sim_step(ctx.h, sim.h, C.byref(mc), gm.h))
         assert b"banksType 'dilate'" in msg, msg

@@ -16,9 +16,10 @@ import oracle
 from fluidnet_b200 import model as fmodel
 from fluidnet_b200 import synth
 from oracle.model import model_input
-from test_gpu_cnn_banks import banks, close, inputs_of, make_batch
-from test_gpu_conv_tc import SENTINEL, check_layer, is_sentinel, layout, make_layer, pack, unpack
-from test_gpu_slab_banks import _problem, _refused
+from scenes import banks, close, inputs_of, plume_batch, step_mconf, to_gpu
+from slab_cases import banked_problem, refused
+from step_cases import MODE_TOL
+from tc_conv import SENTINEL, check_layer, is_sentinel, layout, make_layer, pack, unpack
 
 pytestmark = pytest.mark.gpu
 
@@ -26,14 +27,6 @@ ALL = dict(pDiv=True, UDiv=True, div=True, flags=True)
 U_ONLY = dict(pDiv=False, UDiv=True, div=False, flags=True)
 P_U = dict(pDiv=True, UDiv=True, div=False, flags=True)
 DIV_ONLY = dict(pDiv=False, UDiv=False, div=True, flags=True)
-MODE_TOL = {"fp32": 2e-5, "tf32x3": 2e-5, "tf32": 3e-3}
-
-
-def make_gpu(mnp):
-    return fmodel.ProjectionModel(mnp["layers"], mnp["is3D"], pool=mnp.get("pool"), up=mnp.get("up"),
-                                  poolType=mnp.get("poolType", "avg"), nonlinType=mnp.get("nonlinType", "relu"),
-                                  banks=mnp.get("banks"), **(mnp.get("inputs") or {}))
-
 
 def ins(ch=None, **kw):
     return dict(inputChannels=ch or dict(pDiv=True, UDiv=False, div=True, flags=True), **kw)
@@ -51,9 +44,9 @@ FP32 = {
     "3d-tog-all": (True, "tog", None, ins(ALL), (16, 16, 24), 1),
     "2d-tog-pU-pchan": (False, "tog", None, ins(P_U, normalizeInputChan="pDiv"), (1, 32, 48), 2),
     "2d-n2-concat-U-skip": (False, "default", banks(2, "concat"), ins(U_ONLY, addPressureSkip=True), (1, 36, 52), 2),
-    "3d-yang-n2-add-norm-divchan": (True, "yang", banks(2, "add", 1, 2), ins(normalizeInputFunc="norm",
+    "3d-yang-n2-add-norm-divchan": (True, "yang", banks(2, "add", s=1, j=2), ins(normalizeInputFunc="norm",
                                                                             normalizeInputChan="div"), (6, 8, 10), 1),
-    "3d-n2-concat-s2j4-all": (True, "default", banks(2, "concat", 2, 4), ins(ALL), (6, 10, 12), 2),
+    "3d-n2-concat-s2j4-all": (True, "default", banks(2, "concat", s=2, j=4), ins(ALL), (6, 10, 12), 2),
 }
 TC = {
     "3d-U-norm": (True, "default", None, ins(U_ONLY, normalizeInputFunc="norm"), (6, 10, 14), 2),
@@ -74,11 +67,11 @@ TC = {
 def run_forward(case, mode):
     orc = oracle.Oracle()
     is3d, model_type, bk, inputs, shape, nb = case
-    batch = make_batch(shape, is3d, nb=nb)
+    batch = plume_batch(shape, is3d, nb=nb)
     mnp = synth.make_model(is3d, model_type=model_type, banks=bk, inputs=inputs)
     p0, inp = inputs_of(batch)
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     if mode != "default":
         gm.set_mode(mode)
     tol = MODE_TOL[gm.get_mode()]
@@ -111,13 +104,13 @@ def test_forward_tensor_core_graph(case, mode):
 def test_scale(func, chan):
     """scale_out against the oracle's per entry, for each function and field; normalizeInput off (chan None): 1."""
     orc = oracle.Oracle()
-    batch = make_batch((6, 8, 10), True, nb=2)
+    batch = plume_batch((6, 8, 10), True, nb=2)
     inputs = ins(ALL, normalizeInputFunc=func, normalizeInputChan=chan or "UDiv", normalizeInput=chan is not None)
     mnp = synth.make_model(True, inputs=inputs)
     p0, inp = inputs_of(batch)
     _, _, want = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
     for mode in ("tf32x3", "fp32"):
-        gm = make_gpu(mnp)
+        gm = fmodel.ProjectionModel.from_model(mnp)
         gm.set_mode(mode)
         gm.forward(inp, return_scale=True)
         if chan is None:
@@ -153,7 +146,7 @@ def create_via(gm, creator, mnp, cin="layers"):
 
 def twin(mnp, creator):
     """The model `creator` builds for mnp's single-bank layers, in a ProjectionModel shell."""
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     rc, h = create_via(gm, creator, mnp)
     gm.ctx.check(rc)
     gm.ctx.lib.tfl_cnn_destroy(gm.ctx.h, gm.h)
@@ -166,10 +159,10 @@ def test_default_block_is_the_banked_model(is3d):
     """Every creator builds the model of tfl_cnn_create_model with the default block: the same bits in every mode.
     Each refuses a channel mismatch with the same message, and a NULL cin as a bad argument."""
     shape = (8, 12, 16) if is3d else (1, 24, 20)
-    batch = make_batch(shape, is3d, nb=2)
+    batch = plume_batch(shape, is3d, nb=2)
     mnp = synth.make_model(is3d, inputs=ins())
     _, inp = inputs_of(batch)
-    a = make_gpu(mnp)
+    a = fmodel.ProjectionModel.from_model(mnp)
     cin = [w.shape[1] for w, _ in mnp["layers"]]
     cin[2] += 1
     for creator in CREATORS:
@@ -212,12 +205,12 @@ def test_padded_input_is_the_oracle_input(ch):
     from fluidnet_b200 import tfluids
     orc = oracle.Oracle()
     nb, shape = 2, (6, 9, 13)
-    batch = make_batch(shape, True, nb=nb)
+    batch = plume_batch(shape, True, nb=nb)
     p0, _ = inputs_of(batch)
     x, _, _, _, scales = model_input(orc, {"inputs": ins(ch)}, p0, batch["UDiv"], batch["flags"])
     U1 = batch["UDiv"].copy()
     orc.setWallBcsForward(U1, batch["flags"], as_mask_multiply=True)
-    gm = make_gpu(synth.make_model(True, inputs=ins(ch)))
+    gm = fmodel.ProjectionModel.from_model(synth.make_model(True, inputs=ins(ch)))
     px, py = layout(nb, *shape)
     out = torch.full((nb, 2, shape[0] + 2, py, px, 4), float(SENTINEL), device="cuda")
     dev = [torch.from_numpy(np.ascontiguousarray(a)).cuda() for a in (p0, U1, batch["flags"])]
@@ -273,14 +266,13 @@ def test_step_and_its_graph():
     from fluidnet_b200 import simulate
     orc = oracle.Oracle()
     n = 24
-    batch = make_batch((n, n, n), True, plume=True)
+    batch = plume_batch((n, n, n), True, inflow=n / 128.0 * 4)
     mnp = synth.make_model(True, inputs=ins(ALL, addPressureSkip=True))
-    gm = make_gpu(mnp)
+    gm = fmodel.ProjectionModel.from_model(mnp)
     assert gm.get_mode() == "tf32x3"
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                 vorticityConfinementAmp=3.0, simMethod="convnet")
-    ga = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
-    gb = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
+    mconf = step_mconf(n)
+    ga = to_gpu(batch)
+    gb = to_gpu(batch)
     simulate.simulate_fused(None, mconf, ga, gm)
     oracle.simulate(orc, mconf, batch, mnp)
     for k in ("density", "UDiv", "pDiv"):
@@ -303,17 +295,17 @@ def test_slab_refuses_a_non_default_block():
     from fluidnet_b200 import simulate, tfluids
     from fluidnet_b200.slab import NativeSlabSimulator
     dev = torch.device("cuda", 0)
-    tb, mconf, _ = _problem(32, 16, 16, None)
+    tb, mconf, _ = banked_problem(32, 16, 16, None)
     single = synth.make_model(True)
     sim = NativeSlabSimulator(tb, mconf, single["layers"], dev, rank=0, world=1)
     ctx, mc = sim.ctx, simulate.make_mconf(mconf)
     for inputs in (ins(ALL), ins(normalizeInputFunc="norm"), ins(addPressureSkip=True)):
-        m = make_gpu(synth.make_model(True, inputs=inputs))
-        assert b"input block" in _refused(ctx, lambda: ctx.lib.tfl_slab_sim_step(ctx.h, sim.h, C.byref(mc), m.h))
+        m = fmodel.ProjectionModel.from_model(synth.make_model(True, inputs=inputs))
+        assert b"input block" in refused(ctx, lambda: ctx.lib.tfl_slab_sim_step(ctx.h, sim.h, C.byref(mc), m.h))
         g = torch.zeros(1, 1, 16, 16, 16, device=dev)
         u = torch.zeros(1, 3, 16, 16, 16, device=dev)
         sums = torch.zeros(2, dtype=torch.float64, device=dev)
-        msg = _refused(ctx, lambda: ctx.lib.tfl_cnn_project_from_sums(
+        msg = refused(ctx, lambda: ctx.lib.tfl_cnn_project_from_sums(
             ctx.h, m.h, tfluids._grid(g), tfluids._grid(u), tfluids._grid(g), C.c_void_p(sums.data_ptr()),
             tfluids._grid(g), tfluids._grid(u), C.c_float(1e-5)))
         assert b"input block" in msg
@@ -332,7 +324,7 @@ def test_unbuildable_blocks_are_refused():
             fmodel.ProjectionModel(layers, True, **kw)
     yang = synth.make_model(True, model_type="yang", inputs=ins(ALL))
     with pytest.raises(TflError, match="yang model must not have UDiv"):
-        make_gpu(yang)
+        fmodel.ProjectionModel.from_model(yang)
     tog = synth.make_model(True, model_type="tog")
     with pytest.raises(TflError, match="addPressureSkip"):
         fmodel.ProjectionModel(tog["layers"], True, pool=tog["pool"], up=tog["up"], addPressureSkip=True)

@@ -40,17 +40,14 @@ import torch
 import oracle
 from fluidnet_b200 import synth
 from fluidnet_b200._lib import TflError
-from network_bound import check, excess, forward_bound, tc_covered
-from test_gpu_cnn_bn import make_gpu
+from fluidnet_b200.model import ProjectionModel
+from network_bound import check, excess, forward_bound, projection_reference, tc_covered
+from scenes import banks, bn_model, plume_batch, step_mconf
 
 pytestmark = pytest.mark.gpu
 
 WW_MAX = 128            # widest row of the z-streaming tensor-core kernel (k_conv3_tc_z)
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "myModel2D_layers.npz")
-
-
-def banks(num, agg, kind="mres", s=1, j=3):
-    return {"num": num, "split_stage": s, "join_stage": j, "aggregate": agg, "type": kind}
 
 
 def make_inputs(shape, is3d, nb, kind, seed=11):
@@ -76,7 +73,7 @@ def kernel_path(model, mode, nx):
 def run_case(what, model, shape, nb, mode, kind="plume"):
     """Forward on the GPU in `mode` and the per-voxel check.  Returns max err / E over p and U."""
     pDiv, U, flags = make_inputs(shape, model["is3D"], nb, kind)
-    gm = make_gpu(model)
+    gm = ProjectionModel.from_model(model)
     assert gm.get_mode() == ("tf32x3" if tc_covered(model) else "fp32"), (what, gm.get_mode())
     gm.set_mode(mode)
     gp, gU = gm.forward(tuple(torch.from_numpy(a).cuda() for a in (pDiv, U, flags)), return_scale=True)
@@ -120,9 +117,9 @@ def test_default_3d(case, mode):
 # Banks: 'mres' 2 and 3 banks concat / add (tensor cores: split 1 / join 3; a later split runs on fp32), 'dilate' on
 # grids 2 and 4 do not divide.
 BANKED = {
-    "mres-n2-concat": (banks(2, "concat"), (8, 12, 20), 2, "random"),
-    "mres-n3-add": (banks(3, "add"), (8, 12, 24), 2, "exotic"),
-    "mres-n3-concat": (banks(3, "concat"), (8, 20, 36), 1, "plume"),
+    "mres-n2-concat": (banks(2, "concat", "mres"), (8, 12, 20), 2, "random"),
+    "mres-n3-add": (banks(3, "add", "mres"), (8, 12, 24), 2, "exotic"),
+    "mres-n3-concat": (banks(3, "concat", "mres"), (8, 20, 36), 1, "plume"),
     "mres-n2-add-s2j4": (banks(2, "add", "mres", 2, 4), (6, 10, 12), 2, "random"),
     "dilate-n2-concat": (banks(2, "concat", "dilate"), (7, 10, 29), 2, "random"),
     "dilate-n3-add": (banks(3, "add", "dilate"), (9, 11, 13), 1, "exotic"),
@@ -135,15 +132,6 @@ def test_banks(case, mode):
     run_case("3d " + case, synth.make_model(True, banks=bk), shape, nb, mode, kind)
 
 
-def bn_model(train, bk=None, relu6=False):
-    m = synth.make_model(True, banks=bk, batch_norm=None if train is None else {"train": train})
-    if relu6:
-        m["nonlinType"] = "relu6"
-        first = m["layers"][0] if not isinstance(m["layers"][0], list) else m["layers"][0][0]
-        first[0][...] *= np.float32(30.0)          # the first stage's values cross 6
-    return m
-
-
 # BN with running and batch statistics: single-bank on the tensor cores (and fp32), banked on fp32; relu6 banked on
 # the tensor cores.
 NORM = {
@@ -151,10 +139,10 @@ NORM = {
     "bn-running": (lambda: bn_model(False), (8, 10, 12), 2),
     "bn-batch-relu6": (lambda: bn_model(True, relu6=True), (6, 9, 130), 1),
     "bn-running-relu6": (lambda: bn_model(False, relu6=True), (7, 9, 31), 2),
-    "bn-batch-mres-n2-concat": (lambda: bn_model(True, banks(2, "concat")), (8, 12, 16), 2),
-    "bn-running-dilate-n2-add": (lambda: bn_model(False, banks(2, "add", "dilate")), (7, 10, 13), 2),
-    "relu6-mres-n2-concat": (lambda: bn_model(None, banks(2, "concat"), relu6=True), (8, 12, 16), 2),
-    "relu6-dilate-n3-add": (lambda: bn_model(None, banks(3, "add", "dilate"), relu6=True), (7, 9, 11), 1),
+    "bn-batch-mres-n2-concat": (lambda: bn_model(True, bk=banks(2, "concat", "mres")), (8, 12, 16), 2),
+    "bn-running-dilate-n2-add": (lambda: bn_model(False, bk=banks(2, "add", "dilate")), (7, 10, 13), 2),
+    "relu6-mres-n2-concat": (lambda: bn_model(None, bk=banks(2, "concat", "mres"), relu6=True), (8, 12, 16), 2),
+    "relu6-dilate-n3-add": (lambda: bn_model(None, bk=banks(3, "add", "dilate"), relu6=True), (7, 9, 11), 1),
 }
 
 
@@ -210,7 +198,7 @@ def test_tf32_fails_the_3xtf32_bound():
     """Non-vacuity: the TF32 mode's output at 64^3 on the signed random field exceeds the 3xTF32 bound."""
     model = synth.make_model(True)
     pDiv, U, flags = make_inputs((64, 64, 64), True, 1, "random")
-    gm = make_gpu(model)
+    gm = ProjectionModel.from_model(model)
     gm.set_mode("tf32")
     gp, gU = gm.forward(tuple(torch.from_numpy(a).cuda() for a in (pDiv, U, flags)), return_scale=True)
     ref = forward_bound(oracle.Oracle(), model, pDiv, U, flags, "tf32x3", scale=gm.last_scale)
@@ -229,7 +217,7 @@ UNCOVERED = {c: make for c, make in UNCOVERED.items() if not tc_covered(make())}
 def test_tensor_core_modes_refused(case):
     """The graphs the cases above run in fp32 only: the model starts in fp32 and set_mode refuses both tensor-core
     modes."""
-    gm = make_gpu(UNCOVERED[case]())
+    gm = ProjectionModel.from_model(UNCOVERED[case]())
     assert gm.get_mode() == "fp32"
     for mode in ("tf32x3", "tf32"):
         with pytest.raises(TflError):
@@ -242,35 +230,9 @@ def test_tensor_core_modes_refused(case):
 # ---------------------------------------------------------------------------------------------------------------
 def step_problem(n, seed=21):
     """A plume problem at n^3 with a small signed pDiv (the network's pDiv channel), and its mconf."""
-    flags = synth.make_flags(n, n, n, True, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0, seed=seed)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    pDiv = ((np.random.RandomState(seed).rand(*flags.shape) - 0.5) * 0.2).astype(np.float32)
-    batch = {"pDiv": pDiv, "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], n / 128.0 * 4, 0.15)
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                 vorticityConfinementAmp=3.0, simMethod="convnet")
-    return batch, mconf
-
-
-def projection_reference(state, mconf, gm, mnp):
-    """The float64 projection of one step from `state` (GPU tensors, left as they are) on the scale interval: the
-    operator sequence up to the projection and setConstVals, forward_bound, then the U BCs (x inv + bc: E |inv| plus
-    two roundings) and the +-1e6 clamp (1-Lipschitz)."""
-    from fluidnet_b200 import simulate
-    from network_bound import gamma
-    ob = {k: v.clone() for k, v in state.items()}
-    simulate.simulate(None, mconf, ob, gm, outputDiv=True)
-    p, U, flags, density = simulate.getPUFlagsDensityReference(ob)
-    simulate.setConstVals(ob, p, U, flags, density)
-    assert ob.get("pBC") is None, "a pressure BC takes the operator path, not these cases"
-    ref = forward_bound(oracle.Oracle(), mnp, p.cpu().numpy(), U.cpu().numpy(), flags.cpu().numpy(), gm.get_mode(),
-                        scale=None, threshold=gm.threshold)
-    inv, bc = ob["UBCInvMask"].cpu().numpy().astype(np.float64), ob["UBC"].cpu().numpy().astype(np.float64)
-    Ui = ref["U"] * inv
-    ref["EU"] = ref["EU"] * np.abs(inv) + gamma(2) * (np.abs(Ui) + ref["EU"] * np.abs(inv) + np.abs(bc))
-    ref["U"] = np.clip(Ui + bc, -1e6, 1e6)
-    return ref
+    batch = plume_batch(n, seed=seed, inflow=n / 128.0 * 4)
+    batch["pDiv"] = ((np.random.RandomState(seed).rand(*batch["flags"].shape) - 0.5) * 0.2).astype(np.float32)
+    return batch, step_mconf(n)
 
 
 def check_step(what, p, U, ref):
@@ -285,10 +247,10 @@ def test_fused_step(n):
     """One tfl_simulate_step in 3xTF32 (the fused path: k_vort_bc_mask's statistics, k_cnn_inputs_fused, the
     tensor-core stack, k_cnn_finish_fused)."""
     from fluidnet_b200 import simulate
-    from test_gpu_step_paths import takes_fused_path
+    from step_cases import takes_fused_path
     batch, mconf = step_problem(n)
     mnp = synth.make_model(True)
-    gm = make_gpu(mnp)
+    gm = ProjectionModel.from_model(mnp)
     assert gm.get_mode() == "tf32x3" and takes_fused_path({"mode": gm.get_mode(), "nb": 1, "pbc": False})
     gb = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
     state = {k: v.clone() for k, v in gb.items()}
@@ -302,7 +264,7 @@ def test_fused_step_graph_replay():
     from fluidnet_b200 import simulate
     batch, mconf = step_problem(64, seed=23)
     mnp = synth.make_model(True)
-    gm = make_gpu(mnp)
+    gm = ProjectionModel.from_model(mnp)
     g = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
     stream = torch.cuda.Stream()
     torch.cuda.synchronize()
@@ -325,8 +287,7 @@ def test_emulated_slabs(world):
     test_emulated_slabs_on_one_gpu): each rank's projection (tfl_cnn_project_from_sums on the all-reduced sums) within
     the bound on its owned planes."""
     from fluidnet_b200.slab import SlabSimulator, run_lockstep
-    from test_gpu_slab import _problem
-    batch, mconf, mnp = _problem(48)
+    batch, mconf, mnp = plume_batch(48, inflow=48 / 128.0 * 4), step_mconf(48), synth.make_model(True)
     tb = {k: torch.from_numpy(v) for k, v in batch.items()}
     sims = [SlabSimulator(tb, mconf, mnp["layers"], torch.device("cuda", 0), rank=r, world=world)
             for r in range(world)]

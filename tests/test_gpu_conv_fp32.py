@@ -47,55 +47,23 @@ to gamma_n; the long sums stay far below it.
 """
 import ctypes as C
 import os
-import zlib
 
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+from fp32_conv import (DIRECT, GENERIC, SIGMOID_ULPS, activate, check_guards, gamma, guarded, make_conv,
+                       quantised_batch, run_conv, seed_of, shuffle_model)
+from fp32_conv import GUARD, SENTINEL, debug_lib as debug_lib
 from network_bound import conv_f64
+from scenes import banks
 
-U_ROUND = 2.0 ** -24
-SIGMOID_ULPS = 2.0 ** -20
-SENTINEL = 0x7FC0BEEF                 # a NaN payload that no kernel produces from finite inputs
-GUARD = 1024                          # floats before and after the output that must keep the sentinel
-DIRECT, GENERIC = 1, 2                # what tfl_debug_conv_fp32 reports
 INPUTS = ("exact", "signed", "nonneg")
 # The (cout, k) instantiations of k_conv_direct (launch_conv_direct), each in 2-D and 3-D.
 INSTANCES = [(8, 3), (8, 1), (1, 1), (16, 3), (16, 1), (1, 3), (6, 3), (6, 1), (32, 1), (16, 5), (32, 5), (64, 5),
              (64, 1)]
 GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "myModel2D_layers.npz")
-
-
-def gamma(n):
-    return n * U_ROUND / (1.0 - n * U_ROUND)
-
-
-def make_conv(inputs, cin, cout, k, is3d, shape, nb, seed):
-    """x [nb][cin][nz][ny][nx], w [cout][cin][kz][k][k], b [cout] in float32 (module docstring)."""
-    rs = np.random.RandomState(seed)
-    kz = k if is3d else 1
-    xs, ws = (nb, cin) + tuple(shape), (cout, cin, kz, k, k)
-    if inputs == "exact":
-        x = rs.randint(-8, 9, xs) * 2.0 ** -2
-        w = rs.randint(-16, 17, ws) * 2.0 ** -4
-        b = rs.randint(-64, 65, cout) * 2.0 ** -6
-    else:
-        lo = 0.0 if inputs == "nonneg" else -1.0
-        bw = 1.0 / np.sqrt(cin * kz * k * k)
-        x = rs.uniform(lo, 1.0, xs)
-        w = rs.uniform(lo * bw, bw, ws)
-        b = rs.uniform(lo * bw, bw, cout)
-    return tuple(np.ascontiguousarray(a, np.float32) for a in (x, w, b))
-
-
-def activate(v, act):
-    if act == 1:
-        return np.maximum(v, 0.0)
-    if act == 2:
-        return 1.0 / (1.0 + np.exp(-v))
-    return v
 
 
 def reference(x, w, b, act, exact):
@@ -106,48 +74,6 @@ def reference(x, w, b, act, exact):
     E = np.zeros_like(S) if exact else gamma(n) * S
     ref = activate(pre, act)
     return ref, (E / 4 + SIGMOID_ULPS * ref if act == 2 else E)
-
-
-def _hook():
-    from fluidnet_b200 import tfluids
-    lib = tfluids.context().lib
-    lib.tfl_debug_conv_fp32.argtypes = [C.c_void_p] * 5 + [C.c_int] * 10 + [C.POINTER(C.c_int32)]
-    lib.tfl_debug_pool.argtypes = [C.c_void_p] * 3 + [C.c_int] * 7
-    lib.tfl_debug_pixel_shuffle.argtypes = [C.c_void_p] * 3 + [C.c_int] * 7
-    lib.tfl_debug_bank_join.argtypes = [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p] + [C.c_int] * 7
-    return lib
-
-
-def guarded(n):
-    """A device buffer of n floats between two guards, all holding the sentinel: (whole buffer, output view)."""
-    buf = torch.full((GUARD + n + GUARD,), SENTINEL, dtype=torch.int32, device="cuda").view(torch.float32)
-    return buf, buf[GUARD:GUARD + n]
-
-
-def check_guards(buf, n, what):
-    a = buf.cpu().numpy().view(np.uint32)
-    outside = np.concatenate([a[:GUARD], a[GUARD + n:]])
-    assert (outside == SENTINEL).all(), "%s: %d stray writes around the output" % (what, (outside != SENTINEL).sum())
-    inside = a[GUARD:GUARD + n]
-    assert not (inside == SENTINEL).any(), "%s: %d output values not written" % (what, (inside == SENTINEL).sum())
-    return inside.view(np.float32)
-
-
-def run_conv(x, w, b, act, is3d, generic, what):
-    """One convolution on the GPU.  Returns (out [nb][cout][nz][ny][nx], the kernel that ran)."""
-    from fluidnet_b200 import tfluids
-    lib = _hook()
-    nb, cin, nz, ny, nx = x.shape
-    cout, k = w.shape[0], w.shape[4]
-    n = nb * cout * nz * ny * nx
-    din = torch.from_numpy(x).cuda()
-    buf, out = guarded(n)
-    kernel = C.c_int32(0)
-    ctx = tfluids._ctx_for(din)
-    ctx.check(lib.tfl_debug_conv_fp32(ctx.h, din.data_ptr(), out.data_ptr(), w.ctypes.data, b.ctypes.data, cin, cout,
-                                      k, act, int(is3d), nb, nz, ny, nx, generic, C.byref(kernel)))
-    assert np.array_equal(din.cpu().numpy().view(np.uint32), x.view(np.uint32)), "%s: wrote its input" % what
-    return check_guards(buf, n, what).reshape(nb, cout, nz, ny, nx), kernel.value
 
 
 def check_conv(what, x, w, b, act, is3d, inputs, kernel, ref=None):
@@ -170,10 +96,6 @@ def check_conv(what, x, w, b, act, is3d, inputs, kernel, ref=None):
     diff = gen.view(np.uint32) != got.view(np.uint32)
     assert not diff.any(), "%s: generic and direct differ at %d values, first %s" % (what, diff.sum(), np.argwhere(diff)[0])
     return got
-
-
-def seed_of(what):
-    return zlib.crc32(what.encode())
 
 
 @pytest.mark.gpu
@@ -305,7 +227,7 @@ def test_shipped_model_layer_by_layer():
 def test_conv_hook_rejects_bad_arguments():
     from fluidnet_b200 import tfluids
     from fluidnet_b200._lib import TflError
-    lib = _hook()
+    lib = debug_lib()
     x, w, b = make_conv("signed", 3, 8, 3, True, (2, 2, 2), 1, 0)
     d = torch.zeros(64, device="cuda")
     ctx = tfluids._ctx_for(d)
@@ -357,7 +279,7 @@ def pool_emulation(x, p, is3d, is_max):
 @pytest.mark.parametrize("kind", ["avg", "max"])
 def test_pool_bit_exact(kind, p, is3d, nbc):
     from fluidnet_b200 import tfluids
-    lib = _hook()
+    lib = debug_lib()
     nz, ny, nx = (3 * p if is3d else 1), 5 * p, 7 * p
     x = np.random.RandomState(seed_of("pool%s%d%d%d" % (kind, p, is3d, nbc))).standard_normal(
         (nbc, nz, ny, nx)).astype(np.float32)
@@ -388,7 +310,7 @@ def shuffle_reference(x, n_out, s, is3d):
 @pytest.mark.parametrize("s", [2, 3])
 def test_pixel_shuffle_bit_exact(s, is3d, nb, n_out):
     from fluidnet_b200 import tfluids
-    lib = _hook()
+    lib = debug_lib()
     st = s if is3d else 1
     nz, ny, nx = (3 if is3d else 1), 5, 7
     x = np.random.RandomState(seed_of("shuffle%d%d%d%d" % (s, is3d, nb, n_out))).standard_normal(
@@ -416,7 +338,7 @@ def join_grid(nbanks, is3d):
 
 def run_join(bank_list, agg, out_init, is3d, nbanks=None):
     from fluidnet_b200 import tfluids
-    lib = _hook()
+    lib = debug_lib()
     nbanks = len(bank_list) if nbanks is None else nbanks
     nb, c = bank_list[0].shape[:2]
     nz, ny, nx = bank_list[0].shape[2:]
@@ -480,10 +402,6 @@ def test_bank_join_refuses_bank_counts(nbanks):
 # the graph executor keeps batch entries apart
 # ---------------------------------------------------------------------------------------------------------------
 
-def banks(num, agg, s=1, j=3):
-    return {"num": num, "split_stage": s, "join_stage": j, "aggregate": agg}
-
-
 # (is3d, model_type, poolType, banks, (nz, ny, nx)); every model runs in fp32 mode.
 GRAPHS = {
     "2d-default": (False, "default", "avg", None, (1, 20, 24)),
@@ -496,45 +414,18 @@ GRAPHS = {
     "3d-yang": (True, "yang", "avg", None, (6, 10, 12)),
     "3d-default-n2-concat": (True, "default", "avg", banks(2, "concat"), (8, 12, 16)),
     "3d-default-n3-add": (True, "default", "avg", banks(3, "add"), (8, 12, 16)),
-    "3d-default-n2-concat-s2j4": (True, "default", "avg", banks(2, "concat", 2, 4), (6, 10, 12)),
-    "3d-default-n2-add-s2j4": (True, "default", "avg", banks(2, "add", 2, 4), (6, 10, 12)),
-    "3d-yang-n2-add-s1j2": (True, "yang", "avg", banks(2, "add", 1, 2), (6, 8, 10)),
-    "3d-yang-n2-concat-s1j2": (True, "yang", "avg", banks(2, "concat", 1, 2), (6, 8, 10)),
+    "3d-default-n2-concat-s2j4": (True, "default", "avg", banks(2, "concat", s=2, j=4), (6, 10, 12)),
+    "3d-default-n2-add-s2j4": (True, "default", "avg", banks(2, "add", s=2, j=4), (6, 10, 12)),
+    "3d-yang-n2-add-s1j2": (True, "yang", "avg", banks(2, "add", s=1, j=2), (6, 8, 10)),
+    "3d-yang-n2-concat-s1j2": (True, "yang", "avg", banks(2, "concat", s=1, j=2), (6, 8, 10)),
     "2d-default-n3-concat": (False, "default", "avg", banks(3, "concat"), (1, 24, 20)),
     "2d-tog-n2-concat": (False, "tog", "avg", banks(2, "concat"), (1, 32, 48)),
     "2d-tog-n2-add": (False, "tog", "max", banks(2, "add"), (1, 32, 48)),
     # bank 1's last stage pools (split 1, join 2) / pixel-shuffles (shuffle_model) one entry at a time
-    "2d-tog-n2-concat-s1j2": (False, "tog", "avg", banks(2, "concat", 1, 2), (1, 32, 48)),
-    "3d-shuffle-n2-concat-s2j3": (True, "shuffle", "avg", banks(2, "concat", 2, 3), (8, 12, 16)),
-    "2d-shuffle-n3-concat-s2j3": (False, "shuffle", "max", banks(3, "concat", 2, 3), (1, 24, 32)),
+    "2d-tog-n2-concat-s1j2": (False, "tog", "avg", banks(2, "concat", s=1, j=2), (1, 32, 48)),
+    "3d-shuffle-n2-concat-s2j3": (True, "shuffle", "avg", banks(2, "concat", s=2, j=3), (8, 12, 16)),
+    "2d-shuffle-n3-concat-s2j3": (False, "shuffle", "max", banks(3, "concat", s=2, j=3), (1, 24, 32)),
 }
-
-
-def shuffle_model(is3d, nbanks, seed=4321):
-    """A graph whose last banked stage ends in a pixel shuffle (no stock graph has one before its join): 3 -> 8 (k 3,
-    pool 2), 8 -> 8 (k 1, up 2; one per bank), 8 nbanks -> 8 (k 3, the 'concat' join), 8 -> 1 (k 1)."""
-    rs = np.random.RandomState(seed)
-    kz = lambda k: k if is3d else 1
-    fan = 8 if is3d else 4
-
-    def conv(cout, cin, k):
-        bound = 1.0 / np.sqrt(cin * kz(k) * k * k)
-        w = ((rs.rand(cout, cin, kz(k), k, k) * 2 - 1) * bound).astype(np.float32)
-        return w, ((rs.rand(cout) * 2 - 1) * bound).astype(np.float32)
-
-    layers = [conv(8, 3, 3), [conv(8 * fan, 8, 1) for _ in range(nbanks)], conv(8, 8 * nbanks, 3), conv(1, 8, 1)]
-    return {"is3D": is3d, "layers": layers, "pool": [2, 1, 1, 1], "up": [1, 2, 1, 1]}
-
-
-def quantised_batch(shape, is3d, nb, seed):
-    """flags with Empty / Outflow / Stick cells that differ per entry, U and pDiv on multiples of 2^-8."""
-    from fluidnet_b200 import synth
-    nz, ny, nx = shape
-    flags = synth.make_flags(nx, ny, nz, is3d, nb=nb, geometry=True, exotic=True, seed=seed)
-    U = synth.make_smooth_velocity(flags, is3d, amp=3.0, seed=seed)
-    p = synth.make_density(flags, seed=seed + 1) - np.float32(0.5)
-    q = lambda a: np.ascontiguousarray(np.round(a * 256.0) / 256.0, np.float32)
-    return q(p), q(U), flags
 
 
 @pytest.mark.gpu

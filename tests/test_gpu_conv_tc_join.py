@@ -15,7 +15,7 @@ import numpy as np
 import pytest
 import torch
 
-from test_gpu_conv_tc import KAPPA, SENTINEL, TAIL_ULPS, conv_f64, is_sentinel, layout, pack
+from tc_conv import KAPPA, SENTINEL, is_sentinel, join_reference, layout, pack
 
 pytestmark = pytest.mark.gpu
 
@@ -24,30 +24,6 @@ pytestmark = pytest.mark.gpu
 # a coarsest bank of 1x1x1, batch of three.
 SHAPES = [((10, 8, 60), 1, 2), ((12, 18, 58), 2, 2), ((4, 6, 62), 1, 2), ((8, 20, 120), 1, 3),
           ((4, 4, 4), 2, 3), ((8, 12, 16), 3, 2), ((12, 8, 24), 1, 3)]
-
-
-def up(x, r):
-    return np.repeat(np.repeat(np.repeat(x, r, axis=2), r, axis=3), r, axis=4)
-
-
-def reference(banks, agg, w, b, tail, kappa):
-    ups = [up(x.astype(np.float64), 2 ** i) for i, x in enumerate(banks)]
-    if agg == "concat":
-        x, xa = np.concatenate(ups, axis=1), np.abs(np.concatenate(ups, axis=1))
-    else:
-        x, xa = sum(ups[1:], ups[0]), sum((np.abs(u) for u in ups[1:]), np.abs(ups[0]))
-    pre = conv_f64(x, w, b)
-    S = conv_f64(xa, np.abs(w), np.abs(b))
-    h, Eh = np.maximum(pre, 0.0), kappa * S
-    t = tail.astype(np.float64)
-    w4, b4, w5, b5 = t[:64].reshape(8, 8), t[64:72], t[72:80], t[80]
-    mix = lambda m, v: np.einsum("oc,bczyx->bozyx", m, v)
-    a = np.maximum(mix(w4, h) + b4[:, None, None, None], 0.0)
-    Ea = mix(np.abs(w4), Eh) + TAIL_ULPS * (mix(np.abs(w4), np.abs(h) + Eh) + np.abs(b4)[:, None, None, None])
-    p = np.einsum("o,bozyx->bzyx", w5, a) + b5
-    Ep = (np.einsum("o,bozyx->bzyx", np.abs(w5), Ea)
-          + TAIL_ULPS * (np.einsum("o,bozyx->bzyx", np.abs(w5), a + Ea) + abs(b5)))
-    return p, Ep
 
 
 def run_join(banks, agg, w, b, tail, split, full):
@@ -98,7 +74,7 @@ def test_join_matches_float64(split, agg, case):
     missed = is_sentinel(got)
     assert not missed.any(), "%s: %d voxels not written" % (what, missed.sum())
     assert np.isfinite(got).all(), "%s: non-finite output (a NaN pad column was read)" % what
-    ref, bound = reference(banks, agg, w, b, tail, KAPPA[split])
+    ref, bound = join_reference(banks, agg, w, b, tail, KAPPA[split])
     err = np.abs(got.astype(np.float64) - ref)
     ratio = err / np.maximum(bound, 1e-300)
     print("%s: max err / bound %.3f" % (what, ratio.max()))

@@ -13,8 +13,7 @@ import ctypes as C
 import numpy as np
 import pytest
 
-from test_gpu_conv_tc import LAYERS, make_layer, run_layer
-from test_gpu_conv_tc_zstream import TY, nsm, schedule
+from tc_conv import LAYERS, TY, make_layer, nsm, run_layer, schedule
 
 CAPS = [1, 2, 7]
 # (nz, ny, nx), nb, (z_lo, z_hi) or None for all planes

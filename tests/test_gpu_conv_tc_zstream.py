@@ -9,32 +9,10 @@ kernel); row counts one short of and one past a row block; z chunks of more than
 last chunk; batch entries in one launch; and more items than CTAs.  `schedule` restates the host's choice
 of ZC so that each case can assert the edge it is meant to reach."""
 import pytest
-import torch
 
-from test_gpu_conv_tc import LAYERS, check_layer, make_layer
+from tc_conv import LAYERS, TY, check_layer, make_layer, nsm, schedule
 
 SPLITS = [1, 0]
-TY = {1: 4, 0: 8}
-WW_MAX = 128
-
-
-def schedule(nb, ny, nx, z_lo, z_hi, split, nsm):
-    """(zc, nzc, items) of k_conv3_tc_z: ZC minimises rounds x (ZC + 2), ties to the larger ZC."""
-    assert nx <= WW_MAX
-    cols = nb * -(-ny // TY[split])
-    nzo = z_hi - z_lo
-    best = None
-    for zc in range(1, nzo + 1):
-        items = cols * -(-nzo // zc)
-        grid = min(items, nsm)
-        cost = -(-items // grid) * (zc + 2)
-        if best is None or cost <= best[0]:
-            best = (cost, zc, -(-nzo // zc), items)
-    return best[1:]
-
-
-def nsm():
-    return torch.cuda.get_device_properties(0).multi_processor_count
 
 
 @pytest.mark.gpu

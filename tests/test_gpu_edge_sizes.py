@@ -33,8 +33,8 @@ import oracle
 from cases import bits_equal, describe_diff
 from edge_cases import CASES, CASE_IDS, DT, STRENGTH
 from fluidnet_b200 import synth
-from test_gpu_step_paths import (MODE_TOL, OPS_TOL, case, close_per_entry, make_batch, quad_dims, same_zero_bits,
-                                 takes_fused_path)
+from step_cases import (Guards, MODE_TOL, OPS_TOL, case, close_per_entry, ctx, fill, make_batch, plane_of, quad_dims,
+                        run, same_zero_bits, set_tile_mode, takes_fused_path)
 
 METHODS = list(oracle.ADVECT_METHODS)
 OURS_VEL = {"maccormackOurs", "rk2Ours", "rk3Ours"}       # advectVel methods the tile kernel runs
@@ -66,8 +66,6 @@ ROWS = {
     (1028, 3, 1): "2-D long row, k_jacobi_iter4",
     (3, 600, 1): "2-D per-voxel kernels, very tall",
 }
-
-SENTINEL = 0x7FC5A5A5          # a quiet NaN with a payload
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -178,62 +176,6 @@ def test_table_reaches_every_branch():
 # ---------------------------------------------------------------------------------------------------------------
 # Guarded device copies
 # ---------------------------------------------------------------------------------------------------------------
-class Guards:
-    """Device views of host arrays, each inside its own buffer with `g` sentinel words on either side."""
-
-    def __init__(self, plane):
-        self.g = (max(plane, 64) + 3) // 4 * 4
-        self.bufs = []
-
-    def put(self, a):
-        a = np.ascontiguousarray(a, np.float32)
-        buf = torch.empty(2 * self.g + a.size, dtype=torch.float32, device="cuda")
-        buf.view(torch.int32).fill_(SENTINEL)
-        v = buf[self.g:self.g + a.size].view(a.shape)
-        v.copy_(torch.from_numpy(a))
-        assert v.data_ptr() % 16 == 0 and v.is_contiguous()
-        self.bufs.append((buf, a.size))
-        return v
-
-    def check(self, what):
-        for i, (buf, n) in enumerate(self.bufs):
-            bits = buf.view(torch.int32)
-            assert bool((bits[:self.g] == SENTINEL).all()), "%s: array %d written before its start" % (what, i)
-            assert bool((bits[self.g + n:] == SENTINEL).all()), "%s: array %d written past its end" % (what, i)
-
-
-def ctx():
-    from fluidnet_b200 import tfluids
-    return tfluids.context()
-
-
-def run(what, plane, fn, *arrays):
-    """fn(*views) on guarded device copies of `arrays`; returns (host copies of the views, fn's value, launches)."""
-    gd = Guards(plane)
-    views = [gd.put(a) for a in arrays]
-    c = ctx()
-    c.trace_faults()
-    l0 = c.launch_count()
-    ret = fn(*views)
-    torch.cuda.synchronize()
-    launches = c.launch_count() - l0
-    gd.check(what)
-    assert c.trace_faults() == 0, "%s: trace faults" % what
-    return [v.cpu().numpy() for v in views], ret, launches
-
-
-def set_tile_mode(mode):
-    c = ctx()
-    c.lib.tfl_debug_advect_tile.argtypes = [C.c_void_p, C.c_int]
-    assert c.lib.tfl_debug_advect_tile(c.h, -1 if mode is None else mode) == 0
-
-
-def plane_of(fl):
-    return fl.shape[-1] * fl.shape[-2]
-
-
-def fill(shape, v=123.0):
-    return np.full(shape, v, np.float32)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -449,11 +391,11 @@ def test_step_fused_and_ops(orc, shape):
     two steps each, against the oracle (density bit for bit, U and p within MODE_TOL) and against the operator
     sequence (within OPS_TOL with the same zeros)."""
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     nx, ny, nz = shape
     mnp = synth.make_model(True)
     for nb, mode in STEP_LEGS:
-        gm = make_gpu_model(mnp)
+        gm = ProjectionModel.from_model(mnp)
         gm.set_mode(mode)
         c = case((nz, ny, nx), nb=nb, flags="empty", state="density", mode=mode)
         batch = make_batch(orc, c)
@@ -505,14 +447,14 @@ def test_step_jacobi(orc, shape):
 @pytest.mark.parametrize("shape", [(3, 3), (3, 41)], ids=["3x3", "3x41"])
 def test_step_2d_fp32_model(orc, shape):
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     nx, ny = shape
     flags = synth.make_flags(nx, ny, 1, False)
     U = synth.make_smooth_velocity(flags, False, amp=3.0)
     orc.setWallBcsForward(U, flags)
     batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
     mnp = synth.make_model(False)
-    gm = make_gpu_model(mnp)
+    gm = ProjectionModel.from_model(mnp)
     mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=1.0, vorticityConfinementAmp=0.0,
                                  simMethod="convnet", is3D=False)
     gd = Guards(nx * ny)
@@ -533,10 +475,10 @@ def test_step_2d_fp32_model(orc, shape):
 def test_step_graph_replay_on_a_tiny_grid(orc):
     """A step graph captured at 4x3x3 replays the direct step bit for bit."""
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     c = case((3, 3, 4), flags="empty", state="density")
     batch = make_batch(orc, c)
-    gm = make_gpu_model(synth.make_model(True))
+    gm = ProjectionModel.from_model(synth.make_model(True))
     gd = Guards(12)
     ga, gb = guarded_batch(batch, gd), guarded_batch(batch, gd)
     stream = torch.cuda.Stream()

@@ -35,7 +35,7 @@ def gpu():
 
 @pytest.fixture
 def contexts():
-    from test_gpu_step_paths import Contexts
+    from step_cases import Contexts
     cs = Contexts()
     try:
         yield cs

@@ -10,6 +10,7 @@ import torch
 
 import oracle
 from fluidnet_b200 import _lib, simulate, synth, tfluids
+from scenes import plume_batch, step_mconf
 
 pytestmark = pytest.mark.gpu
 
@@ -20,18 +21,8 @@ def _ok(lib, ctx, rc, what):
     assert rc == 0, "%s: %s" % (what, lib.tfl_last_error(ctx).decode())
 
 
-def _problem():
-    flags = synth.make_flags(N, N, N, True, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], N / 128.0, 0.15)
-    return batch
-
-
 def _mconf(sim_method):
-    return simulate.make_mconf(oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * N / 128,
-                                                    vorticityConfinementAmp=3.0, simMethod=sim_method, maxIter=20))
+    return simulate.make_mconf(step_mconf(N, simMethod=sim_method, maxIter=20))
 
 
 def test_host_sim_refuses_bad_grids():
@@ -147,7 +138,7 @@ def test_repeated_create_use_destroy_gives_the_same_bits():
     """Five cycles of context, PCG solve, model, host-buffer steps, step graph and z-slab step, each torn down in
     another order with the context last: every call succeeds and the last cycle computes the first one's bits."""
     lib = _lib.load()
-    batch = _problem()
+    batch = plume_batch(N, inflow=N / 128.0)
     layers = synth.make_model(True)["layers"]
     orders = [("model", "host", "graph", "slab"), ("slab", "graph", "host", "model"), ("graph", "model", "slab", "host"),
               ("host", "slab", "model", "graph"), ("model", "graph", "slab", "host")]

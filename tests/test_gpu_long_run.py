@@ -48,7 +48,7 @@ def traj2d():
 
 @pytest.fixture
 def contexts():
-    from test_gpu_step_paths import Contexts
+    from step_cases import Contexts
     cs = Contexts()
     try:
         yield cs
@@ -112,7 +112,7 @@ def run_direct(traj, ctx, what, is3d=True, fused=True, on_step=None):
 def auto_halos(traj3d):
     """Run (a): the automatic tile halo on a fresh context.  Returns {step: (velocity halo, scalar halo, longest
     trace reported after the step)}."""
-    from test_gpu_step_paths import Contexts
+    from step_cases import Contexts
     cs = Contexts()
     try:
         ctx = fresh(cs)

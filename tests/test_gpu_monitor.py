@@ -9,11 +9,12 @@ import pytest
 import torch
 import torch.multiprocessing as mp
 
+import monitor_reference as ref
 import oracle
 from fluidnet_b200 import monitor, scene, simulate, synth, tfluids
 from fluidnet_b200._lib import TflError
 from fluidnet_b200.model import ProjectionModel
-import monitor_reference as ref
+from scenes import plume_batch, step_mconf
 
 pytestmark = pytest.mark.gpu
 
@@ -70,14 +71,7 @@ def test_nan_propagates_into_every_maximum():
 
 
 def _plume(n, sim_method):
-    flags = synth.make_flags(n, n, n, True, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], n / 128.0, 0.15)
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                 vorticityConfinementAmp=3.0, simMethod=sim_method, maxIter=34)
-    return batch, mconf
+    return plume_batch(n, inflow=n / 128.0), step_mconf(n, simMethod=sim_method, maxIter=34)
 
 
 def _run_path(batch_np, mconf, model, steps, graph):
@@ -197,7 +191,7 @@ FRAME_STEPS = 12
 
 
 def _slab_problem(kind):
-    from test_gpu_slab_jacobi import _problem as jacobi_problem
+    from slab_cases import jacobi_problem
     tb, mconf = jacobi_problem(48, 48, 48, max_iter=34)
     if kind == "convnet":
         mconf = dict(mconf, simMethod="convnet")
@@ -206,10 +200,10 @@ def _slab_problem(kind):
 
 def _slab_worker(rank, world, kinds, q, qd, inboxes, barrier):
     try:
-        from test_gpu_slab_ranks import _Comm
+        from slab_cases import Comm
         from fluidnet_b200.slab import NativeSlabSimulator
         torch.cuda.set_device(0)
-        comm = _Comm(rank, world, inboxes)
+        comm = Comm(rank, world, inboxes)
         wait = lambda: barrier.wait(TIMEOUT_S)       # noqa: E731
         faults = 0
         for kind in kinds:
@@ -298,7 +292,7 @@ def test_slab_records_equal_the_whole_grid_monitor_at_one_rank():
 def test_slab_records_over_processes_sharing_one_gpu(world):
     """'jacobi': the combined records equal the single-GPU whole-grid monitor bit for bit, every step.  'convnet' (world
     2): they equal the monitor of that run's gathered fields."""
-    from test_gpu_slab_record import _collect
+    from slab_cases import collect
     kinds = ["jacobi", "convnet"] if world == 2 else ["jacobi"]
     tb, mconf = _slab_problem("jacobi")
     allw = _whole_grid_records(tb, mconf, SLAB_STEPS + FRAME_STEPS)
@@ -314,7 +308,7 @@ def test_slab_records_over_processes_sharing_one_gpu(world):
     while len(got) < (len(kinds) * SLAB_STEPS + 1) * world:
         kind, step, rank, idx, rec, z0, z1, U = qd.get(timeout=TIMEOUT_S)
         got[(kind, step, rank)] = (idx, rec, z0, z1, U)
-    res = _collect(procs, q, TIMEOUT_S)
+    res = collect(procs, q, TIMEOUT_S)
     assert len(res) == world and all(r[1] == "ok" for r in res), res
     assert sum(r[2] for r in res) == 0, "trace faults: %r" % res
     orc = oracle.Oracle()

@@ -30,7 +30,7 @@ KEYS = ("pDiv", "UDiv", "density")
 
 @pytest.fixture
 def contexts():
-    from test_gpu_step_paths import Contexts
+    from step_cases import Contexts
     cs = Contexts()
     try:
         cs.use(cs.new())

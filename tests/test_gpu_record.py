@@ -218,7 +218,7 @@ def plain_loop(res, sim_method, model, voxels, frames, decimation, path):
 @pytest.mark.parametrize("which,sim_method", [("plume", "convnet"), ("arch", "convnet"), ("plume", "jacobi"),
                                               ("bunny", "pcg")])
 def test_scene_files_equal_a_plain_loop(which, sim_method, net, tmp_path, orc):
-    from test_scene import write_binvox
+    from scenes import write_binvox
     res, frames = 32, 9
     binvox = None
     if which != "plume":

@@ -2,99 +2,13 @@
 domain split across 2 ranks (NCCL halo exchange + 2-double all-reduce) equal the single-GPU run.
 Advection / forces are bit-exact; the only reduction whose order changes is the input scale of the
 network (sum of two partial sums instead of one), hence 1e-6 * max|field|."""
-import os
-import socket
-
-import numpy as np
 import pytest
 import torch
-import torch.distributed as dist
 import torch.multiprocessing as mp
 
+from slab_cases import collect, convnet_problem, free_port, slab_worker
+
 pytestmark = pytest.mark.gpu
-
-
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
-def _collect(procs, q, timeout_s):
-    """Results of all ranks; if one rank fails (or time runs out) the others are killed instead of
-    being left to hang in a collective."""
-    import queue
-    import time
-    res, t0 = [], time.time()
-    while len(res) < len(procs) and time.time() - t0 < timeout_s:
-        try:
-            r = q.get(timeout=1.0)
-            res.append(r)
-            if r[1] != "ok":
-                break
-        except queue.Empty:
-            if any(p.exitcode not in (None, 0) for p in procs):
-                break
-    for p in procs:
-        p.join(5 if len(res) == len(procs) else 0.1)
-        if p.is_alive():
-            p.kill()
-    return res
-
-
-def _problem(n):
-    import oracle
-    from fluidnet_b200 import synth
-    flags = synth.make_flags(n, n, n, True, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], n / 128.0 * 4, 0.15)
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                 vorticityConfinementAmp=3.0, simMethod="convnet")
-    return batch, mconf, synth.make_model(True)
-
-
-def _worker(rank, world, port, n, steps, q, native=False, peer=True):
-    try:
-        os.environ["MASTER_ADDR"] = "127.0.0.1"
-        os.environ["MASTER_PORT"] = str(port)
-        torch.cuda.set_device(rank)
-        dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
-        from fluidnet_b200 import simulate, model as fmodel
-        from fluidnet_b200.slab import SlabSimulator, NativeSlabSimulator
-        batch, mconf, mnp = _problem(n)
-        tb = {k: torch.from_numpy(v) for k, v in batch.items()}
-        kw = {"peer_halos": peer} if native else {}
-        sim = (NativeSlabSimulator if native else SlabSimulator)(tb, mconf, mnp["layers"], torch.device("cuda", rank),
-                                                               rank, world, **kw)
-        if native and peer:
-            assert sim.halo_transport.startswith("peer memory"), sim.halo_transport
-        for _ in range(steps):
-            sim.step()
-        sim.check()
-        got = {k: sim.gather(k) for k in ("density", "UDiv", "pDiv")}
-        if rank == 0:
-            gb = {k: v.cuda() for k, v in tb.items()}
-            gm = fmodel.ProjectionModel(mnp["layers"], True)
-            for _ in range(steps):
-                simulate.simulate(None, mconf, gb, gm)
-            for k in ("density", "UDiv", "pDiv"):
-                want = gb[k].cpu()
-                err = (got[k] - want).abs().max().item()
-                scale = max(want.abs().max().item(), 1e-6)
-                assert err <= 1e-6 * scale, "%s: %g vs scale %g" % (k, err, scale)
-            # advected density never went through the reduction: bit-exact after one step? after
-            # `steps` steps it has seen the projected velocity, so only the tolerance above applies.
-        dist.barrier()
-        dist.destroy_process_group()
-        q.put((rank, "ok"))
-    except Exception as e:       # pragma: no cover
-        import traceback
-        q.put((rank, "FAIL: %s" % traceback.format_exc()))
-        raise
 
 
 @pytest.mark.parametrize("native,peer", [(False, False), (True, False), (True, True)],
@@ -107,11 +21,11 @@ def test_multi_gpu_slab_matches_single_gpu(world, n, steps, native, peer):
         pytest.skip("needs %d GPUs" % world)
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
-    procs = [ctx.Process(target=_worker, args=(r, world, port, n, steps, q, native, peer)) for r in range(world)]
+    port = free_port()
+    procs = [ctx.Process(target=slab_worker, args=(r, world, port, n, steps, q, native, peer)) for r in range(world)]
     for p in procs:
         p.start()
-    res = _collect(procs, q, 150)
+    res = collect(procs, q, 150)
     assert len(res) == world and all(r[1] == "ok" for r in res), res
 
 
@@ -120,7 +34,7 @@ def test_single_rank_slab_driver_matches_fused_step():
     range) on one GPU."""
     from fluidnet_b200 import simulate, model as fmodel
     from fluidnet_b200.slab import SlabSimulator
-    batch, mconf, mnp = _problem(32)
+    batch, mconf, mnp = convnet_problem(32)
     tb = {k: torch.from_numpy(v) for k, v in batch.items()}
     sim = SlabSimulator(tb, mconf, mnp["layers"], torch.device("cuda", 0), rank=0, world=1)
     gb = {k: v.cuda() for k, v in tb.items()}
@@ -141,7 +55,7 @@ def test_single_rank_library_slab_step_matches_fused_step():
     projection, downloads) against the fused single-GPU step, no NCCL involved."""
     from fluidnet_b200 import simulate, model as fmodel
     from fluidnet_b200.slab import NativeSlabSimulator
-    batch, mconf, mnp = _problem(32)
+    batch, mconf, mnp = convnet_problem(32)
     tb = {k: torch.from_numpy(v) for k, v in batch.items()}
     sim = NativeSlabSimulator(tb, mconf, mnp["layers"], torch.device("cuda", 0), rank=0, world=1)
     gb = {k: v.cuda() for k, v in tb.items()}
@@ -166,7 +80,7 @@ def test_emulated_slabs_on_one_gpu(world, n, steps):
     one GPU and exchanges served in-process: equals the undivided single-GPU run."""
     from fluidnet_b200 import simulate, model as fmodel
     from fluidnet_b200.slab import SlabSimulator, run_lockstep
-    batch, mconf, mnp = _problem(n)
+    batch, mconf, mnp = convnet_problem(n)
     tb = {k: torch.from_numpy(v) for k, v in batch.items()}
     dev = torch.device("cuda", 0)
     sims = [SlabSimulator(tb, mconf, mnp["layers"], dev, rank=r, world=world) for r in range(world)]

@@ -17,37 +17,11 @@ import pytest
 import torch
 import torch.multiprocessing as mp
 
-from test_gpu_conv_tc import KAPPA, SENTINEL, is_sentinel, layout, pack
-from test_gpu_conv_tc_join import reference as join_reference
+from scenes import banks
+from slab_cases import BANKED_TOL, banked_problem, refused, single_gpu
+from tc_conv import KAPPA, SENTINEL, is_sentinel, join_reference, layout, pack
 
 pytestmark = pytest.mark.gpu
-
-TOL = {"tf32x3": 1e-6, "tf32": 3e-3}
-
-
-def banks(num, agg, s=1, j=3):
-    return {"num": num, "split_stage": s, "join_stage": j, "aggregate": agg}
-
-
-def _problem(gnz, ny, nx, bk):
-    import oracle
-    from fluidnet_b200 import synth
-    flags = synth.make_flags(nx, ny, gnz, True, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], nx / 128.0 * 4, 0.15)
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * nx / 128,
-                                 vorticityConfinementAmp=3.0, simMethod="convnet")
-    return {k: torch.from_numpy(v) for k, v in batch.items()}, mconf, synth.make_model(True, banks=bk)
-
-
-def _single_gpu(tb, mconf, mnp, bk, mode, fused=False):
-    from fluidnet_b200 import simulate, model as fmodel
-    gb = {k: v.cuda() for k, v in tb.items()}
-    gm = fmodel.ProjectionModel(mnp["layers"], True, banks=bk)
-    gm.set_mode(mode)
-    return gb, lambda: (simulate.simulate_fused if fused else simulate.simulate)(None, mconf, gb, gm)
 
 
 def _close(got, want, tol, what):
@@ -80,12 +54,12 @@ def test_emulated_slabs_match_single_gpu(case):
     from fluidnet_b200.slab import SlabSimulator, run_lockstep, cnn_margin
     world, gnz, ny, nx, n, agg, mode, margin = case
     bk = banks(n, agg)
-    tb, mconf, mnp = _problem(gnz, ny, nx, bk)
+    tb, mconf, mnp = banked_problem(gnz, ny, nx, bk)
     dev = torch.device("cuda", 0)
     sims = [SlabSimulator(tb, mconf, mnp["layers"], dev, rank=r, world=world, margin=margin, banks=bk, conv_mode=mode)
             for r in range(world)]
     assert all(q.margin == (margin or cnn_margin(n)) for q in sims)
-    gb, step = _single_gpu(tb, mconf, mnp, bk, mode)
+    gb, step = single_gpu(tb, mconf, mnp, bk, mode)
     for it in range(3 if world < 4 else 2):
         run_lockstep(sims)
         step()
@@ -94,7 +68,7 @@ def test_emulated_slabs_match_single_gpu(case):
             want = gb[k].cpu()
             if it == 0 and k == "density":
                 assert torch.equal(got, want), "density is not bit-exact"
-            _close(got, want, TOL[mode], "step %d %s" % (it, k))
+            _close(got, want, BANKED_TOL[mode], "step %d %s" % (it, k))
     assert sims[0].ctx.trace_faults() == 0
 
 
@@ -103,10 +77,10 @@ def test_emulated_slabs_match_single_gpu(case):
 def test_single_rank_drivers_match_fused_step(native, n, agg):
     from fluidnet_b200.slab import SlabSimulator, NativeSlabSimulator
     bk = banks(n, agg)
-    tb, mconf, mnp = _problem(32, 32, 32, bk)
+    tb, mconf, mnp = banked_problem(32, 32, 32, bk)
     cls = NativeSlabSimulator if native else SlabSimulator
     sim = cls(tb, mconf, mnp["layers"], torch.device("cuda", 0), rank=0, world=1, banks=bk)
-    gb, step = _single_gpu(tb, mconf, mnp, bk, "tf32x3", fused=True)
+    gb, step = single_gpu(tb, mconf, mnp, bk, "tf32x3", fused=True)
     for _ in range(2):
         sim.step()
         step()
@@ -218,21 +192,12 @@ def test_join_with_bank_offsets_on_a_plane_range(split, agg, case):
         what, (err > bound).sum(), (err / np.maximum(bound, 1e-300)).max())
 
 
-def _refused(ctx, call):
-    before = ctx.lib.tfl_launch_count(ctx.h)
-    rc = call()
-    msg = ctx.lib.tfl_last_error(ctx.h)
-    assert rc != 0 and b"z-slab" in msg, msg
-    assert ctx.lib.tfl_launch_count(ctx.h) == before, "a refused call launched work"
-    return msg
-
-
 def test_refusals_name_the_z_slab():
     from fluidnet_b200 import simulate, synth, tfluids, model as fmodel
     from fluidnet_b200.slab import SlabSimulator, NativeSlabSimulator
     dev = torch.device("cuda", 0)
     b2 = banks(2, "concat")
-    tb, mconf, mnp2 = _problem(32, 16, 16, b2)
+    tb, mconf, mnp2 = banked_problem(32, 16, 16, b2)
     # a margin one below the minimum, from both drivers
     for cls in (SlabSimulator, NativeSlabSimulator):
         with pytest.raises(ValueError, match="margin >= 3"):
@@ -240,22 +205,22 @@ def test_refusals_name_the_z_slab():
     # the C step: a single-bank slab at margin 2 (and a global grid of 30 planes) stepped with other models
     single = synth.make_model(True)
     sim = NativeSlabSimulator(tb, mconf, single["layers"], dev, rank=0, world=1)
-    tb30, _, _ = _problem(30, 16, 16, b2)
+    tb30, _, _ = banked_problem(30, 16, 16, b2)
     sim30 = NativeSlabSimulator(tb30, mconf, single["layers"], dev, rank=0, world=1, margin=6)
     ctx, mc = sim.ctx, simulate.make_mconf(mconf)
     step = lambda s, m: lambda: ctx.lib.tfl_slab_sim_step(ctx.h, s.h, C.byref(mc), m.h)
     m2 = fmodel.ProjectionModel(mnp2["layers"], True, banks=b2)
-    assert b"margin >= 3" in _refused(ctx, step(sim, m2))
+    assert b"margin >= 3" in refused(ctx, step(sim, m2))
     m3 = fmodel.ProjectionModel(synth.make_model(True, banks=banks(3, "add"))["layers"], True, banks=banks(3, "add"))
-    assert b"divisible" in _refused(ctx, step(sim30, m3))
-    other = banks(2, "concat", 2, 4)
+    assert b"divisible" in refused(ctx, step(sim30, m3))
+    other = banks(2, "concat", s=2, j=4)
     m24 = fmodel.ProjectionModel(synth.make_model(True, banks=other)["layers"], True, banks=other)
-    assert b"tensor-core path only" in _refused(ctx, step(sim, m24))
+    assert b"tensor-core path only" in refused(ctx, step(sim, m24))
     m2.set_mode("fp32")
-    assert b"tensor-core path only" in _refused(ctx, step(sim, m2))
+    assert b"tensor-core path only" in refused(ctx, step(sim, m2))
     tog = synth.make_model(True, model_type="tog")
     mt = fmodel.ProjectionModel(tog["layers"], True, pool=tog.get("pool"), up=tog.get("up"))
-    assert b"tensor-core path only" in _refused(ctx, step(sim, mt))
+    assert b"tensor-core path only" in refused(ctx, step(sim, mt))
     # tfl_cnn_project_from_sums under a slab placement whose margin is too small
     m2.set_mode("tf32x3")
     g = torch.zeros(1, 1, 16, 16, 16, device=dev)
@@ -264,12 +229,12 @@ def test_refusals_name_the_z_slab():
     ctx.set_slab(8, 32, 7, 9)
     try:
         ctx.check(ctx.lib.tfl_set_slab_margin(ctx.h, 2))
-        msg = _refused(ctx, lambda: ctx.lib.tfl_cnn_project_from_sums(
+        msg = refused(ctx, lambda: ctx.lib.tfl_cnn_project_from_sums(
             ctx.h, m2.h, tfluids._grid(g), tfluids._grid(u), tfluids._grid(g), C.c_void_p(sums.data_ptr()),
             tfluids._grid(g), tfluids._grid(u), C.c_float(1e-5)))
         assert b"margin >= 3" in msg
         ctx.check(ctx.lib.tfl_set_slab_margin(ctx.h, 3))      # margin fine, 7 ghost planes below: too shallow
-        msg = _refused(ctx, lambda: ctx.lib.tfl_cnn_project_from_sums(
+        msg = refused(ctx, lambda: ctx.lib.tfl_cnn_project_from_sums(
             ctx.h, m2.h, tfluids._grid(g), tfluids._grid(u), tfluids._grid(g), C.c_void_p(sums.data_ptr()),
             tfluids._grid(g), tfluids._grid(u), C.c_float(1e-5)))
         assert b"ghost planes" in msg
@@ -290,7 +255,7 @@ def _worker(rank, world, port, gnz, steps, q, native, peer):
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
         from fluidnet_b200.slab import SlabSimulator, NativeSlabSimulator
         bk = banks(2, "concat")
-        tb, mconf, mnp = _problem(gnz, 16, 16, bk)
+        tb, mconf, mnp = banked_problem(gnz, 16, 16, bk)
         kw = {"peer_halos": peer} if native else {}
         sim = (NativeSlabSimulator if native else SlabSimulator)(tb, mconf, mnp["layers"], torch.device("cuda", rank),
                                                                rank, world, banks=bk, **kw)
@@ -301,7 +266,7 @@ def _worker(rank, world, port, gnz, steps, q, native, peer):
         sim.check()
         got = {k: sim.gather(k) for k in ("density", "UDiv", "pDiv")}
         if rank == 0:
-            gb, step = _single_gpu(tb, mconf, mnp, bk, "tf32x3")
+            gb, step = single_gpu(tb, mconf, mnp, bk, "tf32x3")
             for _ in range(steps):
                 step()
             for k in ("density", "UDiv", "pDiv"):
@@ -319,14 +284,14 @@ def _worker(rank, world, port, gnz, steps, q, native, peer):
                          ids=["torch_exchange", "library_nccl", "library_peer_memory"])
 @pytest.mark.parametrize("world,gnz", [(2, 32), (4, 44)])
 def test_multi_gpu_banked_slabs_match_single_gpu(world, gnz, native, peer):
-    from test_gpu_slab import _collect, _free_port
+    from slab_cases import collect, free_port
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, world, port, gnz, 2, q, native, peer)) for r in range(world)]
     for p in procs:
         p.start()
-    res = _collect(procs, q, 150)
+    res = collect(procs, q, 150)
     assert len(res) == world and all(r[1] == "ok" for r in res), res

@@ -20,7 +20,7 @@ case, each referenced from the gathered slab state before it:
     ghost planes are not written (the next step's first exchange refreshes them), so p on own_lo - 1 is pinned here
     rather than compared with float64; it enters U's z component on own_lo, which is.
   * After the step: the gathered p and U within the bound E of tests/network_bound.py at every voxel, the reference
-    being projection_reference (tests/test_gpu_cnn_network_f64.py) on the gathered start state with a whole-grid model
+    being projection_reference (tests/network_bound.py) on the gathered start state with a whole-grid model
     in the same mode; after step 1 the density is bit-exact.  Each case prints its largest err / E and the largest per
     distance from the nearest rank boundary (0: the two planes either side of it).
 
@@ -57,8 +57,8 @@ import torch
 
 import oracle
 from fluidnet_b200 import synth
-from network_bound import U64, check, input_fields, scale_interval
-from test_gpu_cnn_network_f64 import projection_reference
+from network_bound import U64, check, input_fields, projection_reference, scale_interval
+from scenes import banks, plume_batch, step_mconf
 
 FLUID, OBSTACLE = 1.0, 2.0
 SLOW = 1e-3                 # U's factor on the slow boundary's planes
@@ -82,10 +82,6 @@ CASES = [
 
 def case_id(c):
     return "w%d-%dx%dx%d-N%d-%s-%s-m%s" % c
-
-
-def banks_of(n, agg):
-    return None if n == 1 else {"num": n, "split_stage": 1, "join_stage": 3, "aggregate": agg}
 
 
 def decompositions(case):
@@ -117,24 +113,18 @@ def plume_and_slow(case):
 def problem(case):
     """Global CPU tensors of the start state, mconf, the model's numpy weights and its banks."""
     world, gnz, ny, nx, n, agg, mode, margin = case
-    flags = synth.make_flags(nx, ny, gnz, True, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0)
+    batch = plume_batch((gnz, ny, nx), inflow=nx / 128.0 * 4)
     plume, slow = plume_and_slow(case)
     if slow is not None:
         lo, hi = reach(n)["U1"]
-        U[:, :, slow - lo:slow + hi] *= np.float32(SLOW)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    pDiv = ((np.random.RandomState(gnz).rand(*flags.shape) - 0.5) * 0.2).astype(np.float32)
-    batch = {"pDiv": pDiv, "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], nx / 128.0 * 4, 0.15)
+        batch["UDiv"][:, :, slow - lo:slow + hi] *= np.float32(SLOW)
+    batch["pDiv"] = ((np.random.RandomState(gnz).rand(*batch["flags"].shape) - 0.5) * 0.2).astype(np.float32)
     # the inflow cylinder is centred on plane max(gnz // 2, 1) - 1; it is z-invariant elsewhere, so a roll moves it
     shift = plume - (max(gnz // 2, 1) - 1)
     for k in BC_KEYS:
         batch[k] = np.ascontiguousarray(np.roll(batch[k], shift, axis=2))
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * nx / 128,
-                                 vorticityConfinementAmp=3.0, simMethod="convnet")
-    bk = banks_of(n, agg)
-    return {k: torch.from_numpy(v) for k, v in batch.items()}, mconf, synth.make_model(True, banks=bk), bk
+    bk = None if n == 1 else banks(n, agg)
+    return {k: torch.from_numpy(v) for k, v in batch.items()}, step_mconf(nx), synth.make_model(True, banks=bk), bk
 
 
 def test_case_table_reaches_every_edge():
@@ -324,9 +314,9 @@ def ratio(got, want, E):
         return np.where(err == 0, 0.0, err / E)
 
 
-def make_model(mnp, bk, mode):
-    from fluidnet_b200 import model as fmodel
-    gm = fmodel.ProjectionModel(mnp["layers"], True, banks=bk)
+def make_model(mnp, mode):
+    from fluidnet_b200.model import ProjectionModel
+    gm = ProjectionModel.from_model(mnp)
     gm.set_mode(mode)
     return gm
 
@@ -341,7 +331,7 @@ def test_slab_steps_per_voxel(case):
     sims = [SlabSimulator(tb, mconf, mnp["layers"], dev, rank=r, world=world, margin=margin, banks=bk, conv_mode=mode)
             for r in range(world)]
     assert all(q.model.get_mode() == mode for q in sims)
-    gm = make_model(mnp, bk, mode)
+    gm = make_model(mnp, mode)
     orc = oracle.Oracle()
     dist = distances(gnz, boundaries(case))
     worst = {"p": 0.0, "U": 0.0}
@@ -390,7 +380,7 @@ def test_world1_library_driver_per_voxel(n, agg, mode):
     tb, mconf, mnp, bk = problem(case)
     dev = torch.device("cuda", 0)
     sim = NativeSlabSimulator(tb, mconf, mnp["layers"], dev, rank=0, world=1, banks=bk, conv_mode=mode)
-    gm = make_model(mnp, bk, mode)
+    gm = make_model(mnp, mode)
     const = {k: tb[k] for k in ("flags",) + BC_KEYS}
     try:
         for step in range(2):

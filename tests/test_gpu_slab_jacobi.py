@@ -3,40 +3,13 @@ step bit for bit -- emulated slabs on one GPU (SlabSimulator + run_lockstep), th
 over 2 / 4 GPUs (skipped on smaller boxes), and the one-launch block kernel against one launch per sweep."""
 import ctypes as C
 
-import numpy as np
 import pytest
 import torch
 import torch.multiprocessing as mp
 
+from slab_cases import KEYS, jacobi_problem, jacobi_reference
+
 pytestmark = pytest.mark.gpu
-
-KEYS = ("pDiv", "UDiv", "density")
-
-
-def _problem(nx, ny, gnz, buoyancy=True, gravity=False, vorticity=True, max_iter=34, seed=7):
-    import oracle
-    from fluidnet_b200 import synth
-    flags = synth.make_flags(nx, ny, gnz, True, nb=1, geometry=True, seed=seed)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], max(nx, gnz) / 128.0 * 4, 0.15)
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=(2.0 * nx / 128) if buoyancy else 0.0,
-                                 gravityScale=0.5 if gravity else 0.0,
-                                 vorticityConfinementAmp=3.0 if vorticity else 0.0, simMethod="jacobi",
-                                 maxIter=max_iter)
-    return {k: torch.from_numpy(v) for k, v in batch.items()}, mconf
-
-
-def _reference(tb, mconf, steps):
-    """Single-GPU operator sequence, state after each step."""
-    from fluidnet_b200 import simulate
-    gb = {k: v.cuda() for k, v in tb.items()}
-    out = []
-    for _ in range(steps):
-        simulate.simulate(None, mconf, gb)
-        out.append({k: gb[k].cpu().clone() for k in KEYS})
-    return out
 
 
 # (world, nx, ny, gnz, margin, maxIter or block-relative, forces)
@@ -64,8 +37,8 @@ def _iters(spec, margin):
 @pytest.mark.parametrize("world,nx,ny,gnz,margin,it,forces", EMU)
 def test_emulated_slabs_bit_identical(world, nx, ny, gnz, margin, it, forces):
     from fluidnet_b200.slab import SlabSimulator, run_lockstep
-    tb, mconf = _problem(nx, ny, gnz, *forces, max_iter=_iters(it, margin))
-    want = _reference(tb, mconf, 3)
+    tb, mconf = jacobi_problem(nx, ny, gnz, *forces, max_iter=_iters(it, margin))
+    want = jacobi_reference(tb, mconf, 3)
     dev = torch.device("cuda", 0)
     sims = [SlabSimulator(tb, mconf, None, dev, rank=r, world=world, margin=margin) for r in range(world)]
     for step in range(3):
@@ -81,7 +54,7 @@ def test_emulated_slabs_bit_identical(world, nx, ny, gnz, margin, it, forces):
 def test_single_rank_library_step_bit_identical(n):
     from fluidnet_b200 import simulate
     from fluidnet_b200.slab import NativeSlabSimulator
-    tb, mconf = _problem(n, n, n, max_iter=34)
+    tb, mconf = jacobi_problem(n, n, n, max_iter=34)
     sim = NativeSlabSimulator(tb, mconf, None, torch.device("cuda", 0), rank=0, world=1)
     gb = {k: v.cuda() for k, v in tb.items()}
     for _ in range(2):
@@ -97,7 +70,7 @@ def test_single_rank_library_step_bit_identical(n):
 def test_refusals():
     from fluidnet_b200 import _lib, simulate
     from fluidnet_b200.slab import NativeSlabSimulator, SlabSimulator
-    tb, mconf = _problem(32, 24, 16, max_iter=5)
+    tb, mconf = jacobi_problem(32, 24, 16, max_iter=5)
     dev = torch.device("cuda", 0)
     sim = NativeSlabSimulator(tb, mconf, None, dev, rank=0, world=1)
     lib = sim.ctx.lib
@@ -216,7 +189,7 @@ def _worker(rank, world, port, q, peer):
         torch.cuda.set_device(rank)
         dist.init_process_group("nccl", rank=rank, world_size=world, device_id=torch.device("cuda", rank))
         from fluidnet_b200.slab import NativeSlabSimulator
-        tb, mconf = _problem(128, 32, 64, max_iter=34)
+        tb, mconf = jacobi_problem(128, 32, 64, max_iter=34)
         sim = NativeSlabSimulator(tb, mconf, None, torch.device("cuda", rank), rank, world, peer_halos=peer)
         for _ in range(2):
             sim.step()
@@ -225,7 +198,7 @@ def _worker(rank, world, port, q, peer):
         assert n == 5 and by > 0, (n, ms, by)
         got = {k: sim.gather(k) for k in KEYS}
         if rank == 0:
-            want = _reference(tb, mconf, 2)[-1]
+            want = jacobi_reference(tb, mconf, 2)[-1]
             for k in KEYS:
                 assert torch.equal(got[k], want[k]), k
         dist.barrier()
@@ -243,12 +216,12 @@ def _worker(rank, world, port, q, peer):
 def test_multi_gpu_library_step_bit_identical(world, peer):
     if torch.cuda.device_count() < world:
         pytest.skip("needs %d GPUs" % world)
-    from test_gpu_slab import _collect, _free_port
+    from slab_cases import collect, free_port
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_worker, args=(r, world, port, q, peer)) for r in range(world)]
     for p in procs:
         p.start()
-    res = _collect(procs, q, 150)
+    res = collect(procs, q, 150)
     assert len(res) == world and all(r[1] == "ok" for r in res), res

@@ -29,12 +29,11 @@ import pytest
 import torch
 import torch.multiprocessing as mp
 
-from test_gpu_slab_record import _collect
+from slab_cases import Comm, TIMEOUT_S, collect
 
 pytestmark = pytest.mark.gpu
 
 KEYS = ("pDiv", "UDiv", "density")
-TIMEOUT_S = 400
 SKEW_S = 0.03                        # far below the ~2 s bound of k_slab_pull / k_sum_pull
 FORCES = [(True, False, True), (True, True, False), (False, True, True), (False, False, False)]
 
@@ -84,27 +83,28 @@ def _problem(case):
     """Global batch, mconf, model layers (None for 'jacobi') and banks of a case."""
     gnz, ny, nx = case["shape"]
     if case["kind"] == "jacobi":
-        from test_gpu_slab_jacobi import _problem as jacobi_problem
+        from slab_cases import jacobi_problem
         tb, mconf = jacobi_problem(nx, ny, gnz, *case["forces"], max_iter=case["iters"])
         return tb, mconf, None, None
-    from test_gpu_slab_banks import _problem as banks_problem, banks
+    from scenes import banks
+    from slab_cases import banked_problem
     bk = banks(*case["bk"]) if case["bk"] else None
-    tb, mconf, mnp = banks_problem(gnz, ny, nx, bk)
+    tb, mconf, mnp = banked_problem(gnz, ny, nx, bk)
     return tb, mconf, mnp["layers"], bk
 
 
 def _references(case):
     """Per step: the single-GPU state and, for 'convnet', the emulated run's (global CPU tensors)."""
-    from test_gpu_slab_jacobi import _reference
+    from slab_cases import jacobi_reference
     tb, mconf, layers, bk = _problem(case)
     if case["kind"] == "jacobi":
-        return {"single": _reference(tb, mconf, case["steps"])}
-    from test_gpu_slab_banks import _single_gpu
+        return {"single": jacobi_reference(tb, mconf, case["steps"])}
+    from slab_cases import single_gpu
     from fluidnet_b200.slab import SlabSimulator, run_lockstep
     dev = torch.device("cuda", 0)
     sims = [SlabSimulator(tb, mconf, layers, dev, rank=r, world=case["world"], banks=bk, conv_mode=case["mode"])
             for r in range(case["world"])]
-    gb, step = _single_gpu(tb, mconf, {"layers": layers}, bk, case["mode"])
+    gb, step = single_gpu(tb, mconf, {"layers": layers}, bk, case["mode"])
     emu, single = [], []
     for _ in range(case["steps"]):
         run_lockstep(sims)
@@ -133,31 +133,6 @@ def _want_traffic(case, rank):
     (_, _, u_width), blocks = jacobi_schedule(gnz, world, rank, margin, iters)
     assert [b[1] for b in blocks] == [0] + widths[1:] and u_width == max(widths), (blocks, widths)
     return [msg(halo, 4), msg(4, 4), msg(u_width, 3)], nblk - 1, msg(sum(widths[1:]), 1)
-
-
-class _Comm:
-    """allgather over one queue per rank; every rank calls it the same number of times, in the same order."""
-
-    def __init__(self, rank, world, inboxes):
-        self.rank, self.world, self.inboxes, self.n, self.early = rank, world, inboxes, 0, {}
-
-    def allgather(self, obj):
-        self.n += 1
-        for r, qr in enumerate(self.inboxes):
-            if r != self.rank:
-                qr.put((self.n, self.rank, obj))
-        got = {self.rank: obj}
-        while len(got) < self.world:
-            key = next((k for k in self.early if k[0] == self.n), None)
-            if key is not None:
-                got[key[1]] = self.early.pop(key)
-                continue
-            n, r, o = self.inboxes[self.rank].get(timeout=TIMEOUT_S)
-            if n == self.n:
-                got[r] = o
-            else:                                   # a faster rank's next allgather
-                self.early[(n, r)] = o
-        return [got[r] for r in range(self.world)]
 
 
 def _run_case(case, ci, rank, world, comm, barrier, qd):
@@ -223,10 +198,10 @@ def _check_case(case, refs, parts, frames):
             emu, single = refs["emulated"][step][k], refs["single"][step][k]
             if not torch.equal(got[k], emu):
                 fails.append("%s differs from the emulated run: %s" % (what, _first_diff(got[k], emu)))
-            from test_gpu_slab_banks import TOL
+            from slab_cases import BANKED_TOL
             err = (got[k] - single).abs().max().item()
             scale = max(single.abs().max().item(), 1e-6)
-            if not err <= TOL[case["mode"]] * scale:
+            if not err <= BANKED_TOL[case["mode"]] * scale:
                 fails.append("%s: %g from the single-GPU step (scale %g)" % (what, err, scale))
     if case["frames"]:
         if [i for i, _ in frames] != list(range(case["steps"])):
@@ -241,7 +216,7 @@ def _check_case(case, refs, parts, frames):
 def _worker(rank, world, q, qd, inboxes, barrier):
     try:
         torch.cuda.set_device(0)
-        comm = _Comm(rank, world, inboxes)
+        comm = Comm(rank, world, inboxes)
         wait = lambda: barrier.wait(TIMEOUT_S)       # noqa: E731
         fails, compared, pending = [], 0, {}
         for ci, case in enumerate(_cases(world)):
@@ -277,7 +252,7 @@ def test_library_step_one_process_per_rank(world):
     procs = [ctx.Process(target=_worker, args=(r, world, q, qd, inboxes, barrier)) for r in range(world)]
     for p in procs:
         p.start()
-    res = _collect(procs, q, TIMEOUT_S)
+    res = collect(procs, q, TIMEOUT_S)
     assert len(res) == world and all(r[1] == "ok" for r in res), res
     fails = [f for r in res for f in r[2]]
     assert not fails, "\n".join(fails)
@@ -289,7 +264,7 @@ def test_missing_peer_refuses_before_any_step():
     before anything is launched, and leaves the context at one rank without a communicator."""
     from fluidnet_b200._lib import TflError
     from fluidnet_b200.slab import NativeSlabSimulator
-    from test_gpu_slab_jacobi import _problem as jacobi_problem
+    from slab_cases import jacobi_problem
     tb, mconf = jacobi_problem(32, 24, 16, max_iter=5)
     dev = torch.device("cuda", 0)
     gathered = []

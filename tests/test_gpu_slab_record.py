@@ -4,7 +4,6 @@ against the single-GPU scene, convnet frames against synchronous downloads, and 
 GPUs."""
 import ctypes as C
 import os
-import socket
 import time
 
 import numpy as np
@@ -14,6 +13,7 @@ import torch.multiprocessing as mp
 
 from fluidnet_b200 import record, scene, synth, tfluids
 from fluidnet_b200._lib import TflError
+from slab_cases import collect, free_port
 
 pytestmark = pytest.mark.gpu
 
@@ -28,26 +28,6 @@ def special_bits(shape, seed):
     specials = np.array([0x80000000, 0x00000001, 0x007FFFFF, 0x80000001, 0x7FC12345, 0x7F800001, 0xFFBADBAD], np.uint32)
     flat[:min(flat.size, specials.size)] = specials[:flat.size]
     return bits
-
-
-def _collect(procs, q, timeout_s):
-    """Results of all ranks; if one rank fails (or time runs out) the others are killed (test_gpu_slab.py's pattern)."""
-    import queue
-    res, t0 = [], time.time()
-    while len(res) < len(procs) and time.time() - t0 < timeout_s:
-        try:
-            r = q.get(timeout=1.0)
-            res.append(r)
-            if r[1] != "ok":
-                break
-        except queue.Empty:
-            if any(p.exitcode not in (None, 0) for p in procs):
-                break
-    for p in procs:
-        p.join(5 if len(res) == len(procs) else 0.1)
-        if p.is_alive():
-            p.kill()
-    return res
 
 
 def _protocol_worker(rank, world, shape, frames, q, qh, barrier, slow_rank):
@@ -120,7 +100,7 @@ def test_slab_frames_from_several_processes_on_one_gpu(world, shape):
              for r in range(world)]
     for p in procs:
         p.start()
-    res = _collect(procs, q, 300)
+    res = collect(procs, q, 300)
     assert len(res) == world and all(r[1] == "ok" for r in res), res
     assert sum(r[2] for r in res) == 36
 
@@ -276,14 +256,6 @@ def test_world1_convnet_frames_equal_synchronous_downloads():
         sim.close()
 
 
-def _free_port():
-    s = socket.socket()
-    s.bind(("127.0.0.1", 0))
-    p = s.getsockname()[1]
-    s.close()
-    return p
-
-
 def _gpu_worker(rank, world, port, out_dir, q):
     try:
         import torch.distributed as dist
@@ -344,9 +316,9 @@ def test_multi_gpu_scene_and_frames(world, tmp_path):
         pytest.skip("needs %d GPUs" % world)
     ctx = mp.get_context("spawn")
     q = ctx.Queue()
-    port = _free_port()
+    port = free_port()
     procs = [ctx.Process(target=_gpu_worker, args=(r, world, port, str(tmp_path), q)) for r in range(world)]
     for p in procs:
         p.start()
-    res = _collect(procs, q, 300)
+    res = collect(procs, q, 300)
     assert len(res) == world and all(r[1] == "ok" for r in res), res

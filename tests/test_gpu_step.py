@@ -16,30 +16,10 @@ import torch
 import oracle
 from cases import bits_equal, describe_diff
 from fluidnet_b200 import synth
+from scenes import close, plume_batch, step_mconf, to_gpu
+from step_cases import MODE_TOL
 
 pytestmark = pytest.mark.gpu
-
-
-def make_batch(n, is3d, plume=True, geometry=True, amp=3.0, shape=None, nb=1, seed=1234):
-    """An n^2 / n^3 grid, or shape = (nz, ny, nx); with nb > 1 every entry has its own velocity field."""
-    nz, ny, nx = shape if shape is not None else ((n if is3d else 1), n, n)
-    flags = synth.make_flags(nx, ny, nz, is3d, nb=nb, geometry=geometry)
-    U = synth.make_smooth_velocity(flags, is3d, amp=amp, seed=seed)
-    oracle.Oracle().setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    if plume:
-        oracle.create_plume_bcs(batch, [1.0], nx / 128.0 * 4, 0.15)
-    return batch
-
-
-def to_gpu(batch):
-    return {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items() if v is not None}
-
-
-def close(got, want, tol, what):
-    err = np.abs(got.astype(np.float64) - want.astype(np.float64)).max()
-    scale = max(np.abs(want).max(), 1e-6)
-    assert err <= tol * scale, "%s: max err %g vs scale %g" % (what, err, scale)
 
 
 @pytest.mark.parametrize("is3d,n", [(False, 64), (True, 20)], ids=["2d64", "3d20"])
@@ -47,7 +27,7 @@ def close(got, want, tol, what):
 def test_step_jacobi_bit_exact(orc, is3d, n, fused):
     """BASELINE config 1: 2-D 64x64 smoke, Jacobi projection, 1 step (and a small 3-D one)."""
     from fluidnet_b200 import simulate
-    batch = make_batch(n, is3d)
+    batch = plume_batch(n, is3d, inflow=n / 128.0 * 4)
     mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=1.0,
                                  vorticityConfinementAmp=(0.0 if not is3d else 3.0),
                                  simMethod="jacobi", maxIter=100, is3D=is3d)
@@ -58,11 +38,6 @@ def test_step_jacobi_bit_exact(orc, is3d, n, fused):
         for k in ("density", "UDiv", "pDiv"):
             got = gb[k].cpu().numpy()
             assert bits_equal(got, batch[k]), "step %d %s: %s" % (step, k, describe_diff(got, batch[k]))
-
-
-# conv arithmetic -> tolerance relative to max|field| (see module docstring; tf32 = single-pass
-# TF32 tensor cores, 10-bit mantissa inputs, is the "fast" mode and NOT the default)
-MODE_TOL = {"fp32": 2e-5, "tf32x3": 2e-5, "tf32": 3e-3}
 
 
 FORWARD_CASES = {          # id: (is3d, (nz, ny, nx), nb, mode, zero_u_entry)
@@ -90,15 +65,15 @@ def test_cnn_projection_forward(orc, case):
     """BASELINE config 2 (shape-reduced for the CPU oracle): model:forward only, for every
     arithmetic mode of the conv stack (37^3 exercises partial tensor-core tiles), on non-cubic grids and
     batches of two.  Each batch entry is checked on its own: its scale, and p / U relative to its own max."""
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     is3d, shape, nb, mode, zero_u = FORWARD_CASES[case]
-    batch = make_batch(0, is3d, plume=False, shape=shape, nb=nb)
+    batch = plume_batch(shape, is3d, nb=nb)
     if zero_u is not None:
         batch["UDiv"][zero_u] = 0.0
     mnp = synth.make_model(is3d)
     p0 = (synth.make_density(batch["flags"], seed=77) - np.float32(0.5)) * np.float32(0.1)
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
-    gm = make_gpu_model(mnp)
+    gm = ProjectionModel.from_model(mnp)
     assert gm.get_mode() == ("tf32x3" if is3d else "fp32")      # defaults
     gm.set_mode(mode)
     gp, gU = gm.forward((torch.from_numpy(p0).cuda(), torch.from_numpy(batch["UDiv"]).cuda(),
@@ -118,18 +93,18 @@ def test_cnn_model_state_across_shapes_and_modes():
     """One model through grid changes (each reallocates its padded activation buffers), mode changes and new
     inputs on the same grid: every result equals that of a fresh model for the same shape and mode, so the zero
     borders of the activation buffers survive between calls."""
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     mnp = synth.make_model(True)
     A, B = ((12, 16, 20), 1), ((9, 13, 31), 2)
-    gm = make_gpu_model(mnp)
+    gm = ProjectionModel.from_model(mnp)
     for (shape, nb), mode, seed in ((A, "tf32x3", 0), (B, "tf32", 0), (A, "fp32", 0), (A, "tf32x3", 1),
                                     (A, "tf32x3", 2), (B, "tf32x3", 1)):
-        batch = make_batch(0, True, plume=False, shape=shape, nb=nb, seed=1234 + seed)
+        batch = plume_batch(shape, nb=nb, seed=1234 + seed)
         p0 = (synth.make_density(batch["flags"], seed=77 + seed) - np.float32(0.5)) * np.float32(0.1)
         inputs = (torch.from_numpy(p0).cuda(), torch.from_numpy(batch["UDiv"]).cuda(),
                   torch.from_numpy(batch["flags"]).cuda())
         gm.set_mode(mode)
-        fresh = make_gpu_model(mnp)
+        fresh = ProjectionModel.from_model(mnp)
         fresh.set_mode(mode)
         what = "%s nb%d %s seed %d" % (shape, nb, mode, seed)
         for got, want, k in zip(gm.forward(inputs), fresh.forward(inputs), ("p", "U")):
@@ -140,13 +115,12 @@ def test_cnn_model_state_across_shapes_and_modes():
 def test_step_convnet(orc, fused):
     """BASELINE config 3 shape-reduced: CNN projection + vorticity confinement + MacCormack."""
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     n = 24
-    batch = make_batch(n, True)
+    batch = plume_batch(n, inflow=n / 128.0 * 4)
     mnp = synth.make_model(True)
-    gm = make_gpu_model(mnp)
-    mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                 vorticityConfinementAmp=3.0, simMethod="convnet")
+    gm = ProjectionModel.from_model(mnp)
+    mconf = step_mconf(n)
     gb = to_gpu(batch)
     for step in range(2):
         (simulate.simulate_fused if fused else simulate.simulate)(None, mconf, gb, gm)
@@ -159,10 +133,10 @@ def test_step_convnet(orc, fused):
 def test_fused_equals_operator_sequence():
     """tfl_simulate_step must equal calling the operators one by one (bitwise)."""
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     n = 32
-    batch = make_batch(n, True)
-    gm = make_gpu_model(synth.make_model(True))
+    batch = plume_batch(n, inflow=n / 128.0 * 4)
+    gm = ProjectionModel.from_model(synth.make_model(True))
     mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=0.5,
                                  vorticityConfinementAmp=3.0, simMethod="convnet")
     a, b = to_gpu(batch), to_gpu(batch)
@@ -182,10 +156,10 @@ def test_host_buffer_step_equals_device_step(method):
     import ctypes as C
     import torch
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     n = 32
-    batch = make_batch(n, True)
-    gm = make_gpu_model(synth.make_model(True))
+    batch = plume_batch(n, inflow=n / 128.0 * 4)
+    gm = ProjectionModel.from_model(synth.make_model(True))
     mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=0.5,
                                  vorticityConfinementAmp=3.0, simMethod=method, maxIter=20)
     dev_batch = to_gpu(batch)
@@ -215,13 +189,13 @@ def test_trained_reference_model_2d(orc):
     its job: it leaves less divergence than it was given."""
     import os
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     z = np.load(os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "myModel2D_layers.npz"))
     mnp = {"is3D": bool(z["is3D"]), "layers": [(z["w%d" % i], z["b%d" % i]) for i in range(int(z["n_layers"]))]}
     assert mnp["is3D"] is False
     n = 64
-    batch = make_batch(n, False, plume=False, amp=1.0)
-    gm = make_gpu_model(mnp, threshold=float(z["normalizeInputThreshold"]))
+    batch = plume_batch(n, False, amp=1.0)
+    gm = ProjectionModel.from_model(mnp, normalizeInputThreshold=float(z["normalizeInputThreshold"]))
     p0 = np.zeros_like(batch["flags"])
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
     gp, gU = gm.forward((torch.from_numpy(p0).cuda(), torch.from_numpy(batch["UDiv"]).cuda(),
@@ -249,14 +223,14 @@ def test_cnn_model_graphs(orc, is3d, n, model_type, pool_type):
     """The other single-bank graphs of lib/model.lua:164-226: 'tog' (pooling, ConvolutionUpsample pixel
     shuffles, 5x5 / 1x1 / 256-channel convolutions) and 'yang' (sigmoid), model:forward against the oracle
     (whose graph semantics are pinned on torch.nn.functional, tests/test_oracle_model_graph.py)."""
-    from gpu_backend import make_gpu_model
-    batch = make_batch(n, is3d, plume=False)
+    from fluidnet_b200.model import ProjectionModel
+    batch = plume_batch(n, is3d)
     mnp = synth.make_model(is3d, model_type=model_type)
     if model_type == "tog":
         mnp["poolType"] = pool_type
     p0 = (synth.make_density(batch["flags"], seed=77) - np.float32(0.5)) * np.float32(0.1)
     wp, wU, wscale = oracle.model_forward(orc, mnp, p0, batch["UDiv"], batch["flags"])
-    gm = make_gpu_model(mnp)
+    gm = ProjectionModel.from_model(mnp)
     assert gm.get_mode() == "fp32"
     gp, gU = gm.forward((torch.from_numpy(p0).cuda(), torch.from_numpy(batch["UDiv"]).cuda(),
                          torch.from_numpy(batch["flags"]).cuda()), return_scale=True)
@@ -317,13 +291,13 @@ def test_fused_step_with_non_idempotent_density_bc():
     BC (invMask = 1 where bc != 0) the three applications do not collapse into one: the fused step must still
     equal the operator sequence."""
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     n = 32
-    batch = make_batch(n, True)
+    batch = plume_batch(n, inflow=n / 128.0 * 4)
     rs = np.random.RandomState(5)
     batch["densityBC"] = (rs.rand(*batch["density"].shape) < 0.1).astype(np.float32) * np.float32(0.25)
     batch["densityBCInvMask"] = np.where(rs.rand(*batch["density"].shape) < 0.5, 1.0, 0.5).astype(np.float32)
-    gm = make_gpu_model(synth.make_model(True))
+    gm = ProjectionModel.from_model(synth.make_model(True))
     mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=0.5,
                                  vorticityConfinementAmp=3.0, simMethod="convnet")
     a, b = to_gpu(batch), to_gpu(batch)
@@ -339,10 +313,10 @@ def test_fused_step_on_unaligned_views():
     """Caller-owned grids that are contiguous but only 4-byte aligned (a view with an odd storage offset):
     the 16-byte kernels must step aside, results equal the aligned run bit for bit."""
     from fluidnet_b200 import simulate
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     n = 32
-    batch = make_batch(n, True)
-    gm = make_gpu_model(synth.make_model(True))
+    batch = plume_batch(n, inflow=n / 128.0 * 4)
+    gm = ProjectionModel.from_model(synth.make_model(True))
     mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=0.5,
                                  vorticityConfinementAmp=3.0, simMethod="convnet")
     a = to_gpu(batch)
@@ -366,7 +340,7 @@ def test_operators_on_a_non_current_device(orc):
     if torch.cuda.device_count() < 2:
         pytest.skip("needs 2 GPUs")
     from fluidnet_b200 import tfluids
-    c = make_batch(20, True, plume=False)
+    c = plume_batch(20)
     want = orc.advectVel(0.1, c["UDiv"], c["flags"], "maccormackOurs", 0.6)
     torch.cuda.set_device(0)
     U = torch.from_numpy(c["UDiv"]).to("cuda:1")
@@ -386,17 +360,12 @@ def test_step_as_cuda_graph_equals_direct_step(orc):
     import torch
     from fluidnet_b200 import simulate, synth
     from fluidnet_b200._lib import TflError
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     n = 32
-    flags = synth.make_flags(n, n, n, True, nb=1, geometry=True)
-    U = synth.make_smooth_velocity(flags, True, amp=3.0)
-    orc.setWallBcsForward(U, flags)
-    batch = {"pDiv": np.zeros_like(flags), "UDiv": U, "flags": flags, "density": synth.make_density(flags)}
-    oracle.create_plume_bcs(batch, [1.0], n / 128.0, 0.15)
+    batch = plume_batch(n, inflow=n / 128.0)
     mnp = synth.make_model(True)
-    for sim_method, model in (("convnet", make_gpu_model(mnp)), ("jacobi", None)):
-        mconf = oracle.default_mconf(dt=0.1, maccormackStrength=0.6, buoyancyScale=2.0 * n / 128,
-                                     vorticityConfinementAmp=3.0, simMethod=sim_method, maxIter=12)
+    for sim_method, model in (("convnet", ProjectionModel.from_model(mnp)), ("jacobi", None)):
+        mconf = step_mconf(n, simMethod=sim_method, maxIter=12)
         ga = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
         gb = {k: torch.from_numpy(v.copy()).cuda() for k, v in batch.items()}
         with pytest.raises(TflError):

@@ -22,10 +22,6 @@ test_case_table_reaches_every_branch (no GPU) keeps the table covering every bra
 (tfl_fused.cu) and both paths of tfl_simulate_step, each at nb = 1 and nb > 1; test_case_paths_are_the_kernels_that_ran
 proves each row's path from the kernels torch.profiler saw, so the restated rule cannot drift from the library's."""
 import ctypes as C
-import json
-import os
-import subprocess
-import sys
 
 import numpy as np
 import pytest
@@ -34,27 +30,10 @@ import torch
 import oracle
 from cases import bits_equal, describe_diff
 from fluidnet_b200 import synth
+from step_cases import (MODE_TOL, OPS_TOL, case, close_per_entry, contexts, make_batch, quad_dims, random_bcs,
+                        run_in_child, same_zero_bits, step_path, takes_fused_path)
 
-MODE_TOL = {"fp32": 2e-5, "tf32x3": 2e-5, "tf32": 3e-3}
-OPS_TOL = 1e-6
 GRAVITY = [0.3, -0.8, 0.52]
-BASE_MCONF = dict(dt=0.1, maccormackStrength=0.6, buoyancyScale=0.5, vorticityConfinementAmp=3.0,
-                  simMethod="convnet")
-
-
-def case(shape, nb=1, flags="geom", state="plume", method="maccormackOurs", tile=None, amp=3.0, mode="tf32x3",
-         pbc=False, threshold=1e-5, **mconf):
-    """shape = (nz, ny, nx); flags: geom (sphere + slab) | empty | open (fluid on the x and z faces) | exotic;
-    state: plume | none (no density, no BCs) | density (no BCs) | ubc (density + velocity BC) |
-    ubc-nodens (velocity BC, no density) | random (random U and density BCs, -0.0 in U and the BCs) |
-    unaligned (plume on 4-byte aligned views); tile: tfl_debug_advect_tile mode (None: automatic);
-    amp: velocity amplitude (traces of amp * dt cells); mconf: overrides of BASE_MCONF."""
-    m = oracle.default_mconf(**BASE_MCONF)
-    m.update(mconf)
-    m["advectionMethod"] = method
-    m["normalizeInputThreshold"] = threshold
-    return dict(shape=shape, nb=nb, flags=flags, state=state, method=method, tile=tile, amp=amp, mode=mode,
-                pbc=pbc, threshold=threshold, mconf=m)
 
 
 CASES = {
@@ -104,26 +83,6 @@ CASES = {
 # ---------------------------------------------------------------------------------------------------------------
 # Which branch each case reaches (restated from tfl_simulate_step and quad_dims, tfl_fused.cu)
 # ---------------------------------------------------------------------------------------------------------------
-def takes_fused_path(c):
-    """fused_step_applies (tfl_api.cu) for the 3-D convnet steps these tests run with the default input block: a
-    tensor-core mode and no pressure BC, at any nb."""
-    return c["mode"] != "fp32" and not c["pbc"]
-
-
-def quad_dims(nb, nz, ny, nx):
-    """(grid, block) of the 4-voxel kernels, or None where the per-voxel kernels run."""
-    if nx % 4 != 0:
-        return None
-    quads = nx // 4
-    if quads >= 32:
-        bx = 32
-    elif quads & (quads - 1) == 0:
-        bx = quads
-    else:
-        return None
-    bz = 2 if nz > 1 else 1
-    by = 256 // (bx * bz)
-    return ((quads + bx - 1) // bx, (ny + by - 1) // by, (nb * nz + bz - 1) // bz), (bx, by, bz)
 
 
 def branches(c):
@@ -179,84 +138,6 @@ def test_case_table_reaches_every_branch():
 # ---------------------------------------------------------------------------------------------------------------
 # State builders (numpy)
 # ---------------------------------------------------------------------------------------------------------------
-def make_flags(c):
-    nz, ny, nx = c["shape"]
-    kind = c["flags"]
-    f = synth.make_flags(nx, ny, nz, True, nb=c["nb"], geometry=kind != "empty", exotic=kind == "exotic")
-    if kind == "open":           # fluid on the x and z faces (the y faces stay solid)
-        f[:, :, :, 1:-1, 0] = synth.FLUID
-        f[:, :, :, 1:-1, -1] = synth.FLUID
-        f[:, :, 0, 1:-1, :] = synth.FLUID
-        f[:, :, -1, 1:-1, :] = synth.FLUID
-    return np.ascontiguousarray(f)
-
-
-def plume_bcs(batch, nb):
-    """createPlumeBCs per batch entry, each with its own velocity, density and radius."""
-    parts = []
-    for b in range(nb):
-        sub = {"UDiv": batch["UDiv"][b:b + 1], "density": batch["density"][b:b + 1]}
-        nx = sub["UDiv"].shape[-1]
-        oracle.create_plume_bcs(sub, [1.0 - 0.3 * b], nx / 128.0 * 4 * (1 + b), 0.15 + 0.05 * b)
-        parts.append(sub)
-    for k in ("UBC", "UBCInvMask", "densityBC", "densityBCInvMask"):
-        batch[k] = np.ascontiguousarray(np.concatenate([p[k] for p in parts]))
-
-
-def random_bcs(batch, seed, density=True):
-    """BC arrays that are the identity pair (invMask 1, bc +0.0) on some quads (4 cells along x) only.  Other
-    quads hold invMask 1 with bc -0.0 (not the identity: x + -0.0 keeps a -0.0), or invMask in {0, 0.5, 1} with
-    values, zeros and -0.0.  The density BC is additive where invMask is 1 and bc != 0."""
-    rs = np.random.RandomState(seed)
-    U = batch["UDiv"]
-    nb, nc, nz, ny, nx = U.shape
-    nq = (nx + 3) // 4
-
-    def per_quad(a):
-        return np.ascontiguousarray(np.repeat(a, 4, axis=-1)[..., :nx])
-
-    def arrays(nch, scale):
-        kind = per_quad(rs.randint(0, 4, size=(nb, 1, nz, ny, nq)))
-        kind = np.broadcast_to(kind, (nb, nch, nz, ny, nx))
-        inv = np.where(kind <= 1, 1.0, rs.choice([0.0, 0.5, 1.0], size=kind.shape)).astype(np.float32)
-        val = (rs.randn(*kind.shape) * scale).astype(np.float32)
-        r = rs.rand(*kind.shape)
-        val[r < 0.3] = 0.0
-        val[(r >= 0.3) & (r < 0.5)] = -0.0
-        bc = np.where(kind == 0, np.float32(0.0), np.where(kind == 1, np.float32(-0.0), val)).astype(np.float32)
-        return np.ascontiguousarray(bc), np.ascontiguousarray(inv)
-
-    batch["UBC"], batch["UBCInvMask"] = arrays(nc, 0.5)
-    if density:
-        dbc, dinv = arrays(1, 0.25)
-        batch["densityBC"], batch["densityBCInvMask"] = np.where(dbc == 0, dbc, np.abs(dbc)), dinv   # +0 / -0 kept
-
-
-def make_batch(orc, c, seed=1234):
-    flags = make_flags(c)
-    U = synth.make_smooth_velocity(flags, True, amp=c["amp"], seed=seed)
-    orc.setWallBcsForward(U, flags)
-    batch = {"pDiv": ((synth.make_density(flags, seed=seed + 1) - np.float32(0.5)) * np.float32(0.1)),
-             "UDiv": U, "flags": flags}
-    state = c["state"]
-    if state != "none" and state != "ubc-nodens":
-        batch["density"] = synth.make_density(flags, seed=seed + 2)
-    if state in ("plume", "unaligned"):
-        plume_bcs(batch, c["nb"])
-    elif state in ("ubc", "ubc-nodens"):
-        tmp = {"UDiv": U, "density": np.zeros_like(flags)}
-        plume_bcs(tmp, c["nb"])
-        batch["UBC"], batch["UBCInvMask"] = tmp["UBC"], tmp["UBCInvMask"]
-    elif state == "random":
-        random_bcs(batch, seed + 3)
-        rs = np.random.RandomState(seed + 4)
-        U[rs.rand(*U.shape) < 0.05] = -0.0
-    if c["pbc"]:
-        inv = np.ones_like(flags)
-        inv[:, :, 2:5, 3:7, 4:9] = 0.0
-        batch["pBCInvMask"] = inv
-        batch["pBC"] = np.where(inv == 0, np.float32(0.05), np.float32(0.0)).astype(np.float32)
-    return {k: np.ascontiguousarray(v, np.float32) for k, v in batch.items()}
 
 
 class LibraryOccupancyOracle(oracle.Oracle):
@@ -296,27 +177,15 @@ def host(batch):
     return {k: v.cpu().numpy() for k, v in batch.items()}
 
 
-def close_per_entry(got, want, tol, what):
-    for b in range(got.shape[0]):
-        err = np.abs(got[b].astype(np.float64) - want[b].astype(np.float64)).max()
-        scale = max(float(np.abs(want[b]).max()), 1e-6)
-        assert err <= tol * scale, "%s[%d]: max err %g vs scale %g (tol %g)" % (what, b, err, scale, tol)
-
-
-def same_zero_bits(got, want):
-    z = (got == 0) | (want == 0)
-    return np.array_equal(got[z].view(np.uint32), want[z].view(np.uint32))
-
-
 @pytest.mark.gpu
 @pytest.mark.parametrize("name", list(CASES))
 def test_step_paths(orc, name):
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     c = CASES[name]
     batch = make_batch(orc, c)
     mnp = synth.make_model(True)
-    gm = make_gpu_model(mnp, threshold=c["threshold"])
+    gm = ProjectionModel.from_model(mnp, normalizeInputThreshold=c["threshold"])
     gm.set_mode(c["mode"])
     mconf = c["mconf"]
     be = LibraryOccupancyOracle() if c["flags"] == "exotic" else orc
@@ -355,18 +224,6 @@ def test_step_paths(orc, name):
 # ---------------------------------------------------------------------------------------------------------------
 # Each row's path, from the kernels that ran
 # ---------------------------------------------------------------------------------------------------------------
-def step_path(kernels):
-    """'quad', 'scalar' (the fused step's 4-voxel or per-voxel kernels) or 'ops' (neither: the operator sequence),
-    from the names of the kernels one step ran."""
-    names = list(kernels)
-    quad = any("k_cnn_finish_fused4" in k for k in names)
-    scalar = any("k_cnn_finish_fused" in k and "k_cnn_finish_fused4" not in k for k in names)
-    assert not (quad and scalar), names
-    if quad or scalar:
-        assert any("k_vort_bc_mask" in k for k in names), names
-        return "quad" if quad else "scalar"
-    assert not any("k_vort_bc_mask" in k for k in names), names
-    return "ops"
 
 
 def expected_path(c):
@@ -374,31 +231,18 @@ def expected_path(c):
     return "ops" if "ops" in b else "scalar" if "scalar" in b else "quad"
 
 
-def run_in_child(module, expr, timeout=900):
-    """json.loads of what `expr` (evaluated after `import <module> as t`) returns in a fresh interpreter.  The profiler
-    runs there: on one H100 run, a profiler session opened in the test process left every capture of
-    test_gpu_launch_tally.py, later in the same process, without a kernel event."""
-    here = os.path.dirname(os.path.abspath(__file__))
-    env = dict(os.environ)
-    env["PYTHONPATH"] = os.pathsep.join(p for p in (here, os.path.dirname(here), env.get("PYTHONPATH")) if p)
-    code = "import json, %s as t; print(json.dumps(%s))" % (module, expr)
-    r = subprocess.run([sys.executable, "-c", code], capture_output=True, text=True, env=env, timeout=timeout)
-    assert r.returncode == 0, r.stderr[-4000:]
-    return json.loads(r.stdout.strip().splitlines()[-1])
-
-
 def case_kernels():
     """{row: (launch tally, {kernel: count})} of one tfl_simulate_step per CASES row, under torch.profiler."""
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
-    from test_gpu_launch_tally import _tally_and_kernels
+    from fluidnet_b200.model import ProjectionModel
+    from step_cases import tally_and_kernels
     orc = oracle.Oracle()
     out = {}
     for name, c in CASES.items():
-        gm = make_gpu_model(synth.make_model(True), threshold=c["threshold"])
+        gm = ProjectionModel.from_model(synth.make_model(True), normalizeInputThreshold=c["threshold"])
         gm.set_mode(c["mode"])
         st = to_gpu(make_batch(orc, c), c["state"] == "unaligned")
-        tally, kernels = _tally_and_kernels(tfluids.context(), lambda: simulate.simulate_fused(None, c["mconf"], st, gm),
+        tally, kernels = tally_and_kernels(tfluids.context(), lambda: simulate.simulate_fused(None, c["mconf"], st, gm),
                                             attempts=6)
         out[name] = (tally, dict(kernels))
     return out
@@ -428,59 +272,6 @@ def _scale_traces(b, cells):
 
 
 GRAPH_EDITS = ("solid block on", "solid block off", "BC quads switched", "traces 2.5 cells", "pDiv")
-
-
-class Contexts:
-    """Library contexts of one test, each with its own arena (where the step keeps the BC quad mask), flag cache
-    (byte flags and clearance) and tile telemetry.  `use(ctx)` makes one the context tfluids calls through, `model`
-    creates a model on it.  close() puts back the context tfluids used before, destroys the models, then the
-    contexts (a model is destroyed through the context it was created on)."""
-
-    def __init__(self):
-        from fluidnet_b200 import tfluids
-        self.tfluids = tfluids
-        self.dev = torch.cuda.current_device()
-        self.saved = tfluids._contexts.get(self.dev)
-        self.made, self.models = [], []
-
-    def new(self):
-        ctx = self.tfluids.Context(self.dev)
-        self.made.append(ctx)
-        return ctx
-
-    def use(self, ctx):
-        self.tfluids._contexts[self.dev] = ctx
-
-    def model(self, ctx, mnp):
-        from gpu_backend import make_gpu_model
-        self.use(ctx)
-        m = make_gpu_model(mnp)
-        assert m.ctx is ctx
-        self.models.append(m)
-        return m
-
-    def close(self):
-        torch.cuda.synchronize()
-        if self.saved is None:
-            self.tfluids._contexts.pop(self.dev, None)
-        else:
-            self.tfluids._contexts[self.dev] = self.saved
-        for m in self.models:
-            if m.h:
-                m.ctx.lib.tfl_cnn_destroy(m.ctx.h, m.h)
-                m.h = None
-        for ctx in self.made:
-            ctx.lib.tfl_destroy(ctx.h)
-            ctx.h = None
-
-
-@pytest.fixture
-def contexts():
-    cs = Contexts()
-    try:
-        yield cs
-    finally:
-        cs.close()
 
 
 @pytest.mark.gpu
@@ -551,11 +342,11 @@ def test_host_buffer_step_without_density(orc):
     """tfl_host_sim_step with density = NULL (no side stream, no density copies) returns what the device step
     without a density field leaves on the device."""
     from fluidnet_b200 import simulate, tfluids
-    from gpu_backend import make_gpu_model
+    from fluidnet_b200.model import ProjectionModel
     c = case((32, 32, 32), state="ubc-nodens")
     batch = make_batch(orc, c)
     assert "density" not in batch
-    gm = make_gpu_model(synth.make_model(True))
+    gm = ProjectionModel.from_model(synth.make_model(True))
     mconf = c["mconf"]
     dev = to_gpu(batch)
     ctx = tfluids.context()

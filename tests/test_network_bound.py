@@ -25,6 +25,7 @@ import oracle
 from oracle.model import F64, batch_norm, network
 from fluidnet_b200 import synth
 from network_bound import (Bound, check, excess, forward_bound, input_fields, model_inputs, scale_intervals)
+from scenes import bn_model
 
 FAULTS = ("plane", "bias", "tf32", "scale", "pad")
 
@@ -173,10 +174,6 @@ def problem(shape, is3d, nb, exotic=True, seed=5):
     U = synth.make_velocity(flags, is3d, amp=2.0, seed=seed) * np.arange(1, nb + 1, dtype=np.float32).reshape(-1, 1, 1, 1, 1)
     pDiv = (rs.rand(*flags.shape).astype(np.float32) - np.float32(0.5)) * np.float32(0.2)
     return pDiv, np.ascontiguousarray(U, np.float32), flags
-
-
-def bn_model(train, **kw):
-    return synth.make_model(True, batch_norm={"train": train}, **kw)
 
 
 SOUND = {

@@ -11,6 +11,7 @@ import torch.nn.functional as F
 import oracle
 from oracle.model import F64, batch_norm, conv64, model_input, network
 from fluidnet_b200 import synth
+from scenes import banks, bn_model
 
 
 def torch_stage(t, model, li, w, b, d, bn):
@@ -83,36 +84,21 @@ def torch_network(x, model):
     return t.numpy()
 
 
-def banks(num, agg, kind="mres", s=1, j=3):
-    return {"num": num, "split_stage": s, "join_stage": j, "aggregate": agg, "type": kind}
-
-
 # (is3d, model_type, banks, (nz, ny, nx))
 GRAPHS = {
     "3d-default": (True, "default", None, (6, 7, 9)),
     "3d-tog": (True, "tog", None, (8, 8, 12)),
     "3d-yang": (True, "yang", None, (5, 6, 7)),
-    "3d-mres-n2-concat": (True, "default", banks(2, "concat"), (8, 8, 12)),
-    "3d-mres-n3-add": (True, "default", banks(3, "add"), (8, 12, 8)),
+    "3d-mres-n2-concat": (True, "default", banks(2, "concat", "mres"), (8, 8, 12)),
+    "3d-mres-n3-add": (True, "default", banks(3, "add", "mres"), (8, 12, 8)),
     "3d-dilate-n2-concat": (True, "default", banks(2, "concat", "dilate"), (5, 7, 9)),
     "3d-dilate-n3-add-s2j4": (True, "default", banks(3, "add", "dilate", 2, 4), (6, 5, 11)),
     "2d-default": (False, "default", None, (1, 11, 13)),
     "2d-tog": (False, "tog", None, (1, 16, 24)),
     "2d-yang": (False, "yang", None, (1, 12, 9)),
-    "2d-mres-n2-add": (False, "default", banks(2, "add"), (1, 16, 12)),
+    "2d-mres-n2-add": (False, "default", banks(2, "add", "mres"), (1, 16, 12)),
     "2d-dilate-n3-concat": (False, "default", banks(3, "concat", "dilate"), (1, 9, 15)),
 }
-
-
-def bn_model(is3d, model_type, bk, train, affine=True, relu6=False, seed=4321):
-    m = synth.make_model(is3d, seed=seed, model_type=model_type, banks=bk,
-                         batch_norm={"train": train, "affine": affine})
-    if relu6:
-        m["nonlinType"] = "relu6"
-        # values well past 6 after the first stage: the clamp is exercised
-        w, b = m["layers"][0] if not isinstance(m["layers"][0], list) else m["layers"][0][0]
-        w *= np.float32(30.0)
-    return m
 
 
 def network_input(nb, shape, is3d, seed):
@@ -129,7 +115,7 @@ def test_bn_network_matches_torch(graph, variant):
     is3d, model_type, bk, shape = GRAPHS[graph]
     train = variant.startswith("train")
     relu6 = "relu6" in variant and model_type != "yang"
-    model = bn_model(is3d, model_type, bk, train, affine="noaffine" not in variant, relu6=relu6)
+    model = bn_model(train, is3d, model_type, bk, affine="noaffine" not in variant, relu6=relu6)
     x = network_input(2, shape, is3d, 17)
     got = network(model, x, F64)
     want = torch_network(x, model)
@@ -140,7 +126,7 @@ def test_bn_network_matches_torch(graph, variant):
 def test_relu6_clamps_in_the_restatement():
     """The first stage of a relu6 model really produces values above 6 before the clamp (so the GPU comparison
     exercises it)."""
-    model = bn_model(True, "default", None, True, relu6=True)
+    model = bn_model(True, relu6=True)
     x = network_input(1, (6, 7, 9), True, 3)
     w, b = model["layers"][0]
     pre = conv64(x.astype(np.float64), w, b, True)

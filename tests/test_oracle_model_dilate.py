@@ -8,9 +8,9 @@ import torch
 import torch.nn.functional as F
 
 import oracle
-from oracle.model import Float32Ops
 from fluidnet_b200 import synth
-from test_oracle_model_banks import torch_stage
+from oracle.model import Float32Ops
+from torch_graph import torch_stage
 
 
 def torch_stage_dilated(t, model, li, w, b, d):

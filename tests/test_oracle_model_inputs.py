@@ -2,16 +2,15 @@
 inputChannels, normalizeInput, normalizeInputFunc, normalizeInputChan, addPressureSkip) against an independent
 float64 evaluation: the divergence, the scale and the channel join restated here in numpy, the convolutions in
 torch.nn.functional.  This pins the semantics the GPU path is then compared with (tests/test_gpu_cnn_inputs.py)."""
-import itertools
-
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as F
 
+import itertools
 import oracle
 from fluidnet_b200 import synth
-from test_oracle_model_graph import torch_stack
+from torch_graph import torch_stack
 
 # Every inputChannels set the reference can build: flags on, and UDiv or div (tfluids.VelocityUpdate needs UDiv).
 SETS = [dict(pDiv=p, UDiv=u, div=d, flags=True) for p, u, d in itertools.product([False, True], repeat=3) if u or d]

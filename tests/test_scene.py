@@ -7,6 +7,7 @@ import pytest
 
 from fluidnet_b200 import formats, scene
 from fluidnet_b200.tfluids import CellType
+from scenes import write_binvox
 
 
 def vol(shape, cells, value=1.0):
@@ -114,20 +115,6 @@ def test_flip_diagonal_asserts_the_swapped_axes_are_equal(axis, shape):
 
 
 # ---- the scene -----------------------------------------------------------------------------------------------
-
-def write_binvox(path, dims, occ_flat):
-    """A .binvox file whose run-length body decodes, through the reference parser's quirks (formats.load_binvox), to
-    occ_flat: one (value, 1) pair per cell -- a run writes count + 1 = 2 cells and moves on by 1, so the next run
-    overwrites the second -- and a final pair the parser drops.  The last cell keeps the value of the one before it
-    (the parser stops there), so occ_flat must end with two equal values."""
-    assert occ_flat[-1] == occ_flat[-2]
-    body = bytearray()
-    for v in occ_flat:
-        body += bytes([int(v), 1])
-    body += bytes([0, 0])
-    head = "#binvox 1\ndim %d %d %d\ntranslate 0 0 0\nscale 1\ndata\n" % tuple(dims)
-    with open(path, "wb") as f:
-        f.write(head.encode("ascii") + bytes(body))
 
 
 def test_model_res_and_binvox_names():

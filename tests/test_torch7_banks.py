@@ -7,58 +7,7 @@ import numpy as np
 import pytest
 
 from fluidnet_b200 import synth, torch7
-from test_torch7_reader import GOLD, REF_MODEL, W
-
-
-def write_graph(path, nodes, is3d):
-    """An nn.gModule whose forwardnodes hold `nodes` = [(module class, fields or None, annotation or None)]."""
-    wr = W()
-
-    def conv(w, b):
-        cls = "cudnn.VolumetricConvolution" if is3d else "cudnn.SpatialConvolution"
-        k = w.shape[-1]
-        items = [("weight", lambda: wr.tensor(w if is3d else w[:, :, 0])), ("bias", lambda: wr.tensor(b)),
-                 ("nInputPlane", lambda: wr.number(w.shape[1])), ("nOutputPlane", lambda: wr.number(w.shape[0])),
-                 ("kH", lambda: wr.number(k)), ("kW", lambda: wr.number(k))]
-        if is3d:
-            items.append(("kT", lambda: wr.number(k)))
-        return lambda: wr.obj(cls, items)
-
-    def node(cls, fields, name):
-        mod = conv(*fields) if fields is not None else (lambda: wr.obj(cls, [("train", lambda: wr.boolean(False))]))
-        data = [("module", mod)]
-        if name:
-            data.append(("annotations", lambda: wr.table([("name", lambda: wr.string(name))])))
-        return lambda: wr.obj("nngraph.Node", [("data", lambda: wr.table(data))])
-
-    items = [(i + 1, node(*n)) for i, n in enumerate(nodes)]
-    wr.obj("nn.gModule", [("forwardnodes", lambda: wr.table(items))])
-    path.write_bytes(bytes(wr.b))
-
-
-def graph_nodes(model, extra=()):
-    """The nodes of lib/model.lua:27-401 for a synth.make_model model (with banks), in forward order."""
-    nodes = [("nn.Identity", None, "input"), ("tfluids.SetWallBcs", None, None), ("nn.JoinTable", None, "pModelInput")]
-    nl = len(model["layers"])
-    for s, layer in enumerate(model["layers"], start=1):
-        convs = layer if isinstance(layer, list) else [layer]
-        for bank, (w, b) in enumerate(convs, start=1):
-            nodes.append((None, (w, b), None if s == nl else "Bank %d: conv stage %d" % (bank, s)))
-            if s < nl:
-                nodes.append(("nn.ReLU", None, "Bank %d: non-linearity" % bank))
-    nodes += list(extra)
-    nodes += [("tfluids.VelocityUpdate", None, "UPred"), ("tfluids.SetWallBcs", None, "U")]
-    return nodes
-
-
-def mconf_of(is3d, **kw):
-    m = {"is3D": is3d, "modelType": "default", "nonlinType": "relu", "poolType": "avg", "banksNum": 1,
-         "banksSplitStage": 1, "banksJoinStage": 3, "banksAggregateMethod": "concat", "banksType": "mres",
-         "banksWeightShare": False, "addBatchNorm": False, "addPressureSkip": False, "normalizeInput": True,
-         "normalizeInputFunc": "std", "normalizeInputChan": "UDiv", "normalizeInputThreshold": 1e-5,
-         "inputChannels": {"pDiv": True, "div": True, "flags": True, "UDiv": False}}
-    m.update(kw)
-    return m
+from torch7_writer import GOLD, REF_MODEL, W, graph_nodes, mconf_of, write_graph
 
 
 @pytest.mark.parametrize("is3d,num,agg", [(True, 2, "concat"), (True, 3, "add"), (False, 2, "concat")])

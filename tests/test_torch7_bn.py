@@ -7,115 +7,7 @@ import numpy as np
 import pytest
 
 from fluidnet_b200 import synth, torch7
-from test_torch7_banks import mconf_of
-from test_torch7_reader import W
-
-
-def bn_graph(model, is3d, nonlin="nn.ReLU", interleave=False, cudnn=True, train=True, old_format=False,
-             drop=None, misplace=False, channels=None, train_of=None):
-    """lib/model.lua's nodes for a synth.make_model(batch_norm=...) model: per stage and bank conv -> non-linearity ->
-    BN (each node's child the next), the banks' chains one after another or interleaved node by node in
-    forwardnodes.  Returns [(class, fields, annotation, [child indices])]."""
-    nodes = [("nn.Identity", None, "input", [1]), ("nn.JoinTable", None, "pModelInput", [])]
-    prev = [1]          # the nodes feeding the next stage
-    nl = len(model["layers"])
-    bnl = model["batchNorm"]["layers"]
-    kind = ("cudnn." if cudnn else "nn.") + ("Volumetric" if is3d else "Spatial") + "BatchNormalization"
-    for s, layer in enumerate(model["layers"], start=1):
-        convs = layer if isinstance(layer, list) else [layer]
-        if s == nl:
-            i = len(nodes)
-            nodes.append((None, convs[0], None, []))
-            for p in prev:
-                nodes[p][3].append(i)
-            break
-        bns = bnl[s - 1] if isinstance(bnl[s - 1], list) else [bnl[s - 1]]
-        chains = []
-        for bank, ((w, b), e) in enumerate(zip(convs, bns), start=1):
-            fields = dict(e)
-            if channels is not None and (s, bank) == channels:
-                fields["running_mean"] = np.zeros(len(e["running_mean"]) + 1, np.float32)
-            tr = train if train_of is None or (s, bank) != train_of else not train
-            chains.append([(None, (w, b), "Bank %d: conv stage %d" % (bank, s)),
-                           (nonlin, None, "Bank %d: non-linearity" % bank),
-                           (kind, ("bn", fields, tr, old_format), None)])
-        if drop is not None:
-            chains = [c if (s, k + 1) != drop else c[:2] for k, c in enumerate(chains)]
-        order = [n for step in zip(*[c + [None] * (3 - len(c)) for c in chains]) for n in step if n is not None] \
-            if interleave else [n for c in chains for n in c]
-        idx = {}
-        for n in order:
-            idx[id(n)] = len(nodes)
-            nodes.append((n[0], n[1], n[2], []))
-        ends = []
-        for c in chains:
-            ids = [idx[id(n)] for n in c]
-            for a, b in zip(ids, ids[1:]):
-                nodes[a][3].append(b)
-            for p in prev:
-                nodes[p][3].append(ids[0])
-            ends.append(ids[-1])
-        if misplace and s == 1:
-            # a BN node fed by the join of the banks, not by a stage's non-linearity
-            j = len(nodes)
-            nodes.append(("nn.JoinTable", None, None, []))
-            k = len(nodes)
-            nodes.append((kind, ("bn", dict(bns[0]), train, False), None, []))
-            nodes[j][3].append(k)
-            for e_ in ends:
-                nodes[e_][3].append(j)
-        prev = ends
-    return nodes
-
-
-def write_bn_graph(path, nodes, is3d):
-    wr = W()
-    written = {}
-
-    def conv(w, b):
-        cls = "cudnn.VolumetricConvolution" if is3d else "cudnn.SpatialConvolution"
-        k = w.shape[-1]
-        items = [("weight", lambda: wr.tensor(w if is3d else w[:, :, 0])), ("bias", lambda: wr.tensor(b)),
-                 ("nInputPlane", lambda: wr.number(w.shape[1])), ("nOutputPlane", lambda: wr.number(w.shape[0])),
-                 ("kH", lambda: wr.number(k)), ("kW", lambda: wr.number(k))]
-        if is3d:
-            items.append(("kT", lambda: wr.number(k)))
-        return lambda: wr.obj(cls, items)
-
-    def bn_mod(cls, fields, train, old):
-        items = [("running_mean", lambda: wr.tensor(fields["running_mean"])), ("eps", lambda: wr.number(fields["eps"])),
-                 ("train", lambda: wr.boolean(train))]
-        items.append(("running_std" if old else "running_var", lambda: wr.tensor(fields["running_var"])))
-        if fields.get("weight") is not None:
-            items += [("weight", lambda: wr.tensor(fields["weight"])), ("bias", lambda: wr.tensor(fields["bias"]))]
-        return lambda: wr.obj(cls, items)
-
-    def node(i):
-        if i in written:
-            wr.i32(4)
-            wr.i32(written[i])
-            return
-        cls, fields, name, children = nodes[i]
-        if fields is None:
-            mod = lambda: wr.obj(cls, [("train", lambda: wr.boolean(True))])
-        elif isinstance(fields[0], str):
-            mod = bn_mod(cls, *fields[1:])
-        else:
-            mod = conv(*fields)
-        data = [("module", mod)]
-        if name:
-            data.append(("annotations", lambda: wr.table([("name", lambda: wr.string(name))])))
-        wr.i32(4)
-        written[i] = wr.next
-        wr.i32(wr.next)
-        wr.next += 1
-        wr.s("V 1")
-        wr.s("nngraph.Node")
-        wr.table([("data", lambda: wr.table(data)),
-                  ("children", lambda: wr.table([(k + 1, (lambda c=c: node(c))) for k, c in enumerate(children)]))])
-
-    wr.obj("nn.gModule", [("forwardnodes", lambda: wr.table([(i + 1, (lambda i=i: node(i))) for i in range(len(nodes))]))])
-    path.write_bytes(bytes(wr.b))
+from torch7_writer import bn_graph, mconf_for, mconf_of, write_bn_graph
 
 
 def load_bn(tmp_path, model, is3d, **kw):
@@ -135,15 +27,6 @@ CASES = {   # (is3d, banks, cudnn / affine, train, interleave)
     "2d-mres-n2-add-interleaved": (False, {"num": 2, "split_stage": 2, "join_stage": 4, "aggregate": "add"},
                                    True, False, True),
 }
-
-
-def mconf_for(is3d, bk, affine, **kw):
-    extra = {"batchNormEps": 1e-4}
-    if bk:
-        extra.update({"banksNum": bk["num"], "banksSplitStage": bk["split_stage"], "banksJoinStage": bk["join_stage"],
-                      "banksAggregateMethod": bk["aggregate"], "banksType": bk.get("type", "mres")})
-    extra.update(kw)
-    return mconf_of(is3d, addBatchNorm=True, batchNormAffine=affine, **extra)
 
 
 @pytest.mark.parametrize("case", list(CASES))

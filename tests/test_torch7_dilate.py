@@ -7,63 +7,7 @@ import numpy as np
 import pytest
 
 from fluidnet_b200 import synth, torch7
-from test_torch7_banks import mconf_of
-from test_torch7_reader import W
-
-
-def conv_module(wr, w, b, is3d, d=1, pad=None, stride=1):
-    """A convolution module: cudnn.{Spatial,Volumetric}Convolution for d = 1, nn.*DilatedConvolution (with the
-    fields of torch's nn package) otherwise; pad defaults to d (k-1)/2."""
-    k = w.shape[-1]
-    pad = d * (k - 1) // 2 if pad is None else pad
-    axes = ("T", "W", "H") if is3d else ("W", "H")
-    if d == 1:
-        cls = "cudnn.VolumetricConvolution" if is3d else "cudnn.SpatialConvolution"
-    else:
-        cls = "nn.VolumetricDilatedConvolution" if is3d else "nn.SpatialDilatedConvolution"
-    items = [("weight", lambda: wr.tensor(w if is3d else w[:, :, 0])), ("bias", lambda: wr.tensor(b)),
-             ("nInputPlane", lambda: wr.number(w.shape[1])), ("nOutputPlane", lambda: wr.number(w.shape[0]))]
-    for a in axes:
-        items += [("k" + a, lambda: wr.number(k)), ("d" + a, lambda: wr.number(stride)),
-                  ("pad" + a, lambda: wr.number(pad))]
-        if d != 1:
-            items.append(("dilation" + a, lambda: wr.number(d)))
-    return lambda: wr.obj(cls, items)
-
-
-def write_dilated(path, model, is3d, dil_of=None, extra=()):
-    """The nodes of lib/model.lua:27-401 for a synth.make_model model; bank i's convolution is dilated by
-    dil_of(bank, stage) (default: 2^(bank-1), as the reference builds it), with keyword overrides from a dict."""
-    wr = W()
-    dil_of = dil_of or (lambda bank, stage: {"d": 2 ** (bank - 1)})
-
-    def plain(cls, name):
-        data = [("module", lambda: wr.obj(cls, [("train", lambda: wr.boolean(False))]))]
-        if name:
-            data.append(("annotations", lambda: wr.table([("name", lambda: wr.string(name))])))
-        return lambda: wr.obj("nngraph.Node", [("data", lambda: wr.table(data))])
-
-    def conv_node(w, b, name, kw):
-        data = [("module", conv_module(wr, w, b, is3d, **kw))]
-        if name:
-            data.append(("annotations", lambda: wr.table([("name", lambda: wr.string(name))])))
-        return lambda: wr.obj("nngraph.Node", [("data", lambda: wr.table(data))])
-
-    nodes = [plain("nn.Identity", "input"), plain("tfluids.SetWallBcs", None), plain("nn.JoinTable", "pModelInput")]
-    nl = len(model["layers"])
-    for s, layer in enumerate(model["layers"], start=1):
-        convs = layer if isinstance(layer, list) else [layer]
-        for bank, (w, b) in enumerate(convs, start=1):
-            name = None if s == nl else "Bank %d: conv stage %d" % (bank, s)
-            kw = dil_of(bank, s) if (s < nl and len(convs) > 1) else {}
-            nodes.append(conv_node(w, b, name, kw))
-            if s < nl:
-                nodes.append(plain("nn.ReLU", "Bank %d: non-linearity" % bank))
-    nodes += [plain(*e) for e in extra]
-    nodes += [plain("tfluids.VelocityUpdate", "UPred"), plain("tfluids.SetWallBcs", "U")]
-    items = [(i + 1, n) for i, n in enumerate(nodes)]
-    wr.obj("nn.gModule", [("forwardnodes", lambda: wr.table(items))])
-    path.write_bytes(bytes(wr.b))
+from torch7_writer import mconf_of, write_dilated
 
 
 def dilate(num, agg, s=1, j=3):

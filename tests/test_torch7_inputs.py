@@ -7,7 +7,7 @@ import numpy as np
 import pytest
 
 from fluidnet_b200 import synth, torch7
-from test_torch7_banks import graph_nodes, mconf_of, write_graph
+from torch7_writer import graph_nodes, mconf_of, write_graph
 
 ALL = {"pDiv": True, "UDiv": True, "div": True, "flags": True}
 U_ONLY = {"pDiv": False, "UDiv": True, "div": False, "flags": True}

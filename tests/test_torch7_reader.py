@@ -3,58 +3,12 @@ this library (SURVEY.md section 8f-2).  A writer for the same format lives here 
 is exercised without Torch7; the trained 2-D model the reference ships is read when /root/reference is
 present and must match the committed fixture (tests/golden/myModel2D_layers.npz)."""
 import os
-import struct
 
 import numpy as np
 import pytest
 
 from fluidnet_b200 import torch7
-
-GOLD = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "myModel2D_layers.npz")
-REF_MODEL = "/root/reference/data/models/myModel2D"
-
-
-class W:
-    """Minimal Torch7 binary writer (torch7/File.lua conventions)."""
-
-    def __init__(self):
-        self.b = bytearray()
-        self.next = 1
-
-    def i32(self, v): self.b += struct.pack("<i", v)
-    def i64(self, v): self.b += struct.pack("<q", v)
-    def s(self, v): self.i32(len(v)); self.b += v.encode()
-
-    def number(self, v): self.i32(1); self.b += struct.pack("<d", v)
-    def string(self, v): self.i32(2); self.s(v)
-    def boolean(self, v): self.i32(5); self.i32(1 if v else 0)
-
-    def table(self, items):
-        self.i32(3); self.i32(self.next); self.next += 1
-        self.i32(len(items))
-        for k, wv in items:
-            (self.number if not isinstance(k, str) else self.string)(k)
-            wv()
-
-    def backref_table(self, idx): self.i32(3); self.i32(idx)
-
-    def tensor(self, a, cls="torch.FloatTensor", storage_cls="torch.FloatStorage"):
-        a = np.ascontiguousarray(a, np.float32)
-        self.i32(4); self.i32(self.next); self.next += 1
-        self.s("V 1"); self.s(cls)
-        self.i32(a.ndim)
-        for d in a.shape: self.i64(d)
-        stride = [int(np.prod(a.shape[i + 1:])) for i in range(a.ndim)]
-        for d in stride: self.i64(d)
-        self.i64(1)
-        self.i32(4); self.i32(self.next); self.next += 1
-        self.s("V 1"); self.s(storage_cls)
-        self.i64(a.size); self.b += a.tobytes()
-
-    def obj(self, cls, items):
-        self.i32(4); self.i32(self.next); self.next += 1
-        self.s("V 1"); self.s(cls)
-        self.table(items)
+from torch7_writer import GOLD, REF_MODEL, W
 
 
 def test_reader_round_trip(tmp_path):
