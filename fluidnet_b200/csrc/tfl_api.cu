@@ -1143,8 +1143,7 @@ struct tfl_step_graph {
   GraphPtr graph;
   GraphExecPtr exec;
   long long launches = 0;       // kernels in one replay outside the PCG loop
-  unsigned long long arena_gen = 0, fcache_gen = 0, act_gen = 0;   // generations of the captured buffers
-  tfl_cnn* cnn = nullptr;       // the captured model (its act_gen is checked), or null
+  BufferGens gens;              // generations of the captured buffers
 };
 
 extern "C" {
@@ -1200,10 +1199,7 @@ int tfl_step_graph_create(tfl_ctx* ctx, const tfl_state* state, const tfl_mconf*
     return fail(ctx, "step_graph: cudaGraphInstantiate failed");
   }
   g->exec.reset(exec);
-  g->arena_gen = ctx->arena_gen;
-  g->fcache_gen = ctx->fcache.gen;
-  g->cnn = cnn;
-  g->act_gen = cnn ? cnn->act_gen : 0;
+  g->gens = buffer_gens(ctx, cnn);
   *out = g.release();
   return 0;
 }
@@ -1212,11 +1208,7 @@ int tfl_step_graph_launch(tfl_ctx* ctx, tfl_step_graph* g) {
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (!g || !g->exec) return fail(ctx, "step_graph is nil");
-  const char* stale = g->arena_gen != ctx->arena_gen      ? "the context's scratch arena"
-                      : g->fcache_gen != ctx->fcache.gen  ? "the context's flag cache"
-                      : g->cnn && g->act_gen != g->cnn->act_gen ? "the model's activation buffers"
-                                                                : nullptr;
-  if (stale)
+  if (const char* stale = reallocated_buffer(ctx, g->gens))
     return fail(ctx, "step_graph: stale graph: %s reallocated since the capture (a call on another grid shape or a "
                      "larger grid); replaying would touch freed memory: capture the step again", stale);
   TFL_CUDA(ctx, cudaGraphLaunch(g->exec.get(), ctx->stream));

@@ -143,6 +143,28 @@ struct tfl_cnn {
   DevPtr<float> part;
 };
 
+// The generations of the library-owned buffers a step graph holds pointers into (the context's scratch arena and flag
+// cache, the model's activation buffers), taken at capture and compared before every replay.
+struct BufferGens {
+  unsigned long long arena = 0, fcache = 0, act = 0;
+  const tfl_cnn* cnn = nullptr;     // the captured model (its act_gen is compared), or null
+};
+inline BufferGens buffer_gens(const tfl_ctx* ctx, const tfl_cnn* cnn) {
+  BufferGens g;
+  g.arena = ctx->arena_gen;
+  g.fcache = ctx->fcache.gen;
+  g.cnn = cnn;
+  g.act = cnn ? cnn->act_gen : 0;
+  return g;
+}
+// The first of those buffers reallocated since `then`, by name, or null.
+inline const char* reallocated_buffer(const tfl_ctx* ctx, const BufferGens& then) {
+  return then.arena != ctx->arena_gen            ? "the context's scratch arena"
+         : then.fcache != ctx->fcache.gen        ? "the context's flag cache"
+         : then.cnn && then.act != then.cnn->act_gen ? "the model's activation buffers"
+                                                  : nullptr;
+}
+
 // Every entry point runs on the context's device whatever the caller's current device is, and leaves the
 // caller's current device as it found it (a host with several contexts / GPUs in one thread).
 // One NVTX range per entry point (named after the function): nsys / ncu --nvtx timelines show the operators.

@@ -1,5 +1,5 @@
 // C ABI of the z-slab driver (include/tfl.h): the NCCL loader, the halo exchange and all-reduce kernels, and
-// tfl_comm_* / tfl_slab_sim_*.
+// tfl_comm_* / tfl_slab_sim_* / tfl_slab_graph_*.
 #include <dlfcn.h>
 #include <string.h>
 #include <algorithm>
@@ -70,12 +70,14 @@ NcclApi* nccl_api() {
 // A rank's inbox: the one allocation its peers store into over peer memory (exported as one CUDA IPC handle).  Every
 // rank's has this layout, in floats, with the counters written and waited on as tfl_peer.cuh describes:
 //   [3 phases][2 from][xbuf_side]        halo messages (from 0: the rank below, 1: the rank above)
-//   [64]                                  their counters, [phase][from], carrying step_no
-//   [2 parities][kMaxRanks][2] doubles    the all-reduce's pair from each rank, parity = step_no & 1
-//   [2 parities][kMaxRanks]               their counters, carrying step_no
-//   [2 parities][2 from][p_side]          the Jacobi p exchange's messages, parity = jseq & 1
-//   [64]                                  their counters, [parity][from], carrying jseq
+//   [64]                                  their counters, [phase][from], carrying the step number
+//   [2 parities][kMaxRanks][2] doubles    the all-reduce's pair from each rank, parity = step number & 1
+//   [2 parities][kMaxRanks]               their counters, carrying the step number
+//   [2 parities][2 from][p_side]          the Jacobi p exchange's messages, parity = p sequence & 1
+//   [64]                                  their counters, [parity][from], carrying the p sequence
 // Alternating parities let a rank push the next all-reduce or p exchange while its peer still reads the current one.
+// The step number and the p sequence live on the device (tfl_slab_sim::seq, SlabSeq), so a replayed step
+// (tfl_slab_graph_launch) advances them exactly as a direct one does.
 struct SlabInbox {
   size_t xbuf_side, p_side;             // floats of one halo message / one p message
   static constexpr int kCounterFloats = 64;
@@ -122,17 +124,27 @@ struct tfl_slab_sim {
   std::vector<float*> all_inbox;               // every rank's inbox (own pointer at [rank]): the all-reduce's targets
   DevPtr<float*> all_inbox_dev;                // the same table on the device
   DevPtr<unsigned int> push_done;              // CTAs of the running push kernel that finished their stores
+  // The exchanges' sequence numbers, two words each (SlabSeq): [0, 2) the step number, which the halo and all-reduce
+  // counters carry, and [2, 4) the p sequence, which the Jacobi p exchanges and tfl_slab_sim_monitor_record advance.
+  DevPtr<unsigned int> seq;
   bool peer_ok = false;
-  unsigned int step_no = 0;
+  unsigned long long peer_gen = 0;             // bumped by every tfl_slab_sim_ipc_connect (the mapped inboxes change)
+  bool capturing = false;                      // tfl_slab_graph_create is capturing a step
+  // The last direct step, which sized every buffer a capture of the same step uses (tfl_slab_graph_create)
+  struct {
+    bool done = false;
+    const tfl_cnn* cnn = nullptr;
+    int sim_method = -1;
+    BufferGens gens;
+  } last;
   EventPtr ev[4][2];
   size_t bytes_sent[3] = {0, 0, 0};
   // Jacobi projection (simMethod 'jacobi'): divergence, second p buffer and mask of the local slab; the p exchanges
-  // land in their own inbox area and carry the monotone sequence number jseq instead of step_no.
+  // land in their own inbox area and carry the p sequence instead of the step number.
   DevPtr<float> div;
   DevPtr<float> p2;
   DevPtr<unsigned char> mask;
   size_t p_side = 0;                // halo planes of one channel
-  unsigned int jseq = 0;
   std::vector<int32_t> jsched;
   std::vector<EventPtr> jev;        // [2 * exchange] begin / end of the last step's p exchanges
   int jx = 0;                       // p exchanges of the last step
@@ -257,7 +269,7 @@ int tfl_slab_sim_create(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32
     return fail(ctx, kFailed);
   if (s->world > 1 &&
       (!(s->inbox = dev_zeros<float>(s->layout().floats())) ||
-       !(s->push_done = dev_zeros<unsigned int>(1))))
+       !(s->push_done = dev_zeros<unsigned int>(1)) || !(s->seq = dev_zeros<unsigned int>(4))))
     return fail(ctx, kFailed);
   for (auto& pr : s->ev)
     for (EventPtr& e : pr)
@@ -348,48 +360,73 @@ __global__ void k_slab_pack(SlabPack d) {
   else d.scatter<false>(d.recv_lo, d.recv_hi);
 }
 
+// The sequence number of one peer-memory exchange, read on the device.  word[0] is the number of the sequence's last
+// exchange.  The push takes word[0] + advance (advance 1: a new number -- the step's first halo exchange, every p
+// exchange; 0: the step's later halos) and leaves it in word[1]; the pull takes word[1] and commits it to word[0].
+// Every CTA reads the word the kernel does not write and writes the same value, so neither kernel races with itself,
+// and stream order carries the number from push to pull and on to the next exchange.  The message and counter of
+// parity 1 lie buf_stride floats / flag_stride words past parity 0's (both 0 for the halos' single slot).
+struct SlabSeq {
+  unsigned int* word;
+  unsigned int advance;
+  long long buf_stride;
+  int flag_stride;
+  template <typename T> __device__ __forceinline__ T* at(T* p0, unsigned int seq, long long stride) const {
+    return p0 ? p0 + (seq & 1u) * stride : nullptr;
+  }
+};
+
 // Peer-memory exchange, sending half: every channel's boundary planes are written straight into the neighbours'
-// inboxes (remote stores over NVLink), then the last CTA publishes the step number in the neighbours' counters.
+// inboxes (remote stores over NVLink), then the last CTA publishes the sequence number in the neighbours' counters.
+// The buffers and counters are given for parity 0.
 __global__ void k_slab_push(SlabPack d, float* peer_lo_buf, float* peer_hi_buf, unsigned int* peer_lo_flag,
-                            unsigned int* peer_hi_flag, unsigned int step, unsigned int* done) {
-  d.gather(peer_lo_buf, peer_hi_buf);
-  last_cta_publish(done, gridDim.x, threadIdx.x == 0, peer_lo_flag, peer_hi_flag, step);
+                            unsigned int* peer_hi_flag, SlabSeq q, unsigned int* done) {
+  const unsigned int seq = q.word[0] + q.advance;
+  if (threadIdx.x == 0) q.word[1] = seq;
+  d.gather(q.at(peer_lo_buf, seq, q.buf_stride), q.at(peer_hi_buf, seq, q.buf_stride));
+  last_cta_publish(done, gridDim.x, threadIdx.x == 0, q.at(peer_lo_flag, seq, q.flag_stride),
+                   q.at(peer_hi_flag, seq, q.flag_stride), seq);
 }
-// ... receiving half: wait until the neighbours' counters have reached this step, then scatter the inbox into the
-// ghost planes.  A neighbour that never arrives raises the fault counter, and nothing is scattered.
+// ... receiving half: wait until the neighbours' counters have reached the push's number, then scatter the inbox into
+// the ghost planes.  A neighbour that never arrives raises the fault counter, and nothing is scattered.
 __global__ void k_slab_pull(SlabPack d, const float* buf_lo, const float* buf_hi, const unsigned int* flag_lo,
-                            const unsigned int* flag_hi, unsigned int step, unsigned long long* faults) {
+                            const unsigned int* flag_hi, SlabSeq q, unsigned long long* faults) {
   __shared__ int ok;
+  const unsigned int seq = q.word[1];
   if (threadIdx.x == 0) {
+    q.word[0] = seq;
     ok = 1;
     const long long t0 = clock64();
     for (int sde = 0; sde < 2; sde++) {
-      const unsigned int* f = sde ? flag_hi : flag_lo;
-      if (f && !wait_seq(f, step, t0, 200)) ok = 0;
+      const unsigned int* f = q.at(sde ? flag_hi : flag_lo, seq, q.flag_stride);
+      if (f && !wait_seq(f, seq, t0, 200)) ok = 0;
     }
     if (!ok && blockIdx.x == 0 && faults) atomicAdd(faults, 1ULL);
   }
   __syncthreads();
   if (!ok) return;
-  d.scatter<true>(buf_lo, buf_hi);
+  d.scatter<true>(q.at(buf_lo, seq, q.buf_stride), q.at(buf_hi, seq, q.buf_stride));
 }
 
 // All-reduce of the two partial sums over peer memory: every rank stores its pair into slot [parity][rank] of every
 // rank's inbox and raises that rank's counter [parity][rank]; then waits for all counters of its own inbox and adds
 // the pairs in rank order (the same order on every rank: identical results everywhere, independent of timing).
+// `step_word` is the step number's word[0] (SlabSeq), which the step's halo exchanges have already advanced.
 __global__ void k_sum_push(const double* __restrict__ mine, float* const* __restrict__ inboxes, SlabInbox box, int rank,
-                           int world, unsigned int step) {
+                           int world, const unsigned int* step_word) {
   const int t = threadIdx.x;
   if (t >= world) return;
+  const unsigned int step = *step_word;
   const int parity = step & 1;
   double* slot = box.sum_slot(inboxes[t], parity, rank);
   slot[0] = mine[0];
   slot[1] = mine[1];
   publish_seq(box.sum_flag(inboxes[t], parity, rank), step);
 }
-__global__ void k_sum_pull(double* __restrict__ out, float* inbox, SlabInbox box, int world, unsigned int step,
-                           unsigned long long* faults) {
+__global__ void k_sum_pull(double* __restrict__ out, float* inbox, SlabInbox box, int world,
+                           const unsigned int* step_word, unsigned long long* faults) {
   __shared__ int ok;
+  const unsigned int step = *step_word;
   const int t = threadIdx.x, parity = step & 1;
   if (t == 0) ok = 1;
   __syncthreads();
@@ -416,23 +453,29 @@ __global__ void k_sum_pull(double* __restrict__ out, float* inbox, SlabInbox box
 // has pushed e + 1, which that neighbour does after scattering e).
 constexpr int kPhaseP = 4;
 
+// Records one of the step's statistics events; while a step is captured (tfl_slab_graph_create) it becomes an
+// event-record node, so that the statistics after a replay time the replayed exchanges.
+int slab_event(tfl_ctx* ctx, const tfl_slab_sim* s, const EventPtr& e) {
+  TFL_CUDA(ctx, cudaEventRecordWithFlags(e.get(), ctx->stream, s->capturing ? cudaEventRecordExternal : cudaEventRecordDefault));
+  return 0;
+}
+
 // Refresh `width` ghost planes on both sides of the listed fields from the neighbours' owned planes.
 int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl_grid*> fields, int width, int phase) {
   const bool pph = phase == kPhaseP;
   if (!pph) {
-    TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][0].get(), ctx->stream));
+    if (slab_event(ctx, s, s->ev[phase][0])) return 1;
     s->bytes_sent[phase] = 0;
   }
   if (s->world > 1 && width > 0 && (ctx->comm || s->peer_ok)) {
     if (width > s->halo) return fail(ctx, "slab exchange of %d planes exceeds the halo (%d)", width, s->halo);
     if (pph) {
-      s->jseq += 1;
       while ((int)s->jev.size() < 2 * (s->jx + 1)) {
         cudaEvent_t e = nullptr;
         TFL_CUDA(ctx, cudaEventCreate(&e));
         s->jev.emplace_back(e);
       }
-      TFL_CUDA(ctx, cudaEventRecord(s->jev[2 * s->jx].get(), ctx->stream));
+      if (slab_event(ctx, s, s->jev[2 * s->jx])) return 1;
     }
     SlabPack d;
     d.nchan = 0;
@@ -450,18 +493,20 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
     const int blocks = (int)std::min<size_t>((2 * side + 255) / 256, 132 * 4);
     if (s->peer_ok) {
       const SlabInbox box = s->layout();
-      const unsigned int seq = pph ? s->jseq : s->step_no, par = seq & 1u;
-      auto buf = [&](float* base, int from) { return pph ? box.p_buf(base, par, from) : box.halo(base, phase, from); };
-      auto flag = [&](float* base, int from) { return pph ? box.p_flag(base, par, from) : box.halo_flag(base, phase, from); };
+      // the step's first halo exchange takes the next step number, every p exchange the next p sequence number
+      const SlabSeq q = pph ? SlabSeq{s->seq.get() + 2, 1u, 2 * (long long)s->p_side, 2}
+                            : SlabSeq{s->seq.get(), phase == 0 ? 1u : 0u, 0, 0};
+      auto buf = [&](float* base, int from) { return pph ? box.p_buf(base, 0, from) : box.halo(base, phase, from); };
+      auto flag = [&](float* base, int from) { return pph ? box.p_flag(base, 0, from) : box.halo_flag(base, phase, from); };
       d.send_lo = d.send_hi = d.recv_lo = d.recv_hi = nullptr;
       // my first owned planes land in the lower neighbour's "from above" slot, my last ones in the upper neighbour's "from below"
       k_slab_push<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(s->peer_inbox[0], 1) : nullptr, hi ? buf(s->peer_inbox[1], 0) : nullptr,
                                                    lo ? flag(s->peer_inbox[0], 1) : nullptr, hi ? flag(s->peer_inbox[1], 0) : nullptr,
-                                                   seq, s->push_done.get());
+                                                   q, s->push_done.get());
       float* inbox = s->inbox.get();
       k_slab_pull<<<blocks, 256, 0, ctx->stream>>>(d, lo ? buf(inbox, 0) : nullptr, hi ? buf(inbox, 1) : nullptr,
                                                    lo ? flag(inbox, 0) : nullptr, hi ? flag(inbox, 1) : nullptr,
-                                                   seq, ctx->counters.get());
+                                                   q, ctx->counters.get());
       sent = (size_t)(lo + hi) * side * 4;
       ctx->launches += 2;
     } else {
@@ -488,15 +533,14 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
       ctx->launches += 2;
     }
     if (pph) {
-      TFL_CUDA(ctx, cudaEventRecord(s->jev[2 * s->jx + 1].get(), ctx->stream));
+      if (slab_event(ctx, s, s->jev[2 * s->jx + 1])) return 1;
       s->jx += 1;
       s->jbytes += sent;
       return 0;
     }
     s->bytes_sent[phase] = sent;
   }
-  if (!pph) TFL_CUDA(ctx, cudaEventRecord(s->ev[phase][1].get(), ctx->stream));
-  return 0;
+  return pph ? 0 : slab_event(ctx, s, s->ev[phase][1]);
 }
 
 struct SlabScope {       // slab placement of the context for the enclosed calls
@@ -537,8 +581,7 @@ int slab_jacobi_projection(tfl_ctx* ctx, tfl_slab_sim* s, int iters) {
   s->jsched.resize((size_t)nblk * TFL_JACOBI_BLOCK_INTS);
   tfl_slab_jacobi_schedule(s->gnz, s->world, s->rank, s->margin, iters, planes, s->jsched.data(), nblk);
   if (slab_exchange(ctx, s, {&st.U}, planes[2], 2)) return 1;
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0].get(), ctx->stream));          // no all-reduce on this path
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][1].get(), ctx->stream));
+  if (slab_event(ctx, s, s->ev[3][0]) || slab_event(ctx, s, s->ev[3][1])) return 1;   // no all-reduce on this path
   tfl_grid dv = st.p;
   dv.data = s->div.get();
   Geo g;
@@ -658,24 +701,31 @@ int tfl_jacobi_slab_block(tfl_ctx* ctx, const tfl_grid* pa, const tfl_grid* pb, 
   return check_launch(ctx, "jacobi_slab_block");
 }
 
-// One tfluids.simulate (lib/simulate.lua:175-327; simMethod 'convnet' or 'jacobi') on this rank's slab.  Asynchronous.
-int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cnn* cnn) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
-  if (!s || !mc) return fail(ctx, "slab_sim_step: nil argument");
+}  // extern "C"
+
+namespace {
+
+// What tfl_slab_sim_step refuses, before anything is launched; the messages start with `who`.
+int slab_step_refusal(tfl_ctx* ctx, const tfl_slab_sim* s, const tfl_mconf* mc, tfl_cnn* cnn, const char* who) {
+  if (!s || !mc) return fail(ctx, "%s: nil argument", who);
   const bool jacobi = mc->sim_method == TFL_SIM_JACOBI;
   if (mc->sim_method == TFL_SIM_PCG)
-    return fail(ctx, "slab_sim_step: simMethod 'pcg' is not decomposed: the IC(0) triangular solves of its "
-                     "preconditioner sweep the whole domain in order and do not shard over z-slabs");
+    return fail(ctx, "%s: simMethod 'pcg' is not decomposed: the IC(0) triangular solves of its "
+                     "preconditioner sweep the whole domain in order and do not shard over z-slabs", who);
   if (!jacobi && mc->sim_method != TFL_SIM_CONVNET)
-    return fail(ctx, "slab_sim_step: mconf.simMethod (%d) is not a valid option", mc->sim_method);
-  if (!jacobi && !cnn) return fail(ctx, "slab_sim_step: simMethod 'convnet' needs a model");
+    return fail(ctx, "%s: mconf.simMethod (%d) is not a valid option", who, mc->sim_method);
+  if (!jacobi && !cnn) return fail(ctx, "%s: simMethod 'convnet' needs a model", who);
   if (!jacobi && cnn_slab_check(ctx, cnn, s->margin, s->gnz, s->ny, s->nx, s->zoff, s->nz, s->own_lo, s->own_hi))
-    return fail(ctx, "slab_sim_step: %s", ctx->err.c_str());
-  if (jacobi && mc->max_iter < 0) return fail(ctx, "slab_sim_step: At least 1 iteration is needed (maxIter < 1)");
-  if (s->world != ctx->comm_world || s->rank != ctx->comm_rank) return fail(ctx, "slab_sim_step: communicator changed");
+    return fail(ctx, "%s: %s", who, ctx->err.c_str());
+  if (jacobi && mc->max_iter < 0) return fail(ctx, "%s: At least 1 iteration is needed (maxIter < 1)", who);
+  if (s->world != ctx->comm_world || s->rank != ctx->comm_rank) return fail(ctx, "%s: communicator changed", who);
+  return 0;
+}
+
+// The step of tfl_slab_sim_step after its refusals: enqueued directly or captured (tfl_slab_graph_create).
+int slab_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cnn* cnn) {
+  const bool jacobi = mc->sim_method == TFL_SIM_JACOBI;
   const tfl_state& st = s->st;
-  s->step_no += 1;                      // what the peers' counters must reach in this step's exchanges
   struct StepMark {                     // the flags are refreshed once per step (the two advections share them)
     tfl_ctx* c;
     explicit StepMark(tfl_ctx* cc) : c(cc) { c->in_slab_step = true; c->fcache.fresh_for = nullptr; }
@@ -727,15 +777,15 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
     SlabScope scope(ctx, s, s->own_lo, s->own_hi);
     if (tfl_cnn_stats(ctx, &st.U, &st.flags, &u1, sums)) return 1;
   }
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][0].get(), ctx->stream));
+  if (slab_event(ctx, s, s->ev[3][0])) return 1;
   if (s->world > 1 && s->peer_ok && s->all_inbox_dev) {
-    k_sum_push<<<1, kMaxRanks, 0, ctx->stream>>>(sums, s->all_inbox_dev.get(), s->layout(), s->rank, s->world, s->step_no);
-    k_sum_pull<<<1, kMaxRanks, 0, ctx->stream>>>(sums, s->inbox.get(), s->layout(), s->world, s->step_no, ctx->counters.get());
+    k_sum_push<<<1, kMaxRanks, 0, ctx->stream>>>(sums, s->all_inbox_dev.get(), s->layout(), s->rank, s->world, s->seq.get());
+    k_sum_pull<<<1, kMaxRanks, 0, ctx->stream>>>(sums, s->inbox.get(), s->layout(), s->world, s->seq.get(), ctx->counters.get());
     ctx->launches += 2;
   } else if (s->world > 1 && ctx->comm) {
     TFL_NCCL(ctx, nccl_api()->AllReduce(sums, sums, 2, ncclDouble, ncclSum, ctx->comm, ctx->stream));
   }
-  TFL_CUDA(ctx, cudaEventRecord(s->ev[3][1].get(), ctx->stream));
+  if (slab_event(ctx, s, s->ev[3][1])) return 1;
   {
     SlabScope scope(ctx, s, s->own_lo, s->own_hi);
     if (tfl_cnn_project_from_sums(ctx, cnn, &st.p, &u1, &st.flags, sums, &st.p, &st.U, mc->normalize_input_threshold)) return 1;
@@ -743,6 +793,128 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
   if (bcs()) return 1;
   SlabScope scope(ctx, s, s->own_lo, s->own_hi);
   return tfl_clamp(ctx, &st.U, -1e6f, 1e6f);
+}
+
+}  // namespace
+
+// ---------------------------------------------------------------------------------------
+// The slab step as a CUDA graph: one tfl_slab_sim_step captured on the context's stream and replayed with one launch.
+// The exchanges need no host: their sequence numbers are read and advanced on the device (SlabSeq), so replays and
+// direct steps interleave freely, on one rank or across ranks.  Pointers and the captured step's host-side choices
+// (advection tile halo, Jacobi path and block schedule) are frozen, and the graph keeps the captured step's
+// exchange statistics to hand to tfl_slab_sim_exchange_stats / _jacobi_stats after each replay; its event-record
+// nodes time the replay.  Buffers the library reallocates are guarded by generation, as in tfl_step_graph.
+// ---------------------------------------------------------------------------------------
+struct tfl_slab_graph {
+  GraphPtr graph;
+  GraphExecPtr exec;
+  tfl_slab_sim* sim = nullptr;
+  long long launches = 0;           // kernels in one replay
+  BufferGens gens;
+  unsigned long long peer_gen = 0;
+  size_t bytes_sent[3] = {0, 0, 0};
+  int jx = 0;
+  size_t jbytes = 0;
+};
+
+extern "C" {
+
+// One tfluids.simulate (lib/simulate.lua:175-327; simMethod 'convnet' or 'jacobi') on this rank's slab.  Asynchronous.
+int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cnn* cnn) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (slab_step_refusal(ctx, s, mc, cnn, "slab_sim_step") || slab_step(ctx, s, mc, cnn)) return 1;
+  s->last.done = true;
+  s->last.cnn = mc->sim_method == TFL_SIM_JACOBI ? nullptr : cnn;
+  s->last.sim_method = mc->sim_method;
+  s->last.gens = buffer_gens(ctx, s->last.cnn);
+  return 0;
+}
+
+void tfl_slab_graph_destroy(tfl_ctx* ctx, tfl_slab_graph* g) {
+  DeviceGuard guard_(ctx);
+  if (g && ctx) cudaStreamSynchronize(ctx->stream);
+  delete g;
+}
+
+int tfl_slab_graph_create(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cnn* cnn, tfl_slab_graph** out) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!out) return fail(ctx, "slab_graph: nil argument");
+  if (slab_step_refusal(ctx, s, mc, cnn, "slab_graph")) return 1;
+  cudaStream_t st = ctx->stream;
+  if (st == nullptr || st == cudaStreamLegacy || st == cudaStreamPerThread)
+    return fail(ctx, "slab_graph: the default stream cannot be captured; give the context a stream (tfl_set_stream)");
+  if (s->world > 1 && !s->peer_ok)
+    return fail(ctx, "slab_graph: world %d without peer memory: only peer-memory exchanges (tfl_slab_sim_ipc_connect) "
+                     "and one rank are captured, not NCCL; step directly (tfl_slab_sim_step)", s->world);
+  const tfl_cnn* model = mc->sim_method == TFL_SIM_JACOBI ? nullptr : cnn;
+  if (!s->last.done || s->last.cnn != model || s->last.sim_method != mc->sim_method)
+    return fail(ctx, "slab_graph: no earlier tfl_slab_sim_step with this sim, model and simMethod; step directly once "
+                     "before capturing (the step's buffers are sized then: capturing must not allocate)");
+  if (const char* what = reallocated_buffer(ctx, s->last.gens))
+    return fail(ctx, "slab_graph: %s reallocated since the last tfl_slab_sim_step with this sim; step directly once "
+                     "more before capturing", what);
+  std::unique_ptr<tfl_slab_graph> g(new tfl_slab_graph());
+  TFL_CUDA(ctx, cudaStreamSynchronize(st));
+  const long long l0 = ctx->launches;
+  size_t bytes_sent[3];                   // the sim's statistics stay those of its last direct step or replay
+  memcpy(bytes_sent, s->bytes_sent, sizeof(bytes_sent));
+  const int jx = s->jx;
+  const size_t jbytes = s->jbytes;
+  if (cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(ctx, "slab_graph: cudaStreamBeginCapture failed");
+  }
+  s->capturing = true;
+  const int rc = slab_step(ctx, s, mc, cnn);
+  s->capturing = false;
+  cudaGraph_t graph = nullptr;
+  const cudaError_t e = cudaStreamEndCapture(st, &graph);
+  g->graph.reset(graph);
+  g->launches = ctx->launches - l0;
+  ctx->launches = l0;
+  memcpy(g->bytes_sent, s->bytes_sent, sizeof(bytes_sent));
+  g->jx = s->jx;
+  g->jbytes = s->jbytes;
+  memcpy(s->bytes_sent, bytes_sent, sizeof(bytes_sent));
+  s->jx = jx;
+  s->jbytes = jbytes;
+  if (rc != 0 || e != cudaSuccess || !graph) {
+    cudaGetLastError();
+    const std::string why = rc != 0 ? ctx->err : std::string(cudaGetErrorString(e));
+    return fail(ctx, "slab_graph: capture failed (%s)", why.c_str());
+  }
+  cudaGraphExec_t exec = nullptr;
+  if (cudaGraphInstantiate(&exec, graph, 0) != cudaSuccess) {
+    cudaGetLastError();
+    return fail(ctx, "slab_graph: cudaGraphInstantiate failed");
+  }
+  g->exec.reset(exec);
+  g->sim = s;
+  g->gens = buffer_gens(ctx, model);
+  g->peer_gen = s->peer_gen;
+  *out = g.release();
+  return 0;
+}
+
+int tfl_slab_graph_launch(tfl_ctx* ctx, tfl_slab_graph* g) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!g || !g->exec) return fail(ctx, "slab_graph is nil");
+  if (const char* stale = reallocated_buffer(ctx, g->gens))
+    return fail(ctx, "slab_graph: stale graph: %s reallocated since the capture (a call on another grid shape or a "
+                     "larger grid); replaying would touch freed memory: capture the step again", stale);
+  if (g->peer_gen != g->sim->peer_gen)
+    return fail(ctx, "slab_graph: stale graph: the peers' inboxes were mapped again (tfl_slab_sim_ipc_connect) since "
+                     "the capture; replaying would store into the old mappings: capture the step again");
+  TFL_CUDA(ctx, cudaGraphLaunch(g->exec.get(), ctx->stream));
+  ctx->launches += g->launches;
+  tfl_slab_sim* s = g->sim;
+  memcpy(s->bytes_sent, g->bytes_sent, sizeof(s->bytes_sent));
+  s->jx = g->jx;
+  s->jbytes = g->jbytes;
+  return 0;
 }
 
 // The step leaves the ghost planes stale; the divergence on the last owned plane reads U_z one plane above it.  So one
@@ -795,6 +967,7 @@ int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* s, const char* handles)
     s->all_inbox.clear();
     s->peer_inbox[0] = s->peer_inbox[1] = nullptr;
     s->peer_ok = false;
+    s->peer_gen++;
   };
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
   drop();

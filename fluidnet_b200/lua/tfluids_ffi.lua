@@ -96,6 +96,10 @@ int tfl_step_graph_create(tfl_ctx*, const tfl_state* state, const tfl_mconf* mco
 int tfl_step_graph_launch(tfl_ctx*, tfl_step_graph* graph);
 int tfl_step_graph_pcg_status(tfl_ctx*, tfl_step_graph* graph, float* residual, int32_t* iterations);
 void tfl_step_graph_destroy(tfl_ctx*, tfl_step_graph* graph);
+typedef struct tfl_slab_graph tfl_slab_graph;
+int tfl_slab_graph_create(tfl_ctx*, tfl_slab_sim* sim, const tfl_mconf* mconf, tfl_cnn* cnn, tfl_slab_graph** out);
+int tfl_slab_graph_launch(tfl_ctx*, tfl_slab_graph* graph);
+void tfl_slab_graph_destroy(tfl_ctx*, tfl_slab_graph* graph);
 int tfl_comm_unique_id(tfl_ctx*, char* id_out);
 int tfl_comm_init(tfl_ctx*, const char* id_bytes, int32_t rank, int32_t world);
 int tfl_comm_destroy(tfl_ctx*);
@@ -367,6 +371,12 @@ function tfluids.slabIpcConnect(sim, allHandles)     -- the 64-byte handles of e
 end
 function tfluids.slabUpload(sim, p, U, density) check(lib.tfl_slab_sim_upload(ctx, sim, p, U, density)) end
 function tfluids.slabStep(sim, cmconf, model) check(lib.tfl_slab_sim_step(ctx, sim, cmconf, model)) end
+function tfluids.slabCaptureStep(sim, cmconf, model)  -- after one tfluids.slabStep on a non-default stream
+  local g = ffi.new('tfl_slab_graph*[1]')
+  check(lib.tfl_slab_graph_create(ctx, sim, cmconf, model, g))
+  return g[0]
+end
+function tfluids.slabLaunchStep(graph) check(lib.tfl_slab_graph_launch(ctx, graph)) end
 function tfluids.slabDownload(sim, p, U, density) check(lib.tfl_slab_sim_download(ctx, sim, p, U, density)) end
 function tfluids.slabJacobiStats(sim)                -- p exchanges of the last 'jacobi' step: count, ms, bytes
   local n, ms, by = ffi.new('int32_t[1]'), ffi.new('float[1]'), ffi.new('int64_t[1]')

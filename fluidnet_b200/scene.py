@@ -310,12 +310,14 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
     """run() on z-slabs: rank `rank` of `world` steps its slab with the library's slab step (NativeSlabSimulator) and
     captures every `output_decimation`-th density frame into a SlabFrameRecorder; rank 0 writes the files.  Every rank
     holds the global flags and BCs.  Without peer memory the frames are gathered synchronously (and the log says so).
+    After frame 1 every rank replays its step from a CUDA graph (SlabStepGraph), as run() does on one GPU, unless its
+    halos go over NCCL, which a graph does not capture.
     After the run the trace faults of all ranks are summed, and a non-zero count raises."""
     import torch
     import torch.distributed as dist
     from . import simulate
     from ._lib import TflError
-    from .slab import NativeSlabSimulator
+    from .slab import NativeSlabSimulator, SlabStepGraph
 
     _, _, local = launcher_world()
     if world > 1 and not dist.is_initialized():
@@ -326,9 +328,10 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
     batch = {"pDiv": zeros(1), "UDiv": zeros(3), "flags": torch.from_numpy(flags_np), "density": zeros(1)}
     simulate.createPlumeBCs(batch, DENSITY_VAL, 1.0 * (res / 128), PLUME_RAD)     # on the host, as the whole-grid scene
     stream = torch.cuda.Stream(device)
-    written, t0, rec, dens, mon, max_u_dt = 0, None, None, None, None, None
+    written, t0, rec, dens, mon, max_u_dt, graph = 0, None, None, None, None, None, None
     with torch.cuda.stream(stream):
         sim = NativeSlabSimulator(batch, mconf, None, device, rank, world, margin, model=model)
+        replay = world == 1 or sim.halo_transport.startswith("peer memory")
         try:
             if stats:
                 mon = sim.monitor(STATS_CAPACITY)
@@ -338,18 +341,24 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
             except TflError as e:
                 transport = "a synchronous gather (%s)" % e
             if rank == 0:
-                log("z-slabs: %d rank(s), margin %d, halos over %s, frames through %s"
-                    % (world, margin, sim.halo_transport, transport))
+                log("z-slabs: %d rank(s), margin %d, halos over %s, frames through %s, %s"
+                    % (world, margin, sim.halo_transport, transport,
+                       "steps replayed from a CUDA graph" if replay else "steps enqueued directly (NCCL is not captured)"))
                 dens = formats.VboxWriter(paths["density"], res, num_frames)
             for i in range(1, num_frames + 1):
                 if i == 2:
                     stream.synchronize()      # frame 1 is not timed
                     t0 = time.perf_counter()
-                sim.step()
+                if graph is not None:
+                    graph.launch()
+                else:
+                    sim.step()
                 if mon is not None:
                     mon.record_frame()        # no collective: a rank keeps its own records until the run ends
                 if i == 1 and rank == 0:
                     write_geometry(paths, res, batch["flags"].to(device))
+                if i == 1 and replay:
+                    graph = SlabStepGraph(sim)
                 if i % output_decimation == 0:
                     if rec is not None:
                         sim.record(rec, dens)
@@ -377,6 +386,8 @@ def run_slabs(res, mconf, model, flags_np, paths, num_frames, output_decimation,
                 rec.close()
             if mon is not None:
                 mon.close()
+            if graph is not None:
+                graph.close()
             sim.close()
     ms = None if t0 is None else 1000.0 * (t1 - t0) / (num_frames - 1)
     if rank == 0:

@@ -531,6 +531,30 @@ class NativeSlabSimulator:
         self.ctx.lib.tfl_comm_destroy(self.ctx.h)
 
 
+class SlabStepGraph:
+    """One NativeSlabSimulator.step captured as a CUDA graph (tfl_slab_graph_*): `launch()` replays it, one launch per
+    step.  Needs a non-default current stream, one earlier sim.step() and, with more than one rank, peer-memory
+    exchanges (NCCL is not captured).  Every rank makes its own; the ranks still take the same steps, in any mix of
+    sim.step() and launch()."""
+
+    def __init__(self, sim):
+        self.sim, self.ctx = sim, sim.ctx           # keep the captured simulator (and its model) alive
+        self.ctx.use_current_stream()
+        h = C.c_void_p()
+        self.ctx.check(self.ctx.lib.tfl_slab_graph_create(self.ctx.h, sim.h, C.byref(sim.mc),
+                                                          sim.model.h if sim.model is not None else None, C.byref(h)))
+        self.h = h
+
+    def launch(self):
+        self.ctx.use_current_stream()
+        self.ctx.check(self.ctx.lib.tfl_slab_graph_launch(self.ctx.h, self.h))
+
+    def close(self):
+        if self.h:
+            self.ctx.lib.tfl_slab_graph_destroy(self.ctx.h, self.h)
+            self.h = None
+
+
 def run_lockstep(sims):
     """Advance several SlabSimulators of ONE decomposition that live in the same process (tests:
     the whole multi-rank logic on a single GPU).  Halo requests are served by direct copies between

@@ -483,6 +483,23 @@ int tfl_jacobi_slab_block(tfl_ctx* ctx, const tfl_grid* pa, const tfl_grid* pb, 
 #define TFL_IPC_HANDLE_BYTES 64
 int tfl_slab_sim_ipc_export(tfl_ctx* ctx, tfl_slab_sim* sim, char* handle_out /* TFL_IPC_HANDLE_BYTES */);
 int tfl_slab_sim_ipc_connect(tfl_ctx* ctx, tfl_slab_sim* sim, const char* handles);
+/* The slab step as a CUDA graph: one tfl_slab_sim_step captured on the context's stream (convnet, single-bank or
+ * banked, or Jacobi with its cooperative block kernel; the exchange-statistics events become event-record nodes) and
+ * replayed with one launch per step.  The exchanges' sequence numbers live on the device, so replays and direct steps
+ * may be interleaved freely, on one rank and across ranks; every rank creates its own graph (capture involves no peer)
+ * and the ranks still take the same steps, as with direct steps alone.  Pointers, mconf and the captured step's
+ * host-side choices (advection tile halo, Jacobi path and block schedule) are frozen into the graph.
+ * tfl_slab_graph_create refuses, by name and before anything is captured: whatever tfl_slab_sim_step refuses (same
+ * messages), the default stream, no earlier tfl_slab_sim_step with this sim, model and simMethod (or a buffer below
+ * reallocated since), and world > 1 without peer memory (NCCL is not captured).
+ * tfl_slab_graph_launch refuses a stale graph, naming the buffer, like tfl_step_graph_launch (the context's scratch
+ * arena and flag cache, the model's activation buffers; also the peers' inboxes mapped again); it adds the captured
+ * step's kernels to tfl_launch_count, and tfl_slab_sim_exchange_stats / _jacobi_stats then report the replayed step.
+ * Destroying the sim, the model or the context while a graph that uses them exists is a caller error. */
+typedef struct tfl_slab_graph tfl_slab_graph;
+int tfl_slab_graph_create(tfl_ctx* ctx, tfl_slab_sim* sim, const tfl_mconf* mconf, tfl_cnn* cnn, tfl_slab_graph** out);
+int tfl_slab_graph_launch(tfl_ctx* ctx, tfl_slab_graph* graph);
+void tfl_slab_graph_destroy(tfl_ctx* ctx, tfl_slab_graph* graph);
 
 /* ---- frame output behind the running step (the save branch of fluid_net_3d_sim.lua:266-291) ------------------------
  * A recorder moves a scalar grid [1][1][nz][ny][nx] to the host in `.vbox` order -- the value at (x, y, z) at index
