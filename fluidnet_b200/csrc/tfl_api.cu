@@ -857,7 +857,9 @@ static int set_const_vals(tfl_ctx* ctx, const tfl_state* s) {       // lib/simul
 }
 
 // Fused pipeline for the convnet path with the tensor-core conv stack: 12 launches with a single-bank
-// stack, every field crosses memory once per stage.  Bit-identical to the operator sequence below.
+// stack and the default input block (one more for 'div' statistics, one more for the pressure skip), every field
+// crosses memory once per stage.  Bit-identical to the operator sequence below, up to the order in which the input
+// scale's double sums are added.
 static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, tfl_cnn* m, const Geo& g) {
   const size_t cells = (size_t)g.n * g.nb;
   const bool has_density = s->density.data != nullptr;
@@ -955,25 +957,36 @@ static int simulate_step_fused(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf
     launch_vort_curl(s->U.data, curl, cnorm, force, fo.vort_amp, g, st);
     ctx->launches += 2;
   }
+  // The input scale's sums: of the masked U or of pDiv in the point-wise stage, of div(U1) in a pass of their own
+  // once U1 is complete, none without normalizeInput.
+  const bool normalized = m->norm_func != kCnnScaleOne;
+  const int stage_stat = normalized && m->norm_chan != kCnnStatDiv ? m->norm_chan : kCnnStatNone;
+  const bool div_stats = normalized && m->norm_chan == kCnnStatDiv;
+  if (ov && stage_stat == kCnnStatPDiv) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in.get(), 0));
   TFL_CUDA(ctx, cudaMemsetAsync(sums, 0, sizeof(double) * 2 * g.nb, st));
   launch_vort_bc_mask(s->U.data, fl8, force, fo.vorticity, u_bc ? s->U_bc_inv_mask.data : nullptr,
-                      u_bc ? s->U_bc.data : nullptr, qmask, 1, sums, g, st);
+                      u_bc ? s->U_bc.data : nullptr, qmask, 1, sums, g, st, stage_stat, s->p.data);
+  if (div_stats) launch_cnn_div_stats_fused(s->U.data, fl8, sums, g, st);
   const ConvTcGeo& tg = m->act_geo;
-  if (ov) TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in.get(), 0));          // pDiv is first read here
-  launch_cnn_inputs_fused(s->p.data, s->U.data, fl8, sums, mc->normalize_input_threshold, scale, m->act[0].get(),
-                          tg.px, tg.py, g, st);
+  if (ov && stage_stat != kCnnStatPDiv)
+    TFL_CUDA(ctx, cudaStreamWaitEvent(st, ctx->ev_p_in.get(), 0));          // pDiv is first read here
+  if (!launch_cnn_inputs_fused(s->p.data, s->U.data, fl8, sums, mc->normalize_input_threshold, scale, m->act[0].get(),
+                               tg.px, tg.py, g, st, m->in_sel, m->norm_func, m->norm_chan))
+    return fail(ctx, "simulate_step (fused): no input kernel for the channel set %d", m->in_sel);
   const int stack = run_conv_stack(m, p_net, st);
+  if (m->skip) launch_cnn_skip(p_net, s->p.data, scale, m->w_skip, g, st);
   launch_cnn_finish_fused(p_net, s->U.data, fl8, scale, s->p.data, u_bc ? s->U_bc_inv_mask.data : nullptr,
                           u_bc ? s->U_bc.data : nullptr, qmask, -1e6f, 1e6f, g, st);
-  ctx->launches += 3 + stack;     // launch_vort_bc_mask, the fused input and finish, and the stack's own
+  // launch_vort_bc_mask, the divergence sums, the fused input, the stack's own, the skip and the finish
+  ctx->launches += 1 + (div_stats ? 1 : 0) + 1 + stack + (m->skip ? 1 : 0) + 1;
   return check_launch(ctx, "simulate_step (fused)");
 }
 
 // Whether tfl_simulate_step takes the fused pipeline for this state, configuration and model.
 // Its point-wise stages are 3-D kernels: the tensor-core stack (tc_ok) serves 3-D models only.
 static bool fused_step_applies(const tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, const tfl_cnn* cnn) {
-  return mc->sim_method == TFL_SIM_CONVNET && cnn && cnn->tc_ok && cnn->mode > 0 && cnn->default_inputs && !ctx->slab &&
-         s->U.nc == 3 && !s->p_bc.data && mc->advection_method >= 0 && mc->advection_method <= 5;
+  return mc->sim_method == TFL_SIM_CONVNET && cnn && cnn->tc_ok && cnn->mode > 0 && !ctx->slab && s->U.nc == 3 &&
+         !s->p_bc.data && mc->advection_method >= 0 && mc->advection_method <= 5;
 }
 
 int tfl_simulate_step(tfl_ctx* ctx, const tfl_state* s, const tfl_mconf* mc, tfl_cnn* cnn) {

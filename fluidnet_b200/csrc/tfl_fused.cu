@@ -11,12 +11,17 @@
 //                        tfluids.addBuoyancy                  (lib/simulate.lua:216-226)
 //   k_vort_bc_mask       vorticityConfinement's AddForceField (third_party/tfluids.cc:1312-1339)
 //                        setConstVals (U)                     (lib/simulate.lua:252)
-//                        tfluids.SetWallBcs mask multiply + the sums behind nn.StandardDeviation
-//                                                             (lib/model.lua:81-117)
-//   k_cnn_inputs_fused   scale, ApplyScale(pDiv, div), VelocityDivergence, FlagsToOccupancy
+//                        tfluids.SetWallBcs mask multiply + the sums behind the input scale of the field
+//                        normalizeInputChan names, U or pDiv  (lib/model.lua:81-117)
+//   k_cnn_div_stats_fused the same sums of div(U1), normalizeInputChan 'div' (lib/model.lua:108-116)
+//   k_cnn_inputs_fused   scale (std, 'norm' or 1), ApplyScale of the inputChannels set (pDiv, UDiv, div),
+//                        VelocityDivergence, FlagsToOccupancy, into one or two float4 planes
 //                                                             (lib/model.lua:86-150)
+//   (launch_cnn_skip)    addPressureSkip, between the convolution stack and the finish (lib/model.lua:357-361)
 //   k_cnn_finish_fused   VelocityUpdate, ApplyScale, SetWallBcs (lib/model.lua:380-390)
 //                        setConstVals (U) ; U:clamp(-1e6, 1e6) (lib/simulate.lua:321, :326)
+// The input block is a template argument of the kernels that depend on it, so the default block (pDiv, div,
+// occupancy; std of U) compiles to the code it has on its own.
 #include <initializer_list>
 #include "tfl_device.cuh"
 #include "tfl_kernels.h"
@@ -83,12 +88,12 @@ __global__ void k_post_advect(const float* __restrict__ tmp_s, const float* __re
 }
 
 // U += confinement force; U = BC(U); then (mask_mode 1) U *= wall mask and accumulate the
-// sums for the input scale.  BATCH (nb > 1): the sums go to each thread's own entry (add_entry_sums); nb = 1 compiles
-// without that branch.
-template <bool BATCH>
+// sums for the input scale: of the masked U (STAT kCnnStatU), of p_div (kCnnStatPDiv), or none (kCnnStatNone).
+// BATCH (nb > 1): the sums go to each thread's own entry (add_entry_sums); nb = 1 compiles without that branch.
+template <bool BATCH, int STAT>
 __global__ void k_vort_bc_mask(float* __restrict__ U, const unsigned char* __restrict__ flags,
                                const float* __restrict__ force, int do_vort, BcPtrs bc, int mask_mode,
-                               double* __restrict__ sums, Geo gin) {
+                               double* __restrict__ sums, Geo gin, const float* __restrict__ p_div) {
   const Geo g = static_geo<true>(gin);
   int b, k, j, i;
   const bool live = thread_cell(g, b, k, j, i);
@@ -121,21 +126,110 @@ __global__ void k_vort_bc_mask(float* __restrict__ U, const unsigned char* __res
       wall_bc_zero_mask(fl, g, k, j, i, z);
       for (int a = 0; a < g.nc; a++) {
         if (z[a]) u[a] = u[a] * 0.0f;
-        const float sq = u[a] * u[a];
-        s += (double)u[a];
+        if (STAT == kCnnStatU) {
+          const float sq = u[a] * u[a];
+          s += (double)u[a];
+          ss += (double)sq;
+        }
+      }
+      if (STAT == kCnnStatPDiv) {
+        const float v = __ldg(p_div + b * g.n + c);
+        const float sq = v * v;
+        s += (double)v;
         ss += (double)sq;
       }
     }
     for (int a = 0; a < g.nc; a++) U[ub + a * g.n + c] = u[a];
   }
-  if (mask_mode) {
+  if (STAT != kCnnStatNone && mask_mode) {
     if (BATCH) add_entry_sums(s, ss, sums, live, b, g);         // a block may straddle two entries
     else block_accumulate(s, ss, sums + 2 * (live ? b : 0));
   }
 }
 
-// First channels-last plane of the conv input: (pDiv/s, div(U1)/s, occupancy, 0); U1 is the
-// already masked velocity left in U by k_vort_bc_mask.
+// tfluids.VelocityDivergence of U1 at cell c (flag f) of a 3-D grid.
+__device__ __forceinline__ float fused_div(const float* __restrict__ ub, int f, const Geo& g, int k, int j, int i,
+                                           int c) {
+  float dv = 0.0f;
+  if (!on_border(g, k, j, i) && (f & kFluid)) {
+    dv = __ldg(ub + c) - __ldg(ub + c + 1) + __ldg(ub + g.n + c) - __ldg(ub + g.n + c + g.nx);
+    if (g.is3d) dv += (__ldg(ub + 2 * g.n + c) - __ldg(ub + 2 * g.n + c + (long long)g.nx * g.ny));
+  }
+  return dv;
+}
+
+// normalizeInputChan 'div': sums[b] += (sum div(U1), sum div(U1)^2), k_cnn_div_stats on the step's byte flags, once
+// k_vort_bc_mask has left U1 in U.
+template <bool BATCH>
+__global__ void k_cnn_div_stats_fused(const float* __restrict__ U1, const unsigned char* __restrict__ flags,
+                                      double* __restrict__ sums, Geo gin) {
+  const Geo g = static_geo<true>(gin);
+  int b, k, j, i;
+  const bool live = thread_cell(g, b, k, j, i);
+  double s = 0.0, ss = 0.0;
+  if (live) {
+    const int c = cell(g, k, j, i);
+    const float dv = fused_div(U1 + (long long)b * g.nc * g.n, flag_i(flags + b * g.n, g, k, j, i), g, k, j, i, c);
+    const float sq = dv * dv;
+    s += (double)dv;
+    ss += (double)sq;
+  }
+  if (BATCH) add_entry_sums(s, ss, sums, live, b, g);
+  else block_accumulate(s, ss, sums + 2 * (live ? b : 0));
+}
+
+// The input scale of entry b from the sums (k_cnn_scale's expressions): SCALE kFusedStdU (nn.StandardDeviation over
+// the nc n values of U), kFusedStdN (over the n values of pDiv or div), kFusedNorm ('norm') or kFusedOne
+// (normalizeInput off: exactly 1).
+enum : int { kFusedStdU = 0, kFusedStdN = 1, kFusedNorm = 2, kFusedOne = 3 };
+template <int SCALE>
+__device__ __forceinline__ float fused_scale(const double* __restrict__ sums, int b, const Geo& g, float threshold) {
+  if (SCALE == kFusedStdU) return scale_from_sums(sums, b, (long long)g.nc * g.n, threshold);
+  if (SCALE == kFusedStdN) return scale_from_sums(sums, b, g.n, threshold);
+  if (SCALE == kFusedNorm) {
+    const float out = sqrtf((float)sums[2 * b + 1]);
+    return (out < threshold) ? threshold : out;
+  }
+  return 1.0f;
+}
+
+// Channel `slot` of the input set SEL (kCnnIn* bits), of the values at one voxel: pDiv/s, U1/s (3), div/s, occupancy in
+// that order (cnn_input_channels), then zeros up to 8.
+template <int SEL, int SLOT>
+__device__ __forceinline__ float input_channel(float p, float u0, float u1, float u2, float d, float occ) {
+  constexpr int kU = (SEL & kCnnInPDiv) ? 1 : 0;
+  constexpr int kD = kU + ((SEL & kCnnInUDiv) ? 3 : 0);
+  constexpr int kOcc = kD + ((SEL & kCnnInDiv) ? 1 : 0);
+  if constexpr ((SEL & kCnnInPDiv) && SLOT == 0) return p;
+  else if constexpr ((SEL & kCnnInUDiv) && SLOT == kU) return u0;
+  else if constexpr ((SEL & kCnnInUDiv) && SLOT == kU + 1) return u1;
+  else if constexpr ((SEL & kCnnInUDiv) && SLOT == kU + 2) return u2;
+  else if constexpr ((SEL & kCnnInDiv) && SLOT == kD) return d;
+  else if constexpr (SLOT == kOcc) return occ;
+  else return 0.0f;
+}
+
+// The conv input of the set SEL at one voxel, channels-last: channels 0-3 on the first float4 plane, 4-7 on the
+// second (written only with UDiv), as k_cnn_inputs_padded lays them out.  U1 is the already masked velocity left in U
+// by k_vort_bc_mask.
+template <int SEL>
+__device__ __forceinline__ void put_inputs(float4* __restrict__ x0, long long o, int v, long long plane, float pd,
+                                           float u0, float u1, float u2, float dv, int f, float sc) {
+  const float p = pd / sc, d = dv / sc;
+  const float occ = (f == kFluid) ? 0.0f : ((f == kObstacle) ? 1.0f : -1.0f);
+  float us[3] = {0.0f, 0.0f, 0.0f};
+  if (SEL & kCnnInUDiv) {
+    us[0] = u0 / sc;
+    us[1] = u1 / sc;
+    us[2] = u2 / sc;
+  }
+#define TFL_CHANNEL(q) input_channel<SEL, q>(p, us[0], us[1], us[2], d, occ)
+  x0[o + v] = make_float4(TFL_CHANNEL(0), TFL_CHANNEL(1), TFL_CHANNEL(2), TFL_CHANNEL(3));
+  if (SEL & kCnnInUDiv) x0[o + v + plane] = make_float4(TFL_CHANNEL(4), TFL_CHANNEL(5), TFL_CHANNEL(6), TFL_CHANNEL(7));
+#undef TFL_CHANNEL
+}
+
+template <int SEL, int SCALE>
 __global__ void k_cnn_inputs_fused(const float* __restrict__ p_div, const float* __restrict__ U1,
                                    const unsigned char* __restrict__ flags, const double* __restrict__ sums,
                                    float threshold, float* __restrict__ scale_out, float4* __restrict__ x0,
@@ -144,19 +238,17 @@ __global__ void k_cnn_inputs_fused(const float* __restrict__ p_div, const float*
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
   const int c = cell(g, k, j, i);
-  const float sc = scale_from_sums(sums, b, (long long)g.nc * g.n, threshold);
+  const float sc = fused_scale<SCALE>(sums, b, g, threshold);
   if (c == 0) scale_out[b] = sc;
   const float* ub = U1 + (long long)b * g.nc * g.n;
   const int f = flag_i(flags + b * g.n, g, k, j, i);
-  float dv = 0.0f;
-  if (!on_border(g, k, j, i) && (f & kFluid)) {
-    dv = __ldg(ub + c) - __ldg(ub + c + 1) + __ldg(ub + g.n + c) - __ldg(ub + g.n + c + g.nx);
-    if (g.is3d) dv += (__ldg(ub + 2 * g.n + c) - __ldg(ub + 2 * g.n + c + (long long)g.nx * g.ny));
-  }
+  const float dv = fused_div(ub, f, g, k, j, i, c);
   const long long plane = (long long)(g.nz + 2) * py * px;
   const long long o = (long long)b * 2 * plane + ((long long)(k + 1) * py + (j + 1)) * px + (i + 1);
-  x0[o] = make_float4(__ldg(p_div + b * g.n + c) / sc, dv / sc,
-                      (f == kFluid) ? 0.0f : ((f == kObstacle) ? 1.0f : -1.0f), 0.0f);
+  float u[3] = {0.0f, 0.0f, 0.0f};
+  if (SEL & kCnnInUDiv)
+    for (int a = 0; a < 3; a++) u[a] = __ldg(ub + a * g.n + c);
+  put_inputs<SEL>(x0, o, 0, plane, (SEL & kCnnInPDiv) ? __ldg(p_div + b * g.n + c) : 0.0f, u[0], u[1], u[2], dv, f, sc);
 }
 
 // U = clamp(BC(setWallBcs(velocityUpdate(U1 / s, p_net) * s)));  p = p_net * s.  In place on U.
@@ -378,10 +470,11 @@ __global__ void __launch_bounds__(256) k_post_advect4(const float* __restrict__ 
   for (int a = 0; a < 3; a++) if (a < g.nc) st4(U + ub + a * g.n + c0, u[a]);
 }
 
-template <bool BATCH>
+template <bool BATCH, int STAT>
 __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, const unsigned char* __restrict__ flags,
                                                        const float* __restrict__ force, int do_vort, BcPtrs bc,
-                                                       int mask_mode, double* __restrict__ sums, Geo gin) {
+                                                       int mask_mode, double* __restrict__ sums, Geo gin,
+                                                       const float* __restrict__ p_div) {
   const Geo g = static_geo<true>(gin);
   int b, k, j, i0;
   const bool live = thread_cell4(g, b, k, j, i0);
@@ -437,6 +530,8 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
       }
     }
     if (mask_mode) {
+      float pd[4];
+      if (STAT == kCnnStatPDiv) ld4(p_div + b * g.n + c0, pd);
 #pragma unroll
       for (int v = 0; v < 4; v++) {
         bool z[3];
@@ -445,22 +540,81 @@ __global__ void __launch_bounds__(256) k_vort_bc_mask4(float* __restrict__ U, co
         for (int a = 0; a < 3; a++) {
           if (a < g.nc) {
             if (z[a]) u[a][v] = u[a][v] * 0.0f;
-            const float sq = u[a][v] * u[a][v];
-            s += (double)u[a][v];
-            ss += (double)sq;
+            if (STAT == kCnnStatU) {
+              const float sq = u[a][v] * u[a][v];
+              s += (double)u[a][v];
+              ss += (double)sq;
+            }
           }
+        }
+        if (STAT == kCnnStatPDiv) {
+          const float sq = pd[v] * pd[v];
+          s += (double)pd[v];
+          ss += (double)sq;
         }
       }
     }
 #pragma unroll
     for (int a = 0; a < 3; a++) if (a < g.nc) st4(U + ub + a * g.n + c0, u[a]);
   }
-  if (mask_mode) {
+  if (STAT != kCnnStatNone && mask_mode) {
     if (BATCH) add_entry_sums(s, ss, sums, live, b, g);         // thread_cell4's z range is [0, nz), as thread_cell's
     else block_accumulate(s, ss, sums + 2 * (live ? b : 0));
   }
 }
 
+// U1 around a quad of a 3-D grid: the x / y / z components of the quad, the x component right of it and the y / z
+// components one row / plane up (0 outside the grid).
+struct QuadU {
+  float ux[4], uy[4], uyp[4], uz[4], uzp[4], uxr;
+};
+__device__ __forceinline__ QuadU quad_u(const float* __restrict__ ub, const Geo& g, int c0, int k, int j, int i0) {
+  const int sy = g.nx, sz = g.nx * g.ny;
+  QuadU q;
+  ld4(ub + c0, q.ux);
+  q.uxr = i0 + 4 < g.nx ? __ldg(ub + c0 + 4) : 0.0f;
+  ld4(ub + g.n + c0, q.uy);
+  zero4(q.uyp); zero4(q.uz); zero4(q.uzp);
+  if (j < g.ny - 1) ld4(ub + g.n + c0 + sy, q.uyp);
+  ld4(ub + 2 * g.n + c0, q.uz);
+  if (k < g.nz - 1) ld4(ub + 2 * g.n + c0 + sz, q.uzp);
+  return q;
+}
+// tfluids.VelocityDivergence at voxel v of the quad (flag f).
+__device__ __forceinline__ float quad_div(const QuadU& q, int f, const Geo& g, int k, int j, int i0, int v) {
+  float dv = 0.0f;
+  if (!on_border(g, k, j, i0 + v) && (f & kFluid)) {
+    dv = q.ux[v] - (v == 3 ? q.uxr : q.ux[v + 1]) + q.uy[v] - q.uyp[v];
+    dv += (q.uz[v] - q.uzp[v]);
+  }
+  return dv;
+}
+
+template <bool BATCH>
+__global__ void __launch_bounds__(256) k_cnn_div_stats_fused4(const float* __restrict__ U1,
+                                                              const unsigned char* __restrict__ flags,
+                                                              double* __restrict__ sums, Geo gin) {
+  const Geo g = static_geo<true>(gin);
+  int b, k, j, i0;
+  const bool live = thread_cell4(g, b, k, j, i0);
+  double s = 0.0, ss = 0.0;
+  if (live) {
+    const int c0 = cell(g, k, j, i0);
+    const Flags4 fc = flags4(flags + b * g.n + c0, true);
+    const QuadU q = quad_u(U1 + (long long)b * g.nc * g.n, g, c0, k, j, i0);
+#pragma unroll
+    for (int v = 0; v < 4; v++) {
+      const float dv = quad_div(q, fc.c[v], g, k, j, i0, v);
+      const float sq = dv * dv;
+      s += (double)dv;
+      ss += (double)sq;
+    }
+  }
+  if (BATCH) add_entry_sums(s, ss, sums, live, b, g);
+  else block_accumulate(s, ss, sums + 2 * (live ? b : 0));
+}
+
+template <int SEL, int SCALE>
 __global__ void __launch_bounds__(256) k_cnn_inputs_fused4(const float* __restrict__ p_div, const float* __restrict__ U1,
                                                            const unsigned char* __restrict__ flags,
                                                            const double* __restrict__ sums, float threshold,
@@ -470,20 +624,14 @@ __global__ void __launch_bounds__(256) k_cnn_inputs_fused4(const float* __restri
   int b, k, j, i0;
   if (!thread_cell4(g, b, k, j, i0)) return;
   const int c0 = cell(g, k, j, i0);
-  const int sy = g.nx, sz = g.nx * g.ny;
-  const float sc = scale_from_sums(sums, b, (long long)g.nc * g.n, threshold);
+  const float sc = fused_scale<SCALE>(sums, b, g, threshold);
   if (c0 == 0) scale_out[b] = sc;
   const float* ub = U1 + (long long)b * g.nc * g.n;
   const Flags4 fc = flags4(flags + b * g.n + c0, true);
-  float ux[4], uy[4], uyp[4], uz[4], uzp[4], pd[4];
-  ld4(ub + c0, ux);
-  const float uxr = i0 + 4 < g.nx ? __ldg(ub + c0 + 4) : 0.0f;
-  ld4(ub + g.n + c0, uy);
-  zero4(uyp); zero4(uz); zero4(uzp);
-  if (j < g.ny - 1) ld4(ub + g.n + c0 + sy, uyp);
-  ld4(ub + 2 * g.n + c0, uz);
-  if (k < g.nz - 1) ld4(ub + 2 * g.n + c0 + sz, uzp);
-  ld4(p_div + b * g.n + c0, pd);
+  const QuadU q = quad_u(ub, g, c0, k, j, i0);
+  float pd[4];
+  if (SEL & kCnnInPDiv) ld4(p_div + b * g.n + c0, pd);
+  else zero4(pd);
   const long long plane = (long long)(g.nz + 2) * py * px;
   const long long o = (long long)b * 2 * plane + ((long long)(k + 1) * py + (j + 1)) * px + (i0 + 1);
 #pragma unroll
@@ -491,10 +639,10 @@ __global__ void __launch_bounds__(256) k_cnn_inputs_fused4(const float* __restri
     const int f = fc.c[v];
     float dv = 0.0f;
     if (!on_border(g, k, j, i0 + v) && (f & kFluid)) {
-      dv = ux[v] - (v == 3 ? uxr : ux[v + 1]) + uy[v] - uyp[v];
-      dv += (uz[v] - uzp[v]);
+      dv = q.ux[v] - (v == 3 ? q.uxr : q.ux[v + 1]) + q.uy[v] - q.uyp[v];
+      dv += (q.uz[v] - q.uzp[v]);
     }
-    x0[o + v] = make_float4(pd[v] / sc, dv / sc, (f == kFluid) ? 0.0f : ((f == kObstacle) ? 1.0f : -1.0f), 0.0f);
+    put_inputs<SEL>(x0, o, v, plane, pd[v], q.ux[v], q.uy[v], q.uz[v], dv, f, sc);
   }
 }
 
@@ -792,30 +940,95 @@ void launch_post_advect(const float* tmp_s, const float* tmp_u, const unsigned c
   launch_dims(g, grid, block);
   k_post_advect<<<grid, block, 0, st>>>(tmp_s, tmp_u, flags, density, U, bc, do_buoy, s[0], s[1], s[2], g);
 }
+template <int STAT>
+static void vort_bc_mask_stat(float* U, const unsigned char* flags, const float* force, int do_vort, const BcPtrs& bc,
+                              int mask_mode, double* sums, const float* p_div, const Geo& g, cudaStream_t st) {
+  dim3 grid, block;
+  if (quad_dims(g, grid, block) &&
+      aligned16({U, flags, force, bc.u_inv, bc.u_bc, STAT == kCnnStatPDiv ? p_div : nullptr})) {
+    if (g.nb > 1)
+      k_vort_bc_mask4<true, STAT><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g, p_div);
+    else
+      k_vort_bc_mask4<false, STAT><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g, p_div);
+    return;
+  }
+  launch_dims(g, grid, block);
+  if (g.nb > 1)
+    k_vort_bc_mask<true, STAT><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g, p_div);
+  else
+    k_vort_bc_mask<false, STAT><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g, p_div);
+}
 void launch_vort_bc_mask(float* U, const unsigned char* flags, const float* force, int do_vort,
                          const float* u_inv, const float* u_bc, const unsigned char* qmask, int mask_mode, double* sums,
-                         const Geo& g, cudaStream_t st) {
-  BcPtrs bc{u_inv, u_bc, nullptr, nullptr, qmask};
-  dim3 grid, block;
-  if (quad_dims(g, grid, block) && aligned16({U, flags, force, u_inv, u_bc})) {
-    if (g.nb > 1) k_vort_bc_mask4<true><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
-    else k_vort_bc_mask4<false><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
-    return;
-  }
-  launch_dims(g, grid, block);
-  if (g.nb > 1) k_vort_bc_mask<true><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
-  else k_vort_bc_mask<false><<<grid, block, 0, st>>>(U, flags, force, do_vort, bc, mask_mode, sums, g);
+                         const Geo& g, cudaStream_t st, int stat, const float* p_div) {
+  const BcPtrs bc{u_inv, u_bc, nullptr, nullptr, qmask};
+  if (stat == kCnnStatU) vort_bc_mask_stat<kCnnStatU>(U, flags, force, do_vort, bc, mask_mode, sums, p_div, g, st);
+  else if (stat == kCnnStatPDiv)
+    vort_bc_mask_stat<kCnnStatPDiv>(U, flags, force, do_vort, bc, mask_mode, sums, p_div, g, st);
+  else vort_bc_mask_stat<kCnnStatNone>(U, flags, force, do_vort, bc, mask_mode, sums, p_div, g, st);
 }
-void launch_cnn_inputs_fused(const float* p_div, const float* U1, const unsigned char* flags, const double* sums,
-                             float threshold, float* scale_out, float* x0, int px, int py, const Geo& g,
-                             cudaStream_t st) {
+void launch_cnn_div_stats_fused(const float* U1, const unsigned char* flags, double* sums, const Geo& g,
+                                cudaStream_t st) {
   dim3 grid, block;
-  if (quad_dims(g, grid, block) && aligned16({p_div, U1, flags, x0})) {
-    k_cnn_inputs_fused4<<<grid, block, 0, st>>>(p_div, U1, flags, sums, threshold, scale_out, (float4*)x0, px, py, g);
+  if (quad_dims(g, grid, block) && aligned16({U1, flags})) {
+    if (g.nb > 1) k_cnn_div_stats_fused4<true><<<grid, block, 0, st>>>(U1, flags, sums, g);
+    else k_cnn_div_stats_fused4<false><<<grid, block, 0, st>>>(U1, flags, sums, g);
     return;
   }
   launch_dims(g, grid, block);
-  k_cnn_inputs_fused<<<grid, block, 0, st>>>(p_div, U1, flags, sums, threshold, scale_out, (float4*)x0, px, py, g);
+  if (g.nb > 1) k_cnn_div_stats_fused<true><<<grid, block, 0, st>>>(U1, flags, sums, g);
+  else k_cnn_div_stats_fused<false><<<grid, block, 0, st>>>(U1, flags, sums, g);
+}
+
+// The arguments of one launch of the input kernels.
+struct InputsArgs {
+  const float *p_div, *U1;
+  const unsigned char* flags;
+  const double* sums;
+  float threshold;
+  float *scale_out, *x0;
+  int px, py;
+};
+template <int SEL, int SCALE>
+static void inputs_fused(const InputsArgs& a, const Geo& g, cudaStream_t st) {
+  dim3 grid, block;
+  if (quad_dims(g, grid, block) && aligned16({(SEL & kCnnInPDiv) ? a.p_div : nullptr, a.U1, a.flags, a.x0})) {
+    k_cnn_inputs_fused4<SEL, SCALE><<<grid, block, 0, st>>>(a.p_div, a.U1, a.flags, a.sums, a.threshold, a.scale_out,
+                                                            (float4*)a.x0, a.px, a.py, g);
+    return;
+  }
+  launch_dims(g, grid, block);
+  k_cnn_inputs_fused<SEL, SCALE><<<grid, block, 0, st>>>(a.p_div, a.U1, a.flags, a.sums, a.threshold, a.scale_out,
+                                                         (float4*)a.x0, a.px, a.py, g);
+}
+template <int SEL>
+static void inputs_fused_sel(int scale, const InputsArgs& a, const Geo& g, cudaStream_t st) {
+  switch (scale) {
+    case kFusedStdU: inputs_fused<SEL, kFusedStdU>(a, g, st); break;
+    case kFusedStdN: inputs_fused<SEL, kFusedStdN>(a, g, st); break;
+    case kFusedNorm: inputs_fused<SEL, kFusedNorm>(a, g, st); break;
+    default: inputs_fused<SEL, kFusedOne>(a, g, st); break;
+  }
+}
+bool launch_cnn_inputs_fused(const float* p_div, const float* U1, const unsigned char* flags, const double* sums,
+                             float threshold, float* scale_out, float* x0, int px, int py, const Geo& g,
+                             cudaStream_t st, int sel, int func, int chan) {
+  const InputsArgs a{p_div, U1, flags, sums, threshold, scale_out, x0, px, py};
+  const int scale = func == kCnnScaleOne    ? kFusedOne
+                    : func == kCnnScaleNorm ? kFusedNorm
+                    : chan == kCnnStatU     ? kFusedStdU
+                                            : kFusedStdN;
+  constexpr int P = kCnnInPDiv, U = kCnnInUDiv, D = kCnnInDiv;
+  switch (sel) {     // the sets tfl_cnn_create accepts: UDiv or div, with or without pDiv
+    case P | D: inputs_fused_sel<P | D>(scale, a, g, st); break;
+    case P | U | D: inputs_fused_sel<P | U | D>(scale, a, g, st); break;
+    case P | U: inputs_fused_sel<P | U>(scale, a, g, st); break;
+    case U | D: inputs_fused_sel<U | D>(scale, a, g, st); break;
+    case U: inputs_fused_sel<U>(scale, a, g, st); break;
+    case D: inputs_fused_sel<D>(scale, a, g, st); break;
+    default: return false;
+  }
+  return true;
 }
 void launch_cnn_finish_fused(const float* p_net, float* U, const unsigned char* flags, const float* scale, float* p_out,
                              const float* u_inv, const float* u_bc, const unsigned char* qmask, float lo, float hi,

@@ -67,7 +67,8 @@ void launch_clamp(float* x, float lo, float hi, long long n, cudaStream_t st);
 // CNN pre/post stages (exact float semantics of lib/model.lua's non-conv nodes).
 // The input block (tfl_cnn_inputs): channel set bits, the field the scale is computed from, the scale function.
 enum : int { kCnnInPDiv = 1, kCnnInUDiv = 2, kCnnInDiv = 4 };
-enum : int { kCnnStatU = 0, kCnnStatPDiv = 1, kCnnStatDiv = 2 };
+// kCnnStatNone: the fused step's point-wise stage sums nothing (normalizeInput off, or 'div', summed after it).
+enum : int { kCnnStatU = 0, kCnnStatPDiv = 1, kCnnStatDiv = 2, kCnnStatNone = 3 };
 enum : int { kCnnScaleStd = 0, kCnnScaleNorm = 1, kCnnScaleOne = 2 };
 // U1 = wall mask * U; sums[b] += (sum f, sum f^2) over the planes [own_lo, own_hi) of f = U1 (stat kCnnStatU) or
 // p_div (kCnnStatPDiv); kCnnStatDiv accumulates nothing here (launch_cnn_div_stats, once U1 is complete).
@@ -104,11 +105,19 @@ void launch_vort_curl(const float* U, float* curl, float* cnorm, float* force, f
                       cudaStream_t st);
 bool launch_vort_curl_quad(const float* U, float* curl, float* cnorm, float* force, float strength, const Geo& g,
                            cudaStream_t st);
-void launch_vort_bc_mask(float* U, const unsigned char* flags, const float* force, int do_vort, const float* u_inv, const float* u_bc, const unsigned char* qmask, int mask_mode, double* sums,
-                         const Geo& g, cudaStream_t st);
-void launch_cnn_inputs_fused(const float* p_div, const float* U1, const unsigned char* flags, const double* sums,
+// sums[b] += (sum f, sum f^2) of f = the masked U (stat kCnnStatU) or p_div (kCnnStatPDiv); any other stat: no sums.
+void launch_vort_bc_mask(float* U, const unsigned char* flags, const float* force, int do_vort, const float* u_inv,
+                         const float* u_bc, const unsigned char* qmask, int mask_mode, double* sums, const Geo& g,
+                         cudaStream_t st, int stat, const float* p_div);
+// normalizeInputChan 'div': sums[b] += (sum div, sum div^2) of U1 (launch_cnn_div_stats on byte flags).
+void launch_cnn_div_stats_fused(const float* U1, const unsigned char* flags, double* sums, const Geo& g,
+                                cudaStream_t st);
+// The conv input of the channel set `sel` (kCnnIn* bits) with the scale of `func` (kCnnScale*) computed from the sums
+// of the field `chan` (kCnnStat*), in the layout of launch_cnn_inputs_padded with planes = 2 when sel has UDiv;
+// scale_out[b] receives the scale.  false (nothing launched) for a set no model has.
+bool launch_cnn_inputs_fused(const float* p_div, const float* U1, const unsigned char* flags, const double* sums,
                              float threshold, float* scale_out, float* x0, int px, int py, const Geo& g,
-                             cudaStream_t st);
+                             cudaStream_t st, int sel, int func, int chan);
 void launch_cnn_finish_fused(const float* p_net, float* U, const unsigned char* flags, const float* scale, float* p_out,
                              const float* u_inv, const float* u_bc, const unsigned char* qmask, float lo, float hi,
                              const Geo& g, cudaStream_t st);
