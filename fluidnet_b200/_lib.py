@@ -58,7 +58,7 @@ SYMBOLS = [
     "tfl_memcpy_d2h", "tfl_memcpy_d2d", "tfl_advect_scalar", "tfl_advect_vel",
     "tfl_set_wall_bcs_forward", "tfl_velocity_divergence_forward", "tfl_velocity_update_forward",
     "tfl_add_buoyancy", "tfl_add_gravity", "tfl_vorticity_confinement",
-    "tfl_solve_linear_system_jacobi", "tfl_solve_linear_system_pcg", "tfl_precond_from_string", "tfl_normalize_pressure_mean",
+    "tfl_solve_linear_system_jacobi", "tfl_solve_linear_system_jacobi_dev", "tfl_solve_linear_system_pcg", "tfl_precond_from_string", "tfl_normalize_pressure_mean",
     "tfl_volumetric_up_sampling_nearest_forward", "tfl_rectangular_blur", "tfl_signed_distance_field", "tfl_velocity_divergence_backward",
     "tfl_velocity_update_backward", "tfl_volumetric_up_sampling_nearest_backward", "tfl_empty_domain", "tfl_flags_to_occupancy", "tfl_apply_bc",
     "tfl_clamp", "tfl_cnn_create", "tfl_cnn_create_graph", "tfl_cnn_create_banked", "tfl_cnn_create_model", "tfl_cnn_create_model_ex", "tfl_cnn_create_model_norm", "tfl_cnn_destroy", "tfl_cnn_set_mode", "tfl_cnn_get_mode", "tfl_cnn_project", "tfl_simulate_step",
@@ -116,6 +116,8 @@ def load():
     lib.tfl_vorticity_confinement.argtypes = [C.c_void_p, G, G, C.c_float]
     lib.tfl_solve_linear_system_jacobi.argtypes = [C.c_void_p, G, G, G, C.c_int, C.c_float, C.c_int,
                                                    C.POINTER(C.c_float), C.POINTER(C.c_int)]
+    lib.tfl_solve_linear_system_jacobi_dev.argtypes = [C.c_void_p, G, G, G, C.c_int, C.c_float, C.c_int, C.c_void_p,
+                                                       C.c_void_p]
     lib.tfl_solve_linear_system_pcg.argtypes = [C.c_void_p, G, G, G, C.c_int, C.c_int, C.c_float, C.c_int,
                                                 C.POINTER(C.c_float), C.POINTER(C.c_int)]
     lib.tfl_precond_from_string.argtypes = [C.c_char_p]

@@ -210,7 +210,7 @@ int tfl_create(tfl_ctx** out, int device) {
   if (!(c->own_stream = new_stream(cudaStreamDefault))) return 1;
   c->stream = c->own_stream.get();
   if (!(c->counters = dev_zeros<unsigned long long>(16))) return 1;
-  for (StreamPtr* q : {&c->side_stream, &c->copy_in, &c->copy_out})
+  for (StreamPtr* q : {&c->side_stream, &c->copy_in, &c->copy_out, &c->jacobi_body})
     if (!(*q = new_stream(cudaStreamNonBlocking))) return 1;
   for (EventPtr* e : {&c->ev_fork, &c->ev_join, &c->ev_u_in, &c->ev_d_in, &c->ev_p_in, &c->ev_d_ready, &c->ev_d_out})
     if (!(*e = new_event(cudaEventDisableTiming))) return 1;
@@ -512,16 +512,163 @@ int tfl_advect_vel(tfl_ctx* ctx, float dt, const tfl_grid* U, const tfl_grid* fl
   return in_place ? copy_planes(ctx, U->data, tmp, g.nb * g.nc, g) : 0;
 }
 
-int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags,
-                                   const tfl_grid* div, int is_3d, float p_tol, int max_iter,
-                                   float* residual, int* iterations) {
-  DeviceGuard guard_(ctx);
-  NvtxRange range_(__func__);
+}  // extern "C"
+
+namespace {
+int jacobi_check_args(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div, int is_3d,
+                      int max_iter) {
   if (check_scalar(ctx, flags, "flags") || check_scalar(ctx, p, "p") || check_scalar(ctx, div, "div")) return 1;
   if (!same_spatial(flags, p) || !same_spatial(flags, div)) return fail(ctx, "size mismatch");
   if (!is_3d && flags->nz != 1) return fail(ctx, "d > 1 for a 2D domain");
   if (max_iter < 1) return fail(ctx, "At least 1 iteration is needed (maxIter < 1)");
   if (ctx->slab) return fail(ctx, "Jacobi on a z-slab goes through the multi-GPU driver (halo exchange per sweep)");
+  return 0;
+}
+
+// Whether the context's stream is being captured into a graph (*capturing), or fails naming `who`.
+int stream_capturing(tfl_ctx* ctx, const char* who, bool* capturing) {
+  cudaStream_t st = ctx->stream;
+  cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
+  const cudaError_t e = cudaStreamIsCapturing(st, &cs);
+  const bool default_stream = st == nullptr || st == cudaStreamLegacy || st == cudaStreamPerThread;
+  if (default_stream && (e != cudaSuccess || cs != cudaStreamCaptureStatusNone)) {
+    cudaGetLastError();
+    return fail(ctx, "%s: the default stream cannot be captured; give the context a stream (tfl_set_stream)", who);
+  }
+  TFL_CUDA(ctx, e);
+  *capturing = cs != cudaStreamCaptureStatusNone;
+  return 0;
+}
+
+// The chunked path's sweeps of the tolerance solve: sweep k reads pPrev and writes p for even k, the reverse for odd k,
+// and is followed by its residual.  A captured solve's loop body is kJacobiBodySweeps sweeps (even, so every pass
+// starts on the same buffers); a direct one enqueues chunks of 8, 16, ... up to kJacobiMaxChunk sweeps and reads
+// state.done after each, so it waits about log2(iterations / 8) + iterations / 256 times and runs at most one chunk
+// of no-op launches after the solve has stopped.
+constexpr int kJacobiBodySweeps = 16;
+constexpr int kJacobiFirstChunk = 8, kJacobiMaxChunk = 256;
+void jacobi_tol_sweeps(const unsigned char* mask, const float* div, float* p, float* p_prev, const Geo& g, int k0,
+                       int count, const JacobiTolArgs& t, cudaStream_t st) {
+  for (int k = k0; k < k0 + count; k++) {
+    launch_jacobi_iter(mask, div, (k & 1) ? p : p_prev, (k & 1) ? p_prev : p, g, st, &t.state->done);
+    launch_jacobi_residual(p, p_prev, g, t, st);
+  }
+}
+
+// The tolerance solve of both Jacobi entry points, enqueued without a host wait on the resident path and inside a
+// capture.  *state_out receives the device state (in the scratch arena), which holds the result once the stream
+// reaches it.
+int jacobi_tol_solve(tfl_ctx* ctx, const char* who, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
+                     int is_3d, float p_tol, int max_iter, float* dev_residual, int32_t* dev_iterations,
+                     bool capturing, JacobiState** state_out) {
+  Geo g;
+  if (make_geo(ctx, flags, is_3d, &g)) return 1;
+  const size_t cells = (size_t)g.n * g.nb;
+  const size_t bytes =
+      carve_bytes({cells * 4, cells, sizeof(double) * (size_t)jacobi_tol_slots(g), sizeof(JacobiState)});
+  if (capturing && bytes > ctx->arena_bytes)     // growing the arena synchronises, which would end the capture
+    return fail(ctx, "%s: the scratch arena would grow inside a capture; run the solve once on this grid before "
+                     "capturing it", who);
+  if (arena_reserve(ctx, bytes)) return 1;
+  Carver cv(ctx);
+  float* p_prev = cv.take<float>(cells);
+  unsigned char* mask = cv.take<unsigned char>(cells);
+  JacobiTolArgs t;
+  t.slots = cv.take<double>((size_t)jacobi_tol_slots(g));
+  t.state = cv.take<JacobiState>(1);
+  t.res_out = dev_residual;
+  t.iter_out = dev_iterations;
+  t.tol = p_tol;
+  t.max_iter = max_iter;
+  cudaStream_t st = ctx->stream;
+  launch_jacobi_mask(flags->data, mask, g, st);
+  ctx->launches += 1;
+  // p <- 0, pPrev <- 0 (generic/tfluids.cu:1854-1855)
+  TFL_CUDA(ctx, cudaMemsetAsync(p->data, 0, cells * 4, st));
+  TFL_CUDA(ctx, cudaMemsetAsync(p_prev, 0, cells * 4, st));
+  TFL_CUDA(ctx, cudaMemsetAsync(t.state, 0, sizeof(JacobiState), st));
+  *state_out = t.state;
+  if (launch_jacobi_tol_resident(mask, div->data, p_prev, p->data, g, max_iter, t, st)) {
+    ctx->launches += 1;
+    return check_launch(ctx, who);
+  }
+  if (capturing) {
+    // one WHILE node whose body is a chunk of sweeps; the residual that stops the solve clears the node's handle
+    cudaGraphConditionalHandle loop;
+    TFL_CUDA(ctx, capture_while_handle(st, 1, &loop));
+    t.loop = loop;
+    t.has_loop = 1;
+    cudaStream_t bs = ctx->jacobi_body.get();
+    TFL_CUDA(ctx, capture_while_body(st, loop, bs));
+    jacobi_tol_sweeps(mask, div->data, p->data, p_prev, g, 0, kJacobiBodySweeps, t, bs);
+    const cudaError_t le = cudaGetLastError();
+    cudaGraph_t body = nullptr;
+    const cudaError_t ee = cudaStreamEndCapture(bs, &body);      // ends the body's capture on every path
+    TFL_CUDA(ctx, le);
+    TFL_CUDA(ctx, ee);
+    ctx->launches += 2 * kJacobiBodySweeps;                      // one pass of the body
+  } else {
+    if (!ctx->jacobi_host && !(ctx->jacobi_host = pinned_alloc<int>(1))) return fail(ctx, "%s: cudaMallocHost failed", who);
+    int k = 0;
+    for (int chunk = kJacobiFirstChunk;; chunk = std::min(2 * chunk, kJacobiMaxChunk)) {
+      const int n = std::min(chunk, max_iter - k);
+      jacobi_tol_sweeps(mask, div->data, p->data, p_prev, g, k, n, t, st);
+      ctx->launches += 2 * n;
+      k += n;
+      if (k >= max_iter) break;                                  // the last residual stops the solve
+      TFL_CUDA(ctx, cudaMemcpyAsync(ctx->jacobi_host.get(), &t.state->done, sizeof(int), cudaMemcpyDeviceToHost, st));
+      TFL_CUDA(ctx, cudaStreamSynchronize(st));
+      if (*ctx->jacobi_host) break;
+    }
+  }
+  launch_jacobi_copy_back(p->data, p_prev, (long long)cells, t.state, st);
+  ctx->launches += 1;
+  return check_launch(ctx, who);
+}
+}  // namespace
+
+extern "C" {
+
+int tfl_solve_linear_system_jacobi_dev(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
+                                       int is_3d, float p_tol, int max_iter, float* dev_residual,
+                                       int32_t* dev_iterations) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!ctx) return 1;
+  if (jacobi_check_args(ctx, p, flags, div, is_3d, max_iter)) return 1;
+  bool capturing = false;
+  if (stream_capturing(ctx, "solveLinearSystemJacobiDevice", &capturing)) return 1;
+  JacobiState* state = nullptr;
+  return jacobi_tol_solve(ctx, "solveLinearSystemJacobiDevice", p, flags, div, is_3d, p_tol, max_iter, dev_residual,
+                          dev_iterations, capturing, &state);
+}
+
+int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags,
+                                   const tfl_grid* div, int is_3d, float p_tol, int max_iter,
+                                   float* residual, int* iterations) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (jacobi_check_args(ctx, p, flags, div, is_3d, max_iter)) return 1;
+  if (p_tol > 0.0f || residual || iterations) {       // what reads the device (the step's solve passes neither)
+    bool capturing = false;
+    if (stream_capturing(ctx, "solveLinearSystemJacobi", &capturing)) return 1;
+    if (capturing)
+      return fail(ctx, "solveLinearSystemJacobi: the stream is being captured and this call reads its result on the "
+                       "host; capture tfl_solve_linear_system_jacobi_dev instead");
+  }
+  if (p_tol > 0.0f) {
+    JacobiState* state = nullptr;
+    if (jacobi_tol_solve(ctx, "solveLinearSystemJacobi", p, flags, div, is_3d, p_tol, max_iter, nullptr, nullptr,
+                         false, &state))
+      return 1;
+    if (!residual && !iterations) return 0;
+    JacobiState h;
+    TFL_CUDA(ctx, cudaMemcpyAsync(&h, state, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (residual) *residual = h.res;
+    if (iterations) *iterations = h.iter;
+    return 0;
+  }
   Geo g;
   if (make_geo(ctx, flags, is_3d, &g)) return 1;
   const size_t cells = (size_t)g.n * g.nb;

@@ -49,6 +49,8 @@ struct tfl_ctx {
     bool density_sent = false;
   } ov;
   PcgScratch pcg;                           // grow-only buffers of the PCG solve
+  StreamPtr jacobi_body;                    // captures the loop body of a captured Jacobi tolerance solve
+  PinnedPtr<int> jacobi_host;               // the Jacobi tolerance solve's read of its done word
   PcgGraphScratch* pcg_graph = nullptr;     // set while tfl_step_graph_create captures: PCG solves are captured there
   // Byte copy of the step's flags and their clearance field (advection fast path), kept between steps:
   // each step re-derives the bytes, compares them with the copy on the device and rebuilds the

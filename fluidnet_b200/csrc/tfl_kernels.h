@@ -47,8 +47,9 @@ bool launch_advect_scalar_tile(float dt, const float* src, const float* U, const
 int launch_clearance(const unsigned char* flags, unsigned char* clear, unsigned char* tmp, const Geo& g, const int* gate,
                      cudaStream_t st);
 void launch_jacobi_mask(const float* flags, unsigned char* mask, const Geo& g, cudaStream_t st);
+// done: optional device word (JacobiState::done); the sweep does nothing once it is set.
 void launch_jacobi_iter(const unsigned char* mask, const float* div, const float* prev, float* cur,
-                        const Geo& g, cudaStream_t st);
+                        const Geo& g, cudaStream_t st, const int* done = nullptr);
 // One block of `sweeps` sweeps on local planes [z_lo, z_hi) that shrink by shr_lo / shr_hi planes per sweep
 // (sweep s reads pa and writes pb for even s, the reverse for odd s).  launch_jacobi_block runs them in one
 // cooperative launch and returns its block depth in planes (4, or 6 with `deep`), or 0 when the shape / device does
@@ -59,6 +60,35 @@ int launch_jacobi_block(const unsigned char* mask, const float* div, float* pa, 
 void launch_jacobi_range_sweeps(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,
                                 int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, cudaStream_t st);
 void launch_sqdiff(const float* a, const float* b, long long n, int nb, double* out, cudaStream_t st);
+// The Jacobi solve run to a tolerance on the device (tfl_solve_linear_system_jacobi_dev): the host loop's state.
+struct JacobiState {
+  int done;            // set once the solve has stopped
+  int iter;            // the host loop's iteration counter
+  unsigned arrived;    // CTAs of the current residual launch that have written their slot
+  int last;            // index of the last sweep run: it wrote p when even, pPrev when odd
+  float res;           // residual of the last sweep
+};
+struct JacobiTolArgs {
+  double* slots = nullptr;          // per-CTA partial sums of (p - pPrev)^2 per batch entry (jacobi_tol_slots doubles)
+  JacobiState* state = nullptr;     // zeroed before the first sweep
+  float* res_out = nullptr;         // optional device copies of the final residual and iteration count
+  int* iter_out = nullptr;
+  float tol = 0.0f;
+  int max_iter = 0;
+  cudaGraphConditionalHandle loop = 0;   // the WHILE node of a captured solve (has_loop): cleared when it stops
+  int has_loop = 0;
+};
+// Doubles of JacobiTolArgs::slots either path below needs on grid g.
+long long jacobi_tol_slots(const Geo& g);
+// The whole solve in one cooperative launch (k_jacobi_resident<4, true>): sweep 0 reads p_prev and writes p, p gets
+// the result, state and the outputs are written.  false (nothing launched) when the grid does not qualify (3-D,
+// nz >= 4, up to 3 x 2^20 cells, nx % 128, ny % 8, aligned, co-resident).
+bool launch_jacobi_tol_resident(const unsigned char* mask, const float* div, float* p_prev, float* p, const Geo& g,
+                                int max_iter, const JacobiTolArgs& t, cudaStream_t st);
+// The device-driven loop on every other grid: after each launch_jacobi_iter with done = &state->done, one residual
+// launch; once the loop has stopped, the copy back moves the result into p when it ended in p_prev.
+void launch_jacobi_residual(const float* p, const float* p_prev, const Geo& g, const JacobiTolArgs& t, cudaStream_t st);
+void launch_jacobi_copy_back(float* p, const float* p_prev, long long cells, const JacobiState* state, cudaStream_t st);
 // changed: optional device word that is OR-ed with 1 when a byte differs from what `o` held before.
 void launch_flags_to_u8(const float* f, unsigned char* o, long long n, int* changed, cudaStream_t st);
 void launch_apply_bc(float* x, const float* inv, const float* bc, long long n, cudaStream_t st);
@@ -186,6 +216,12 @@ struct PcgGraphScratch {
   long long body_launches = 0; // kernels in one pass of the loop body
   bool captured = false;       // a solve was captured
 };
+// A conditional WHILE node in a stream capture (the PCG solve of a step graph, the Jacobi tolerance solve).
+// capture_while_handle: a handle on the graph st is capturing, reset to `initial` at every launch of the graph.
+// capture_while_body: the node, after what st has captured so far, and the capture of stream `body` into the node's
+// body graph, which the caller ends with cudaStreamEndCapture(body).  A body kernel re-arms or clears the handle.
+cudaError_t capture_while_handle(cudaStream_t st, unsigned initial, cudaGraphConditionalHandle* loop);
+cudaError_t capture_while_body(cudaStream_t st, cudaGraphConditionalHandle loop, cudaStream_t body);
 size_t pcg_workspace_bytes(int nb, int nz, int ny, int nx);
 const char* pcg_status_string(int rc);
 // precond: 0 none, 1 ilu0, 2 ic0.  Returns 0 or a status for pcg_status_string.  Synchronises `st`.

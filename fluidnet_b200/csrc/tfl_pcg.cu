@@ -934,6 +934,34 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
   return 0;
 }
 
+cudaError_t capture_while_handle(cudaStream_t st, unsigned initial, cudaGraphConditionalHandle* loop) {
+  cudaStreamCaptureStatus cap_status;
+  cudaGraph_t graph = nullptr;
+  cudaError_t e = cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, nullptr, nullptr);
+  if (e != cudaSuccess) return e;
+  if (cap_status != cudaStreamCaptureStatusActive) return cudaErrorStreamCaptureInvalidated;
+  return cudaGraphConditionalHandleCreate(loop, graph, initial, cudaGraphCondAssignDefault);
+}
+
+cudaError_t capture_while_body(cudaStream_t st, cudaGraphConditionalHandle loop, cudaStream_t body) {
+  cudaStreamCaptureStatus cap_status;
+  cudaGraph_t graph = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t ndeps = 0;
+  cudaError_t e = cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, &deps, &ndeps);
+  if (e != cudaSuccess) return e;
+  cudaGraphNodeParams np = {};
+  np.type = cudaGraphNodeTypeConditional;
+  np.conditional.handle = loop;
+  np.conditional.type = cudaGraphCondTypeWhile;
+  np.conditional.size = 1;
+  cudaGraphNode_t node;
+  if ((e = cudaGraphAddNode(&node, graph, deps, ndeps, &np)) != cudaSuccess) return e;
+  if ((e = cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies)) != cudaSuccess) return e;
+  return cudaStreamBeginCaptureToGraph(body, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                       cudaStreamCaptureModeRelaxed);
+}
+
 int pcg_graph_alloc(PcgGraphScratch& gs, PcgScratch& sc, int nb, int nz, int ny, int nx, int is3d) {
   PcgGeo g;
   if (pcg_geometry(sc, nb, nz, ny, nx, is3d, g)) return 4;
@@ -987,30 +1015,14 @@ int pcg_solve_graph(PcgGraphScratch& gs, PcgScratch& sc, void* workspace, float*
   *launches += 2;
 
   // the WHILE node after what is captured so far; the first test arms it
-  cudaStreamCaptureStatus cap_status;
-  cudaGraph_t graph = nullptr;
-  const cudaGraphNode_t* deps = nullptr;
-  size_t ndeps = 0;
-  PCG_CUDA(cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, &deps, &ndeps));
-  if (cap_status != cudaStreamCaptureStatusActive) return 3;
   cudaGraphConditionalHandle loop;
-  PCG_CUDA(cudaGraphConditionalHandleCreate(&loop, graph, 0, cudaGraphCondAssignDefault));
+  PCG_CUDA(capture_while_handle(st, 0, &loop));
   k_pcg_continue<<<1, 1, 0, st>>>(s.header, loop, nullptr);
   *launches += 1;
-  PCG_CUDA(cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, &deps, &ndeps));
-  cudaGraphNodeParams np = {};
-  np.type = cudaGraphNodeTypeConditional;
-  np.conditional.handle = loop;
-  np.conditional.type = cudaGraphCondTypeWhile;
-  np.conditional.size = 1;
-  cudaGraphNode_t node;
-  PCG_CUDA(cudaGraphAddNode(&node, graph, deps, ndeps, &np));
-  PCG_CUDA(cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies));
 
   // the body, captured on the graph's own stream into the node's body graph
   cudaStream_t bs = gs.body_stream.get();
-  PCG_CUDA(cudaStreamBeginCaptureToGraph(bs, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
-                                         cudaStreamCaptureModeRelaxed));
+  PCG_CUDA(capture_while_body(st, loop, bs));
   long long body = 0;
   cudaError_t be = cudaSuccess;
   float* p_old = s.p0;

@@ -683,9 +683,11 @@ __global__ void k_jacobi_mask(const float* __restrict__ flags, unsigned char* __
   mask[b * g.n + cell(g, k, j, i)] = (unsigned char)m;
 }
 
-template <bool IS3D>
+// GATED (the tolerance solve's device-driven loop, JacobiTolArgs): the sweep does nothing once *done is set.
+template <bool IS3D, bool GATED>
 __global__ void k_jacobi_iter(const unsigned char* __restrict__ mask, const float* __restrict__ div,
-                              const float* __restrict__ prev, float* __restrict__ cur, Geo gin) {
+                              const float* __restrict__ prev, float* __restrict__ cur, Geo gin, const int* done) {
+  if (GATED && __ldcg(done)) return;
   const Geo g = static_geo<IS3D>(gin);
   int b, k, j, i;
   if (!thread_cell(g, b, k, j, i)) return;
@@ -739,10 +741,11 @@ __device__ __forceinline__ void jacobi_update4(unsigned m4, float4 ctr, float le
 
 // Same update, 4 consecutive x cells per thread (float4 rows, one 32-bit load for the 4 mask
 // bytes): 8 memory instructions per 4 cells instead of 40.  Requires nx % 4 == 0.
-template <bool IS3D>
+template <bool IS3D, bool GATED>
 __global__ void __launch_bounds__(256)
 k_jacobi_iter4(const unsigned char* __restrict__ mask, const float* __restrict__ div,
-               const float* __restrict__ prev, float* __restrict__ cur, Geo gin) {
+               const float* __restrict__ prev, float* __restrict__ cur, Geo gin, const int* done) {
+  if (GATED && __ldcg(done)) return;
   const Geo g = static_geo<IS3D>(gin);
   const int i0 = (blockIdx.x * blockDim.x + threadIdx.x) * 4;
   const int j = blockIdx.y * blockDim.y + threadIdx.y;
@@ -778,10 +781,12 @@ k_jacobi_iter4(const unsigned char* __restrict__ mask, const float* __restrict__
 // exchanged through shared memory, x neighbours with warp shuffles.  Per-cell arithmetic is the
 // same expression as above (bit-identical).  Requires 3-D, nx % 128 == 0, ny % 8 == 0.
 constexpr int kJY = 8;
+template <bool GATED>
 __global__ void __launch_bounds__(256)
 k_jacobi_march(const unsigned char* __restrict__ mask, const float* __restrict__ div,
-               const float* __restrict__ prev, float* __restrict__ cur, Geo g, int zchunk) {
+               const float* __restrict__ prev, float* __restrict__ cur, Geo g, int zchunk, const int* done) {
   __shared__ float4 rows[2][kJY][32];
+  if (GATED && __ldcg(done)) return;
   const int tx = threadIdx.x, ty = threadIdx.y;
   const int i0 = (blockIdx.x * 32 + tx) * 4;
   const int j = blockIdx.y * kJY + ty;
@@ -833,6 +838,37 @@ k_jacobi_march(const unsigned char* __restrict__ mask, const float* __restrict__
   }
 }
 
+// The tolerance solve (JacobiTolArgs).  The residual after a sweep is (float) max over the batch entries of
+// sqrt(sum (p - pPrev)^2), each sum in double; its partial sums go to slots and are added in an order fixed by the
+// slot count alone, so the same inputs give the same residual bits on every run.
+// Sum of slots[0, n) by one warp: lane l adds slots l, l + 32, ... in turn, then a butterfly adds the lanes.  Every
+// lane gets the same bits (a + b == b + a).
+__device__ __forceinline__ double warp_fixed_sum(const double* slots, int n, int lane) {
+  double v = 0.0;
+  for (int c = lane; c < n; c += 32) v += __ldcg(slots + c);
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+// The host loop's test after sweep s (0-based) with residual res: stop when res < tol, before the counter counts the
+// sweep, or once the counter reaches max_iter.  *iter receives the counter.
+__device__ __forceinline__ bool jacobi_stops(float res, float tol, int s, int max_iter, int* iter) {
+  if (res < tol) {
+    *iter = s;
+    return true;
+  }
+  *iter = s + 1;
+  return s + 1 >= max_iter;
+}
+__device__ __forceinline__ void jacobi_record_stop(const JacobiTolArgs& t, float res, int iter, int last) {
+  t.state->res = res;
+  t.state->iter = iter;
+  t.state->last = last;
+  t.state->done = 1;
+  if (t.res_out) *t.res_out = res;
+  if (t.iter_out) *t.iter_out = iter;
+}
+
 // Jacobi sweeps in ONE cooperative launch with the CTA's cells resident on the SM: the whole-grid solve of
 // tfl_solve_linear_system_jacobi (planes [0, nz), no shrink) and the sweep blocks of the z-slab step (tfl_slab_sim_step).
 // A 256-thread group owns a 128 x 8 x KZ block for the whole launch (every CTA stays resident): its p values live in
@@ -850,11 +886,53 @@ k_jacobi_march(const unsigned char* __restrict__ mask, const float* __restrict__
 // at most 132 * 4 * 4096 * KZ / 4 cells on an H100: 2.16M with KZ = 4, 3.24M with KZ = 6 -- the deepest block whose
 // shared memory (kJG x KZ x (18 rows of 32 float4 + the x halo)) fits one SM: 217.5 KiB.  The dispatcher takes the
 // shallowest KZ that fits.  The x halo goes through shared memory to spare registers.
+// TOL: the tolerance solve of tfl_solve_linear_system_jacobi_dev on planes [0, nz) with no shrink, pa = pPrev and
+// pb = p.  `sweeps` is maxIter and `t` the stop test.  After each sweep every CTA writes its sum of (p - pPrev)^2 per
+// batch entry into t.slots[sweep parity][entry][CTA]; the grid-wide barrier that separates the sweeps orders those
+// writes, and then every CTA adds the slots of each entry in the same fixed order, takes the largest norm and makes the
+// host loop's stop decision itself.  Every CTA computes the same bits, so all stop after the same sweep with no
+// further barrier.  A slot of parity s & 1 is rewritten two sweeps later, after a barrier every reader has passed.  A
+// solve that ends on pa copies its registers into pb.
 constexpr int kJG = 4;        // blocks per CTA: fewer, fatter CTAs make the grid-wide barrier (one atomic per CTA) cheaper
-template <int KZ>
+// The stop test of k_jacobi_resident<KZ, true> after sweep s, sq being the thread's sum: the CTA's per-entry sums into
+// the slots, the grid-wide barrier, then every CTA's own reduction of the slots and decision.  CTA 0 records the stop.
+__device__ __forceinline__ bool jacobi_resident_stop(const JacobiTolArgs& t, cooperative_groups::grid_group& grid,
+                                                  double sq, int s, int max_iter, int nblocks, int nxy, int nchunks,
+                                                  int nb) {
+  __shared__ double psum[kJG * kJY];                       // per warp: written before the barrier, read before it
+  __shared__ double wmax[kJG * kJY];                       // per warp: written after the barrier, read after it
+  const int lane = threadIdx.x, warp = threadIdx.z * kJY + threadIdx.y, tid = warp * 32 + lane;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) sq += __shfl_down_sync(0xffffffffu, sq, o);
+  if (lane == 0) psum[warp] = sq;
+  __syncthreads();
+  double* slots = t.slots + (size_t)(s & 1) * nb * gridDim.x;
+  for (int e = tid; e < nb; e += 32 * kJG * kJY) {         // groups of other entries (or none) add nothing
+    double v = 0.0;
+    for (int z = 0; z < kJG; z++) {
+      const int blk = blockIdx.x * kJG + z;
+      if (blk < nblocks && blk / nxy / nchunks == e)
+        for (int w = 0; w < kJY; w++) v += psum[z * kJY + w];
+    }
+    __stcg(slots + (size_t)e * gridDim.x + blockIdx.x, v);
+  }
+  grid.sync();
+  double worst = 0.0;
+  for (int e = warp; e < nb; e += kJG * kJY)
+    worst = fmax(worst, sqrt(warp_fixed_sum(slots + (size_t)e * gridDim.x, gridDim.x, lane)));
+  if (lane == 0) wmax[warp] = worst;
+  __syncthreads();
+  for (int w = 0; w < kJG * kJY; w++) worst = fmax(worst, wmax[w]);
+  const float res = (float)worst;
+  int iter;
+  const bool stop = jacobi_stops(res, t.tol, s, max_iter, &iter);
+  if (stop && blockIdx.x == 0 && tid == 0) jacobi_record_stop(t, res, iter, s);
+  return stop;
+}
+template <int KZ, bool TOL>
 __global__ void __launch_bounds__(256 * kJG, 1)
 k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb, Geo g,
-                  int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks) {
+                  int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks, JacobiTolArgs t) {
   cooperative_groups::grid_group grid = cooperative_groups::this_grid();
   extern __shared__ float4 jsm[];
   // thread group threadIdx.z of the CTA owns block blockIdx.x * kJG + threadIdx.z (x tile fastest, then y, then z chunk)
@@ -888,6 +966,7 @@ k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restric
     pc[k] = in ? __ldcg((const float4*)(pa + base + (long long)k * sz)) : zero4;
   }
   for (int s = 0; s < sweeps; s++) {
+    double sq = 0.0;                                       // TOL: this thread's sum of (p - pPrev)^2 in the sweep
     const float* prev = (s & 1) ? pb : pa;                 // sweep 0 reads pa and writes pb
     float* cur = (s & 1) ? pa : pb;
     const float* pp = prev + base;                         // per-sweep pointers keep the plane offsets 32-bit
@@ -925,10 +1004,26 @@ k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restric
         const float4 o4 = make_float4(out[0], out[1], out[2], out[3]);
         *(float4*)(cp + k * sz) = o4;
         pc[k] = o4;
+        if constexpr (TOL) {                               // k_sqdiff's terms: a float difference squared in double
+          const float d[4] = {out[0] - ctr.x, out[1] - ctr.y, out[2] - ctr.z, out[3] - ctr.w};
+#pragma unroll
+          for (int q = 0; q < 4; q++) sq += (double)d[q] * (double)d[q];
+        }
       }
       below = ctr;
     }
-    if (s + 1 < sweeps) grid.sync();                       // also orders the shared rows against the next sweep
+    if constexpr (TOL) {
+      if (jacobi_resident_stop(t, grid, sq, s, sweeps, nblocks, nxt * nyt, nchunks, g.nb)) {
+        if (s & 1) {                                       // the last sweep wrote pPrev (pa): p takes its values
+#pragma unroll
+          for (int k = 0; k < KZ; k++)
+            if (k < np) *(float4*)(pb + base + (long long)k * sz) = pc[k];
+        }
+        return;
+      }
+    } else {
+      if (s + 1 < sweeps) grid.sync();                     // also orders the shared rows against the next sweep
+    }
   }
 }
 
@@ -954,6 +1049,66 @@ __global__ void k_sqdiff(const float* __restrict__ a, const float* __restrict__ 
     for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
     if (lane == 0) atomicAdd(out + b, acc);
   }
+}
+
+// The residual of the tolerance solve's device-driven loop after one sweep: k_sqdiff's sums, each CTA's into its slot
+// t.slots[entry][CTA].  The last CTA to arrive adds the slots in a fixed order, applies the host loop's test and, when
+// the solve stops, sets state.done (every later gated sweep and residual returns at once) and clears the WHILE node
+// of a captured solve.  While the solve runs, state.iter is the index of the sweep being tested.
+__global__ void __launch_bounds__(256)
+k_jacobi_residual(const float* __restrict__ a, const float* __restrict__ bb, long long n, JacobiTolArgs t) {
+  __shared__ double red[8];
+  __shared__ bool last;
+  JacobiState* st = t.state;
+  if (__ldcg(&st->done)) return;
+  const int b = blockIdx.y;
+  const float* pa = a + b * n;
+  const float* pb = bb + b * n;
+  double acc = 0.0;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
+    const float d = pa[i] - pb[i];
+    acc += (double)d * (double)d;
+  }
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
+  if (lane == 0) red[w] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < 8; k++) acc += red[k];
+    __stcg(t.slots + (size_t)b * gridDim.x + blockIdx.x, acc);
+    __threadfence();
+    last = atomicAdd(&st->arrived, 1u) + 1 == gridDim.x * gridDim.y;
+  }
+  __syncthreads();
+  if (!last) return;
+  __threadfence();
+  double worst = 0.0;
+  for (int e = w; e < (int)gridDim.y; e += 8)
+    worst = fmax(worst, sqrt(warp_fixed_sum(t.slots + (size_t)e * gridDim.x, gridDim.x, lane)));
+  if (lane == 0) red[w] = worst;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int k = 1; k < 8; k++) worst = fmax(worst, red[k]);
+    const float res = (float)worst;
+    const int s = st->iter;
+    int iter;
+    st->arrived = 0;
+    if (jacobi_stops(res, t.tol, s, t.max_iter, &iter)) {
+      jacobi_record_stop(t, res, iter, s);
+      if (t.has_loop) cudaGraphSetConditional(t.loop, 0u);
+    } else {
+      st->iter = iter;
+    }
+  }
+}
+
+// p <- pPrev once the device-driven loop has stopped with its last sweep on pPrev (an odd sweep index).
+__global__ void k_jacobi_copy_back(float* __restrict__ p, const float* __restrict__ p_prev, long long cells,
+                                   const JacobiState* __restrict__ st) {
+  if (!(st->last & 1)) return;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (long long)gridDim.x * blockDim.x)
+    p[i] = p_prev[i];
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1117,8 +1272,10 @@ bool jacobi_aligned(const unsigned char* mask, const float* div, const float* pa
   return (uintptr_t)mask % 4 == 0 && (uintptr_t)div % 16 == 0 && (uintptr_t)pa % 16 == 0 && (uintptr_t)pb % 16 == 0;
 }
 }  // namespace
-void launch_jacobi_iter(const unsigned char* mask, const float* div, const float* prev, float* cur,
-                        const Geo& g, cudaStream_t st) {
+namespace {
+template <bool GATED>
+void jacobi_iter(const unsigned char* mask, const float* div, const float* prev, float* cur, const Geo& g,
+                 const int* done, cudaStream_t st) {
   const bool aligned = jacobi_aligned(mask, div, prev, cur);
   // The marching kernel pays off once the fields no longer fit L2 (>= 4M cells); smaller grids keep
   // more CTAs in flight with the flat float4 kernel.  (Tests force it through nx == 128 / 256 shapes
@@ -1131,7 +1288,7 @@ void launch_jacobi_iter(const unsigned char* mask, const float* div, const float
     while (zchunk > 4 && (long long)xy_ctas * ((g.nz + zchunk - 1) / zchunk) < 592) zchunk >>= 1;
     dim3 block(32, kJY, 1);
     dim3 grid(g.nx / 128, g.ny / kJY, ((g.nz + zchunk - 1) / zchunk) * g.nb);
-    k_jacobi_march<<<grid, block, 0, st>>>(mask, div, prev, cur, g, zchunk);
+    k_jacobi_march<GATED><<<grid, block, 0, st>>>(mask, div, prev, cur, g, zchunk, done);
     return;
   }
   if (g.nx % 4 == 0 && aligned) {
@@ -1142,15 +1299,24 @@ void launch_jacobi_iter(const unsigned char* mask, const float* div, const float
     block.z = g.nz == 1 ? 1 : 2;
     dim3 grid((qx + block.x - 1) / block.x, (g.ny + block.y - 1) / block.y,
               ((long long)g.nb * nzr + block.z - 1) / block.z);
-    if (g.is3d) k_jacobi_iter4<true><<<grid, block, 0, st>>>(mask, div, prev, cur, g);
-    else k_jacobi_iter4<false><<<grid, block, 0, st>>>(mask, div, prev, cur, g);
+    if (g.is3d) k_jacobi_iter4<true, GATED><<<grid, block, 0, st>>>(mask, div, prev, cur, g, done);
+    else k_jacobi_iter4<false, GATED><<<grid, block, 0, st>>>(mask, div, prev, cur, g, done);
     return;
   }
-  TFL_LAUNCH3(k_jacobi_iter, g, st, mask, div, prev, cur, g);
+  dim3 grid, block;
+  launch_dims(g, grid, block);
+  if (g.is3d) k_jacobi_iter<true, GATED><<<grid, block, 0, st>>>(mask, div, prev, cur, g, done);
+  else k_jacobi_iter<false, GATED><<<grid, block, 0, st>>>(mask, div, prev, cur, g, done);
+}
+}  // namespace
+void launch_jacobi_iter(const unsigned char* mask, const float* div, const float* prev, float* cur,
+                        const Geo& g, cudaStream_t st, const int* done) {
+  if (done) jacobi_iter<true>(mask, div, prev, cur, g, done, st);
+  else jacobi_iter<false>(mask, div, prev, cur, g, nullptr, st);
 }
 namespace {
-// Resident CTAs of k_jacobi_resident<KZ> on the current device (0 when it cannot be launched cooperatively).
-template <int KZ>
+// Resident CTAs of k_jacobi_resident<KZ, TOL> on the current device (0 when it cannot be launched cooperatively).
+template <int KZ, bool TOL>
 int jacobi_block_capacity(int smem) {
   static int capacities[64];         // per device (0: not asked yet, -1: cannot)
   int dev = 0;
@@ -1161,26 +1327,29 @@ int jacobi_block_capacity(int smem) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
     capacity = -1;
-    if (coop && cudaFuncSetAttribute(k_jacobi_resident<KZ>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_jacobi_resident<KZ>, 256 * kJG, smem) == cudaSuccess &&
+    if (coop && cudaFuncSetAttribute(k_jacobi_resident<KZ, TOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_jacobi_resident<KZ, TOL>, 256 * kJG, smem) == cudaSuccess &&
         sms * per_sm > 0)
       capacity = sms * per_sm;
     cudaGetLastError();
   }
   return capacity > 0 ? capacity : 0;
 }
-template <int KZ>
+int jacobi_block_count(const Geo& g, int z_lo, int z_hi, int kz) {
+  return (g.nx / 128) * (g.ny / kJY) * ((z_hi - z_lo + kz - 1) / kz) * g.nb;
+}
+template <int KZ, bool TOL = false>
 int try_jacobi_block(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo, int z_hi,
-                     int shr_lo, int shr_hi, int sweeps, cudaStream_t st) {
+                     int shr_lo, int shr_hi, int sweeps, cudaStream_t st, JacobiTolArgs t = JacobiTolArgs()) {
   const int smem = kJG * (KZ * (kJY + 2) * 32 + KZ * kJY * 32 + KZ * kJY * 2 / 4) * (int)sizeof(float4);
-  int nblocks = (g.nx / 128) * (g.ny / kJY) * ((z_hi - z_lo + KZ - 1) / KZ) * g.nb;
+  int nblocks = jacobi_block_count(g, z_lo, z_hi, KZ);
   const int ctas = (nblocks + kJG - 1) / kJG;
-  if (ctas > jacobi_block_capacity<KZ>(smem)) return 0;
+  if (ctas > jacobi_block_capacity<KZ, TOL>(smem)) return 0;
   dim3 block(32, kJY, kJG), grid(ctas, 1, 1);
   Geo gg = g;
   void* args[] = {(void*)&mask, (void*)&div, (void*)&pa, (void*)&pb, (void*)&gg, (void*)&z_lo, (void*)&z_hi,
-                  (void*)&shr_lo, (void*)&shr_hi, (void*)&sweeps, (void*)&nblocks};
-  if (cudaLaunchCooperativeKernel((const void*)k_jacobi_resident<KZ>, grid, block, args, smem, st) != cudaSuccess) {
+                  (void*)&shr_lo, (void*)&shr_hi, (void*)&sweeps, (void*)&nblocks, (void*)&t};
+  if (cudaLaunchCooperativeKernel((const void*)k_jacobi_resident<KZ, TOL>, grid, block, args, smem, st) != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
@@ -1194,6 +1363,33 @@ int launch_jacobi_block(const unsigned char* mask, const float* div, float* pa, 
   // the shallowest block that fits: more, thinner CTAs spread a small range over more SMs
   const int kz = try_jacobi_block<4>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);
   return kz || !deep ? kz : try_jacobi_block<6>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);
+}
+// The tolerance solve's resident path: the grids launch_jacobi_block takes for the whole-grid solve (3-D, nz >= 4,
+// at most 3 x 2^20 cells), with KZ = 4.
+namespace {
+bool jacobi_tol_resident_shape(const Geo& g) {
+  return g.is3d && g.nz >= 4 && g.n * g.nb <= (3LL << 20) && g.nx % 128 == 0 && g.ny % kJY == 0;
+}
+long long jacobi_residual_ctas(long long n) { return std::min((n + 1023) / 1024, 592LL); }
+}  // namespace
+long long jacobi_tol_slots(const Geo& g) {
+  const long long chunked = jacobi_residual_ctas(g.n) * g.nb;
+  if (!jacobi_tol_resident_shape(g)) return chunked;
+  const long long ctas = (jacobi_block_count(g, 0, g.nz, 4) + kJG - 1) / kJG;
+  return std::max(chunked, 2 * ctas * g.nb);
+}
+bool launch_jacobi_tol_resident(const unsigned char* mask, const float* div, float* p_prev, float* p, const Geo& g,
+                                int max_iter, const JacobiTolArgs& t, cudaStream_t st) {
+  if (!jacobi_tol_resident_shape(g) || !jacobi_aligned(mask, div, p_prev, p) || max_iter < 1) return false;
+  return try_jacobi_block<4, true>(mask, div, p_prev, p, g, 0, g.nz, 0, 0, max_iter, st, t) != 0;
+}
+void launch_jacobi_residual(const float* p, const float* p_prev, const Geo& g, const JacobiTolArgs& t,
+                            cudaStream_t st) {
+  k_jacobi_residual<<<dim3((unsigned)jacobi_residual_ctas(g.n), g.nb), 256, 0, st>>>(p, p_prev, g.n, t);
+}
+void launch_jacobi_copy_back(float* p, const float* p_prev, long long cells, const JacobiState* state,
+                             cudaStream_t st) {
+  k_jacobi_copy_back<<<(unsigned)std::min((cells + 1023) / 1024, 1184LL), 256, 0, st>>>(p, p_prev, cells, state);
 }
 void launch_jacobi_range_sweeps(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,
                                 int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, cudaStream_t st) {

@@ -51,6 +51,9 @@ int tfl_add_gravity(tfl_ctx*, const tfl_grid* U, const tfl_grid* flags, const fl
 int tfl_vorticity_confinement(tfl_ctx*, const tfl_grid* U, const tfl_grid* flags, float strength);
 int tfl_solve_linear_system_jacobi(tfl_ctx*, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
                                    int is_3d, float p_tol, int max_iter, float* residual, int* iterations);
+int tfl_solve_linear_system_jacobi_dev(tfl_ctx*, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
+                                       int is_3d, float p_tol, int max_iter, float* dev_residual,
+                                       int32_t* dev_iterations);
 int tfl_precond_from_string(const char* name);
 int tfl_solve_linear_system_pcg(tfl_ctx*, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
                                 int is_3d, int precond, float tol, int max_iter, float* residual, int* iterations);
@@ -269,6 +272,13 @@ function tfluids.solveLinearSystemJacobi(p, flags, div, is3D, pTol, maxIter, ver
   local res = ffi.new('float[1]')
   check(lib.tfl_solve_linear_system_jacobi(ctx, p.c, flags.c, div.c, is3D and 1 or 0, pTol, maxIter, res, nil))
   return res[0]
+end
+
+-- The same solve with no host wait: the residual (float) and the iteration count (int32) go to the device pointers
+-- residual and iterations (each may be nil, e.g. from tfl_alloc).
+function tfluids.solveLinearSystemJacobiDevice(p, flags, div, is3D, pTol, maxIter, residual, iterations)
+  check(lib.tfl_solve_linear_system_jacobi_dev(ctx, p.c, flags.c, div.c, is3D and 1 or 0, pTol, maxIter,
+                                               ffi.cast('float*', residual), ffi.cast('int32_t*', iterations)))
 end
 
 function tfluids.solveLinearSystemPCG(p, flags, div, is3D, tol, maxIter, precondType, verbose)

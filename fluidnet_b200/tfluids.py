@@ -274,6 +274,27 @@ def solveLinearSystemJacobi(p, flags, div, is3D, pTol=None, maxIter=None, verbos
     return float(res.value)
 
 
+def solveLinearSystemJacobiDevice(p, flags, div, is3D, pTol, maxIter):
+    """solveLinearSystemJacobi with its results left on the device: returns (residual [1] float32, iterations [1]
+    int32) CUDA tensors, written in stream order on torch's current stream.  Does not wait for the device on
+    L2-resident 3-D grids or inside a CUDA graph capture (capture it once the same solve has run outside the
+    capture); other grids outside a capture wait once per chunk of up to 256 sweeps (tfl.h)."""
+    assert p.dim() == 5 and flags.dim() == 5 and div.dim() == 5, 'Dimension mismatch'
+    assert flags.size(1) == 1, 'flags is not scalar'
+    assert p.size() == flags.size(), 'size mismatch'
+    assert div.size() == flags.size(), 'size mismatch'
+    if not is3D:
+        assert flags.size(2) == 1, 'd > 1 for a 2D domain'
+    assert p.is_contiguous() and flags.is_contiguous() and div.is_contiguous()
+    c = _ctx_for(p)
+    residual = torch.empty(1, dtype=torch.float32, device=p.device)
+    iterations = torch.empty(1, dtype=torch.int32, device=p.device)
+    c.check(c.lib.tfl_solve_linear_system_jacobi_dev(c.h, _grid(p), _grid(flags), _grid(div), 1 if is3D else 0,
+                                                     float(pTol), int(maxIter), C.c_void_p(residual.data_ptr()),
+                                                     C.c_void_p(iterations.data_ptr())))
+    return residual, iterations
+
+
 def solveLinearSystemPCG(p, flags, div, is3D, tol=None, maxIter=None, precondType=None, verbose=None):
     """init.lua:645-676 (same argument order and defaults). Returns the max residual across the
     batch elements and connected fluid components."""

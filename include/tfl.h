@@ -124,11 +124,27 @@ int tfl_add_gravity(tfl_ctx* ctx, const tfl_grid* U, const tfl_grid* flags,
 int tfl_vorticity_confinement(tfl_ctx* ctx, const tfl_grid* U, const tfl_grid* flags,
                               float strength);
 /* tfluids.solveLinearSystemJacobi (init.lua:693-734; generic/tfluids.cu:1765-1927).
- * Synchronises once at the end to return the residual (the reference syncs every
- * iteration, generic/tfluids.cu:1886). residual may be NULL (no sync then, if p_tol <= 0). */
+ * p_tol > 0 runs tfl_solve_linear_system_jacobi_dev, then synchronises once, at the end, when residual or
+ * iterations is non-NULL (the reference syncs every iteration, generic/tfluids.cu:1886).  p_tol <= 0 runs max_iter
+ * sweeps and synchronises only when residual or iterations is non-NULL.  A call that reads its result on the host
+ * (p_tol > 0, or a non-NULL residual or iterations) refuses inside a stream capture: capture the _dev entry point. */
 int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags,
                                    const tfl_grid* div, int is_3d, float p_tol, int max_iter,
                                    float* residual, int* iterations);
+/* The same solve with its results left on the device: p, and the float residual and iteration count of the host loop
+ * (dev_residual / dev_iterations, device pointers, each may be NULL), bit for bit those of
+ * tfl_solve_linear_system_jacobi.  The residual's per-entry sums are added in a fixed order, so identical solves give
+ * identical bits.  L2-resident 3-D grids (nx % 128 == 0, ny % 8 == 0, nz >= 4, up to 3 x 2^20 cells) run the whole
+ * solve in one cooperative launch and never wait.  Other grids run a device-driven loop: inside a stream capture it
+ * is one conditional WHILE node and never waits; otherwise the host enqueues chunks of 8, 16, ... 256 sweeps and reads
+ * a device word after each, about log2(iterations / 8) + iterations / 256 waits.  Capturable on a non-default
+ * stream once the solve has run outside the capture on the same grid (the context's scratch arena must not grow in
+ * the capture); the graph then holds pointers into that arena, so replay it only while no larger call on the context
+ * has regrown it.  tfl_launch_count counts a captured solve's loop body once.  Refuses, before enqueueing anything,
+ * on a z-slab context, for max_iter < 1 and for a capture on the default stream. */
+int tfl_solve_linear_system_jacobi_dev(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags, const tfl_grid* div,
+                                       int is_3d, float p_tol, int max_iter, float* dev_residual,
+                                       int32_t* dev_iterations);
 
 /* tfluids.solveLinearSystemPCG (init.lua:645-676; generic/tfluids.cu:1245-1759, CUDA only in the
  * reference: host flood fill + CSR assembly, cuSPARSE ic0/ilu0 + csrsv + csrmv, cuBLAS dots).
