@@ -69,6 +69,7 @@ SYMBOLS = [
     "tfl_slab_sim_exchange_stats", "tfl_slab_sim_ipc_export", "tfl_slab_sim_ipc_connect",
     "tfl_slab_sim_jacobi_stats", "tfl_slab_jacobi_schedule", "tfl_jacobi_slab_block", "tfl_slab_cnn_margin",
     "tfl_slab_graph_create", "tfl_slab_graph_launch", "tfl_slab_graph_destroy",
+    "tfl_slab_sim_set_jacobi_tolerance", "tfl_slab_sim_jacobi_status",
     "tfl_recorder_create", "tfl_recorder_destroy", "tfl_recorder_capture", "tfl_recorder_take", "tfl_recorder_release",
     "tfl_recorder_create_slab", "tfl_recorder_ipc_export", "tfl_recorder_ipc_connect", "tfl_recorder_capture_slab",
     "tfl_monitor_create", "tfl_monitor_destroy", "tfl_monitor_record", "tfl_monitor_take", "tfl_slab_sim_monitor_record",
@@ -195,6 +196,8 @@ def load():
     lib.tfl_slab_graph_destroy.argtypes = [C.c_void_p, C.c_void_p]
     lib.tfl_slab_sim_jacobi_stats.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_int32), C.POINTER(C.c_float),
                                               C.POINTER(C.c_int64)]
+    lib.tfl_slab_sim_set_jacobi_tolerance.argtypes = [C.c_void_p, C.c_void_p, C.c_float]
+    lib.tfl_slab_sim_jacobi_status.argtypes = [C.c_void_p, C.c_void_p, C.POINTER(C.c_float), C.POINTER(C.c_int32)]
     lib.tfl_slab_jacobi_schedule.argtypes = [C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32,
                                              C.POINTER(C.c_int32), C.POINTER(C.c_int32), C.c_int32]
     lib.tfl_slab_cnn_margin.argtypes = [C.c_int32]

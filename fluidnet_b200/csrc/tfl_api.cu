@@ -524,8 +524,8 @@ int jacobi_check_args(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid* flags, co
   if (ctx->slab) return fail(ctx, "Jacobi on a z-slab goes through the multi-GPU driver (halo exchange per sweep)");
   return 0;
 }
+}  // namespace
 
-// Whether the context's stream is being captured into a graph (*capturing), or fails naming `who`.
 int stream_capturing(tfl_ctx* ctx, const char* who, bool* capturing) {
   cudaStream_t st = ctx->stream;
   cudaStreamCaptureStatus cs = cudaStreamCaptureStatusNone;
@@ -540,6 +540,7 @@ int stream_capturing(tfl_ctx* ctx, const char* who, bool* capturing) {
   return 0;
 }
 
+namespace {
 // The chunked path's sweeps of the tolerance solve: sweep k reads pPrev and writes p for even k, the reverse for odd k,
 // and is followed by its residual.  A captured solve's loop body is kJacobiBodySweeps sweeps (even, so every pass
 // starts on the same buffers); a direct one enqueues chunks of 8, 16, ... up to kJacobiMaxChunk sweeps and reads

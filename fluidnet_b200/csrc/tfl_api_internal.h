@@ -202,6 +202,9 @@ inline int fail(tfl_ctx* ctx, const char* fmt, ...) {
     if (e_ != cudaSuccess) return fail(ctx, "%s: %s", #call, cudaGetErrorString(e_));  \
   } while (0)
 
+// Whether the context's stream is being captured into a graph (*capturing), or fails naming `who`.
+int stream_capturing(tfl_ctx* ctx, const char* who, bool* capturing);
+
 inline int check_launch(tfl_ctx* ctx, const char* what) {
   cudaError_t e = cudaGetLastError();
   if (e != cudaSuccess) return fail(ctx, "%s: launch failed: %s", what, cudaGetErrorString(e));

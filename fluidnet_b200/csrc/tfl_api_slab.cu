@@ -75,11 +75,15 @@ NcclApi* nccl_api() {
 //   [2 parities][kMaxRanks]               their counters, carrying the step number
 //   [2 parities][2 from][p_side]          the Jacobi p exchange's messages, parity = p sequence & 1
 //   [64]                                  their counters, [parity][from], carrying the p sequence
+//   [2 parities][r_side] doubles          the Jacobi tolerance solve's per-plane residuals of one block, [sweep][global
+//                                         plane]: every rank stores its owned planes, parity = r sequence & 1
+//   [2 parities][kMaxRanks]               their counters, [parity][rank], carrying the r sequence
 // Alternating parities let a rank push the next all-reduce or p exchange while its peer still reads the current one.
-// The step number and the p sequence live on the device (tfl_slab_sim::seq, SlabSeq), so a replayed step
+// The step number and the p and r sequences live on the device (tfl_slab_sim::seq, SlabSeq), so a replayed step
 // (tfl_slab_graph_launch) advances them exactly as a direct one does.
 struct SlabInbox {
   size_t xbuf_side, p_side;             // floats of one halo message / one p message
+  size_t r_side;                        // doubles of one block's residuals: halo sweeps x gnz planes
   static constexpr int kCounterFloats = 64;
   static constexpr int kSumSlotFloats = 2 * kMaxRanks * 2 * 2;
   static constexpr int kSumFloats = kSumSlotFloats + 2 * kMaxRanks;
@@ -102,7 +106,28 @@ struct SlabInbox {
   __host__ __device__ unsigned int* p_flag(float* inbox, int parity, int from) const {
     return (unsigned int*)(p_area(inbox) + 4 * p_side) + parity * 2 + from;
   }
-  size_t floats() const { return 6 * xbuf_side + kCounterFloats + kSumFloats + 4 * p_side + kCounterFloats; }
+  // behind the p area, at an even float offset (xbuf_side and p_side are multiples of the even halo)
+  __host__ __device__ double* r_buf(float* inbox, int parity) const {
+    return reinterpret_cast<double*>(p_area(inbox) + 4 * p_side + kCounterFloats) + (size_t)parity * r_side;
+  }
+  __host__ __device__ unsigned int* r_flag(float* inbox, int parity, int rank) const {
+    return reinterpret_cast<unsigned int*>(r_buf(inbox, 2)) + parity * kMaxRanks + rank;
+  }
+  size_t floats() const {
+    return 6 * xbuf_side + kCounterFloats + kSumFloats + 4 * p_side + kCounterFloats + 4 * r_side + 2 * kMaxRanks;
+  }
+};
+
+// The z-slab Jacobi tolerance solve's device state (slab_jacobi_tol), zeroed at the start of every solve.
+struct SlabTolState {
+  int done;        // the solve has stopped: every gated kernel and p exchange of the loop returns at once
+  int blk;         // blocks decided so far
+  int iter;        // the iteration counter of the whole-grid loop
+  float res;       // residual of the last sweep run
+  int stop_blk;    // the block of the stopping sweep
+  int rollback;    // the stop fell before the last sweep of its block: p is rebuilt from the block's start
+  int odd;         // the final iterate lies in p2 (an odd count of kept sweeps in the stopping block)
+  int fix;         // the stop fell on the last sweep of a block that leaves p stale below the owned planes
 };
 
 struct tfl_slab_sim {
@@ -125,7 +150,8 @@ struct tfl_slab_sim {
   DevPtr<float*> all_inbox_dev;                // the same table on the device
   DevPtr<unsigned int> push_done;              // CTAs of the running push kernel that finished their stores
   // The exchanges' sequence numbers, two words each (SlabSeq): [0, 2) the step number, which the halo and all-reduce
-  // counters carry, and [2, 4) the p sequence, which the Jacobi p exchanges and tfl_slab_sim_monitor_record advance.
+  // counters carry, [2, 4) the p sequence, which the Jacobi p exchanges and tfl_slab_sim_monitor_record advance, and
+  // [4, 6) the r sequence of the tolerance solve's residual gathers.
   DevPtr<unsigned int> seq;
   bool peer_ok = false;
   unsigned long long peer_gen = 0;             // bumped by every tfl_slab_sim_ipc_connect (the mapped inboxes change)
@@ -149,7 +175,17 @@ struct tfl_slab_sim {
   std::vector<EventPtr> jev;        // [2 * exchange] begin / end of the last step's p exchanges
   int jx = 0;                       // p exchanges of the last step
   size_t jbytes = 0;
-  SlabInbox layout() const { return {xbuf_side, p_side}; }
+  // Jacobi to a tolerance (tfl_slab_sim_set_jacobi_tolerance; slab_jacobi_tol): allocated when a tolerance is first set
+  float p_tol = 0.0f;
+  bool tol_stepped = false;         // a step has run with a tolerance (tfl_slab_sim_jacobi_status)
+  bool tol_last = false;            // the last step ran with one: its p exchange count comes from tol_state
+  std::vector<int> tol_widths;      // width of the p exchange before each block of the last step's solve (0: none)
+  DevPtr<float> p_save;             // p at the start of the running block, ghost planes included
+  DevPtr<double> tol_slots;         // [halo sweeps][owned planes][tiles] per-tile residuals of the running block
+  DevPtr<double> tol_send, tol_recv;   // [halo sweeps][gnz] per-plane residuals: this rank's planes / every rank's
+  DevPtr<SlabTolState> tol_state;
+  DevPtr<int> tol_rerun;            // [halo]: 0 for each sweep of the stopping block that runs again
+  SlabInbox layout() const { return {xbuf_side, p_side, (size_t)halo * gnz}; }
 };
 
 int ipc_export(tfl_ctx* ctx, void* dev, char* out, size_t bytes) {
@@ -269,7 +305,7 @@ int tfl_slab_sim_create(tfl_ctx* ctx, int32_t gnz, int32_t ny, int32_t nx, int32
     return fail(ctx, kFailed);
   if (s->world > 1 &&
       (!(s->inbox = dev_zeros<float>(s->layout().floats())) ||
-       !(s->push_done = dev_zeros<unsigned int>(1)) || !(s->seq = dev_zeros<unsigned int>(4))))
+       !(s->push_done = dev_zeros<unsigned int>(1)) || !(s->seq = dev_zeros<unsigned int>(6))))
     return fail(ctx, kFailed);
   for (auto& pr : s->ev)
     for (EventPtr& e : pr)
@@ -366,14 +402,19 @@ __global__ void k_slab_pack(SlabPack d) {
 // Every CTA reads the word the kernel does not write and writes the same value, so neither kernel races with itself,
 // and stream order carries the number from push to pull and on to the next exchange.  The message and counter of
 // parity 1 lie buf_stride floats / flag_stride words past parity 0's (both 0 for the halos' single slot).
+// gate (the tolerance solve's p exchanges): unless null, the exchange runs only while *gate == run_if; otherwise both
+// kernels return at once on every rank alike and leave the words as they are.
 struct SlabSeq {
   unsigned int* word;
   unsigned int advance;
   long long buf_stride;
   int flag_stride;
+  const int* gate = nullptr;
+  int run_if = 0;
   template <typename T> __device__ __forceinline__ T* at(T* p0, unsigned int seq, long long stride) const {
     return p0 ? p0 + (seq & 1u) * stride : nullptr;
   }
+  __device__ __forceinline__ bool skipped() const { return gate && __ldcg(gate) != run_if; }
 };
 
 // Peer-memory exchange, sending half: every channel's boundary planes are written straight into the neighbours'
@@ -381,6 +422,7 @@ struct SlabSeq {
 // The buffers and counters are given for parity 0.
 __global__ void k_slab_push(SlabPack d, float* peer_lo_buf, float* peer_hi_buf, unsigned int* peer_lo_flag,
                             unsigned int* peer_hi_flag, SlabSeq q, unsigned int* done) {
+  if (q.skipped()) return;
   const unsigned int seq = q.word[0] + q.advance;
   if (threadIdx.x == 0) q.word[1] = seq;
   d.gather(q.at(peer_lo_buf, seq, q.buf_stride), q.at(peer_hi_buf, seq, q.buf_stride));
@@ -392,6 +434,7 @@ __global__ void k_slab_push(SlabPack d, float* peer_lo_buf, float* peer_hi_buf, 
 __global__ void k_slab_pull(SlabPack d, const float* buf_lo, const float* buf_hi, const unsigned int* flag_lo,
                             const unsigned int* flag_hi, SlabSeq q, unsigned long long* faults) {
   __shared__ int ok;
+  if (q.skipped()) return;
   const unsigned int seq = q.word[1];
   if (threadIdx.x == 0) {
     q.word[0] = seq;
@@ -448,6 +491,100 @@ __global__ void k_sum_pull(double* __restrict__ out, float* inbox, SlabInbox box
   }
 }
 
+// ---- Jacobi to a tolerance on z-slabs (slab_jacobi_tol) ----
+// dst <- src (n floats) while *gate == run_if.
+__global__ void k_slab_gated_copy(float* __restrict__ dst, const float* __restrict__ src, long long n, const int* gate,
+                                  int run_if) {
+  if (__ldcg(gate) != run_if) return;
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    dst[i] = src[i];
+}
+
+// Gather, sending half: the block's per-tile residuals (k sweeps x nown owned planes x `tiles`) added tile by tile into
+// one double per sweep and plane, stored at [sweep][z0 + plane] of `local` (one rank, NCCL) or of the r area of every
+// rank's inbox (peer memory: then every rank's counter [parity][rank] takes the r sequence's next number).
+__global__ void k_tol_push(const double* __restrict__ slots, int k, int nown, int tiles, int z0, int gnz,
+                           double* local, float* const* __restrict__ inboxes, SlabInbox box, int rank, int world,
+                           unsigned int* rword, const int* done) {
+  if (__ldcg(done)) return;
+  const unsigned int seq = inboxes ? rword[0] + 1 : 0u;
+  if (inboxes && threadIdx.x == 0) rword[1] = seq;
+  for (int e = threadIdx.x; e < k * nown; e += blockDim.x) {
+    const int sw = e / nown;
+    const double* sl = slots + (size_t)e * tiles;
+    double v = 0.0;
+    for (int t = 0; t < tiles; t++) v += sl[t];
+    const size_t at = (size_t)sw * gnz + z0 + (e - sw * nown);
+    if (!inboxes) local[at] = v;
+    else for (int r = 0; r < world; r++) box.r_buf(inboxes[r], seq & 1)[at] = v;
+  }
+  if (!inboxes) return;
+  __threadfence_system();
+  __syncthreads();
+  if ((int)threadIdx.x < world) store_release_sys(box.r_flag(inboxes[threadIdx.x], seq & 1, rank), seq);
+}
+
+// Gather, receiving half, and the stop decision of one block of k sweeps: wait for every rank's residuals (peer
+// memory), add the planes of each sweep in ascending global z from zero, then apply the whole-grid loop's test in
+// sweep order to global sweep blk * kb + s.  Every rank adds the same doubles in the same order and so decides alike.
+// A stop records where p is (SlabTolState) and arms the rerun of the kept sweeps when it fell inside the block.  In a
+// graph the WHILE node over the middle blocks runs again while the solve goes on and a middle block is left.
+__global__ void k_tol_decide(const double* local, float* inbox, SlabInbox box, int world, unsigned int* rword,
+                             SlabTolState* st, int* rerun, float tol, int max_iter, int kb, int k, int nblk,
+                             int fix_at_end, int gnz, cudaGraphConditionalHandle loop, int has_loop,
+                             unsigned long long* faults) {
+  extern __shared__ double res2[];
+  __shared__ int ok;
+  if (__ldcg(&st->done)) return;
+  const int t = threadIdx.x;
+  const volatile double* vec = local;
+  if (inbox) {
+    const unsigned int seq = rword[1];
+    if (t == 0) ok = 1;
+    __syncthreads();
+    if (t == 0) rword[0] = seq;
+    if (t < world && !wait_seq(box.r_flag(inbox, seq & 1, t), seq, clock64(), 100)) ok = 0;
+    __syncthreads();
+    if (!ok) {                       // a rank that never arrived: stop here, counted as a fault
+      if (t == 0) {
+        if (faults) atomicAdd(faults, 1ULL);
+        st->done = 1;
+        if (has_loop) cudaGraphSetConditional(loop, 0u);
+      }
+      return;
+    }
+    vec = box.r_buf(inbox, seq & 1);
+  }
+  for (int sw = t; sw < k; sw += blockDim.x) {
+    double v = 0.0;
+    for (int z = 0; z < gnz; z++) v += vec[(size_t)sw * gnz + z];
+    res2[sw] = v;
+  }
+  __syncthreads();
+  if (t != 0) return;
+  const int b = st->blk;
+  int stop = -1, iter = 0;
+  float res = 0.0f;
+  for (int sw = 0; sw < k && stop < 0; sw++) {
+    res = (float)sqrt(res2[sw]);
+    if (jacobi_stops(res, tol, b * kb + sw, max_iter, &iter)) stop = sw;
+  }
+  st->iter = iter;
+  st->res = res;
+  st->blk = b + 1;
+  if (stop >= 0) {
+    const int keep = stop + 1;
+    st->stop_blk = b;
+    st->rollback = keep < k;
+    st->odd = keep & 1;
+    st->fix = fix_at_end && keep == k;
+    if (keep < k)
+      for (int i = 0; i < keep; i++) rerun[i] = 0;
+    st->done = 1;
+  }
+  if (has_loop) cudaGraphSetConditional(loop, stop < 0 && b + 1 < nblk - 1 ? 1u : 0u);
+}
+
 // The Jacobi p exchange: several per step, so its inbox slots alternate with the parity of a sequence number (a rank
 // may push exchange e + 1 while its neighbour still scatters exchange e; it cannot push e + 2 before the neighbour
 // has pushed e + 1, which that neighbour does after scattering e).
@@ -461,15 +598,19 @@ int slab_event(tfl_ctx* ctx, const tfl_slab_sim* s, const EventPtr& e) {
 }
 
 // Refresh `width` ghost planes on both sides of the listed fields from the neighbours' owned planes.
-int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl_grid*> fields, int width, int phase) {
-  const bool pph = phase == kPhaseP;
+// gate / run_if (p exchanges of the tolerance solve, SlabSeq): the peer-memory kernels run only while *gate == run_if;
+// such an exchange records no events and is not counted here (tfl_slab_sim_jacobi_stats counts it from the device).
+// NCCL exchanges cannot be gated: the caller enqueues them only when they run.
+int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl_grid*> fields, int width, int phase,
+                  const int* gate = nullptr, int run_if = 0) {
+  const bool pph = phase == kPhaseP, counted = !gate;
   if (!pph) {
     if (slab_event(ctx, s, s->ev[phase][0])) return 1;
     s->bytes_sent[phase] = 0;
   }
   if (s->world > 1 && width > 0 && (ctx->comm || s->peer_ok)) {
     if (width > s->halo) return fail(ctx, "slab exchange of %d planes exceeds the halo (%d)", width, s->halo);
-    if (pph) {
+    if (pph && counted) {
       while ((int)s->jev.size() < 2 * (s->jx + 1)) {
         cudaEvent_t e = nullptr;
         TFL_CUDA(ctx, cudaEventCreate(&e));
@@ -494,7 +635,7 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
     if (s->peer_ok) {
       const SlabInbox box = s->layout();
       // the step's first halo exchange takes the next step number, every p exchange the next p sequence number
-      const SlabSeq q = pph ? SlabSeq{s->seq.get() + 2, 1u, 2 * (long long)s->p_side, 2}
+      const SlabSeq q = pph ? SlabSeq{s->seq.get() + 2, 1u, 2 * (long long)s->p_side, 2, gate, run_if}
                             : SlabSeq{s->seq.get(), phase == 0 ? 1u : 0u, 0, 0};
       auto buf = [&](float* base, int from) { return pph ? box.p_buf(base, 0, from) : box.halo(base, phase, from); };
       auto flag = [&](float* base, int from) { return pph ? box.p_flag(base, 0, from) : box.halo_flag(base, phase, from); };
@@ -533,6 +674,7 @@ int slab_exchange(tfl_ctx* ctx, tfl_slab_sim* s, std::initializer_list<const tfl
       ctx->launches += 2;
     }
     if (pph) {
+      if (!counted) return 0;
       if (slab_event(ctx, s, s->jev[2 * s->jx + 1])) return 1;
       s->jx += 1;
       s->jbytes += sent;
@@ -570,9 +712,146 @@ int run_jacobi_block(tfl_ctx* ctx, const unsigned char* mask, const float* div, 
   return 0;
 }
 
-// lib/simulate.lua:275-303 with pTol = 0 on this rank's slab: divergence, `iters` Jacobi sweeps from p = 0 in the
-// blocks of tfl_slab_jacobi_schedule, velocity update on the owned planes.  Every cell sees the single-GPU sweep's
-// operands, so p and U are bit-identical to tfl_simulate_step's.
+// The Jacobi solve to s->p_tol on this rank's slab, from p = p2 = 0 on a prepared divergence and mask (`planes` and `g`
+// of slab_jacobi_projection); leaves the whole-grid loop's final iterate in p on the owned planes and the plane below.
+// Blocks of `halo` sweeps (the schedule's at world > 1, without its closing 1-plane exchange; at one rank the same
+// lengths over the whole slab), each one:
+//   p exchange (gated on done)  ->  p_save <- p  ->  per sweep: the gated sweep and its per-plane residual
+//   ->  k_tol_push (+ the NCCL all-reduce)  ->  k_tol_decide
+// Every block starts on p (halo is even).  A direct step enqueues 1, 2, 4 .. 32 blocks at a time and reads done after
+// each chunk (one block at a time over NCCL, whose exchanges cannot be gated); a captured one is block 0, one WHILE
+// node over the middle blocks and the last block.  Then, gated by the decision: p <- p_save and the stopping block's
+// kept sweeps again (on the widest block range, which keeps the owned planes and the plane below right for every
+// block), p <- p2 when the result lies there, and the 1-plane p exchange when the stop left p stale below the owned
+// planes.
+int slab_jacobi_tol(tfl_ctx* ctx, tfl_slab_sim* s, int iters, const int32_t planes[3], const Geo& g) {
+  struct Blk { int k, w, z_lo, z_hi, shr_lo, shr_hi, fix_at_end; };
+  std::vector<Blk> blocks;
+  const int kb = s->halo;
+  if (s->world == 1) {
+    for (int b0 = 0; b0 < iters; b0 += kb) blocks.push_back({std::min(kb, iters - b0), 0, 0, s->nz, 0, 0, 0});
+  } else {
+    const int nsched = (int)(s->jsched.size() / TFL_JACOBI_BLOCK_INTS);
+    for (int b = 0; b < nsched; b++) {
+      const int32_t* o = s->jsched.data() + (size_t)b * TFL_JACOBI_BLOCK_INTS;
+      if (o[0] > 0) blocks.push_back({o[0], o[1], o[2], o[3], o[4], o[5], b + 1 < nsched ? 1 : 0});
+    }
+  }
+  const int nblk = (int)blocks.size();
+  s->tol_widths.clear();
+  int kmax = 0;
+  for (const Blk& o : blocks) {
+    s->tol_widths.push_back(o.w);
+    kmax = std::max(kmax, o.k);
+  }
+  const tfl_state& st = s->st;
+  float* p = st.p.data;
+  float* p2 = s->p2.get();
+  const unsigned char* mask = s->mask.get();
+  const float* div = s->div.get();
+  SlabTolState* S = s->tol_state.get();
+  const int* done = &S->done;
+  const int nown = s->z1 - s->z0, tiles = jacobi_plane_tiles(s->nx, s->ny);
+  const bool peer = s->world > 1 && s->peer_ok && s->all_inbox_dev, nccl = s->world > 1 && !peer && ctx->comm;
+  const unsigned copy_blocks = (unsigned)std::min<size_t>((s->cells + 1023) / 1024, 1184);
+  const SlabInbox box = s->layout();
+  TFL_CUDA(ctx, cudaMemsetAsync(S, 0, sizeof(SlabTolState), ctx->stream));
+  TFL_CUDA(ctx, cudaMemsetAsync(s->tol_rerun.get(), 1, sizeof(int) * kb, ctx->stream));     // nonzero: skipped
+  auto block = [&](const Blk& o, cudaGraphConditionalHandle loop, int has_loop) -> int {
+    cudaStream_t q = ctx->stream;
+    if (o.w > 0 && slab_exchange(ctx, s, {&st.p}, o.w, kPhaseP, done, 0)) return 1;
+    // where the fixed count takes the cooperative block kernel, so does the tolerance: one launch that also saves the
+    // block's start and leaves the per-plane residuals; elsewhere the copy, then a sweep and a residual pass per sweep
+    JacobiTolArgs t;
+    t.slots = s->tol_slots.get();
+    t.gate = done;
+    t.save = s->p_save.get();
+    t.own_lo = s->own_lo;
+    t.own_hi = s->own_hi;
+    if (launch_jacobi_block_planes(mask, div, p, p2, g, o.z_lo, o.z_hi, o.shr_lo, o.shr_hi, o.k, t, q)) {
+      ctx->launches += 1;
+    } else {
+      k_slab_gated_copy<<<copy_blocks, 256, 0, q>>>(s->p_save.get(), p, (long long)s->cells, done, 0);
+      for (int sw = 0; sw < o.k; sw++) {
+        Geo gs = g;
+        gs.zlo = o.z_lo + sw * o.shr_lo;
+        gs.zhi = o.z_hi - sw * o.shr_hi;
+        float* prev = (sw & 1) ? p2 : p;
+        float* cur = (sw & 1) ? p : p2;
+        launch_jacobi_iter(mask, div, prev, cur, gs, q, done);
+        launch_jacobi_plane_residual(cur, prev, s->nx, s->ny, s->own_lo, nown,
+                                     s->tol_slots.get() + (size_t)sw * nown * tiles, done, q);
+      }
+      ctx->launches += 2 * o.k + 1;
+    }
+    k_tol_push<<<1, 256, 0, q>>>(s->tol_slots.get(), o.k, nown, tiles, s->z0, s->gnz, s->tol_send.get(),
+                                 peer ? s->all_inbox_dev.get() : nullptr, box, s->rank, s->world, s->seq.get() + 4, done);
+    if (nccl)
+      TFL_NCCL(ctx, nccl_api()->AllReduce(s->tol_send.get(), s->tol_recv.get(), (size_t)kb * s->gnz, ncclDouble,
+                                          ncclSum, ctx->comm, q));
+    k_tol_decide<<<1, 256, sizeof(double) * kb, q>>>(nccl ? s->tol_recv.get() : s->tol_send.get(),
+                                                      peer ? s->inbox.get() : nullptr, box, s->world, s->seq.get() + 4,
+                                                      S, s->tol_rerun.get(), s->p_tol, iters, kb, o.k, nblk,
+                                                      o.fix_at_end, s->gnz, loop, has_loop, ctx->counters.get());
+    ctx->launches += 2;
+    return 0;
+  };
+  if (s->capturing) {
+    const int has_loop = nblk >= 3;             // the middle blocks are alike: the WHILE node's body is one of them
+    cudaGraphConditionalHandle loop = 0;
+    if (has_loop) TFL_CUDA(ctx, capture_while_handle(ctx->stream, 0, &loop));
+    if (block(blocks[0], loop, has_loop)) return 1;
+    if (has_loop) {
+      cudaStream_t main = ctx->stream, bs = ctx->jacobi_body.get();
+      TFL_CUDA(ctx, capture_while_body(main, loop, bs));
+      ctx->stream = bs;
+      const int rc = block(blocks[1], loop, 1);
+      ctx->stream = main;
+      const cudaError_t le = cudaGetLastError();
+      cudaGraph_t body = nullptr;
+      const cudaError_t ee = cudaStreamEndCapture(bs, &body);      // ends the body's capture on every path
+      if (rc) return 1;
+      TFL_CUDA(ctx, le);
+      TFL_CUDA(ctx, ee);
+    }
+    if (nblk >= 2 && block(blocks[nblk - 1], loop, has_loop)) return 1;
+  } else {
+    if (!ctx->jacobi_host && !(ctx->jacobi_host = pinned_alloc<int>(1))) return fail(ctx, "slab_sim_step: cudaMallocHost failed");
+    int b = 0;
+    for (int chunk = 1; b < nblk; chunk = std::min(2 * chunk, 32)) {
+      for (int i = 0; i < (nccl ? 1 : chunk) && b < nblk; i++, b++)
+        if (block(blocks[b], 0, 0)) return 1;
+      if (b >= nblk) break;                     // the last block's decision stops the solve
+      TFL_CUDA(ctx, cudaMemcpyAsync(ctx->jacobi_host.get(), done, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
+      TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+      if (*ctx->jacobi_host) break;
+    }
+  }
+  // the stopping block again from its start, up to its stopping sweep
+  k_slab_gated_copy<<<copy_blocks, 256, 0, ctx->stream>>>(p, s->p_save.get(), (long long)s->cells, &S->rollback, 1);
+  const int lo = s->rank > 0, hi = s->rank < s->world - 1;
+  for (int sw = 0; sw + 1 < kmax; sw++) {
+    Geo gs = g;
+    gs.zlo = planes[0] + sw * lo;
+    gs.zhi = planes[1] - sw * hi;
+    launch_jacobi_iter(mask, div, (sw & 1) ? p2 : p, (sw & 1) ? p : p2, gs, ctx->stream, s->tol_rerun.get() + sw);
+  }
+  k_slab_gated_copy<<<copy_blocks, 256, 0, ctx->stream>>>(p, p2, (long long)s->cells, &S->odd, 1);
+  ctx->launches += kmax + 1;
+  if (peer) return slab_exchange(ctx, s, {&st.p}, 1, kPhaseP, &S->fix, 1);
+  if (nccl) {                                   // direct only (NCCL is not captured): the host learns the stop
+    SlabTolState h;
+    TFL_CUDA(ctx, cudaMemcpyAsync(&h, S, sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+    TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+    if (h.fix) return slab_exchange(ctx, s, {&st.p}, 1, kPhaseP, &S->fix, 1);
+  }
+  return 0;
+}
+
+// lib/simulate.lua:275-303 on this rank's slab: divergence, `iters` Jacobi sweeps from p = 0 in the blocks of
+// tfl_slab_jacobi_schedule, velocity update on the owned planes.  Every cell sees the single-GPU sweep's operands, so
+// with pTol = 0 p and U are bit-identical to tfl_simulate_step's; with a tolerance (slab_jacobi_tol) they are those of
+// the whole-grid operators with tfl_solve_linear_system_jacobi_dev as the solve.
 int slab_jacobi_projection(tfl_ctx* ctx, tfl_slab_sim* s, int iters) {
   const tfl_state& st = s->st;
   int32_t planes[3];
@@ -594,22 +873,27 @@ int slab_jacobi_projection(tfl_ctx* ctx, tfl_slab_sim* s, int iters) {
   }
   TFL_CUDA(ctx, cudaMemsetAsync(st.p.data, 0, s->cells * 4, ctx->stream));   // generic/tfluids.cu:1854-1855
   TFL_CUDA(ctx, cudaMemsetAsync(s->p2.get(), 0, s->cells * 4, ctx->stream));
-  float* buf[2] = {st.p.data, s->p2.get()};
-  int done = 0;
   s->jx = 0;
   s->jbytes = 0;
-  for (int b = 0; b < nblk; b++) {
-    const int32_t* o = s->jsched.data() + (size_t)b * TFL_JACOBI_BLOCK_INTS;
-    if (o[1] > 0) {
-      tfl_grid pc = st.p;
-      pc.data = buf[done & 1];
-      if (slab_exchange(ctx, s, {&pc}, o[1], kPhaseP)) return 1;
+  s->tol_last = s->p_tol > 0.0f;
+  if (s->tol_last) {
+    if (slab_jacobi_tol(ctx, s, iters, planes, g)) return 1;
+  } else {
+    float* buf[2] = {st.p.data, s->p2.get()};
+    int done = 0;
+    for (int b = 0; b < nblk; b++) {
+      const int32_t* o = s->jsched.data() + (size_t)b * TFL_JACOBI_BLOCK_INTS;
+      if (o[1] > 0) {
+        tfl_grid pc = st.p;
+        pc.data = buf[done & 1];
+        if (slab_exchange(ctx, s, {&pc}, o[1], kPhaseP)) return 1;
+      }
+      if (run_jacobi_block(ctx, s->mask.get(), s->div.get(), buf[done & 1], buf[(done + 1) & 1], g, o[2], o[3], o[4], o[5], o[0], -1) < 0)
+        return 1;
+      done += o[0];
     }
-    if (run_jacobi_block(ctx, s->mask.get(), s->div.get(), buf[done & 1], buf[(done + 1) & 1], g, o[2], o[3], o[4], o[5], o[0], -1) < 0)
-      return 1;
-    done += o[0];
+    if (done & 1) TFL_CUDA(ctx, cudaMemcpyAsync(st.p.data, s->p2.get(), s->cells * 4, cudaMemcpyDeviceToDevice, ctx->stream));
   }
-  if (done & 1) TFL_CUDA(ctx, cudaMemcpyAsync(st.p.data, s->p2.get(), s->cells * 4, cudaMemcpyDeviceToDevice, ctx->stream));
   if (check_launch(ctx, "slab_sim_step (jacobi)")) return 1;
   SlabScope scope(ctx, s, s->own_lo, s->own_hi);
   return tfl_velocity_update_forward(ctx, &st.U, &st.flags, &st.p);
@@ -719,6 +1003,13 @@ int slab_step_refusal(tfl_ctx* ctx, const tfl_slab_sim* s, const tfl_mconf* mc, 
     return fail(ctx, "%s: %s", who, ctx->err.c_str());
   if (jacobi && mc->max_iter < 0) return fail(ctx, "%s: At least 1 iteration is needed (maxIter < 1)", who);
   if (s->world != ctx->comm_world || s->rank != ctx->comm_rank) return fail(ctx, "%s: communicator changed", who);
+  if (jacobi && s->p_tol > 0.0f) {        // the direct tolerance step reads its stop word on the host
+    bool capturing = false;
+    if (stream_capturing(ctx, who, &capturing)) return 1;
+    if (capturing)
+      return fail(ctx, "%s: the stream is being captured and a step with a Jacobi tolerance waits for its stop decision "
+                       "on the host; capture it with tfl_slab_graph_create instead", who);
+  }
   return 0;
 }
 
@@ -815,6 +1106,9 @@ struct tfl_slab_graph {
   size_t bytes_sent[3] = {0, 0, 0};
   int jx = 0;
   size_t jbytes = 0;
+  bool jacobi = false;
+  bool tol = false;                 // the captured step solves to a tolerance: its statistics come from the device
+  std::vector<int> tol_widths;
 };
 
 extern "C" {
@@ -824,6 +1118,7 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tfl_cn
   DeviceGuard guard_(ctx);
   NvtxRange range_(__func__);
   if (slab_step_refusal(ctx, s, mc, cnn, "slab_sim_step") || slab_step(ctx, s, mc, cnn)) return 1;
+  if (mc->sim_method == TFL_SIM_JACOBI && s->tol_last) s->tol_stepped = true;
   s->last.done = true;
   s->last.cnn = mc->sim_method == TFL_SIM_JACOBI ? nullptr : cnn;
   s->last.sim_method = mc->sim_method;
@@ -862,6 +1157,8 @@ int tfl_slab_graph_create(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tf
   memcpy(bytes_sent, s->bytes_sent, sizeof(bytes_sent));
   const int jx = s->jx;
   const size_t jbytes = s->jbytes;
+  const bool tol_last = s->tol_last;
+  const std::vector<int> tol_widths = s->tol_widths;
   if (cudaStreamBeginCapture(st, cudaStreamCaptureModeRelaxed) != cudaSuccess) {
     cudaGetLastError();
     return fail(ctx, "slab_graph: cudaStreamBeginCapture failed");
@@ -877,9 +1174,14 @@ int tfl_slab_graph_create(tfl_ctx* ctx, tfl_slab_sim* s, const tfl_mconf* mc, tf
   memcpy(g->bytes_sent, s->bytes_sent, sizeof(bytes_sent));
   g->jx = s->jx;
   g->jbytes = s->jbytes;
+  g->jacobi = mc->sim_method == TFL_SIM_JACOBI;
+  g->tol = g->jacobi && s->tol_last;
+  g->tol_widths = s->tol_widths;
   memcpy(s->bytes_sent, bytes_sent, sizeof(bytes_sent));
   s->jx = jx;
   s->jbytes = jbytes;
+  s->tol_last = tol_last;
+  s->tol_widths = tol_widths;
   if (rc != 0 || e != cudaSuccess || !graph) {
     cudaGetLastError();
     const std::string why = rc != 0 ? ctx->err : std::string(cudaGetErrorString(e));
@@ -914,6 +1216,11 @@ int tfl_slab_graph_launch(tfl_ctx* ctx, tfl_slab_graph* g) {
   memcpy(s->bytes_sent, g->bytes_sent, sizeof(s->bytes_sent));
   s->jx = g->jx;
   s->jbytes = g->jbytes;
+  if (g->jacobi) s->tol_last = g->tol;
+  if (g->tol) {
+    s->tol_stepped = true;
+    s->tol_widths = g->tol_widths;
+  }
   return 0;
 }
 
@@ -1019,6 +1326,20 @@ int tfl_slab_sim_jacobi_stats(tfl_ctx* ctx, tfl_slab_sim* s, int32_t* exchanges,
   NvtxRange range_(__func__);
   if (!s) return fail(ctx, "slab_sim is nil");
   TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (s->tol_last) {      // the exchanges before the stopping block's and the 1-plane one; not timed inside the loop
+    SlabTolState h;
+    TFL_CUDA(ctx, cudaMemcpy(&h, s->tol_state.get(), sizeof(h), cudaMemcpyDeviceToHost));
+    int n = 0;
+    size_t planes = 0;
+    const bool moved = s->world > 1 && (s->peer_ok || ctx->comm);
+    for (int b = 0; moved && b <= h.stop_blk && b < (int)s->tol_widths.size(); b++)
+      if (s->tol_widths[b] > 0) { n++; planes += s->tol_widths[b]; }
+    if (moved && h.fix) { n++; planes += 1; }
+    if (exchanges) *exchanges = n;
+    if (ms) *ms = -1.0f;
+    if (bytes) *bytes = (int64_t)(planes * s->plane * 4 * ((s->rank > 0) + (s->rank < s->world - 1)));
+    return 0;
+  }
   float total = 0.0f;
   for (int i = 0; i < s->jx; i++) {
     float t = 0.0f;
@@ -1028,6 +1349,54 @@ int tfl_slab_sim_jacobi_stats(tfl_ctx* ctx, tfl_slab_sim* s, int32_t* exchanges,
   if (exchanges) *exchanges = s->jx;
   if (ms) *ms = total;
   if (bytes) *bytes = (int64_t)s->jbytes;
+  return 0;
+}
+
+int tfl_slab_sim_set_jacobi_tolerance(tfl_ctx* ctx, tfl_slab_sim* s, float p_tol) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!ctx) return 1;
+  if (!s) return fail(ctx, "slab_sim_set_jacobi_tolerance: nil argument");
+  if (!(p_tol >= 0.0f)) return fail(ctx, "slab_sim_set_jacobi_tolerance: pTol must be >= 0 (got %g)", p_tol);
+  if (p_tol > 0.0f && !s->p_save) {             // allocated here, so that no step (and no capture) allocates
+    bool capturing = false;
+    if (stream_capturing(ctx, "slab_sim_set_jacobi_tolerance", &capturing)) return 1;
+    if (capturing)
+      return fail(ctx, "slab_sim_set_jacobi_tolerance: the stream is being captured; set the tolerance before capturing");
+    const size_t nown = (size_t)(s->z1 - s->z0), tiles = (size_t)jacobi_plane_tiles(s->nx, s->ny);
+    const size_t per_block = (size_t)s->halo * s->gnz;
+    if (!(s->p_save = dev_zeros<float>(s->cells)) || !(s->tol_slots = dev_zeros<double>(s->halo * nown * tiles)) ||
+        !(s->tol_send = dev_zeros<double>(per_block)) || !(s->tol_recv = dev_zeros<double>(per_block)) ||
+        !(s->tol_state = dev_zeros<SlabTolState>(1)) || !(s->tol_rerun = dev_zeros<int>(s->halo))) {
+      s->p_save.reset();
+      return fail(ctx, "slab_sim_set_jacobi_tolerance: allocation failed");
+    }
+  }
+  s->p_tol = p_tol;
+  return 0;
+}
+
+int tfl_slab_sim_jacobi_status(tfl_ctx* ctx, tfl_slab_sim* s, float* residual, int32_t* iterations) {
+  DeviceGuard guard_(ctx);
+  NvtxRange range_(__func__);
+  if (!ctx) return 1;
+  if (!s) return fail(ctx, "slab_sim_jacobi_status: nil argument");
+  if (!s->tol_stepped)
+    return fail(ctx, "slab_sim_jacobi_status: no step has solved to a Jacobi tolerance yet "
+                     "(tfl_slab_sim_set_jacobi_tolerance, then a 'jacobi' step)");
+  if (!s->tol_last)
+    return fail(ctx, "slab_sim_jacobi_status: the last 'jacobi' step ran the fixed count (pTol 0): it has no residual "
+                     "or iteration count of its own");
+  bool capturing = false;
+  if (stream_capturing(ctx, "slab_sim_jacobi_status", &capturing)) return 1;
+  if (capturing)
+    return fail(ctx, "slab_sim_jacobi_status: the stream is being captured and this call waits for the device; read "
+                     "the status after the graph's launch");
+  SlabTolState h;
+  TFL_CUDA(ctx, cudaMemcpyAsync(&h, s->tol_state.get(), sizeof(h), cudaMemcpyDeviceToHost, ctx->stream));
+  TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
+  if (residual) *residual = h.res;
+  if (iterations) *iterations = h.iter;
   return 0;
 }
 

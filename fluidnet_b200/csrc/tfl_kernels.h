@@ -68,6 +68,16 @@ struct JacobiState {
   int last;            // index of the last sweep run: it wrote p when even, pPrev when odd
   float res;           // residual of the last sweep
 };
+// The host loop's test after sweep s (0-based) with residual res: stop when res < tol, before the counter counts the
+// sweep, or once the counter reaches max_iter.  *iter receives the counter.
+__device__ __forceinline__ bool jacobi_stops(float res, float tol, int s, int max_iter, int* iter) {
+  if (res < tol) {
+    *iter = s;
+    return true;
+  }
+  *iter = s + 1;
+  return s + 1 >= max_iter;
+}
 struct JacobiTolArgs {
   double* slots = nullptr;          // per-CTA partial sums of (p - pPrev)^2 per batch entry (jacobi_tol_slots doubles)
   JacobiState* state = nullptr;     // zeroed before the first sweep
@@ -77,6 +87,11 @@ struct JacobiTolArgs {
   int max_iter = 0;
   cudaGraphConditionalHandle loop = 0;   // the WHILE node of a captured solve (has_loop): cleared when it stops
   int has_loop = 0;
+  // launch_jacobi_block_planes (the z-slab tolerance solve): slots receive the per-plane residuals, save the block's
+  // start; nothing runs while *gate is set
+  const int* gate = nullptr;
+  float* save = nullptr;
+  int own_lo = 0, own_hi = 0;
 };
 // Doubles of JacobiTolArgs::slots either path below needs on grid g.
 long long jacobi_tol_slots(const Geo& g);
@@ -89,6 +104,18 @@ bool launch_jacobi_tol_resident(const unsigned char* mask, const float* div, flo
 // launch; once the loop has stopped, the copy back moves the result into p when it ended in p_prev.
 void launch_jacobi_residual(const float* p, const float* p_prev, const Geo& g, const JacobiTolArgs& t, cudaStream_t st);
 void launch_jacobi_copy_back(float* p, const float* p_prev, long long cells, const JacobiState* state, cudaStream_t st);
+// One block of the z-slab tolerance solve in one cooperative launch (k_jacobi_resident_planes<4>): the sweeps of
+// launch_jacobi_block with 4-plane blocks, plus t.save <- pa on [z_lo, z_hi) first and, per sweep, the owned planes'
+// residuals in t.slots[sweep][plane][tile] with launch_jacobi_plane_residual's bits.  Returns 4, or 0 (nothing
+// launched) where launch_jacobi_block would return 0 without `deep`.
+int launch_jacobi_block_planes(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo,
+                               int z_hi, int shr_lo, int shr_hi, int sweeps, const JacobiTolArgs& t, cudaStream_t st);
+// The z-slab tolerance solve's per-plane residual of one sweep (one batch entry): slots[plane][tile] receives the sum
+// of (cur - prev)^2 over each 128 x 8 tile of local planes [z_lo, z_lo + planes), jacobi_plane_tiles(nx, ny) tiles per
+// plane, in an order fixed by nx and ny alone.  Does nothing once *done is set.
+int jacobi_plane_tiles(int nx, int ny);
+void launch_jacobi_plane_residual(const float* cur, const float* prev, int nx, int ny, int z_lo, int planes,
+                                  double* slots, const int* done, cudaStream_t st);
 // changed: optional device word that is OR-ed with 1 when a byte differs from what `o` held before.
 void launch_flags_to_u8(const float* f, unsigned char* o, long long n, int* changed, cudaStream_t st);
 void launch_apply_bc(float* x, const float* inv, const float* bc, long long n, cudaStream_t st);

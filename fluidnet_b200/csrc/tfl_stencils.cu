@@ -850,16 +850,6 @@ __device__ __forceinline__ double warp_fixed_sum(const double* slots, int n, int
   for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
   return v;
 }
-// The host loop's test after sweep s (0-based) with residual res: stop when res < tol, before the counter counts the
-// sweep, or once the counter reaches max_iter.  *iter receives the counter.
-__device__ __forceinline__ bool jacobi_stops(float res, float tol, int s, int max_iter, int* iter) {
-  if (res < tol) {
-    *iter = s;
-    return true;
-  }
-  *iter = s + 1;
-  return s + 1 >= max_iter;
-}
 __device__ __forceinline__ void jacobi_record_stop(const JacobiTolArgs& t, float res, int iter, int last) {
   t.state->res = res;
   t.state->iter = iter;
@@ -929,10 +919,18 @@ __device__ __forceinline__ bool jacobi_resident_stop(const JacobiTolArgs& t, coo
   if (stop && blockIdx.x == 0 && tid == 0) jacobi_record_stop(t, res, iter, s);
   return stop;
 }
-template <int KZ, bool TOL>
-__global__ void __launch_bounds__(256 * kJG, 1)
-k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb, Geo g,
-                  int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks, JacobiTolArgs t) {
+// PLANES (TOL false; the kernel k_jacobi_resident_planes): a block of the z-slab tolerance solve (JacobiTolArgs::planes).  Nothing runs once *t.gate is set;
+// otherwise every CTA first stores its cells of pa, and the planes next to [z_lo, z_hi), into t.save (the block's start,
+// for a rollback: a rerun of fewer sweeps reads nothing further out that reaches the owned planes or the one below), and
+// each sweep
+// leaves, for every owned plane [own_lo, own_hi) of its block, the tile's sum of (p - pPrev)^2 in
+// t.slots[(sweep * owned planes + plane - own_lo) * tiles + tile]: each thread adds its 4 cells in x order, the warp's
+// lanes by the shuffle tree and the group's 8 warps in order -- k_jacobi_plane_residual's order, so both paths leave
+// the same bits.  The partials of the 8 warps go through KZ x kJY doubles per group behind the groups' shared memory.
+template <int KZ, bool TOL, bool PLANES>
+__device__ __forceinline__ void jacobi_resident(const unsigned char* __restrict__ mask, const float* __restrict__ div,
+                                                float* pa, float* pb, const Geo& g, int z_lo, int z_hi, int shr_lo,
+                                                int shr_hi, int sweeps, int nblocks, const JacobiTolArgs& t) {
   cooperative_groups::grid_group grid = cooperative_groups::this_grid();
   extern __shared__ float4 jsm[];
   // thread group threadIdx.z of the CTA owns block blockIdx.x * kJG + threadIdx.z (x tile fastest, then y, then z chunk)
@@ -942,6 +940,9 @@ k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restric
   float4 (*dvs)[kJY][32] = reinterpret_cast<float4 (*)[kJY][32]>(gsm + KZ * (kJY + 2) * 32);   // [KZ][kJY][32]
   float (*xh)[kJY][2] = reinterpret_cast<float (*)[kJY][2]>(gsm + KZ * (2 * kJY + 2) * 32);     // [KZ][kJY][2]: x halo
   const int tx = threadIdx.x, ty = threadIdx.y;
+  if constexpr (PLANES) {
+    if (__ldcg(t.gate)) return;
+  }
   const int blk = blockIdx.x * kJG + threadIdx.z;
   const bool live = blk < nblocks;                         // a group without a block only takes part in the barriers
   const int nxt = g.nx / 128, nyt = g.ny / kJY;
@@ -964,6 +965,14 @@ k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restric
     m4[k] = in ? __ldg((const unsigned*)(mask + base + (long long)k * sz)) : 0x01010101u;
     dvs[k][ty][tx] = in ? __ldg((const float4*)(div + base + (long long)k * sz)) : zero4;
     pc[k] = in ? __ldcg((const float4*)(pa + base + (long long)k * sz)) : zero4;
+    if constexpr (PLANES) {
+      if (in) __stcg((float4*)(t.save + base + (long long)k * sz), pc[k]);
+    }
+  }
+  if constexpr (PLANES) {       // and the planes next to the range that sweep 0 reads
+    if (live && k0 == z_lo && k0 > 0) __stcg((float4*)(t.save + base - sz), __ldcg((const float4*)(pa + base - sz)));
+    if (live && k0 + np == z_hi && z_hi < g.nz)
+      __stcg((float4*)(t.save + base + (long long)np * sz), __ldcg((const float4*)(pa + base + (long long)np * sz)));
   }
   for (int s = 0; s < sweeps; s++) {
     double sq = 0.0;                                       // TOL: this thread's sum of (p - pPrev)^2 in the sweep
@@ -1009,8 +1018,30 @@ k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restric
 #pragma unroll
           for (int q = 0; q < 4; q++) sq += (double)d[q] * (double)d[q];
         }
+        if constexpr (PLANES) {                            // in, live and the plane are uniform over the warp
+          if (k0 + k >= t.own_lo && k0 + k < t.own_hi) {
+            const float d[4] = {out[0] - ctr.x, out[1] - ctr.y, out[2] - ctr.z, out[3] - ctr.w};
+            double v = 0.0;
+#pragma unroll
+            for (int q = 0; q < 4; q++) v += (double)d[q] * (double)d[q];
+#pragma unroll
+            for (int o = 16; o > 0; o >>= 1) v += __shfl_down_sync(0xffffffffu, v, o);
+            if (tx == 0) reinterpret_cast<double*>(jsm + kJG * kGroupF4)[(threadIdx.z * KZ + k) * kJY + ty] = v;
+          }
+        }
       }
       below = ctr;
+    }
+    if constexpr (PLANES) {
+      asm volatile("bar.sync %0, 256;" ::"r"(1 + (int)threadIdx.z) : "memory");    // the warps' partials are in place
+      const int k = tx;
+      if (ty == 0 && k < KZ && k >= klo && k < khi && k0 + k >= t.own_lo && k0 + k < t.own_hi) {
+        const double* w8 = reinterpret_cast<const double*>(jsm + kJG * kGroupF4) + (threadIdx.z * KZ + k) * kJY;
+        double v = 0.0;
+        for (int w = 0; w < kJY; w++) v += w8[w];
+        const int nown = t.own_hi - t.own_lo;
+        t.slots[((size_t)s * nown + (k0 + k - t.own_lo)) * (nxt * nyt) + by * nxt + bx] = v;
+      }
     }
     if constexpr (TOL) {
       if (jacobi_resident_stop(t, grid, sq, s, sweeps, nblocks, nxt * nyt, nchunks, g.nb)) {
@@ -1025,6 +1056,25 @@ k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restric
       if (s + 1 < sweeps) grid.sync();                     // also orders the shared rows against the next sweep
     }
   }
+}
+
+template <int KZ, bool TOL>
+__global__ void __launch_bounds__(256 * kJG, 1)
+k_jacobi_resident(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb, Geo g,
+                  int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks, JacobiTolArgs t) {
+  jacobi_resident<KZ, TOL, false>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, nblocks, t);
+}
+template <int KZ>
+__global__ void __launch_bounds__(256 * kJG, 1)
+k_jacobi_resident_planes(const unsigned char* __restrict__ mask, const float* __restrict__ div, float* pa, float* pb,
+                         Geo g, int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int nblocks, JacobiTolArgs t) {
+  jacobi_resident<KZ, false, true>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, nblocks, t);
+}
+// The kernel of k_jacobi_resident<KZ, TOL> (PLANES false) or k_jacobi_resident_planes<KZ>.
+template <int KZ, bool TOL, bool PLANES>
+const void* jacobi_resident_kernel() {
+  if constexpr (PLANES) return (const void*)k_jacobi_resident_planes<KZ>;
+  else return (const void*)k_jacobi_resident<KZ, TOL>;
 }
 
 // sum over one batch element of (a - b)^2, accumulated in double: out[b] += ...
@@ -1109,6 +1159,35 @@ __global__ void k_jacobi_copy_back(float* __restrict__ p, const float* __restric
   if (!(st->last & 1)) return;
   for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < cells; i += (long long)gridDim.x * blockDim.x)
     p[i] = p_prev[i];
+}
+
+// The z-slab tolerance solve's residual after one sweep, per plane: for each of `planes` planes from local plane z_lo,
+// the sum of (cur - prev)^2 over 128 x 8 tiles, one CTA per tile and plane.  A thread adds its 4 x cells in x order,
+// a warp's lanes are added by a fixed shuffle tree and the 8 warps in order, so a tile's sum depends on the plane's
+// values and nx, ny alone -- not on the slab a plane belongs to.  slots[(plane * tiles_y + ty) * tiles_x + tx].
+__global__ void __launch_bounds__(256)
+k_jacobi_plane_residual(const float* __restrict__ cur, const float* __restrict__ prev, int nx, int ny, int z_lo,
+                        double* __restrict__ slots, const int* done) {
+  __shared__ double warps[kJY];
+  if (__ldcg(done)) return;
+  const int i0 = (blockIdx.x * 32 + threadIdx.x) * 4, j = blockIdx.y * kJY + threadIdx.y;
+  double acc = 0.0;
+  if (j < ny) {
+    const long long c = ((long long)(z_lo + blockIdx.z) * ny + j) * nx;
+    for (int q = 0; q < 4 && i0 + q < nx; q++) {
+      const float d = cur[c + i0 + q] - prev[c + i0 + q];
+      acc += (double)d * (double)d;
+    }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) acc += __shfl_down_sync(0xffffffffu, acc, o);
+  if (threadIdx.x == 0) warps[threadIdx.y] = acc;
+  __syncthreads();
+  if (threadIdx.x == 0 && threadIdx.y == 0) {
+    double v = 0.0;
+    for (int w = 0; w < kJY; w++) v += warps[w];
+    slots[((size_t)blockIdx.z * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = v;
+  }
 }
 
 // ---------------------------------------------------------------------------------------
@@ -1316,7 +1395,7 @@ void launch_jacobi_iter(const unsigned char* mask, const float* div, const float
 }
 namespace {
 // Resident CTAs of k_jacobi_resident<KZ, TOL> on the current device (0 when it cannot be launched cooperatively).
-template <int KZ, bool TOL>
+template <int KZ, bool TOL, bool PLANES = false>
 int jacobi_block_capacity(int smem) {
   static int capacities[64];         // per device (0: not asked yet, -1: cannot)
   int dev = 0;
@@ -1327,8 +1406,9 @@ int jacobi_block_capacity(int smem) {
     cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev);
     cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev);
     capacity = -1;
-    if (coop && cudaFuncSetAttribute(k_jacobi_resident<KZ, TOL>, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
-        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_jacobi_resident<KZ, TOL>, 256 * kJG, smem) == cudaSuccess &&
+    const void* kernel = jacobi_resident_kernel<KZ, TOL, PLANES>();
+    if (coop && cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem) == cudaSuccess &&
+        cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kernel, 256 * kJG, smem) == cudaSuccess &&
         sms * per_sm > 0)
       capacity = sms * per_sm;
     cudaGetLastError();
@@ -1338,18 +1418,19 @@ int jacobi_block_capacity(int smem) {
 int jacobi_block_count(const Geo& g, int z_lo, int z_hi, int kz) {
   return (g.nx / 128) * (g.ny / kJY) * ((z_hi - z_lo + kz - 1) / kz) * g.nb;
 }
-template <int KZ, bool TOL = false>
+template <int KZ, bool TOL = false, bool PLANES = false>
 int try_jacobi_block(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo, int z_hi,
                      int shr_lo, int shr_hi, int sweeps, cudaStream_t st, JacobiTolArgs t = JacobiTolArgs()) {
-  const int smem = kJG * (KZ * (kJY + 2) * 32 + KZ * kJY * 32 + KZ * kJY * 2 / 4) * (int)sizeof(float4);
+  const int smem = kJG * (KZ * (kJY + 2) * 32 + KZ * kJY * 32 + KZ * kJY * 2 / 4) * (int)sizeof(float4) +
+                   (PLANES ? kJG * KZ * kJY * (int)sizeof(double) : 0);
   int nblocks = jacobi_block_count(g, z_lo, z_hi, KZ);
   const int ctas = (nblocks + kJG - 1) / kJG;
-  if (ctas > jacobi_block_capacity<KZ, TOL>(smem)) return 0;
+  if (ctas > jacobi_block_capacity<KZ, TOL, PLANES>(smem)) return 0;
   dim3 block(32, kJY, kJG), grid(ctas, 1, 1);
   Geo gg = g;
   void* args[] = {(void*)&mask, (void*)&div, (void*)&pa, (void*)&pb, (void*)&gg, (void*)&z_lo, (void*)&z_hi,
                   (void*)&shr_lo, (void*)&shr_hi, (void*)&sweeps, (void*)&nblocks, (void*)&t};
-  if (cudaLaunchCooperativeKernel((const void*)k_jacobi_resident<KZ, TOL>, grid, block, args, smem, st) != cudaSuccess) {
+  if (cudaLaunchCooperativeKernel(jacobi_resident_kernel<KZ, TOL, PLANES>(), grid, block, args, smem, st) != cudaSuccess) {
     cudaGetLastError();
     return 0;
   }
@@ -1363,6 +1444,13 @@ int launch_jacobi_block(const unsigned char* mask, const float* div, float* pa, 
   // the shallowest block that fits: more, thinner CTAs spread a small range over more SMs
   const int kz = try_jacobi_block<4>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);
   return kz || !deep ? kz : try_jacobi_block<6>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st);
+}
+int launch_jacobi_block_planes(const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g, int z_lo,
+                               int z_hi, int shr_lo, int shr_hi, int sweeps, const JacobiTolArgs& t, cudaStream_t st) {
+  if (!g.is3d || g.nb != 1 || !jacobi_aligned(mask, div, pa, pb) || (uintptr_t)t.save % 16 != 0 || g.nx % 128 != 0 ||
+      g.ny % kJY != 0 || sweeps < 1 || z_lo >= z_hi)
+    return 0;
+  return try_jacobi_block<4, false, true>(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, st, t);
 }
 // The tolerance solve's resident path: the grids launch_jacobi_block takes for the whole-grid solve (3-D, nz >= 4,
 // at most 3 x 2^20 cells), with KZ = 4.
@@ -1399,6 +1487,12 @@ void launch_jacobi_range_sweeps(const unsigned char* mask, const float* div, flo
     gs.zhi = z_hi - s * shr_hi;
     launch_jacobi_iter(mask, div, (s & 1) ? pb : pa, (s & 1) ? pa : pb, gs, st);
   }
+}
+int jacobi_plane_tiles(int nx, int ny) { return ((nx + 127) / 128) * ((ny + kJY - 1) / kJY); }
+void launch_jacobi_plane_residual(const float* cur, const float* prev, int nx, int ny, int z_lo, int planes,
+                                  double* slots, const int* done, cudaStream_t st) {
+  k_jacobi_plane_residual<<<dim3((nx + 127) / 128, (ny + kJY - 1) / kJY, planes), dim3(32, kJY), 0, st>>>(
+      cur, prev, nx, ny, z_lo, slots, done);
 }
 void launch_sqdiff(const float* a, const float* b, long long n, int nb, double* out, cudaStream_t st) {
   long long blocks = (n + 1023) / 1024;

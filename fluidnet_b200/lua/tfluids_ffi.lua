@@ -116,6 +116,8 @@ int tfl_slab_sim_step(tfl_ctx*, tfl_slab_sim* sim, const tfl_mconf* mconf, tfl_c
 int tfl_slab_sim_ipc_export(tfl_ctx*, tfl_slab_sim* sim, char* handle_out);
 int tfl_slab_sim_ipc_connect(tfl_ctx*, tfl_slab_sim* sim, const char* handles);
 int tfl_slab_sim_jacobi_stats(tfl_ctx*, tfl_slab_sim* sim, int32_t* exchanges, float* ms, int64_t* bytes);
+int tfl_slab_sim_set_jacobi_tolerance(tfl_ctx*, tfl_slab_sim* sim, float p_tol);
+int tfl_slab_sim_jacobi_status(tfl_ctx*, tfl_slab_sim* sim, float* residual, int32_t* iterations);
 int tfl_slab_jacobi_schedule(int32_t gnz, int32_t world, int32_t rank, int32_t margin, int32_t max_iter,
                              int32_t planes[3], int32_t* blocks, int32_t cap);
 int tfl_slab_cnn_margin(int32_t banks_num);
@@ -392,6 +394,13 @@ function tfluids.slabJacobiStats(sim)                -- p exchanges of the last 
   local n, ms, by = ffi.new('int32_t[1]'), ffi.new('float[1]'), ffi.new('int64_t[1]')
   check(lib.tfl_slab_sim_jacobi_stats(ctx, sim, n, ms, by))
   return n[0], ms[0], tonumber(by[0])
+end
+-- pTol of later 'jacobi' steps of a slab sim (0: the fixed count of maxIter sweeps)
+function tfluids.slabSetJacobiTolerance(sim, pTol) check(lib.tfl_slab_sim_set_jacobi_tolerance(ctx, sim, pTol)) end
+function tfluids.slabJacobiStatus(sim)               -- residual, iterations of the last tolerance step (waits once)
+  local res, it = ffi.new('float[1]'), ffi.new('int32_t[1]')
+  check(lib.tfl_slab_sim_jacobi_status(ctx, sim, res, it))
+  return res[0], it[0]
 end
 function tfluids.slabJacobiSchedule(gnz, world, rank, margin, maxIter)   -- {planes = {lo, hi, uWidth}, blocks = {...}}
   local planes = ffi.new('int32_t[3]')

@@ -455,6 +455,18 @@ class NativeSlabSimulator:
         self.ctx.check(self.ctx.lib.tfl_slab_sim_jacobi_stats(self.ctx.h, self.h, C.byref(n), C.byref(ms), C.byref(by)))
         return n.value, ms.value, by.value
 
+    def set_jacobi_tolerance(self, p_tol):
+        """pTol of later 'jacobi' steps (tfl_slab_sim_set_jacobi_tolerance): 0 is the fixed count of maxIter sweeps,
+        > 0 solves to the tolerance as the whole-grid solveLinearSystemJacobiDevice does.  A SlabStepGraph keeps the
+        tolerance it was captured with."""
+        self.ctx.check(self.ctx.lib.tfl_slab_sim_set_jacobi_tolerance(self.ctx.h, self.h, float(p_tol)))
+
+    def jacobi_status(self):
+        """(residual, iterations) of the last step that solved to a tolerance, direct or replayed.  Synchronises."""
+        res, it = C.c_float(), C.c_int32()
+        self.ctx.check(self.ctx.lib.tfl_slab_sim_jacobi_status(self.ctx.h, self.h, C.byref(res), C.byref(it)))
+        return res.value, it.value
+
     def check(self):
         """Raises if any stencil / trace left the local slab since the last check: on any rank, or without
         torch.distributed on this one."""

@@ -458,8 +458,29 @@ int tfl_slab_sim_step(tfl_ctx* ctx, tfl_slab_sim* sim, const tfl_mconf* mconf, t
 /* Device time (ms) of the last step's three halo exchanges and of its all-reduce (0 on the Jacobi path), and the
  * bytes this rank sent in each exchange.  Synchronises. */
 int tfl_slab_sim_exchange_stats(tfl_ctx* ctx, tfl_slab_sim* sim, float ms[4], int64_t bytes[3]);
-/* The last step's p exchanges of the Jacobi path: count, summed device time (ms), bytes sent.  Synchronises. */
+/* The last step's p exchanges of the Jacobi path: count, summed device time (ms), bytes sent.  Synchronises.  After a
+ * step that solved to a tolerance (direct or replayed) the count and bytes are those of the exchanges that ran, read
+ * from the device, and ms is -1: those exchanges run inside the device-driven loop and are not timed. */
 int tfl_slab_sim_jacobi_stats(tfl_ctx* ctx, tfl_slab_sim* sim, int32_t* exchanges, float* ms, int64_t* bytes);
+/* Jacobi to a tolerance on z-slabs: the pTol of later 'jacobi' steps of this sim (convnet steps ignore it).  0, the
+ * default, is the fixed count of mconf->max_iter sweeps described at tfl_slab_sim_step, with the same launches and
+ * bits.  With p_tol > 0 the solve is the whole-grid loop of tfl_solve_linear_system_jacobi_dev over the global domain:
+ * p = pPrev = 0; after each sweep res = (float) sqrt(sum over the global grid of (p - pPrev)^2); stop when res < p_tol
+ * before the counter counts the sweep, or when it reaches max_iter; p is that loop's last iterate.  Owned p, U and
+ * density equal the whole-grid operator sequence with tfl_solve_linear_system_jacobi_dev as its solve bit for bit, and
+ * the iteration count equals its count.  The residual adds per-plane sums in ascending global z, each over fixed
+ * 128 x 8 tiles, so its bits are the same at every world size; they differ from the whole-grid residual's in the last
+ * bits.  The solve runs in blocks of 2 * margin + 2 sweeps, each followed by one gather of the per-plane residuals
+ * and one stop decision that every rank makes alike; a direct step waits for the device once per chunk of 1, 2, 4 ..
+ * 32 blocks (once per block over NCCL), a captured one (tfl_slab_graph_create) is one conditional WHILE node and does
+ * not wait.  A graph keeps the tolerance it was captured with.  Refuses negative and NaN values by name; the first
+ * p_tol > 0 allocates the solve's buffers (a stream being captured is refused then). */
+int tfl_slab_sim_set_jacobi_tolerance(tfl_ctx* ctx, tfl_slab_sim* sim, float p_tol);
+/* The last 'jacobi' step's residual and iteration count, direct or replayed, when that step solved to a tolerance.
+ * Synchronises once.  Refused, by name, before any step with a tolerance, after a fixed-count (pTol 0) 'jacobi' step,
+ * and while the context's stream is being captured.  tfl_slab_sim_step with a tolerance is refused on a stream that is
+ * being captured (it waits for its stop decision on the host): capture it with tfl_slab_graph_create. */
+int tfl_slab_sim_jacobi_status(tfl_ctx* ctx, tfl_slab_sim* sim, float* residual, int32_t* iterations);
 /* The Jacobi sweep schedule of rank `rank` (pure function; the step, and any host that emulates it, use it).  With
  * halo = 2 * margin + 2, a block of k sweeps after a p exchange of width w computes owned +- (w - 1 - s) planes in its
  * sweep s (0-based) on each side with a neighbour, and the whole local slab up to the global ends on the others.
