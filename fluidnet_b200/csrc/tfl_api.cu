@@ -210,7 +210,7 @@ int tfl_create(tfl_ctx** out, int device) {
   if (!(c->own_stream = new_stream(cudaStreamDefault))) return 1;
   c->stream = c->own_stream.get();
   if (!(c->counters = dev_zeros<unsigned long long>(16))) return 1;
-  for (StreamPtr* q : {&c->side_stream, &c->copy_in, &c->copy_out, &c->jacobi_body})
+  for (StreamPtr* q : {&c->side_stream, &c->copy_in, &c->copy_out, &c->loop_body})
     if (!(*q = new_stream(cudaStreamNonBlocking))) return 1;
   for (EventPtr* e : {&c->ev_fork, &c->ev_join, &c->ev_u_in, &c->ev_d_in, &c->ev_p_in, &c->ev_d_ready, &c->ev_d_out})
     if (!(*e = new_event(cudaEventDisableTiming))) return 1;
@@ -599,28 +599,18 @@ int jacobi_tol_solve(tfl_ctx* ctx, const char* who, const tfl_grid* p, const tfl
     TFL_CUDA(ctx, capture_while_handle(st, 1, &loop));
     t.loop = loop;
     t.has_loop = 1;
-    cudaStream_t bs = ctx->jacobi_body.get();
-    TFL_CUDA(ctx, capture_while_body(st, loop, bs));
-    jacobi_tol_sweeps(mask, div->data, p->data, p_prev, g, 0, kJacobiBodySweeps, t, bs);
-    const cudaError_t le = cudaGetLastError();
-    cudaGraph_t body = nullptr;
-    const cudaError_t ee = cudaStreamEndCapture(bs, &body);      // ends the body's capture on every path
-    TFL_CUDA(ctx, le);
-    TFL_CUDA(ctx, ee);
+    const cudaError_t loop_capture = capture_while(st, loop, ctx->loop_body.get(), [&](cudaStream_t bs) {
+      jacobi_tol_sweeps(mask, div->data, p->data, p_prev, g, 0, kJacobiBodySweeps, t, bs);
+      return cudaSuccess;
+    });
+    TFL_CUDA(ctx, loop_capture);
     ctx->launches += 2 * kJacobiBodySweeps;                      // one pass of the body
-  } else {
-    if (!ctx->jacobi_host && !(ctx->jacobi_host = pinned_alloc<int>(1))) return fail(ctx, "%s: cudaMallocHost failed", who);
-    int k = 0;
-    for (int chunk = kJacobiFirstChunk;; chunk = std::min(2 * chunk, kJacobiMaxChunk)) {
-      const int n = std::min(chunk, max_iter - k);
-      jacobi_tol_sweeps(mask, div->data, p->data, p_prev, g, k, n, t, st);
-      ctx->launches += 2 * n;
-      k += n;
-      if (k >= max_iter) break;                                  // the last residual stops the solve
-      TFL_CUDA(ctx, cudaMemcpyAsync(ctx->jacobi_host.get(), &t.state->done, sizeof(int), cudaMemcpyDeviceToHost, st));
-      TFL_CUDA(ctx, cudaStreamSynchronize(st));
-      if (*ctx->jacobi_host) break;
-    }
+  } else if (run_until_done(ctx, who, &t.state->done, max_iter, kJacobiFirstChunk, kJacobiMaxChunk, [&](int k, int n) {
+               jacobi_tol_sweeps(mask, div->data, p->data, p_prev, g, k, n, t, st);
+               ctx->launches += 2 * n;
+               return 0;
+             })) {
+    return 1;
   }
   launch_jacobi_copy_back(p->data, p_prev, (long long)cells, t.state, st);
   ctx->launches += 1;
@@ -684,46 +674,33 @@ int tfl_solve_linear_system_jacobi(tfl_ctx* ctx, const tfl_grid* p, const tfl_gr
   // p <- 0, pPrev <- 0 (generic/tfluids.cu:1854-1855).
   TFL_CUDA(ctx, cudaMemsetAsync(p->data, 0, cells * 4, st));
   TFL_CUDA(ctx, cudaMemsetAsync(p_prev, 0, cells * 4, st));
-  float* cur = p->data;
-  float* prev = p_prev;
+  // Sweep k reads pPrev and writes p for even k, the reverse for odd k.  On an L2-resident grid all sweeps but the
+  // last run in one cooperative kernel (one launch per sweep when it does not fit the SMs); larger grids are
+  // bandwidth-bound per sweep.
+  int k = 0;
+  if (max_iter > 2 && g.is3d && g.nz >= 4 && g.n * g.nb <= (3LL << 20)) {
+    k = max_iter - 1;
+    run_jacobi_block(ctx, mask, div->data, p_prev, p->data, g, 0, g.nz, 0, 0, k, -1);
+  }
+  run_jacobi_block(ctx, mask, div->data, (k & 1) ? p->data : p_prev, (k & 1) ? p_prev : p->data, g, 0, g.nz, 0, 0,
+                   max_iter - k, 0);
   float res = 0.0f;
-  int iter = 0;
-  const bool need_every = p_tol > 0.0f;     // residual < pTol can only trigger for pTol > 0
-  std::vector<double> h(g.nb);
-  // A fixed number of sweeps on an L2-resident grid: all but the last inside one cooperative kernel (sweep 0
-  // reads p_prev and writes p, as the loop below does); the loop then runs the last sweep and the residual.
-  // Larger grids are bandwidth-bound per sweep and do not fit the SMs.
-  if (!need_every && max_iter > 2 && g.is3d && g.nz >= 4 && g.n * g.nb <= (3LL << 20)) {
-    const int fused = max_iter - 1;
-    if (launch_jacobi_block(mask, div->data, p_prev, p->data, g, 0, g.nz, 0, 0, fused, /*deep=*/false, st)) {
-      ctx->launches += 1;
-      iter = fused;
-      if (fused & 1) { cur = p_prev; prev = p->data; }        // the last fused sweep wrote p
-    }
-  }
-  for (;;) {
-    launch_jacobi_iter(mask, div->data, prev, cur, g, st);
+  if (residual) {
+    std::vector<double> h(g.nb);
+    TFL_CUDA(ctx, cudaMemsetAsync(sq, 0, sizeof(double) * g.nb, st));
+    launch_sqdiff(p->data, p_prev, g.n, g.nb, sq, st);
     ctx->launches += 1;
-    const bool last = (iter + 1 >= max_iter);
-    if (need_every || (last && residual)) {
-      TFL_CUDA(ctx, cudaMemsetAsync(sq, 0, sizeof(double) * g.nb, st));
-      launch_sqdiff(p->data, p_prev, g.n, g.nb, sq, st);
-      ctx->launches += 1;
-      TFL_CUDA(ctx, cudaMemcpyAsync(h.data(), sq, sizeof(double) * g.nb, cudaMemcpyDeviceToHost, st));
-      TFL_CUDA(ctx, cudaStreamSynchronize(st));
-      double worst = 0.0;
-      for (int b = 0; b < g.nb; b++) { const double nr = sqrt(h[b]); if (nr > worst) worst = nr; }
-      res = (float)worst;
-      if (res < p_tol) break;
-    }
-    iter++;
-    if (iter >= max_iter) break;
-    float* t = cur; cur = prev; prev = t;
+    TFL_CUDA(ctx, cudaMemcpyAsync(h.data(), sq, sizeof(double) * g.nb, cudaMemcpyDeviceToHost, st));
+    TFL_CUDA(ctx, cudaStreamSynchronize(st));
+    double worst = 0.0;
+    for (int b = 0; b < g.nb; b++) { const double nr = sqrt(h[b]); if (nr > worst) worst = nr; }
+    res = (float)worst;
   }
-  if (cur == p_prev) TFL_CUDA(ctx, cudaMemcpyAsync(p->data, p_prev, cells * 4, cudaMemcpyDeviceToDevice, st));
+  // an odd last sweep (max_iter even) wrote pPrev
+  if (!(max_iter & 1)) TFL_CUDA(ctx, cudaMemcpyAsync(p->data, p_prev, cells * 4, cudaMemcpyDeviceToDevice, st));
   if (check_launch(ctx, "solveLinearSystemJacobi")) return 1;
   if (residual) *residual = res;
-  if (iterations) *iterations = iter;
+  if (iterations) *iterations = max_iter;
   return 0;
 }
 
@@ -764,7 +741,8 @@ int tfl_solve_linear_system_pcg(tfl_ctx* ctx, const tfl_grid* p, const tfl_grid*
   const int rc =
       ctx->pcg_graph
           ? pcg_solve_graph(*ctx->pcg_graph, ctx->pcg, ctx->arena.get(), p->data, flags->data, div->data, flags->nb,
-                            flags->nz, flags->ny, flags->nx, is_3d, precond, tol, max_iter, &ctx->launches, ctx->stream)
+                            flags->nz, flags->ny, flags->nx, is_3d, precond, tol, max_iter, &ctx->launches, ctx->stream,
+                            ctx->loop_body.get())
           : pcg_solve(ctx->pcg, ctx->arena.get(), p->data, flags->data, div->data, flags->nb, flags->nz, flags->ny,
                       flags->nx, is_3d, precond, tol, max_iter, residual, iterations, &ctx->launches, ctx->stream);
   return pcg_report(ctx, rc, "solveLinearSystemPCG");

@@ -693,25 +693,6 @@ struct SlabScope {       // slab placement of the context for the enclosed calls
   ~SlabScope() { ctx->slab = false; ctx->slab_margin = 2; }
 };
 
-// One block of sweeps on a prepared mask: the cooperative block kernel or one launch per sweep (path -1: automatic,
-// 0: per sweep, 1: one launch, refused when it does not apply).  Returns the path taken, -1 on refusal.
-// The automatic path takes the one-launch kernel only with 4-plane blocks (ranges up to 2.16M cells on an H100):
-// measured on an H100 at 400 W, 34 / 100 sweeps of 128^3 run at 8.4 / 7.3 us per sweep in one launch against
-// 8.9 / 8.2 per launch, but a 6-sweep block on an 8-rank slab of 256^3 (256^2 x 42 planes, 6-plane blocks) takes
-// 154 us against 94 us in per-sweep launches.
-int run_jacobi_block(tfl_ctx* ctx, const unsigned char* mask, const float* div, float* pa, float* pb, const Geo& g,
-                     int z_lo, int z_hi, int shr_lo, int shr_hi, int sweeps, int path) {
-  if (sweeps < 1) return 0;
-  if (path != 0 && launch_jacobi_block(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, path == 1, ctx->stream)) {
-    ctx->launches += 1;
-    return 1;
-  }
-  if (path == 1) return -1;
-  launch_jacobi_range_sweeps(mask, div, pa, pb, g, z_lo, z_hi, shr_lo, shr_hi, sweeps, ctx->stream);
-  ctx->launches += sweeps;
-  return 0;
-}
-
 // The Jacobi solve to s->p_tol on this rank's slab, from p = p2 = 0 on a prepared divergence and mask (`planes` and `g`
 // of slab_jacobi_projection); leaves the whole-grid loop's final iterate in p on the owned planes and the plane below.
 // Blocks of `halo` sweeps (the schedule's at world > 1, without its closing 1-plane exchange; at one rank the same
@@ -802,30 +783,26 @@ int slab_jacobi_tol(tfl_ctx* ctx, tfl_slab_sim* s, int iters, const int32_t plan
     if (has_loop) TFL_CUDA(ctx, capture_while_handle(ctx->stream, 0, &loop));
     if (block(blocks[0], loop, has_loop)) return 1;
     if (has_loop) {
-      cudaStream_t main = ctx->stream, bs = ctx->jacobi_body.get();
-      TFL_CUDA(ctx, capture_while_body(main, loop, bs));
-      ctx->stream = bs;
-      const int rc = block(blocks[1], loop, 1);
-      ctx->stream = main;
-      const cudaError_t le = cudaGetLastError();
-      cudaGraph_t body = nullptr;
-      const cudaError_t ee = cudaStreamEndCapture(bs, &body);      // ends the body's capture on every path
+      // the body block enqueues on ctx->stream, slab_exchange included
+      cudaStream_t main = ctx->stream;
+      int rc = 0;
+      const cudaError_t loop_capture = capture_while(main, loop, ctx->loop_body.get(), [&](cudaStream_t bs) {
+        ctx->stream = bs;
+        rc = block(blocks[1], loop, 1);
+        ctx->stream = main;
+        return rc ? cudaErrorUnknown : cudaSuccess;     // ctx->err names a failed block
+      });
       if (rc) return 1;
-      TFL_CUDA(ctx, le);
-      TFL_CUDA(ctx, ee);
+      TFL_CUDA(ctx, loop_capture);
     }
     if (nblk >= 2 && block(blocks[nblk - 1], loop, has_loop)) return 1;
   } else {
-    if (!ctx->jacobi_host && !(ctx->jacobi_host = pinned_alloc<int>(1))) return fail(ctx, "slab_sim_step: cudaMallocHost failed");
-    int b = 0;
-    for (int chunk = 1; b < nblk; chunk = std::min(2 * chunk, 32)) {
-      for (int i = 0; i < (nccl ? 1 : chunk) && b < nblk; i++, b++)
-        if (block(blocks[b], 0, 0)) return 1;
-      if (b >= nblk) break;                     // the last block's decision stops the solve
-      TFL_CUDA(ctx, cudaMemcpyAsync(ctx->jacobi_host.get(), done, sizeof(int), cudaMemcpyDeviceToHost, ctx->stream));
-      TFL_CUDA(ctx, cudaStreamSynchronize(ctx->stream));
-      if (*ctx->jacobi_host) break;
-    }
+    if (run_until_done(ctx, "slab_sim_step", done, nblk, 1, nccl ? 1 : 32, [&](int b0, int n) {
+          for (int b = b0; b < b0 + n; b++)
+            if (block(blocks[b], 0, 0)) return 1;
+          return 0;
+        }))
+      return 1;
   }
   // the stopping block again from its start, up to its stopping sweep
   k_slab_gated_copy<<<copy_blocks, 256, 0, ctx->stream>>>(p, s->p_save.get(), (long long)s->cells, &S->rollback, 1);

@@ -239,16 +239,40 @@ struct PcgGraphScratch {
   // [0] status of the first failed solve since the last read (pcg_status_string, sticky), [1] iterations and [2]
   // residual (float bits) of the last solve, [4..5] passes of the loop body since the last read (u64)
   DevPtr<int> words;
-  StreamPtr body_stream;       // captures the loop body
   long long body_launches = 0; // kernels in one pass of the loop body
   bool captured = false;       // a solve was captured
 };
-// A conditional WHILE node in a stream capture (the PCG solve of a step graph, the Jacobi tolerance solve).
+// A conditional WHILE node in a stream capture (the PCG solve of a step graph, the Jacobi tolerance solves).
 // capture_while_handle: a handle on the graph st is capturing, reset to `initial` at every launch of the graph.
-// capture_while_body: the node, after what st has captured so far, and the capture of stream `body` into the node's
-// body graph, which the caller ends with cudaStreamEndCapture(body).  A body kernel re-arms or clears the handle.
+// capture_while: the node, after what st has captured so far, with what enqueue(bs) enqueues on stream bs as its body
+// graph.  It ends that capture on every path and returns the first failure of: enqueue (cudaSuccess or the error it
+// met), a launch, ending the capture.  A body kernel re-arms or clears the handle.
 cudaError_t capture_while_handle(cudaStream_t st, unsigned initial, cudaGraphConditionalHandle* loop);
-cudaError_t capture_while_body(cudaStream_t st, cudaGraphConditionalHandle loop, cudaStream_t body);
+template <typename Enqueue>
+cudaError_t capture_while(cudaStream_t st, cudaGraphConditionalHandle loop, cudaStream_t bs, Enqueue&& enqueue) {
+  cudaStreamCaptureStatus cap_status;
+  cudaGraph_t graph = nullptr;
+  const cudaGraphNode_t* deps = nullptr;
+  size_t ndeps = 0;
+  cudaError_t e = cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, &deps, &ndeps);
+  if (e != cudaSuccess) return e;
+  cudaGraphNodeParams np = {};
+  np.type = cudaGraphNodeTypeConditional;
+  np.conditional.handle = loop;
+  np.conditional.type = cudaGraphCondTypeWhile;
+  np.conditional.size = 1;
+  cudaGraphNode_t node;
+  if ((e = cudaGraphAddNode(&node, graph, deps, ndeps, &np)) != cudaSuccess) return e;
+  if ((e = cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies)) != cudaSuccess) return e;
+  if ((e = cudaStreamBeginCaptureToGraph(bs, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
+                                         cudaStreamCaptureModeRelaxed)) != cudaSuccess)
+    return e;
+  e = enqueue(bs);
+  if (e == cudaSuccess) e = cudaGetLastError();
+  cudaGraph_t body = nullptr;
+  const cudaError_t ee = cudaStreamEndCapture(bs, &body);
+  return e != cudaSuccess ? e : ee;
+}
 size_t pcg_workspace_bytes(int nb, int nz, int ny, int nx);
 const char* pcg_status_string(int rc);
 // precond: 0 none, 1 ilu0, 2 ic0.  Returns 0 or a status for pcg_status_string.  Synchronises `st`.
@@ -258,11 +282,11 @@ int pcg_solve(PcgScratch& sc, void* workspace, float* p, const float* flags, con
 // Allocates gs for solves on this grid (before a capture: status 4 for ny > 960, 3 for a CUDA failure).
 int pcg_graph_alloc(PcgGraphScratch& gs, PcgScratch& sc, int nb, int nz, int ny, int nx, int is3d);
 // pcg_solve for a stream being captured: the same kernels per iteration, no host read.  The iteration loop is a
-// conditional WHILE node whose body the device re-arms; the result goes to gs.words.  `launches` gets the kernels
-// outside the loop, gs.body_launches those of one pass of the body.
+// conditional WHILE node whose body the device re-arms, captured on loop_body; the result goes to gs.words.
+// `launches` gets the kernels outside the loop, gs.body_launches those of one pass of the body.
 int pcg_solve_graph(PcgGraphScratch& gs, PcgScratch& sc, void* workspace, float* p, const float* flags,
                     const float* div, int nb, int nz, int ny, int nx, int is3d, int precond, float tol, int max_iter,
-                    long long* launches, cudaStream_t st);
+                    long long* launches, cudaStream_t st, cudaStream_t loop_body);
 // Debug: the preconditioner alone.  Same labelling, system and sweeps as pcg_solve; z = M^-1 r in the
 // natural layout (0 outside every system of two or more cells); geometry = NYP, planes per CTA,
 // chunks, cooperative grid of the sweeps.  Synchronises `st`.

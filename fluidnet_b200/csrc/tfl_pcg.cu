@@ -943,25 +943,6 @@ cudaError_t capture_while_handle(cudaStream_t st, unsigned initial, cudaGraphCon
   return cudaGraphConditionalHandleCreate(loop, graph, initial, cudaGraphCondAssignDefault);
 }
 
-cudaError_t capture_while_body(cudaStream_t st, cudaGraphConditionalHandle loop, cudaStream_t body) {
-  cudaStreamCaptureStatus cap_status;
-  cudaGraph_t graph = nullptr;
-  const cudaGraphNode_t* deps = nullptr;
-  size_t ndeps = 0;
-  cudaError_t e = cudaStreamGetCaptureInfo(st, &cap_status, nullptr, &graph, &deps, &ndeps);
-  if (e != cudaSuccess) return e;
-  cudaGraphNodeParams np = {};
-  np.type = cudaGraphNodeTypeConditional;
-  np.conditional.handle = loop;
-  np.conditional.type = cudaGraphCondTypeWhile;
-  np.conditional.size = 1;
-  cudaGraphNode_t node;
-  if ((e = cudaGraphAddNode(&node, graph, deps, ndeps, &np)) != cudaSuccess) return e;
-  if ((e = cudaStreamUpdateCaptureDependencies(st, &node, 1, cudaStreamSetCaptureDependencies)) != cudaSuccess) return e;
-  return cudaStreamBeginCaptureToGraph(body, np.conditional.phGraph_out[0], nullptr, nullptr, 0,
-                                       cudaStreamCaptureModeRelaxed);
-}
-
 int pcg_graph_alloc(PcgGraphScratch& gs, PcgScratch& sc, int nb, int nz, int ny, int nx, int is3d) {
   PcgGeo g;
   if (pcg_geometry(sc, nb, nz, ny, nx, is3d, g)) return 4;
@@ -974,7 +955,6 @@ int pcg_graph_alloc(PcgGraphScratch& gs, PcgScratch& sc, int nb, int nz, int ny,
   gs.prog_words = 2ll * g.chunks;
   if (!(gs.prog = dev_zeros<unsigned long long>((size_t)gs.prog_words))) return 3;
   if (!(gs.words = dev_zeros<int>(8))) return 3;
-  if (!(gs.body_stream = new_stream(cudaStreamNonBlocking))) return 3;
   return 0;
 }
 
@@ -990,7 +970,7 @@ int pcg_graph_alloc(PcgGraphScratch& gs, PcgScratch& sc, int nb, int nz, int ny,
 // published by that sweep.
 int pcg_solve_graph(PcgGraphScratch& gs, PcgScratch& sc, void* workspace, float* p, const float* flags,
                     const float* div, int nb, int nz, int ny, int nx, int is3d, int precond, float tol, int max_iter,
-                    long long* launches, cudaStream_t st) {
+                    long long* launches, cudaStream_t st, cudaStream_t loop_body) {
   PcgSystem s;
   int rc = pcg_label(sc, workspace, flags, nb, nz, ny, nx, is3d, launches, st, s);
   if (rc) return rc;
@@ -1020,29 +1000,27 @@ int pcg_solve_graph(PcgGraphScratch& gs, PcgScratch& sc, void* workspace, float*
   k_pcg_continue<<<1, 1, 0, st>>>(s.header, loop, nullptr);
   *launches += 1;
 
-  // the body, captured on the graph's own stream into the node's body graph
-  cudaStream_t bs = gs.body_stream.get();
-  PCG_CUDA(capture_while_body(st, loop, bs));
+  // the body, captured on loop_body into the node's body graph
   long long body = 0;
-  cudaError_t be = cudaSuccess;
-  float* p_old = s.p0;
-  float* p_new = s.p1;
-  for (int rep = 0; rep < 2 && be == cudaSuccess; rep++) {
-    be = cudaMemsetAsync(s.header, 0, 4, bs);
-    if (be == cudaSuccess && !no_precond) be = sweep(false, &body, bs);
-    if (be != cudaSuccess) break;
-    k_direction_spmv<<<ew_blocks, g.NYP, 0, bs>>>(s.cf, s.comp, no_precond ? s.r : s.z, p_old, p_new, s.w, cs, g,
-                                                  no_precond);
-    k_update<<<ew_blocks, 256, 0, bs>>>(s.cf, s.comp, p_new, s.w, s.x, s.r, cs, g.slots, no_precond);
-    k_scalars<<<comp_blocks, 256, 0, bs>>>(cs, s.header + 3, 0, tol2, max_iter, 0, no_precond);
-    body += 3;
-    float* tswap = p_old; p_old = p_new; p_new = tswap;
-  }
-  k_pcg_continue<<<1, 1, 0, bs>>>(s.header, loop, (unsigned long long*)(gs.words.get() + 4));
-  body += 1;
-  cudaGraph_t body_graph = nullptr;
-  const cudaError_t ee = cudaStreamEndCapture(bs, &body_graph);     // ends the body's capture on every path
-  if (be != cudaSuccess || ee != cudaSuccess) return 3;
+  const cudaError_t be = capture_while(st, loop, loop_body, [&](cudaStream_t bs) {
+    float* p_old = s.p0;
+    float* p_new = s.p1;
+    for (int rep = 0; rep < 2; rep++) {
+      cudaError_t e = cudaMemsetAsync(s.header, 0, 4, bs);
+      if (e == cudaSuccess && !no_precond) e = sweep(false, &body, bs);
+      if (e != cudaSuccess) return e;
+      k_direction_spmv<<<ew_blocks, g.NYP, 0, bs>>>(s.cf, s.comp, no_precond ? s.r : s.z, p_old, p_new, s.w, cs, g,
+                                                    no_precond);
+      k_update<<<ew_blocks, 256, 0, bs>>>(s.cf, s.comp, p_new, s.w, s.x, s.r, cs, g.slots, no_precond);
+      k_scalars<<<comp_blocks, 256, 0, bs>>>(cs, s.header + 3, 0, tol2, max_iter, 0, no_precond);
+      body += 3;
+      float* tswap = p_old; p_old = p_new; p_new = tswap;
+    }
+    k_pcg_continue<<<1, 1, 0, bs>>>(s.header, loop, (unsigned long long*)(gs.words.get() + 4));
+    body += 1;
+    return cudaSuccess;
+  });
+  if (be != cudaSuccess) return 3;
   gs.body_launches = body;
 
   k_xsum<<<ew_blocks, 256, 0, st>>>(s.cf, s.comp, s.x, cs, g.slots);
